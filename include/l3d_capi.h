@@ -11,7 +11,9 @@
  * Conventions: plain pointers and sizes only; the caller owns every host buffer, the library owns every device
  * buffer; no ownership passes through the ABI (unlike SparseMatrix*& in cudawrapper.h:80).  Every entry returns
  * 0 on success or a negative l3d_status; l3d_last_error() gives the message (the reference prints CUDA errors to
- * cerr and carries on, dataArray.h:198-237).  A context is single-owner (not thread-safe), one per GPU, and runs
+ * cerr and carries on, dataArray.h:198-237).  A call that fails leaves its stage (views, matches, score sweep,
+ * collinear lists, affinity matrix), and every stage computed from it, without a result: later calls that need one
+ * return L3D_ERR_STATE.  A context is single-owner (not thread-safe), one per GPU, and runs
  * on its own non-default stream.  There is NO CPU fallback: without a usable CUDA device l3d_ctx_create fails.
  */
 #ifndef L3D_CAPI_H_

@@ -8,7 +8,7 @@
 //                       (positional lock-step product, per-row sequential sums, clamps) is kept operation for operation,
 //                       so the result is bit-identical to the reference kernels; the linear search for the transposed
 //                       slot (cudawrapper.cu:524-542) is replaced by a precomputed permutation.
-#include "l3d_ctx.cuh"
+#include "l3d_cub.cuh"
 #include "l3d_sweep.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
@@ -472,39 +472,36 @@ struct KeptFlag { const unsigned char* f; __host__ __device__ int operator()(lon
 extern "C" {
 
 // device part shared by l3d_affinity_edges / l3d_affinity_matrix: similarities of all kept matches, then the candidates with
-// sim > min_affinity compacted IN EMISSION ORDER into S.d_aff_oi / oj / ow.  Returns their number (or < 0).
+// sim > min_affinity compacted IN EMISSION ORDER into A.d_aff_oi / oj / ow.  Returns their number (or < 0).
 static long long affinity_candidates(l3d_ctx* c, float two_sigA_sqr, float med_scene_depth_lines, float min_affinity)
 {
     SweepState& S = c->sweep;
+    AffinityState& A = c->aff;
     const long long total = S.total;
     if (total == 0) return 0;
     const int V = c->num_views;
     int rc;
-    DevBuf &d_sim = S.d_aff_sim, &d_flag = S.d_aff_flag, &d_gi = S.d_aff_gi, &d_gj = S.d_aff_gj, &d_pos = S.d_aff_pos;
+    DevBuf &d_sim = A.d_aff_sim, &d_flag = A.d_aff_flag, &d_gi = A.d_aff_gi, &d_gj = A.d_aff_gj, &d_pos = A.d_aff_pos;
     cudaStream_t st = c->stream;
     // the kept matches (filterMatches survivors), compacted in emission order: everything below works on this list, not on the
     // whole match store (2.5e9 entries at BASELINE configs[4])
     const long long BLK = 1ll << 30;
     long long K = 0;
-    if ((rc = l3d_reserve(c, d_pos, 16, "kept count"))) return rc;
+    L3D_RESERVE(d_pos, 16, "kept count");
     std::vector<long long> kept_in_block;
     for (long long base = 0; base < total; base += BLK) {
         const int nblk = (int)std::min(BLK, total - base);
         cub::CountingInputIterator<long long> idx(base);
         cub::TransformInputIterator<int, KeptFlag, cub::CountingInputIterator<long long> > flags(idx, KeptFlag{(const unsigned char*)S.d_eflag.p});
-        size_t tb = 0;
-        cub::DeviceReduce::Sum(nullptr, tb, flags, (int*)d_pos.p, nblk, st);
-        if ((rc = l3d_reserve(c, S.d_sort_tmp, tb, "reduce temp"))) return rc;
-        tb = S.d_sort_tmp.cap;
-        L3D_CUDA(c, cub::DeviceReduce::Sum(S.d_sort_tmp.p, tb, flags, (int*)d_pos.p, nblk, st), "kept count");
+        if ((rc = l3d_cub(c, "kept count", [&](void* tmp, size_t& bytes) { return cub::DeviceReduce::Sum(tmp, bytes, flags, (int*)d_pos.p, nblk, st); }))) return rc;
         int cnt = 0;
         L3D_CUDA(c, cudaMemcpyAsync(&cnt, d_pos.p, 4, cudaMemcpyDeviceToHost, st), "kept count");
         L3D_CUDA(c, cudaStreamSynchronize(st), "kept count");
         kept_in_block.push_back(cnt); K += cnt;
     }
-    S.n_kept = K;
+    A.n_kept = K;
     if (K == 0) return 0;
-    if ((rc = l3d_reserve(c, S.d_kx, 8 * (size_t)K, "kept list"))) return rc;
+    L3D_RESERVE(A.d_kx, 8 * K, "kept list");
     {
         long long done = 0; size_t bi = 0;
         for (long long base = 0; base < total; base += BLK, ++bi) {
@@ -512,33 +509,25 @@ static long long affinity_candidates(l3d_ctx* c, float two_sigA_sqr, float med_s
             if (kept_in_block[bi] == 0) continue;
             cub::CountingInputIterator<long long> idx(base);
             cub::TransformInputIterator<int, KeptFlag, cub::CountingInputIterator<long long> > flags(idx, KeptFlag{(const unsigned char*)S.d_eflag.p});
-            size_t tb = 0;
-            cub::DeviceSelect::Flagged(nullptr, tb, idx, flags, (long long*)S.d_kx.p + done, (int*)d_pos.p, nblk, st);
-            if ((rc = l3d_reserve(c, S.d_sort_tmp, tb, "select temp"))) return rc;
-            tb = S.d_sort_tmp.cap;
-            L3D_CUDA(c, cub::DeviceSelect::Flagged(S.d_sort_tmp.p, tb, idx, flags, (long long*)S.d_kx.p + done, (int*)d_pos.p, nblk, st), "kept list");
+            if ((rc = l3d_cub(c, "kept list", [&](void* tmp, size_t& bytes) {
+                     return cub::DeviceSelect::Flagged(tmp, bytes, idx, flags, (long long*)A.d_kx.p + done, (int*)d_pos.p, nblk, st); }))) return rc;
             done += kept_in_block[bi];
         }
         c->launches += 2 * (long long)kept_in_block.size();
     }
-    if ((rc = l3d_reserve(c, d_sim, 4 * (size_t)K, "affinity sims"))) return rc;
-    if ((rc = l3d_reserve(c, d_flag, 4 * (size_t)K, "affinity flags"))) return rc;
-    if ((rc = l3d_reserve(c, d_gi, 8 * (size_t)K, "affinity gi"))) return rc;
-    if ((rc = l3d_reserve(c, d_gj, 8 * (size_t)K, "affinity gj"))) return rc;
-    if ((rc = l3d_reserve(c, d_pos, 8 * (size_t)(K + 1), "affinity pos"))) return rc;
+    L3D_RESERVE(d_sim, 4 * K, "affinity sims"); L3D_RESERVE(d_flag, 4 * K, "affinity flags");
+    L3D_RESERVE(d_gi, 8 * K, "affinity gi"); L3D_RESERVE(d_gj, 8 * K, "affinity gj"); L3D_RESERVE(d_pos, 8 * (K + 1), "affinity pos");
     std::vector<int> rank_of_view(V);
     for (int i = 0; i < V; ++i) rank_of_view[S.order[i]] = i;
-    if ((rc = l3d_reserve(c, S.d_order, 4 * (size_t)V, "order"))) return rc;
-    if ((rc = l3d_reserve(c, S.d_rankofview, 4 * (size_t)V, "rank of view"))) return rc;
-    if ((rc = l3d_reserve(c, S.d_region_off, 8 * (size_t)(V + 1), "region offsets"))) return rc;
+    L3D_RESERVE(S.d_order, 4 * V, "order"); L3D_RESERVE(A.d_rankofview, 4 * V, "rank of view"); L3D_RESERVE(S.d_region_off, 8 * (V + 1), "region offsets");
     L3D_CUDA(c, cudaMemcpyAsync(S.d_order.p, S.order.data(), 4 * (size_t)V, cudaMemcpyHostToDevice, st), "order");
-    L3D_CUDA(c, cudaMemcpyAsync(S.d_rankofview.p, rank_of_view.data(), 4 * (size_t)V, cudaMemcpyHostToDevice, st), "rank of view");
+    L3D_CUDA(c, cudaMemcpyAsync(A.d_rankofview.p, rank_of_view.data(), 4 * (size_t)V, cudaMemcpyHostToDevice, st), "rank of view");
     L3D_CUDA(c, cudaMemcpyAsync(S.d_region_off.p, S.region_off.data(), 8 * (size_t)(V + 1), cudaMemcpyHostToDevice, st), "region offsets");
     const unsigned int nb = (unsigned int)((K + 255) / 256);
     SwStore M;
     M.vt = (const SwView*)S.d_vt.p; M.pairs = (const L3DPairDev*)c->d_pairs.p; M.row_off = (const long long*)S.d_rowoff.p; M.num_pairs = c->num_pairs; M.knn = c->knn;
     M.recs = (const l3d_match_rec*)c->d_recs.p; M.e_val = (const unsigned int*)S.d_eval.p; M.e_flag = (const unsigned char*)S.d_eflag.p;
-    k_affinity<<<nb, 256, 0, st>>>(c->views(), (const long long*)S.d_region_off.p, (const int*)S.d_order.p, V, K, (const long long*)S.d_kx.p, M, (const int*)S.d_est_best.p,
+    k_affinity<<<nb, 256, 0, st>>>(c->views(), (const long long*)S.d_region_off.p, (const int*)S.d_order.p, V, K, (const long long*)A.d_kx.p, M, (const int*)S.d_est_best.p,
                                    (const double*)S.d_est_P.p, two_sigA_sqr, med_scene_depth_lines, min_affinity, (float*)d_sim.p, (int*)d_flag.p,
                                    (long long*)d_gi.p, (long long*)d_gj.p);
     if (c->collin.valid) {
@@ -547,59 +536,45 @@ static long long affinity_candidates(l3d_ctx* c, float two_sigA_sqr, float med_s
         const long long N = c->total_segs;
         std::vector<long long> segrank_off((size_t)V + 1, 0);
         for (int i = 0; i < V; ++i) segrank_off[i + 1] = segrank_off[i] + c->h_views[S.order[i]].nseg;
-        if ((rc = l3d_reserve(c, S.d_segrank_off, 8 * ((size_t)V + 1), "segment rank offsets"))) return rc;
-        if ((rc = l3d_reserve(c, S.d_evcnt, 4 * (size_t)(N + 1), "event counts"))) return rc;
-        if ((rc = l3d_reserve(c, S.d_evptr, 8 * (size_t)(N + 1), "event offsets"))) return rc;
-        L3D_CUDA(c, cudaMemcpyAsync(S.d_segrank_off.p, segrank_off.data(), 8 * ((size_t)V + 1), cudaMemcpyHostToDevice, st), "segment rank offsets");
-        L3D_CUDA(c, cudaMemsetAsync(S.d_evcnt.p, 0, 4 * (size_t)(N + 1), st), "event counts");
+        L3D_RESERVE(A.d_segrank_off, 8 * (V + 1), "segment rank offsets");
+        L3D_RESERVE(A.d_evcnt, 4 * (N + 1), "event counts"); L3D_RESERVE(A.d_evptr, 8 * (N + 1), "event offsets");
+        L3D_CUDA(c, cudaMemcpyAsync(A.d_segrank_off.p, segrank_off.data(), 8 * ((size_t)V + 1), cudaMemcpyHostToDevice, st), "segment rank offsets");
+        L3D_CUDA(c, cudaMemsetAsync(A.d_evcnt.p, 0, 4 * (size_t)(N + 1), st), "event counts");
         const unsigned int nbs = (unsigned int)((N + 127) / 128);
-#define EV_ARGS c->views(), (const long long*)S.d_region_off.p, (const int*)S.d_order.p, (const long long*)S.d_segrank_off.p, V, N, M,                      \
+#define EV_ARGS c->views(), (const long long*)S.d_region_off.p, (const int*)S.d_order.p, (const long long*)A.d_segrank_off.p, V, N, M,                      \
                 (const int2*)S.d_ranges.p, (const int*)S.d_est_best.p,                                                                                        \
-                (const double*)S.d_est_P.p, K, (const long long*)S.d_kx.p, (const float*)d_sim.p, (const int*)d_flag.p, (const long long*)CL.d_ptr.p,             \
+                (const double*)S.d_est_P.p, K, (const long long*)A.d_kx.p, (const float*)d_sim.p, (const int*)d_flag.p, (const long long*)CL.d_ptr.p,             \
                 (const int*)CL.d_idx.p, two_sigA_sqr,                                                                                                         \
                 med_scene_depth_lines, min_affinity
-        k_aff_events<false><<<nbs, 128, 0, st>>>(EV_ARGS, (int*)S.d_evcnt.p, nullptr, nullptr, nullptr, nullptr, nullptr);
-        size_t tbe = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, tbe, (const int*)nullptr, (long long*)nullptr, N + 1, st);
-        if ((rc = l3d_reserve(c, S.d_sort_tmp, tbe, "scan temp"))) return rc;
-        tbe = S.d_sort_tmp.cap;
-        L3D_CUDA(c, cub::DeviceScan::ExclusiveSum(S.d_sort_tmp.p, tbe, (const int*)S.d_evcnt.p, (long long*)S.d_evptr.p, N + 1, st), "event scan");
+        k_aff_events<false><<<nbs, 128, 0, st>>>(EV_ARGS, (int*)A.d_evcnt.p, nullptr, nullptr, nullptr, nullptr, nullptr);
+        if ((rc = l3d_cub(c, "event scan", [&](void* tmp, size_t& bytes) {
+                 return cub::DeviceScan::ExclusiveSum(tmp, bytes, (const int*)A.d_evcnt.p, (long long*)A.d_evptr.p, N + 1, st); }))) return rc;
         long long nev = 0;
-        L3D_CUDA(c, cudaMemcpyAsync(&nev, (long long*)S.d_evptr.p + N, 8, cudaMemcpyDeviceToHost, st), "event count");
+        L3D_CUDA(c, cudaMemcpyAsync(&nev, (long long*)A.d_evptr.p + N, 8, cudaMemcpyDeviceToHost, st), "event count");
         L3D_CUDA(c, cudaStreamSynchronize(st), "affinity events");
         c->launches += 4;
         if (nev == 0) return 0;
         if (nev >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "affinity: more than 2^31 candidate events");
-        if ((rc = l3d_reserve(c, S.d_aff_oi, 8 * (size_t)nev, "edges i"))) return rc;
-        if ((rc = l3d_reserve(c, S.d_aff_oj, 8 * (size_t)nev, "edges j"))) return rc;
-        if ((rc = l3d_reserve(c, S.d_aff_ow, 4 * (size_t)nev, "edges w"))) return rc;
-        if ((rc = l3d_reserve(c, S.d_aff_par, 4 * (size_t)nev, "edge parents"))) return rc;
-        k_aff_events<true><<<nbs, 128, 0, st>>>(EV_ARGS, nullptr, (const long long*)S.d_evptr.p, (long long*)S.d_aff_oi.p, (long long*)S.d_aff_oj.p,
-                                                (float*)S.d_aff_ow.p, (int*)S.d_aff_par.p);
+        L3D_RESERVE(A.d_aff_oi, 8 * nev, "edges i"); L3D_RESERVE(A.d_aff_oj, 8 * nev, "edges j");
+        L3D_RESERVE(A.d_aff_ow, 4 * nev, "edges w"); L3D_RESERVE(A.d_aff_par, 4 * nev, "edge parents");
+        k_aff_events<true><<<nbs, 128, 0, st>>>(EV_ARGS, nullptr, (const long long*)A.d_evptr.p, (long long*)A.d_aff_oi.p, (long long*)A.d_aff_oj.p,
+                                                (float*)A.d_aff_ow.p, (int*)A.d_aff_par.p);
 #undef EV_ARGS
         ++c->launches;
         L3D_CUDA(c, cudaGetLastError(), "k_aff_events");
-        S.aff_has_parents = true;
+        A.aff_has_parents = true;
         return nev;
     }
-    S.aff_has_parents = false;
-    size_t tb = 0;
+    A.aff_has_parents = false;
     if (K >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "affinity: more than 2^31 kept matches");
-    cub::DeviceScan::ExclusiveSum(nullptr, tb, (const int*)d_flag.p, (long long*)d_pos.p, (int)K, st);
-    if ((rc = l3d_reserve(c, S.d_sort_tmp, tb, "scan temp"))) return rc;
-    tb = S.d_sort_tmp.cap;   // scan over the kept matches; the edge count is pos[K-1] + flag[K-1]
-    L3D_CUDA(c, cub::DeviceScan::ExclusiveSum(S.d_sort_tmp.p, tb, (const int*)d_flag.p, (long long*)d_pos.p, (int)K, st), "affinity scan");
-    long long last_pos = 0; int last_flag = 0;
-    L3D_CUDA(c, cudaMemcpyAsync(&last_pos, (long long*)d_pos.p + K - 1, 8, cudaMemcpyDeviceToHost, st), "count");
-    L3D_CUDA(c, cudaMemcpyAsync(&last_flag, (int*)d_flag.p + K - 1, 4, cudaMemcpyDeviceToHost, st), "count");
+    ScanTotal t;      // scan over the kept matches; the edge count is pos[K-1] + flag[K-1]
+    if ((rc = l3d_scan_total(c, (const int*)d_flag.p, (long long*)d_pos.p, (int)K, (const int*)d_flag.p, t, "affinity scan"))) return rc;
     L3D_CUDA(c, cudaStreamSynchronize(st), "affinity");
-    const long long ne = last_pos + last_flag;
+    const long long ne = t.last_out + t.last_src;
     c->launches += 3;
     if (ne == 0) return 0;
-    DevBuf &o_i = S.d_aff_oi, &o_j = S.d_aff_oj, &o_w = S.d_aff_ow;
-    if ((rc = l3d_reserve(c, o_i, 8 * (size_t)ne, "edges i"))) return rc;
-    if ((rc = l3d_reserve(c, o_j, 8 * (size_t)ne, "edges j"))) return rc;
-    if ((rc = l3d_reserve(c, o_w, 4 * (size_t)ne, "edges w"))) return rc;
+    DevBuf &o_i = A.d_aff_oi, &o_j = A.d_aff_oj, &o_w = A.d_aff_ow;
+    L3D_RESERVE(o_i, 8 * ne, "edges i"); L3D_RESERVE(o_j, 8 * ne, "edges j"); L3D_RESERVE(o_w, 4 * ne, "edges w");
     k_affinity_compact<<<nb, 256, 0, st>>>(K, (const int*)d_flag.p, (const long long*)d_pos.p, (const float*)d_sim.p, (const long long*)d_gi.p,
                                            (const long long*)d_gj.p, (long long*)o_i.p, (long long*)o_j.p, (float*)o_w.p);
     ++c->launches;
@@ -616,13 +591,13 @@ long long l3d_affinity_edges(l3d_ctx* c, float two_sigA_sqr, float med_scene_dep
     if (!c) return L3D_ERR_INVALID;
     if (!c->sweep.valid) return l3d_fail(c, L3D_ERR_STATE, "l3d_affinity_edges: call l3d_score_sweep first");
     cudaSetDevice(c->device);
-    SweepState& S = c->sweep;
+    const AffinityState& A = c->aff;
     const long long ne = affinity_candidates(c, two_sigA_sqr, med_scene_depth_lines, min_affinity);
     if (ne <= 0 || !out_gi || ne > cap) return ne;
     cudaStream_t st = c->stream;
-    L3D_CUDA(c, cudaMemcpyAsync(out_gi, S.d_aff_oi.p, 8 * (size_t)ne, cudaMemcpyDeviceToHost, st), "download edges");
-    L3D_CUDA(c, cudaMemcpyAsync(out_gj, S.d_aff_oj.p, 8 * (size_t)ne, cudaMemcpyDeviceToHost, st), "download edges");
-    L3D_CUDA(c, cudaMemcpyAsync(out_w, S.d_aff_ow.p, 4 * (size_t)ne, cudaMemcpyDeviceToHost, st), "download edges");
+    L3D_CUDA(c, cudaMemcpyAsync(out_gi, A.d_aff_oi.p, 8 * (size_t)ne, cudaMemcpyDeviceToHost, st), "download edges");
+    L3D_CUDA(c, cudaMemcpyAsync(out_gj, A.d_aff_oj.p, 8 * (size_t)ne, cudaMemcpyDeviceToHost, st), "download edges");
+    L3D_CUDA(c, cudaMemcpyAsync(out_w, A.d_aff_ow.p, 4 * (size_t)ne, cudaMemcpyDeviceToHost, st), "download edges");
     L3D_CUDA(c, cudaStreamSynchronize(st), "affinity download");
     return ne;
 }
@@ -638,51 +613,48 @@ long long l3d_affinity_edges(l3d_ctx* c, float two_sigA_sqr, float med_scene_dep
 long long l3d_affinity_matrix(l3d_ctx* c, float two_sigA_sqr, float med_scene_depth_lines, float min_affinity, int* out_i, int* out_j,
                               float* out_w, long long cap_edges, long long* out_local2global, long long cap_ids, long long* num_ids)
 {
-    if (!c || !num_ids) return L3D_ERR_INVALID;
+    if (!c) return L3D_ERR_INVALID;
+    AffinityState& A = c->aff;
+    const bool cached = A.valid && A.two_sigA_sqr == two_sigA_sqr && A.med == med_scene_depth_lines && A.min_aff == min_affinity;
+    if (!cached) c->drop(Stage::Affinity);
+    if (!num_ids) return L3D_ERR_INVALID;
     if (!c->sweep.valid) return l3d_fail(c, L3D_ERR_STATE, "l3d_affinity_matrix: call l3d_score_sweep first");
     cudaSetDevice(c->device);
-    SweepState& S = c->sweep;
-    AffinityState& A = c->aff;
     cudaStream_t st = c->stream;
     int rc;
-    if (!A.valid || A.two_sigA_sqr != two_sigA_sqr || A.med != med_scene_depth_lines || A.min_aff != min_affinity) {
-        A.valid = false;
+    if (!cached) {
         const long long ne = affinity_candidates(c, two_sigA_sqr, med_scene_depth_lines, min_affinity);
         if (ne < 0) return ne;
         A.K = 0; A.n_ids = 0;
         if (ne > 0) {
             if (ne >= (1ll << 32) || c->total_segs >= (1ll << 32)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_affinity_matrix: more than 2^32 candidates / segments");
             const long long N = c->total_segs;
-#define RES(buf, bytes, what) if ((rc = l3d_reserve(c, buf, (size_t)std::max<long long>((long long)(bytes), 16), what))) return rc
-            RES(A.d_key, 8 * ne, "pair keys"); RES(A.d_key2, 8 * ne, "pair keys"); RES(A.d_val, 4 * ne, "pair vals"); RES(A.d_val2, 4 * ne, "pair vals");
-            RES(A.d_keep, 4 * ne, "keep flags"); RES(A.d_q, 8 * (ne + 1), "edge positions"); RES(A.d_time, 8 * N, "appearance times");
-            RES(A.d_nflag, 4 * N, "node flags"); RES(A.d_npos, 8 * (N + 1), "node positions"); RES(A.d_idof, 4 * N, "id of segment");
+            L3D_RESERVE(A.d_key, 8 * ne, "pair keys"); L3D_RESERVE(A.d_key2, 8 * ne, "pair keys"); L3D_RESERVE(A.d_val, 4 * ne, "pair vals"); L3D_RESERVE(A.d_val2, 4 * ne, "pair vals");
+            L3D_RESERVE(A.d_keep, 4 * ne, "keep flags"); L3D_RESERVE(A.d_q, 8 * (ne + 1), "edge positions"); L3D_RESERVE(A.d_time, 8 * N, "appearance times");
+            L3D_RESERVE(A.d_nflag, 4 * N, "node flags"); L3D_RESERVE(A.d_npos, 8 * (N + 1), "node positions"); L3D_RESERVE(A.d_idof, 4 * N, "id of segment");
             const int bseg = bits_i64(N);
-            size_t tb1 = 0, tb2 = 0, tb3 = 0;
-            cub::DeviceRadixSort::SortPairs(nullptr, tb1, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (unsigned int*)nullptr, (unsigned int*)nullptr, (int)ne, 0, 32 + bseg, st);
-            cub::DeviceScan::ExclusiveSum(nullptr, tb2, (const int*)nullptr, (long long*)nullptr, std::max(ne, N), st);
-            cub::DeviceRadixSort::SortPairs(nullptr, tb3, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (unsigned int*)nullptr, (unsigned int*)nullptr, (int)std::min<long long>(N, 2 * ne), 0, 64, st);
-            RES(S.d_sort_tmp, std::max(tb1, std::max(tb2, tb3)), "sort temp");
             const unsigned int nbe = (unsigned int)((ne + 255) / 256), nbn = (unsigned int)((N + 255) / 256);
-            k_aff_keys<<<nbe, 256, 0, st>>>(ne, (const long long*)S.d_aff_oi.p, (const long long*)S.d_aff_oj.p, (unsigned long long*)A.d_key.p, (unsigned int*)A.d_val.p);
-            size_t tb = S.d_sort_tmp.cap;
-            cub::DeviceRadixSort::SortPairs(S.d_sort_tmp.p, tb, (const unsigned long long*)A.d_key.p, (unsigned long long*)A.d_key2.p, (const unsigned int*)A.d_val.p, (unsigned int*)A.d_val2.p, (int)ne, 0, 32 + bseg, st);
+            const long long* oi = (const long long*)A.d_aff_oi.p; const long long* oj = (const long long*)A.d_aff_oj.p;
+            k_aff_keys<<<nbe, 256, 0, st>>>(ne, oi, oj, (unsigned long long*)A.d_key.p, (unsigned int*)A.d_val.p);
+            if ((rc = l3d_cub(c, "pair sort", [&](void* tmp, size_t& bytes) {
+                     return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const unsigned long long*)A.d_key.p, (unsigned long long*)A.d_key2.p, (const unsigned int*)A.d_val.p,
+                                                            (unsigned int*)A.d_val2.p, (int)ne, 0, 32 + bseg, st); }))) return rc;
             {   // unused(): fixpoint over the conditional events (one round + one confirming round without collinearity links)
-                const int* par = S.aff_has_parents ? (const int*)S.d_aff_par.p : nullptr;
-                RES(A.d_keep2, 4 * ne, "keep flags"); RES(A.d_found, 4 * N, "found flags"); RES(A.d_changed, 16, "changed flag");
+                const int* par = A.aff_has_parents ? (const int*)A.d_aff_par.p : nullptr;
+                L3D_RESERVE(A.d_keep2, 4 * ne, "keep flags"); L3D_RESERVE(A.d_found, 4 * N, "found flags"); L3D_RESERVE(A.d_changed, 16, "changed flag");
                 L3D_CUDA(c, cudaMemsetAsync(A.d_keep.p, 0, 4 * ne, st), "clear keep");
                 L3D_CUDA(c, cudaMemsetAsync(A.d_found.p, 0, 4 * N, st), "clear found");
                 int* acc_prev = (int*)A.d_keep.p; int* acc_new = (int*)A.d_keep2.p;
                 for (int round = 0;; ++round) {
                     if (round > 100000) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_affinity_matrix: unused() fixpoint did not converge");
                     L3D_CUDA(c, cudaMemsetAsync(A.d_changed.p, 0, 4, st), "clear changed");
-                    k_aff_round<<<nbe, 256, 0, st>>>(ne, (const unsigned long long*)A.d_key2.p, (const unsigned int*)A.d_val2.p, par, (const long long*)S.d_aff_oi.p,
+                    k_aff_round<<<nbe, 256, 0, st>>>(ne, (const unsigned long long*)A.d_key2.p, (const unsigned int*)A.d_val2.p, par, oi,
                                                      acc_prev, (const int*)A.d_found.p, acc_new, (int*)A.d_changed.p);
                     std::swap(acc_prev, acc_new);
                     ++c->launches;
                     if (!par) break;                 // all events direct: the head of every run, final after one round
                     L3D_CUDA(c, cudaMemsetAsync(A.d_found.p, 0, 4 * N, st), "clear found");
-                    k_aff_found<<<nbe, 256, 0, st>>>(ne, par, (const long long*)S.d_aff_oi.p, acc_prev, (int*)A.d_found.p);
+                    k_aff_found<<<nbe, 256, 0, st>>>(ne, par, oi, acc_prev, (int*)A.d_found.p);
                     int changed = 0;
                     L3D_CUDA(c, cudaMemcpyAsync(&changed, A.d_changed.p, 4, cudaMemcpyDeviceToHost, st), "changed flag");
                     L3D_CUDA(c, cudaStreamSynchronize(st), "affinity fixpoint");
@@ -691,29 +663,26 @@ long long l3d_affinity_matrix(l3d_ctx* c, float two_sigA_sqr, float med_scene_de
                 }
                 if (acc_prev != (int*)A.d_keep.p) L3D_CUDA(c, cudaMemcpyAsync(A.d_keep.p, acc_prev, 4 * ne, cudaMemcpyDeviceToDevice, st), "keep flags");
             }
-            tb = S.d_sort_tmp.cap;
-            cub::DeviceScan::ExclusiveSum(S.d_sort_tmp.p, tb, (const int*)A.d_keep.p, (long long*)A.d_q.p, ne, st);
+            if ((rc = l3d_cub(c, "edge scan", [&](void* tmp, size_t& bytes) {
+                     return cub::DeviceScan::ExclusiveSum(tmp, bytes, (const int*)A.d_keep.p, (long long*)A.d_q.p, ne, st); }))) return rc;
             L3D_CUDA(c, cudaMemsetAsync(A.d_time.p, 0xFF, 8 * N, st), "init times");
-            k_aff_time<<<nbe, 256, 0, st>>>(ne, (const int*)A.d_keep.p, (const long long*)A.d_q.p, (const long long*)S.d_aff_oi.p, (const long long*)S.d_aff_oj.p, (unsigned long long*)A.d_time.p);
+            k_aff_time<<<nbe, 256, 0, st>>>(ne, (const int*)A.d_keep.p, (const long long*)A.d_q.p, oi, oj, (unsigned long long*)A.d_time.p);
             k_aff_nodeflags<<<nbn, 256, 0, st>>>(N, (const unsigned long long*)A.d_time.p, (int*)A.d_nflag.p);
-            tb = S.d_sort_tmp.cap;
-            cub::DeviceScan::ExclusiveSum(S.d_sort_tmp.p, tb, (const int*)A.d_nflag.p, (long long*)A.d_npos.p, N, st);
-            long long lq = 0, lp = 0; int lk = 0, lf = 0;
-            L3D_CUDA(c, cudaMemcpyAsync(&lq, (long long*)A.d_q.p + ne - 1, 8, cudaMemcpyDeviceToHost, st), "count");
-            L3D_CUDA(c, cudaMemcpyAsync(&lk, (int*)A.d_keep.p + ne - 1, 4, cudaMemcpyDeviceToHost, st), "count");
-            L3D_CUDA(c, cudaMemcpyAsync(&lp, (long long*)A.d_npos.p + N - 1, 8, cudaMemcpyDeviceToHost, st), "count");
-            L3D_CUDA(c, cudaMemcpyAsync(&lf, (int*)A.d_nflag.p + N - 1, 4, cudaMemcpyDeviceToHost, st), "count");
+            ScanTotal edges, nodes;         // both totals under one synchronisation
+            if ((rc = l3d_scan_total(c, (const int*)A.d_nflag.p, (long long*)A.d_npos.p, N, (const int*)A.d_nflag.p, nodes, "node scan"))) return rc;
+            if ((rc = l3d_read_total(c, (const long long*)A.d_q.p, (const int*)A.d_keep.p, ne, edges, "edge count"))) return rc;
             L3D_CUDA(c, cudaStreamSynchronize(st), "affinity matrix");
-            A.K = lq + lk; A.n_ids = lp + lf;
-            RES(A.d_nkey, 8 * A.n_ids, "node keys"); RES(A.d_nkey2, 8 * A.n_ids, "node keys"); RES(A.d_nval, 4 * A.n_ids, "node vals"); RES(A.d_nval2, 4 * A.n_ids, "node vals");
-            RES(A.d_l2g, 8 * A.n_ids, "local2global"); RES(A.d_ei, 4 * 2 * A.K, "A i"); RES(A.d_ej, 4 * 2 * A.K, "A j"); RES(A.d_ew, 4 * 2 * A.K, "A w");
-#undef RES
+            A.K = edges.last_out + edges.last_src; A.n_ids = nodes.last_out + nodes.last_src;
+            L3D_RESERVE(A.d_nkey, 8 * A.n_ids, "node keys"); L3D_RESERVE(A.d_nkey2, 8 * A.n_ids, "node keys"); L3D_RESERVE(A.d_nval, 4 * A.n_ids, "node vals");
+            L3D_RESERVE(A.d_nval2, 4 * A.n_ids, "node vals"); L3D_RESERVE(A.d_l2g, 8 * A.n_ids, "local2global");
+            L3D_RESERVE(A.d_ei, 4 * 2 * A.K, "A i"); L3D_RESERVE(A.d_ej, 4 * 2 * A.K, "A j"); L3D_RESERVE(A.d_ew, 4 * 2 * A.K, "A w");
             k_aff_nodes<<<nbn, 256, 0, st>>>(N, (const int*)A.d_nflag.p, (const long long*)A.d_npos.p, (const unsigned long long*)A.d_time.p, (unsigned long long*)A.d_nkey.p, (unsigned int*)A.d_nval.p);
-            tb = S.d_sort_tmp.cap;
-            cub::DeviceRadixSort::SortPairs(S.d_sort_tmp.p, tb, (const unsigned long long*)A.d_nkey.p, (unsigned long long*)A.d_nkey2.p, (const unsigned int*)A.d_nval.p, (unsigned int*)A.d_nval2.p, (int)A.n_ids, 0, 64, st);
+            if ((rc = l3d_cub(c, "node sort", [&](void* tmp, size_t& bytes) {
+                     return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const unsigned long long*)A.d_nkey.p, (unsigned long long*)A.d_nkey2.p, (const unsigned int*)A.d_nval.p,
+                                                            (unsigned int*)A.d_nval2.p, (int)A.n_ids, 0, 64, st); }))) return rc;
             k_aff_ids<<<(unsigned int)((A.n_ids + 255) / 256), 256, 0, st>>>(A.n_ids, (const unsigned int*)A.d_nval2.p, (int*)A.d_idof.p, (long long*)A.d_l2g.p);
-            k_aff_emit<<<nbe, 256, 0, st>>>(ne, (const int*)A.d_keep.p, (const long long*)A.d_q.p, (const long long*)S.d_aff_oi.p, (const long long*)S.d_aff_oj.p,
-                                            (const float*)S.d_aff_ow.p, (const int*)A.d_idof.p, (int*)A.d_ei.p, (int*)A.d_ej.p, (float*)A.d_ew.p);
+            k_aff_emit<<<nbe, 256, 0, st>>>(ne, (const int*)A.d_keep.p, (const long long*)A.d_q.p, oi, oj, (const float*)A.d_aff_ow.p, (const int*)A.d_idof.p,
+                                            (int*)A.d_ei.p, (int*)A.d_ej.p, (float*)A.d_ew.p);
             c->launches += 8 + 30;
             L3D_CUDA(c, cudaGetLastError(), "affinity matrix kernels");
         }
@@ -749,57 +718,46 @@ static int rdd_core(l3d_ctx* c, int n, long long nnz, const int* d_ei, const int
 {
     RddState& R = c->rdd;
     int rc;
-#define RES(buf, bytes, what) if ((rc = l3d_reserve(c, buf, (size_t)(bytes), what))) return rc
-    RES(R.d_krow, 8 * nnz, "rdd keys"); RES(R.d_kcol, 8 * nnz, "rdd keys"); RES(R.d_k2, 8 * nnz, "rdd keys"); RES(R.d_idx, 4 * nnz, "rdd idx"); RES(R.d_idx2, 4 * nnz, "rdd idx");
-    RES(R.d_P, 4 * nnz, "rdd P"); RES(R.d_Pn, 4 * nnz, "rdd P'"); RES(R.d_W, 4 * nnz, "rdd W");
-    RES(R.d_prow, 4 * nnz, "rdd rows"); RES(R.d_pcol, 4 * nnz, "rdd cols"); RES(R.d_wmaj, 4 * nnz, "rdd cols"); RES(R.d_wmin, 4 * nnz, "rdd rows");
-    RES(R.d_rowptr, 4 * ((size_t)n + 1), "rdd rowptr"); RES(R.d_colptr, 4 * ((size_t)n + 1), "rdd colptr"); RES(R.d_tslot, 4 * nnz, "rdd tslot");
-    size_t sb = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, sb, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (unsigned int*)nullptr, (unsigned int*)nullptr, (int)nnz, 0, 64, c->stream);
-    RES(R.d_tmp, sb, "rdd sort temp");
-#undef RES
+    L3D_RESERVE(R.d_krow, 8 * nnz, "rdd keys"); L3D_RESERVE(R.d_kcol, 8 * nnz, "rdd keys"); L3D_RESERVE(R.d_k2, 8 * nnz, "rdd keys");
+    L3D_RESERVE(R.d_idx, 4 * nnz, "rdd idx"); L3D_RESERVE(R.d_idx2, 4 * nnz, "rdd idx");
+    L3D_RESERVE(R.d_P, 4 * nnz, "rdd P"); L3D_RESERVE(R.d_Pn, 4 * nnz, "rdd P'"); L3D_RESERVE(R.d_W, 4 * nnz, "rdd W");
+    L3D_RESERVE(R.d_prow, 4 * nnz, "rdd rows"); L3D_RESERVE(R.d_pcol, 4 * nnz, "rdd cols"); L3D_RESERVE(R.d_wmaj, 4 * nnz, "rdd cols"); L3D_RESERVE(R.d_wmin, 4 * nnz, "rdd rows");
+    L3D_RESERVE(R.d_rowptr, 4 * ((long long)n + 1), "rdd rowptr"); L3D_RESERVE(R.d_colptr, 4 * ((long long)n + 1), "rdd colptr"); L3D_RESERVE(R.d_tslot, 4 * nnz, "rdd tslot");
     cudaStream_t st = c->stream;
     const unsigned int nb = (unsigned int)((nnz + 255) / 256);
     k_rdd_keys<<<nb, 256, 0, st>>>(nnz, d_ei, d_ej, (unsigned long long*)R.d_krow.p, (unsigned long long*)R.d_kcol.p, (unsigned int*)R.d_idx.p);
-    size_t tb = R.d_tmp.cap;
-    // P: row-sorted (stable, like std::list::sort with sortCLEdgesByRow, sparsematrix.cc:22-25 / 104-107)
-    cub::DeviceRadixSort::SortPairs(R.d_tmp.p, tb, (const unsigned long long*)R.d_krow.p, (unsigned long long*)R.d_k2.p, (const unsigned int*)R.d_idx.p, (unsigned int*)R.d_idx2.p, (int)nnz, 0, 64, st);
+    // P: row-sorted (stable, like std::list::sort with sortCLEdgesByRow, sparsematrix.cc:22-25 / 104-107), W: col-sorted
+    auto sort_by = [&](const DevBuf& keys) {
+        return l3d_cub(c, "rdd sort", [&](void* tmp, size_t& bytes) {
+            return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const unsigned long long*)keys.p, (unsigned long long*)R.d_k2.p, (const unsigned int*)R.d_idx.p,
+                                                   (unsigned int*)R.d_idx2.p, (int)nnz, 0, 64, st); });
+    };
+    if ((rc = sort_by(R.d_krow))) return rc;
     k_rdd_gather<<<nb, 256, 0, st>>>(nnz, (const unsigned long long*)R.d_k2.p, (const unsigned int*)R.d_idx2.p, d_ew, (float*)R.d_P.p, (int*)R.d_prow.p, (int*)R.d_pcol.p);
-    // W: col-sorted
-    tb = R.d_tmp.cap;
-    cub::DeviceRadixSort::SortPairs(R.d_tmp.p, tb, (const unsigned long long*)R.d_kcol.p, (unsigned long long*)R.d_k2.p, (const unsigned int*)R.d_idx.p, (unsigned int*)R.d_idx2.p, (int)nnz, 0, 64, st);
+    if ((rc = sort_by(R.d_kcol))) return rc;
     k_rdd_gather<<<nb, 256, 0, st>>>(nnz, (const unsigned long long*)R.d_k2.p, (const unsigned int*)R.d_idx2.p, d_ew, (float*)R.d_W.p, (int*)R.d_wmaj.p, (int*)R.d_wmin.p);
     k_rdd_ptr<<<(n + 256) / 256, 256, 0, st>>>(n, (int)nnz, (const int*)R.d_prow.p, (int*)R.d_rowptr.p);
     k_rdd_ptr<<<(n + 256) / 256, 256, 0, st>>>(n, (int)nnz, (const int*)R.d_wmaj.p, (int*)R.d_colptr.p);
     k_rdd_tslot<<<nb, 256, 0, st>>>(nnz, (const int*)R.d_prow.p, (const int*)R.d_pcol.p, (const int*)R.d_rowptr.p, (int*)R.d_tslot.p);
     // padded value arrays (rows / columns on float4 boundaries)
-    if ((rc = l3d_reserve(c, R.d_len4, 4 * ((size_t)n + 1), "rdd len4"))) return rc;
-    if ((rc = l3d_reserve(c, R.d_rp4, 4 * ((size_t)n + 1), "rdd rp4"))) return rc;
-    if ((rc = l3d_reserve(c, R.d_cp4, 4 * ((size_t)n + 1), "rdd cp4"))) return rc;
+    L3D_RESERVE(R.d_len4, 4 * ((long long)n + 1), "rdd len4"); L3D_RESERVE(R.d_rp4, 4 * ((long long)n + 1), "rdd rp4"); L3D_RESERVE(R.d_cp4, 4 * ((long long)n + 1), "rdd cp4");
     int tot4[2] = {0, 0};
     for (int pass = 0; pass < 2; ++pass) {
         const int* ptr = (const int*)(pass ? R.d_colptr.p : R.d_rowptr.p);
         int* p4 = (int*)(pass ? R.d_cp4.p : R.d_rp4.p);
         L3D_CUDA(c, cudaMemsetAsync(R.d_len4.p, 0, 4 * ((size_t)n + 1), st), "rdd len4");
         k_rdd_len4<<<(n + 255) / 256, 256, 0, st>>>(n, ptr, (int*)R.d_len4.p);
-        tb = R.d_tmp.cap;
-        size_t need = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, need, (const int*)R.d_len4.p, p4, n + 1, st);
-        if (need > tb) { if ((rc = l3d_reserve(c, R.d_tmp, need, "rdd scan temp"))) return rc; tb = R.d_tmp.cap; }
-        L3D_CUDA(c, cub::DeviceScan::ExclusiveSum(R.d_tmp.p, tb, (const int*)R.d_len4.p, p4, n + 1, st), "rdd scan");
+        if ((rc = l3d_cub(c, "rdd scan", [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, (const int*)R.d_len4.p, p4, n + 1, st); }))) return rc;
         L3D_CUDA(c, cudaMemcpyAsync(&tot4[pass], p4 + n, 4, cudaMemcpyDeviceToHost, st), "rdd padded size");
     }
     L3D_CUDA(c, cudaStreamSynchronize(st), "rdd padded size");
     const size_t pbytes = 16 * (size_t)std::max(tot4[0], 1), wbytes = 16 * (size_t)std::max(tot4[1], 1);
-    if ((rc = l3d_reserve(c, R.d_Pp, pbytes, "rdd P padded"))) return rc;
-    if ((rc = l3d_reserve(c, R.d_Pnp, pbytes, "rdd P' padded"))) return rc;
-    if ((rc = l3d_reserve(c, R.d_Wp, wbytes, "rdd W padded"))) return rc;
+    L3D_RESERVE(R.d_Pp, pbytes, "rdd P padded"); L3D_RESERVE(R.d_Pnp, pbytes, "rdd P' padded"); L3D_RESERVE(R.d_Wp, wbytes, "rdd W padded");
     L3D_CUDA(c, cudaMemsetAsync(R.d_Pp.p, 0, pbytes, st), "rdd pad"); L3D_CUDA(c, cudaMemsetAsync(R.d_Wp.p, 0, wbytes, st), "rdd pad");
     k_rdd_pad<<<nb, 256, 0, st>>>(nnz, (const int*)R.d_prow.p, (const int*)R.d_rowptr.p, (const int*)R.d_rp4.p, (const float*)R.d_P.p, (float*)R.d_Pp.p);
     k_rdd_pad<<<nb, 256, 0, st>>>(nnz, (const int*)R.d_wmaj.p, (const int*)R.d_colptr.p, (const int*)R.d_cp4.p, (const float*)R.d_W.p, (float*)R.d_Wp.p);
     if (4ll * std::max(tot4[0], tot4[1]) >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_rdd: padded matrix too large for 32-bit slots");
-    if ((rc = l3d_reserve(c, R.d_plan, 16 * (size_t)nnz, "rdd plan"))) return rc;
-    if ((rc = l3d_reserve(c, R.d_dst, 4 * (size_t)nnz, "rdd dst"))) return rc;
+    L3D_RESERVE(R.d_plan, 16 * nnz, "rdd plan"); L3D_RESERVE(R.d_dst, 4 * nnz, "rdd dst");
     k_rdd_plan<<<nb, 256, 0, st>>>(nnz, (const int*)R.d_prow.p, (const int*)R.d_pcol.p, (const int*)R.d_rowptr.p, (const int*)R.d_colptr.p,
                                    (const int*)R.d_rp4.p, (const int*)R.d_cp4.p, (const int*)R.d_tslot.p, (int4*)R.d_plan.p, (int*)R.d_dst.p);
     // P' starts as a copy of the un-normalised P (cudawrapper.cu:724), then P is row-normalised (727)
@@ -807,15 +765,18 @@ static int rdd_core(l3d_ctx* c, int n, long long nnz, const int* d_ei, const int
     const unsigned int nbn = (unsigned int)((4ll * n + 255) / 256);
     auto normalize = [&](float* Pbuf) { k_rdd_normalize_q<<<nbn, 256, 0, st>>>(n, (const int*)R.d_rowptr.p, (const int*)R.d_rp4.p, Pbuf); };
     normalize((float*)R.d_Pp.p);
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    if (kernel_ms) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, st); }
+    ScopedEvent e0, e1;
+    if (kernel_ms) {
+        if ((rc = e0.create(c)) || (rc = e1.create(c))) return rc;
+        cudaEventRecord(e0.e, st);
+    }
     float* P = (float*)R.d_Pp.p; float* Pn = (float*)R.d_Pnp.p;
     for (int it = 0; it < iters; ++it) {
         k_rdd_step8<<<(unsigned int)((nnz + 255) / 256), 256, 0, st>>>(nnz, (const int4*)R.d_plan.p, (const int*)R.d_dst.p, P, (const float*)R.d_Wp.p, Pn);
         std::swap(P, Pn);
         if (it < iters - 1) normalize(P);       // no normalisation after the last step (cudawrapper.cu:751)
     }
-    if (kernel_ms) cudaEventRecord(e1, st);
+    if (kernel_ms) cudaEventRecord(e1.e, st);
     k_rdd_unpad<<<nb, 256, 0, st>>>(nnz, (const int*)R.d_prow.p, (const int*)R.d_rowptr.p, (const int*)R.d_rp4.p, P, (float*)R.d_P.p);
     const float* result = (const float*)R.d_P.p;
     if (symmetrise) {
@@ -829,7 +790,7 @@ static int rdd_core(l3d_ctx* c, int n, long long nnz, const int* d_ei, const int
     L3D_CUDA(c, cudaMemcpyAsync(out_i, R.d_prow.p, 4 * nnz, cudaMemcpyDeviceToHost, st), "rdd download");
     L3D_CUDA(c, cudaMemcpyAsync(out_j, R.d_pcol.p, 4 * nnz, cudaMemcpyDeviceToHost, st), "rdd download");
     L3D_CUDA(c, cudaStreamSynchronize(st), "rdd");
-    if (kernel_ms) { cudaEventElapsedTime(kernel_ms, e0, e1); cudaEventDestroy(e0); cudaEventDestroy(e1); }
+    if (kernel_ms) cudaEventElapsedTime(kernel_ms, e0.e, e1.e);
     return L3D_OK;
 }
 
@@ -842,7 +803,7 @@ int l3d_rdd(l3d_ctx* c, int n, long long nnz, const int* ei, const int* ej, cons
     cudaSetDevice(c->device);
     RddState& R = c->rdd;
     int rc;
-    if ((rc = l3d_reserve(c, R.d_ei, 4 * (size_t)nnz, "rdd i")) || (rc = l3d_reserve(c, R.d_ej, 4 * (size_t)nnz, "rdd j")) || (rc = l3d_reserve(c, R.d_ew, 4 * (size_t)nnz, "rdd w"))) return rc;
+    L3D_RESERVE(R.d_ei, 4 * nnz, "rdd i"); L3D_RESERVE(R.d_ej, 4 * nnz, "rdd j"); L3D_RESERVE(R.d_ew, 4 * nnz, "rdd w");
     L3D_CUDA(c, cudaMemcpyAsync(R.d_ei.p, ei, 4 * nnz, cudaMemcpyHostToDevice, c->stream), "rdd upload");
     L3D_CUDA(c, cudaMemcpyAsync(R.d_ej.p, ej, 4 * nnz, cudaMemcpyHostToDevice, c->stream), "rdd upload");
     L3D_CUDA(c, cudaMemcpyAsync(R.d_ew.p, ew, 4 * nnz, cudaMemcpyHostToDevice, c->stream), "rdd upload");
@@ -875,18 +836,13 @@ int l3d_argsort_f32(l3d_ctx* c, long long n, const float* keys, unsigned int* pe
     cudaSetDevice(c->device);
     RddState& R = c->rdd;
     int rc;
-    if ((rc = l3d_reserve(c, R.d_ew, 4 * (size_t)n, "sort keys"))) return rc;
-    if ((rc = l3d_reserve(c, R.d_ei, 4 * (size_t)n, "sort keys"))) return rc;
-    if ((rc = l3d_reserve(c, R.d_idx, 4 * (size_t)n, "sort idx"))) return rc;
-    if ((rc = l3d_reserve(c, R.d_idx2, 4 * (size_t)n, "sort idx"))) return rc;
-    size_t sb = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, sb, (float*)nullptr, (float*)nullptr, (unsigned int*)nullptr, (unsigned int*)nullptr, (int)n, 0, 32, c->stream);
-    if ((rc = l3d_reserve(c, R.d_tmp, sb, "sort temp"))) return rc;
+    L3D_RESERVE(R.d_ew, 4 * n, "sort keys"); L3D_RESERVE(R.d_ei, 4 * n, "sort keys"); L3D_RESERVE(R.d_idx, 4 * n, "sort idx"); L3D_RESERVE(R.d_idx2, 4 * n, "sort idx");
     cudaStream_t st = c->stream;
     L3D_CUDA(c, cudaMemcpyAsync(R.d_ew.p, keys, 4 * (size_t)n, cudaMemcpyHostToDevice, st), "sort upload");
     k_iota<<<(unsigned int)((n + 255) / 256), 256, 0, st>>>(n, (unsigned int*)R.d_idx.p);
-    size_t tb = R.d_tmp.cap;
-    L3D_CUDA(c, cub::DeviceRadixSort::SortPairs(R.d_tmp.p, tb, (const float*)R.d_ew.p, (float*)R.d_ei.p, (const unsigned int*)R.d_idx.p, (unsigned int*)R.d_idx2.p, (int)n, 0, 32, st), "argsort");
+    if ((rc = l3d_cub(c, "argsort", [&](void* tmp, size_t& bytes) {
+             return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const float*)R.d_ew.p, (float*)R.d_ei.p, (const unsigned int*)R.d_idx.p, (unsigned int*)R.d_idx2.p, (int)n, 0, 32, st); })))
+        return rc;
     c->launches += 6;
     L3D_CUDA(c, cudaMemcpyAsync(perm_out, R.d_idx2.p, 4 * (size_t)n, cudaMemcpyDeviceToHost, st), "sort download");
     L3D_CUDA(c, cudaStreamSynchronize(st), "argsort");

@@ -1,7 +1,7 @@
 // l3d_capi.cu — context, device memory and the C-ABI entry points declared in include/l3d_capi.h.
 // Host C++ only orchestrates: every byte of arithmetic on the hot path runs in the kernels of l3d_match.cu /
 // l3d_pipeline.cu.  There is no CPU fallback: every entry needs a live CUDA context and fails loudly otherwise.
-#include "l3d_ctx.cuh"
+#include "l3d_cub.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_reduce.cuh>
@@ -24,15 +24,17 @@ int l3d_fail(l3d_ctx* c, int code, const char* what, cudaError_t e)
     return code;
 }
 
-int l3d_reserve(l3d_ctx* c, DevBuf& b, size_t bytes, const char* what)
+// The old allocation goes first, so that growing a large buffer never needs both sizes at once.  A failed reserve leaves the
+// buffer empty; the stage it belongs to has been dropped by the entry point that reserves it.
+int DevBuf::reserve(l3d_ctx* c, size_t bytes, const char* what)
 {
-    if (bytes <= b.cap) return L3D_OK;
-    if (b.p) { cudaFree(b.p); b.p = nullptr; b.cap = 0; }
+    if (bytes <= cap) return L3D_OK;
+    if (p) { cudaFree(p); p = nullptr; cap = 0; }
     size_t want = bytes + bytes / 8 + 256;
-    cudaError_t e = cudaMalloc(&b.p, want);
-    if (e != cudaSuccess) { e = cudaMalloc(&b.p, bytes); want = bytes; }
-    if (e != cudaSuccess) { b.p = nullptr; return l3d_fail(c, L3D_ERR_NOMEM, what, e); }
-    b.cap = want;
+    cudaError_t e = cudaMalloc(&p, want);
+    if (e != cudaSuccess) { e = cudaMalloc(&p, bytes); want = bytes; }
+    if (e != cudaSuccess) { p = nullptr; return l3d_fail(c, L3D_ERR_NOMEM, what, e); }
+    cap = want;
     return L3D_OK;
 }
 
@@ -70,8 +72,6 @@ void l3d_ctx_destroy(l3d_ctx* c)
     if (!c) return;
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
-    for (DevBuf* b : c->all_bufs()) if (b->p) cudaFree(b->p);
-    if (c->h_stage) cudaFreeHost(c->h_stage);
     for (cudaEvent_t e : c->events) cudaEventDestroy(e);
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
     cudaStreamDestroy(c->stream);
@@ -109,8 +109,8 @@ static int set_views_common(l3d_ctx* c, int V, const l3d_view_desc* views)
 static int finish_views(l3d_ctx* c)
 {
     int rc;
-    if ((rc = l3d_reserve(c, c->d_views, sizeof(L3DViewDev) * (size_t)c->num_views, "views"))) return rc;
-    if ((rc = l3d_reserve(c, c->d_cache, sizeof(float4) * 3 * (size_t)c->total_segs, "segment cache"))) return rc;
+    if ((rc = c->d_views.reserve(c, sizeof(L3DViewDev) * (size_t)c->num_views, "views"))) return rc;
+    if ((rc = c->d_cache.reserve(c, sizeof(float4) * 3 * (size_t)c->total_segs, "segment cache"))) return rc;
     L3D_CUDA(c, cudaMemcpyAsync(c->d_views.p, c->h_views.data(), sizeof(L3DViewDev) * c->num_views, cudaMemcpyHostToDevice, c->stream), "upload views");
     if (c->total_segs > 0) {
         unsigned int blocks = (unsigned int)((c->total_segs + 255) / 256);
@@ -118,35 +118,39 @@ static int finish_views(l3d_ctx* c)
         ++c->launches;
         L3D_CUDA(c, cudaGetLastError(), "k_prep_segments");
     }
-    c->have_views = true; c->have_matches = false; c->sweep.valid = false; c->collin.valid = false; c->aff.valid = false;
+    c->have_views = true;
     return L3D_OK;
 }
 
 int l3d_set_views(l3d_ctx* c, int V, const l3d_view_desc* views, const float* const* segs_host)
 {
-    if (!c || V <= 0 || !views || !segs_host) return l3d_fail(c, L3D_ERR_INVALID, "l3d_set_views: bad arguments");
+    if (!c) return L3D_ERR_INVALID;
+    c->drop(Stage::Views);
+    if (V <= 0 || !views || !segs_host) return l3d_fail(c, L3D_ERR_INVALID, "l3d_set_views: bad arguments");
     cudaSetDevice(c->device);
     int rc = set_views_common(c, V, views);
     if (rc) return rc;
     size_t bytes = sizeof(float4) * (size_t)c->total_segs;
-    if ((rc = l3d_reserve(c, c->d_segs, bytes, "segments"))) return rc;
+    if ((rc = c->d_segs.reserve(c, bytes, "segments"))) return rc;
     if (bytes > c->h_stage_cap) {           // pinned staging so the H2D is one full-speed async copy
-        if (c->h_stage) cudaFreeHost(c->h_stage);
-        c->h_stage = nullptr; c->h_stage_cap = 0;
-        L3D_CUDA(c, cudaMallocHost(&c->h_stage, bytes), "pinned staging");
-        c->h_stage_cap = bytes;
+        void* p = nullptr;
+        c->h_stage.reset(); c->h_stage_cap = 0;
+        L3D_CUDA(c, cudaMallocHost(&p, bytes), "pinned staging");
+        c->h_stage.reset(p); c->h_stage_cap = bytes;
     }
     L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync before staging");
     for (int v = 0; v < V; ++v)
-        if (views[v].nseg) memcpy((char*)c->h_stage + sizeof(float4) * c->h_views[v].seg_off, segs_host[v], sizeof(float4) * (size_t)views[v].nseg);
-    if (bytes) L3D_CUDA(c, cudaMemcpyAsync(c->d_segs.p, c->h_stage, bytes, cudaMemcpyHostToDevice, c->stream), "upload segments");
+        if (views[v].nseg) memcpy((char*)c->h_stage.get() + sizeof(float4) * c->h_views[v].seg_off, segs_host[v], sizeof(float4) * (size_t)views[v].nseg);
+    if (bytes) L3D_CUDA(c, cudaMemcpyAsync(c->d_segs.p, c->h_stage.get(), bytes, cudaMemcpyHostToDevice, c->stream), "upload segments");
     c->segs_ext = nullptr;
     return finish_views(c);
 }
 
 int l3d_set_views_flat(l3d_ctx* c, int V, const l3d_view_desc* views, const float* segs_flat, int on_device)
 {
-    if (!c || V <= 0 || !views || !segs_flat) return l3d_fail(c, L3D_ERR_INVALID, "l3d_set_views_flat: bad arguments");
+    if (!c) return L3D_ERR_INVALID;
+    c->drop(Stage::Views);
+    if (V <= 0 || !views || !segs_flat) return l3d_fail(c, L3D_ERR_INVALID, "l3d_set_views_flat: bad arguments");
     cudaSetDevice(c->device);
     int rc = set_views_common(c, V, views);
     if (rc) return rc;
@@ -155,25 +159,28 @@ int l3d_set_views_flat(l3d_ctx* c, int V, const l3d_view_desc* views, const floa
         if (((uintptr_t)segs_flat & 15) != 0) return l3d_fail(c, L3D_ERR_INVALID, "l3d_set_views_flat: device array must be 16-byte aligned");
         c->segs_ext = (const float4*)segs_flat;
     } else {
-        if ((rc = l3d_reserve(c, c->d_segs, bytes, "segments"))) return rc;
+        if ((rc = c->d_segs.reserve(c, bytes, "segments"))) return rc;
         if (bytes) L3D_CUDA(c, cudaMemcpyAsync(c->d_segs.p, segs_flat, bytes, cudaMemcpyHostToDevice, c->stream), "upload segments");
         c->segs_ext = nullptr;
     }
     return finish_views(c);
 }
 
+// new camera blocks for the same views: the matches and the sweep stay usable, the affinity matrix is recomputed
 int l3d_update_view_params(l3d_ctx* c, int V, const l3d_view_desc* views)
 {
-    if (!c || !views || V != c->num_views || !c->have_views) return l3d_fail(c, L3D_ERR_STATE, "l3d_update_view_params: views not set / count mismatch");
+    if (!c) return L3D_ERR_INVALID;
+    c->drop(Stage::Affinity);
+    if (!views || V != c->num_views || !c->have_views) return l3d_fail(c, L3D_ERR_STATE, "l3d_update_view_params: views not set / count mismatch");
     cudaSetDevice(c->device);
+    L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync before view update");
     for (int v = 0; v < V; ++v) {
         L3DViewDev& d = c->h_views[v];
         memcpy(d.RtKinv_d, views[v].RtKinv_d, sizeof(d.RtKinv_d)); memcpy(d.C_d, views[v].C_d, sizeof(d.C_d));
         d.k = views[v].k; d.median_depth = views[v].median_depth;
     }
-    c->aff.valid = false;
-    L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync before view update");
-    L3D_CUDA(c, cudaMemcpyAsync(c->d_views.p, c->h_views.data(), sizeof(L3DViewDev) * V, cudaMemcpyHostToDevice, c->stream), "upload views");
+    const cudaError_t e = cudaMemcpyAsync(c->d_views.p, c->h_views.data(), sizeof(L3DViewDev) * V, cudaMemcpyHostToDevice, c->stream);
+    if (e != cudaSuccess) { c->drop(Stage::Views); return l3d_fail(c, L3D_ERR_CUDA, "upload views", e); }   // host and device views differ
     return L3D_OK;
 }
 
@@ -189,18 +196,11 @@ int l3d_match_pairs_range(l3d_ctx* c, int num_pairs, const int32_t* pairs, const
 { return match_impl(c, num_pairs, pairs, F, nullptr, epi_overlap, knn, first_pair, last_pair); }
 
 int l3d_match_pairs_f64(l3d_ctx* c, int num_pairs, const int32_t* pairs, const double* Fd, float epi_overlap, int knn, int first_pair, int last_pair)
-{
-    if (!c) return L3D_ERR_INVALID;
-    if (num_pairs > 0 && !Fd) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs_f64: bad arguments");
-    return match_impl(c, num_pairs, pairs, nullptr, Fd, epi_overlap, knn, first_pair, last_pair);
-}
+{ return match_impl(c, num_pairs, pairs, nullptr, Fd, epi_overlap, knn, first_pair, last_pair); }
 
 int l3d_match_pairs_host(l3d_ctx* c, int num_pairs, const int32_t* pairs, const float* F, float epi_overlap, int knn, int32_t* counts_out,
                          l3d_match_rec* recs_out, int chunks)
 {
-    if (!c) return L3D_ERR_INVALID;
-    if (!counts_out || !recs_out || chunks < 1) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs_host: bad arguments");
-    if (knn <= 0) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs_host: kNN <= 0 has no fixed row stride; use l3d_match_pairs + l3d_get_pair_matches");
     HostOut h = {counts_out, recs_out, std::min(chunks, 64)};
     return match_impl(c, num_pairs, pairs, F, nullptr, epi_overlap, knn, 0, num_pairs, &h);
 }
@@ -209,6 +209,9 @@ static int match_impl(l3d_ctx* c, int num_pairs, const int32_t* pairs, const flo
                       const HostOut* host)
 {
     if (!c) return L3D_ERR_INVALID;
+    c->drop(Stage::Matches);
+    if (host && (!host->counts || !host->recs || host->chunks < 1)) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs_host: bad arguments");
+    if (host && knn <= 0) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs_host: kNN <= 0 has no fixed row stride; use l3d_match_pairs + l3d_get_pair_matches");
     if (!c->have_views) return l3d_fail(c, L3D_ERR_STATE, "l3d_match_pairs: call l3d_set_views first");
     if (num_pairs < 0 || (num_pairs && (!pairs || (!F && !Fd)))) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs: bad arguments");
     if (first_pair < 0 || last_pair < first_pair || last_pair > num_pairs) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs_range: bad pair range");
@@ -242,12 +245,12 @@ static int match_impl(l3d_ctx* c, int num_pairs, const int32_t* pairs, const flo
     }
     c->num_pairs = num_pairs; c->knn = knn; c->epi = epi_overlap; c->total_rows = rows; c->pair_evals = evals;
     int rc;
-    if ((rc = l3d_reserve(c, c->d_pairs, sizeof(L3DPairDev) * (size_t)std::max(num_pairs, 1), "pairs"))) return rc;
-    if ((rc = l3d_reserve(c, c->d_tiles, sizeof(int2) * std::max<size_t>(c->h_tiles.size(), 1), "tiles"))) return rc;
-    if ((rc = l3d_reserve(c, c->d_arcs, sizeof(uint4) * (size_t)std::max<long long>(narcs, 1), "target arcs"))) return rc;
-    if ((rc = l3d_reserve(c, c->d_basis, sizeof(L3DPairBasis) * (size_t)std::max(num_pairs, 1), "pair bases"))) return rc;
-    if ((rc = l3d_reserve(c, c->d_counts, sizeof(int) * (size_t)std::max<long long>(rows, 1), "match counts"))) return rc;
-    if (!keep_all && (rc = l3d_reserve(c, c->d_recs, sizeof(l3d_match_rec) * (size_t)std::max<long long>(rows, 1) * knn, "match records"))) return rc;
+    L3D_RESERVE(c->d_pairs, sizeof(L3DPairDev) * (size_t)std::max(num_pairs, 1), "pairs");
+    L3D_RESERVE(c->d_tiles, sizeof(int2) * std::max<size_t>(c->h_tiles.size(), 1), "tiles");
+    L3D_RESERVE(c->d_arcs, sizeof(uint4) * (size_t)std::max<long long>(narcs, 1), "target arcs");
+    L3D_RESERVE(c->d_basis, sizeof(L3DPairBasis) * (size_t)std::max(num_pairs, 1), "pair bases");
+    L3D_RESERVE(c->d_counts, sizeof(int) * (size_t)std::max<long long>(rows, 1), "match counts");
+    if (!keep_all) L3D_RESERVE(c->d_recs, sizeof(l3d_match_rec) * (size_t)std::max<long long>(rows, 1) * knn, "match records");
     if (num_pairs) L3D_CUDA(c, cudaMemcpyAsync(c->d_pairs.p, c->h_pairs.data(), sizeof(L3DPairDev) * num_pairs, cudaMemcpyHostToDevice, c->stream), "upload pairs");
     if (!c->h_tiles.empty()) L3D_CUDA(c, cudaMemcpyAsync(c->d_tiles.p, c->h_tiles.data(), sizeof(int2) * c->h_tiles.size(), cudaMemcpyHostToDevice, c->stream), "upload tiles");
     if (rows) L3D_CUDA(c, cudaMemsetAsync(c->d_counts.p, 0, sizeof(int) * rows, c->stream), "clear counts");   // rows of pairs with Nt == 0
@@ -261,17 +264,15 @@ static int match_impl(l3d_ctx* c, int num_pairs, const int32_t* pairs, const flo
         const bool on = epi_overlap >= 0.01f && getenv("L3D_NO_LEVEL1") == nullptr;
         int end_bit = 36;                       // key = pair << 36 | class << 32 | start of the arc
         while (end_bit < 64 && (1ll << (end_bit - 36)) < npr) ++end_bit;
-        size_t tb = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, tb, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (const unsigned int*)nullptr, (unsigned int*)nullptr, (int)narcs, 0, end_bit, c->stream);
-        if ((rc = l3d_reserve(c, c->d_arcraw, 16 * (size_t)narcs, "raw arcs")) || (rc = l3d_reserve(c, c->d_arckeys, 8 * (size_t)narcs, "arc keys")) ||
-            (rc = l3d_reserve(c, c->d_arckeys2, 8 * (size_t)narcs, "arc keys")) || (rc = l3d_reserve(c, c->d_arcvals, 4 * (size_t)narcs, "arc order")) ||
-            (rc = l3d_reserve(c, c->d_arcvals2, 4 * (size_t)narcs, "arc order")) || (rc = l3d_reserve(c, c->d_arctmp, tb, "arc sort temp"))) return rc;
+        L3D_RESERVE(c->d_arcraw, 16 * narcs, "raw arcs"); L3D_RESERVE(c->d_arckeys, 8 * narcs, "arc keys"); L3D_RESERVE(c->d_arckeys2, 8 * narcs, "arc keys");
+        L3D_RESERVE(c->d_arcvals, 4 * narcs, "arc order"); L3D_RESERVE(c->d_arcvals2, 4 * narcs, "arc order");
         k_pair_arcs<<<(unsigned int)npr, 256, 0, c->stream>>>(c->segs(), c->views(), (const L3DPairDev*)c->d_pairs.p, first_pair, on ? 1 : 0,
                                                              1.0 / (double)std::max(epi_overlap, 0.01f) + 0.5, (uint4*)c->d_arcraw.p,
                                                              (unsigned long long*)c->d_arckeys.p, (unsigned int*)c->d_arcvals.p, (L3DPairBasis*)c->d_basis.p);
         L3D_CUDA(c, cudaGetLastError(), "k_pair_arcs");
-        L3D_CUDA(c, cub::DeviceRadixSort::SortPairs(c->d_arctmp.p, tb, (const unsigned long long*)c->d_arckeys.p, (unsigned long long*)c->d_arckeys2.p,
-                                                    (const unsigned int*)c->d_arcvals.p, (unsigned int*)c->d_arcvals2.p, (int)narcs, 0, end_bit, c->stream), "arc sort");
+        if ((rc = l3d_cub(c, "arc sort", [&](void* tmp, size_t& bytes) {
+                 return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const unsigned long long*)c->d_arckeys.p, (unsigned long long*)c->d_arckeys2.p,
+                                                        (const unsigned int*)c->d_arcvals.p, (unsigned int*)c->d_arcvals2.p, (int)narcs, 0, end_bit, c->stream); }))) return rc;
         k_arcs_gather<<<(unsigned int)((narcs + 255) / 256), 256, 0, c->stream>>>(narcs, (const unsigned long long*)c->d_arckeys2.p, (const unsigned int*)c->d_arcvals2.p,
                                                                                  (const uint4*)c->d_arcraw.p, (const L3DPairDev*)c->d_pairs.p, first_pair, (uint4*)c->d_arcs.p);
         L3D_CUDA(c, cudaGetLastError(), "k_arcs_gather");
@@ -279,7 +280,7 @@ static int match_impl(l3d_ctx* c, int num_pairs, const int32_t* pairs, const flo
     }
     const double* cache_d = nullptr;
     if (Fd && c->total_segs > 0) {      // matchingCPU's rays / plane normals in double; camera blocks may have been updated since set_views
-        if ((rc = l3d_reserve(c, c->d_cache_d, sizeof(double) * 9 * (size_t)c->total_segs, "double segment cache"))) return rc;
+        L3D_RESERVE(c->d_cache_d, sizeof(double) * 9 * (size_t)c->total_segs, "double segment cache");
         k_prep_segments_f64<<<(unsigned int)((c->total_segs + 255) / 256), 256, 0, c->stream>>>(c->segs(), c->views(), c->num_views, c->total_segs, (double*)c->d_cache_d.p);
         ++c->launches;
         L3D_CUDA(c, cudaGetLastError(), "k_prep_segments_f64");
@@ -295,20 +296,18 @@ static int match_impl(l3d_ctx* c, int num_pairs, const int32_t* pairs, const flo
                 epi_overlap, (int*)c->d_counts.p, nullptr, cache_d, arcs, basis);
             ++c->launches;
             L3D_CUDA(c, cudaGetLastError(), "k_match_all (count)");
-            size_t tb = 0;
-            cub::DeviceReduce::Max(nullptr, tb, (const int*)c->d_counts.p, (int*)nullptr, (int)std::min<long long>(rows, INT_MAX), c->stream);
             if (rows > INT_MAX) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: more than 2^31 rows with kNN <= 0");
-            if ((rc = l3d_reserve(c, c->d_scan_tmp, tb, "reduce temp"))) return rc;
-            if ((rc = l3d_reserve(c, c->d_rowptr, 16, "row max"))) return rc;
+            L3D_RESERVE(c->d_rowptr, 16, "row max");
             int* d_max = (int*)c->d_rowptr.p;
-            L3D_CUDA(c, cub::DeviceReduce::Max(c->d_scan_tmp.p, tb, (const int*)c->d_counts.p, d_max, (int)rows, c->stream), "row maximum");
+            if ((rc = l3d_cub(c, "row maximum", [&](void* tmp, size_t& bytes) {
+                     return cub::DeviceReduce::Max(tmp, bytes, (const int*)c->d_counts.p, d_max, (int)rows, c->stream); }))) return rc;
             c->launches += 1;
             L3D_CUDA(c, cudaMemcpyAsync(&stride, d_max, sizeof(int), cudaMemcpyDeviceToHost, c->stream), "row maximum");
             L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync");
             stride = std::max(stride, 1);
         }
         knn = stride; c->knn = stride;
-        if ((rc = l3d_reserve(c, c->d_recs, sizeof(l3d_match_rec) * (size_t)std::max<long long>(rows, 1) * stride, "match records"))) return rc;
+        L3D_RESERVE(c->d_recs, sizeof(l3d_match_rec) * (size_t)std::max<long long>(rows, 1) * stride, "match records");
         if (!c->h_tiles.empty()) {
             const size_t per_warp = sizeof(l3d_match_rec) * (size_t)stride;
             int wpb = 4;
@@ -369,7 +368,7 @@ static int match_impl(l3d_ctx* c, int num_pairs, const int32_t* pairs, const flo
             L3D_CUDA(c, cudaStreamWaitEvent(c->stream, c->events[chunks], 0), "event wait");
         }
     }
-    c->have_matches = true; c->sweep.valid = false;
+    c->have_matches = true;
     return L3D_OK;
 }
 
@@ -378,7 +377,7 @@ int l3d_match_device_buffers(l3d_ctx* c, void** counts_dev, void** recs_dev)
     if (!c || !counts_dev || !recs_dev) return L3D_ERR_INVALID;
     if (!c->have_matches) return l3d_fail(c, L3D_ERR_STATE, "l3d_match_device_buffers: no match result");
     *counts_dev = c->d_counts.p; *recs_dev = c->d_recs.p;
-    c->sweep.valid = false;                 // the caller may overwrite rows
+    c->drop(Stage::Sweep);                  // the caller may overwrite rows
     return L3D_OK;
 }
 
@@ -440,15 +439,12 @@ long long l3d_match_total_matches(l3d_ctx* c)
     int rc;
     long long total = 0;
     const long long BLK = 1ll << 30;
-    if ((rc = l3d_reserve(c, c->d_rowptr, 16, "match total"))) return rc;
+    L3D_RESERVE(c->d_rowptr, 16, "match total");
     for (long long base = 0; base < c->total_rows; base += BLK) {
         const int n = (int)std::min(BLK, c->total_rows - base);
-        size_t tb = 0;
-        cub::DeviceReduce::Sum(nullptr, tb, (const int*)c->d_counts.p + base, (long long*)c->d_rowptr.p, n, c->stream);
-        if ((rc = l3d_reserve(c, c->d_scan_tmp, tb, "reduce temp"))) return rc;
-        tb = c->d_scan_tmp.cap;
         long long part = 0;
-        L3D_CUDA(c, cub::DeviceReduce::Sum(c->d_scan_tmp.p, tb, (const int*)c->d_counts.p + base, (long long*)c->d_rowptr.p, n, c->stream), "match total");
+        if ((rc = l3d_cub(c, "match total", [&](void* tmp, size_t& bytes) {
+                 return cub::DeviceReduce::Sum(tmp, bytes, (const int*)c->d_counts.p + base, (long long*)c->d_rowptr.p, n, c->stream); }))) return rc;
         L3D_CUDA(c, cudaMemcpyAsync(&part, c->d_rowptr.p, 8, cudaMemcpyDeviceToHost, c->stream), "match total");
         L3D_CUDA(c, cudaStreamSynchronize(c->stream), "match total");
         total += part;
@@ -480,21 +476,15 @@ long long l3d_get_matches_csr(l3d_ctx* c, int64_t* row_ptr_out, l3d_match_rec* r
     const long long rows = c->total_rows;
     if (rows == 0) { row_ptr_out[0] = 0; return 0; }
     int rc;
-    if ((rc = l3d_reserve(c, c->d_rowptr, sizeof(long long) * (size_t)(rows + 1), "row_ptr"))) return rc;
+    L3D_RESERVE(c->d_rowptr, sizeof(long long) * (size_t)(rows + 1), "row_ptr");
     cub::TransformInputIterator<long long, CastI64, const int*> in((const int*)c->d_counts.p, CastI64());
-    size_t tmp_bytes = 0;
-    // rows+1 items: the element past the end is never read by an exclusive scan's last output
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, in, (long long*)c->d_rowptr.p, rows, c->stream);
-    if ((rc = l3d_reserve(c, c->d_scan_tmp, tmp_bytes, "scan temp"))) return rc;
-    L3D_CUDA(c, cub::DeviceScan::ExclusiveSum(c->d_scan_tmp.p, tmp_bytes, in, (long long*)c->d_rowptr.p, rows, c->stream), "row_ptr scan");
+    ScanTotal t;
+    if ((rc = l3d_scan_total(c, in, (long long*)c->d_rowptr.p, rows, (const int*)c->d_counts.p, t, "row_ptr scan"))) return rc;
     c->launches += 2;   // cub: decoupled look-back init + scan kernels
-    long long last_ptr = 0; int last_cnt = 0;
-    L3D_CUDA(c, cudaMemcpyAsync(&last_ptr, (const long long*)c->d_rowptr.p + rows - 1, sizeof(long long), cudaMemcpyDeviceToHost, c->stream), "read total");
-    L3D_CUDA(c, cudaMemcpyAsync(&last_cnt, (const int*)c->d_counts.p + rows - 1, sizeof(int), cudaMemcpyDeviceToHost, c->stream), "read total");
     L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync");
-    const long long total = last_ptr + last_cnt;
+    const long long total = t.last_out + t.last_src;
     L3D_CUDA(c, cudaMemcpyAsync((long long*)c->d_rowptr.p + rows, &total, sizeof(long long), cudaMemcpyHostToDevice, c->stream), "write total");
-    if ((rc = l3d_reserve(c, c->d_csr, sizeof(l3d_match_rec) * (size_t)std::max<long long>(total, 1), "csr records"))) return rc;
+    L3D_RESERVE(c->d_csr, sizeof(l3d_match_rec) * (size_t)std::max<long long>(total, 1), "csr records");
     long long cells = rows * c->knn;
     k_compact_matches<<<(unsigned int)((cells + 255) / 256), 256, 0, c->stream>>>((const int*)c->d_counts.p, (const long long*)c->d_rowptr.p,
                                                                                    (const l3d_match_rec*)c->d_recs.p, c->knn, rows, (l3d_match_rec*)c->d_csr.p);
@@ -521,8 +511,8 @@ static int match_dense_impl(l3d_ctx* c, int sv, int tv, const float* F, float ep
     float4* d_dep = (float4*)depths; float* d_ov = overlaps;
     if (!on_dev) {
         int rc;
-        if ((rc = l3d_reserve(c, c->d_dense_dep, sizeof(float4) * cells, "dense depths"))) return rc;
-        if ((rc = l3d_reserve(c, c->d_dense_ov, sizeof(float) * cells, "dense overlaps"))) return rc;
+        L3D_RESERVE(c->d_dense_dep, sizeof(float4) * cells, "dense depths");
+        L3D_RESERVE(c->d_dense_ov, sizeof(float) * cells, "dense overlaps");
         d_dep = (float4*)c->d_dense_dep.p; d_ov = (float*)c->d_dense_ov.p;
     }
     L3DMat3 Fm; memcpy(Fm.m, F, sizeof(Fm.m));
@@ -551,22 +541,21 @@ int l3d_fp32_peak_probe(l3d_ctx* c, double* tflops_out)
     if (!c || !tflops_out) return L3D_ERR_INVALID;
     cudaSetDevice(c->device);
     int rc;
-    if ((rc = l3d_reserve(c, c->d_scan_tmp, 256, "probe"))) return rc;
+    L3D_RESERVE(c->cub_tmp, 256, "probe");      // result sink
     const int iters = 4096, blocks = c->num_sms * 8;
-    cudaEvent_t e0, e1;
-    L3D_CUDA(c, cudaEventCreate(&e0), "event"); L3D_CUDA(c, cudaEventCreate(&e1), "event");
+    ScopedEvent e0, e1;
+    if ((rc = e0.create(c)) || (rc = e1.create(c))) return rc;
     double best = 0.0;
     for (int rep = 0; rep < 5; ++rep) {
-        cudaEventRecord(e0, c->stream);
-        k_fp32_peak<<<blocks, 256, 0, c->stream>>>((float*)c->d_scan_tmp.p, iters, 1.0000001f, 1e-9f);
-        cudaEventRecord(e1, c->stream);
+        cudaEventRecord(e0.e, c->stream);
+        k_fp32_peak<<<blocks, 256, 0, c->stream>>>((float*)c->cub_tmp.p, iters, 1.0000001f, 1e-9f);
+        cudaEventRecord(e1.e, c->stream);
         ++c->launches;
         L3D_CUDA(c, cudaStreamSynchronize(c->stream), "k_fp32_peak");
-        float ms = 0.f; cudaEventElapsedTime(&ms, e0, e1);
+        float ms = 0.f; cudaEventElapsedTime(&ms, e0.e, e1.e);
         double tf = 2.0 * 16.0 * iters * 256.0 * blocks / (ms * 1e-3) / 1e12;
         if (rep > 0 && tf > best) best = tf;
     }
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
     *tflops_out = best;
     return L3D_OK;
 }
@@ -604,7 +593,7 @@ int l3d_match_dense_pairs(l3d_ctx* c, int npairs, const int32_t* pairs, const fl
     if (jobs.empty()) return L3D_OK;
     if (tiles >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_dense_pairs: more than 2^31 tiles");
     int rc;
-    if ((rc = l3d_reserve(c, c->d_dense_jobs, sizeof(L3DDenseJob) * jobs.size(), "dense jobs"))) return rc;
+    L3D_RESERVE(c->d_dense_jobs, sizeof(L3DDenseJob) * jobs.size(), "dense jobs");
     L3D_CUDA(c, cudaMemcpyAsync(c->d_dense_jobs.p, jobs.data(), sizeof(L3DDenseJob) * jobs.size(), cudaMemcpyHostToDevice, c->stream), "dense jobs");
     L3D_CUDA(c, cudaStreamSynchronize(c->stream), "dense jobs");       // `jobs` is a local
     k_match_dense_batch<<<(unsigned int)tiles, DK_THREADS, l3d_dense_smem_bytes(), c->stream>>>((const L3DDenseJob*)c->d_dense_jobs.p, (int)jobs.size(), epi);

@@ -15,9 +15,7 @@
 // two segments (the four on-segment tests are OR-ed, the distances max-ed), so evaluating (row, column) instead of the
 // kernel's (max index, min index) gives the same bit.  The pre-filter only rejects cells whose FIRST point-to-line
 // distance provably exceeds the threshold (0.01 % margin >> the 2^-23 rounding of the divide), which forces a zero.
-#include "l3d_ctx.cuh"
-
-#include <cub/device/device_scan.cuh>
+#include "l3d_cub.cuh"
 
 #define CL_WARPS 8
 #define CL_RPW 4
@@ -130,22 +128,24 @@ extern "C" {
 int l3d_find_collinear(l3d_ctx* c, float dist_t, int semantics)
 {
     if (!c) return L3D_ERR_INVALID;
-    if (!c->have_views) return l3d_fail(c, L3D_ERR_STATE, "l3d_find_collinear: call l3d_set_views first");
-    if (semantics != L3D_SEM_REF_GPU && semantics != L3D_SEM_REF_CPU) return l3d_fail(c, L3D_ERR_INVALID, "l3d_find_collinear: bad semantics");
-    cudaSetDevice(c->device);
     CollinState& K = c->collin;
-    if (!(dist_t > 1e-12f)) { if (K.valid) c->aff.valid = false; K.valid = false; K.dist_t = 0.0f; return L3D_OK; }
-    if (K.valid && K.dist_t == dist_t && K.sem == semantics) return L3D_OK;            // already computed (view.cc:154-158)
-    K.valid = false; c->aff.valid = false;
+    const bool off = !(dist_t > 1e-12f);
+    const bool sem_ok = semantics == L3D_SEM_REF_GPU || semantics == L3D_SEM_REF_CPU;
+    // already off, or already computed (view.cc:154-158): the lists and the affinity matrix built on them stay
+    const bool unchanged = sem_ok && (off ? !K.valid : K.valid && K.dist_t == dist_t && K.sem == semantics);
+    if (!unchanged) c->drop(Stage::Collinear);
+    if (!c->have_views) return l3d_fail(c, L3D_ERR_STATE, "l3d_find_collinear: call l3d_set_views first");
+    if (!sem_ok) return l3d_fail(c, L3D_ERR_INVALID, "l3d_find_collinear: bad semantics");
+    if (off || unchanged) return L3D_OK;
+    cudaSetDevice(c->device);
     const long long N = c->total_segs;
     if (N == 0) { K.total = 0; K.valid = true; K.dist_t = dist_t; K.sem = semantics; return L3D_OK; }
     std::vector<int2> tiles;
     for (int v = 0; v < c->num_views; ++v)
         for (int r = 0; r < c->h_views[v].nseg; r += CL_ROWS) tiles.push_back(make_int2(v, r));
     int rc;
-    if ((rc = l3d_reserve(c, K.d_tiles, sizeof(int2) * tiles.size(), "collinear tiles"))) return rc;
-    if ((rc = l3d_reserve(c, K.d_cnt, 4 * (size_t)(N + 1), "collinear counts"))) return rc;
-    if ((rc = l3d_reserve(c, K.d_ptr, 8 * (size_t)(N + 1), "collinear offsets"))) return rc;
+    L3D_RESERVE(K.d_tiles, sizeof(int2) * tiles.size(), "collinear tiles");
+    L3D_RESERVE(K.d_cnt, 4 * (N + 1), "collinear counts"); L3D_RESERVE(K.d_ptr, 8 * (N + 1), "collinear offsets");
     cudaStream_t st = c->stream;
     L3D_CUDA(c, cudaMemcpyAsync(K.d_tiles.p, tiles.data(), sizeof(int2) * tiles.size(), cudaMemcpyHostToDevice, st), "collinear tiles");
     L3D_CUDA(c, cudaMemsetAsync(K.d_cnt.p, 0, 4 * (size_t)(N + 1), st), "collinear counts");
@@ -154,15 +154,12 @@ int l3d_find_collinear(l3d_ctx* c, float dist_t, int semantics)
         k_collinear<false, true><<<nb, 32 * CL_WARPS, 0, st>>>(c->segs(), c->views(), (const int2*)K.d_tiles.p, dist_t, (int*)K.d_cnt.p, nullptr, nullptr);
     else
         k_collinear<false, false><<<nb, 32 * CL_WARPS, 0, st>>>(c->segs(), c->views(), (const int2*)K.d_tiles.p, dist_t, (int*)K.d_cnt.p, nullptr, nullptr);
-    size_t tb = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, tb, (const int*)nullptr, (long long*)nullptr, N + 1, st);
-    if ((rc = l3d_reserve(c, K.d_tmp, tb, "collinear scan temp"))) return rc;
-    tb = K.d_tmp.cap;
-    L3D_CUDA(c, cub::DeviceScan::ExclusiveSum(K.d_tmp.p, tb, (const int*)K.d_cnt.p, (long long*)K.d_ptr.p, N + 1, st), "collinear scan");
+    if ((rc = l3d_cub(c, "collinear scan", [&](void* tmp, size_t& bytes) {
+             return cub::DeviceScan::ExclusiveSum(tmp, bytes, (const int*)K.d_cnt.p, (long long*)K.d_ptr.p, N + 1, st); }))) return rc;
     long long total = 0;
     L3D_CUDA(c, cudaMemcpyAsync(&total, (long long*)K.d_ptr.p + N, 8, cudaMemcpyDeviceToHost, st), "collinear total");
     L3D_CUDA(c, cudaStreamSynchronize(st), "collinear count");
-    if ((rc = l3d_reserve(c, K.d_idx, 4 * (size_t)std::max<long long>(total, 1), "collinear lists"))) return rc;
+    L3D_RESERVE(K.d_idx, 4 * total, "collinear lists");
     if (total > 0) {
         if (semantics == L3D_SEM_REF_CPU)
             k_collinear<true, true><<<nb, 32 * CL_WARPS, 0, st>>>(c->segs(), c->views(), (const int2*)K.d_tiles.p, dist_t, nullptr, (const long long*)K.d_ptr.p, (int*)K.d_idx.p);

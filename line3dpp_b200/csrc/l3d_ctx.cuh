@@ -2,10 +2,23 @@
 #pragma once
 #include "l3d_match.cuh"
 
+#include <algorithm>
+#include <memory>
 #include <string>
+#include <utility>
 #include <vector>
 
-struct DevBuf { void* p = nullptr; size_t cap = 0; };   // grow-only device allocation
+// grow-only device allocation, freed with its owner
+struct DevBuf {
+    void* p = nullptr; size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    DevBuf(DevBuf&& o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+    DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
+    ~DevBuf() { if (p) cudaFree(p); }
+    int reserve(l3d_ctx* c, size_t bytes, const char* what);
+};
 
 // state of the per-view scoring sweep (l3d_pipeline.cu)
 struct SweepState {
@@ -16,49 +29,41 @@ struct SweepState {
     long long total = 0;
     // match store (l3d_sweep.cuh): view table, chunk descriptors, chunk offsets, entries
     DevBuf d_vt, d_vp, d_pairc, d_rowoff, d_pinfo, d_bpair, d_ekv, d_rays, d_rmf, d_rflag, d_invpos, d_csize, d_ccur, d_cstart, d_eval, d_escore, d_eflag, d_gstage, d_gpub, d_dir64, d_export, d_export_ok,
-        d_ranges, d_est_best, d_est_P, d_M, d_vmax, d_sort_tmp, d_aff_sim, d_aff_flag, d_aff_gi, d_aff_gj, d_aff_pos, d_aff_oi, d_aff_oj,
-        d_aff_ow, d_kx, d_order, d_rankofview, d_region_off, d_est_pos, d_est_out_best, d_est_out_P, d_segrank_off, d_evcnt, d_evptr, d_aff_par;
-    long long n_est = 0, n_kept = 0;
+        d_ranges, d_est_best, d_est_P, d_M, d_vmax, d_order, d_region_off, d_est_pos, d_est_out_best, d_est_out_P;
+    long long n_est = 0;
     float ms_setup = 0.f, ms_chain = 0.f, ms_filter = 0.f;   // device time of the last sweep's three phases
-    bool aff_has_parents = false;           // d_aff_par valid: candidates carry parents (collinearity links)
-    std::vector<DevBuf*> bufs()
-    { return {&d_vt, &d_vp, &d_pairc, &d_rowoff, &d_pinfo, &d_bpair, &d_ekv, &d_rays, &d_rmf, &d_rflag, &d_invpos, &d_csize, &d_ccur, &d_cstart, &d_eval, &d_escore, &d_eflag, &d_gstage, &d_gpub, &d_dir64,
-              &d_export, &d_export_ok, &d_ranges, &d_est_best, &d_est_P, &d_M, &d_vmax, &d_sort_tmp, &d_aff_sim, &d_aff_flag, &d_aff_gi, &d_aff_gj,
-              &d_aff_pos, &d_aff_oi, &d_aff_oj, &d_aff_ow, &d_kx, &d_order, &d_rankofview, &d_region_off, &d_est_pos,
-              &d_est_out_best, &d_est_out_P, &d_segrank_off, &d_evcnt, &d_evptr, &d_aff_par}; }
 };
 
 // device state of the affinity-matrix bookkeeping (l3d_affinity.cu)
 struct AffinityState {
     bool valid = false; float two_sigA_sqr = 0.f, med = 0.f, min_aff = 0.f; long long K = 0, n_ids = 0;
+    // candidate edges of the kept matches (affinity_candidates)
+    DevBuf d_aff_sim, d_aff_flag, d_aff_gi, d_aff_gj, d_aff_pos, d_aff_oi, d_aff_oj, d_aff_ow, d_aff_par, d_kx, d_rankofview, d_segrank_off, d_evcnt, d_evptr;
+    long long n_kept = 0;
+    bool aff_has_parents = false;           // d_aff_par valid: candidates carry parents (collinearity links)
     DevBuf d_key, d_key2, d_val, d_val2, d_keep, d_keep2, d_found, d_changed, d_q, d_time, d_nflag, d_npos, d_idof, d_nkey, d_nkey2, d_nval, d_nval2, d_l2g, d_ei, d_ej, d_ew;
-    std::vector<DevBuf*> bufs()
-    { return {&d_key, &d_key2, &d_val, &d_val2, &d_keep, &d_keep2, &d_found, &d_changed, &d_q, &d_time, &d_nflag, &d_npos, &d_idof, &d_nkey, &d_nkey2, &d_nval, &d_nval2, &d_l2g,
-              &d_ei, &d_ej, &d_ew}; }
 };
 
 // per-view lists of potentially collinear segments (l3d_collinear.cu), CSR over the global segment index
 struct CollinState {
     bool valid = false; float dist_t = 0.f; int sem = 0; long long total = 0;
-    DevBuf d_tiles, d_cnt, d_ptr, d_idx, d_tmp;
-    std::vector<DevBuf*> bufs() { return {&d_tiles, &d_cnt, &d_ptr, &d_idx, &d_tmp}; }
+    DevBuf d_tiles, d_cnt, d_ptr, d_idx;
 };
 
 // device state of the line bundling (l3d_optimize.cu)
 struct OptState {
     DevBuf d_p, d_pout, d_valid, d_resptr, d_rescam, d_resxy, d_obs, d_cams, d_x, d_xc, d_g, d_H, d_S, d_diag, d_free, d_part, d_tot;
-    std::vector<DevBuf*> bufs()
-    { return {&d_p, &d_pout, &d_valid, &d_resptr, &d_rescam, &d_resxy, &d_obs, &d_cams, &d_x, &d_xc, &d_g, &d_H, &d_S, &d_diag, &d_free, &d_part, &d_tot}; }
 };
 
 // device buffers of the diffusion (l3d_affinity.cu)
 struct RddState {
-    DevBuf d_ei, d_ej, d_ew, d_krow, d_kcol, d_k2, d_idx, d_idx2, d_P, d_Pn, d_W, d_prow, d_pcol, d_wmaj, d_wmin, d_rowptr, d_colptr, d_tslot, d_tmp, d_len4, d_rp4, d_cp4,
+    DevBuf d_ei, d_ej, d_ew, d_krow, d_kcol, d_k2, d_idx, d_idx2, d_P, d_Pn, d_W, d_prow, d_pcol, d_wmaj, d_wmin, d_rowptr, d_colptr, d_tslot, d_len4, d_rp4, d_cp4,
         d_Pp, d_Pnp, d_Wp, d_plan, d_dst;
-    std::vector<DevBuf*> bufs()
-    { return {&d_ei, &d_ej, &d_ew, &d_krow, &d_kcol, &d_k2, &d_idx, &d_idx2, &d_P, &d_Pn, &d_W, &d_prow, &d_pcol, &d_wmaj, &d_wmin, &d_rowptr,
-              &d_colptr, &d_tslot, &d_tmp, &d_len4, &d_rp4, &d_cp4, &d_Pp, &d_Pnp, &d_Wp, &d_plan, &d_dst}; }
 };
+
+// The results a context holds, each computed from the ones before it:
+//   Views -> Matches -> Sweep -> Affinity,   Views -> Collinear -> Affinity
+enum class Stage { Views, Matches, Sweep, Collinear, Affinity };
 
 struct l3d_ctx {
     int device = 0, num_sms = 0;
@@ -66,6 +71,7 @@ struct l3d_ctx {
     std::vector<cudaEvent_t> events;
     std::string err;
     long long launches = 0;
+    DevBuf cub_tmp;                         // temporary storage of every cub call (all on `stream`, one at a time)
 
     // views
     bool have_views = false;
@@ -74,7 +80,8 @@ struct l3d_ctx {
     std::vector<L3DViewDev> h_views;
     DevBuf d_segs, d_cache, d_cache_d, d_views;
     const float4* segs_ext = nullptr;       // caller-owned device segment array (l3d_set_views_flat on_device)
-    void* h_stage = nullptr; size_t h_stage_cap = 0;
+    std::unique_ptr<void, cudaError_t (*)(void*)> h_stage{nullptr, cudaFreeHost};    // pinned staging of l3d_set_views
+    size_t h_stage_cap = 0;
 
     // last match result
     bool have_matches = false;
@@ -84,7 +91,7 @@ struct l3d_ctx {
     long long total_rows = 0, pair_evals = 0;
     std::vector<L3DPairDev> h_pairs;
     std::vector<int2> h_tiles;
-    DevBuf d_pairs, d_tiles, d_counts, d_recs, d_rowptr, d_csr, d_scan_tmp, d_dense_dep, d_dense_ov, d_dense_jobs, d_arcs, d_basis, d_arcraw, d_arckeys, d_arckeys2, d_arcvals, d_arcvals2, d_arctmp;
+    DevBuf d_pairs, d_tiles, d_counts, d_recs, d_rowptr, d_csr, d_dense_dep, d_dense_ov, d_dense_jobs, d_arcs, d_basis, d_arcraw, d_arckeys, d_arckeys2, d_arcvals, d_arcvals2;
 
     SweepState sweep;
     RddState rdd;
@@ -94,23 +101,41 @@ struct l3d_ctx {
 
     const float4* segs() const { return segs_ext ? segs_ext : (const float4*)d_segs.p; }
     const L3DViewDev* views() const { return (const L3DViewDev*)d_views.p; }
-    std::vector<DevBuf*> all_bufs()
+
+    // Forget stage `s` and every stage computed from it.  An entry point that computes a stage drops it before it touches
+    // any state and marks it present again only when it returns L3D_OK.
+    void drop(Stage s)
     {
-        std::vector<DevBuf*> b = {&d_segs, &d_cache, &d_cache_d, &d_views, &d_pairs, &d_tiles, &d_counts, &d_recs, &d_rowptr, &d_csr, &d_scan_tmp, &d_dense_dep, &d_dense_ov, &d_dense_jobs, &d_arcs, &d_basis, &d_arcraw, &d_arckeys, &d_arckeys2, &d_arcvals, &d_arcvals2, &d_arctmp};
-        for (DevBuf* x : sweep.bufs()) b.push_back(x);
-        for (DevBuf* x : rdd.bufs()) b.push_back(x);
-        for (DevBuf* x : aff.bufs()) b.push_back(x);
-        for (DevBuf* x : collin.bufs()) b.push_back(x);
-        for (DevBuf* x : opt.bufs()) b.push_back(x);
-        return b;
+        switch (s) {
+        case Stage::Views:     have_views = false; drop(Stage::Matches); drop(Stage::Collinear); break;
+        case Stage::Matches:   have_matches = false; drop(Stage::Sweep); break;
+        case Stage::Sweep:     sweep.valid = false; drop(Stage::Affinity); break;
+        case Stage::Collinear: collin.valid = false; drop(Stage::Affinity); break;
+        case Stage::Affinity:  aff.valid = false; break;
+        }
     }
 };
 
 int l3d_fail(l3d_ctx* c, int code, const char* what, cudaError_t e = cudaSuccess);
-int l3d_reserve(l3d_ctx* c, DevBuf& b, size_t bytes, const char* what);
 
 #define L3D_CUDA(ctx, call, what)                                                     \
     do {                                                                              \
         cudaError_t _e = (call);                                                      \
         if (_e != cudaSuccess) return l3d_fail((ctx), L3D_ERR_CUDA, (what), _e);      \
     } while (0)
+
+// grows `buf` to at least max(bytes, 16) bytes or returns the failure from the enclosing function (which declares `int rc`)
+#define L3D_RESERVE(buf, bytes, what)                                                                             \
+    do {                                                                                                          \
+        if ((rc = (buf).reserve(c, (size_t)std::max<long long>((long long)(bytes), 16), (what)))) return rc;      \
+    } while (0)
+
+// CUDA event destroyed with its scope
+struct ScopedEvent {
+    cudaEvent_t e = nullptr;
+    ScopedEvent() = default;
+    ScopedEvent(const ScopedEvent&) = delete;
+    ScopedEvent& operator=(const ScopedEvent&) = delete;
+    ~ScopedEvent() { if (e) cudaEventDestroy(e); }
+    int create(l3d_ctx* c) { L3D_CUDA(c, cudaEventCreate(&e), "event"); return L3D_OK; }
+};

@@ -335,13 +335,11 @@ int l3d_optimize_lines(l3d_ctx* c, int num_lines, const double* p1p2, const long
     cudaSetDevice(c->device);
     OptState& O = c->opt;
     int rc;
-#define RES(buf, bytes, what) if ((rc = l3d_reserve(c, buf, (size_t)std::max<long long>((long long)(bytes), 16), what))) return rc
-    RES(O.d_p, 48ll * L, "opt lines"); RES(O.d_pout, 48ll * L, "opt lines out"); RES(O.d_valid, 4ll * L, "opt valid"); RES(O.d_resptr, 8ll * (L + 1), "opt res ptr");
-    RES(O.d_rescam, 4 * NR, "opt res cam"); RES(O.d_resxy, 32 * NR, "opt res xy"); RES(O.d_obs, (long long)sizeof(OptObs) * NR, "opt observations");
-    RES(O.d_cams, 128ll * num_cams, "opt cameras"); RES(O.d_x, 32ll * L, "opt x"); RES(O.d_xc, 32ll * L, "opt x candidate"); RES(O.d_g, 32ll * L, "opt gradient");
-    RES(O.d_H, 80ll * L, "opt JtJ"); RES(O.d_S, 32ll * L, "opt scaling"); RES(O.d_diag, 32ll * L, "opt diagonal"); RES(O.d_free, 4ll * L, "opt free flags");
-    RES(O.d_part, 48ll * L, "opt partial sums"); RES(O.d_tot, 64, "opt totals");
-#undef RES
+    L3D_RESERVE(O.d_p, 48ll * L, "opt lines"); L3D_RESERVE(O.d_pout, 48ll * L, "opt lines out"); L3D_RESERVE(O.d_valid, 4ll * L, "opt valid"); L3D_RESERVE(O.d_resptr, 8ll * (L + 1), "opt res ptr");
+    L3D_RESERVE(O.d_rescam, 4 * NR, "opt res cam"); L3D_RESERVE(O.d_resxy, 32 * NR, "opt res xy"); L3D_RESERVE(O.d_obs, (long long)sizeof(OptObs) * NR, "opt observations");
+    L3D_RESERVE(O.d_cams, 128ll * num_cams, "opt cameras"); L3D_RESERVE(O.d_x, 32ll * L, "opt x"); L3D_RESERVE(O.d_xc, 32ll * L, "opt x candidate"); L3D_RESERVE(O.d_g, 32ll * L, "opt gradient");
+    L3D_RESERVE(O.d_H, 80ll * L, "opt JtJ"); L3D_RESERVE(O.d_S, 32ll * L, "opt scaling"); L3D_RESERVE(O.d_diag, 32ll * L, "opt diagonal"); L3D_RESERVE(O.d_free, 4ll * L, "opt free flags");
+    L3D_RESERVE(O.d_part, 48ll * L, "opt partial sums"); L3D_RESERVE(O.d_tot, 64, "opt totals");
     cudaStream_t st = c->stream;
     L3D_CUDA(c, cudaMemcpyAsync(O.d_p.p, p1p2, 48ull * L, cudaMemcpyHostToDevice, st), "opt upload");
     L3D_CUDA(c, cudaMemcpyAsync(O.d_resptr.p, res_ptr, 8ull * (L + 1), cudaMemcpyHostToDevice, st), "opt upload");

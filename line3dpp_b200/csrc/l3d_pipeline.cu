@@ -23,7 +23,7 @@
 // Arithmetic contract as in l3d_device.cuh (-fmad=false): the float parts repeat K_score_matches operation by
 // operation (same libdevice expf/acosf), the double parts repeat the host code of view.cc / line3D.cc (IEEE double, no
 // contraction); pinned against the unmodified reference in tests/test_ref_full_gpu.py.
-#include "l3d_ctx.cuh"
+#include "l3d_cub.cuh"
 #include "l3d_device_f64.cuh"
 #include "l3d_sweep.cuh"
 
@@ -751,13 +751,13 @@ extern "C" {
 int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float min_best_score, float min_best_perc)
 {
     if (!c) return L3D_ERR_INVALID;
+    c->drop(Stage::Sweep);
     if (!c->have_matches) return l3d_fail(c, L3D_ERR_STATE, "l3d_score_sweep: call l3d_match_pairs first");
     cudaSetDevice(c->device);
     const int V = c->num_views, NP = c->num_pairs, knn = c->knn;
     const long long slots = c->total_rows * knn;
     if (slots >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_score_sweep: more than 2^31 match slots");
     SweepState& S = c->sweep;
-    S.valid = false; c->aff.valid = false;
     const bool cpu_sem = c->semantics == L3D_SEM_REF_CPU;
     // processing order = ascending camID (std::map iteration, line3D.cc:704)
     S.order.resize(V);
@@ -794,15 +794,14 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
 
     int rc;
     cudaStream_t st = c->stream;
-#define RES(buf, bytes, what) if ((rc = l3d_reserve(c, buf, (size_t)std::max<long long>((long long)(bytes), 16), what))) return rc
-    RES(S.d_vt, sizeof(SwView) * (size_t)V, "view table"); RES(S.d_vp, sizeof(SwChunk) * vp.size(), "chunk descriptors"); RES(S.d_pairc, 8 * (size_t)NP, "pair chunks");
-    RES(S.d_rowoff, 8 * (size_t)(NP + 1), "pair row offsets"); RES(S.d_order, 4 * (size_t)V, "order"); RES(S.d_region_off, 8 * (size_t)(V + 1), "region offsets");
+    L3D_RESERVE(S.d_vt, sizeof(SwView) * (size_t)V, "view table"); L3D_RESERVE(S.d_vp, sizeof(SwChunk) * vp.size(), "chunk descriptors"); L3D_RESERVE(S.d_pairc, 8 * (size_t)NP, "pair chunks");
+    L3D_RESERVE(S.d_rowoff, 8 * (size_t)(NP + 1), "pair row offsets"); L3D_RESERVE(S.d_order, 4 * (size_t)V, "order"); L3D_RESERVE(S.d_region_off, 8 * (size_t)(V + 1), "region offsets");
     const long long nblocks = (slots + SW_SETUP_THREADS - 1) / SW_SETUP_THREADS;
-    RES(S.d_pinfo, sizeof(SwPairInfo) * (size_t)(NP + 1), "pair table"); RES(S.d_bpair, 4 * std::max<long long>(nblocks, 1), "first pair of every block");
-    RES(S.d_rays, 72 * c->total_segs, "segment rays"); RES(S.d_rmf, 16 * c->total_segs, "mid-point rays"); RES(S.d_rflag, slots, "record flags"); RES(S.d_invpos, 4 * slots, "inverse positions");
-    RES(S.d_csize, 4 * (NC + 1), "chunk sizes"); RES(S.d_ccur, 4 * (NC + 1), "chunk cursors"); RES(S.d_cstart, 8 * (NC + 1), "chunk offsets");
-    RES(S.d_ranges, 8 * c->total_segs, "ranges"); RES(S.d_est_best, 4 * c->total_segs, "estimates"); RES(S.d_est_P, 48 * c->total_segs, "estimate points");
-    RES(S.d_M, 4 * (size_t)V, "match counts"); RES(S.d_vmax, 4 * (size_t)V, "view max");
+    L3D_RESERVE(S.d_pinfo, sizeof(SwPairInfo) * (size_t)(NP + 1), "pair table"); L3D_RESERVE(S.d_bpair, 4 * std::max<long long>(nblocks, 1), "first pair of every block");
+    L3D_RESERVE(S.d_rays, 72 * c->total_segs, "segment rays"); L3D_RESERVE(S.d_rmf, 16 * c->total_segs, "mid-point rays"); L3D_RESERVE(S.d_rflag, slots, "record flags"); L3D_RESERVE(S.d_invpos, 4 * slots, "inverse positions");
+    L3D_RESERVE(S.d_csize, 4 * (NC + 1), "chunk sizes"); L3D_RESERVE(S.d_ccur, 4 * (NC + 1), "chunk cursors"); L3D_RESERVE(S.d_cstart, 8 * (NC + 1), "chunk offsets");
+    L3D_RESERVE(S.d_ranges, 8 * c->total_segs, "ranges"); L3D_RESERVE(S.d_est_best, 4 * c->total_segs, "estimates"); L3D_RESERVE(S.d_est_P, 48 * c->total_segs, "estimate points");
+    L3D_RESERVE(S.d_M, 4 * (size_t)V, "match counts"); L3D_RESERVE(S.d_vmax, 4 * (size_t)V, "view max");
     L3D_CUDA(c, cudaMemcpyAsync(S.d_vt.p, vt.data(), sizeof(SwView) * (size_t)V, cudaMemcpyHostToDevice, st), "view table");
     if (!vp.empty()) L3D_CUDA(c, cudaMemcpyAsync(S.d_vp.p, vp.data(), sizeof(SwChunk) * vp.size(), cudaMemcpyHostToDevice, st), "chunk descriptors");
     if (NP) L3D_CUDA(c, cudaMemcpyAsync(S.d_pairc.p, pairc.data(), 8 * (size_t)NP, cudaMemcpyHostToDevice, st), "pair chunks");
@@ -837,9 +836,9 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
     L3D_CUDA(c, cudaMemsetAsync(S.d_M.p, 0, 4 * (size_t)V, st), "init counts");
     L3D_CUDA(c, cudaMemsetAsync(S.d_vmax.p, 0, 4 * (size_t)V, st), "init maxima");
 
-    cudaEvent_t ev[4];
-    for (int q = 0; q < 4; ++q) cudaEventCreate(&ev[q]);
-    cudaEventRecord(ev[0], st);
+    ScopedEvent ev[4];
+    for (ScopedEvent& e : ev) if ((rc = e.create(c))) return rc;
+    cudaEventRecord(ev[0].e, st);
     const float4* segs = c->segs(); const float4* cache = (const float4*)c->d_cache.p;
     const L3DViewDev* views = c->views(); const L3DPairDev* pairs = (const L3DPairDev*)c->d_pairs.p;
     const int* counts = (const int*)c->d_counts.p; const l3d_match_rec* recs = (const l3d_match_rec*)c->d_recs.p;
@@ -850,11 +849,8 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
         k_sw_rays<<<(unsigned int)((c->total_segs + 255) / 256), 256, 0, st>>>(segs, views, V, c->total_segs, (double*)S.d_rays.p, (float4*)S.d_rmf.p);
         k_sw_flags<<<nbs, SW_SETUP_THREADS, 0, st>>>((const double*)S.d_rays.p, cache, (const float4*)S.d_rmf.p, views, (const SwPairInfo*)S.d_pinfo.p, (const int*)S.d_bpair.p,
                                                      counts, recs, knn, slots, (unsigned char*)S.d_rflag.p, (int*)S.d_csize.p);
-        size_t tb = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, tb, (const int*)S.d_csize.p, (long long*)S.d_cstart.p, NC + 1, st);
-        RES(S.d_sort_tmp, tb, "scan temp");
-        tb = S.d_sort_tmp.cap;
-        L3D_CUDA(c, cub::DeviceScan::ExclusiveSum(S.d_sort_tmp.p, tb, (const int*)S.d_csize.p, (long long*)S.d_cstart.p, NC + 1, st), "chunk scan");
+        if ((rc = l3d_cub(c, "chunk scan", [&](void* tmp, size_t& bytes) {
+                 return cub::DeviceScan::ExclusiveSum(tmp, bytes, (const int*)S.d_csize.p, (long long*)S.d_cstart.p, NC + 1, st); }))) return rc;
         k_sw_regions<<<(V + 256) / 256, 256, 0, st>>>(V, (SwView*)S.d_vt.p, (const long long*)S.d_cstart.p, NC, (const int*)S.d_order.p, (long long*)S.d_region_off.p);
         L3D_CUDA(c, cudaMemcpyAsync(S.region_off.data(), S.d_region_off.p, 8 * (size_t)(V + 1), cudaMemcpyDeviceToHost, st), "region offsets");
         L3D_CUDA(c, cudaStreamSynchronize(st), "score sweep set-up");
@@ -868,10 +864,10 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
     long long Umax = 1;
     for (int i = 0; i < V; ++i) Umax = std::max(Umax, S.region_off[i + 1] - S.region_off[i]);
     if (Umax >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_score_sweep: view with more than 2^31 matches");
-    RES(S.d_eval, 4 * total, "entry records"); RES(S.d_escore, 4 * total, "entry scores"); RES(S.d_eflag, total, "entry flags");
-    RES(S.d_ekv, 8 * total, "unsorted entries");
-    RES(S.d_gstage, 2 * 48 * Umax, "long-list scratch"); RES(S.d_gpub, 2 * 4 * Umax, "long-list scratch");
-    if (cpu_sem) RES(S.d_dir64, 2 * 32 * Umax, "long-list scratch");
+    L3D_RESERVE(S.d_eval, 4 * total, "entry records"); L3D_RESERVE(S.d_escore, 4 * total, "entry scores"); L3D_RESERVE(S.d_eflag, total, "entry flags");
+    L3D_RESERVE(S.d_ekv, 8 * total, "unsorted entries");
+    L3D_RESERVE(S.d_gstage, 2 * 48 * Umax, "long-list scratch"); L3D_RESERVE(S.d_gpub, 2 * 4 * Umax, "long-list scratch");
+    if (cpu_sem) L3D_RESERVE(S.d_dir64, 2 * 32 * Umax, "long-list scratch");
     unsigned int* e_val = (unsigned int*)S.d_eval.p; float* e_score = (float*)S.d_escore.p; unsigned char* e_flag = (unsigned char*)S.d_eflag.p;
     if (total > 0) {
         k_sw_scatter<<<nbs, SW_SETUP_THREADS, 0, st>>>((const SwPairInfo*)S.d_pinfo.p, (const int*)S.d_bpair.p, recs, knn, slots, (const unsigned char*)S.d_rflag.p,
@@ -888,7 +884,7 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
         const double ang = std::sqrt((double)q_thr * (double)two_sigA_sqr);           // degrees
         cos_thr = ang < 89.0 ? (float)(std::cos(ang * L3D_PI_D / 180.0) * (1.0 - 1e-4)) : -1.0f;
     }
-    cudaEventRecord(ev[1], st);
+    cudaEventRecord(ev[1].e, st);
     // ---- the chain: one launch per view, ascending camID
     if (total > 0) {
         SwScoreArgs<false> A;
@@ -950,7 +946,7 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
         }
         L3D_CUDA(c, cudaGetLastError(), "score sweep launch");
     }
-    cudaEventRecord(ev[2], st);
+    cudaEventRecord(ev[2].e, st);
     // ---- filterMatches + best estimates for all views
     {
         const long long N = c->total_segs;
@@ -966,20 +962,14 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
         // compact the estimates on the device: flags -> exclusive scan -> gather (best match record + P1,P2)
         S.n_est = 0;
         if (N > 0) {
-            RES(S.d_est_pos, 8 * (size_t)(N + 1), "estimate positions");
+            L3D_RESERVE(S.d_est_pos, 8 * (size_t)(N + 1), "estimate positions");
             cub::TransformInputIterator<long long, HasEstimate, const int*> flags((const int*)S.d_est_best.p, HasEstimate());
-            size_t tb = 0;
-            cub::DeviceScan::ExclusiveSum(nullptr, tb, flags, (long long*)S.d_est_pos.p, N, st);
-            RES(S.d_sort_tmp, tb, "scan temp");
-            tb = S.d_sort_tmp.cap;
-            L3D_CUDA(c, cub::DeviceScan::ExclusiveSum(S.d_sort_tmp.p, tb, flags, (long long*)S.d_est_pos.p, N, st), "estimate scan");
-            long long last_pos = 0; int last_best = -1;
-            L3D_CUDA(c, cudaMemcpyAsync(&last_pos, (long long*)S.d_est_pos.p + N - 1, 8, cudaMemcpyDeviceToHost, st), "estimate count");
-            L3D_CUDA(c, cudaMemcpyAsync(&last_best, (int*)S.d_est_best.p + N - 1, 4, cudaMemcpyDeviceToHost, st), "estimate count");
+            ScanTotal t;
+            if ((rc = l3d_scan_total(c, flags, (long long*)S.d_est_pos.p, N, (const int*)S.d_est_best.p, t, "estimate scan"))) return rc;
             L3D_CUDA(c, cudaStreamSynchronize(st), "score sweep");
-            S.n_est = last_pos + (last_best >= 0 ? 1 : 0);
-            RES(S.d_est_out_best, sizeof(l3d_match) * (size_t)std::max<long long>(S.n_est, 1), "estimate records");
-            RES(S.d_est_out_P, 48 * (size_t)std::max<long long>(S.n_est, 1), "estimate points");
+            S.n_est = t.last_out + HasEstimate()(t.last_src);
+            L3D_RESERVE(S.d_est_out_best, sizeof(l3d_match) * (size_t)std::max<long long>(S.n_est, 1), "estimate records");
+            L3D_RESERVE(S.d_est_out_P, 48 * (size_t)std::max<long long>(S.n_est, 1), "estimate points");
             if (S.n_est > 0) {
                 k_collect_estimates<<<(unsigned int)((N + 255) / 256), 256, 0, st>>>(views, V, N, d_vt, (const int*)S.d_est_best.p, (const long long*)S.d_est_pos.p, pairs,
                                                                                    d_rowoff, NP, knn, recs, e_val, e_score, (const double*)S.d_est_P.p,
@@ -988,15 +978,13 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
                 L3D_CUDA(c, cudaGetLastError(), "k_collect_estimates");
             }
         }
-        cudaEventRecord(ev[3], st);
+        cudaEventRecord(ev[3].e, st);
         L3D_CUDA(c, cudaStreamSynchronize(st), "score sweep");
-        cudaEventElapsedTime(&S.ms_setup, ev[0], ev[1]); cudaEventElapsedTime(&S.ms_chain, ev[1], ev[2]); cudaEventElapsedTime(&S.ms_filter, ev[2], ev[3]);
-        for (int q = 0; q < 4; ++q) cudaEventDestroy(ev[q]);
+        cudaEventElapsedTime(&S.ms_setup, ev[0].e, ev[1].e); cudaEventElapsedTime(&S.ms_chain, ev[1].e, ev[2].e); cudaEventElapsedTime(&S.ms_filter, ev[2].e, ev[3].e);
         if (getenv("L3D_SWEEP_TIMING")) fprintf(stderr, "[l3d] score sweep: set-up %.3f ms, chain %.3f ms (%d views), filter+estimates %.3f ms\n", S.ms_setup, S.ms_chain, V, S.ms_filter);
         S.h_M.resize(V);
         for (int i = 0; i < V; ++i) S.h_M[i] = M[S.order[i]];
     }
-#undef RES
     S.valid = true;
     return L3D_OK;
 }
@@ -1015,8 +1003,8 @@ long long l3d_get_view_matches(l3d_ctx* c, int view, int kept_only, l3d_match* o
     const int n = (int)(S.region_off[i + 1] - ro);
     if (n == 0) return 0;
     int rc;
-    if ((rc = l3d_reserve(c, S.d_export, sizeof(l3d_match) * (size_t)n, "export records"))) return rc;
-    if ((rc = l3d_reserve(c, S.d_export_ok, (size_t)n, "export flags"))) return rc;
+    L3D_RESERVE(S.d_export, sizeof(l3d_match) * (size_t)n, "export records");
+    L3D_RESERVE(S.d_export_ok, (size_t)n, "export flags");
     k_sw_export<<<(n + 255) / 256, 256, 0, c->stream>>>(c->views(), view, ro, n, (const L3DPairDev*)c->d_pairs.p, (const long long*)S.d_rowoff.p, c->num_pairs, c->knn,
                                                      (const l3d_match_rec*)c->d_recs.p, (const unsigned int*)S.d_eval.p, (const float*)S.d_escore.p,
                                                      (const unsigned char*)S.d_eflag.p, (unsigned char)(kept_only ? (SW_ACTIVE | SW_KEPT) : SW_ACTIVE),

@@ -310,6 +310,87 @@ def test_capi_error_behaviour(gpu_ctx):
     fresh.close()
 
 
+def _ctx_with_views(nviews=3):
+    from line3dpp_b200 import capi
+    sc = synth.make_scene(nviews, 50, 2, "dense")
+    ctx = capi.Context(0)
+    descs = util.scene_descs(sc)
+    ctx.set_views(descs, sc.segs)
+    return ctx, sc, descs
+
+
+def test_failed_match_leaves_no_result():
+    """a match call that fails in argument checking leaves no match result behind, not the old one mixed with the new pairs"""
+    import ctypes as C
+    ctx, sc, _ = _ctx_with_views()
+    L = ctx.L
+    ctx.match_pairs([[0, 1]], util.pair_F(sc, [(0, 1)]))
+    assert ctx.match_total_rows() == len(sc.segs[0])
+    pairs = np.array([[0, 1], [0, 7]], np.int32)            # longer than the last list; view 7 does not exist
+    F = np.zeros((2, 9), np.float32)
+    assert L.l3d_match_pairs(ctx.h, 2, pairs.ctypes.data_as(C.c_void_p), F.ctypes.data_as(C.c_void_p), C.c_float(0.25), 10) == -1
+    assert ctx.match_total_rows() == -1
+    assert L.l3d_match_stride(ctx.h) == -3 and L.l3d_match_semantics(ctx.h) == -3
+    ctx.close()
+
+
+def test_failed_set_views_leaves_no_views():
+    """a set_views call with a negative segment count leaves no views: matching then asks for set_views"""
+    import ctypes as C
+    from line3dpp_b200 import capi
+    ctx, sc, descs = _ctx_with_views()
+    descs[2].nseg = -1
+    with pytest.raises(capi.L3DError, match=r"failed \(-1\)"):
+        ctx.set_views(descs, sc.segs)
+    assert ctx.L.l3d_match_pairs(ctx.h, 0, None, None, C.c_float(0.25), 10) == -3
+    ctx.close()
+
+
+def test_failed_set_views_flat_leaves_no_views():
+    """a misaligned device segment array is rejected, and the views set before are gone with it"""
+    import ctypes as C
+    import torch
+    from line3dpp_b200 import capi
+    ctx, sc, descs = _ctx_with_views()
+    flat = torch.zeros(sum(len(s) for s in sc.segs) * 4 + 1, dtype=torch.float32, device="cuda")
+    with pytest.raises(capi.L3DError, match=r"failed \(-1\)"):
+        ctx.set_views_flat(descs, flat.data_ptr() + 4, on_device=True)
+    assert ctx.L.l3d_match_pairs(ctx.h, 0, None, None, C.c_float(0.25), 10) == -3
+    ctx.close()
+
+
+@pytest.mark.parametrize("rematch", ["match_pairs", "device_buffers"])
+def test_new_match_drops_affinity(rematch):
+    """the affinity matrix is computed from the match result: a new match result, or one handed out for writing, drops it"""
+    import ctypes as C
+    from line3dpp_b200 import capi
+    sc = synth.make_scene(14, 500, 31, "ring3")
+    V = sc.num_views
+    RtKinv, Cw = synth.camera_blocks(sc)
+    k = [2.5 / sc.K[v][0, 0] for v in range(V)]          # spatial regulariser of 2.5 px (View::getSpecificSpatialReg)
+    descs = capi.make_view_descs(sc.cam_ids, [sc.width] * V, [sc.height] * V, [len(s) for s in sc.segs], RtKinv, Cw, Cw, k, sc.median_depth)
+    pairs = synth.view_pairs(sc.neighbors, sc.cam_ids)
+    F = util.pair_F(sc, pairs)
+    ctx = capi.Context(0)
+    L = ctx.L
+    L.l3d_affinity_matrix.restype = L.l3d_rdd_affinity.restype = C.c_longlong
+    ctx.set_views(descs, sc.segs)
+    ctx.match_pairs(pairs, F)
+    assert L.l3d_score_sweep(ctx.h, C.c_float(200), C.c_float(.5), C.c_float(.75), C.c_float(.1)) == 0
+    nids = C.c_longlong(0)
+    nE = L.l3d_affinity_matrix(ctx.h, C.c_float(200), C.c_float(float(np.median(sc.median_depth))), C.c_float(.5), None, None, None,
+                               C.c_longlong(0), None, C.c_longlong(0), C.byref(nids))
+    assert nE > 0
+    oi, oj, ow = np.zeros(nE, np.int32), np.zeros(nE, np.int32), np.zeros(nE, np.float32)
+    if rematch == "match_pairs":
+        ctx.match_pairs(pairs, F)
+    else:
+        ctx.match_device_buffers()
+    p = lambda a: a.ctypes.data_as(C.c_void_p)
+    assert L.l3d_rdd_affinity(ctx.h, 10, p(oi), p(oj), p(ow), C.c_longlong(nE)) == -3
+    ctx.close()
+
+
 def test_knn_above_32_vs_reference_wrapper(loaded, scene, ref_gold):
     """kNN > 32 (beyond the fused kernel's per-row key list; the reference accepts any kNN, cudawrapper.cu:637-645): the keep-all
     passes + per-row cut must give the reference wrapper's matches, in its pop order (overlap descending)."""
