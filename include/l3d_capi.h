@@ -13,7 +13,8 @@
  * 0 on success or a negative l3d_status; l3d_last_error() gives the message (the reference prints CUDA errors to
  * cerr and carries on, dataArray.h:198-237).  A call that fails leaves its stage (views, matches, score sweep,
  * collinear lists, affinity matrix), and every stage computed from it, without a result: later calls that need one
- * return L3D_ERR_STATE.  A context is single-owner (not thread-safe), one per GPU, and runs
+ * return L3D_ERR_STATE.  The image calls (l3d_undistort_u8, l3d_undistort_map, l3d_remap_u8) are not part of that chain: whether
+ * they succeed or fail, every stage and its result stay as they were.  A context is single-owner (not thread-safe), one per GPU, and runs
  * on its own non-default stream.  There is NO CPU fallback: without a usable CUDA device l3d_ctx_create fails.
  */
 #ifndef L3D_CAPI_H_
@@ -235,6 +236,32 @@ long long l3d_rdd_affinity(l3d_ctx* ctx, int iters, int32_t* out_i, int32_t* out
 int l3d_optimize_lines(l3d_ctx* ctx, int num_lines, const double* p1p2, const long long* res_ptr, const int32_t* res_cam,
                        const double* res_xy, int num_cams, const double* cams, int max_iter, double* p1p2_out, int32_t* valid_out,
                        double* summary);
+
+/* ---- lens undistortion of 8-bit images: Line3D::undistortImage (line3D.cc:83-109), i.e. OpenCV's initUndistortRectifyMap with
+ * fixed-point maps (CV_16SC2 pixel + CV_16UC1 1/32-px fraction) followed by remap(INTER_LINEAR, BORDER_CONSTANT 0), output the size
+ * and type of the input, K unchanged.  The camera matrix is [[fx,0,cx],[0,fy,cy],[0,0,1]] (skew is ignored, as in the reference);
+ * the distortion vector is (k1, k2, p1, p2, k3) = (radial[0], radial[1], tangential[0], tangential[1], radial[2]).  The map is
+ * defined by the formula of DESIGN.md §4a, which OpenCV builds reproduce to within one 1/32-px step; the remap is bit-exact to
+ * OpenCV's.  Pixels are interleaved (channels 1 or 3); pitches are row strides in bytes.
+ * Rejected with L3D_ERR_INVALID: width or height outside [1, 32767], channels other than 1 or 3, a pitch below width*channels,
+ * null pointers, src == dst, fx or fy zero or not finite, a principal point or coefficient that is not finite.
+ * on_device != 0: every pointer is a device address on this GPU and the call is asynchronous on the context's stream;
+ * on_device == 0: host buffers, staged through the context's own device buffers, and the call returns when the output is written. */
+typedef struct {
+    int32_t width, height, channels;
+    int64_t src_pitch, dst_pitch;
+    const uint8_t* src;
+    uint8_t* dst;
+    double fx, fy, cx, cy;
+    double radial[3], tangential[2];
+} l3d_undistort_desc;
+/* undistort n images in one launch; images, sizes, channel counts and cameras may all differ */
+int l3d_undistort_u8(l3d_ctx* ctx, int n, const l3d_undistort_desc* descs, int on_device);
+/* the fixed-point maps of one image (src, dst and the pitches are not used): map_xy int16[height*width*2] (x, y per pixel),
+ * map_frac uint16[height*width] = (v & 31) * 32 + (u & 31); rows packed.  What cv::remap takes as its two maps. */
+int l3d_undistort_map(l3d_ctx* ctx, const l3d_undistort_desc* desc, int16_t* map_xy, uint16_t* map_frac, int on_device);
+/* cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) of one image with caller-given maps in that layout (the camera is not used) */
+int l3d_remap_u8(l3d_ctx* ctx, const l3d_undistort_desc* desc, const int16_t* map_xy, const uint16_t* map_frac, int on_device);
 
 /* stable ascending argsort of float keys on the device: the weight sort of performClustering (clustering.cc:13-14) for
  * large edge lists.  perm_out[i] = index of the i-th smallest key, ties in input order. */

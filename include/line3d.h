@@ -13,6 +13,9 @@
  *     types (P1().x is a member, not Eigen's x()): a frontend that reads the result lines needs that one-character change.
  *   - addImage takes the image SIZE and explicit 2D segments (the reference's own line_segments argument,
  *     line3D.h:102-108); LSD detection inside addImage (line3D.cc:249-372) is outside the hot path (SURVEY.md §2 row 13).
+ *   - undistortImage (line3D.h:119-122) takes the owning Image8u and the POD vectors; with Eigen / OpenCV headers the reference's
+ *     cv::Mat signature is an inline overload for CV_8UC1 / CV_8UC3.  It runs on the GPU and its map is defined by an explicit
+ *     formula, which OpenCV builds reproduce to within one 1/32-px step (DESIGN.md §4a).
  *   - save3DLinesAsBIN (boost archive) is not provided; TXT / OBJ / STL are.
  *   - use_GPU selects the SCORING SEMANTICS of the reference's two paths; both run on the GPU (there is no CPU path).
  */
@@ -20,7 +23,9 @@
 #define L3DPP_B200_LINE3D_H_
 
 #include <cstddef>
+#include <cstring>
 #include <list>
+#include <stdexcept>
 #include <string>
 #include <vector>
 
@@ -36,10 +41,20 @@
 
 namespace L3DPP {
 
+struct Vector2d { double x, y; Vector2d() : x(0), y(0) {} Vector2d(double a, double b) : x(a), y(b) {} };
 struct Vector3d { double x, y, z; Vector3d() : x(0), y(0), z(0) {} Vector3d(double a, double b, double c) : x(a), y(b), z(c) {} };
 struct Matrix3d { double m[9]; double& operator()(int r, int c) { return m[r * 3 + c]; } double operator()(int r, int c) const { return m[r * 3 + c]; } };
 struct Vec4f { float v[4]; float operator()(int i) const { return v[i]; } };
 struct Vector4f { float v[4]; float operator()(int i) const { return v[i]; } };
+
+/* an 8-bit image that owns its pixels: rows x cols, 1 or 3 interleaved channels, rows packed (the layout of a continuous CV_8UC1 /
+ * CV_8UC3 cv::Mat) */
+struct Image8u {
+    int cols, rows, channels;
+    std::vector<unsigned char> data;
+    Image8u() : cols(0), rows(0), channels(1) {}
+    Image8u(int r, int c, int ch) : cols(c), rows(r), channels(ch), data((size_t)(r > 0 ? r : 0) * (c > 0 ? c : 0) * (ch > 0 ? ch : 0)) {}
+};
 
 /* defaults: commons.h:41-69 */
 const int L3D_DEF_MAX_IMG_WIDTH = -1;
@@ -167,6 +182,35 @@ public:
     size_t numImages();                                                /* line3D.h:205 */
     std::string createOutputFilename();                                /* line3D.h:224 */
     static Matrix3d rotationFromQ(const double Qw, const double Qx, const double Qy, const double Qz);   /* line3D.h:219-220 */
+
+    /* line3D.h:119-122: lens undistortion as the reference does it with OpenCV (initUndistortRectifyMap with fixed-point maps +
+     * remap, bilinear, border 0; include/l3d_capi.h l3d_undistort_u8).  Uses K(0,0), K(1,1), K(0,2), K(1,2) only; out gets the size
+     * and channels of in (in == out is allowed).  Runs on the calling thread's current CUDA device through a context that lives for
+     * the call.  Throws std::invalid_argument for an image or camera l3d_undistort_u8 rejects, std::runtime_error on a CUDA failure
+     * or without a usable device. */
+    static void undistortImage(const Image8u& in, Image8u& out, const Vector3d& radial_coeffs, const Vector2d& tangential_coeffs, const Matrix3d& K);
+
+#ifdef L3DPP_WITH_EIGEN_OPENCV
+    /* The reference's exact signature for CV_8UC1 / CV_8UC3 images; honours the row step of inImg and create()s outImg.  A template
+     * only so that this header also compiles against cv::Mat stand-ins that carry no pixels; calls are written as for the reference. */
+    template <class MatT = cv::Mat>
+    static void undistortImage(const cv::Mat& inImg, cv::Mat& outImg, const Eigen::Vector3d& radial_coeffs, const Eigen::Vector2d& tangential_coeffs,
+                               const Eigen::Matrix3d& K)
+    {
+        const MatT& in = inImg;
+        MatT& out = outImg;
+        if (in.type() != CV_8UC1 && in.type() != CV_8UC3) throw std::invalid_argument("undistortImage: only CV_8UC1 and CV_8UC3 images");
+        Image8u a(in.rows, in.cols, in.channels()), b;
+        const size_t row = (size_t)in.cols * in.channels(), in_step = static_cast<size_t>(in.step);
+        for (int r = 0; r < in.rows; ++r) std::memcpy(a.data.data() + r * row, in.data + r * in_step, row);
+        Matrix3d Kp;
+        for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) Kp(r, c) = K(r, c);
+        undistortImage(a, b, Vector3d(radial_coeffs(0), radial_coeffs(1), radial_coeffs(2)), Vector2d(tangential_coeffs(0), tangential_coeffs(1)), Kp);
+        out.create(in.rows, in.cols, in.type());
+        const size_t out_step = static_cast<size_t>(out.step);
+        for (int r = 0; r < b.rows; ++r) std::memcpy(out.data + r * out_step, b.data.data() + r * row, row);
+    }
+#endif
 
     /* --- additions (not in the reference) --- */
     const Line3DStats& stats() const;

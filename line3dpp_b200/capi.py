@@ -20,6 +20,39 @@ class ViewDesc(C.Structure):
                 ("k", C.c_float), ("median_depth", C.c_float)]
 
 
+class UndistortDesc(C.Structure):
+    """l3d_undistort_desc: one 8-bit image and its camera"""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("channels", C.c_int32), ("src_pitch", C.c_int64), ("dst_pitch", C.c_int64),
+                ("src", C.c_void_p), ("dst", C.c_void_p), ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
+                ("radial", C.c_double * 3), ("tangential", C.c_double * 2)]
+
+
+def make_undistort_desc(width, height, channels, K, radial=(0, 0, 0), tangential=(0, 0), src=0, src_pitch=None, dst=0, dst_pitch=None):
+    """K: 3x3 camera matrix (fx, fy, cx, cy are read, skew is ignored); src / dst: addresses; pitches in bytes (default packed)"""
+    K = np.asarray(K, np.float64).reshape(3, 3)
+    row = int(width) * int(channels)
+    d = UndistortDesc()
+    d.width, d.height, d.channels = int(width), int(height), int(channels)
+    d.src_pitch = row if src_pitch is None else int(src_pitch)
+    d.dst_pitch = row if dst_pitch is None else int(dst_pitch)
+    d.src, d.dst = int(src) or None, int(dst) or None
+    d.fx, d.fy, d.cx, d.cy = float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2])
+    d.radial[:] = [float(v) for v in radial]
+    d.tangential[:] = [float(v) for v in tangential]
+    return d
+
+
+def _image_rows(a):
+    """(array, row pitch in bytes) of a uint8 HxW / HxWx3 image whose pixels are packed within each row; other layouts are copied"""
+    a = np.asarray(a)
+    if a.dtype != np.uint8 or a.ndim not in (2, 3) or (a.ndim == 3 and a.shape[2] != 3):
+        raise ValueError("expected a uint8 HxW or HxWx3 image")
+    c = 1 if a.ndim == 2 else 3
+    if a.strides[1] != c or (a.ndim == 3 and a.strides[2] != 1) or a.strides[0] < a.shape[1] * c:
+        a = np.ascontiguousarray(a)
+    return a, a.strides[0]
+
+
 REC_DT = np.dtype([("tgt_seg", "<u4"), ("overlap", "<f4"), ("d_p1", "<f4"), ("d_p2", "<f4"), ("d_q1", "<f4"),
                    ("d_q2", "<f4")])
 MATCH_DT = np.dtype([("src_cam", "<u4"), ("src_seg", "<u4"), ("tgt_cam", "<u4"), ("tgt_seg", "<u4"),
@@ -248,6 +281,51 @@ class Context:
         dp = (C.c_void_p * len(pairs))(*[int(x) for x in depth_ptrs])
         op = (C.c_void_p * len(pairs))(*[int(x) for x in overlap_ptrs])
         self._chk(self.L.l3d_match_dense_pairs(self.h, len(pairs), _p(pairs), _p(F), C.c_float(epi_overlap), dp, op), "l3d_match_dense_pairs")
+
+    # ---- lens undistortion (stateless: no pipeline stage changes)
+    def undistort(self, images, K, radial=(0, 0, 0), tangential=(0, 0), out=None):
+        """Line3D::undistortImage for a list of uint8 HxW / HxWx3 images in ONE batched call.  K, radial, tangential: one camera for
+        all images or one per image.  out: optional list of preallocated outputs (any row pitch).  Returns the output arrays."""
+        n = len(images)
+        per = lambda v, nd: [v] * n if np.ndim(v) == nd else list(v)
+        Ks, rads, tans = per(K, 2), per(radial, 1), per(tangential, 1)
+        descs, keep = (UndistortDesc * n)(), []
+        outs = []
+        for i, img in enumerate(images):
+            a, sp = _image_rows(img)
+            o = np.empty_like(a) if out is None else out[i]
+            if o.shape != a.shape or o.dtype != np.uint8 or o.strides[1:] != a.strides[1:]:
+                raise ValueError("output must be a uint8 array of the input's shape with packed rows")
+            keep += [a, o]
+            descs[i] = make_undistort_desc(a.shape[1], a.shape[0], 1 if a.ndim == 2 else 3, Ks[i], rads[i], tans[i], a.ctypes.data, sp,
+                                           o.ctypes.data, o.strides[0])
+            outs.append(o)
+        self._chk(self.L.l3d_undistort_u8(self.h, n, descs, 0), "l3d_undistort_u8")
+        return outs
+
+    def undistort_device(self, descs):
+        """l3d_undistort_u8 on device addresses (a ctypes array of UndistortDesc); asynchronous on the context's stream"""
+        self._chk(self.L.l3d_undistort_u8(self.h, len(descs), descs, 1), "l3d_undistort_u8")
+
+    def undistort_map(self, width, height, K, radial=(0, 0, 0), tangential=(0, 0)):
+        """the fixed-point maps cv::remap takes: (map_xy int16 [h, w, 2], map_frac uint16 [h, w])"""
+        d = make_undistort_desc(width, height, 1, K, radial, tangential)
+        xy = np.empty((height, width, 2), np.int16)
+        fr = np.empty((height, width), np.uint16)
+        self._chk(self.L.l3d_undistort_map(self.h, C.byref(d), _p(xy), _p(fr), 0), "l3d_undistort_map")
+        return xy, fr
+
+    def remap(self, image, map_xy, map_frac):
+        """cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) of a uint8 HxW / HxWx3 image with fixed-point maps"""
+        a, sp = _image_rows(image)
+        xy = np.ascontiguousarray(map_xy, np.int16)
+        fr = np.ascontiguousarray(map_frac, np.uint16)
+        if xy.shape != a.shape[:2] + (2,) or fr.shape != a.shape[:2]:
+            raise ValueError("maps must be [h, w, 2] int16 and [h, w] uint16")
+        o = np.empty(a.shape, np.uint8)
+        d = make_undistort_desc(a.shape[1], a.shape[0], 1 if a.ndim == 2 else 3, np.eye(3), src=a.ctypes.data, src_pitch=sp, dst=o.ctypes.data)
+        self._chk(self.L.l3d_remap_u8(self.h, C.byref(d), _p(xy), _p(fr), 0), "l3d_remap_u8")
+        return o
 
     def match_dense(self, src_view, tgt_view, F, epi_overlap, ns, nt, nofilter=False, dev_ptrs=None):
         F = np.ascontiguousarray(F, np.float32).reshape(9)

@@ -61,6 +61,23 @@ struct RddState {
         d_Pp, d_Pnp, d_Wp, d_plan, d_dst;
 };
 
+// per-image parameters of the undistortion kernels (l3d_undistort.cu); ir0, ir2, ir4, ir5 = the non-trivial entries of
+// inv([[fx,0,cx],[0,fy,cy],[0,0,1]])
+struct L3DUndistImage {
+    const unsigned char* src;
+    unsigned char* dst;
+    long long src_pitch, dst_pitch, tile0;   // tile0: first tile of this image in the batch grid
+    int width, height, channels, tiles_x;
+    int full_radial, tangential;             // 0: k2 = k3 = 0, resp. p1 = p2 = 0 (those terms are skipped)
+    double ir0, ir2, ir4, ir5, fx, fy, cx, cy, k1, k2, k3, p1, p2;
+};
+
+// buffers of the undistortion calls: not a pipeline stage, nothing else reads them
+struct UndistortState {
+    std::vector<L3DUndistImage> h_imgs;
+    DevBuf d_imgs, d_src, d_dst, d_map_xy, d_map_frac;   // d_src .. d_map_frac: host-mode staging
+};
+
 // The results a context holds, each computed from the ones before it:
 //   Views -> Matches -> Sweep -> Affinity,   Views -> Collinear -> Affinity
 enum class Stage { Views, Matches, Sweep, Collinear, Affinity };
@@ -98,6 +115,7 @@ struct l3d_ctx {
     AffinityState aff;
     CollinState collin;
     OptState opt;
+    UndistortState undist;
 
     const float4* segs() const { return segs_ext ? segs_ext : (const float4*)d_segs.p; }
     const L3DViewDev* views() const { return (const L3DViewDev*)d_views.p; }

@@ -1,0 +1,295 @@
+// l3d_undistort.cu — lens undistortion of 8-bit images: what Line3D::undistortImage computes with OpenCV (line3D.cc:83-109,
+// initUndistortRectifyMap with fixed-point CV_16SC2 + CV_16UC1 maps, then remap INTER_LINEAR / BORDER_CONSTANT 0), and the three
+// C-ABI entry points declared in include/l3d_capi.h.  The arithmetic contract is DESIGN.md §4a; tests/undistort_model.py restates it.
+//
+// None of these calls belongs to the pipeline: they never drop a stage and touch only the buffers of UndistortState.
+#include "l3d_ctx.cuh"
+
+#include <climits>
+#include <cmath>
+#include <cstring>
+
+#define UD_TW 128       // columns per tile of k_undistort_u8 (one per thread)
+#define UD_TH 16        // rows per tile
+
+// cvRound(t * 32) as OpenCV's x86 build does it: round half to even; a value that is not finite or does not fit int32 gives INT_MIN
+__device__ __forceinline__ int ud_fix(double t)
+{
+    const double r = rint(t * 32.0);
+    return (r >= -2147483648.0 && r <= 2147483647.0) ? (int)r : INT_MIN;
+}
+
+// Fixed-point source position (u*32, v*32) of the pixel whose normalised coordinates are x = ir2 + j*ir0, y = i*ir4 + ir5
+// (the zero entries of ir only add signed zeros).  x2 = x*x and y2 = y*y come from the caller so that a tile computes them once
+// per column / row.  Terms whose coefficients are zero are skipped: that changes at most the sign of a zero, which the rounding
+// erases.  Plain IEEE double operations in the reference's order (the library is compiled with -fmad=false).
+__device__ __forceinline__ void ud_map_point(const L3DUndistImage& d, double x, double x2, double y, double y2, int& iu, int& iv)
+{
+    const double r2 = x2 + y2;
+    const double kr = 1.0 + (d.full_radial ? ((d.k3 * r2 + d.k2) * r2 + d.k1) : d.k1) * r2;
+    double xd = x * kr, yd = y * kr;
+    if (d.tangential) {
+        const double _2xy = 2.0 * x * y;
+        xd = xd + d.p1 * _2xy + d.p2 * (r2 + 2.0 * x2);
+        yd = yd + d.p1 * (r2 + 2.0 * y2) + d.p2 * _2xy;
+    }
+    iu = ud_fix(d.fx * xd + d.cx);
+    iv = ud_fix(d.fy * yd + d.cy);
+}
+
+__device__ __forceinline__ short ud_sat16(int v) { return (short)max(-32768, min(32767, v)); }
+
+// OpenCV's map entry: integer pixel (saturated to int16) and the 1/32-px fractions packed as ty*32 + tx
+__device__ __forceinline__ void ud_entry(int iu, int iv, short2& xy, unsigned short& frac)
+{
+    xy = make_short2(ud_sat16(iu >> 5), ud_sat16(iv >> 5));
+    frac = (unsigned short)(((iv & 31) << 5) + (iu & 31));
+}
+
+// remap's bilinear tap sum for one destination pixel: weights (32-tx|tx)*(32-ty|ty)*32 sum to 32768; a tap outside the image
+// reads the border value 0; result (sum + 16384) >> 15 clamped to 8 bits
+template <int C>
+__device__ __forceinline__ void ud_tap_sum(const unsigned char* __restrict__ src, long long pitch, int W, int H, short2 xy, unsigned short frac,
+                                           unsigned char* __restrict__ out)
+{
+    const int tx = frac & 31, ty = frac >> 5;
+    const int w[4] = {(32 - tx) * (32 - ty) * 32, tx * (32 - ty) * 32, (32 - tx) * ty * 32, tx * ty * 32};
+    int acc[C];
+#pragma unroll
+    for (int c = 0; c < C; ++c) acc[c] = 0;
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+        const int X = xy.x + (t & 1), Y = xy.y + (t >> 1);
+        if ((unsigned)X < (unsigned)W && (unsigned)Y < (unsigned)H) {
+            const unsigned char* p = src + (long long)Y * pitch + (long long)X * C;
+#pragma unroll
+            for (int c = 0; c < C; ++c) acc[c] += w[t] * (int)__ldg(p + c);
+        }
+    }
+#pragma unroll
+    for (int c = 0; c < C; ++c) out[c] = (unsigned char)max(0, min(255, (acc[c] + 16384) >> 15));
+}
+
+// the maps of one image, OpenCV's layout: map_xy short2[H*W], map_frac ushort[H*W], rows packed
+__global__ void __launch_bounds__(UD_TW) k_undistort_map(L3DUndistImage d, short2* __restrict__ map_xy, unsigned short* __restrict__ map_frac)
+{
+    const int j = blockIdx.x * UD_TW + threadIdx.x, i = blockIdx.y;
+    if (j >= d.width) return;
+    const double x = (double)j * d.ir0 + d.ir2, y = (double)i * d.ir4 + d.ir5;
+    int iu, iv;
+    ud_map_point(d, x, x * x, y, y * y, iu, iv);
+    const long long o = (long long)i * d.width + j;
+    ud_entry(iu, iv, map_xy[o], map_frac[o]);
+}
+
+// remap of one image with caller-given maps (same layout)
+template <int C>
+__global__ void __launch_bounds__(UD_TW) k_remap_u8(L3DUndistImage d, const short2* __restrict__ map_xy, const unsigned short* __restrict__ map_frac)
+{
+    const int j = blockIdx.x * UD_TW + threadIdx.x, i = blockIdx.y;
+    if (j >= d.width) return;
+    const long long o = (long long)i * d.width + j;
+    ud_tap_sum<C>(d.src, d.src_pitch, d.width, d.height, map_xy[o], map_frac[o], d.dst + (long long)i * d.dst_pitch + (long long)j * C);
+}
+
+template <int C>
+__device__ __forceinline__ void ud_tile_rows(const L3DUndistImage& d, int j, int i0, int rows, double x, double x2, const double2* s_y)
+{
+    unsigned char* out = d.dst + (long long)i0 * d.dst_pitch + (long long)j * C;
+    for (int r = 0; r < rows; ++r, out += d.dst_pitch) {
+        int iu, iv;
+        ud_map_point(d, x, x2, s_y[r].x, s_y[r].y, iu, iv);
+        short2 xy; unsigned short frac;
+        ud_entry(iu, iv, xy, frac);
+        ud_tap_sum<C>(d.src, d.src_pitch, d.width, d.height, xy, frac, out);
+    }
+}
+
+// The fused hot path over a batch: map entries in registers, never stored.  One CTA = UD_TW columns x UD_TH rows of one image;
+// the tiles of all images form one grid (image found by binary search over tile0), grey and RGB images alike.
+__global__ void __launch_bounds__(UD_TW) k_undistort_u8(const L3DUndistImage* __restrict__ imgs, int n)
+{
+    __shared__ double2 s_y[UD_TH];          // (y, y*y) of the tile's rows
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (imgs[mid].tile0 <= (long long)blockIdx.x) lo = mid; else hi = mid - 1;
+    }
+    const L3DUndistImage d = imgs[lo];
+    const long long t = (long long)blockIdx.x - d.tile0;
+    const int i0 = (int)(t / d.tiles_x) * UD_TH, j = (int)(t % d.tiles_x) * UD_TW + threadIdx.x;
+    if (threadIdx.x < UD_TH) {
+        const double y = (double)(i0 + threadIdx.x) * d.ir4 + d.ir5;
+        s_y[threadIdx.x] = make_double2(y, y * y);
+    }
+    __syncthreads();
+    if (j >= d.width) return;
+    const double x = (double)j * d.ir0 + d.ir2;
+    const int rows = min(UD_TH, d.height - i0);
+    if (d.channels == 3) ud_tile_rows<3>(d, j, i0, rows, x, x * x, s_y);
+    else ud_tile_rows<1>(d, j, i0, rows, x, x * x, s_y);
+}
+
+// ------------------------------------------------------------------------------------------------ host side
+// checks one descriptor; `image`: the pixel pointers and pitches are used, `camera`: the intrinsics and coefficients are used
+static int ud_check(l3d_ctx* c, const l3d_undistort_desc& u, bool image, bool camera, const char* what)
+{
+    char buf[160];
+    auto bad = [&](const char* why) { snprintf(buf, sizeof(buf), "%s: %s", what, why); return l3d_fail(c, L3D_ERR_INVALID, buf); };
+    if (u.width < 1 || u.width > 32767 || u.height < 1 || u.height > 32767) return bad("width and height must lie in [1, 32767]");
+    if (u.channels != 1 && u.channels != 3) return bad("channels must be 1 or 3");
+    if (image) {
+        const long long row = (long long)u.width * u.channels;
+        if (u.src_pitch < row || u.dst_pitch < row) return bad("row pitch below width * channels");
+        if (!u.src || !u.dst) return bad("null image pointer");
+        if (u.src == u.dst) return bad("src == dst (no in-place undistortion)");
+    }
+    if (camera) {
+        if (!std::isfinite(u.fx) || !std::isfinite(u.fy) || u.fx == 0.0 || u.fy == 0.0) return bad("fx and fy must be finite and non-zero");
+        bool finite = std::isfinite(u.cx) && std::isfinite(u.cy);
+        for (int k = 0; k < 3; ++k) finite = finite && std::isfinite(u.radial[k]);
+        for (int k = 0; k < 2; ++k) finite = finite && std::isfinite(u.tangential[k]);
+        if (!finite) return bad("principal point and coefficients must be finite");
+    }
+    return L3D_OK;
+}
+
+// kernel parameters of one image; the inverse camera matrix is formed like OpenCV's 3x3 inversion (cofactors / determinant)
+static L3DUndistImage ud_image(const l3d_undistort_desc& u, const unsigned char* src, long long src_pitch, unsigned char* dst, long long dst_pitch)
+{
+    L3DUndistImage d;
+    memset(&d, 0, sizeof(d));
+    d.src = src; d.dst = dst; d.src_pitch = src_pitch; d.dst_pitch = dst_pitch;
+    d.width = u.width; d.height = u.height; d.channels = u.channels;
+    d.tiles_x = (u.width + UD_TW - 1) / UD_TW;
+    const double det = u.fx * u.fy, id = 1.0 / det;
+    d.ir0 = u.fy * id; d.ir2 = -(u.cx * u.fy) * id; d.ir4 = u.fx * id; d.ir5 = -(u.fx * u.cy) * id;
+    d.fx = u.fx; d.fy = u.fy; d.cx = u.cx; d.cy = u.cy;
+    d.k1 = u.radial[0]; d.k2 = u.radial[1]; d.k3 = u.radial[2]; d.p1 = u.tangential[0]; d.p2 = u.tangential[1];
+    d.full_radial = d.k2 != 0.0 || d.k3 != 0.0;
+    d.tangential = d.p1 != 0.0 || d.p2 != 0.0;
+    return d;
+}
+
+static dim3 ud_grid(const l3d_undistort_desc& u) { return dim3((unsigned)((u.width + UD_TW - 1) / UD_TW), (unsigned)u.height); }
+
+extern "C" {
+
+int l3d_undistort_u8(l3d_ctx* c, int n, const l3d_undistort_desc* descs, int on_device)
+{
+    if (!c) return L3D_ERR_INVALID;
+    if (n < 0 || (n && !descs)) return l3d_fail(c, L3D_ERR_INVALID, "l3d_undistort_u8: bad arguments");
+    for (int i = 0; i < n; ++i) {
+        int rc = ud_check(c, descs[i], true, true, "l3d_undistort_u8");
+        if (rc) return rc;
+    }
+    if (n == 0) return L3D_OK;
+    cudaSetDevice(c->device);
+    UndistortState& s = c->undist;
+    int rc;
+    size_t staged = 0;                      // host mode: packed copies of every image on the device
+    if (!on_device) {
+        for (int i = 0; i < n; ++i) staged += (size_t)descs[i].width * descs[i].channels * descs[i].height;
+        L3D_RESERVE(s.d_src, staged, "undistort source staging");
+        L3D_RESERVE(s.d_dst, staged, "undistort output staging");
+    }
+    s.h_imgs.resize(n);
+    long long tiles = 0;
+    size_t off = 0;
+    for (int i = 0; i < n; ++i) {
+        const l3d_undistort_desc& u = descs[i];
+        const long long row = (long long)u.width * u.channels;
+        if (on_device) s.h_imgs[i] = ud_image(u, u.src, u.src_pitch, u.dst, u.dst_pitch);
+        else {
+            unsigned char* src = (unsigned char*)s.d_src.p + off;
+            L3D_CUDA(c, cudaMemcpy2DAsync(src, row, u.src, u.src_pitch, row, u.height, cudaMemcpyHostToDevice, c->stream), "upload image");
+            s.h_imgs[i] = ud_image(u, src, row, (unsigned char*)s.d_dst.p + off, row);
+            off += (size_t)row * u.height;
+        }
+        s.h_imgs[i].tile0 = tiles;
+        tiles += (long long)s.h_imgs[i].tiles_x * ((u.height + UD_TH - 1) / UD_TH);
+    }
+    if (tiles >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_undistort_u8: more than 2^31 tiles in one call");
+    L3D_RESERVE(s.d_imgs, sizeof(L3DUndistImage) * (size_t)n, "undistort descriptors");
+    // pageable host memory: the copy is staged before the call returns, so h_imgs may be rewritten by the next call right away
+    L3D_CUDA(c, cudaMemcpyAsync(s.d_imgs.p, s.h_imgs.data(), sizeof(L3DUndistImage) * n, cudaMemcpyHostToDevice, c->stream), "upload descriptors");
+    k_undistort_u8<<<(unsigned int)tiles, UD_TW, 0, c->stream>>>((const L3DUndistImage*)s.d_imgs.p, n);
+    ++c->launches;
+    L3D_CUDA(c, cudaGetLastError(), "k_undistort_u8");
+    if (!on_device) {
+        off = 0;
+        for (int i = 0; i < n; ++i) {
+            const l3d_undistort_desc& u = descs[i];
+            const size_t row = (size_t)u.width * u.channels;
+            L3D_CUDA(c, cudaMemcpy2DAsync(u.dst, u.dst_pitch, (const unsigned char*)s.d_dst.p + off, row, row, u.height, cudaMemcpyDeviceToHost, c->stream),
+                     "download image");
+            off += row * u.height;
+        }
+        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "l3d_undistort_u8");
+    }
+    return L3D_OK;
+}
+
+int l3d_undistort_map(l3d_ctx* c, const l3d_undistort_desc* desc, int16_t* map_xy, uint16_t* map_frac, int on_device)
+{
+    if (!c) return L3D_ERR_INVALID;
+    if (!desc || !map_xy || !map_frac) return l3d_fail(c, L3D_ERR_INVALID, "l3d_undistort_map: null pointer");
+    if (on_device && (((uintptr_t)map_xy & 3) || ((uintptr_t)map_frac & 1))) return l3d_fail(c, L3D_ERR_INVALID, "l3d_undistort_map: misaligned map");
+    int rc = ud_check(c, *desc, false, true, "l3d_undistort_map");
+    if (rc) return rc;
+    cudaSetDevice(c->device);
+    UndistortState& s = c->undist;
+    const size_t px = (size_t)desc->width * desc->height;
+    short2* xy = (short2*)map_xy; unsigned short* fr = map_frac;
+    if (!on_device) {
+        L3D_RESERVE(s.d_map_xy, 4 * px, "undistort map");
+        L3D_RESERVE(s.d_map_frac, 2 * px, "undistort map fractions");
+        xy = (short2*)s.d_map_xy.p; fr = (unsigned short*)s.d_map_frac.p;
+    }
+    k_undistort_map<<<ud_grid(*desc), UD_TW, 0, c->stream>>>(ud_image(*desc, nullptr, 0, nullptr, 0), xy, fr);
+    ++c->launches;
+    L3D_CUDA(c, cudaGetLastError(), "k_undistort_map");
+    if (!on_device) {
+        L3D_CUDA(c, cudaMemcpyAsync(map_xy, xy, 4 * px, cudaMemcpyDeviceToHost, c->stream), "download map");
+        L3D_CUDA(c, cudaMemcpyAsync(map_frac, fr, 2 * px, cudaMemcpyDeviceToHost, c->stream), "download map fractions");
+        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "l3d_undistort_map");
+    }
+    return L3D_OK;
+}
+
+int l3d_remap_u8(l3d_ctx* c, const l3d_undistort_desc* desc, const int16_t* map_xy, const uint16_t* map_frac, int on_device)
+{
+    if (!c) return L3D_ERR_INVALID;
+    if (!desc || !map_xy || !map_frac) return l3d_fail(c, L3D_ERR_INVALID, "l3d_remap_u8: null pointer");
+    if (on_device && (((uintptr_t)map_xy & 3) || ((uintptr_t)map_frac & 1))) return l3d_fail(c, L3D_ERR_INVALID, "l3d_remap_u8: misaligned map");
+    int rc = ud_check(c, *desc, true, false, "l3d_remap_u8");
+    if (rc) return rc;
+    cudaSetDevice(c->device);
+    UndistortState& s = c->undist;
+    const l3d_undistort_desc& u = *desc;
+    const size_t px = (size_t)u.width * u.height, row = (size_t)u.width * u.channels;
+    L3DUndistImage d = ud_image(u, u.src, u.src_pitch, u.dst, u.dst_pitch);
+    const short2* xy = (const short2*)map_xy; const unsigned short* fr = map_frac;
+    if (!on_device) {
+        L3D_RESERVE(s.d_src, row * u.height, "remap source staging");
+        L3D_RESERVE(s.d_dst, row * u.height, "remap output staging");
+        L3D_RESERVE(s.d_map_xy, 4 * px, "remap map");
+        L3D_RESERVE(s.d_map_frac, 2 * px, "remap map fractions");
+        L3D_CUDA(c, cudaMemcpy2DAsync(s.d_src.p, row, u.src, u.src_pitch, row, u.height, cudaMemcpyHostToDevice, c->stream), "upload image");
+        L3D_CUDA(c, cudaMemcpyAsync(s.d_map_xy.p, map_xy, 4 * px, cudaMemcpyHostToDevice, c->stream), "upload map");
+        L3D_CUDA(c, cudaMemcpyAsync(s.d_map_frac.p, map_frac, 2 * px, cudaMemcpyHostToDevice, c->stream), "upload map fractions");
+        d.src = (const unsigned char*)s.d_src.p; d.dst = (unsigned char*)s.d_dst.p; d.src_pitch = d.dst_pitch = (long long)row;
+        xy = (const short2*)s.d_map_xy.p; fr = (const unsigned short*)s.d_map_frac.p;
+    }
+    if (u.channels == 3) k_remap_u8<3><<<ud_grid(u), UD_TW, 0, c->stream>>>(d, xy, fr);
+    else k_remap_u8<1><<<ud_grid(u), UD_TW, 0, c->stream>>>(d, xy, fr);
+    ++c->launches;
+    L3D_CUDA(c, cudaGetLastError(), "k_remap_u8");
+    if (!on_device) {
+        L3D_CUDA(c, cudaMemcpy2DAsync(u.dst, u.dst_pitch, s.d_dst.p, row, row, u.height, cudaMemcpyDeviceToHost, c->stream), "download image");
+        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "l3d_remap_u8");
+    }
+    return L3D_OK;
+}
+
+} // extern "C"

@@ -9,6 +9,7 @@
 #include "../../include/line3d.h"
 #include <nvtx3/nvToolsExt.h>      // header-only; ranges show up in nsys / ncu timelines
 #include "../../include/l3d_capi.h"
+#include <cuda_runtime_api.h>          // cudaGetDevice: undistortImage runs on the caller's current device
 
 #include <algorithm>
 #include <chrono>
@@ -816,6 +817,31 @@ Matrix3d Line3D::rotationFromQ(const double Qw, const double Qx, const double Qy
     return R;
 }
 
+void Line3D::undistortImage(const Image8u& in, Image8u& out, const Vector3d& radial, const Vector2d& tangential, const Matrix3d& K)
+{
+    if (in.data.size() != (size_t)in.rows * in.cols * in.channels || in.rows < 0 || in.cols < 0)
+        throw std::invalid_argument("undistortImage: the pixel buffer does not match rows x cols x channels");
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) throw std::runtime_error("undistortImage: no usable CUDA device");
+    l3d_ctx* ctx = nullptr;
+    if (l3d_ctx_create(dev, &ctx) != L3D_OK) throw std::runtime_error("undistortImage: no usable CUDA device");
+    Image8u res(in.rows, in.cols, in.channels);       // a separate buffer: in and out may be the same image
+    l3d_undistort_desc d;
+    std::memset(&d, 0, sizeof(d));
+    d.width = in.cols; d.height = in.rows; d.channels = in.channels;
+    d.src_pitch = d.dst_pitch = (int64_t)in.cols * in.channels;
+    d.src = in.data.data(); d.dst = res.data.data();
+    d.fx = K(0, 0); d.fy = K(1, 1); d.cx = K(0, 2); d.cy = K(1, 2);
+    d.radial[0] = radial.x; d.radial[1] = radial.y; d.radial[2] = radial.z;
+    d.tangential[0] = tangential.x; d.tangential[1] = tangential.y;
+    const int rc = l3d_undistort_u8(ctx, 1, &d, 0);
+    const std::string msg = std::string("undistortImage: ") + l3d_last_error(ctx);
+    l3d_ctx_destroy(ctx);
+    if (rc == L3D_ERR_INVALID) throw std::invalid_argument(msg);
+    if (rc != L3D_OK) throw std::runtime_error(msg);
+    out = std::move(res);
+}
+
 }  // namespace L3DPP
 
 // ================================================================================================ C wrapper (tests / Python)
@@ -933,4 +959,17 @@ int l3dpp_set_lines(void* h, int nlines, const int* nseg, const double* segs6, c
     return 0;
 }
 int l3dpp_save_txt(void* h, const char* folder) { Line3D* L = (Line3D*)h; L->save3DLinesAsTXT(folder); return L->lastError()[0] ? -1 : 0; }
+// Line3D::undistortImage on a packed image; K row-major, radial[3], tangential[2].  0, -1 (std::invalid_argument) or -2 (std::runtime_error)
+int l3dpp_undistort_image(const unsigned char* src, unsigned char* dst, int rows, int cols, int channels, const double* radial, const double* tangential,
+                          const double* K)
+{
+    Image8u in(rows, cols, channels), out;
+    if (!in.data.empty()) memcpy(in.data.data(), src, in.data.size());
+    Matrix3d Km; memcpy(Km.m, K, 72);
+    try {
+        Line3D::undistortImage(in, out, Vector3d(radial[0], radial[1], radial[2]), Vector2d(tangential[0], tangential[1]), Km);
+    } catch (const std::invalid_argument&) { return -1; } catch (const std::exception&) { return -2; }
+    memcpy(dst, out.data.data(), out.data.size());
+    return 0;
+}
 }
