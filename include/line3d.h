@@ -11,12 +11,17 @@
  *     Eigen::Matrix3d, Eigen::Vector3d, std::vector<cv::Vec4f>) is available as an inline overload that converts and
  *     forwards; tests/test_cpu.py compiles it against the header stand-ins of oracle/ref_shim.  get3Dlines() returns the POD
  *     types (P1().x is a member, not Eigen's x()): a frontend that reads the result lines needs that one-character change.
- *   - addImage takes the image SIZE and explicit 2D segments (the reference's own line_segments argument,
- *     line3D.h:102-108); LSD detection inside addImage (line3D.cc:249-372) is outside the hot path (SURVEY.md §2 row 13).
+ *   - addImage takes the image SIZE and the 2D segments (the reference's own line_segments argument, line3D.h:102-108).  With no
+ *     segments it reads the reference's segment cache <output_folder>/L3D++_data/segments_L3D++_<camID>_<w>x<h>_3000.bin
+ *     (line3D.cc:295-309; segmentCachePath in include/line3d_io.h) when load_segments is true and the file exists, so a
+ *     folder the reference has run on gives it exactly the segments the reference used.  LSD detection inside addImage
+ *     (line3D.cc:249-372) is outside this library (SURVEY.md §2 row 13): without segments and without a cache file the view is
+ *     rejected and lastError() names the file that was looked for.
  *   - undistortImage (line3D.h:119-122) takes the owning Image8u and the POD vectors; with Eigen / OpenCV headers the reference's
  *     cv::Mat signature is an inline overload for CV_8UC1 / CV_8UC3.  It runs on the GPU and its map is defined by an explicit
  *     formula, which OpenCV builds reproduce to within one 1/32-px step (DESIGN.md §4a).
- *   - save3DLinesAsBIN (boost archive) is not provided; TXT / OBJ / STL are.
+ *   - save3DLinesAsBIN writes the reference's Boost binary archive without Boost (csrc/line3d_bin.cc, DESIGN.md §6a), like the
+ *     TXT / OBJ / STL writers; read3DLinesBIN reads such files back.
  *   - use_GPU selects the SCORING SEMANTICS of the reference's two paths; both run on the GPU (there is no CPU path).
  */
 #ifndef L3DPP_B200_LINE3D_H_
@@ -88,6 +93,9 @@ class Segment3D {   /* segment3D.h:35-94 */
 public:
     Segment3D();
     Segment3D(const Vector3d& P1, const Vector3d& P2);
+    /* every stored field as given, nothing recomputed: how a segment read from a .bin file (read3DLinesBIN) keeps its bits */
+    Segment3D(const Vector3d& P1, const Vector3d& P2, const Vector3d& dir, float length, bool valid)
+        : P1_(P1), P2_(P2), dir_(dir), length_(length), valid_(valid) {}
     float distance_Point2Line(const Vector3d& P) const;
     void translate(const Vector3d& t);
     Vector3d P1() const { return P1_; }
@@ -132,8 +140,8 @@ struct Line3DStats {
 
 class Line3D {
 public:
-    /* line3D.h:80-85.  output_folder / load_segments / max_img_width / max_line_segments only matter for the
-     * detection cache and the output filename (createOutputFilename). */
+    /* line3D.h:80-85.  output_folder / load_segments / max_img_width only matter for the segment cache (addImage without
+     * segments) and the output filename (createOutputFilename); max_line_segments is stored and not used (it bounds detection). */
     Line3D(const std::string& output_folder, const bool load_segments = L3D_DEF_LOAD_AND_STORE_SEGMENTS,
            const int max_img_width = L3D_DEF_MAX_IMG_WIDTH, const unsigned int max_line_segments = L3D_DEF_MAX_NUM_SEGMENTS,
            const bool neighbors_by_worldpoints = true, const bool use_GPU = true, const int cuda_device = 0);
@@ -141,15 +149,18 @@ public:
     Line3D(const Line3D&) = delete;
     Line3D& operator=(const Line3D&) = delete;
 
-    /* line3D.h:104-108 with (image_width, image_height) instead of cv::Mat& image; line_segments must be non-empty */
+    /* line3D.h:104-108 with (image_width, image_height) instead of cv::Mat& image.  An empty line_segments list reads the segment
+     * cache segmentCachePath(output_folder, camID, image_width, image_height, max_img_width) when load_segments is true; its
+     * segments are used as stored (line3D.cc:303-307: already upscaled, length-filtered and longest first, not truncated). */
     /* Returns false (and sets lastError(), which a later successful addImage does not clear) if the view was rejected. */
     bool addImage(const unsigned int camID, const int image_width, const int image_height, const Matrix3d& K, const Matrix3d& R,
                   const Vector3d& t, const float median_depth, const std::list<unsigned int>& wps_or_neighbors,
                   const std::vector<Vec4f>& line_segments);
 
 #ifdef L3DPP_WITH_EIGEN_OPENCV
-    /* The reference's exact signature (line3D.h:104-108).  The image only contributes its size; line_segments must be given
-     * (line detection is outside this library, SURVEY.md §2 row 13): with an empty list the call fails like any other rejected view. */
+    /* The reference's exact signature (line3D.h:104-108).  The image only contributes its size.  With an empty list (the frontends'
+     * call, main_vsfm.cpp:306) the segments come from the segment cache as above; line detection is outside this library
+     * (SURVEY.md §2 row 13), so without a cache file the call fails like any other rejected view. */
     bool addImage(const unsigned int camID, cv::Mat& image, const Eigen::Matrix3d& K, const Eigen::Matrix3d& R, const Eigen::Vector3d& t,
                   const float median_depth, const std::list<unsigned int>& wps_or_neighbors,
                   const std::vector<cv::Vec4f>& line_segments = std::vector<cv::Vec4f>())
@@ -177,6 +188,9 @@ public:
     void saveResultAsSTL(const std::string& output_folder);            /* line3D.h:183-185 */
     void saveResultAsOBJ(const std::string& output_folder);
     void save3DLinesAsTXT(const std::string& output_folder);
+    /* line3D.h:185: <output_folder>/<createOutputFilename()>.bin, the reference's Boost binary archive of get3Dlines() (every
+     * field at full precision; read it back with read3DLinesBIN, include/line3d_io.h).  With no 3D lines nothing is written. */
+    void save3DLinesAsBIN(const std::string& output_folder);
     Vector4f getSegmentCoords2D(const Segment2D& seg2D);               /* line3D.h:196-198 */
     Vector4f getSegmentCoords2D(const unsigned int camID, const unsigned int segID);
     size_t numImages();                                                /* line3D.h:205 */

@@ -1,6 +1,6 @@
 /* include/line3d_io.h — input format of the VisualSfM frontend (SURVEY.md §8f-2): what main_vsfm.cpp:143-310 reads from an
  * .nvm file before it calls Line3D::addImage, as a library function so that a frontend built on include/line3d.h needs no
- * parsing code of its own.  Host-only; no CUDA involved. */
+ * parsing code of its own; and the reference's binary result file and segment cache.  Host-only; no CUDA involved. */
 #ifndef L3DPP_LINE3D_IO_H_
 #define L3DPP_LINE3D_IO_H_
 #include "line3d.h"
@@ -48,6 +48,24 @@ bool readColmap(const std::string& sfm_folder, std::vector<SfMCamera>& cameras, 
 
 /* K of main_vsfm.cpp:266-278: focal on the diagonal, principal point at the image centre (float arithmetic like the reference) */
 Matrix3d intrinsicsFromFocal(float focal, int image_width, int image_height);
+
+/* The reference's two binary files, Boost binary_oarchive layout without Boost (csrc/line3d_bin.cc, DESIGN.md §6a).  The readers
+ * take input from outside the program: a malformed, truncated or foreign file returns false with *error set, never crashes and
+ * never allocates more than the file's size warrants.  The writers return false with *error set when the file cannot be written. */
+
+/* <name>.bin of save3DLinesAsBIN (line3D.cc:2690-2711): std::vector<FinalLine3D> with every double of P1 / P2 / dir, the float
+ * length, the valid flag and every residual's (camID, segID).  Segments are restored bit for bit (no field is recomputed). */
+bool read3DLinesBIN(const std::string& path, std::vector<FinalLine3D>& lines, std::string* error = 0);
+bool write3DLinesBIN(const std::string& path, const std::vector<FinalLine3D>& lines, std::string* error = 0);
+
+/* one view's segment cache (DataArray<float4>, line3D.cc:295-309, 363-366): (x1, y1, x2, y2) per segment in file order */
+bool readSegmentCache(const std::string& path, std::vector<Vec4f>& segments, std::string* error = 0);
+bool writeSegmentCache(const std::string& path, const std::vector<Vec4f>& segments, std::string* error = 0);
+
+/* <output_folder>/L3D++_data/segments_L3D++_<camID>_<w>x<h>_3000.bin (line3D.cc:271-300).  <w>x<h> is the image size, or the size
+ * cv::resize(img, out, Size(), s, s) gives with s = float(max_img_width) / float(max(w, h)) when max_img_width > 0 and the larger
+ * side exceeds it.  The suffix is L3D_DEF_MAX_NUM_SEGMENTS, whatever max_line_segments is. */
+std::string segmentCachePath(const std::string& output_folder, unsigned int camID, int image_width, int image_height, int max_img_width);
 
 }  // namespace L3DPP
 #endif

@@ -7,6 +7,7 @@
 // (2036-2071), graph clustering (clustering.cc:6-48) and the cluster -> 3D segment tail (2079-2452) + writers.
 // All matching / scoring / affinity / diffusion arithmetic runs on the GPU; without a GPU the constructor fails.
 #include "../../include/line3d.h"
+#include "../../include/line3d_io.h"   // segment cache + .bin writer (csrc/line3d_bin.cc)
 #include <nvtx3/nvToolsExt.h>      // header-only; ranges show up in nsys / ncu timelines
 #include "../../include/l3d_capi.h"
 #include <cuda_runtime_api.h>          // cudaGetDevice: undistortImage runs on the caller's current device
@@ -358,6 +359,17 @@ bool Line3D::addImage(const unsigned int camID, const int w, const int h, const 
     // everything that needs no shared state first (the reference's frontends call addImage from an OpenMP loop) ...
     HostView v;
     v.id = camID; v.width = w; v.height = h; v.K = K; v.R = R; v.t = t; v.lines = line_segments; v.wps_or_neighbors = wps_or_neighbors;
+    // no segments given: the reference's segment cache, used as stored (detectLineSegments line3D.cc:295-309).  output_folder,
+    // load_segments and max_img_width are fixed at construction, so this needs no lock either.
+    std::string no_segments;
+    if (line_segments.empty()) {
+        const std::string path = segmentCachePath(P.output_folder, camID, w, h, P.max_img_width);
+        std::string e;
+        if (!P.load_segments) no_segments = "no line segments given, and load_segments is off so the segment cache " + path + " was not read";
+        else if (!std::ifstream(path.c_str(), std::ios::binary)) no_segments = "no line segments given and no segment cache " + path + " (line detection is outside this library)";
+        else if (!readSegmentCache(path, v.lines, &e)) no_segments = "unreadable segment cache " + e;
+        else if (v.lines.empty()) no_segments = "the segment cache " + path + " holds no segments";
+    }
     v.min_line_length = std::sqrt(float((unsigned)w * (unsigned)w + (unsigned)h * (unsigned)h)) * 0.005f;                           // view.cc:17-18
     v.pp = Vector3d(K(0, 2), K(1, 2), 1.0);
     const Matrix3d Rt = transposed(R);
@@ -371,7 +383,7 @@ bool Line3D::addImage(const unsigned int camID, const int w, const int h, const 
     auto failed = [&](const std::string& what) { P.fail("addImage [" + std::to_string(camID) + "]: " + what); return false; };
     if (std::max(w, h) < 800) return failed("image is too small for reliable results (larger side should be >= 800px)");   // line3D.cc:119
     if (wps_or_neighbors.empty()) return failed(P.by_wps ? "view has no worldpoints" : "view has no visual neighbors");    // line3D.cc:154
-    if (line_segments.empty()) return failed("no line segments given (LSD detection is outside this library's scope)");
+    if (v.lines.empty()) return failed(no_segments);
     if (P.views.count(camID)) return failed("camera ID already in use");                                                     // line3D.cc:130
     if (P.by_wps) for (unsigned int wp : wps_or_neighbors) P.wps2views[wp].push_back(camID);
     P.views[camID] = v;
@@ -765,6 +777,16 @@ void Line3D::save3DLinesAsTXT(const std::string& folder)   // line3D.cc:2631-268
     }
 }
 
+// the reference's Boost binary archive of lines3D_ (line3D.cc:2690-2711), written by csrc/line3d_bin.cc
+void Line3D::save3DLinesAsBIN(const std::string& folder)
+{
+    std::lock_guard<std::mutex> g(p_->mtx);
+    p_->err.clear();
+    if (p_->lines3D.empty()) { p_->fail("no 3D lines to save!"); return; }
+    std::string e;
+    if (!write3DLinesBIN(folder + "/" + createOutputFilename() + ".bin", p_->lines3D, &e)) p_->fail(e);
+}
+
 // Wavefront OBJ as the reference writes it (line3D.cc:2568-2628): all vertices first ("v x y z", two per 3D segment,
 // default ostream formatting), then one "l a b" element per segment with 1-based vertex indices.
 void Line3D::saveResultAsOBJ(const std::string& folder)
@@ -851,6 +873,11 @@ void* l3dpp_create(int neighbors_by_worldpoints, int use_gpu, int device)
 {
     try { return new Line3D("", true, -1, 3000, neighbors_by_worldpoints != 0, use_gpu != 0, device); } catch (...) { return nullptr; }
 }
+// the full constructor: output folder, segment cache switch and max_img_width as Line3D takes them
+void* l3dpp_create_in(const char* output_folder, int load_segments, int max_img_width, int neighbors_by_worldpoints, int use_gpu, int device)
+{
+    try { return new Line3D(output_folder, load_segments != 0, max_img_width, 3000, neighbors_by_worldpoints != 0, use_gpu != 0, device); } catch (...) { return nullptr; }
+}
 void l3dpp_destroy(void* h) { delete (Line3D*)h; }
 const char* l3dpp_last_error(void* h) { return ((Line3D*)h)->lastError(); }
 void* l3dpp_ctx(void* h) { return ((Line3D*)h)->impl()->ctx; }
@@ -934,6 +961,8 @@ long long l3dpp_get_residuals(void* h, l3dpp_residual* out, long long cap)
         for (const Segment2D& s : *L[i].underlyingCluster_.residuals()) { if (out && n < cap) { out[n].line = (int)i; out[n].cam = s.camID(); out[n].seg = s.segID(); } ++n; }
     return n;
 }
+// get3Dlines() as a handle of the l3dpp_bin_* functions (csrc/line3d_bin.cc): every field, for comparison with a .bin file
+void* l3dpp_lines_handle(void* h) { std::vector<FinalLine3D>* v = new std::vector<FinalLine3D>(); ((Line3D*)h)->get3Dlines(*v); return v; }
 int l3dpp_save_obj(void* h, const char* folder) { Line3D* L = (Line3D*)h; L->saveResultAsOBJ(folder); return L->lastError()[0] ? -1 : 0; }
 int l3dpp_save_stl(void* h, const char* folder) { Line3D* L = (Line3D*)h; L->saveResultAsSTL(folder); return L->lastError()[0] ? -1 : 0; }
 int l3dpp_output_filename(void* h, char* buf, int cap)
@@ -959,6 +988,7 @@ int l3dpp_set_lines(void* h, int nlines, const int* nseg, const double* segs6, c
     return 0;
 }
 int l3dpp_save_txt(void* h, const char* folder) { Line3D* L = (Line3D*)h; L->save3DLinesAsTXT(folder); return L->lastError()[0] ? -1 : 0; }
+int l3dpp_save_bin(void* h, const char* folder) { Line3D* L = (Line3D*)h; L->save3DLinesAsBIN(folder); return L->lastError()[0] ? -1 : 0; }
 // Line3D::undistortImage on a packed image; K row-major, radial[3], tangential[2].  0, -1 (std::invalid_argument) or -2 (std::runtime_error)
 int l3dpp_undistort_image(const unsigned char* src, unsigned char* dst, int rows, int cols, int channels, const double* radial, const double* tangential,
                           const double* K)

@@ -26,14 +26,22 @@ def _p(a):
 class Line3D:
     """addImage / matchImages / reconstruct3Dlines with the reference's argument meaning (line3D.h:80-166)."""
 
-    def __init__(self, neighbors_by_worldpoints=True, use_gpu=True, device=0):
+    def __init__(self, neighbors_by_worldpoints=True, use_gpu=True, device=0, output_folder=None, load_segments=True, max_img_width=-1):
+        """output_folder / load_segments / max_img_width: the reference's constructor arguments; with an output folder, add_image
+        with no segments reads the segment cache under <output_folder>/L3D++_data/ (segment_cache_path)"""
         self.L = capi.lib()
         self.L.l3dpp_create.restype = C.c_void_p
+        self.L.l3dpp_create_in.restype = C.c_void_p
         self.L.l3dpp_ctx.restype = C.c_void_p
         self.L.l3dpp_last_error.restype = C.c_char_p
         for n in ("l3dpp_get_affinity", "l3dpp_get_segments3d", "l3dpp_get_residuals", "l3d_get_view_matches", "l3d_get_estimates"):
             getattr(self.L, n).restype = C.c_longlong
-        self.h = C.c_void_p(self.L.l3dpp_create(int(neighbors_by_worldpoints), int(use_gpu), int(device)))
+        if output_folder is None:
+            h = self.L.l3dpp_create(int(neighbors_by_worldpoints), int(use_gpu), int(device))
+        else:
+            h = self.L.l3dpp_create_in(str(output_folder).encode(), int(load_segments), int(max_img_width), int(neighbors_by_worldpoints),
+                                       int(use_gpu), int(device))
+        self.h = C.c_void_p(h)
         if not self.h:
             raise capi.L3DError("L3DPP::Line3D: no usable CUDA device (no CPU fallback)")
         self.ctx = C.c_void_p(self.L.l3dpp_ctx(self.h))
@@ -51,9 +59,10 @@ class Line3D:
             raise capi.L3DError(f"{what}: {self.L.l3dpp_last_error(self.h).decode()}")
         return rc
 
-    def add_image(self, cam, width, height, K, R, t, median_depth, wps_or_neighbors, segs):
+    def add_image(self, cam, width, height, K, R, t, median_depth, wps_or_neighbors, segs=()):
+        """segs: float32 [n, 4]; empty: read the view's segment cache (see __init__)"""
         lst = np.ascontiguousarray(wps_or_neighbors, np.uint32)
-        segs = np.ascontiguousarray(segs, np.float32)
+        segs = np.ascontiguousarray(segs, np.float32).reshape(-1, 4)
         f64 = lambda a: np.ascontiguousarray(a, np.float64)
         self._chk(self.L.l3dpp_add_image(self.h, C.c_uint(int(cam)), int(width), int(height), _p(f64(K)), _p(f64(R)), _p(f64(t)),
                                          C.c_float(float(median_depth)), _p(lst), len(lst), _p(segs), len(segs)), "addImage")
@@ -147,3 +156,102 @@ class Line3D:
 
     def save_txt(self, folder):
         self._chk(self.L.l3dpp_save_txt(self.h, folder.encode()), "save3DLinesAsTXT")
+
+    def lines(self):
+        """get3Dlines() with every field, in the layout read_lines_bin returns"""
+        self.L.l3dpp_lines_handle.restype = C.c_void_p
+        return _lines_from_handle(_io_lib(), C.c_void_p(self.L.l3dpp_lines_handle(self.h)))
+
+    def save_bin(self, folder):
+        """save3DLinesAsBIN: <folder>/<createOutputFilename()>.bin; nothing is written (and L3DError is raised) without 3D lines"""
+        self._chk(self.L.l3dpp_save_bin(self.h, str(folder).encode()), "save3DLinesAsBIN")
+
+    def output_filename(self):
+        buf = C.create_string_buffer(1024)
+        self._chk(self.L.l3dpp_output_filename(self.h, buf, 1024), "createOutputFilename")
+        return buf.value.decode()
+
+
+# ---- the reference's binary files (include/line3d_io.h, csrc/line3d_bin.cc); host only, no GPU needed
+LINE_DT = np.dtype([("nseg", "<i4"), ("nres", "<i4"), ("reference_view", "<u4"), ("_pad", "<i4")])
+BIN_SEG_DT = np.dtype([("line", "<i4"), ("valid", "<i4"), ("length", "<f4"), ("_pad", "<i4"), ("p1", "<f8", 3), ("p2", "<f8", 3),
+                       ("dir", "<f8", 3)])
+
+
+def _io_lib():
+    L = capi.lib()
+    for n in ("l3dpp_bin_open", "l3dpp_segcache_open"):
+        getattr(L, n).restype = C.c_void_p
+    L.l3dpp_segcache_count.restype = C.c_longlong
+    return L
+
+
+def read_lines_bin(path):
+    """read3DLinesBIN: a .bin result file as numpy arrays.  Returns dict(lines: LINE_DT [L] (segment / residual counts, reference
+    view), clusters: BIN_SEG_DT [L] (each cluster's own 3D line), segments: BIN_SEG_DT [S], residuals: RESID_DT [R]); segments and
+    residuals of line i are consecutive and carry line = i.  Raises L3DError with the reader's message on a malformed file."""
+    L = _io_lib()
+    err = C.create_string_buffer(1024)
+    h = L.l3dpp_bin_open(str(path).encode(), err, 1024)
+    if not h:
+        raise capi.L3DError(err.value.decode())
+    return _lines_from_handle(L, C.c_void_p(h))
+
+
+def _lines_from_handle(L, h):
+    """the arrays of a std::vector<FinalLine3D> handle (l3dpp_bin_*); closes the handle"""
+    try:
+        nl, ns, nr = C.c_longlong(), C.c_longlong(), C.c_longlong()
+        L.l3dpp_bin_sizes(h, C.byref(nl), C.byref(ns), C.byref(nr))
+        out = dict(lines=np.zeros(nl.value, LINE_DT), clusters=np.zeros(nl.value, BIN_SEG_DT), segments=np.zeros(ns.value, BIN_SEG_DT),
+                   residuals=np.zeros(nr.value, RESID_DT))
+        L.l3dpp_bin_get(h, _p(out["lines"]), _p(out["clusters"]), _p(out["segments"]), _p(out["residuals"]))
+    finally:
+        L.l3dpp_bin_close(h)
+    return out
+
+
+def write_lines_bin(path, d):
+    """write3DLinesBIN of a dict as read_lines_bin returns it"""
+    lines = np.ascontiguousarray(d["lines"], LINE_DT)
+    clusters = np.ascontiguousarray(d["clusters"], BIN_SEG_DT)
+    segs = np.ascontiguousarray(d["segments"], BIN_SEG_DT)
+    res = np.ascontiguousarray(d["residuals"], RESID_DT)
+    if len(clusters) != len(lines) or lines["nseg"].sum() != len(segs) or lines["nres"].sum() != len(res):
+        raise ValueError("clusters must have one entry per line, and the per-line counts must add up to the segment / residual arrays")
+    err = C.create_string_buffer(1024)
+    if _io_lib().l3dpp_bin_write(str(path).encode(), C.c_longlong(len(lines)), _p(lines), _p(clusters), _p(segs), _p(res), err, 1024) != 0:
+        raise capi.L3DError(err.value.decode())
+
+
+def read_segment_cache(path):
+    """readSegmentCache: a view's cached 2D segments as float32 [n, 4] (x1, y1, x2, y2)"""
+    L = _io_lib()
+    err = C.create_string_buffer(1024)
+    h = L.l3dpp_segcache_open(str(path).encode(), err, 1024)
+    if not h:
+        raise capi.L3DError(err.value.decode())
+    h = C.c_void_p(h)
+    try:
+        out = np.zeros((L.l3dpp_segcache_count(h), 4), np.float32)
+        L.l3dpp_segcache_get(h, _p(out))
+    finally:
+        L.l3dpp_segcache_close(h)
+    return out
+
+
+def write_segment_cache(path, segs):
+    """writeSegmentCache of float32 [n, 4] segments"""
+    segs = np.ascontiguousarray(segs, np.float32).reshape(-1, 4)
+    err = C.create_string_buffer(1024)
+    if _io_lib().l3dpp_segcache_write(str(path).encode(), _p(segs), C.c_longlong(len(segs)), err, 1024) != 0:
+        raise capi.L3DError(err.value.decode())
+
+
+def segment_cache_path(output_folder, cam, width, height, max_img_width=-1):
+    """segmentCachePath: <output_folder>/L3D++_data/segments_L3D++_<cam>_<w>x<h>_3000.bin"""
+    buf = C.create_string_buffer(4096)
+    n = _io_lib().l3dpp_segcache_path(str(output_folder).encode(), C.c_uint(int(cam)), int(width), int(height), int(max_img_width), buf, 4096)
+    if n < 0:
+        raise ValueError("path too long")
+    return buf.value.decode()
