@@ -9,6 +9,7 @@
 //                       so the result is bit-identical to the reference kernels; the linear search for the transposed
 //                       slot (cudawrapper.cu:524-542) is replaced by a precomputed permutation.
 #include "l3d_cub.cuh"
+#include "l3d_device_f64.cuh"
 #include "l3d_sweep.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
@@ -22,51 +23,15 @@
 #include <cstdlib>
 #include <vector>
 
-#define L3D_EPS_D 1e-12
-#define L3D_PI_D 3.14159265358979323846
-
-struct A3 { double x, y, z; };
-__device__ __forceinline__ A3 a3(double x, double y, double z) { A3 r; r.x = x; r.y = y; r.z = z; return r; }
-__device__ __forceinline__ A3 asub(A3 a, A3 b) { return a3(a.x - b.x, a.y - b.y, a.z - b.z); }
-__device__ __forceinline__ double adot(A3 a, A3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
-__device__ __forceinline__ double anorm(A3 a) { return sqrt(adot(a, a)); }
-struct ASeg { A3 P1, P2, dir; float length; };
-// Segment3D(P1,P2) (segment3D.h:48-66)
-__device__ __forceinline__ ASeg make_seg(const double* p)
-{
-    ASeg s;
-    A3 P1 = a3(p[0], p[1], p[2]), P2 = a3(p[3], p[4], p[5]);
-    s.length = (float)anorm(asub(P1, P2));
-    if (s.length > L3D_EPS_D) {
-        s.P1 = P1; s.P2 = P2;
-        A3 d = asub(P2, P1);
-        double n2 = adot(d, d);
-        if (n2 > 0) { double n = sqrt(n2); d = a3(d.x / n, d.y / n, d.z / n); }
-        s.dir = d;
-    } else { s.P1 = s.P2 = s.dir = a3(0, 0, 0); s.length = 0.0f; }
-    return s;
-}
-// Segment3D::distance_Point2Line (segment3D.h:69-73): P1 + (dir * (P-P1)^T) * dir, evaluated as (outer product) * dir
-__device__ __forceinline__ float dist_p2l(const ASeg& s, A3 P)
-{
-    A3 w = asub(P, s.P1);
-    double d[3] = {s.dir.x, s.dir.y, s.dir.z}, ww[3] = {w.x, w.y, w.z}, h[3];
-#pragma unroll
-    for (int i = 0; i < 3; ++i) h[i] = (d[i] * ww[0]) * d[0] + (d[i] * ww[1]) * d[1] + (d[i] * ww[2]) * d[2];
-    A3 hp = a3(s.P1.x + h[0], s.P1.y + h[1], s.P1.z + h[2]);
-    return (float)anorm(asub(hp, P));
-}
-
 // Line3D::similarity(s1, m1, seg2, truncate = false) (line3D.cc:1467-1553) for two segments that both have a 3D estimate:
 // P1/P2 = their estimates (6 doubles each), m1/m2 = depths of their best matches, v1/v2 = their views
 __device__ __forceinline__ float aff_similarity(const L3DViewDev* v1, const L3DViewDev* v2, const double* P1, const double* P2, float4 m1, float4 m2,
                                                 float two_sigA_sqr, float med_scene_depth_lines)
 {
-    const ASeg s1 = make_seg(P1), s2 = make_seg(P2);
+    const Seg3D s1 = seg3d(d3(P1[0], P1[1], P1[2]), d3(P1[3], P1[4], P1[5]));
+    const Seg3D s2 = seg3d(d3(P2[0], P2[1], P2[2]), d3(P2[3], P2[4], P2[5]));
     if (s1.length < L3D_EPS_D || s2.length < L3D_EPS_D) return 0.0f;
-    float dot_p = (float)adot(s1.dir, s2.dir);                               // angleBetweenSeg3D (line3D.cc:1571-1583)
-    float angle = (float)((double)acosf(fmaxf(fminf(dot_p, 1.0f), -1.0f)) / L3D_PI_D * (double)180.0f);
-    if (angle > 90.0f) angle = 180.0f - angle;
+    const float angle = undirected_angle_deg((float)ddot(s1.dir, s2.dir));         // angleBetweenSeg3D (line3D.cc:1571-1583)
     float sim_a = expf(-angle * angle / two_sigA_sqr);
     float cutoff1 = v1->median_depth, cutoff2 = v2->median_depth;
     if (med_scene_depth_lines > L3D_EPS_D) { cutoff1 = fminf(cutoff1, med_scene_depth_lines); cutoff2 = fminf(cutoff2, med_scene_depth_lines); }
@@ -101,9 +66,7 @@ k_affinity(const L3DViewDev* __restrict__ views, const long long* __restrict__ r
     const long long x = kx[q];                   // the q-th kept match in emission order
     int flag = 0; float sim = 0.0f; long long gi = -1, gj = -1;
     {
-        int lo = 0, hi = V - 1;                  // processing rank whose region contains x
-        while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (region_off[mid] <= x) lo = mid; else hi = mid - 1; }
-        const int v1i = order[lo];
+        const int v1i = order[last_le(V, x, [&](int i) { return region_off[i]; })];      // the view whose region contains x
         const SwEntry me = sw_decode(M.e_val[x], M.pairs, M.row_off, M.num_pairs, M.knn, M.recs);
         const L3DViewDev* v1 = views + v1i;
         const L3DViewDev* v2 = views + me.tgt_view;
@@ -137,8 +100,7 @@ k_aff_events(const L3DViewDev* __restrict__ views, const long long* __restrict__
 {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= N) return;
-    int lo = 0, hi = V - 1;                      // processing rank of segment t
-    while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (segrank_off[mid] <= t) lo = mid; else hi = mid - 1; }
+    const int lo = last_le(V, t, [&](int i) { return segrank_off[i]; });          // processing rank of segment t
     const int v1i = order[lo];
     const L3DViewDev* v1 = views + v1i;
     const long long g = v1->seg_off + (t - segrank_off[lo]);

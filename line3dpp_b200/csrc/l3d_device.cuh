@@ -34,6 +34,16 @@ struct L3DPairDev {
     long long arc_off;      // first entry of this pair in the array of target arcs (level-1 pre-filter, k_pair_arcs)
 };
 
+// "which entry owns index x" over a table of first indices: the last i in [0, n) with key(i) <= x, 0 if there is none.
+// key(i) must not decrease with i; n >= 1.
+template <typename T, typename Key>
+__device__ __forceinline__ int last_le(int n, T x, Key key)
+{
+    int lo = 0, hi = n - 1;
+    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (key(mid) <= x) lo = mid; else hi = mid - 1; }
+    return lo;
+}
+
 // ---- level-1 pre-filter: the pencil parameter -----------------------------------------------------------------------
 // All epipolar lines F*p of one view pair pass through the epipole E of the target image, i.e. they live in the 2-D subspace
 // {e : e . E = 0} of R^3.  With image coordinates divided by L3D_ARC_SCALE (so that points are ~unit vectors and the subspace is

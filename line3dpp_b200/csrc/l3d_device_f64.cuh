@@ -1,5 +1,8 @@
 // l3d_device_f64.cuh — double-precision device arithmetic: the host-side double code of view.cc / line3D.cc and the
 // reference's CPU twins (matchingCPU line3D.cc:900-1015, scoringCPU 1208-1294) restated for the device.
+// This is the single home of the device's double geometry: the 3-vector and its operations, Segment3D and the
+// undirected angle between 3D segments.  Every kernel that needs one of them includes this header instead of
+// restating it, so a parity fix lands in one place.
 //
 // ARITHMETIC CONTRACT.  Compiled with -fmad=false; IEEE double add/mul/div/sqrt on the GPU round exactly like the host's,
 // so everything here that uses only those operations is bit-identical to oracle/l3d_oracle.cc (built with
@@ -8,6 +11,7 @@
 #include "l3d_device.cuh"
 
 #define L3D_EPS_D 1e-12
+#define L3D_PI_D 3.14159265358979323846
 
 struct D3 { double x, y, z; };
 __device__ __forceinline__ D3 d3(double x, double y, double z) { D3 r; r.x = x; r.y = y; r.z = z; return r; }
@@ -25,6 +29,44 @@ __device__ __forceinline__ D3 dmulmat(const double* M, D3 v)
 { return d3(M[0] * v.x + M[1] * v.y + M[2] * v.z, M[3] * v.x + M[4] * v.y + M[5] * v.z, M[6] * v.x + M[7] * v.y + M[8] * v.z); }
 // View::getNormalizedRay (view.cc:317-321)
 __device__ __forceinline__ D3 dray(const double* M, double x, double y) { return dnormalized(dmulmat(M, d3(x, y, 1.0))); }
+
+// Segment3D(P1, P2) (segment3D.h:48-66): a segment whose float length is not above 1e-12 collapses to zero.
+// n2 > 1e-20 already implies (float)sqrt(n2) > 1e-12; testing it first keeps the sqrt off the common path of callers
+// that only need the direction.  Selects rather than if/else: the branching form gave k_aff_events<false> 102 registers
+// instead of 94, one resident CTA less per SM, and made it 20 % slower.
+struct Seg3D { D3 P1, P2, dir; float length; };
+__device__ __forceinline__ Seg3D seg3d(D3 P1, D3 P2)
+{
+    const D3 d = dsub(P1, P2);
+    const double n2 = ddot(d, d);
+    const float length = (float)sqrt(n2);
+    const bool valid = n2 > 1e-20 || length > L3D_EPS_D;
+    const D3 zero = d3(0, 0, 0);
+    Seg3D s;
+    s.P1 = valid ? P1 : zero;
+    s.P2 = valid ? P2 : zero;
+    s.dir = valid ? dnormalized(dsub(P2, P1)) : zero;
+    s.length = valid ? length : 0.0f;
+    return s;
+}
+// Segment3D::distance_Point2Line (segment3D.h:69-73): P1 + (dir * (P-P1)^T) * dir, evaluated as (outer product) * dir
+__device__ __forceinline__ float dist_p2l(const Seg3D& s, D3 P)
+{
+    const D3 w = dsub(P, s.P1);
+    const double d[3] = {s.dir.x, s.dir.y, s.dir.z}, ww[3] = {w.x, w.y, w.z};
+    double h[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) h[i] = (d[i] * ww[0]) * d[0] + (d[i] * ww[1]) * d[1] + (d[i] * ww[2]) * d[2];
+    return (float)dnorm(dsub(d3(s.P1.x + h[0], s.P1.y + h[1], s.P1.z + h[2]), P));
+}
+// undirected angle in degrees, [0, 90], from the float cosine of two directions: D_undirected_angle_3D_DEG
+// (cudawrapper.cu:46-53) and angleBetweenSeg3D (line3D.cc:1571-1583) alike: float acos, DOUBLE divide by pi, times 180, back to float
+__device__ __forceinline__ float undirected_angle_deg(float c)
+{
+    float angle = (float)((double)acosf(fmaxf(fminf(c, 1.0f), -1.0f)) / L3D_PI_D * (double)180.0f);
+    if (angle > 90.0f) angle = 180.0f - angle;
+    return angle;
+}
 
 // ---- matchingCPU -------------------------------------------------------------------------------------------------
 // per-segment cache of the double path: viewing rays of both endpoints and the normalised normal of their plane

@@ -25,12 +25,7 @@ __global__ void __launch_bounds__(256) k_prep_segments(const float4* __restrict_
 {
     long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= total) return;
-    int lo = 0, hi = num_views - 1;            // last view with seg_off <= idx
-    while (lo < hi) {
-        int mid = (lo + hi + 1) >> 1;
-        if (views[mid].seg_off <= idx) lo = mid; else hi = mid - 1;
-    }
-    const L3DViewDev* v = views + lo;
+    const L3DViewDev* v = views + last_le(num_views, idx, [&](int i) { return views[i].seg_off; });
     float4 s = segs[idx];
     float3 r1 = normalize3(mulmat_h(v->RtKinv, s.x, s.y));
     float3 r2 = normalize3(mulmat_h(v->RtKinv, s.z, s.w));
@@ -46,12 +41,7 @@ __global__ void __launch_bounds__(256) k_prep_segments_f64(const float4* __restr
 {
     long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= total) return;
-    int lo = 0, hi = num_views - 1;
-    while (lo < hi) {
-        int mid = (lo + hi + 1) >> 1;
-        if (views[mid].seg_off <= idx) lo = mid; else hi = mid - 1;
-    }
-    const L3DViewDev* v = views + lo;
+    const L3DViewDev* v = views + last_le(num_views, idx, [&](int i) { return views[i].seg_off; });
     float4 s = segs[idx];
     D3 r1 = dray(v->RtKinv_d, (double)s.x, (double)s.y), r2 = dray(v->RtKinv_d, (double)s.z, (double)s.w);
     D3 n = dnormalized(dcross(r1, r2));
@@ -737,11 +727,7 @@ __global__ void __launch_bounds__(DK_THREADS, DK_MINB)
 k_match_dense_batch(const L3DDenseJob* __restrict__ jobs, int njobs, float epi)
 {
     __shared__ int job_s;
-    if (threadIdx.x == 0) {
-        int lo = 0, hi = njobs - 1;
-        while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (jobs[mid].tile0 <= (long long)blockIdx.x) lo = mid; else hi = mid - 1; }
-        job_s = lo;
-    }
+    if (threadIdx.x == 0) job_s = last_le(njobs, (long long)blockIdx.x, [&](int i) { return jobs[i].tile0; });
     __syncthreads();
     const L3DDenseJob& J = jobs[job_s];
     const int t = (int)((long long)blockIdx.x - J.tile0);

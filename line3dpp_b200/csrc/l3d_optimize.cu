@@ -19,6 +19,7 @@
 // tree; parity is pinned on the reference's own before/after result fixtures (tests/golden/line3dpp_ref_opt_pairs_v1.npz).
 // This file keeps nvcc's default FMA contraction off like the rest of the library (-fmad=false); nothing here is bit-pinned.
 #include "l3d_ctx.cuh"
+#include "l3d_device_f64.cuh"
 
 #include <algorithm>
 #include <cfloat>
@@ -139,12 +140,6 @@ __device__ bool solve4(const double* A, const double* D2, const double* b, doubl
     return isfinite(y[0]) && isfinite(y[1]) && isfinite(y[2]) && isfinite(y[3]);
 }
 
-struct D3 { double x, y, z; };
-__device__ __forceinline__ D3 d3(double x, double y, double z) { D3 r; r.x = x; r.y = y; r.z = z; return r; }
-__device__ __forceinline__ D3 dcross(D3 a, D3 b) { return d3(a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x); }
-__device__ __forceinline__ double dnorm(D3 a) { return sqrt(a.x * a.x + a.y * a.y + a.z * a.z); }
-__device__ __forceinline__ D3 dunit(D3 a) { const double n2 = a.x * a.x + a.y * a.y + a.z * a.z; if (n2 > 0) { const double n = sqrt(n2); return d3(a.x / n, a.y / n, a.z / n); } return a; }
-
 __global__ void __launch_bounds__(128)
 k_opt_obs(long long nres, const double* __restrict__ res_xy, OptObs* __restrict__ obs)
 {
@@ -167,13 +162,13 @@ k_opt_init(int L, const double* __restrict__ p1p2, const long long* __restrict__
     if (i >= L) return;
     const double* p = p1p2 + 6 * i;
     const D3 P1 = d3(p[0], p[1], p[2]), P2 = d3(p[3], p[4], p[5]);
-    const D3 l = dunit(d3(P2.x - P1.x, P2.y - P1.y, P2.z - P1.z));
+    const D3 l = dnormalized(d3(P2.x - P1.x, P2.y - P1.y, P2.z - P1.z));
     const D3 m = dcross(d3(0.5 * (P1.x + P2.x), 0.5 * (P1.y + P2.y), 0.5 * (P1.z + P2.z)), l);
     D3 e1, e2;
     if (dnorm(m) < 1e-12) {      // line through the origin of the working frame: any basis of the plane normal to l (the reference
         const D3 t = fabs(l.x) < 0.9 ? d3(1, 0, 0) : d3(0, 1, 0);   // takes Eigen's FullPivLU kernel; a set of measure zero)
-        e1 = dunit(dcross(l, t)); e2 = dcross(l, e1);
-    } else { e1 = dunit(m); e2 = dunit(dcross(l, m)); }
+        e1 = dnormalized(dcross(l, t)); e2 = dcross(l, e1);
+    } else { e1 = dnormalized(m); e2 = dnormalized(dcross(l, m)); }
     // sx = (Q - I)(Q + I)^-1 with Q = [l e1 e2]
     const double Q[3][3] = {{l.x, e1.x, e2.x}, {l.y, e1.y, e2.y}, {l.z, e1.z, e2.z}};
     double A[3][3], B[3][3], Bi[3][3];

@@ -39,34 +39,17 @@
 
 #define L3D_PI_1_32_F 0.098174771f
 #define L3D_PI_31_32_F 3.043417886f
-#define L3D_PI_D 3.14159265358979323846
-
-// View::unprojectSegment + Segment3D ctor (view.cc:356-371, segment3D.h:48-66): degenerate segments collapse to zero
-struct DSeg { D3 P1, P2, dir; float length; };
-__device__ __forceinline__ DSeg dunproject(const L3DViewDev* v, float4 s, float d1, float d2)
-{
-    D3 C = d3(v->C_d[0], v->C_d[1], v->C_d[2]);
-    D3 r1 = dray(v->RtKinv_d, (double)s.x, (double)s.y), r2 = dray(v->RtKinv_d, (double)s.z, (double)s.w);
-    D3 P1 = d3(C.x + r1.x * (double)d1, C.y + r1.y * (double)d1, C.z + r1.z * (double)d1);
-    D3 P2 = d3(C.x + r2.x * (double)d2, C.y + r2.y * (double)d2, C.z + r2.z * (double)d2);
-    DSeg o;
-    o.length = (float)dnorm(dsub(P1, P2));
-    if (o.length > L3D_EPS_D) { o.P1 = P1; o.P2 = P2; o.dir = dnormalized(dsub(P2, P1)); }
-    else { o.P1 = o.P2 = o.dir = d3(0, 0, 0); o.length = 0.0f; }
-    return o;
-}
 
 // per-segment double rays, computed once per sweep: View::getNormalizedRay (view.cc:317-321) of the two end points and of the
-// mid point (segmentQualityAngle, view.cc:466-484) - the same values dunproject / the orientation check would recompute per match
+// mid point (segmentQualityAngle, view.cc:466-484) - the same values the orientation check and View::unprojectSegment
+// (view.cc:356-371) would recompute per match
 struct SegRaysQ { D3 r1, r2, rm; };
 __global__ void __launch_bounds__(256)
 k_sw_rays(const float4* __restrict__ segs, const L3DViewDev* __restrict__ views, int V, long long N, double* __restrict__ rays, float4* __restrict__ rmf)
 {
     const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= N) return;
-    int lo = 0, hi = V - 1;
-    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (views[mid].seg_off <= g) lo = mid; else hi = mid - 1; }
-    const L3DViewDev* Vw = views + lo;
+    const L3DViewDev* Vw = views + last_le(V, g, [&](int i) { return views[i].seg_off; });
     const float4 s = segs[g];
     const D3 r1 = dray(Vw->RtKinv_d, (double)s.x, (double)s.y), r2 = dray(Vw->RtKinv_d, (double)s.z, (double)s.w);
     const D3 rm = dray(Vw->RtKinv_d, 0.5 * ((double)s.x + (double)s.z), 0.5 * ((double)s.y + (double)s.w));
@@ -81,15 +64,13 @@ __device__ __forceinline__ SegRaysQ sw_load_rays(const double* __restrict__ rays
     q.r1 = d3(__ldg(p), __ldg(p + 1), __ldg(p + 2)); q.r2 = d3(__ldg(p + 3), __ldg(p + 4), __ldg(p + 5)); q.rm = d3(__ldg(p + 6), __ldg(p + 7), __ldg(p + 8));
     return q;
 }
-// dunproject with the cached rays: same expressions, same results
+// the end points View::unprojectSegment (view.cc:356-371) computes, with the cached rays; seg3d() makes the Segment3D of them
 __device__ __forceinline__ void sw_unproject_pts(const L3DViewDev* v, const SegRaysQ& q, float d1, float d2, D3* P1, D3* P2)
 {
     const D3 C = d3(v->C_d[0], v->C_d[1], v->C_d[2]);
     *P1 = d3(C.x + q.r1.x * (double)d1, C.y + q.r1.y * (double)d1, C.z + q.r1.z * (double)d1);
     *P2 = d3(C.x + q.r2.x * (double)d2, C.y + q.r2.y * (double)d2, C.z + q.r2.z * (double)d2);
 }
-// Segment3D's degeneracy test `(float)|P1-P2| > 1e-12` (segment3D.h:50-66); n2 = |P1-P2|^2
-__device__ __forceinline__ bool sw_nondegenerate(double n2) { return n2 > 1e-20 ? true : (double)(float)sqrt(n2) > L3D_EPS_D; }
 
 // checkMatchOrientation (line3D.cc:811-858) for the match (segment of view V with rays q, depths d1,d2): unprojectMatch
 // (1556-1568) + View::segmentQualityAngle (view.cc:466-484): keep iff pi/32 < acos(clamp(ray_mid . dir)) < 31 pi/32.
@@ -108,9 +89,7 @@ __device__ __forceinline__ bool sw_orientation_ok(const L3DViewDev* V, const Seg
         if (c < c1 - 1e-9 && c > c2 + 1e-9) return true;
         if (c > c1 + 1e-9 || c < c2 - 1e-9) return false;
     }
-    D3 dir = d3(0, 0, 0);
-    if (sw_nondegenerate(ddot(dsub(P1, P2), dsub(P1, P2)))) dir = dnormalized(d);
-    const double ang = acos(fmin(fmax(ddot(q.rm, dir), -1.0), 1.0));
+    const double ang = acos(fmin(fmax(ddot(q.rm, seg3d(P1, P2).dir), -1.0), 1.0));
     return ang > (double)L3D_PI_1_32_F && ang < (double)L3D_PI_31_32_F;
 }
 
@@ -235,8 +214,7 @@ k_sw_chunksort(const L3DViewDev* __restrict__ views, int V, long long N, const S
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const long long gs = (long long)blockIdx.x * CS_WARPS + wid;
     if (gs >= N) return;
-    int lo = 0, hi = V - 1;
-    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (views[mid].seg_off <= gs) lo = mid; else hi = mid - 1; }
+    const int lo = last_le(V, gs, [&](int i) { return views[i].seg_off; });
     const SwView me = vt[lo];
     const int np = me.np;
     if (np == 0) return;
@@ -250,8 +228,7 @@ k_sw_chunksort(const L3DViewDev* __restrict__ views, int V, long long N, const S
         for (int j = lane; j < n; j += 32) { const uint2 kv = e_kv[x0 + j]; sk[wid][j] = kv.x; sv[wid][j] = kv.y; }
         __syncwarp();
         for (int j = lane; j < n; j += 32) {
-            int cl = 0, chh = np - 1;
-            while (cl < chh) { const int mid = (cl + chh + 1) >> 1; if (scb[wid][mid] <= j) cl = mid; else chh = mid - 1; }
+            const int cl = last_le(np, j, [&](int c) { return scb[wid][c]; });
             const int a = scb[wid][cl], b = scb[wid][cl + 1];
             const unsigned int key = sk[wid][j], val = sv[wid][j];
             int rank = 0;
@@ -336,9 +313,7 @@ __device__ __forceinline__ float sw_sim(const SwOwn& o, const float4* __restrict
     const float4 tb = sb[i];
     const float dp = o.dir.x * tb.x + o.dir.y * tb.y + o.dir.z * tb.z;
     if (fabsf(dp) < cos_thr) return 0.0f;
-    // D_undirected_angle_3D_DEG (cudawrapper.cu:46-53): float acos, DOUBLE divide by pi, times 180, back to float
-    float angle = (float)((double)acosf(fmaxf(fminf(dp, 1.0f), -1.0f)) / L3D_PI_D * (double)180.0f);
-    if (angle > 90.0f) angle = 180.0f - angle;
+    const float angle = undirected_angle_deg(dp);
     const float sim_a = expf(-angle * angle / angle_reg);
     const float sim_p1 = expf(-e1 * e1 / o.pos_reg1), sim_p2 = expf(-e2 * e2 / o.pos_reg2);
     float sim = fminf(sim_a, fminf(sim_p1, sim_p2));
@@ -416,9 +391,7 @@ __device__ __forceinline__ float sw_score_cpu(const float4* __restrict__ sa, con
     auto sim_of = [&](int i) -> float {
         const double4 D2 = d64[i];
         if ((float)D1.w < L3D_EPS_D || (float)D2.w < L3D_EPS_D) return 0.0f;
-        const float dot_p = (float)(D1.x * D2.x + D1.y * D2.y + D1.z * D2.z);
-        float angle = (float)((double)acosf(fmaxf(fminf(dot_p, 1.0f), -1.0f)) / L3D_PI_D * (double)180.0f);
-        if (angle > 90.0f) angle = 180.0f - angle;
+        const float angle = undirected_angle_deg((float)(D1.x * D2.x + D1.y * D2.y + D1.z * D2.z));
         const float sim_a = expf(-angle * angle / angle_reg);
         const float4 d2 = sa[i];
         const float e1 = ma.x - d2.x, e2 = ma.y - d2.y;
@@ -465,16 +438,9 @@ __device__ __forceinline__ float2 sw_target_reg(const L3DViewDev* V, const SwSeg
     Q.r1 = d3(sg.q1[0], sg.q1[1], sg.q1[2]); Q.r2 = d3(sg.q2[0], sg.q2[1], sg.q2[2]); Q.rm = d3(0, 0, 0);
     D3 P1, P2;
     sw_unproject_pts(V, Q, d1, d2, &P1, &P2);
-    const D3 dd = dsub(P1, P2);
-    const double n2 = ddot(dd, dd);
-    const bool nondeg = sw_nondegenerate(n2);
-    if (!nondeg) P1 = P2 = d3(0, 0, 0);                                   // Segment3D ctor (segment3D.h:58-63)
-    if (CPU) {
-        D3 dir = d3(0, 0, 0); float len = 0.0f;
-        if (nondeg) { dir = dnormalized(dsub(P2, P1)); len = (float)sqrt(n2); }
-        *d64_out = make_double4(dir.x, dir.y, dir.z, (double)len);
-    }
-    return make_float2((float)(dnorm(dsub(P1, Ct)) * (double)kT), (float)(dnorm(dsub(P2, Ct)) * (double)kT));
+    const Seg3D S = seg3d(P1, P2);
+    if (CPU) *d64_out = make_double4(S.dir.x, S.dir.y, S.dir.z, (double)S.length);
+    return make_float2((float)(dnorm(dsub(S.P1, Ct)) * (double)kT), (float)(dnorm(dsub(S.P2, Ct)) * (double)kT));
 }
 
 template <bool CPU>
@@ -503,9 +469,8 @@ __device__ __forceinline__ void sw_score_range(const SwScoreArgs<CPU>& A, const 
             const long long x = x0 + j;
             const unsigned int val = A.e_val[x];
             const l3d_match_rec rec = A.recs[val & ~SW_INV];
-            int lo = 0, hi = nch - 1;               // chunk of entry j: last q with boundary[q] <= j
-            if (cb_smem) { while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (cb[mid] <= j) lo = mid; else hi = mid - 1; } }
-            else { while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (A.cstart[chbase + mid] <= x) lo = mid; else hi = mid - 1; } }
+            const int lo = cb_smem ? last_le(nch, j, [&](int q) { return cb[q]; })          // chunk of entry j
+                                   : last_le(nch, x, [&](int q) { return A.cstart[chbase + q]; });
             const int si = lo / np;
             int other, pub; float kT; D3 Ct;
             chunk_info(lo - si * np, &other, &pub, &kT, &Ct);
@@ -667,8 +632,7 @@ k_sw_filter(const float4* __restrict__ segs, const L3DViewDev* __restrict__ view
 {
     const long long gs = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (gs >= N) return;
-    int lo = 0, hi = V - 1;
-    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (views[mid].seg_off <= gs) lo = mid; else hi = mid - 1; }
+    const int lo = last_le(V, gs, [&](int i) { return views[i].seg_off; });
     const L3DViewDev* Vw = views + lo;
     const SwView me = vt[lo];
     const int s = (int)(gs - Vw->seg_off);
@@ -694,7 +658,14 @@ k_sw_filter(const float4* __restrict__ segs, const L3DViewDev* __restrict__ view
     est_best[gs] = best >= 0 ? (int)(best - me.region_off) : -1;
     if (best >= 0) {
         const float4 dep = sw_depths(e_val[best], recs);
-        const DSeg S3 = dunproject(Vw, segs[gs], dep.x, dep.y);       // unprojectMatch(best_match, true)
+        // unprojectMatch(best_match, true).  The rays are the ones k_sw_rays cached, recomputed from the 16-byte segment:
+        // reading the 48 bytes of cached rays made this kernel 1.3 % slower on an H100 80GB HBM3 (700 W).
+        const float4 sg = segs[gs];
+        SegRaysQ q;
+        q.r1 = dray(Vw->RtKinv_d, (double)sg.x, (double)sg.y); q.r2 = dray(Vw->RtKinv_d, (double)sg.z, (double)sg.w); q.rm = d3(0, 0, 0);
+        D3 P1, P2;
+        sw_unproject_pts(Vw, q, dep.x, dep.y, &P1, &P2);
+        const Seg3D S3 = seg3d(P1, P2);
         double* o = est_P + 6 * gs;
         o[0] = S3.P1.x; o[1] = S3.P1.y; o[2] = S3.P1.z; o[3] = S3.P2.x; o[4] = S3.P2.y; o[5] = S3.P2.z;
     }
@@ -733,8 +704,7 @@ k_collect_estimates(const L3DViewDev* __restrict__ views, int V, long long N, co
     if (g >= N) return;
     const int b = est_best[g];
     if (b < 0) return;
-    int lo = 0, hi = V - 1;
-    while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (views[mid].seg_off <= g) lo = mid; else hi = mid - 1; }
+    const int lo = last_le(V, g, [&](int i) { return views[i].seg_off; });
     const long long x = vt[lo].region_off + b;
     const SwEntry e = sw_decode(e_val[x], pairs, row_off, num_pairs, knn, recs);
     l3d_match m;

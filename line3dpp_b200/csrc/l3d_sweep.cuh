@@ -29,9 +29,7 @@ struct SwEntry { int seg, tgt_view, tgt_seg; float4 dep; float overlap; };
 // pair of a record row: last p with row_off[p] <= row
 __device__ __forceinline__ int sw_pair_of_row(const long long* __restrict__ row_off, int num_pairs, long long row)
 {
-    int lo = 0, hi = num_pairs - 1;
-    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (__ldg(row_off + mid) <= row) lo = mid; else hi = mid - 1; }
-    return lo;
+    return last_le(num_pairs, row, [&](int i) { return __ldg(row_off + i); });
 }
 
 // what matches_[view][seg] holds for this entry: Match{src = (view, seg), tgt = (tgt_view, tgt_seg), depths from the entry's side}

@@ -110,12 +110,7 @@ __device__ __forceinline__ void ud_tile_rows(const L3DUndistImage& d, int j, int
 __global__ void __launch_bounds__(UD_TW) k_undistort_u8(const L3DUndistImage* __restrict__ imgs, int n)
 {
     __shared__ double2 s_y[UD_TH];          // (y, y*y) of the tile's rows
-    int lo = 0, hi = n - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (imgs[mid].tile0 <= (long long)blockIdx.x) lo = mid; else hi = mid - 1;
-    }
-    const L3DUndistImage d = imgs[lo];
+    const L3DUndistImage d = imgs[last_le(n, (long long)blockIdx.x, [&](int i) { return imgs[i].tile0; })];
     const long long t = (long long)blockIdx.x - d.tile0;
     const int i0 = (int)(t / d.tiles_x) * UD_TH, j = (int)(t % d.tiles_x) * UD_TW + threadIdx.x;
     if (threadIdx.x < UD_TH) {
