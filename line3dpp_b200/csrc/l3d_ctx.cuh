@@ -28,7 +28,7 @@ struct SweepState {
     std::vector<long long> region_off;      // per processing rank (+1): first entry of the view's region
     long long total = 0;
     // match store (l3d_sweep.cuh): view table, chunk descriptors, chunk offsets, entries
-    DevBuf d_vt, d_vp, d_pairc, d_rowoff, d_pinfo, d_bpair, d_ekv, d_rays, d_rmf, d_rflag, d_invpos, d_csize, d_ccur, d_cstart, d_eval, d_escore, d_eflag, d_gstage, d_gpub, d_dir64, d_export, d_export_ok,
+    DevBuf d_vt, d_cinfo, d_rowoff, d_pinfo, d_bpair, d_ekv, d_rays, d_rmf, d_rflag, d_invpos, d_csize, d_ccur, d_cstart, d_eval, d_escore, d_eflag, d_gstage, d_gtab, d_export, d_export_ok,
         d_ranges, d_est_best, d_est_P, d_M, d_vmax, d_order, d_region_off, d_est_pos, d_est_out_best, d_est_out_P;
     long long n_est = 0;
     float ms_setup = 0.f, ms_chain = 0.f, ms_filter = 0.f;   // device time of the last sweep's three phases

@@ -199,15 +199,16 @@ k_sw_scatter(const SwPairInfo* __restrict__ pinfo, const int* __restrict__ block
     }
 }
 
-// P5: one warp per segment: the segment's entries (all its chunks, contiguous) are read into shared memory, every entry finds its
-// place inside its chunk by counting the smaller keys (keys are unique inside a chunk), and is written back in list order together
-// with its initial flag (direct entries are active from the start) and, for inverse entries, the place its source will find it at.
+// P5: one warp per segment: every entry of the segment (all its chunks, contiguous) finds its place inside its chunk by counting
+// the smaller keys (keys are unique inside a chunk), and is written in list order together with its initial flag (direct entries
+// are active from the start) and, for inverse entries, the place its source will find it at.  Keys and chunk boundaries are read
+// from shared-memory copies when the segment fits (n <= CS_MAXN, np <= CS_MAXNP), else straight from e_kv / cstart.
 #define CS_WARPS 8
 #define CS_MAXN 192
 #define CS_MAXNP 64
 __global__ void __launch_bounds__(32 * CS_WARPS)
 k_sw_chunksort(const L3DViewDev* __restrict__ views, int V, long long N, const SwView* __restrict__ vt, const long long* __restrict__ cstart,
-               uint2* __restrict__ e_kv, unsigned int* __restrict__ e_val, unsigned char* __restrict__ e_flag, unsigned int* __restrict__ invpos)
+               const uint2* __restrict__ e_kv, unsigned int* __restrict__ e_val, unsigned char* __restrict__ e_flag, unsigned int* __restrict__ invpos)
 {
     __shared__ unsigned int sk[CS_WARPS][CS_MAXN], sv[CS_WARPS][CS_MAXN];
     __shared__ int scb[CS_WARPS][CS_MAXNP + 1];
@@ -223,37 +224,27 @@ k_sw_chunksort(const L3DViewDev* __restrict__ views, int V, long long N, const S
     const int n = (int)(x1 - x0);
     if (n == 0) return;
     const long long ro = me.region_off;
+    // bound(c): start of chunk c relative to x0; key(i), val(i): entry i
+    auto place = [&](auto bound, auto key, auto val) {
+        for (int j = lane; j < n; j += 32) {
+            const int cl = last_le(np, j, bound);
+            const int a = bound(cl), b = bound(cl + 1);
+            const unsigned int kj = key(j), vj = val(j);
+            int rank = 0;
+            for (int i = a; i < b; ++i) rank += key(i) < kj ? 1 : 0;
+            const long long pos = x0 + a + rank;
+            e_val[pos] = vj;
+            if (vj & SW_INV) { e_flag[pos] = 0; invpos[vj & ~SW_INV] = (unsigned int)(pos - ro); }
+            else e_flag[pos] = SW_ACTIVE;
+        }
+    };
     if (n <= CS_MAXN && np <= CS_MAXNP) {
         for (int c = lane; c <= np; c += 32) scb[wid][c] = (int)(cstart[ch0 + c] - x0);
         for (int j = lane; j < n; j += 32) { const uint2 kv = e_kv[x0 + j]; sk[wid][j] = kv.x; sv[wid][j] = kv.y; }
         __syncwarp();
-        for (int j = lane; j < n; j += 32) {
-            const int cl = last_le(np, j, [&](int c) { return scb[wid][c]; });
-            const int a = scb[wid][cl], b = scb[wid][cl + 1];
-            const unsigned int key = sk[wid][j], val = sv[wid][j];
-            int rank = 0;
-            for (int i = a; i < b; ++i) rank += sk[wid][i] < key ? 1 : 0;
-            const long long pos = x0 + a + rank;
-            e_val[pos] = val;
-            if (val & SW_INV) { e_flag[pos] = 0; invpos[val & ~SW_INV] = (unsigned int)(pos - ro); }
-            else e_flag[pos] = SW_ACTIVE;
-        }
-    } else {        // long lists / many neighbours: a lane per chunk, insertion sort in place
-        for (int c = lane; c < np; c += 32) {
-            const long long a = cstart[ch0 + c], b = cstart[ch0 + c + 1];
-            for (long long i = a + 1; i < b; ++i) {
-                const uint2 kv = e_kv[i];
-                long long j = i - 1;
-                while (j >= a && e_kv[j].x > kv.x) { e_kv[j + 1] = e_kv[j]; --j; }
-                e_kv[j + 1] = kv;
-            }
-            for (long long i = a; i < b; ++i) {
-                const unsigned int v = e_kv[i].y;
-                e_val[i] = v;
-                if (v & SW_INV) { e_flag[i] = 0; invpos[v & ~SW_INV] = (unsigned int)(i - ro); }
-                else e_flag[i] = SW_ACTIVE;
-            }
-        }
+        place([&](int c) { return scb[wid][c]; }, [&](int i) { return sk[wid][i]; }, [&](int i) { return sv[wid][i]; });
+    } else {
+        place([&](int c) { return (int)(cstart[ch0 + c] - x0); }, [&](int i) { return e_kv[x0 + i].x; }, [&](int i) { return e_kv[x0 + i].y; });
     }
 }
 
@@ -268,20 +259,41 @@ k_sw_chunksort(const L3DViewDev* __restrict__ views, int V, long long N, const S
 #define SW_SEGS_MAX 16        // segments per CTA: chosen per view at launch time so that the view's CTAs are ONE resident wave
                               // (tools/sweep_score.py: 750 CTAs on 740 slots cost 20.7 ms per 1000 views, 600 CTAs 14.7 ms)
 #define SW_CAP_MAX 4096       // list entries staged in shared memory per CTA, upper bound (longer ranges: global scratch)
+#define SW_CAP_MAX_CPU 2048   // the same for REF_CPU
 
-// staged entry: a = (depth1, depth2, target view or -1 if inactive, index of its segment in the CTA), b = (dir.xyz, view to announce a
-// positive score to or -1), r = (reg1, reg2) target regularisers; REF_CPU adds d64 = (double dir.xyz, length)
+// staged entry: a = (depth1, depth2, target view or -1 if inactive, index of its chunk in the CTA), b = (dir.xyz, view to announce a
+// positive score to or -1), r = (reg1, reg2) target regularisers, act = the ordered list of active entries; REF_CPU adds
+// d64 = (double dir.xyz, length).  16 + 16 + 8 + 4 = 44 bytes, rounded up to 48 for the alignment of d64.
 struct SwPtrs { float4* a; float4* b; float2* r; double4* d64; int* act; };
+__host__ __device__ constexpr size_t sw_entry_bytes(bool cpu) { return cpu ? 48 + 32 : 48; }
+// the arrays of `cap` staged entries from `base` (16-byte aligned): the shared-memory staging and the global scratch alike
+__host__ __device__ __forceinline__ SwPtrs sw_carve(unsigned char* base, size_t cap, bool cpu)
+{
+    SwPtrs P;
+    P.a = (float4*)base; P.b = P.a + cap; P.r = (float2*)(P.b + cap); P.act = (int*)(P.r + cap);
+    P.d64 = cpu ? (double4*)(base + 48 * cap) : nullptr;
+    return P;
+}
+
+// per-CTA tables: chunk boundaries of the CTA's segments, relative to the CTA's first entry (cb) and in the list of its active
+// entries (cbA); what every chunk of the view points at (SwChunkInfo: other view, view to announce a positive score to or -1, the
+// other view's k and double camera centre; built on the host); the rays of the segments.  The first two are held in shared memory
+// up to these sizes and read from global memory beyond them - where they live is the only difference.
+#define SW_MAXCH 512          // chunk boundaries held in shared memory (SW_SEGS * np + 1)
+#define SW_MAXNP 64           // chunk descriptors held in shared memory
+struct SwChunkInfo { int other, pub; float k; float pad; double Cx, Cy, Cz; };
+struct SwSegInfo { float r1[3], r2[3]; double q1[3], q2[3]; };
 
 template <bool CPU>
 struct SwScoreArgs {
     const float4* cache; const double* rays; const L3DViewDev* views; const l3d_match_rec* recs; int v;
-    const SwView* vt; const SwChunk* vp; const int2* pairc; const long long* cstart;
+    const SwView* vt; const SwChunkInfo* cinfo; const long long* cstart;
     const unsigned int* e_val; float* e_score; unsigned char* e_flag; const unsigned int* invpos;
     int* view_max_bits; int* M;
-    SwPtrs g;                       // global scratch (one view's region) for entry ranges longer than the shared-memory capacity
+    unsigned char* gstage;          // global scratch (one view's region) for entry ranges longer than the shared-memory capacity
+    int* gtab;                      // global scratch for cb, cbA of CTAs with more than SW_MAXCH chunks: 2 (nch + 1) ints per CTA
     float angle_reg, sim_t, q_thr, cos_thr;
-    int segs, cap;                  // this launch: segments per CTA, staged entries per CTA (dynamic shared memory = 48 (+32 REF_CPU) bytes x cap)
+    int segs, cap;                  // this launch: segments per CTA, staged entries per CTA (dynamic shared memory = sw_entry_bytes x cap)
 };
 
 // similarity of K_score_matches' inner loop (cudawrapper.cu:318-347) between the own entry and staged entry i, tests ordered
@@ -321,33 +333,14 @@ __device__ __forceinline__ float sw_sim(const SwOwn& o, const float4* __restrict
     return sim;
 }
 
-// K_score_matches' accumulation (cudawrapper.cu:304-359) over the staged list [lo, hi) in list order: inactive entries (target
-// view < 0) and entries of the own target camera are not in the reference's loop.  Used when the chunk tables are not in shared memory.
-__device__ __forceinline__ float sw_score_gpu_list(const float4* __restrict__ sa, const float4* __restrict__ sb, float2 rg, int lo, int hi, int me, float k,
-                                                   float angle_reg, float sim_t, float q_thr, float cos_thr)
-{
-    const SwOwn o = sw_own(sa[me], sb[me], rg, k, q_thr);
-    const int tgt_cam_src = __float_as_int(sa[me].z);
-    float score3D = 0.0f, current_max_sim = 0.0f;
-    int current_cam = -1;
-    for (int i = lo; i < hi; ++i) {
-        const int tgt_cam_tgt = __float_as_int(sa[i].z);
-        if (tgt_cam_tgt < 0 || tgt_cam_src == tgt_cam_tgt) continue;
-        const float sim = sw_sim(o, sa, sb, i, angle_reg, sim_t, cos_thr);
-        current_max_sim = fmaxf(current_max_sim, sim);
-        if (current_cam != tgt_cam_tgt) { score3D += current_max_sim; current_max_sim = 0.0f; current_cam = tgt_cam_tgt; }
-    }
-    score3D += current_max_sim;
-    return score3D;
-}
-
-// The same accumulation, chunk by chunk over the ACTIVE entries only (ord = their indices in list order, cbA = chunk boundaries
-// in that list).  A chunk is a run of entries with one target camera: its first entry flushes what the previous camera left
-// pending (score += max(pending, sim); pending = 0), the others raise pending - exactly the reference's sequence of float
+// K_score_matches' accumulation (cudawrapper.cu:304-359) walks the segment's list and skips inactive entries and those of the own
+// target camera.  Here it runs chunk by chunk over the ACTIVE entries only (ord = their indices in list order, cbA = chunk
+// boundaries in that list).  A chunk is a run of entries with one target camera: its first entry flushes what the previous camera
+// left pending (score += max(pending, sim); pending = 0), the others raise pending - exactly the reference's sequence of float
 // additions, because the entries it skips contribute nothing (x + 0 == x) and a camera without active entries does not appear
 // in the reference's list at all.
 __device__ __forceinline__ float sw_score_gpu_chunks(const float4* __restrict__ sa, const float4* __restrict__ sb, float2 rg, const int* __restrict__ ord,
-                                                     const int* __restrict__ cbA, const int* __restrict__ chunk_cam, int c0, int np, int my_chunk, int me,
+                                                     const int* __restrict__ cbA, const SwChunkInfo* __restrict__ cinfo, int c0, int np, int my_chunk, int me,
                                                      float k, float angle_reg, float sim_t, float q_thr, float cos_thr)
 {
     const SwOwn o = sw_own(sa[me], sb[me], rg, k, q_thr);
@@ -359,7 +352,7 @@ __device__ __forceinline__ float sw_score_gpu_chunks(const float4* __restrict__ 
         int t = cbA[cc];
         const int te = cbA[cc + 1];
         if (t == te || cc == my_chunk) continue;
-        const int cam = chunk_cam[c];
+        const int cam = cinfo[c].other;
         if (cam == my_cam) continue;
         if (cam != current_cam) {
             const float sim = sw_sim(o, sa, sb, ord[t], angle_reg, sim_t, cos_thr);
@@ -376,8 +369,8 @@ __device__ __forceinline__ float sw_score_gpu_chunks(const float4* __restrict__ 
 
 // scoringCPU (line3D.cc:1208-1294) + similarityForScoring (1417-1446) + angleBetweenSeg3D (1571-1583): the score is the sum
 // over target cameras of the best similarity among that camera's matches, built with the reference's running update (add the
-// first value of a camera, replace it when a larger one arrives) in list order.  ord != nullptr: [lo, hi) indexes the ordered
-// list of active entries, else the staged list itself (inactive entries carry a negative camera).
+// first value of a camera, replace it when a larger one arrives) in list order; [lo, hi) indexes the ordered list of active
+// entries ord.
 #define SC_MAP 48
 __device__ __forceinline__ float sw_score_cpu(const float4* __restrict__ sa, const double4* __restrict__ d64, float2 rg, const int* __restrict__ ord, int lo,
                                               int hi, int me, float k, float angle_reg, float sim_t)
@@ -402,7 +395,7 @@ __device__ __forceinline__ float sw_score_cpu(const float4* __restrict__ sa, con
     int cams[SC_MAP]; float best[SC_MAP]; int ncam = 0;
     float score3D = 0.0f;
     for (int t = lo; t < hi; ++t) {
-        const int i = ord ? ord[t] : t;
+        const int i = ord[t];
         const int cam = __float_as_int(sa[i].z);
         if (cam < 0 || cam == my_cam) continue;
         const float sim = sim_of(i);
@@ -413,7 +406,7 @@ __device__ __forceinline__ float sw_score_cpu(const float4* __restrict__ sa, con
         else {      // more target cameras than map slots: recover this camera's running maximum from the earlier entries
             bool seen = false; float cur = 0.0f;
             for (int u = lo; u < t; ++u) {
-                const int j = ord ? ord[u] : u;
+                const int j = ord[u];
                 if (__float_as_int(sa[j].z) == cam) { const float sj = sim_of(j); if (!seen) { cur = sj; seen = true; } else if (sj > cur) cur = sj; }
             }
             if (seen) { if (sim > cur) { score3D -= cur; score3D += sim; } } else score3D += sim;
@@ -422,17 +415,10 @@ __device__ __forceinline__ float sw_score_cpu(const float4* __restrict__ sa, con
     return score3D;
 }
 
-// per-CTA tables in shared memory: chunk boundaries of the CTA's segments (relative to x0), what every chunk of the view points
-// at (other view, its double camera centre and k, whether a positive score has to be announced there), the rays of the segments
-#define SW_MAXCH 512          // chunk boundaries held in shared memory (SW_SEGS * np + 1); beyond that: global look-ups
-#define SW_MAXNP 64           // chunk descriptors held in shared memory
-struct SwChunkInfo { int other, pub; float k; float pad; double Cx, Cy, Cz; };
-struct SwSegInfo { float r1[3], r2[3]; double q1[3], q2[3]; };
-
 // regularizers_tgt (line3D.cc:1350-1352) == View::regularizerFrom3Dpoint (view.cc:445-448): |P - C_tgt| * k_tgt in double, stored as
 // float; REF_CPU also needs the double 3D segment (direction, float length) scoringCPU works on
 template <bool CPU>
-__device__ __forceinline__ float2 sw_target_reg(const L3DViewDev* V, const SwSegInfo& sg, float d1, float d2, D3 Ct, float kT, double4* d64_out)
+__device__ __forceinline__ float2 sw_target_reg(const L3DViewDev* V, const SwSegInfo& sg, float d1, float d2, const SwChunkInfo& ci, double4* d64_out)
 {
     SegRaysQ Q;
     Q.r1 = d3(sg.q1[0], sg.q1[1], sg.q1[2]); Q.r2 = d3(sg.q2[0], sg.q2[1], sg.q2[2]); Q.rm = d3(0, 0, 0);
@@ -440,28 +426,19 @@ __device__ __forceinline__ float2 sw_target_reg(const L3DViewDev* V, const SwSeg
     sw_unproject_pts(V, Q, d1, d2, &P1, &P2);
     const Seg3D S = seg3d(P1, P2);
     if (CPU) *d64_out = make_double4(S.dir.x, S.dir.y, S.dir.z, (double)S.length);
-    return make_float2((float)(dnorm(dsub(S.P1, Ct)) * (double)kT), (float)(dnorm(dsub(S.P2, Ct)) * (double)kT));
+    const D3 Ct = d3(ci.Cx, ci.Cy, ci.Cz);
+    return make_float2((float)(dnorm(dsub(S.P1, Ct)) * (double)ci.k), (float)(dnorm(dsub(S.P2, Ct)) * (double)ci.k));
 }
 
 template <bool CPU>
-__device__ __forceinline__ void sw_score_range(const SwScoreArgs<CPU>& A, const SwPtrs P, const int* __restrict__ cb, int* __restrict__ cbA, bool cb_smem,
-                                               const SwChunkInfo* __restrict__ cinfo, const int* __restrict__ ccam, bool cinfo_smem,
-                                               const SwSegInfo* __restrict__ sinfo, int* __restrict__ wcnt, int s0, int nsegs, long long x0, int n)
+__device__ __forceinline__ void sw_score_range(const SwScoreArgs<CPU>& A, const SwPtrs P, const int* __restrict__ cb, int* __restrict__ cbA,
+                                               const SwChunkInfo* __restrict__ cinfo, const SwSegInfo* __restrict__ sinfo, int* __restrict__ wcnt,
+                                               int nsegs, long long x0, int n)
 {
     const L3DViewDev* V = A.views + A.v;
-    const SwView me = A.vt[A.v];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const int np = me.np;
+    const int np = A.vt[A.v].np;
     const int nch = nsegs * np;
-    const long long chbase = me.chunk_base + (long long)s0 * np;
-    auto chunk_info = [&](int c, int* other, int* pub, float* kT, D3* Ct) {
-        if (cinfo_smem) { const SwChunkInfo ci = cinfo[c]; *other = ci.other; *pub = ci.pub; *kT = ci.k; *Ct = d3(ci.Cx, ci.Cy, ci.Cz); }
-        else {
-            const SwChunk ck = A.vp[me.vp_off + c];
-            const L3DViewDev* T = A.views + ck.other;
-            *other = ck.other; *pub = (!ck.inv && A.pairc[ck.pair].y >= 0) ? ck.other : -1; *kT = T->k; *Ct = d3(T->C_d[0], T->C_d[1], T->C_d[2]);
-        }
-    };
     // ---- stage: a = (depth1, depth2, target view [inverse entries: -2 - view until they are known to be active], chunk index in the CTA)
     for (int j0 = 0; j0 < n; j0 += SW_THREADS) {
         const int j = j0 + threadIdx.x;
@@ -469,11 +446,9 @@ __device__ __forceinline__ void sw_score_range(const SwScoreArgs<CPU>& A, const 
             const long long x = x0 + j;
             const unsigned int val = A.e_val[x];
             const l3d_match_rec rec = A.recs[val & ~SW_INV];
-            const int lo = cb_smem ? last_le(nch, j, [&](int q) { return cb[q]; })          // chunk of entry j
-                                   : last_le(nch, x, [&](int q) { return A.cstart[chbase + q]; });
+            const int lo = last_le(nch, j, [&](int q) { return cb[q]; });          // chunk of entry j
             const int si = lo / np;
-            int other, pub; float kT; D3 Ct;
-            chunk_info(lo - si * np, &other, &pub, &kT, &Ct);
+            const SwChunkInfo ci = cinfo[lo - si * np];
             const bool inv = (val & SW_INV) != 0u;
             const float d1 = inv ? rec.d_q1 : rec.d_p1, d2 = inv ? rec.d_q2 : rec.d_p2;
             const SwSegInfo& sg = sinfo[si];
@@ -483,10 +458,10 @@ __device__ __forceinline__ void sw_score_range(const SwScoreArgs<CPU>& A, const 
                 const float3 P2 = make_float3(Cf.x + d2 * sg.r2[0], Cf.y + d2 * sg.r2[1], Cf.z + d2 * sg.r2[2]);
                 const float3 dir = normalize3(make_float3(P2.x - P1.x, P2.y - P1.y, P2.z - P1.z));
                 // where a positive score has to be announced: the target view, if it is still to be processed (line3D.cc:1680)
-                P.b[j] = make_float4(dir.x, dir.y, dir.z, __int_as_float(inv ? -1 : pub));
+                P.b[j] = make_float4(dir.x, dir.y, dir.z, __int_as_float(inv ? -1 : ci.pub));
             }
-            if (!inv) P.r[j] = sw_target_reg<CPU>(V, sg, d1, d2, Ct, kT, CPU ? P.d64 + j : nullptr);      // inverse entries: only if they turn out active
-            P.a[j] = make_float4(d1, d2, __int_as_float(inv ? -2 - other : other), __int_as_float(lo));
+            if (!inv) P.r[j] = sw_target_reg<CPU>(V, sg, d1, d2, ci, CPU ? P.d64 + j : nullptr);      // inverse entries: only if they turn out active
+            P.a[j] = make_float4(d1, d2, __int_as_float(inv ? -2 - ci.other : ci.other), __int_as_float(lo));
         }
     }
     // ---- everything above only read what the set-up kernels wrote: it may overlap the previous view's kernel (programmatic
@@ -506,10 +481,9 @@ __device__ __forceinline__ void sw_score_range(const SwScoreArgs<CPU>& A, const 
                 if (A.e_flag[x] & SW_ACTIVE) {
                     active = true;
                     const int lo = __float_as_int(ma.w), si = lo / np;
-                    int other, pub; float kT; D3 Ct;
-                    chunk_info(lo - si * np, &other, &pub, &kT, &Ct);
-                    P.a[j].z = __int_as_float(other);
-                    P.r[j] = sw_target_reg<CPU>(V, sinfo[si], ma.x, ma.y, Ct, kT, CPU ? P.d64 + j : nullptr);
+                    const SwChunkInfo ci = cinfo[lo - si * np];
+                    P.a[j].z = __int_as_float(ci.other);
+                    P.r[j] = sw_target_reg<CPU>(V, sinfo[si], ma.x, ma.y, ci, CPU ? P.d64 + j : nullptr);
                 } else { P.a[j].z = __int_as_float(-1); A.e_score[x] = 0.0f; }
             }
         }
@@ -524,34 +498,22 @@ __device__ __forceinline__ void sw_score_range(const SwScoreArgs<CPU>& A, const 
         __syncthreads();
     }
     // chunk boundaries in the list of active entries
-    const bool chunked = !CPU && cb_smem && cinfo_smem;
-    if (cb_smem) {
-        for (int q = threadIdx.x; q <= nch; q += SW_THREADS) {
-            const int bound = cb[q];
-            int lo = 0, hi = nact;
-            while (lo < hi) { const int mid = (lo + hi) >> 1; if (P.act[mid] < bound) lo = mid + 1; else hi = mid; }
-            cbA[q] = lo;
-        }
-        __syncthreads();
+    for (int q = threadIdx.x; q <= nch; q += SW_THREADS) {
+        const int bound = cb[q];
+        int lo = 0, hi = nact;
+        while (lo < hi) { const int mid = (lo + hi) >> 1; if (P.act[mid] < bound) lo = mid + 1; else hi = mid; }
+        cbA[q] = lo;
     }
+    __syncthreads();
     // ---- score the active entries, publish
-    const float k = V->k;
     float vmax = 0.0f;
     for (int q = threadIdx.x; q < nact; q += SW_THREADS) {
         const int j = P.act[q];
         const int my_chunk = __float_as_int(P.a[j].w);
         const int si = my_chunk / np;
-        float sc;
-        if (chunked) {
-            sc = sw_score_gpu_chunks(P.a, P.b, P.r[j], P.act, cbA, ccam, si * np, np, my_chunk, j, k, A.angle_reg, A.sim_t, A.q_thr, A.cos_thr);
-        } else if (cb_smem) {
-            sc = CPU ? sw_score_cpu(P.a, P.d64, P.r[j], P.act, cbA[si * np], cbA[(si + 1) * np], j, k, A.angle_reg, A.sim_t)
-                     : sw_score_gpu_list(P.a, P.b, P.r[j], cb[si * np], cb[(si + 1) * np], j, k, A.angle_reg, A.sim_t, A.q_thr, A.cos_thr);
-        } else {
-            const int lo = (int)(A.cstart[chbase + (long long)si * np] - x0), hi = (int)(A.cstart[chbase + (long long)(si + 1) * np] - x0);
-            sc = CPU ? sw_score_cpu(P.a, P.d64, P.r[j], nullptr, lo, hi, j, k, A.angle_reg, A.sim_t)
-                     : sw_score_gpu_list(P.a, P.b, P.r[j], lo, hi, j, k, A.angle_reg, A.sim_t, A.q_thr, A.cos_thr);
-        }
+        const float k = __ldg(&A.views[A.v].k);     // re-read per entry: a register held across this loop spills vmax (REF_GPU)
+        const float sc = CPU ? sw_score_cpu(P.a, P.d64, P.r[j], P.act, cbA[si * np], cbA[(si + 1) * np], j, k, A.angle_reg, A.sim_t)
+                             : sw_score_gpu_chunks(P.a, P.b, P.r[j], P.act, cbA, cinfo, si * np, np, my_chunk, j, k, A.angle_reg, A.sim_t, A.q_thr, A.cos_thr);
         const long long x = x0 + j;
         const int T = __float_as_int(P.b[j].w);
         if (T >= 0 && sc > 0.0f) {      // storeInverseMatches; an inverse match that fails T's orientation check has no entry there
@@ -566,16 +528,17 @@ __device__ __forceinline__ void sw_score_range(const SwScoreArgs<CPU>& A, const 
     if (threadIdx.x == 0 && nact) atomicAdd(A.M + A.v, nact);
 }
 
-template <bool CPU>
+// SMEM: the host knows that every CTA of the launch holds its chunk tables in shared memory, so the scoring loop addresses them as
+// such (LDS, not generic loads); otherwise each CTA decides where its tables live.
+template <bool CPU, bool SMEM>
 __global__ void __launch_bounds__(SW_THREADS, CPU ? (SW_THREADS <= 256 ? 3 : 2) : (SW_THREADS <= 256 ? 5 : SW_THREADS <= 320 ? 4 : SW_THREADS <= 384 ? 3 : 2))
 k_sw_score(const SwScoreArgs<CPU> A)
 {
     const int CAP = A.cap;
     asm volatile("griddepcontrol.launch_dependents;");       // the next view's kernel may start its independent part
     extern __shared__ __align__(16) unsigned char sw_smem[];
-    __shared__ int cb[SW_MAXCH + 1], cbA[SW_MAXCH + 1];
-    __shared__ SwChunkInfo cinfo[SW_MAXNP];
-    __shared__ int ccam[SW_MAXNP];
+    __shared__ int cb_s[SW_MAXCH + 1], cbA_s[SW_MAXCH + 1];
+    __shared__ SwChunkInfo cinfo_s[SW_MAXNP];
     __shared__ SwSegInfo sinfo[SW_SEGS_MAX];
     __shared__ int wcnt[SW_THREADS / 32];
     const L3DViewDev* V = A.views + A.v;
@@ -587,17 +550,18 @@ k_sw_score(const SwScoreArgs<CPU> A)
     const long long x0 = A.cstart[chbase];
     const int n = (int)(A.cstart[chbase + nch] - x0);
     if (n == 0) return;
-    const bool cb_smem = nch <= SW_MAXCH, cinfo_smem = np <= SW_MAXNP;
-    if (cb_smem) for (int q = threadIdx.x; q <= nch; q += SW_THREADS) cb[q] = (int)(A.cstart[chbase + q] - x0);
-    if (cinfo_smem)
-        for (int c = threadIdx.x; c < np; c += SW_THREADS) {
-            const SwChunk ck = A.vp[me.vp_off + c];
-            const L3DViewDev* T = A.views + ck.other;
-            SwChunkInfo ci;
-            ci.other = ck.other; ci.pub = (!ck.inv && A.pairc[ck.pair].y >= 0) ? ck.other : -1; ci.k = T->k; ci.pad = 0.f;
-            ci.Cx = T->C_d[0]; ci.Cy = T->C_d[1]; ci.Cz = T->C_d[2];
-            cinfo[c] = ci; ccam[c] = ck.other;
-        }
+    // where the tables and the staged entries live; the global ones are slices of scratch shared with the kernels of the
+    // neighbouring views, so a CTA that uses them writes nothing before those kernels are done.  That includes cb: it could be
+    // read from cstart before the wait instead, but then the staging would need a second look-up path.
+    const bool cb_smem = SMEM || nch <= SW_MAXCH, ci_smem = SMEM || np <= SW_MAXNP, staged_smem = n <= CAP;
+    int* const gtab = A.gtab + 2 * ((long long)s0 * np + blockIdx.x);
+    int* cb = cb_smem ? cb_s : gtab;
+    int* cbA = cb_smem ? cbA_s : gtab + nch + 1;
+    const SwChunkInfo* cinfo = ci_smem ? cinfo_s : A.cinfo + me.ci_off;
+    const SwPtrs P = staged_smem ? sw_carve(sw_smem, CAP, CPU) : sw_carve(A.gstage + sw_entry_bytes(CPU) * (x0 - me.region_off), n, CPU);
+    if (!cb_smem || !staged_smem) asm volatile("griddepcontrol.wait;" ::: "memory");
+    for (int q = threadIdx.x; q <= nch; q += SW_THREADS) cb[q] = (int)(A.cstart[chbase + q] - x0);
+    if (ci_smem) for (int c = threadIdx.x; c < np; c += SW_THREADS) cinfo_s[c] = A.cinfo[me.ci_off + c];
     if (threadIdx.x < nsegs) {
         const long long gs = V->seg_off + s0 + threadIdx.x;
         const SegRays R = load_rays(A.cache, gs);
@@ -608,17 +572,7 @@ k_sw_score(const SwScoreArgs<CPU> A)
         sinfo[threadIdx.x] = si;
     }
     __syncthreads();
-    SwPtrs P;
-    if (n <= CAP) {
-        P.a = (float4*)sw_smem; P.b = P.a + CAP; P.r = (float2*)(P.b + CAP); P.act = (int*)(P.r + CAP);
-        P.d64 = CPU ? (double4*)(sw_smem + (size_t)CAP * 48) : nullptr;           // 16 + 16 + 8 + 4 = 44 -> rounded up to 48 for the double4 alignment
-    } else {
-        // the global scratch is shared with the kernels of the neighbouring views: only touch it once they are done
-        asm volatile("griddepcontrol.wait;" ::: "memory");
-        const long long rel = x0 - me.region_off;
-        P.a = A.g.a + rel; P.b = A.g.b + rel; P.r = A.g.r + rel; P.act = A.g.act + rel; P.d64 = CPU ? A.g.d64 + rel : nullptr;
-    }
-    sw_score_range<CPU>(A, P, cb, cbA, cb_smem, cinfo, ccam, cinfo_smem, sinfo, wcnt, s0, nsegs, x0, n);
+    sw_score_range<CPU>(A, P, cb, cbA, cinfo, sinfo, wcnt, nsegs, x0, n);
 }
 
 // ---------------------------------------------------------------------------------------------- after the chain
@@ -738,14 +692,15 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
     // chunk descriptors of every view in list order: REF_GPU sorts a segment's matches by (tgt cam, tgt seg) (sortMatches,
     // line3D.cc:1196-1205): chunks by the other view's camID.  REF_CPU keeps the append order (scoringCPU does not sort): first
     // the inverse matches, stored by the earlier views in their processing order, then the direct ones in matching order.
+    struct SwChunk { int pair, inv, other; };      // chunk c of a view: pair index, inverse?, the other view
     std::vector<std::vector<SwChunk> > chunks(V);
     for (int p = 0; p < NP; ++p) {
         const L3DPairDev& P = c->h_pairs[p];
-        chunks[P.src].push_back(SwChunk{p, 0, P.tgt, 0});
-        if (rank[P.tgt] > rank[P.src]) chunks[P.tgt].push_back(SwChunk{p, 1, P.src, 0});   // tgt still unprocessed when src stores its inverse matches (line3D.cc:1680)
+        chunks[P.src].push_back(SwChunk{p, 0, P.tgt});
+        if (rank[P.tgt] > rank[P.src]) chunks[P.tgt].push_back(SwChunk{p, 1, P.src});   // tgt still unprocessed when src stores its inverse matches (line3D.cc:1680)
     }
-    std::vector<SwChunk> vp; std::vector<SwView> vt(V); std::vector<int2> pairc(NP, make_int2(-1, -1));
-    long long NC = 0;
+    std::vector<SwChunkInfo> cinfo; std::vector<SwView> vt(V); std::vector<int2> pairc(NP, make_int2(-1, -1));
+    long long NC = 0, tab_max = 0;
     for (int i = 0; i < V; ++i) {
         const int v = S.order[i];
         std::vector<SwChunk>& L = chunks[v];
@@ -753,10 +708,17 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
         else std::stable_sort(L.begin(), L.end(), [&](const SwChunk& a, const SwChunk& b) {
             if (a.inv != b.inv) return a.inv > b.inv;
             return a.inv ? rank[a.other] < rank[b.other] : a.pair < b.pair; });
-        vt[v].vp_off = (int)vp.size(); vt[v].np = (int)L.size(); vt[v].chunk_base = NC; vt[v].region_off = 0;
-        for (int k = 0; k < (int)L.size(); ++k) { if (L[k].inv) pairc[L[k].pair].y = k; else pairc[L[k].pair].x = k; }
-        vp.insert(vp.end(), L.begin(), L.end());
-        NC += (long long)c->h_views[v].nseg * (long long)L.size();
+        vt[v].ci_off = (int)cinfo.size(); vt[v].np = (int)L.size(); vt[v].chunk_base = NC; vt[v].region_off = 0;
+        for (int k = 0; k < (int)L.size(); ++k) {
+            if (L[k].inv) pairc[L[k].pair].y = k; else pairc[L[k].pair].x = k;
+            const L3DViewDev& T = c->h_views[L[k].other];
+            // a positive score of a direct match is announced to the other view if that holds the inverse match (is processed later)
+            const int pub = !L[k].inv && rank[L[k].other] > i ? L[k].other : -1;
+            cinfo.push_back(SwChunkInfo{L[k].other, pub, T.k, 0.f, T.C_d[0], T.C_d[1], T.C_d[2]});
+        }
+        const long long nseg = c->h_views[v].nseg;
+        NC += nseg * (long long)L.size();
+        tab_max = std::max(tab_max, nseg * ((long long)L.size() + 1));     // chunk boundaries of all its CTAs: nseg * np + CTAs
     }
     std::vector<long long> row_off(NP + 1);
     for (int p = 0; p < NP; ++p) row_off[p] = c->h_pairs[p].row_off;
@@ -764,7 +726,7 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
 
     int rc;
     cudaStream_t st = c->stream;
-    L3D_RESERVE(S.d_vt, sizeof(SwView) * (size_t)V, "view table"); L3D_RESERVE(S.d_vp, sizeof(SwChunk) * vp.size(), "chunk descriptors"); L3D_RESERVE(S.d_pairc, 8 * (size_t)NP, "pair chunks");
+    L3D_RESERVE(S.d_vt, sizeof(SwView) * (size_t)V, "view table"); L3D_RESERVE(S.d_cinfo, sizeof(SwChunkInfo) * cinfo.size(), "chunk descriptors");
     L3D_RESERVE(S.d_rowoff, 8 * (size_t)(NP + 1), "pair row offsets"); L3D_RESERVE(S.d_order, 4 * (size_t)V, "order"); L3D_RESERVE(S.d_region_off, 8 * (size_t)(V + 1), "region offsets");
     const long long nblocks = (slots + SW_SETUP_THREADS - 1) / SW_SETUP_THREADS;
     L3D_RESERVE(S.d_pinfo, sizeof(SwPairInfo) * (size_t)(NP + 1), "pair table"); L3D_RESERVE(S.d_bpair, 4 * std::max<long long>(nblocks, 1), "first pair of every block");
@@ -773,8 +735,7 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
     L3D_RESERVE(S.d_ranges, 8 * c->total_segs, "ranges"); L3D_RESERVE(S.d_est_best, 4 * c->total_segs, "estimates"); L3D_RESERVE(S.d_est_P, 48 * c->total_segs, "estimate points");
     L3D_RESERVE(S.d_M, 4 * (size_t)V, "match counts"); L3D_RESERVE(S.d_vmax, 4 * (size_t)V, "view max");
     L3D_CUDA(c, cudaMemcpyAsync(S.d_vt.p, vt.data(), sizeof(SwView) * (size_t)V, cudaMemcpyHostToDevice, st), "view table");
-    if (!vp.empty()) L3D_CUDA(c, cudaMemcpyAsync(S.d_vp.p, vp.data(), sizeof(SwChunk) * vp.size(), cudaMemcpyHostToDevice, st), "chunk descriptors");
-    if (NP) L3D_CUDA(c, cudaMemcpyAsync(S.d_pairc.p, pairc.data(), 8 * (size_t)NP, cudaMemcpyHostToDevice, st), "pair chunks");
+    if (!cinfo.empty()) L3D_CUDA(c, cudaMemcpyAsync(S.d_cinfo.p, cinfo.data(), sizeof(SwChunkInfo) * cinfo.size(), cudaMemcpyHostToDevice, st), "chunk descriptors");
     L3D_CUDA(c, cudaMemcpyAsync(S.d_rowoff.p, row_off.data(), 8 * (size_t)(NP + 1), cudaMemcpyHostToDevice, st), "pair row offsets");
     L3D_CUDA(c, cudaMemcpyAsync(S.d_order.p, S.order.data(), 4 * (size_t)V, cudaMemcpyHostToDevice, st), "order");
     std::vector<SwPairInfo> pinfo((size_t)NP + 1);
@@ -798,7 +759,7 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
     }
     L3D_CUDA(c, cudaMemcpyAsync(S.d_pinfo.p, pinfo.data(), sizeof(SwPairInfo) * (size_t)(NP + 1), cudaMemcpyHostToDevice, st), "pair table");
     L3D_CUDA(c, cudaMemcpyAsync(S.d_bpair.p, bpair.data(), 4 * bpair.size(), cudaMemcpyHostToDevice, st), "first pair of every block");
-    L3D_CUDA(c, cudaStreamSynchronize(st), "score sweep tables");      // pinfo / bpair are locals
+    L3D_CUDA(c, cudaStreamSynchronize(st), "score sweep tables");      // cinfo / pinfo / bpair are locals
     L3D_CUDA(c, cudaMemsetAsync(S.d_csize.p, 0, 4 * (size_t)(NC + 1), st), "init chunk sizes");
     L3D_CUDA(c, cudaMemsetAsync(S.d_ccur.p, 0, 4 * (size_t)(NC + 1), st), "init chunk cursors");
     L3D_CUDA(c, cudaMemsetAsync(S.d_rflag.p, 0, (size_t)slots, st), "init record flags");
@@ -812,7 +773,7 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
     const float4* segs = c->segs(); const float4* cache = (const float4*)c->d_cache.p;
     const L3DViewDev* views = c->views(); const L3DPairDev* pairs = (const L3DPairDev*)c->d_pairs.p;
     const int* counts = (const int*)c->d_counts.p; const l3d_match_rec* recs = (const l3d_match_rec*)c->d_recs.p;
-    const SwView* d_vt = (const SwView*)S.d_vt.p; const int2* d_pairc = (const int2*)S.d_pairc.p; const long long* d_rowoff = (const long long*)S.d_rowoff.p;
+    const SwView* d_vt = (const SwView*)S.d_vt.p; const long long* d_rowoff = (const long long*)S.d_rowoff.p;
     const unsigned int nbs = (unsigned int)nblocks;
     S.region_off.assign(V + 1, 0); S.total = 0;
     if (NP > 0 && slots > 0) {
@@ -836,14 +797,16 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
     if (Umax >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_score_sweep: view with more than 2^31 matches");
     L3D_RESERVE(S.d_eval, 4 * total, "entry records"); L3D_RESERVE(S.d_escore, 4 * total, "entry scores"); L3D_RESERVE(S.d_eflag, total, "entry flags");
     L3D_RESERVE(S.d_ekv, 8 * total, "unsorted entries");
-    L3D_RESERVE(S.d_gstage, 2 * 48 * Umax, "long-list scratch"); L3D_RESERVE(S.d_gpub, 2 * 4 * Umax, "long-list scratch");
-    if (cpu_sem) L3D_RESERVE(S.d_dir64, 2 * 32 * Umax, "long-list scratch");
+    // global scratch of the chain, double-buffered (two kernels may be in flight): staged entries of the longest region, chunk
+    // tables of the view with the most chunk boundaries
+    const size_t per_entry = sw_entry_bytes(cpu_sem);
+    L3D_RESERVE(S.d_gstage, 2 * per_entry * Umax, "long-list scratch"); L3D_RESERVE(S.d_gtab, 2 * 2 * 4 * tab_max, "chunk table scratch");
     unsigned int* e_val = (unsigned int*)S.d_eval.p; float* e_score = (float*)S.d_escore.p; unsigned char* e_flag = (unsigned char*)S.d_eflag.p;
     if (total > 0) {
         k_sw_scatter<<<nbs, SW_SETUP_THREADS, 0, st>>>((const SwPairInfo*)S.d_pinfo.p, (const int*)S.d_bpair.p, recs, knn, slots, (const unsigned char*)S.d_rflag.p,
                                                        (const long long*)S.d_cstart.p, (int*)S.d_ccur.p, (uint2*)S.d_ekv.p, cpu_sem ? 1 : 0);
         k_sw_chunksort<<<(unsigned int)((c->total_segs + CS_WARPS - 1) / CS_WARPS), 32 * CS_WARPS, 0, st>>>(views, V, c->total_segs, d_vt, (const long long*)S.d_cstart.p,
-                                                                                                         (uint2*)S.d_ekv.p, e_val, e_flag, (unsigned int*)S.d_invpos.p);
+                                                                                                         (const uint2*)S.d_ekv.p, e_val, e_flag, (unsigned int*)S.d_invpos.p);
         c->launches += 2;
     }
 
@@ -859,26 +822,19 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
     if (total > 0) {
         SwScoreArgs<false> A;
         A.cache = cache; A.rays = (const double*)S.d_rays.p; A.views = views; A.recs = recs; A.v = 0;
-        A.vt = d_vt; A.vp = (const SwChunk*)S.d_vp.p; A.pairc = d_pairc; A.cstart = (const long long*)S.d_cstart.p;
+        A.vt = d_vt; A.cinfo = (const SwChunkInfo*)S.d_cinfo.p; A.cstart = (const long long*)S.d_cstart.p;
         A.e_val = e_val; A.e_score = e_score; A.e_flag = e_flag; A.invpos = (const unsigned int*)S.d_invpos.p;
         A.view_max_bits = (int*)S.d_vmax.p; A.M = (int*)S.d_M.p;
-        SwPtrs gbuf[2];
-        for (int q = 0; q < 2; ++q) {
-            gbuf[q].a = (float4*)S.d_gstage.p + (size_t)q * Umax * 3;      // 40 B per entry = 2.5 float4: 3 keeps every part 16-byte aligned
-            gbuf[q].b = gbuf[q].a + Umax; gbuf[q].r = (float2*)(gbuf[q].b + Umax);
-            gbuf[q].act = (int*)S.d_gpub.p + (size_t)q * Umax;
-            gbuf[q].d64 = cpu_sem ? (double4*)S.d_dir64.p + (size_t)q * Umax : nullptr;
-        }
-        A.g = gbuf[0];
         int launched = 0;
         A.angle_reg = two_sigA_sqr; A.sim_t = min_similarity; A.q_thr = q_thr; A.cos_thr = cos_thr;
         SwScoreArgs<true> B;
         static_assert(sizeof(SwScoreArgs<true>) == sizeof(SwScoreArgs<false>), "same layout");
         std::memcpy((void*)&B, (const void*)&A, sizeof(A));
-        const size_t per_entry = cpu_sem ? 48 + 32 : 48;
-        L3D_CUDA(c, cudaFuncSetAttribute(k_sw_score<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(48 * SW_CAP_MAX)), "k_sw_score shared memory");
-        L3D_CUDA(c, cudaFuncSetAttribute(k_sw_score<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(80 * 2048)), "k_sw_score shared memory");
-        const int cap_max = cpu_sem ? 2048 : SW_CAP_MAX;
+        for (auto kern : {k_sw_score<false, true>, k_sw_score<false, false>})
+            L3D_CUDA(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sw_entry_bytes(false) * SW_CAP_MAX)), "k_sw_score shared memory");
+        for (auto kern : {k_sw_score<true, true>, k_sw_score<true, false>})
+            L3D_CUDA(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sw_entry_bytes(true) * SW_CAP_MAX_CPU)), "k_sw_score shared memory");
+        const int cap_max = cpu_sem ? SW_CAP_MAX_CPU : SW_CAP_MAX;
         const int occ_regs = cpu_sem ? 3 : 5;               // resident CTAs per SM the register budget allows (launch bounds)
         const int force_segs = getenv("L3D_SW_SEGS") ? atoi(getenv("L3D_SW_SEGS")) : 0;      // tools/sweep_score.py: override the geometry choice
         for (int i = 0; i < V; ++i) {
@@ -908,10 +864,12 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
             // programmatic dependent launch: this view's kernel may stage its lists while the previous view's kernel is still scoring
             // (it waits before it reads the bits that kernel publishes).  The first one follows ordinary kernels: plain stream order.
             cfg.attrs = attr; cfg.numAttrs = launched ? 1 : 0;
-            A.g = gbuf[launched & 1]; B.g = gbuf[launched & 1];       // long-list scratch: double-buffered, two kernels may be in flight
+            A.gstage = B.gstage = (unsigned char*)S.d_gstage.p + (launched & 1) * per_entry * Umax;     // double-buffered scratch
+            A.gtab = B.gtab = (int*)S.d_gtab.p + (launched & 1) * 2 * tab_max;
             ++launched;
-            if (cpu_sem) { B.v = v; L3D_CUDA(c, cudaLaunchKernelEx(&cfg, k_sw_score<true>, B), "k_sw_score"); }
-            else { A.v = v; L3D_CUDA(c, cudaLaunchKernelEx(&cfg, k_sw_score<false>, A), "k_sw_score"); }
+            const bool smem_tables = vt[v].np <= SW_MAXNP && segs * vt[v].np <= SW_MAXCH;
+            if (cpu_sem) { B.v = v; L3D_CUDA(c, cudaLaunchKernelEx(&cfg, smem_tables ? k_sw_score<true, true> : k_sw_score<true, false>, B), "k_sw_score"); }
+            else { A.v = v; L3D_CUDA(c, cudaLaunchKernelEx(&cfg, smem_tables ? k_sw_score<false, true> : k_sw_score<false, false>, A), "k_sw_score"); }
             ++c->launches;
         }
         L3D_CUDA(c, cudaGetLastError(), "score sweep launch");

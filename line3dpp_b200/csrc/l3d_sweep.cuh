@@ -20,9 +20,8 @@
 struct SwView {               // per view (by view index)
     long long chunk_base;     // first chunk of the view: chunk(seg, c) = chunk_base + seg * np + c
     long long region_off;     // first entry of the view's region
-    int vp_off, np;           // the view's chunk descriptors: vp[vp_off .. vp_off + np)
+    int ci_off, np;           // the view's chunk descriptors: cinfo[ci_off .. ci_off + np)
 };
-struct SwChunk { int pair, inv, other, pad; };   // chunk c of a view: pair index, inverse?, the other view
 
 struct SwEntry { int seg, tgt_view, tgt_seg; float4 dep; float overlap; };
 

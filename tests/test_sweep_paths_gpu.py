@@ -1,15 +1,16 @@
-"""The scoring sweep (l3d_score_sweep, csrc/l3d_pipeline.cu) on scenes wide enough to take the paths it picks by size: views with
-more than 64 neighbour chunks, more than 512 chunk boundaries per CTA, lists longer than the shared-memory staging capacity and
-segments matched into more than 48 target cameras.  The other suites never cross these thresholds (at most 25 chunks per view).
+"""The scoring sweep (l3d_score_sweep, csrc/l3d_pipeline.cu) on scenes wide enough that its tables outgrow shared memory and are
+read from global memory instead: views with more than 64 neighbour chunks, more than 512 chunk boundaries per CTA, segments with
+more than 192 entries, lists longer than the shared-memory staging capacity; and segments matched into more than 48 target
+cameras.  The other suites never cross these thresholds (at most 25 chunks per view).
 
-  W1  70 views, dense neighbours (np = 69), REF_GPU: global chunk descriptors, the list scoring loop, the chunk-sort fallback
-  W2  64 views, ring +-30 (np = 60), REF_GPU: chunked scoring up to 8 segments per CTA, global chunk boundaries from 9 on
+  W1  70 views, dense neighbours (np = 69), REF_GPU: chunk descriptors and chunk-sort keys read from global memory
+  W2  64 views, ring +-30 (np = 60), REF_GPU: chunk boundaries in shared memory up to 8 segments per CTA, in global memory from 9 on
   W3  W2 with a heavy tail (one segment matched by 120 pieces of its line in each of 41 views): the automatic geometry
       overflows the staging capacity and scores that CTA out of the global scratch
   W4  52 views, dense (np = 51), REF_CPU: segments with more than 48 target cameras (the per-camera maximum beyond the 48-slot map)
 
-Every test first asserts, from what the product exports, that the path it is about is taken (np from the pair list; the
-active entries of a segment are a lower bound of its list length), so none of them can pass without reaching its path.
+Every test first asserts, from what the product exports, that the threshold it is about is crossed (np from the pair list; the
+active entries of a segment are a lower bound of its list length), so none of them can pass without crossing it.
 The verbatim reference's results are stored in tests/golden/ref_gpu_wide_v1.npz (REF_GPU, W1-W3) and
 tests/golden/ref_full_wide_cpu_v1.npz (REF_CPU, W4), made by tests/golden/make_ref_wide_golden.py."""
 import ctypes as C
@@ -27,7 +28,7 @@ G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 GPU_GOLDEN = os.path.join(G, "ref_gpu_wide_v1.npz")
 CPU_GOLDEN = os.path.join(G, "ref_full_wide_cpu_v1.npz")
 
-# the sweep's size thresholds (csrc/l3d_pipeline.cu)
+# the sweep's capacity thresholds (csrc/l3d_pipeline.cu): beyond them a table is read from global instead of shared memory
 SW_MAXCH = 512            # chunk boundaries per CTA held in shared memory
 SW_MAXNP = 64             # chunk descriptors held in shared memory
 CS_MAXN = 192             # entries of one segment the chunk sort handles in shared memory
@@ -166,10 +167,10 @@ def check_ref_gpu_preconditions(name, L, sc):
     counts = [active_per_segment(L, sc, cam) for cam in sc.cam_ids]
     longest = max(int(c.max()) for c in counts)
     if name == "w1":
-        assert (npv > SW_MAXNP).all(), npv            # global chunk descriptors, list scoring, chunk-sort fallback
+        assert (npv > SW_MAXNP).all(), npv            # chunk descriptors and chunk-sort keys read from global memory
     else:
         assert (npv <= SW_MAXNP).all() and (8 * npv <= SW_MAXCH).all() and (9 * npv > SW_MAXCH).all(), npv
-    assert longest > CS_MAXN, longest                 # the chunk sort's global fallback
+    assert longest > CS_MAXN, longest                 # chunk-sort keys read from global memory
     if name == "w3":
         # the heavy segment alone holds more than any CTA can stage, whatever geometry the sweep picks: global scratch
         n = int(counts[-1][heavy_segment(sc)])
@@ -192,8 +193,8 @@ def test_ref_gpu_wide_vs_verbatim_reference(monkeypatch, scenes, gpu_golden, nam
 
 @pytest.mark.parametrize("name", ["w1", "w2", "w3", "w4"])
 def test_sweep_geometry_invariance(monkeypatch, scenes, name):
-    """the segments per CTA (L3D_SW_SEGS) move every view across the chunked / list, shared / global and staged / scratch
-    boundaries; none of that may change a bit of the scored and kept lists, score3D or the estimates"""
+    """the segments per CTA (L3D_SW_SEGS) move every view across the shared / global boundaries of the chunk tables and of the
+    staged entries; none of that may change a bit of the scored and kept lists, score3D or the estimates"""
     sc = scenes[name]
     cpu_sem = name == "w4"
     L = run(monkeypatch, sc, name, cpu_sem=cpu_sem)
