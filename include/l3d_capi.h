@@ -13,7 +13,8 @@
  * 0 on success or a negative l3d_status; l3d_last_error() gives the message (the reference prints CUDA errors to
  * cerr and carries on, dataArray.h:198-237).  A call that fails leaves its stage (views, matches, score sweep,
  * collinear lists, affinity matrix), and every stage computed from it, without a result: later calls that need one
- * return L3D_ERR_STATE.  The image calls (l3d_undistort_u8, l3d_undistort_map, l3d_remap_u8) are not part of that chain: whether
+ * return L3D_ERR_STATE.  The image calls (l3d_undistort_u8, l3d_undistort_map, l3d_remap_u8) and the tie-point calls
+ * (l3d_triangulate_points, l3d_median_depths) are not part of that chain: whether
  * they succeed or fail, every stage and its result stay as they were.  A context is single-owner (not thread-safe), one per GPU, and runs
  * on its own non-default stream.  There is NO CPU fallback: without a usable CUDA device l3d_ctx_create fails.
  */
@@ -262,6 +263,26 @@ int l3d_undistort_u8(l3d_ctx* ctx, int n, const l3d_undistort_desc* descs, int o
 int l3d_undistort_map(l3d_ctx* ctx, const l3d_undistort_desc* desc, int16_t* map_xy, uint16_t* map_frac, int on_device);
 /* cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) of one image with caller-given maps in that layout (the camera is not used) */
 int l3d_remap_u8(l3d_ctx* ctx, const l3d_undistort_desc* desc, const int16_t* map_xy, const uint16_t* map_frac, int on_device);
+
+/* ---- tie-point triangulation: linearHomTriangulation of the reference's Pix4D frontend (main_pix4d.cpp:34-70, 354-372) for every point
+ * in one launch.  Point i has the observations [obs_ptr[i], obs_ptr[i+1]) (obs_ptr[0] = 0): camera obs_cam[o] in [0, n_cams) and image
+ * point (obs_xy[2o], obs_xy[2o+1]); P: the 3x4 projection matrix of every camera, 12 doubles row-major.  A point with fewer than three
+ * observations is invalid with X = 0, as the reference skips it.  Otherwise A^T A (4x4, double) is accumulated from the rows Sx P[cam]
+ * in observation order, its eigenvector v of the smallest eigenvalue is found by cyclic Jacobi in double, X = v.xyz / v.w, and
+ * valid = |X| > L3D_EPS (1e-12) compared as the reference does: NaN is invalid, +-Inf is valid.  Not bit-exact to Eigen's JacobiSVD:
+ * the contract is the tolerance of DESIGN.md §6b.  X_out: 3 doubles per point; valid_out: 0 / 1 per point.
+ * on_device != 0: every pointer is a device address on this GPU and the call is asynchronous on the context's stream; an observation
+ * of a camera outside [0, n_cams) then makes its point invalid.  on_device == 0: host arrays, checked (L3D_ERR_INVALID for a decreasing
+ * obs_ptr or an unknown camera), staged through the context's own buffers; the call returns when the outputs are written. */
+int l3d_triangulate_points(l3d_ctx* ctx, long long n_points, const int64_t* obs_ptr, const int32_t* obs_cam, const double* obs_xy, int n_cams,
+                           const double* P, double* X_out, int32_t* valid_out, int on_device);
+/* per-camera median depth of main_pix4d.cpp:386-418: camera c lists the points [list_ptr[c], list_ptr[c+1]) of list_pts (ids into X /
+ * valid, repeats allowed); count_out[c] = the number of list entries whose point is valid, median_out[c] = the element at count/2 of
+ * their float depths (float)|X - C[c]| sorted ascending, 0 when there are none.  One device pass: depths, a segmented sort, a pick;
+ * exact given X.  At most 2^31 - 1 list entries per call.  on_device as for l3d_triangulate_points (a point id outside [0, n_points)
+ * counts as invalid on the device and is rejected on the host). */
+int l3d_median_depths(l3d_ctx* ctx, int n_cams, const int64_t* list_ptr, const int32_t* list_pts, long long n_points, const double* X,
+                      const int32_t* valid, const double* C, int32_t* count_out, float* median_out, int on_device);
 
 /* stable ascending argsort of float keys on the device: the weight sort of performClustering (clustering.cc:13-14) for
  * large edge lists.  perm_out[i] = index of the i-th smallest key, ties in input order. */

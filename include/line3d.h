@@ -196,6 +196,26 @@ public:
     size_t numImages();                                                /* line3D.h:205 */
     std::string createOutputFilename();                                /* line3D.h:224 */
     static Matrix3d rotationFromQ(const double Qw, const double Qx, const double Qy, const double Qz);   /* line3D.h:219-220 */
+    /* line3D.cc:2714-2727: Rz(yaw) * Ry(pitch) * Rx(roll), each as Eigen's AngleAxisd(angle, unit axis).toRotationMatrix() forms it
+     * (the mavmap frontend's camera rotation).  Returns the POD Matrix3d, like rotationFromQ. */
+    static Matrix3d rotationFromRPY(const double roll, const double pitch, const double yaw);
+    /* line3D.cc:2784-2852: K, R, t with P = K [R|t] (P: 3x4, row-major) by the reference's RQ decomposition: Givens rotations
+     * Rx, Ry, Rz on P's left 3x3 block, the column-sign fix (positive diagonal of K), R = (Rx Ry Rz Sign)^T, t = K^-1 P4 with K
+     * before normalisation, then K divided by K(2,2). */
+    static void decomposeProjectionMatrix(const double P[12], Matrix3d& K, Matrix3d& R, Vector3d& t);
+#ifdef L3DPP_WITH_EIGEN_OPENCV
+    /* the reference's signature (line3D.h:230-233); a P that is not 3x4 leaves the outputs untouched (the reference prints a message) */
+    static void decomposeProjectionMatrix(const Eigen::MatrixXd P_in, Eigen::Matrix3d& K_out, Eigen::Matrix3d& R_out, Eigen::Vector3d& t_out)
+    {
+        if (P_in.rows() != 3 || P_in.cols() != 4) return;
+        double P[12];
+        for (int r = 0; r < 3; ++r) for (int c = 0; c < 4; ++c) P[4 * r + c] = P_in(r, c);
+        Matrix3d K, R; Vector3d t;
+        decomposeProjectionMatrix(P, K, R, t);
+        for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) { K_out(r, c) = K(r, c); R_out(r, c) = R(r, c); }
+        t_out(0) = t.x; t_out(1) = t.y; t_out(2) = t.z;
+    }
+#endif
 
     /* line3D.h:119-122: lens undistortion as the reference does it with OpenCV (initUndistortRectifyMap with fixed-point maps +
      * remap, bilinear, border 0; include/l3d_capi.h l3d_undistort_u8).  Uses K(0,0), K(1,1), K(0,2), K(1,2) only; out gets the size

@@ -1,6 +1,6 @@
-/* include/line3d_io.h — input format of the VisualSfM frontend (SURVEY.md §8f-2): what main_vsfm.cpp:143-310 reads from an
- * .nvm file before it calls Line3D::addImage, as a library function so that a frontend built on include/line3d.h needs no
- * parsing code of its own; and the reference's binary result file and segment cache.  Host-only; no CUDA involved. */
+/* include/line3d_io.h — input formats of the reference's six frontends (SURVEY.md §8f-2): what main_*.cpp read from an SfM model
+ * before they call Line3D::addImage, as library functions so that a frontend built on include/line3d.h needs no parsing code of its
+ * own; and the reference's binary result file and segment cache.  Host code; readPix4D triangulates through include/l3d_capi.h. */
 #ifndef L3DPP_LINE3D_IO_H_
 #define L3DPP_LINE3D_IO_H_
 #include "line3d.h"
@@ -25,14 +25,14 @@ struct NVMCamera {
 /* Reads an NVM_V3 file like main_vsfm.cpp:143-250.  Returns false and sets *error on an unreadable or empty model. */
 bool readNVM(const std::string& path, std::vector<NVMCamera>& cameras, std::string* error = 0);
 
-/* one camera of a Bundler or COLMAP model, ready for Line3D::addImage.  Bundler has no K in the file (focal only: build it with
- * intrinsicsFromFocal once the image size is known, main_bundler.cpp:340-351); COLMAP stores K per camera model. */
+/* one camera of a Bundler, COLMAP, mavmap, OpenMVG or Pix4D model, ready for Line3D::addImage.  Bundler has no K in the file (focal
+ * only: build it with intrinsicsFromFocal once the image size is known, main_bundler.cpp:340-351); the others store K. */
 struct SfMCamera {
-    unsigned int id;                       /* camID handed to addImage: bundler camera index / COLMAP IMAGE_ID */
+    unsigned int id;                       /* camID handed to addImage: bundler / mavmap / Pix4D camera index, COLMAP IMAGE_ID, OpenMVG id_view */
     std::string image;                     /* image file name (bundler: from the optional list file, may be empty) */
-    bool has_K; Matrix3d K;                /* COLMAP only */
+    bool has_K; Matrix3d K;                /* all but Bundler */
     float focal;                           /* bundler only */
-    double radial[3], tangential[2];       /* distortion the frontend undistorts with (bundler: k1 k2 0; COLMAP: per camera model) */
+    double radial[3], tangential[2];       /* distortion the frontend undistorts with (bundler: k1 k2 0; others: per camera model) */
     Matrix3d R; Vector3d t, C;             /* x_cam = R X + t,  C = -R^T t */
     std::list<unsigned int> worldpoints;
     float median_depth;                    /* 0 if the camera sees no world point (it is skipped by the frontends) */
@@ -45,6 +45,34 @@ bool readBundler(const std::string& bundle_file, const std::string& image_list_f
 /* cameras.txt / images.txt / points3D.txt of a COLMAP text model like main_colmap.cpp:140-349 (models SIMPLE_PINHOLE, PINHOLE,
  * SIMPLE_RADIAL, RADIAL, OPENCV, FULL_OPENCV; images whose camera is unknown are dropped).  Cameras are returned in file order. */
 bool readColmap(const std::string& sfm_folder, std::vector<SfMCamera>& cameras, std::string* error = 0);
+
+/* The mavmap, OpenMVG and Pix4D models (csrc/line3d_sfm.cc, DESIGN.md §6b).  Like the readers above: false with *error naming the
+ * file, the line or JSON path and the problem on malformed input, which never crashes the reader and never makes it allocate more
+ * than the input's size warrants.  Every camera has has_K set. */
+
+/* mavmap's result file like main_mavmap.cpp:153-250: leading '#' lines skipped, a line shorter than 28 characters ends the list, every
+ * field carries a trailing comma, only the PINHOLE model; R = rotationFromRPY(roll, pitch, yaw) and [R|t] inverted (R^T, -R^T t),
+ * C = the stored position; id = position in the file.  mavmap has no world points: worldpoints stays empty and median_depth 0 (the
+ * frontend passes sequentialNeighbors lists with neighbors_by_worldpoints = false and matches with const_regularization_depth). */
+bool readMavmap(const std::string& path, std::vector<SfMCamera>& cameras, std::string* error = 0);
+
+/* up to num_neighbors / 2 earlier cameras, nearest first, then later cameras until num_neighbors (main_mavmap.cpp:312-321) */
+std::list<unsigned int> sequentialNeighbors(unsigned int i, unsigned int n_cams, unsigned int num_neighbors);
+
+/* OpenMVG's sfm_data.json like main_openmvg.cpp:136-410: views, intrinsics (pinhole_radial_k1 / _k3, pinhole_brown_t2; other models
+ * carry no distortion; an entry without polymorphic_name keeps the model of the entry before it, as the reference's loop does),
+ * extrinsics (t = -R C, C as stored), structure (world point ids and float depths |C - X| per view, file order).  A view is returned,
+ * in view order with id = id_view, when it has intrinsics and at least one world point.  The images are not looked for: a frontend
+ * skips the views whose image it cannot load.  Numbers are read with a correctly rounded strtod. */
+bool readOpenMVG(const std::string& sfm_data_json, std::vector<SfMCamera>& cameras, std::string* error = 0);
+
+/* <params_folder>/<project_prefix>[_]calibrated_camera_parameters.txt and ..._tp_pix4d.txt like main_pix4d.cpp:163-420.  Every tie point
+ * with more than two observations is triangulated on the GPU (l3d_triangulate_points) and every camera's median depth is taken over
+ * its valid points (l3d_median_depths), on device cuda_device; without a usable device the reader returns false.  A camera is
+ * returned, id = position in the camera file, when more than two of its points are valid; worldpoints is every observation of its
+ * key image, duplicates included.  A key image missing from the camera file is camera 0, as the reference's std::map lookup makes it. */
+bool readPix4D(const std::string& params_folder, const std::string& project_prefix, std::vector<SfMCamera>& cameras, std::string* error = 0,
+               int cuda_device = 0);
 
 /* K of main_vsfm.cpp:266-278: focal on the diagonal, principal point at the image centre (float arithmetic like the reference) */
 Matrix3d intrinsicsFromFocal(float focal, int image_width, int image_height);

@@ -282,6 +282,43 @@ class Context:
         op = (C.c_void_p * len(pairs))(*[int(x) for x in overlap_ptrs])
         self._chk(self.L.l3d_match_dense_pairs(self.h, len(pairs), _p(pairs), _p(F), C.c_float(epi_overlap), dp, op), "l3d_match_dense_pairs")
 
+    # ---- tie points (stateless: no pipeline stage changes)
+    def triangulate_points(self, obs_ptr, obs_cam, obs_xy, P):
+        """l3d_triangulate_points on host arrays: obs_ptr int64 [n+1] (CSR over points), obs_cam int32 [m], obs_xy float64 [m, 2],
+        P float64 [cams, 3, 4].  Returns (X float64 [n, 3], valid int32 [n])."""
+        ptr = np.ascontiguousarray(obs_ptr, np.int64)
+        cam = np.ascontiguousarray(obs_cam, np.int32)
+        xy = np.ascontiguousarray(obs_xy, np.float64).reshape(-1, 2)
+        P = np.ascontiguousarray(P, np.float64).reshape(-1, 12)
+        n = len(ptr) - 1
+        if n < 0 or len(cam) != len(xy) or (n >= 0 and ptr[-1] != len(cam)):
+            raise ValueError("obs_ptr must have n+1 entries ending at the number of observations")
+        X = np.zeros((n, 3), np.float64); valid = np.zeros(n, np.int32)
+        self._chk(self.L.l3d_triangulate_points(self.h, C.c_longlong(n), _p(ptr), _p(cam), _p(xy), len(P), _p(P), _p(X), _p(valid), 0),
+                  "l3d_triangulate_points")
+        return X, valid
+
+    def triangulate_points_device(self, n, obs_ptr, obs_cam, obs_xy, n_cams, P, X_out, valid_out):
+        """l3d_triangulate_points on device addresses; asynchronous on the context's stream"""
+        a = [C.c_void_p(int(x)) for x in (obs_ptr, obs_cam, obs_xy, P, X_out, valid_out)]
+        self._chk(self.L.l3d_triangulate_points(self.h, C.c_longlong(n), a[0], a[1], a[2], int(n_cams), a[3], a[4], a[5], 1), "l3d_triangulate_points")
+
+    def median_depths(self, list_ptr, list_pts, X, valid, centres):
+        """l3d_median_depths on host arrays: per camera the points list_pts[list_ptr[c]:list_ptr[c+1]] and its centre.  Returns
+        (count int32 [cams], median float32 [cams])."""
+        lptr = np.ascontiguousarray(list_ptr, np.int64)
+        lpts = np.ascontiguousarray(list_pts, np.int32)
+        X = np.ascontiguousarray(X, np.float64).reshape(-1, 3)
+        valid = np.ascontiguousarray(valid, np.int32)
+        Cs = np.ascontiguousarray(centres, np.float64).reshape(-1, 3)
+        nc = len(lptr) - 1
+        if nc != len(Cs) or len(valid) != len(X) or lptr[-1] != len(lpts):
+            raise ValueError("list_ptr needs one entry per camera + 1 and must end at len(list_pts); valid needs one flag per point")
+        cnt = np.zeros(nc, np.int32); med = np.zeros(nc, np.float32)
+        self._chk(self.L.l3d_median_depths(self.h, nc, _p(lptr), _p(lpts), C.c_longlong(len(X)), _p(X), _p(valid), _p(Cs), _p(cnt), _p(med), 0),
+                  "l3d_median_depths")
+        return cnt, med
+
     # ---- lens undistortion (stateless: no pipeline stage changes)
     def undistort(self, images, K, radial=(0, 0, 0), tangential=(0, 0), out=None):
         """Line3D::undistortImage for a list of uint8 HxW / HxWx3 images in ONE batched call.  K, radial, tangential: one camera for

@@ -78,6 +78,12 @@ struct UndistortState {
     DevBuf d_imgs, d_src, d_dst, d_map_xy, d_map_frac;   // d_src .. d_map_frac: host-mode staging
 };
 
+// buffers of the triangulation and median-depth calls (l3d_triangulate.cu): not a pipeline stage either; the d_* of host mode
+// stage the caller's arrays
+struct TriangulateState {
+    DevBuf d_ptr, d_cam, d_xy, d_P, d_X, d_valid, d_lptr, d_lpts, d_C, d_cnt, d_med, d_keys, d_keys2;
+};
+
 // The results a context holds, each computed from the ones before it:
 //   Views -> Matches -> Sweep -> Affinity,   Views -> Collinear -> Affinity
 enum class Stage { Views, Matches, Sweep, Collinear, Affinity };
@@ -116,6 +122,7 @@ struct l3d_ctx {
     CollinState collin;
     OptState opt;
     UndistortState undist;
+    TriangulateState tri;
 
     const float4* segs() const { return segs_ext ? segs_ext : (const float4*)d_segs.p; }
     const L3DViewDev* views() const { return (const L3DViewDev*)d_views.p; }

@@ -255,3 +255,69 @@ def segment_cache_path(output_folder, cam, width, height, max_img_width=-1):
     if n < 0:
         raise ValueError("path too long")
     return buf.value.decode()
+
+
+# ---- SfM models (include/line3d_io.h, csrc/line3d_io.cc + csrc/line3d_sfm.cc); host only except read_pix4d, which triangulates on a GPU
+def _sfm_cameras(L, h):
+    """the cameras of an l3dpp_sfm_* handle as dicts (id, image, K, R, t, C, radial, tangential, median_depth, worldpoints); closes it"""
+    p = lambda a: a.ctypes.data_as(C.c_void_p)
+    cams = []
+    try:
+        for i in range(L.l3dpp_sfm_num_cameras(h)):
+            head, K, R, t, Cc, dist = np.zeros(5), np.zeros(9), np.zeros(9), np.zeros(3), np.zeros(3), np.zeros(5)
+            name = C.create_string_buffer(4096)
+            L.l3dpp_sfm_camera(h, i, p(head), p(K), p(R), p(t), p(Cc), p(dist), name, 4096)
+            w = np.zeros(max(int(head[4]), 1), np.uint32)
+            L.l3dpp_sfm_worldpoints(h, i, p(w), int(head[4]))
+            cams.append(dict(id=int(head[0]), image=name.value.decode(errors="replace"), K=K.reshape(3, 3), R=R.reshape(3, 3), t=t, C=Cc,
+                             radial=dist[:3].copy(), tangential=dist[3:].copy(), median_depth=np.float32(head[3]), worldpoints=w[:int(head[4])]))
+    finally:
+        L.l3dpp_sfm_close(h)
+    return cams
+
+
+def _read_sfm(kind, path, aux="", device=0):
+    L = capi.lib()
+    L.l3dpp_sfm_read.restype = C.c_void_p
+    err = C.create_string_buffer(4096)
+    h = L.l3dpp_sfm_read(int(kind), str(path).encode(), str(aux).encode(), int(device), err, 4096)
+    if not h:
+        raise capi.L3DError(err.value.decode(errors="replace"))
+    return _sfm_cameras(L, C.c_void_p(h))
+
+
+def read_mavmap(path):
+    """readMavmap: the cameras of a mavmap result file (no world points; see sequential_neighbors).  Raises L3DError on malformed input."""
+    return _read_sfm(2, path)
+
+
+def read_openmvg(sfm_data_json):
+    """readOpenMVG: the cameras of an OpenMVG sfm_data.json with world-point lists and median depths"""
+    return _read_sfm(3, sfm_data_json)
+
+
+def read_pix4d(params_folder, project_prefix, device=0):
+    """readPix4D: the cameras of a Pix4D project; its tie points are triangulated on GPU `device` (L3DError without one)"""
+    return _read_sfm(4, params_folder, project_prefix, device)
+
+
+def sequential_neighbors(i, n_cams, num_neighbors):
+    """sequentialNeighbors: the mavmap frontend's neighbour list of camera i"""
+    out = np.zeros(max(int(num_neighbors), 1), np.uint32)
+    n = capi.lib().l3dpp_sequential_neighbors(C.c_uint(int(i)), C.c_uint(int(n_cams)), C.c_uint(int(num_neighbors)), _p(out), len(out))
+    return out[:n].tolist()
+
+
+def rotation_from_rpy(roll, pitch, yaw):
+    """Line3D::rotationFromRPY"""
+    R = np.zeros(9)
+    capi.lib().l3dpp_rotation_from_rpy(C.c_double(roll), C.c_double(pitch), C.c_double(yaw), _p(R))
+    return R.reshape(3, 3)
+
+
+def decompose_projection_matrix(P):
+    """Line3D::decomposeProjectionMatrix of a 3x4 P: (K, R, t)"""
+    P = np.ascontiguousarray(P, np.float64).reshape(12)
+    K, R, t = np.zeros(9), np.zeros(9), np.zeros(3)
+    capi.lib().l3dpp_decompose_projection(_p(P), _p(K), _p(R), _p(t))
+    return K.reshape(3, 3), R.reshape(3, 3), t
