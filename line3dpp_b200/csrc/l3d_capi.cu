@@ -58,10 +58,9 @@ int l3d_ctx_create(int device, l3d_ctx** out)
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, device);
     c->num_sms = prop.multiProcessorCount;
-    e = cudaFuncSetAttribute(k_match_topk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l3d_match_smem_bytes());
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_match_all, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l3d_match_smem_bytes());
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_match_topk_f64, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l3d_match_smem_bytes());
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_match_dense, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l3d_dense_smem_bytes());
+    for (const auto& by_keep : l3d_match_kernels)
+        for (auto k : by_keep)
+            if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l3d_match_smem_bytes());
     if (e != cudaSuccess) { cudaStreamDestroy(c->stream); delete c; return L3D_ERR_CUDA; }
     *out = c;
     return L3D_OK;
@@ -189,8 +188,201 @@ int l3d_match_pairs(l3d_ctx* c, int num_pairs, const int32_t* pairs, const float
 { return l3d_match_pairs_range(c, num_pairs, pairs, F, epi_overlap, knn, 0, num_pairs); }
 
 struct HostOut { int32_t* counts; l3d_match_rec* recs; int chunks; };
+// Checks the arguments, fills h_pairs and the tiles of the pairs [first_pair, last_pair), uploads both and sizes the result buffers.
+// *narcs: the number of level-1 table entries of the matched pairs.
+static int stage_pairs(l3d_ctx* c, int num_pairs, const int32_t* pairs, const float* F, const double* Fd, float epi_overlap, int knn,
+                       int first_pair, int last_pair, const HostOut* host, long long* narcs)
+{
+    if (host && (!host->counts || !host->recs || host->chunks < 1)) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs_host: bad arguments");
+    if (host && knn <= 0) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs_host: kNN <= 0 has no fixed row stride; use l3d_match_pairs + l3d_get_pair_matches");
+    if (!c->have_views) return l3d_fail(c, L3D_ERR_STATE, "l3d_match_pairs: call l3d_set_views first");
+    if (num_pairs < 0 || (num_pairs && (!pairs || (!F && !Fd)))) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs: bad arguments");
+    if (first_pair < 0 || last_pair < first_pair || last_pair > num_pairs) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs_range: bad pair range");
+    if (knn > 32 && host) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs_host: kNN > 32 has no fixed row stride; use l3d_match_pairs + l3d_get_pair_matches");
+    cudaSetDevice(c->device);
+    L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync before pair staging");   // h_pairs/h_tiles may still be in flight
+    c->h_pairs.resize(num_pairs);
+    c->h_tiles.clear();
+    long long rows = 0, evals = 0;
+    for (int i = 0; i < num_pairs; ++i) {
+        int s = pairs[2 * i], t = pairs[2 * i + 1];
+        if (s < 0 || t < 0 || s >= c->num_views || t >= c->num_views) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs: view index out of range");
+        L3DPairDev& p = c->h_pairs[i];
+        p.src = s; p.tgt = t; p.row_off = rows;
+        if (Fd) {     // REF_CPU: the double matrix decides; the float copy (eigen2dataArray-style cast) only feeds the conservative filter
+            memcpy(p.Fd, Fd + 9 * (size_t)i, sizeof(p.Fd));
+            for (int k = 0; k < 9; ++k) p.F[k] = (float)p.Fd[k];
+        } else { memcpy(p.F, F + 9 * (size_t)i, sizeof(p.F)); memset(p.Fd, 0, sizeof(p.Fd)); }
+        int Ns = c->h_views[s].nseg, Nt = c->h_views[t].nseg;
+        if (Nt >= (1 << 24)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: more than 2^24 segments in one view");
+        p.arc_off = *narcs;
+        if (i >= first_pair && i < last_pair) *narcs += Nt;
+        if (Nt > 0 && i >= first_pair && i < last_pair)
+            for (int r0 = 0; r0 < Ns; r0 += MK_ROWS) c->h_tiles.push_back(make_int2(i, r0));
+        rows += Ns;
+        if (i >= first_pair && i < last_pair) evals += (long long)Ns * Nt;     // evaluated HERE
+    }
+    c->num_pairs = num_pairs; c->knn = knn; c->epi = epi_overlap; c->total_rows = rows; c->pair_evals = evals;
+    int rc;
+    L3D_RESERVE(c->d_pairs, sizeof(L3DPairDev) * (size_t)std::max(num_pairs, 1), "pairs");
+    L3D_RESERVE(c->d_tiles, sizeof(int2) * std::max<size_t>(c->h_tiles.size(), 1), "tiles");
+    L3D_RESERVE(c->d_arcs, sizeof(uint4) * (size_t)std::max<long long>(*narcs, 1), "target arcs");
+    L3D_RESERVE(c->d_basis, sizeof(L3DPairBasis) * (size_t)std::max(num_pairs, 1), "pair bases");
+    L3D_RESERVE(c->d_counts, sizeof(int) * (size_t)std::max<long long>(rows, 1), "match counts");
+    if (knn > 0 && knn <= 32) L3D_RESERVE(c->d_recs, sizeof(l3d_match_rec) * (size_t)std::max<long long>(rows, 1) * knn, "match records");
+    if (num_pairs) L3D_CUDA(c, cudaMemcpyAsync(c->d_pairs.p, c->h_pairs.data(), sizeof(L3DPairDev) * num_pairs, cudaMemcpyHostToDevice, c->stream), "upload pairs");
+    if (!c->h_tiles.empty()) L3D_CUDA(c, cudaMemcpyAsync(c->d_tiles.p, c->h_tiles.data(), sizeof(int2) * c->h_tiles.size(), cudaMemcpyHostToDevice, c->stream), "upload tiles");
+    if (rows) L3D_CUDA(c, cudaMemsetAsync(c->d_counts.p, 0, sizeof(int) * rows, c->stream), "clear counts");   // rows of pairs with Nt == 0
+    return L3D_OK;
+}
+
+// Level-1 tables of the pairs matched here (l3d_device.cuh "pencil parameter"): raw arcs + keys, one sort, packed entries in window
+// order.  Below epi_overlap 0.01 the extended arcs would span the whole line: everything is then handed to the float filter.
+static int build_level1(l3d_ctx* c, int first_pair, int last_pair, long long narcs, float epi_overlap)
+{
+    if (last_pair <= first_pair || narcs <= 0) return L3D_OK;
+    if (narcs >= (1ll << 31) - 2) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: more than 2^31 (pair, target segment) combinations in one call");
+    const int npr = last_pair - first_pair;
+    const bool on = epi_overlap >= 0.01f && getenv("L3D_NO_LEVEL1") == nullptr;
+    int end_bit = 36;                       // key = pair << 36 | class << 32 | start of the arc
+    while (end_bit < 64 && (1ll << (end_bit - 36)) < npr) ++end_bit;
+    int rc;
+    L3D_RESERVE(c->d_arcraw, 16 * narcs, "raw arcs"); L3D_RESERVE(c->d_arckeys, 8 * narcs, "arc keys"); L3D_RESERVE(c->d_arckeys2, 8 * narcs, "arc keys");
+    L3D_RESERVE(c->d_arcvals, 4 * narcs, "arc order"); L3D_RESERVE(c->d_arcvals2, 4 * narcs, "arc order");
+    k_pair_arcs<<<(unsigned int)npr, 256, 0, c->stream>>>(c->segs(), c->views(), (const L3DPairDev*)c->d_pairs.p, first_pair, on ? 1 : 0,
+                                                         1.0 / (double)std::max(epi_overlap, 0.01f) + 0.5, (uint4*)c->d_arcraw.p,
+                                                         (unsigned long long*)c->d_arckeys.p, (unsigned int*)c->d_arcvals.p, (L3DPairBasis*)c->d_basis.p);
+    L3D_CUDA(c, cudaGetLastError(), "k_pair_arcs");
+    if ((rc = l3d_cub(c, "arc sort", [&](void* tmp, size_t& bytes) {
+             return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const unsigned long long*)c->d_arckeys.p, (unsigned long long*)c->d_arckeys2.p,
+                                                    (const unsigned int*)c->d_arcvals.p, (unsigned int*)c->d_arcvals2.p, (int)narcs, 0, end_bit, c->stream); }))) return rc;
+    k_arcs_gather<<<(unsigned int)((narcs + 255) / 256), 256, 0, c->stream>>>(narcs, (const unsigned long long*)c->d_arckeys2.p, (const unsigned int*)c->d_arcvals2.p,
+                                                                             (const uint4*)c->d_arcraw.p, (const L3DPairDev*)c->d_pairs.p, first_pair, (uint4*)c->d_arcs.p);
+    L3D_CUDA(c, cudaGetLastError(), "k_arcs_gather");
+    c->launches += 2 + 8;
+    return L3D_OK;
+}
+
+// matchingCPU's rays / plane normals in double (REF_CPU); the camera blocks may have been updated since set_views
+static int build_cache_d(l3d_ctx* c)
+{
+    if (c->total_segs == 0) return L3D_OK;
+    int rc;
+    L3D_RESERVE(c->d_cache_d, sizeof(double) * 9 * (size_t)c->total_segs, "double segment cache");
+    k_prep_segments_f64<<<(unsigned int)((c->total_segs + 255) / 256), 256, 0, c->stream>>>(c->segs(), c->views(), c->num_views, c->total_segs, (double*)c->d_cache_d.p);
+    ++c->launches;
+    L3D_CUDA(c, cudaGetLastError(), "k_prep_segments_f64");
+    return L3D_OK;
+}
+
+// one launch of k_match_topk<c->semantics, keep> over the tiles [t0, t1)
+static int launch_match(l3d_ctx* c, Keep keep, MatchArgs a, size_t t0, size_t t1, const char* what)
+{
+    a.tiles += t0;
+    void* args[] = {&a};
+    cudaLaunchKernel((const void*)l3d_match_kernels[c->semantics][(int)keep], dim3((unsigned int)(t1 - t0)), dim3(MK_THREADS), args, l3d_match_smem_bytes(), c->stream);
+    ++c->launches;
+    L3D_CUDA(c, cudaGetLastError(), what);
+    return L3D_OK;
+}
+
+// The kNN best matches of every row: one launch, or (l3d_match_pairs_host) `chunks` launches over contiguous tile ranges with the D2H
+// copy of every finished chunk's rows queued on a second stream, so that the PCIe transfer of chunk k hides behind the arithmetic of
+// chunk k+1.
+static int run_topk(l3d_ctx* c, const MatchArgs& a, const HostOut* host)
+{
+    const long long rows = c->total_rows, knn = a.knn;
+    const size_t ntiles = c->h_tiles.size();
+    const int chunks = host ? std::max(1, std::min<int>(host->chunks, (int)std::max<size_t>(ntiles, 1))) : 1;
+    int rc;
+    if (host) {
+        if (!c->copy_stream) L3D_CUDA(c, cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking), "copy stream");
+        while ((int)c->events.size() < chunks + 1) {
+            cudaEvent_t e; L3D_CUDA(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming), "event");
+            c->events.push_back(e);
+        }
+    }
+    auto row_of_tile = [&](size_t t) { return t >= ntiles ? rows : c->h_pairs[c->h_tiles[t].x].row_off + c->h_tiles[t].y; };
+    long long row_done = 0;
+    for (int k = 0; k < chunks; ++k) {
+        const size_t t0 = ntiles * (size_t)k / chunks, t1 = ntiles * (size_t)(k + 1) / chunks;
+        if (t1 > t0 && (rc = launch_match(c, Keep::TopK, a, t0, t1, "k_match_topk"))) return rc;
+        if (host) {
+            const long long r1 = k == chunks - 1 ? rows : row_of_tile(t1);      // rows [row_done, r1) are final after this launch
+            if (r1 > row_done) {
+                L3D_CUDA(c, cudaEventRecord(c->events[k], c->stream), "event record");
+                L3D_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->events[k], 0), "event wait");
+                L3D_CUDA(c, cudaMemcpyAsync(host->counts + row_done, (const int*)c->d_counts.p + row_done, sizeof(int) * (size_t)(r1 - row_done), cudaMemcpyDeviceToHost, c->copy_stream), "download counts");
+                L3D_CUDA(c, cudaMemcpyAsync(host->recs + row_done * knn, (const l3d_match_rec*)c->d_recs.p + row_done * knn,
+                                            sizeof(l3d_match_rec) * (size_t)(r1 - row_done) * knn, cudaMemcpyDeviceToHost, c->copy_stream), "download records");
+                row_done = r1;
+            }
+        }
+    }
+    if (host) {     // the context's stream (the one callers time and synchronise) completes only after the last copy
+        L3D_CUDA(c, cudaEventRecord(c->events[chunks], c->copy_stream), "event record");
+        L3D_CUDA(c, cudaStreamWaitEvent(c->stream, c->events[chunks], 0), "event wait");
+    }
+    return L3D_OK;
+}
+
+// "Keep all matches" (kNN <= 0, cudawrapper.cu:628-636, line3D.cc:988-996): count pass -> row stride = largest row -> store pass ->
+// rows sorted.  big_k > 0 (kNN > 32 exceeds the fused kernel's per-row key list): the same passes, and every row is cut to its big_k
+// best afterwards (same matches as the reference's priority queue, line3D.cc:999-1006 / cudawrapper.cu:637-645).
+static int run_keep_all(l3d_ctx* c, MatchArgs a, int big_k)
+{
+    const long long rows = c->total_rows;
+    const size_t ntiles = c->h_tiles.size();
+    int rc, stride = 1;
+    if (ntiles) {
+        a.knn = 0; a.recs = nullptr;
+        if ((rc = launch_match(c, Keep::Count, a, 0, ntiles, "k_match_topk (count)"))) return rc;
+        if (rows > INT_MAX) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: more than 2^31 rows with kNN <= 0");
+        L3D_RESERVE(c->d_rowptr, 16, "row max");
+        int* d_max = (int*)c->d_rowptr.p;
+        if ((rc = l3d_cub(c, "row maximum", [&](void* tmp, size_t& bytes) {
+                 return cub::DeviceReduce::Max(tmp, bytes, (const int*)c->d_counts.p, d_max, (int)rows, c->stream); }))) return rc;
+        c->launches += 1;
+        L3D_CUDA(c, cudaMemcpyAsync(&stride, d_max, sizeof(int), cudaMemcpyDeviceToHost, c->stream), "row maximum");
+        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync");
+        stride = std::max(stride, 1);
+    }
+    c->knn = stride;
+    L3D_RESERVE(c->d_recs, sizeof(l3d_match_rec) * (size_t)std::max<long long>(rows, 1) * stride, "match records");
+    if (ntiles) {
+        const size_t per_warp = sizeof(l3d_match_rec) * (size_t)stride;
+        int wpb = 4;
+        while (wpb > 1 && per_warp * wpb > 200 * 1024) wpb >>= 1;
+        if (per_warp * wpb > 200 * 1024) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: a row with more than 8500 matches (kNN <= 0)");
+        a.knn = stride; a.recs = (l3d_match_rec*)c->d_recs.p;
+        if ((rc = launch_match(c, Keep::Store, a, 0, ntiles, "k_match_topk (store)"))) return rc;
+        L3D_CUDA(c, cudaFuncSetAttribute(k_sort_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(per_warp * wpb)), "k_sort_rows smem");
+        const long long blocks = std::min<long long>((rows + wpb - 1) / wpb, (long long)c->num_sms * 16);
+        k_sort_rows<<<(unsigned int)blocks, wpb * 32, per_warp * wpb, c->stream>>>((int*)c->d_counts.p, (l3d_match_rec*)c->d_recs.p, stride, rows, big_k);
+        L3D_CUDA(c, cudaGetLastError(), "k_sort_rows");
+        ++c->launches;
+    }
+    return L3D_OK;
+}
+
 static int match_impl(l3d_ctx* c, int num_pairs, const int32_t* pairs, const float* F, const double* Fd, float epi_overlap, int knn, int first_pair, int last_pair,
-                      const HostOut* host = nullptr);
+                      const HostOut* host = nullptr)
+{
+    if (!c) return L3D_ERR_INVALID;
+    c->drop(Stage::Matches);
+    int rc;
+    long long narcs = 0;
+    if ((rc = stage_pairs(c, num_pairs, pairs, F, Fd, epi_overlap, knn, first_pair, last_pair, host, &narcs))) return rc;
+    if ((rc = build_level1(c, first_pair, last_pair, narcs, epi_overlap))) return rc;
+    if (Fd && (rc = build_cache_d(c))) return rc;
+    c->semantics = Fd ? L3D_SEM_REF_CPU : L3D_SEM_REF_GPU;
+    const MatchArgs a = {c->segs(), (const float4*)c->d_cache.p, Fd ? (const double*)c->d_cache_d.p : nullptr, c->views(), (const L3DPairDev*)c->d_pairs.p,
+                         (const int2*)c->d_tiles.p, (const uint4*)c->d_arcs.p, (const L3DPairBasis*)c->d_basis.p, (int*)c->d_counts.p,
+                         (l3d_match_rec*)c->d_recs.p, knn, epi_overlap};
+    if ((rc = knn > 0 && knn <= 32 ? run_topk(c, a, host) : run_keep_all(c, a, knn > 32 ? knn : 0))) return rc;
+    c->have_matches = true;
+    return L3D_OK;
+}
 
 int l3d_match_pairs_range(l3d_ctx* c, int num_pairs, const int32_t* pairs, const float* F, float epi_overlap, int knn, int first_pair, int last_pair)
 { return match_impl(c, num_pairs, pairs, F, nullptr, epi_overlap, knn, first_pair, last_pair); }
@@ -203,173 +395,6 @@ int l3d_match_pairs_host(l3d_ctx* c, int num_pairs, const int32_t* pairs, const 
 {
     HostOut h = {counts_out, recs_out, std::min(chunks, 64)};
     return match_impl(c, num_pairs, pairs, F, nullptr, epi_overlap, knn, 0, num_pairs, &h);
-}
-
-static int match_impl(l3d_ctx* c, int num_pairs, const int32_t* pairs, const float* F, const double* Fd, float epi_overlap, int knn, int first_pair, int last_pair,
-                      const HostOut* host)
-{
-    if (!c) return L3D_ERR_INVALID;
-    c->drop(Stage::Matches);
-    if (host && (!host->counts || !host->recs || host->chunks < 1)) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs_host: bad arguments");
-    if (host && knn <= 0) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs_host: kNN <= 0 has no fixed row stride; use l3d_match_pairs + l3d_get_pair_matches");
-    if (!c->have_views) return l3d_fail(c, L3D_ERR_STATE, "l3d_match_pairs: call l3d_set_views first");
-    if (num_pairs < 0 || (num_pairs && (!pairs || (!F && !Fd)))) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs: bad arguments");
-    if (first_pair < 0 || last_pair < first_pair || last_pair > num_pairs) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs_range: bad pair range");
-    // kNN > 32 exceeds the fused kernel's per-row key list: the keep-all passes run instead and every row is cut to its kNN best
-    // afterwards (same matches as the reference's priority queue, line3D.cc:999-1006 / cudawrapper.cu:637-645)
-    const int big_k = knn > 32 ? knn : 0;
-    const bool keep_all = knn <= 0 || big_k > 0;
-    if (big_k && host) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs_host: kNN > 32 has no fixed row stride; use l3d_match_pairs + l3d_get_pair_matches");
-    cudaSetDevice(c->device);
-    L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync before pair staging");   // h_pairs/h_tiles may still be in flight
-    c->h_pairs.resize(num_pairs);
-    c->h_tiles.clear();
-    long long rows = 0, evals = 0, narcs = 0;
-    for (int i = 0; i < num_pairs; ++i) {
-        int s = pairs[2 * i], t = pairs[2 * i + 1];
-        if (s < 0 || t < 0 || s >= c->num_views || t >= c->num_views) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs: view index out of range");
-        L3DPairDev& p = c->h_pairs[i];
-        p.src = s; p.tgt = t; p.row_off = rows;
-        if (Fd) {     // REF_CPU: the double matrix decides; the float copy (eigen2dataArray-style cast) only feeds the conservative filter
-            memcpy(p.Fd, Fd + 9 * (size_t)i, sizeof(p.Fd));
-            for (int k = 0; k < 9; ++k) p.F[k] = (float)p.Fd[k];
-        } else { memcpy(p.F, F + 9 * (size_t)i, sizeof(p.F)); memset(p.Fd, 0, sizeof(p.Fd)); }
-        int Ns = c->h_views[s].nseg, Nt = c->h_views[t].nseg;
-        if (Nt >= (1 << 24)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: more than 2^24 segments in one view");
-        p.arc_off = narcs;
-        if (i >= first_pair && i < last_pair) narcs += Nt;
-        if (Nt > 0 && i >= first_pair && i < last_pair)
-            for (int r0 = 0; r0 < Ns; r0 += MK_ROWS) c->h_tiles.push_back(make_int2(i, r0));
-        rows += Ns;
-        if (i >= first_pair && i < last_pair) evals += (long long)Ns * Nt;     // evaluated HERE
-    }
-    c->num_pairs = num_pairs; c->knn = knn; c->epi = epi_overlap; c->total_rows = rows; c->pair_evals = evals;
-    int rc;
-    L3D_RESERVE(c->d_pairs, sizeof(L3DPairDev) * (size_t)std::max(num_pairs, 1), "pairs");
-    L3D_RESERVE(c->d_tiles, sizeof(int2) * std::max<size_t>(c->h_tiles.size(), 1), "tiles");
-    L3D_RESERVE(c->d_arcs, sizeof(uint4) * (size_t)std::max<long long>(narcs, 1), "target arcs");
-    L3D_RESERVE(c->d_basis, sizeof(L3DPairBasis) * (size_t)std::max(num_pairs, 1), "pair bases");
-    L3D_RESERVE(c->d_counts, sizeof(int) * (size_t)std::max<long long>(rows, 1), "match counts");
-    if (!keep_all) L3D_RESERVE(c->d_recs, sizeof(l3d_match_rec) * (size_t)std::max<long long>(rows, 1) * knn, "match records");
-    if (num_pairs) L3D_CUDA(c, cudaMemcpyAsync(c->d_pairs.p, c->h_pairs.data(), sizeof(L3DPairDev) * num_pairs, cudaMemcpyHostToDevice, c->stream), "upload pairs");
-    if (!c->h_tiles.empty()) L3D_CUDA(c, cudaMemcpyAsync(c->d_tiles.p, c->h_tiles.data(), sizeof(int2) * c->h_tiles.size(), cudaMemcpyHostToDevice, c->stream), "upload tiles");
-    if (rows) L3D_CUDA(c, cudaMemsetAsync(c->d_counts.p, 0, sizeof(int) * rows, c->stream), "clear counts");   // rows of pairs with Nt == 0
-    const uint4* arcs = (const uint4*)c->d_arcs.p;
-    const L3DPairBasis* basis = (const L3DPairBasis*)c->d_basis.p;
-    if (last_pair > first_pair && narcs > 0) {
-        // level-1 tables of the pairs matched here (l3d_device.cuh "pencil parameter"): raw arcs + keys, one sort, packed entries in window
-        // order.  Below epi_overlap 0.01 the extended arcs would span the whole line: everything is then handed to the float filter.
-        if (narcs >= (1ll << 31) - 2) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: more than 2^31 (pair, target segment) combinations in one call");
-        const int npr = last_pair - first_pair;
-        const bool on = epi_overlap >= 0.01f && getenv("L3D_NO_LEVEL1") == nullptr;
-        int end_bit = 36;                       // key = pair << 36 | class << 32 | start of the arc
-        while (end_bit < 64 && (1ll << (end_bit - 36)) < npr) ++end_bit;
-        L3D_RESERVE(c->d_arcraw, 16 * narcs, "raw arcs"); L3D_RESERVE(c->d_arckeys, 8 * narcs, "arc keys"); L3D_RESERVE(c->d_arckeys2, 8 * narcs, "arc keys");
-        L3D_RESERVE(c->d_arcvals, 4 * narcs, "arc order"); L3D_RESERVE(c->d_arcvals2, 4 * narcs, "arc order");
-        k_pair_arcs<<<(unsigned int)npr, 256, 0, c->stream>>>(c->segs(), c->views(), (const L3DPairDev*)c->d_pairs.p, first_pair, on ? 1 : 0,
-                                                             1.0 / (double)std::max(epi_overlap, 0.01f) + 0.5, (uint4*)c->d_arcraw.p,
-                                                             (unsigned long long*)c->d_arckeys.p, (unsigned int*)c->d_arcvals.p, (L3DPairBasis*)c->d_basis.p);
-        L3D_CUDA(c, cudaGetLastError(), "k_pair_arcs");
-        if ((rc = l3d_cub(c, "arc sort", [&](void* tmp, size_t& bytes) {
-                 return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const unsigned long long*)c->d_arckeys.p, (unsigned long long*)c->d_arckeys2.p,
-                                                        (const unsigned int*)c->d_arcvals.p, (unsigned int*)c->d_arcvals2.p, (int)narcs, 0, end_bit, c->stream); }))) return rc;
-        k_arcs_gather<<<(unsigned int)((narcs + 255) / 256), 256, 0, c->stream>>>(narcs, (const unsigned long long*)c->d_arckeys2.p, (const unsigned int*)c->d_arcvals2.p,
-                                                                                 (const uint4*)c->d_arcraw.p, (const L3DPairDev*)c->d_pairs.p, first_pair, (uint4*)c->d_arcs.p);
-        L3D_CUDA(c, cudaGetLastError(), "k_arcs_gather");
-        c->launches += 2 + 8;
-    }
-    const double* cache_d = nullptr;
-    if (Fd && c->total_segs > 0) {      // matchingCPU's rays / plane normals in double; camera blocks may have been updated since set_views
-        L3D_RESERVE(c->d_cache_d, sizeof(double) * 9 * (size_t)c->total_segs, "double segment cache");
-        k_prep_segments_f64<<<(unsigned int)((c->total_segs + 255) / 256), 256, 0, c->stream>>>(c->segs(), c->views(), c->num_views, c->total_segs, (double*)c->d_cache_d.p);
-        ++c->launches;
-        L3D_CUDA(c, cudaGetLastError(), "k_prep_segments_f64");
-        cache_d = (const double*)c->d_cache_d.p;
-    }
-    c->semantics = Fd ? L3D_SEM_REF_CPU : L3D_SEM_REF_GPU;
-    if (keep_all) {
-        // "keep all matches" (cudawrapper.cu:628-636, line3D.cc:988-996): count pass -> row stride = largest row -> store pass -> sort rows
-        int stride = 1;
-        if (!c->h_tiles.empty()) {
-            k_match_all<<<(unsigned int)c->h_tiles.size(), MK_THREADS, l3d_match_smem_bytes(), c->stream>>>(
-                c->segs(), (const float4*)c->d_cache.p, c->views(), (const L3DPairDev*)c->d_pairs.p, (const int2*)c->d_tiles.p, 0,
-                epi_overlap, (int*)c->d_counts.p, nullptr, cache_d, arcs, basis);
-            ++c->launches;
-            L3D_CUDA(c, cudaGetLastError(), "k_match_all (count)");
-            if (rows > INT_MAX) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: more than 2^31 rows with kNN <= 0");
-            L3D_RESERVE(c->d_rowptr, 16, "row max");
-            int* d_max = (int*)c->d_rowptr.p;
-            if ((rc = l3d_cub(c, "row maximum", [&](void* tmp, size_t& bytes) {
-                     return cub::DeviceReduce::Max(tmp, bytes, (const int*)c->d_counts.p, d_max, (int)rows, c->stream); }))) return rc;
-            c->launches += 1;
-            L3D_CUDA(c, cudaMemcpyAsync(&stride, d_max, sizeof(int), cudaMemcpyDeviceToHost, c->stream), "row maximum");
-            L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync");
-            stride = std::max(stride, 1);
-        }
-        knn = stride; c->knn = stride;
-        L3D_RESERVE(c->d_recs, sizeof(l3d_match_rec) * (size_t)std::max<long long>(rows, 1) * stride, "match records");
-        if (!c->h_tiles.empty()) {
-            const size_t per_warp = sizeof(l3d_match_rec) * (size_t)stride;
-            int wpb = 4;
-            while (wpb > 1 && per_warp * wpb > 200 * 1024) wpb >>= 1;
-            if (per_warp * wpb > 200 * 1024) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: a row with more than 8500 matches (kNN <= 0)");
-            k_match_all<<<(unsigned int)c->h_tiles.size(), MK_THREADS, l3d_match_smem_bytes(), c->stream>>>(
-                c->segs(), (const float4*)c->d_cache.p, c->views(), (const L3DPairDev*)c->d_pairs.p, (const int2*)c->d_tiles.p, stride,
-                epi_overlap, (int*)c->d_counts.p, (l3d_match_rec*)c->d_recs.p, cache_d, arcs, basis);
-            L3D_CUDA(c, cudaGetLastError(), "k_match_all (store)");
-            L3D_CUDA(c, cudaFuncSetAttribute(k_sort_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(per_warp * wpb)), "k_sort_rows smem");
-            const long long blocks = std::min<long long>((rows + wpb - 1) / wpb, (long long)c->num_sms * 16);
-            k_sort_rows<<<(unsigned int)blocks, wpb * 32, per_warp * wpb, c->stream>>>((int*)c->d_counts.p, (l3d_match_rec*)c->d_recs.p, stride, rows, big_k);
-            L3D_CUDA(c, cudaGetLastError(), "k_sort_rows");
-            c->launches += 2;
-        }
-    } else {
-        // One launch, or (l3d_match_pairs_host) `chunks` launches over contiguous tile ranges with the D2H copy of every finished
-        // chunk's rows queued on a second stream, so that the PCIe transfer of chunk k hides behind the arithmetic of chunk k+1.
-        const size_t ntiles = c->h_tiles.size();
-        const int chunks = host ? std::max(1, std::min<int>(host->chunks, (int)std::max<size_t>(ntiles, 1))) : 1;
-        if (host) {
-            if (!c->copy_stream) L3D_CUDA(c, cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking), "copy stream");
-            while ((int)c->events.size() < chunks + 1) {
-                cudaEvent_t e; L3D_CUDA(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming), "event");
-                c->events.push_back(e);
-            }
-        }
-        auto row_of_tile = [&](size_t t) { return t >= ntiles ? rows : c->h_pairs[c->h_tiles[t].x].row_off + c->h_tiles[t].y; };
-        long long row_done = 0;
-        for (int k = 0; k < chunks; ++k) {
-            const size_t t0 = ntiles * (size_t)k / chunks, t1 = ntiles * (size_t)(k + 1) / chunks;
-            if (t1 > t0) {
-                if (cache_d)
-                    k_match_topk_f64<<<(unsigned int)(t1 - t0), MK_THREADS, l3d_match_smem_bytes(), c->stream>>>(
-                        c->segs(), (const float4*)c->d_cache.p, c->views(), (const L3DPairDev*)c->d_pairs.p, (const int2*)c->d_tiles.p + t0, knn,
-                        epi_overlap, (int*)c->d_counts.p, (l3d_match_rec*)c->d_recs.p, cache_d, arcs, basis);
-                else
-                    k_match_topk<<<(unsigned int)(t1 - t0), MK_THREADS, l3d_match_smem_bytes(), c->stream>>>(
-                        c->segs(), (const float4*)c->d_cache.p, c->views(), (const L3DPairDev*)c->d_pairs.p, (const int2*)c->d_tiles.p + t0, knn,
-                        epi_overlap, (int*)c->d_counts.p, (l3d_match_rec*)c->d_recs.p, arcs, basis);
-                ++c->launches;
-                L3D_CUDA(c, cudaGetLastError(), "k_match_topk");
-            }
-            if (host) {
-                const long long r1 = k == chunks - 1 ? rows : row_of_tile(t1);      // rows [row_done, r1) are final after this launch
-                if (r1 > row_done) {
-                    L3D_CUDA(c, cudaEventRecord(c->events[k], c->stream), "event record");
-                    L3D_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->events[k], 0), "event wait");
-                    L3D_CUDA(c, cudaMemcpyAsync(host->counts + row_done, (const int*)c->d_counts.p + row_done, sizeof(int) * (size_t)(r1 - row_done), cudaMemcpyDeviceToHost, c->copy_stream), "download counts");
-                    L3D_CUDA(c, cudaMemcpyAsync(host->recs + row_done * knn, (const l3d_match_rec*)c->d_recs.p + row_done * knn,
-                                                sizeof(l3d_match_rec) * (size_t)(r1 - row_done) * knn, cudaMemcpyDeviceToHost, c->copy_stream), "download records");
-                    row_done = r1;
-                }
-            }
-        }
-        if (host) {     // the context's stream (the one callers time and synchronise) completes only after the last copy
-            L3D_CUDA(c, cudaEventRecord(c->events[chunks], c->copy_stream), "event record");
-            L3D_CUDA(c, cudaStreamWaitEvent(c->stream, c->events[chunks], 0), "event wait");
-        }
-    }
-    c->have_matches = true;
-    return L3D_OK;
 }
 
 int l3d_match_device_buffers(l3d_ctx* c, void** counts_dev, void** recs_dev)
@@ -498,6 +523,18 @@ long long l3d_get_matches_csr(l3d_ctx* c, int64_t* row_ptr_out, l3d_match_rec* r
 }
 
 // ------------------------------------------------------------------------------------------------ dense contract
+// view pair (sv, tv) of the dense contract: its segments and cached rays, F (row-major, 9 floats), the camera centres and the outputs
+static L3DDenseJob dense_job(const l3d_ctx* c, int sv, int tv, const float* F, float4* depths, float* overlaps, int rows_per_cta)
+{
+    const L3DViewDev& vs = c->h_views[sv]; const L3DViewDev& vt = c->h_views[tv];
+    const float4* cache = (const float4*)c->d_cache.p;
+    L3DDenseJob J = {c->segs() + vs.seg_off, c->segs() + vt.seg_off, cache + 3 * vs.seg_off, cache + 3 * vt.seg_off, depths, overlaps, {},
+                     make_float3(vs.C[0], vs.C[1], vs.C[2]), make_float3(vt.C[0], vt.C[1], vt.C[2]), vs.nseg, vt.nseg, rows_per_cta,
+                     (vt.nseg + DK_WARPS * DK_T * 32 - 1) / (DK_WARPS * DK_T * 32), 0};
+    memcpy(J.F.m, F, sizeof(J.F.m));
+    return J;
+}
+
 static int match_dense_impl(l3d_ctx* c, int sv, int tv, const float* F, float epi, float* depths, float* overlaps, int on_dev, bool filter)
 {
     if (!c) return L3D_ERR_INVALID;
@@ -515,17 +552,11 @@ static int match_dense_impl(l3d_ctx* c, int sv, int tv, const float* F, float ep
         L3D_RESERVE(c->d_dense_ov, sizeof(float) * cells, "dense overlaps");
         d_dep = (float4*)c->d_dense_dep.p; d_ov = (float*)c->d_dense_ov.p;
     }
-    L3DMat3 Fm; memcpy(Fm.m, F, sizeof(Fm.m));
-    dim3 grid((Nt + DK_THREADS - 1) / DK_THREADS, (Ns + DKN_ROWS - 1) / DKN_ROWS);
-    const int R = l3d_dense_rows_per_cta(Ns, Nt, c->num_sms);
-    dim3 gridf((Nt + DK_WARPS * DK_T * 32 - 1) / (DK_WARPS * DK_T * 32), (Ns + R - 1) / R);
-    const float4* cache = (const float4*)c->d_cache.p;
+    const L3DDenseJob J = dense_job(c, sv, tv, F, d_dep, d_ov, l3d_dense_rows_per_cta(Ns, Nt, c->num_sms));
     if (filter)
-        k_match_dense<<<gridf, DK_THREADS, l3d_dense_smem_bytes(), c->stream>>>(c->segs() + vs.seg_off, Ns, c->segs() + vt.seg_off, Nt, cache + 3 * vs.seg_off, cache + 3 * vt.seg_off, Fm,
-                                                          make_float3(vs.C[0], vs.C[1], vs.C[2]), make_float3(vt.C[0], vt.C[1], vt.C[2]), epi, d_dep, d_ov, R);
+        k_match_dense<<<dim3(J.colb, (Ns + J.rows_per_cta - 1) / J.rows_per_cta), DK_THREADS, l3d_dense_smem_bytes(), c->stream>>>(J, epi);
     else
-        k_match_dense_nofilter<<<grid, DK_THREADS, 0, c->stream>>>(c->segs() + vs.seg_off, Ns, c->segs() + vt.seg_off, Nt, cache + 3 * vs.seg_off, cache + 3 * vt.seg_off, Fm,
-                                                                   make_float3(vs.C[0], vs.C[1], vs.C[2]), make_float3(vt.C[0], vt.C[1], vt.C[2]), epi, d_dep, d_ov);
+        k_match_dense_nofilter<<<dim3((Nt + DK_THREADS - 1) / DK_THREADS, (Ns + DKN_ROWS - 1) / DKN_ROWS), DK_THREADS, 0, c->stream>>>(J, epi);
     ++c->launches;
     L3D_CUDA(c, cudaGetLastError(), "k_match_dense");
     if (!on_dev) {
@@ -572,22 +603,15 @@ int l3d_match_dense_pairs(l3d_ctx* c, int npairs, const int32_t* pairs, const fl
     if (npairs == 0) return L3D_OK;
     cudaSetDevice(c->device);
     std::vector<L3DDenseJob> jobs;
-    const float4* cache = (const float4*)c->d_cache.p;
     long long tiles = 0;
     for (int i = 0; i < npairs; ++i) {
         const int sv = pairs[2 * i], tv = pairs[2 * i + 1];
         if (sv < 0 || tv < 0 || sv >= c->num_views || tv >= c->num_views || !depths_dev[i] || !overlaps_dev[i]) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_dense_pairs: bad pair");
-        const L3DViewDev& vs = c->h_views[sv]; const L3DViewDev& vt = c->h_views[tv];
-        if (vs.nseg == 0 || vt.nseg == 0) continue;
-        L3DDenseJob J;
-        J.ssegs = c->segs() + vs.seg_off; J.tsegs = c->segs() + vt.seg_off; J.scache = cache + 3 * vs.seg_off; J.tcache = cache + 3 * vt.seg_off;
-        J.depths = (float4*)depths_dev[i]; J.overlaps = overlaps_dev[i];
-        memcpy(J.F.m, F + 9 * (size_t)i, sizeof(J.F.m));
-        J.Cs = make_float3(vs.C[0], vs.C[1], vs.C[2]); J.Ct = make_float3(vt.C[0], vt.C[1], vt.C[2]);
-        J.Ns = vs.nseg; J.Nt = vt.nseg; J.rows_per_cta = DK_ROWS;       // whole waves do not matter inside a batch: the tallest tile amortises the per-tile set-up best
-        J.colb = (vt.nseg + DK_WARPS * DK_T * 32 - 1) / (DK_WARPS * DK_T * 32);
+        if (c->h_views[sv].nseg == 0 || c->h_views[tv].nseg == 0) continue;
+        // whole waves do not matter inside a batch: the tallest tile amortises the per-tile set-up best
+        L3DDenseJob J = dense_job(c, sv, tv, F + 9 * (size_t)i, (float4*)depths_dev[i], overlaps_dev[i], DK_ROWS);
         J.tile0 = tiles;
-        tiles += (long long)J.colb * ((vs.nseg + DK_ROWS - 1) / DK_ROWS);
+        tiles += (long long)J.colb * ((J.Ns + DK_ROWS - 1) / DK_ROWS);
         jobs.push_back(J);
     }
     if (jobs.empty()) return L3D_OK;

@@ -13,7 +13,8 @@
 //                     evaluates those 32 at a time with the exact, reference-order arithmetic; per-row survivor keys live in shared
 //                     memory and the k best are selected and written once.  Replaces K_match_lines + the dense D2H + host
 //                     priority-queue pass (cudawrapper.cu:186-253, 570-650).  Instruction-issue / latency bound; compulsory HBM
-//                     traffic ~0.1 B/pair-eval.
+//                     traffic ~0.1 B/pair-eval.  One instantiation per semantics (REF_GPU / REF_CPU exact arithmetic) and keep
+//                     policy (top-k, or the count and store passes of "keep all matches").
 //   k_match_dense   : the reference's device contract (float4 depths + float overlap for EVERY cell,
 //                     cudawrapper.cu:186-253), same filter + exact path, coalesced 20 B/cell writes: HBM-write bound.
 #include "l3d_match.cuh"
@@ -69,7 +70,7 @@ struct MatchSmem {
     float3 Cs, Ct;
     float epi; int knn, Nt;
     int cap;                                         // keys a row list collects before it is cut to its k best (and the score-to-beat rises); 16 instead of 32 was measured 7 % slower
-    // REF_CPU semantics (k_match_topk_f64): the exact path is matchingCPU's double arithmetic; the float filter stays the same
+    // REF_CPU semantics only: the exact path is matchingCPU's double arithmetic; the float filter stays the same
     const double* cache_d; const float4* ssegs;
     double Fd[9]; D3 Csd, Ctd;
     // keep-all modes (kNN <= 0, cudawrapper.cu:628-636): output row base / record array; knn then holds the row stride
@@ -120,34 +121,54 @@ __device__ __noinline__ void prune_row(MatchSmem& S, int row, int lane)
     __syncwarp();
 }
 
-// matchingCPU's evaluation of one candidate (line3D.cc:925-1003): double overlap, double depths > 1e-12
-__device__ __noinline__ bool eval_candidate_f64(const MatchSmem& S, int rl, unsigned int j, float* ov_out, float* dep)
+// depths (d_p1, d_p2, d_q1, d_q2) of target j for row rl, stored as Match stores them (floats, commons.h:186-203); true when all
+// four are in front of the cameras: > 0 in float (REF_GPU, cudawrapper.cu:186-253) or > 1e-12 in double (REF_CPU, line3D.cc:925-1003)
+template <int SEM>
+__device__ __forceinline__ bool target_depths(const MatchSmem& S, int rl, unsigned int j, float* d)
 {
+    if (SEM == L3D_SEM_REF_CPU) {
+        const SegRaysD s = load_rays_d(S.cache_d, S.src_base + rl), t = load_rays_d(S.cache_d, S.toff + j);
+        double dd[4];
+        exact_depths_f64(s, t, S.Csd, S.Ctd, dd);
+        d[0] = (float)dd[0]; d[1] = (float)dd[1]; d[2] = (float)dd[2]; d[3] = (float)dd[3];
+        return dd[0] > L3D_EPS_D && dd[1] > L3D_EPS_D && dd[2] > L3D_EPS_D && dd[3] > L3D_EPS_D;
+    }
+    const SegRays s = load_rays(S.cache, S.src_base + rl), t = load_rays(S.cache, S.toff + j);
+    exact_depths(s, t, S.Cs, S.Ct, d);
+    return d[0] > 0.0f && d[1] > 0.0f && d[2] > 0.0f && d[3] > 0.0f;
+}
+
+// exact evaluation of candidate j for row rl (has == false: padding lane, never a match): the overlap must exceed epi and reach
+// the row's current k-th best (below it the candidate can never be selected), and the depths must be positive (target_depths).
+// REF_GPU: K_match_lines' float overlap with the row's cached epipolar lines, inline (the lanes stay converged through it);
+// REF_CPU: matchingCPU's double overlap (line3D.cc:925-1003) with epipolar lines from the double F, out of line.
+template <int SEM> __device__ bool eval_candidate(const MatchSmem& S, int rl, unsigned int j, bool has, float* ov, float* d);
+template <> __device__ __forceinline__ bool eval_candidate<L3D_SEM_REF_GPU>(const MatchSmem& S, int rl, unsigned int j, bool has, float* ov, float* d)
+{
+    const float4 rA = S.rowA[rl], rB = S.rowB[rl];
+    bool inv;
+    *ov = exact_overlap(__ldg(S.tsegs + j), make_float3(rA.x, rA.y, rA.z), make_float3(rA.w, rB.x, rB.y), &inv);
+    return has && *ov > S.epi && *ov >= S.row_thr[rl] && target_depths<L3D_SEM_REF_GPU>(S, rl, j, d);
+}
+template <> __device__ __noinline__ bool eval_candidate<L3D_SEM_REF_CPU>(const MatchSmem& S, int rl, unsigned int j, bool has, float* ov, float* d)
+{
+    if (!has) return false;
     const float4 sp = __ldg(S.ssegs + rl);
     const D3 e1 = dmulmat(S.Fd, d3((double)sp.x, (double)sp.y, 1.0)), e2 = dmulmat(S.Fd, d3((double)sp.z, (double)sp.w, 1.0));
     bool valid;
-    const float ov = exact_overlap_f64(__ldg(S.tsegs + j), e1, e2, &valid);
-    if (!(valid && ov > S.epi && ov >= S.row_thr[rl])) return false;
-    const SegRaysD s = load_rays_d(S.cache_d, S.src_base + rl), t = load_rays_d(S.cache_d, S.toff + j);
-    double d[4];
-    exact_depths_f64(s, t, S.Csd, S.Ctd, d);
-    if (!(d[0] > L3D_EPS_D && d[1] > L3D_EPS_D && d[2] > L3D_EPS_D && d[3] > L3D_EPS_D)) return false;
-    *ov_out = ov;
-    dep[0] = (float)d[0]; dep[1] = (float)d[1]; dep[2] = (float)d[2]; dep[3] = (float)d[3];     // Match stores floats (commons.h:186-203)
-    return true;
+    *ov = exact_overlap_f64(__ldg(S.tsegs + j), e1, e2, &valid);
+    return valid && *ov > S.epi && *ov >= S.row_thr[rl] && target_depths<L3D_SEM_REF_CPU>(S, rl, j, d);
 }
 
 // exact evaluation of up to 32 queued candidates (one per lane).  Out of line on purpose: the hot filter loop must
 // stay inside the instruction cache (the first version inlined this 5x -> 64 KB of SASS, 55 % "no instruction" stalls).
-// KEEP: 0 = keep the kNN best per row; 1 = only count the survivors of every row; 2 = store every survivor (row stride
-// S.knn, slot = arrival order; k_sort_rows puts the rows into the reference's ascending-target order afterwards)
-template <int MODE, int KEEP>
+// A match is kept per KEEP: TopK pushes its key into the row list (cut to the kNN best when full), Count only counts it,
+// Store writes its record (row stride S.knn, slot = arrival order; k_sort_rows puts the rows into the reference's
+// ascending-target order afterwards).
+template <int SEM, Keep KEEP>
 __device__ __noinline__ void exact_batch(MatchSmem& S, unsigned int entry, bool has, int lane)
 {
-    const float4* __restrict__ tsegs = S.tsegs; const float4* __restrict__ cache = S.cache;
-    const long long src_base = S.src_base, toff = S.toff;
-    const float3 Cs = S.Cs, Ct = S.Ct;
-    const float epi = S.epi; const int knn = S.knn;
+    const int knn = S.knn;
     bool pending = false;
     unsigned long long key = 0ull;
     int rl = 0;
@@ -156,24 +177,11 @@ __device__ __noinline__ void exact_batch(MatchSmem& S, unsigned int entry, bool 
         unsigned int j = entry & 0xFFFFFFu;
         if (j >= (unsigned int)S.Nt) j = 0u, has = false;         // padding segment of a partial stage
         float ov = 0.0f, d[4];
-        bool ok = false;
-        if (MODE) { if (has) ok = eval_candidate_f64(S, rl, j, &ov, d); }
-        else {
-            float4 q = __ldg(tsegs + j);
-            float4 rA = S.rowA[rl], rB = S.rowB[rl];
-            bool inv;
-            ov = exact_overlap(q, make_float3(rA.x, rA.y, rA.z), make_float3(rA.w, rB.x, rB.y), &inv);
-            if (has && ov > epi && ov >= S.row_thr[rl]) {      // below the current k-th best it can never be selected
-                SegRays s = load_rays(cache, src_base + rl), t = load_rays(cache, toff + j);
-                exact_depths(s, t, Cs, Ct, d);
-                ok = d[0] > 0.0f && d[1] > 0.0f && d[2] > 0.0f && d[3] > 0.0f;
-            }
-        }
-        if (ok) {
-            if (KEEP == 0) { key = make_key(ov, j); pending = true; }
+        if (eval_candidate<SEM>(S, rl, j, has, &ov, d)) {
+            if (KEEP == Keep::TopK) { key = make_key(ov, j); pending = true; }
             else {
                 const int slot = atomicAdd(&S.list_cnt[rl], 1);         // a row belongs to one warp: no cross-warp contention
-                if (KEEP == 2 && slot < knn) {
+                if (KEEP == Keep::Store && slot < knn) {
                     l3d_match_rec rec;
                     rec.tgt_seg = j; rec.overlap = ov; rec.d_p1 = d[0]; rec.d_p2 = d[1]; rec.d_q1 = d[2]; rec.d_q2 = d[3];
                     S.recs_out[(S.R0 + rl) * knn + slot] = rec;
@@ -181,7 +189,7 @@ __device__ __noinline__ void exact_batch(MatchSmem& S, unsigned int entry, bool 
             }
         }
     }
-    while (KEEP == 0) {
+    while (KEEP == Keep::TopK) {
         if (pending) {
             int slot = atomicAdd(&S.list_cnt[rl], 1);
             if (slot < S.cap) { S.lists[rl][slot] = key; pending = false; }
@@ -210,8 +218,9 @@ __device__ __noinline__ void exact_batch(MatchSmem& S, unsigned int entry, bool 
     __syncwarp();
 }
 
-// select the k best survivors of each of this warp's rows and write them once (once per CTA: out of line)
-template <int MODE, int KEEP>
+// write the match count of each of this warp's rows; TopK also selects the k best survivors and writes their records (once
+// per CTA: out of line)
+template <int SEM, Keep KEEP>
 __device__ __noinline__ void finalize_rows(MatchSmem& S, int warp, int lane, int nrows, long long R0, int* __restrict__ counts_out,
                                            l3d_match_rec* __restrict__ recs_out)
 {
@@ -220,7 +229,7 @@ __device__ __noinline__ void finalize_rows(MatchSmem& S, int warp, int lane, int
         const int rl = warp * MK_RPW + r;
         if (rl >= nrows) break;
         const long long R = R0 + rl;
-        if (KEEP != 0) { if (lane == 0) counts_out[R] = S.list_cnt[rl]; continue; }
+        if (KEEP != Keep::TopK) { if (lane == 0) counts_out[R] = S.list_cnt[rl]; continue; }
         const int n = min(S.list_cnt[rl], S.cap);
         if (lane == 0) counts_out[R] = min(n, knn);
         if (n == 0) continue;
@@ -229,15 +238,7 @@ __device__ __noinline__ void finalize_rows(MatchSmem& S, int warp, int lane, int
         if (lane < n && rank < knn) {
             unsigned int j = key_tgt(key);
             float d[4];
-            if (MODE) {
-                const SegRaysD s = load_rays_d(S.cache_d, S.src_base + rl), t = load_rays_d(S.cache_d, S.toff + j);
-                double dd[4];
-                exact_depths_f64(s, t, S.Csd, S.Ctd, dd);
-                d[0] = (float)dd[0]; d[1] = (float)dd[1]; d[2] = (float)dd[2]; d[3] = (float)dd[3];
-            } else {
-                SegRays s = load_rays(S.cache, S.src_base + rl), t = load_rays(S.cache, S.toff + j);
-                exact_depths(s, t, S.Cs, S.Ct, d);
-            }
+            target_depths<SEM>(S, rl, j, d);
             l3d_match_rec rec;
             rec.tgt_seg = j; rec.overlap = key_overlap(key);
             rec.d_p1 = d[0]; rec.d_p2 = d[1]; rec.d_q1 = d[2]; rec.d_q2 = d[3];
@@ -369,7 +370,7 @@ k_arcs_gather(long long n, const unsigned long long* __restrict__ keys, const un
 
 // level 2: the float filter on up to 64 level-1 survivors (two per lane: both gathers of the target segment in flight together);
 // its survivors are queued for the exact path
-template <int MODE, int KEEP>
+template <int SEM, Keep KEEP>
 __device__ __forceinline__ void filter_batch(MatchSmem& S, unsigned int e0, bool has0, unsigned int e1, bool has1, int warp, int lane,
                                              unsigned int lt_mask, int& qn2)
 {
@@ -386,38 +387,44 @@ __device__ __forceinline__ void filter_batch(MatchSmem& S, unsigned int e0, bool
         if (p1) S.queue2[warp][qn2 + __popc(b1 & lt_mask)] = e1;
         qn2 += __popc(b1);
         __syncwarp();
-        while (qn2 >= 32) { qn2 -= 32; exact_batch<MODE, KEEP>(S, S.queue2[warp][qn2 + lane], true, lane); }
+        while (qn2 >= 32) { qn2 -= 32; exact_batch<SEM, KEEP>(S, S.queue2[warp][qn2 + lane], true, lane); }
     }
 }
 
-template <int MODE, int KEEP>
-__device__ __forceinline__ void match_topk_body(const float4* __restrict__ segs, const float4* __restrict__ cache, const L3DViewDev* __restrict__ views,
-             const L3DPairDev* __restrict__ pairs, const int2* __restrict__ tiles, int knn, float epi,
-             int* __restrict__ counts_out, l3d_match_rec* __restrict__ recs_out, const double* __restrict__ cache_d,
-             const uint4* __restrict__ arcs, const L3DPairBasis* __restrict__ basis)
+// One instantiation per semantics (L3D_SEM_*: the exact path's arithmetic; the staging, scan and float filter are the same) and
+// keep policy.  TopK is the production kernel.  kNN <= 0 ("keep all matches", cudawrapper.cu:628-636 / line3D.cc:988-996) runs
+// Count (A.knn unused), then Store with the row stride found by Count in A.knn.
+// The pair, view and basis records are read with explicit __ldg: pointers taken from a parameter block carry no __restrict__.
+template <int SEM, Keep KEEP>
+__global__ void __launch_bounds__(MK_THREADS, MK_MINB) k_match_topk(const MatchArgs A)
 {
+    const float4* segs = A.segs;
+    const int knn = A.knn; const float epi = A.epi;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     MatchSmem& S = *reinterpret_cast<MatchSmem*>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int2 tile = tiles[blockIdx.x];
-    const L3DPairDev* P = pairs + tile.x;
+    const int2 tile = __ldg(A.tiles + blockIdx.x);
+    const L3DPairDev* P = A.pairs + tile.x;
+    const L3DPairBasis* PB = A.basis + tile.x;
     const int row0 = tile.y;
-    const L3DViewDev* vs = views + P->src;
-    const L3DViewDev* vt = views + P->tgt;
-    const long long soff = vs->seg_off, toff = vt->seg_off;
-    const int Ns = vs->nseg, Nt = vt->nseg;
+    const L3DViewDev* vs = A.views + __ldg(&P->src);
+    const L3DViewDev* vt = A.views + __ldg(&P->tgt);
+    const long long soff = __ldg(&vs->seg_off), toff = __ldg(&vt->seg_off);
+    const int Ns = __ldg(&vs->nseg), Nt = __ldg(&vt->nseg);
+    const long long R0 = __ldg(&P->row_off) + row0;
     const int nrows = min(MK_ROWS, Ns - row0);
     const float4* tsegs = segs + toff;
-    const uint4* tarcs = arcs + P->arc_off;
+    const uint4* tarcs = A.arcs + __ldg(&P->arc_off);
     const int RES = MK_STAGES * MK_TT;                     // entries resident at a time; larger target views take several passes
     const int npass = (Nt + RES - 1) / RES;
     if (tid == 0) {
-        S.tsegs = tsegs; S.cache = cache; S.src_base = soff + row0; S.toff = toff; S.epi = epi; S.knn = knn; S.Nt = Nt; S.cap = MK_CAP;
-        S.Cs = make_float3(vs->C[0], vs->C[1], vs->C[2]); S.Ct = make_float3(vt->C[0], vt->C[1], vt->C[2]);
-        S.cache_d = cache_d; S.ssegs = segs + soff + row0; S.R0 = P->row_off + row0; S.recs_out = recs_out;
-        if (MODE) {
-            for (int i = 0; i < 9; ++i) S.Fd[i] = P->Fd[i];
-            S.Csd = d3(vs->C_d[0], vs->C_d[1], vs->C_d[2]); S.Ctd = d3(vt->C_d[0], vt->C_d[1], vt->C_d[2]);
+        S.tsegs = tsegs; S.cache = A.cache; S.src_base = soff + row0; S.toff = toff; S.epi = epi; S.knn = knn; S.Nt = Nt; S.cap = MK_CAP;
+        S.Cs = make_float3(__ldg(&vs->C[0]), __ldg(&vs->C[1]), __ldg(&vs->C[2])); S.Ct = make_float3(__ldg(&vt->C[0]), __ldg(&vt->C[1]), __ldg(&vt->C[2]));
+        S.R0 = R0; S.recs_out = A.recs;
+        if (SEM == L3D_SEM_REF_CPU) {
+            S.cache_d = A.cache_d; S.ssegs = segs + soff + row0;
+            for (int i = 0; i < 9; ++i) S.Fd[i] = __ldg(&P->Fd[i]);
+            S.Csd = d3(__ldg(&vs->C_d[0]), __ldg(&vs->C_d[1]), __ldg(&vs->C_d[2])); S.Ctd = d3(__ldg(&vt->C_d[0]), __ldg(&vt->C_d[1]), __ldg(&vt->C_d[2]));
         }
         for (int i = 0; i < MK_STAGES; ++i) mbar_init(&S.bars[i], 1);
         mbar_fence_init();
@@ -427,17 +434,20 @@ __device__ __forceinline__ void match_topk_body(const float4* __restrict__ segs,
             tma_load_1d(S.stage[i], tarcs + (size_t)i * MK_TT, bytes, &S.bars[i]);
         }
     }
-    if (tid >= MK_THREADS - (L3D_ARC_NCLS + 2)) S.cls_off[MK_THREADS - 1 - tid] = basis[tile.x].cls_off[MK_THREADS - 1 - tid];
+    if (tid >= MK_THREADS - (L3D_ARC_NCLS + 2)) S.cls_off[MK_THREADS - 1 - tid] = __ldg(&PB->cls_off[MK_THREADS - 1 - tid]);
     if (tid < MK_ROWS) {
         S.list_cnt[tid] = 0;
         S.row_thr[tid] = 0.0f;
         if (tid < nrows) {
             float4 s = __ldg(segs + soff + row0 + tid);
-            float3 e1 = mulmat_h(P->F, s.x, s.y), e2 = mulmat_h(P->F, s.z, s.w);     // epipolar lines F*p (cudawrapper.cu:216-217)
+            float F[9];
+            for (int i = 0; i < 9; ++i) F[i] = __ldg(&P->F[i]);
+            float3 e1 = mulmat_h(F, s.x, s.y), e2 = mulmat_h(F, s.z, s.w);     // epipolar lines F*p (cudawrapper.cu:216-217)
             float g = L3D_FILTER_C1 * fmaxf(sqrtf(e1.x * e1.x + e1.y * e1.y), sqrtf(e2.x * e2.x + e2.y * e2.y));
             S.rowA[tid] = make_float4(e1.x, e1.y, e1.z, e2.x);
             S.rowB[tid] = make_float4(e2.y, e2.z, g, 0.95f * epi);
-            const L3DPairBasis B = basis[tile.x];
+            L3DPairBasis B;
+            for (int i = 0; i < 3; ++i) { B.u[i] = __ldg(&PB->u[i]); B.v[i] = __ldg(&PB->v[i]); }
             bool off1, off2;
             S.rowK[tid] = make_uint2(line_kappa(B, e1, &off1), line_kappa(B, e2, &off2));
             S.rowall[tid] = (off1 || off2) ? 1 : 0;
@@ -518,7 +528,7 @@ __device__ __forceinline__ void match_topk_body(const float4* __restrict__ segs,
                         __syncwarp();
                         if (qn >= 64) {
                             qn -= 64;
-                            filter_batch<MODE, KEEP>(S, S.queue[warp][qn + lane], true, S.queue[warp][qn + 32 + lane], true, warp, lane, lt_mask, qn2);
+                            filter_batch<SEM, KEEP>(S, S.queue[warp][qn + lane], true, S.queue[warp][qn + 32 + lane], true, warp, lane, lt_mask, qn2);
                         }
                     }
                 }
@@ -527,48 +537,24 @@ __device__ __forceinline__ void match_topk_body(const float4* __restrict__ segs,
     }
     if (qn > 0) {
         const bool h0 = lane < qn, h1 = lane + 32 < qn;
-        filter_batch<MODE, KEEP>(S, h0 ? S.queue[warp][lane] : 0u, h0, h1 ? S.queue[warp][lane + 32] : 0u, h1, warp, lane, lt_mask, qn2);
+        filter_batch<SEM, KEEP>(S, h0 ? S.queue[warp][lane] : 0u, h0, h1 ? S.queue[warp][lane + 32] : 0u, h1, warp, lane, lt_mask, qn2);
     }
     __syncwarp();
     if (qn2 > 0) {
         const bool has = lane < qn2;
-        exact_batch<MODE, KEEP>(S, has ? S.queue2[warp][lane] : 0u, has, lane);
+        exact_batch<SEM, KEEP>(S, has ? S.queue2[warp][lane] : 0u, has, lane);
     }
     __syncwarp();
 
-    finalize_rows<MODE, KEEP>(S, warp, lane, nrows, P->row_off + row0, counts_out, recs_out);
+    finalize_rows<SEM, KEEP>(S, warp, lane, nrows, R0, A.counts, A.recs);
 }
 
-__global__ void __launch_bounds__(MK_THREADS, MK_MINB)
-k_match_topk(const float4* __restrict__ segs, const float4* __restrict__ cache, const L3DViewDev* __restrict__ views,
-             const L3DPairDev* __restrict__ pairs, const int2* __restrict__ tiles, int knn, float epi,
-             int* __restrict__ counts_out, l3d_match_rec* __restrict__ recs_out, const uint4* __restrict__ arcs, const L3DPairBasis* __restrict__ basis)
-{ match_topk_body<0, 0>(segs, cache, views, pairs, tiles, knn, epi, counts_out, recs_out, nullptr, arcs, basis); }
-
-// REF_CPU semantics: same tiling, staging and filter; the exact path is matchingCPU's double arithmetic
-__global__ void __launch_bounds__(MK_THREADS, MK_MINB)
-k_match_topk_f64(const float4* __restrict__ segs, const float4* __restrict__ cache, const L3DViewDev* __restrict__ views,
-                 const L3DPairDev* __restrict__ pairs, const int2* __restrict__ tiles, int knn, float epi,
-                 int* __restrict__ counts_out, l3d_match_rec* __restrict__ recs_out, const double* __restrict__ cache_d,
-                 const uint4* __restrict__ arcs, const L3DPairBasis* __restrict__ basis)
-{ match_topk_body<1, 0>(segs, cache, views, pairs, tiles, knn, epi, counts_out, recs_out, cache_d, arcs, basis); }
-
-// kNN <= 0 ("keep all matches", cudawrapper.cu:628-636 / line3D.cc:988-996): pass 1 counts the survivors of every row
-// (stride == 0), pass 2 stores them with the row stride found by pass 1.  cache_d != nullptr selects REF_CPU arithmetic.
-__global__ void __launch_bounds__(MK_THREADS, MK_MINB)
-k_match_all(const float4* __restrict__ segs, const float4* __restrict__ cache, const L3DViewDev* __restrict__ views,
-            const L3DPairDev* __restrict__ pairs, const int2* __restrict__ tiles, int stride, float epi,
-            int* __restrict__ counts_out, l3d_match_rec* __restrict__ recs_out, const double* __restrict__ cache_d,
-            const uint4* __restrict__ arcs, const L3DPairBasis* __restrict__ basis)
-{
-    if (cache_d) {
-        if (stride == 0) match_topk_body<1, 1>(segs, cache, views, pairs, tiles, 0, epi, counts_out, recs_out, cache_d, arcs, basis);
-        else match_topk_body<1, 2>(segs, cache, views, pairs, tiles, stride, epi, counts_out, recs_out, cache_d, arcs, basis);
-    } else {
-        if (stride == 0) match_topk_body<0, 1>(segs, cache, views, pairs, tiles, 0, epi, counts_out, recs_out, nullptr, arcs, basis);
-        else match_topk_body<0, 2>(segs, cache, views, pairs, tiles, stride, epi, counts_out, recs_out, nullptr, arcs, basis);
-    }
-}
+static_assert(L3D_SEM_REF_GPU == 0 && L3D_SEM_REF_CPU == 1 && (int)Keep::TopK == 0 && (int)Keep::Count == 1 && (int)Keep::Store == 2,
+              "l3d_match_kernels is indexed [L3D_SEM_*][Keep]");
+void (*const l3d_match_kernels[2][3])(MatchArgs) = {
+    {k_match_topk<L3D_SEM_REF_GPU, Keep::TopK>, k_match_topk<L3D_SEM_REF_GPU, Keep::Count>, k_match_topk<L3D_SEM_REF_GPU, Keep::Store>},
+    {k_match_topk<L3D_SEM_REF_CPU, Keep::TopK>, k_match_topk<L3D_SEM_REF_CPU, Keep::Count>, k_match_topk<L3D_SEM_REF_CPU, Keep::Store>},
+};
 
 // keep-all rows arrive in queue order; the reference appends them in ascending target order.  One warp per row, the row
 // staged in shared memory (stride * 24 B per warp), rank = number of smaller target indices (unique per row).
@@ -715,11 +701,9 @@ __device__ __forceinline__ void dense_tile(const float4* __restrict__ ssegs, int
     if (qn > 0) dense_exact_batch(S, lane < qn ? S.queue[warp][lane] : 0u, lane < qn, warp, x0);
 }
 
-__global__ void __launch_bounds__(DK_THREADS, DK_MINB)
-k_match_dense(const float4* __restrict__ ssegs, int Ns, const float4* __restrict__ tsegs, int Nt,
-              const float4* __restrict__ scache, const float4* __restrict__ tcache, L3DMat3 F, float3 Cs, float3 Ct,
-              float epi, float4* __restrict__ depths, float* __restrict__ overlaps, int rows_per_cta)
-{ dense_tile(ssegs, Ns, tsegs, Nt, scache, tcache, F, Cs, Ct, epi, depths, overlaps, rows_per_cta, blockIdx.x, blockIdx.y); }
+// one view pair: a 2-D grid of (column block, row block) tiles
+__global__ void __launch_bounds__(DK_THREADS, DK_MINB) k_match_dense(const L3DDenseJob J, float epi)
+{ dense_tile(J.ssegs, J.Ns, J.tsegs, J.Nt, J.scache, J.tcache, J.F, J.Cs, J.Ct, epi, J.depths, J.overlaps, J.rows_per_cta, blockIdx.x, blockIdx.y); }
 
 // The same contract for MANY view pairs in one launch (l3d_match_dense_pairs): a 1-D grid over the tiles of all jobs, so the tail of
 // one pair's tiles overlaps the head of the next pair's instead of leaving SMs idle at the end of every 88 us launch.
@@ -735,11 +719,10 @@ k_match_dense_batch(const L3DDenseJob* __restrict__ jobs, int njobs, float epi)
 }
 
 // same contract, NO pre-filter: every cell goes through the exact path.  Test-only cross-check of the filter.
-__global__ void __launch_bounds__(DK_THREADS)
-k_match_dense_nofilter(const float4* __restrict__ ssegs, int Ns, const float4* __restrict__ tsegs, int Nt,
-                       const float4* __restrict__ scache, const float4* __restrict__ tcache, L3DMat3 F, float3 Cs,
-                       float3 Ct, float epi, float4* __restrict__ depths, float* __restrict__ overlaps)
+__global__ void __launch_bounds__(DK_THREADS) k_match_dense_nofilter(const L3DDenseJob J, float epi)
 {
+    const float4 *ssegs = J.ssegs, *tsegs = J.tsegs, *scache = J.scache, *tcache = J.tcache;
+    const int Ns = J.Ns, Nt = J.Nt; const L3DMat3& F = J.F; const float3 Cs = J.Cs, Ct = J.Ct;
     const int x = blockIdx.x * DK_THREADS + threadIdx.x;
     const int row0 = blockIdx.y * DKN_ROWS;
     const int nrows = min(DKN_ROWS, Ns - row0);
@@ -758,8 +741,8 @@ k_match_dense_nofilter(const float4* __restrict__ ssegs, int Ns, const float4* _
             res = make_float4(d[0], d[1], d[2], d[3]);
         }
         const size_t o = (size_t)(row0 + r) * Nt + x;
-        depths[o] = res;
-        overlaps[o] = ov;
+        J.depths[o] = res;
+        J.overlaps[o] = ov;
     }
 }
 

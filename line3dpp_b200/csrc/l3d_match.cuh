@@ -42,20 +42,19 @@ size_t l3d_dense_smem_bytes();
 
 __global__ void k_prep_segments(const float4* __restrict__ segs, const L3DViewDev* __restrict__ views, int num_views,
                                 long long total, float4* __restrict__ cache);
-__global__ void k_match_topk(const float4* __restrict__ segs, const float4* __restrict__ cache,
-                             const L3DViewDev* __restrict__ views, const L3DPairDev* __restrict__ pairs,
-                             const int2* __restrict__ tiles, int knn, float epi, int* __restrict__ counts_out,
-                             l3d_match_rec* __restrict__ recs_out, const uint4* __restrict__ arcs, const L3DPairBasis* __restrict__ basis);
-__global__ void k_match_topk_f64(const float4* __restrict__ segs, const float4* __restrict__ cache,
-                                 const L3DViewDev* __restrict__ views, const L3DPairDev* __restrict__ pairs,
-                                 const int2* __restrict__ tiles, int knn, float epi, int* __restrict__ counts_out,
-                                 l3d_match_rec* __restrict__ recs_out, const double* __restrict__ cache_d, const uint4* __restrict__ arcs,
-                                 const L3DPairBasis* __restrict__ basis);
-__global__ void k_match_all(const float4* __restrict__ segs, const float4* __restrict__ cache,
-                            const L3DViewDev* __restrict__ views, const L3DPairDev* __restrict__ pairs,
-                            const int2* __restrict__ tiles, int stride, float epi, int* __restrict__ counts_out,
-                            l3d_match_rec* __restrict__ recs_out, const double* __restrict__ cache_d, const uint4* __restrict__ arcs,
-                            const L3DPairBasis* __restrict__ basis);
+// parameters of k_match_topk, passed by value
+struct MatchArgs {
+    const float4* segs; const float4* cache; const double* cache_d;       // segments, their float / double ray caches (cache_d: REF_CPU)
+    const L3DViewDev* views; const L3DPairDev* pairs; const int2* tiles;  // tiles: (pair, first source row) of every CTA
+    const uint4* arcs; const L3DPairBasis* basis;                         // level-1 tables (k_pair_arcs, k_arcs_gather)
+    int* counts; l3d_match_rec* recs;                                     // per-row match count and records
+    int knn;                                                              // TopK: k; Store: row stride; Count: unused
+    float epi;
+};
+// what k_match_topk keeps of the matches of a row: the kNN best, only their number, or all of them
+enum class Keep { TopK, Count, Store };
+template <int SEM, Keep KEEP> __global__ void k_match_topk(MatchArgs A);    // SEM: L3D_SEM_REF_GPU / L3D_SEM_REF_CPU
+extern void (*const l3d_match_kernels[2][3])(MatchArgs);                   // every instantiation of k_match_topk: [SEM][KEEP]
 // level-1 pre-filter tables: one CTA per view pair of [first_pair, first_pair + gridDim.x): raw arcs + sort keys; after the sort
 // k_arcs_gather writes the packed entries in window order
 __global__ void k_pair_arcs(const float4* __restrict__ segs, const L3DViewDev* __restrict__ views, const L3DPairDev* __restrict__ pairs,
@@ -66,19 +65,14 @@ __global__ void k_arcs_gather(long long n, const unsigned long long* __restrict_
 __global__ void k_sort_rows(int* __restrict__ counts, l3d_match_rec* __restrict__ recs, int stride, long long rows, int topk);
 __global__ void k_prep_segments_f64(const float4* __restrict__ segs, const L3DViewDev* __restrict__ views, int num_views,
                                     long long total, double* __restrict__ cache);
-__global__ void k_match_dense(const float4* __restrict__ ssegs, int Ns, const float4* __restrict__ tsegs, int Nt,
-                              const float4* __restrict__ scache, const float4* __restrict__ tcache, L3DMat3 F, float3 Cs,
-                              float3 Ct, float epi, float4* __restrict__ depths, float* __restrict__ overlaps, int rows_per_cta);
 int l3d_dense_rows_per_cta(int Ns, int Nt, int num_sms);
-struct L3DDenseJob {            // one view pair of a batched dense launch
+struct L3DDenseJob {            // one view pair of the dense contract; colb / tile0: its tiles in a batched launch
     const float4* ssegs; const float4* tsegs; const float4* scache; const float4* tcache; float4* depths; float* overlaps;
     L3DMat3 F; float3 Cs, Ct; int Ns, Nt, rows_per_cta, colb; long long tile0;
 };
+__global__ void k_match_dense(L3DDenseJob J, float epi);
 __global__ void k_match_dense_batch(const L3DDenseJob* __restrict__ jobs, int njobs, float epi);
-__global__ void k_match_dense_nofilter(const float4* __restrict__ ssegs, int Ns, const float4* __restrict__ tsegs, int Nt,
-                                       const float4* __restrict__ scache, const float4* __restrict__ tcache, L3DMat3 F,
-                                       float3 Cs, float3 Ct, float epi, float4* __restrict__ depths,
-                                       float* __restrict__ overlaps);
+__global__ void k_match_dense_nofilter(L3DDenseJob J, float epi);
 __global__ void k_compact_matches(const int* __restrict__ counts, const long long* __restrict__ row_ptr,
                                   const l3d_match_rec* __restrict__ recs, int knn, long long rows,
                                   l3d_match_rec* __restrict__ out);
