@@ -226,7 +226,7 @@ static int stage_pairs(l3d_ctx* c, int num_pairs, const int32_t* pairs, const fl
     int rc;
     L3D_RESERVE(c->d_pairs, sizeof(L3DPairDev) * (size_t)std::max(num_pairs, 1), "pairs");
     L3D_RESERVE(c->d_tiles, sizeof(int2) * std::max<size_t>(c->h_tiles.size(), 1), "tiles");
-    L3D_RESERVE(c->d_arcs, sizeof(uint4) * (size_t)std::max<long long>(*narcs, 1), "target arcs");
+    L3D_RESERVE(c->d_arcs, (sizeof(uint4) + sizeof(float4)) * (size_t)std::max<long long>(*narcs, 1), "target arcs");   // arcs, then their segments
     L3D_RESERVE(c->d_basis, sizeof(L3DPairBasis) * (size_t)std::max(num_pairs, 1), "pair bases");
     L3D_RESERVE(c->d_counts, sizeof(int) * (size_t)std::max<long long>(rows, 1), "match counts");
     if (knn > 0 && knn <= 32) L3D_RESERVE(c->d_recs, sizeof(l3d_match_rec) * (size_t)std::max<long long>(rows, 1) * knn, "match records");
@@ -236,8 +236,11 @@ static int stage_pairs(l3d_ctx* c, int num_pairs, const int32_t* pairs, const fl
     return L3D_OK;
 }
 
-// Level-1 tables of the pairs matched here (l3d_device.cuh "pencil parameter"): raw arcs + keys, one sort, packed entries in window
-// order.  Below epi_overlap 0.01 the extended arcs would span the whole line: everything is then handed to the float filter.
+// d_arcs holds the narcs packed arcs, then the target segment of every arc in the same order
+static float4* level1_segs(l3d_ctx* c, long long narcs) { return (float4*)((uint4*)c->d_arcs.p + narcs); }
+
+// Level-1 tables of the pairs matched here (l3d_device.cuh "pencil parameter"): raw arcs + keys, one sort, packed arcs and their target
+// segments in window order.  Below epi_overlap 0.01 the extended arcs would span the whole line: everything is then handed to the float filter.
 static int build_level1(l3d_ctx* c, int first_pair, int last_pair, long long narcs, float epi_overlap)
 {
     if (last_pair <= first_pair || narcs <= 0) return L3D_OK;
@@ -257,7 +260,8 @@ static int build_level1(l3d_ctx* c, int first_pair, int last_pair, long long nar
              return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const unsigned long long*)c->d_arckeys.p, (unsigned long long*)c->d_arckeys2.p,
                                                     (const unsigned int*)c->d_arcvals.p, (unsigned int*)c->d_arcvals2.p, (int)narcs, 0, end_bit, c->stream); }))) return rc;
     k_arcs_gather<<<(unsigned int)((narcs + 255) / 256), 256, 0, c->stream>>>(narcs, (const unsigned long long*)c->d_arckeys2.p, (const unsigned int*)c->d_arcvals2.p,
-                                                                             (const uint4*)c->d_arcraw.p, (const L3DPairDev*)c->d_pairs.p, first_pair, (uint4*)c->d_arcs.p);
+                                                                             (const uint4*)c->d_arcraw.p, c->segs(), c->views(), (const L3DPairDev*)c->d_pairs.p,
+                                                                             first_pair, (uint4*)c->d_arcs.p, level1_segs(c, narcs));
     L3D_CUDA(c, cudaGetLastError(), "k_arcs_gather");
     c->launches += 2 + 8;
     return L3D_OK;
@@ -377,7 +381,7 @@ static int match_impl(l3d_ctx* c, int num_pairs, const int32_t* pairs, const flo
     if (Fd && (rc = build_cache_d(c))) return rc;
     c->semantics = Fd ? L3D_SEM_REF_CPU : L3D_SEM_REF_GPU;
     const MatchArgs a = {c->segs(), (const float4*)c->d_cache.p, Fd ? (const double*)c->d_cache_d.p : nullptr, c->views(), (const L3DPairDev*)c->d_pairs.p,
-                         (const int2*)c->d_tiles.p, (const uint4*)c->d_arcs.p, (const L3DPairBasis*)c->d_basis.p, (int*)c->d_counts.p,
+                         (const int2*)c->d_tiles.p, (const uint4*)c->d_arcs.p, level1_segs(c, narcs), (const L3DPairBasis*)c->d_basis.p, (int*)c->d_counts.p,
                          (l3d_match_rec*)c->d_recs.p, knn, epi_overlap};
     if ((rc = knn > 0 && knn <= 32 ? run_topk(c, a, host) : run_keep_all(c, a, knn > 32 ? knn : 0))) return rc;
     c->have_matches = true;

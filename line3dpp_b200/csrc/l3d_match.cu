@@ -4,13 +4,16 @@
 //                     segment (the reference recomputes 4 mat-vecs + 5 normalisations per surviving PAIR,
 //                     cudawrapper.cu:148-154).
 //   k_pair_arcs,    : level-1 tables of the view pairs of one call (l3d_device.cuh "pencil parameter"): every target segment as an arc of
-//   k_arcs_gather     the epipolar pencil, grouped by arc length and sorted by arc start (one radix sort in between, l3d_capi.cu).
-//   k_match_topk    : production kernel.  One CTA = 64 source segments of one view pair; the pair's arc table is staged in shared
-//                     memory by 1-D TMA (cp.async.bulk + mbarrier, 3 x 16 KB in flight from the first instruction); a warp owns 8 rows
-//                     and, per row, binary-searches the window of every arc class, scans only those entries (13 integer instructions
-//                     each), compacts the survivors with ballots into a per-warp queue, runs the conservative float filter on 64 of
-//                     them at a time (27 flop + 2 rcp each, target segment gathered from L2), queues its survivors again and
-//                     evaluates those 32 at a time with the exact, reference-order arithmetic; per-row survivor keys live in shared
+//   k_arcs_gather     the epipolar pencil, grouped by arc length and sorted by arc start (one radix sort in between, l3d_capi.cu); the
+//                     table carries each arc's target segment in a parallel array (32 B per pair and target).
+//   k_match_topk    : production kernel.  One CTA = 64 source segments of one view pair; the pair's table (arcs + segments) is staged
+//                     in shared memory by 1-D TMA (cp.async.bulk + mbarrier, 3 stages x 512 entries x 32 B in flight from the first
+//                     instruction; larger target views take several passes); a warp owns 8 rows and, per row, binary-searches the
+//                     window of every arc class and scans only those entries, all windows as one concatenation (full warps): each
+//                     lane runs the arc test (13 integer instructions) and the conservative float filter (27 flop + 2 rcp on the
+//                     staged target segment) on its entry, branch-free, the survivors of both are ballot-compacted into a per-warp
+//                     queue of ring positions (emptied before every refill) and evaluated 32 at a time on the staged segment with the
+//                     exact, reference-order arithmetic; per-row survivor keys live in shared
 //                     memory and the k best are selected and written once.  Replaces K_match_lines + the dense D2H + host
 //                     priority-queue pass (cudawrapper.cu:186-253, 570-650).  Instruction-issue / latency bound; compulsory HBM
 //                     traffic ~0.1 B/pair-eval.  One instantiation per semantics (REF_GPU / REF_CPU exact arithmetic) and keep
@@ -53,6 +56,7 @@ __global__ void __launch_bounds__(256) k_prep_segments_f64(const float4* __restr
 // ------------------------------------------------------------------------------------------------ fused match + top-k
 struct MatchSmem {
     uint4 stage[MK_STAGES][MK_TT];                   // TMA-staged target arcs in window order (arc_may_match, l3d_device.cuh)
+    float4 stage_seg[MK_STAGES][MK_TT];              // their target segments, same order (two arrays: both 16-byte loads of a warp are conflict-free)
     uint2 rowK[MK_ROWS];                             // pencil parameters of the row's two epipolar lines (l3d_device.cuh)
     int cls_off[L3D_ARC_NCLS + 2];                   // first sorted entry of every arc class of this view pair, and the end (k_pair_arcs)
     unsigned char rowall[MK_ROWS];                   // 1: an epipolar line of this row is not a pencil member to within the margins (source point at the epipole): no level 1
@@ -61,14 +65,14 @@ struct MatchSmem {
     float4 rowB[MK_ROWS];                            // (e2.y, e2.z, g, 0.95 * score-to-beat)
     float row_thr[MK_ROWS];                          // overlap of the current k-th best survivor (0 until k are known)
     int list_cnt[MK_ROWS];
-    unsigned int queue[MK_WARPS][128];               // level-1 survivors per warp: (row_local << 24) | tgt, filtered 64 at a time (up to 64 pushed per step)
-    unsigned int queue2[MK_WARPS][96];               // level-2 survivors (filter_may_survive), evaluated exactly 32 at a time
+    unsigned int queue[MK_WARPS][96];                // survivors of both filters per warp: (row_local << 24) | position in the ring, evaluated
+                                                     // exactly 32 at a time (up to 64 pushed per scan step onto at most 31 waiting)
     unsigned long long bars[MK_STAGES];
     // per-CTA constants of the (rarely executed, deliberately out-of-line) exact path
-    const float4* tsegs; const float4* cache;
+    const float4* cache;
     long long src_base, toff;
     float3 Cs, Ct;
-    float epi; int knn, Nt;
+    float epi; int knn;
     int cap;                                         // keys a row list collects before it is cut to its k best (and the score-to-beat rises); 16 instead of 32 was measured 7 % slower
     // REF_CPU semantics only: the exact path is matchingCPU's double arithmetic; the float filter stays the same
     const double* cache_d; const float4* ssegs;
@@ -138,25 +142,26 @@ __device__ __forceinline__ bool target_depths(const MatchSmem& S, int rl, unsign
     return d[0] > 0.0f && d[1] > 0.0f && d[2] > 0.0f && d[3] > 0.0f;
 }
 
-// exact evaluation of candidate j for row rl (has == false: padding lane, never a match): the overlap must exceed epi and reach
-// the row's current k-th best (below it the candidate can never be selected), and the depths must be positive (target_depths).
+// exact evaluation of candidate j (target segment q) for row rl (has == false: padding lane, never a match): the overlap must exceed
+// epi and reach the row's current k-th best (below it the candidate can never be selected), and the depths must be positive
+// (target_depths).
 // REF_GPU: K_match_lines' float overlap with the row's cached epipolar lines, inline (the lanes stay converged through it);
 // REF_CPU: matchingCPU's double overlap (line3D.cc:925-1003) with epipolar lines from the double F, out of line.
-template <int SEM> __device__ bool eval_candidate(const MatchSmem& S, int rl, unsigned int j, bool has, float* ov, float* d);
-template <> __device__ __forceinline__ bool eval_candidate<L3D_SEM_REF_GPU>(const MatchSmem& S, int rl, unsigned int j, bool has, float* ov, float* d)
+template <int SEM> __device__ bool eval_candidate(const MatchSmem& S, int rl, unsigned int j, float4 q, bool has, float* ov, float* d);
+template <> __device__ __forceinline__ bool eval_candidate<L3D_SEM_REF_GPU>(const MatchSmem& S, int rl, unsigned int j, float4 q, bool has, float* ov, float* d)
 {
     const float4 rA = S.rowA[rl], rB = S.rowB[rl];
     bool inv;
-    *ov = exact_overlap(__ldg(S.tsegs + j), make_float3(rA.x, rA.y, rA.z), make_float3(rA.w, rB.x, rB.y), &inv);
+    *ov = exact_overlap(q, make_float3(rA.x, rA.y, rA.z), make_float3(rA.w, rB.x, rB.y), &inv);
     return has && *ov > S.epi && *ov >= S.row_thr[rl] && target_depths<L3D_SEM_REF_GPU>(S, rl, j, d);
 }
-template <> __device__ __noinline__ bool eval_candidate<L3D_SEM_REF_CPU>(const MatchSmem& S, int rl, unsigned int j, bool has, float* ov, float* d)
+template <> __device__ __noinline__ bool eval_candidate<L3D_SEM_REF_CPU>(const MatchSmem& S, int rl, unsigned int j, float4 q, bool has, float* ov, float* d)
 {
     if (!has) return false;
     const float4 sp = __ldg(S.ssegs + rl);
     const D3 e1 = dmulmat(S.Fd, d3((double)sp.x, (double)sp.y, 1.0)), e2 = dmulmat(S.Fd, d3((double)sp.z, (double)sp.w, 1.0));
     bool valid;
-    *ov = exact_overlap_f64(__ldg(S.tsegs + j), e1, e2, &valid);
+    *ov = exact_overlap_f64(q, e1, e2, &valid);
     return valid && *ov > S.epi && *ov >= S.row_thr[rl] && target_depths<L3D_SEM_REF_CPU>(S, rl, j, d);
 }
 
@@ -174,10 +179,10 @@ __device__ __noinline__ void exact_batch(MatchSmem& S, unsigned int entry, bool 
     int rl = 0;
     if (has) {
         rl = (int)(entry >> 24);
-        unsigned int j = entry & 0xFFFFFFu;
-        if (j >= (unsigned int)S.Nt) j = 0u, has = false;         // padding segment of a partial stage
+        const unsigned int pos = entry & 0xFFFFFFu;                  // position in the resident ring: target index and segment are staged
+        const unsigned int j = (&S.stage[0][0])[pos].w;
         float ov = 0.0f, d[4];
-        if (eval_candidate<SEM>(S, rl, j, has, &ov, d)) {
+        if (eval_candidate<SEM>(S, rl, j, (&S.stage_seg[0][0])[pos], has, &ov, d)) {
             if (KEEP == Keep::TopK) { key = make_key(ov, j); pending = true; }
             else {
                 const int slot = atomicAdd(&S.list_cnt[rl], 1);         // a row belongs to one warp: no cross-warp contention
@@ -352,10 +357,11 @@ k_pair_arcs(const float4* __restrict__ segs, const L3DViewDev* __restrict__ view
     }
 }
 
-// packed entries in sorted order (arc_may_match, l3d_device.cuh)
+// packed entries in sorted order (arc_may_match, l3d_device.cuh) and, in a parallel array, their target segments
 __global__ void __launch_bounds__(256)
 k_arcs_gather(long long n, const unsigned long long* __restrict__ keys, const unsigned int* __restrict__ vals, const uint4* __restrict__ raw,
-              const L3DPairDev* __restrict__ pairs, int first_pair, uint4* __restrict__ out)
+              const float4* __restrict__ segs, const L3DViewDev* __restrict__ views, const L3DPairDev* __restrict__ pairs, int first_pair,
+              uint4* __restrict__ out, float4* __restrict__ out_segs)
 {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -363,32 +369,45 @@ k_arcs_gather(long long n, const unsigned long long* __restrict__ keys, const un
     const unsigned int src = vals[i];
     const uint4 r = raw[src];
     const bool wide = ((k >> 32) & 0xFull) == (unsigned long long)L3D_ARC_NCLS;
-    const unsigned int j = src - (unsigned int)pairs[first_pair + (int)(k >> 36)].arc_off;
+    const L3DPairDev* P = pairs + first_pair + (int)(k >> 36);
+    const unsigned int j = src - (unsigned int)P->arc_off;
     const unsigned int w16 = (r.y + 65535u) >> 16, e1 = (r.z + 65535u) >> 16, eh = (r.w + 65535u) >> 16;
     out[i] = wide ? make_uint4(0u, 0u, L3D_ARC_WIDE, j) : make_uint4(r.x, e1 | (w16 << 16), eh, j);
+    out_segs[i] = segs[views[P->tgt].seg_off + j];
 }
 
-// level 2: the float filter on up to 64 level-1 survivors (two per lane: both gathers of the target segment in flight together);
-// its survivors are queued for the exact path
-template <int SEM, Keep KEEP>
-__device__ __forceinline__ void filter_batch(MatchSmem& S, unsigned int e0, bool has0, unsigned int e1, bool has1, int warp, int lane,
-                                             unsigned int lt_mask, int& qn2)
+// thread 0: start the TMA copies of the level-1 entries [base, base + cnt) of a pair into the ring; the arcs and the segments of a
+// stage complete on the stage's barrier together
+__device__ __forceinline__ void stage_entries(MatchSmem& S, const uint4* arcs, const float4* asegs, int base, int cnt)
 {
-    float4 q0 = make_float4(0.f, 0.f, 0.f, 0.f), q1 = q0;
-    if (has0) q0 = __ldg(S.tsegs + (e0 & 0xFFFFFFu));
-    if (has1) q1 = __ldg(S.tsegs + (e1 & 0xFFFFFFu));
-    bool p0 = false, p1 = false;
-    if (has0) { const int rl = (int)(e0 >> 24); p0 = filter_may_survive(q0, S.rowA[rl], S.rowB[rl]); }
-    if (has1) { const int rl = (int)(e1 >> 24); p1 = filter_may_survive(q1, S.rowA[rl], S.rowB[rl]); }
-    const unsigned int b0 = __ballot_sync(0xffffffffu, p0), b1 = __ballot_sync(0xffffffffu, p1);
-    if (b0 | b1) {
-        if (p0) S.queue2[warp][qn2 + __popc(b0 & lt_mask)] = e0;
-        qn2 += __popc(b0);
-        if (p1) S.queue2[warp][qn2 + __popc(b1 & lt_mask)] = e1;
-        qn2 += __popc(b1);
-        __syncwarp();
-        while (qn2 >= 32) { qn2 -= 32; exact_batch<SEM, KEEP>(S, S.queue2[warp][qn2 + lane], true, lane); }
+    for (int i = 0; i < MK_STAGES && i * MK_TT < cnt; ++i) {
+        const unsigned int bytes = (unsigned int)min(MK_TT, cnt - i * MK_TT) * 16u;
+        const size_t o = (size_t)base + (size_t)i * MK_TT;
+        mbar_expect_tx(&S.bars[i], 2u * bytes);
+        tma_load_1d(S.stage[i], arcs + o, bytes, &S.bars[i]);
+        tma_load_1d(S.stage_seg[i], asegs + o, bytes, &S.bars[i]);
     }
+}
+
+// Does staged entry i pass both filters for a row (kappas k1, k2; rall: the row skips level 1; rA / rB: its float filter constants)?
+// Level 1 (arc_may_match) and level 2 (filter_may_survive on the staged target segment) are both evaluated and ANDed without a branch:
+// the arc test rejects only about a quarter of a window's entries.
+__device__ __forceinline__ bool entry_may_match(const MatchSmem& S, int i, unsigned int k1, unsigned int k2, bool rall, float4 rA, float4 rB)
+{
+    const uint4 arc = (&S.stage[0][0])[i];
+    return (arc_may_match(arc, k1, k2) | rall) & filter_may_survive((&S.stage_seg[0][0])[i], rA, rB);
+}
+
+// Entry index of position G + lane (clamped to the last position, tot - 1) of a row's concatenated window pieces (np pieces, lane q < np:
+// position pE and shift pshift of piece q, positions strictly increasing).  Warp-uniform G; piece of G by one ballot, the pieces that
+// start inside [G, G + 32) as bits of one reduction.
+__device__ __forceinline__ int flat_entry(int G, int lane, int np, int pE, int pshift, int tot)
+{
+    const bool mine = lane < np;
+    const int r0 = __popc(__ballot_sync(0xffffffffu, mine && pE <= G)) - 1;
+    const unsigned int starts = __reduce_or_sync(0xffffffffu, mine && pE > G && pE < G + 32 ? 1u << (pE - G) : 0u);
+    const int r = r0 + __popc(starts & ((2u << lane) - 1u));
+    return min(G + lane, tot - 1) + __shfl_sync(0xffffffffu, pshift, r);
 }
 
 // One instantiation per semantics (L3D_SEM_*: the exact path's arithmetic; the staging, scan and float filter are the same) and
@@ -413,12 +432,12 @@ __global__ void __launch_bounds__(MK_THREADS, MK_MINB) k_match_topk(const MatchA
     const int Ns = __ldg(&vs->nseg), Nt = __ldg(&vt->nseg);
     const long long R0 = __ldg(&P->row_off) + row0;
     const int nrows = min(MK_ROWS, Ns - row0);
-    const float4* tsegs = segs + toff;
     const uint4* tarcs = A.arcs + __ldg(&P->arc_off);
+    const float4* tasegs = A.arc_segs + __ldg(&P->arc_off);
     const int RES = MK_STAGES * MK_TT;                     // entries resident at a time; larger target views take several passes
     const int npass = (Nt + RES - 1) / RES;
     if (tid == 0) {
-        S.tsegs = tsegs; S.cache = A.cache; S.src_base = soff + row0; S.toff = toff; S.epi = epi; S.knn = knn; S.Nt = Nt; S.cap = MK_CAP;
+        S.cache = A.cache; S.src_base = soff + row0; S.toff = toff; S.epi = epi; S.knn = knn; S.cap = MK_CAP;
         S.Cs = make_float3(__ldg(&vs->C[0]), __ldg(&vs->C[1]), __ldg(&vs->C[2])); S.Ct = make_float3(__ldg(&vt->C[0]), __ldg(&vt->C[1]), __ldg(&vt->C[2]));
         S.R0 = R0; S.recs_out = A.recs;
         if (SEM == L3D_SEM_REF_CPU) {
@@ -428,11 +447,7 @@ __global__ void __launch_bounds__(MK_THREADS, MK_MINB) k_match_topk(const MatchA
         }
         for (int i = 0; i < MK_STAGES; ++i) mbar_init(&S.bars[i], 1);
         mbar_fence_init();
-        for (int i = 0; i < MK_STAGES && i * MK_TT < Nt; ++i) {        // the first pass is in flight while the rows are set up
-            const unsigned int bytes = (unsigned int)min(MK_TT, Nt - i * MK_TT) * 16u;
-            mbar_expect_tx(&S.bars[i], bytes);
-            tma_load_1d(S.stage[i], tarcs + (size_t)i * MK_TT, bytes, &S.bars[i]);
-        }
+        stage_entries(S, tarcs, tasegs, 0, min(RES, Nt));              // the first pass is in flight while the rows are set up
     }
     if (tid >= MK_THREADS - (L3D_ARC_NCLS + 2)) S.cls_off[MK_THREADS - 1 - tid] = __ldg(&PB->cls_off[MK_THREADS - 1 - tid]);
     if (tid < MK_ROWS) {
@@ -458,24 +473,21 @@ __global__ void __launch_bounds__(MK_THREADS, MK_MINB) k_match_topk(const MatchA
     const unsigned int lt_mask = (1u << lane) - 1u;
     const uint4* ent = &S.stage[0][0];
     const int my_rows = min(MK_RPW, nrows - warp * MK_RPW);
-    int qn = 0, qn2 = 0;   // warp-uniform fill of the two candidate queues
+    int qn = 0;    // warp-uniform fill of the candidate queue
 
     for (int pass = 0; pass < npass; ++pass) {
         const int base = pass * RES, cnt = min(RES, Nt - base);
         if (pass > 0) {                                // everybody is done with the resident entries: refill
             __syncthreads();
-            if (tid == 0)
-                for (int i = 0; i < MK_STAGES && i * MK_TT < cnt; ++i) {
-                    const unsigned int bytes = (unsigned int)min(MK_TT, cnt - i * MK_TT) * 16u;
-                    mbar_expect_tx(&S.bars[i], bytes);
-                    tma_load_1d(S.stage[i], tarcs + (size_t)base + (size_t)i * MK_TT, bytes, &S.bars[i]);
-                }
+            if (tid == 0) stage_entries(S, tarcs, tasegs, base, cnt);
         }
         for (int i = 0; i < MK_STAGES && i * MK_TT < cnt; ++i) mbar_wait(&S.bars[i], (unsigned int)(pass & 1));
         for (int r = 0; r < my_rows; ++r) {
             const int rl = warp * MK_RPW + r;
             const uint2 kr = S.rowK[rl];
             const bool rall = S.rowall[rl] != 0;
+            const float4 rA = S.rowA[rl];
+            float4 rB = S.rowB[rl];                     // rB.w: the score-to-beat, re-read after exact batches (a stale value only rejects less)
             // short arc [ka, kb] between the two kappa values: a target of class c can only match if its arc starts in [ka - 2^(CLS0 + c), kb]
             const bool fwd = (kr.y - kr.x) < 0x80000000u;
             const unsigned int ka = fwd ? kr.x : kr.y, kb = fwd ? kr.y : kr.x;
@@ -508,41 +520,41 @@ __global__ void __launch_bounds__(MK_THREADS, MK_MINB) k_match_topk(const MatchA
                 } else if (lane == 2 * L3D_ARC_NCLS) { plo = min(max(S.cls_off[L3D_ARC_NCLS] - base, 0), cnt); phi = cnt; }
                 if (rall) { plo = 0; phi = lane == 0 ? cnt : 0; }
             }
-            unsigned int pieces = __ballot_sync(0xffffffffu, phi > plo);
-            while (pieces) {
-                const int p = __ffs(pieces) - 1;
-                pieces &= pieces - 1u;
-                const int lo = __shfl_sync(0xffffffffu, plo, p), hi = __shfl_sync(0xffffffffu, phi, p);
-                for (int j0 = lo; j0 < hi; j0 += 64) {          // two entries per lane: half the loop / vote / push overhead per entry
-                    const int ia = j0 + lane, ib = ia + 32;
-                    bool pa = false, pb = false;
-                    unsigned int ta = 0u, tb = 0u;
-                    if (ia < hi) { const uint4 e = ent[ia]; pa = arc_may_match(e, kr.x, kr.y) || rall; ta = e.w; }
-                    if (ib < hi) { const uint4 e = ent[ib]; pb = arc_may_match(e, kr.x, kr.y) || rall; tb = e.w; }
-                    const unsigned int ba = __ballot_sync(0xffffffffu, pa), bb = __ballot_sync(0xffffffffu, pb);
-                    if (ba | bb) {
-                        if (pa) S.queue[warp][qn + __popc(ba & lt_mask)] = ((unsigned int)rl << 24) | ta;
-                        qn += __popc(ba);
-                        if (pb) S.queue[warp][qn + __popc(bb & lt_mask)] = ((unsigned int)rl << 24) | tb;
-                        qn += __popc(bb);
-                        __syncwarp();
-                        if (qn >= 64) {
-                            qn -= 64;
-                            filter_batch<SEM, KEEP>(S, S.queue[warp][qn + lane], true, S.queue[warp][qn + 32 + lane], true, warp, lane, lt_mask, qn2);
-                        }
+            // The pieces are scanned as one concatenation, so that every step but the row's last fills all 64 lanes: a window piece
+            // averages a few dozen entries.  Lane q < np holds the q-th non-empty piece: its position E in the concatenation and the
+            // shift (first entry - E) that turns a position of that piece into an entry index.
+            const int len = phi - plo;
+            const unsigned int ne = __ballot_sync(0xffffffffu, len > 0);
+            int ex = len;
+            for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, ex, o); if (lane >= o) ex += v; }
+            const int tot = __shfl_sync(0xffffffffu, ex, 31), np = __popc(ne);
+            ex -= len;
+            const int src = lane < np ? (int)__fns(ne, 0u, lane + 1) : 0;
+            const int pE = __shfl_sync(0xffffffffu, ex, src), pshift = __shfl_sync(0xffffffffu, plo - ex, src);
+            for (int G = 0; G < tot; G += 64) {                 // two entries per lane: half the loop / vote / push overhead per entry
+                const int ia = flat_entry(G, lane, np, pE, pshift, tot), ib = flat_entry(G + 32, lane, np, pE, pshift, tot);
+                const bool pa = entry_may_match(S, ia, kr.x, kr.y, rall, rA, rB) & (G + lane < tot);
+                const bool pb = entry_may_match(S, ib, kr.x, kr.y, rall, rA, rB) & (G + 32 + lane < tot);
+                const unsigned int ba = __ballot_sync(0xffffffffu, pa), bb = __ballot_sync(0xffffffffu, pb);
+                if (ba | bb) {
+                    if (pa) S.queue[warp][qn + __popc(ba & lt_mask)] = ((unsigned int)rl << 24) | (unsigned int)ia;
+                    qn += __popc(ba);
+                    if (pb) S.queue[warp][qn + __popc(bb & lt_mask)] = ((unsigned int)rl << 24) | (unsigned int)ib;
+                    qn += __popc(bb);
+                    __syncwarp();
+                    if (qn >= 32) {
+                        do { qn -= 32; exact_batch<SEM, KEEP>(S, S.queue[warp][qn + lane], true, lane); } while (qn >= 32);
+                        rB.w = S.rowB[rl].w;
                     }
                 }
             }
         }
-    }
-    if (qn > 0) {
-        const bool h0 = lane < qn, h1 = lane + 32 < qn;
-        filter_batch<SEM, KEEP>(S, h0 ? S.queue[warp][lane] : 0u, h0, h1 ? S.queue[warp][lane + 32] : 0u, h1, warp, lane, lt_mask, qn2);
-    }
-    __syncwarp();
-    if (qn2 > 0) {
-        const bool has = lane < qn2;
-        exact_batch<SEM, KEEP>(S, has ? S.queue2[warp][lane] : 0u, has, lane);
+        __syncwarp();
+        if (qn > 0) {                                  // the queue holds ring positions: empty it before the ring is refilled
+            const bool has = lane < qn;
+            exact_batch<SEM, KEEP>(S, has ? S.queue[warp][lane] : 0u, has, lane);
+            qn = 0;
+        }
     }
     __syncwarp();
 

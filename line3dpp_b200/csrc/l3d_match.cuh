@@ -13,10 +13,10 @@
 #endif
 #define MK_ROWS (MK_WARPS * MK_RPW)     /* source rows per CTA  */
 #ifndef MK_TT
-#define MK_TT 1024                      /* target segments per TMA stage (16 KB) */
+#define MK_TT 512                       /* level-1 entries (target segments) per TMA stage (16 B arc + 16 B segment each: 16 KB) */
 #endif
 #ifndef MK_STAGES
-#define MK_STAGES 3                     /* TMA ring depth: 3072 target segments resident without reuse */
+#define MK_STAGES 3                     /* TMA ring depth: 1536 target segments resident; larger target views take several passes */
 #endif
 #ifndef MK_CAP
 #define MK_CAP 32                       /* survivor keys kept per row before pruning to k (<= 32: one key per lane) */
@@ -46,7 +46,8 @@ __global__ void k_prep_segments(const float4* __restrict__ segs, const L3DViewDe
 struct MatchArgs {
     const float4* segs; const float4* cache; const double* cache_d;       // segments, their float / double ray caches (cache_d: REF_CPU)
     const L3DViewDev* views; const L3DPairDev* pairs; const int2* tiles;  // tiles: (pair, first source row) of every CTA
-    const uint4* arcs; const L3DPairBasis* basis;                         // level-1 tables (k_pair_arcs, k_arcs_gather)
+    const uint4* arcs; const float4* arc_segs;                            // level-1 table (k_arcs_gather): packed arcs and their target segments,
+    const L3DPairBasis* basis;                                            // both in window order; the pencil bases (k_pair_arcs)
     int* counts; l3d_match_rec* recs;                                     // per-row match count and records
     int knn;                                                              // TopK: k; Store: row stride; Count: unused
     float epi;
@@ -56,12 +57,13 @@ enum class Keep { TopK, Count, Store };
 template <int SEM, Keep KEEP> __global__ void k_match_topk(MatchArgs A);    // SEM: L3D_SEM_REF_GPU / L3D_SEM_REF_CPU
 extern void (*const l3d_match_kernels[2][3])(MatchArgs);                   // every instantiation of k_match_topk: [SEM][KEEP]
 // level-1 pre-filter tables: one CTA per view pair of [first_pair, first_pair + gridDim.x): raw arcs + sort keys; after the sort
-// k_arcs_gather writes the packed entries in window order
+// k_arcs_gather writes the packed arcs and, in a parallel array, their target segments, in window order
 __global__ void k_pair_arcs(const float4* __restrict__ segs, const L3DViewDev* __restrict__ views, const L3DPairDev* __restrict__ pairs,
                             int first_pair, int enabled, double ext, uint4* __restrict__ raw, unsigned long long* __restrict__ keys,
                             unsigned int* __restrict__ vals, L3DPairBasis* __restrict__ basis);
 __global__ void k_arcs_gather(long long n, const unsigned long long* __restrict__ keys, const unsigned int* __restrict__ vals,
-                              const uint4* __restrict__ raw, const L3DPairDev* __restrict__ pairs, int first_pair, uint4* __restrict__ out);
+                              const uint4* __restrict__ raw, const float4* __restrict__ segs, const L3DViewDev* __restrict__ views,
+                              const L3DPairDev* __restrict__ pairs, int first_pair, uint4* __restrict__ out, float4* __restrict__ out_segs);
 __global__ void k_sort_rows(int* __restrict__ counts, l3d_match_rec* __restrict__ recs, int stride, long long rows, int topk);
 __global__ void k_prep_segments_f64(const float4* __restrict__ segs, const L3DViewDev* __restrict__ views, int num_views,
                                     long long total, double* __restrict__ cache);
