@@ -1,8 +1,10 @@
 // l3d_affinity.cu — pairwise affinities between 3D hypotheses and the replicator-dynamics diffusion.
 //
-//   k_affinity        : Line3D::similarity (line3D.cc:1467-1553) for every kept match whose two segments both have a
-//                       3D estimate; the reference does this on the host under three mutexes (computingAffinityMatrix,
-//                       line3D.cc:1852-1979).  One thread per match slot, deterministic output order.
+//   l3d_affinity_matrix : computingAffinityMatrix (line3D.cc:1852-1979), which the reference runs on the host under three
+//                       mutexes, in five steps: the kept matches in emission order; their candidates - Line3D::similarity
+//                       (line3D.cc:1467-1553) above min_affinity and, with collinearity links, the links through target and
+//                       source (1904-1974) - counted per kept match (k_aff_count), scanned and written in the reference's order
+//                       (k_aff_fill); unused() as a fixpoint over a stable pair sort; local ids by first appearance; the CLEdge list.
 //   l3d_rdd           : replicator_dynamics_diffusion_GPU (cudawrapper.cu:708-766) on CSR/CSC SoA arrays instead of two
 //                       AoS float4 COO copies: 20 B/nnz/iteration of compulsory traffic instead of >= 64.  The arithmetic
 //                       (positional lock-step product, per-row sequential sums, clamps) is kept operation for operation,
@@ -55,114 +57,115 @@ struct SwStore {
 // depths of the best match of global segment g (its estimate), b = est_best[g]
 __device__ __forceinline__ float4 sw_best_depths(const SwStore& M, int view, int b) { return sw_depths(M.e_val[M.vt[view].region_off + b], M.recs); }
 
+// Parameters of the candidate kernels.  kx[0, K) are the kept matches in emission order: regions in processing order, each one
+// segment-major (l3d_sweep.cuh), so the kept matches of a segment are consecutive and lie within its ranges[] entry.
+struct AffArgs {
+    const L3DViewDev* views; const int* order; const long long* region_off; int V;     // order, region_off: per processing rank
+    SwStore M;
+    const int* est_best; const double* est_P; const int2* ranges;
+    const long long* kx; long long K;
+    const long long* cptr; const int* cidx;             // collinear lists, CSR over global segments; null: links off
+    float two_sigA_sqr, med_scene_depth_lines, min_affinity;
+};
+
+// kept match q: source segment gi in view v1, target gj in view v2, their similarity if both have an estimate, and whether it
+// exceeds min_affinity
+struct AffMatch { int v1, v2; long long gi, gj; float sim; bool pass; };
+__device__ __forceinline__ AffMatch aff_match(const AffArgs& a, long long q)
+{
+    const long long x = a.kx[q];
+    const SwEntry me = sw_decode(a.M.e_val[x], a.M.pairs, a.M.row_off, a.M.num_pairs, a.M.knn, a.M.recs);
+    AffMatch m;
+    m.v1 = a.order[last_le(a.V, x, [&](int i) { return a.region_off[i]; })];          // the view whose region contains x
+    m.v2 = me.tgt_view;
+    m.gi = a.views[m.v1].seg_off + me.seg; m.gj = a.views[m.v2].seg_off + me.tgt_seg;
+    const int b1 = a.est_best[m.gi], b2 = a.est_best[m.gj];
+    m.sim = 0.0f; m.pass = false;
+    if (b1 >= 0 && b2 >= 0) {
+        m.sim = aff_similarity(a.views + m.v1, a.views + m.v2, a.est_P + 6 * m.gi, a.est_P + 6 * m.gj, sw_best_depths(a.M, m.v1, b1),
+                               sw_best_depths(a.M, m.v2, b2), a.two_sigA_sqr, a.med_scene_depth_lines);
+        m.pass = m.sim > a.min_affinity;
+    }
+    return m;
+}
+
+// The links of estimate gs (view v1) through segment g of view v: the segments collinear with g that have an estimate and a
+// similarity with gs above min_affinity, in list order (line3D.cc:1904-1937 with g the target, 1941-1974 with g = gs).
+// emit(g2, sim) for each; returns their number.
+template <class Emit>
+__device__ __forceinline__ int aff_links(const AffArgs& a, int v1, long long gs, int v, long long g, Emit&& emit)
+{
+    const long long k0 = a.cptr[g], k1 = a.cptr[g + 1];
+    if (k0 == k1) return 0;
+    const float4 m1 = sw_best_depths(a.M, v1, a.est_best[gs]);
+    const L3DViewDev* vg = a.views + v;
+    int n = 0;
+    for (long long k = k0; k < k1; ++k) {
+        const long long g2 = vg->seg_off + a.cidx[k];
+        const int b2 = a.est_best[g2];
+        if (b2 < 0) continue;
+        const float s = aff_similarity(a.views + v1, vg, a.est_P + 6 * gs, a.est_P + 6 * g2, m1, sw_best_depths(a.M, v, b2), a.two_sigA_sqr,
+                                       a.med_scene_depth_lines);
+        if (s > a.min_affinity) { emit(g2, s); ++n; }
+    }
+    return n;
+}
+
+// The links through source gi (view v1) follow kept match q's events if q is gi's last kept match and one of gi's kept matches
+// passed: passed(p) for p = q, q - 1, ... down to gi's first.
+template <class Passed>
+__device__ __forceinline__ bool aff_source_links_after(const AffArgs& a, long long q, int v1, long long gi, Passed&& passed)
+{
+    const long long ro = a.M.vt[v1].region_off;
+    const int2 r = a.ranges[gi];
+    if (q + 1 < a.K && a.kx[q + 1] <= ro + r.y) return false;
+    for (long long p = q; p >= 0 && a.kx[p] >= ro + r.x; --p)
+        if (passed(p)) return true;
+    return false;
+}
+
+// Candidates, count: one thread per kept match writes its similarity, segments and pass flag and, with links, its number of
+// events: the direct edge and the links through the target if it passes, then the links through the source if aff_source_links_after.
+// Without links the pass flag is the count.  LINKS == (a.cptr != null), a template argument so that the instantiation without links
+// has only the registers it needs (76, as many as the similarity alone; 96 with links).
+template <bool LINKS>
 __global__ void __launch_bounds__(256)
-k_affinity(const L3DViewDev* __restrict__ views, const long long* __restrict__ region_off, const int* __restrict__ order,
-           int V, long long K, const long long* __restrict__ kx, const SwStore M, const int* __restrict__ est_best,
-           const double* __restrict__ est_P, float two_sigA_sqr, float med_scene_depth_lines, float min_affinity,
-           float* __restrict__ sim_out, int* __restrict__ flag_out, long long* __restrict__ gi_out, long long* __restrict__ gj_out)
+k_aff_count(const AffArgs a, float* __restrict__ sim, int* __restrict__ flag, long long* __restrict__ gi, long long* __restrict__ gj,
+            int* __restrict__ cnt)
 {
     const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (q >= K) return;
-    const long long x = kx[q];                   // the q-th kept match in emission order
-    int flag = 0; float sim = 0.0f; long long gi = -1, gj = -1;
-    {
-        const int v1i = order[last_le(V, x, [&](int i) { return region_off[i]; })];      // the view whose region contains x
-        const SwEntry me = sw_decode(M.e_val[x], M.pairs, M.row_off, M.num_pairs, M.knn, M.recs);
-        const L3DViewDev* v1 = views + v1i;
-        const L3DViewDev* v2 = views + me.tgt_view;
-        gi = v1->seg_off + me.seg; gj = v2->seg_off + me.tgt_seg;
-        const int b1 = est_best[gi], b2 = est_best[gj];
-        if (b1 >= 0 && b2 >= 0) {
-            sim = aff_similarity(v1, v2, est_P + 6 * gi, est_P + 6 * gj, sw_best_depths(M, v1i, b1), sw_best_depths(M, me.tgt_view, b2),
-                                 two_sigA_sqr, med_scene_depth_lines);
-            flag = sim > min_affinity ? 1 : 0;
-        }
-    }
-    sim_out[q] = sim; flag_out[q] = flag; gi_out[q] = gi; gj_out[q] = gj;
+    if (q >= a.K) return;
+    const AffMatch m = aff_match(a, q);
+    sim[q] = m.sim; flag[q] = m.pass ? 1 : 0; gi[q] = m.gi; gj[q] = m.gj;
+    if (!LINKS) return;
+    const auto none = [](long long, float) {};
+    int n = m.pass ? 1 + aff_links(a, m.v1, m.gi, m.v2, m.gj, none) : 0;
+    if (aff_source_links_after(a, q, m.v1, m.gi, [&](long long p) { return p == q ? m.pass : aff_match(a, p).pass; }))
+        n += aff_links(a, m.v1, m.gi, m.v1, m.gi, none);
+    cnt[q] = n;
 }
 
-// ---- affinity candidates WITH collinearity links (line3D.cc:1904-1974), one thread per segment in estimate order ----
-// Events of estimate i, in the reference's order: for every kept match with sim > min_affinity the direct edge, then one
-// edge to every segment collinear with the match's target (if that one has an estimate and sim > min_affinity); after
-// the matches, if any direct edge exists, the edges to the segments collinear with i itself.  Whether an event really
-// enters A_ depends on unused() and, for the collinear ones, on their parent having passed unused() - that is resolved
-// by l3d_affinity_matrix.  par: -1 direct, >= 0 index of the parent direct event, -2 "any direct event of my source".
-// FILL = false counts (evcnt[t]); FILL = true writes at evptr[t].
-template <bool FILL>
-__global__ void __launch_bounds__(128)
-k_aff_events(const L3DViewDev* __restrict__ views, const long long* __restrict__ region_off, const int* __restrict__ order,
-             const long long* __restrict__ segrank_off, int V, long long N, const SwStore M,
-             const int2* __restrict__ ranges, const int* __restrict__ est_best, const double* __restrict__ est_P,
-             long long K, const long long* __restrict__ kx, const float* __restrict__ sim_slot, const int* __restrict__ flag_slot, const long long* __restrict__ cptr,
-             const int* __restrict__ cidx, float two_sigA_sqr, float med_scene_depth_lines, float min_affinity, int* __restrict__ evcnt,
-             const long long* __restrict__ evptr, long long* __restrict__ out_i, long long* __restrict__ out_j, float* __restrict__ out_w,
-             int* __restrict__ out_par)
-{
-    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= N) return;
-    const int lo = last_le(V, t, [&](int i) { return segrank_off[i]; });          // processing rank of segment t
-    const int v1i = order[lo];
-    const L3DViewDev* v1 = views + v1i;
-    const long long g = v1->seg_off + (t - segrank_off[lo]);
-    const int b1 = est_best[g];
-    long long n = 0;
-    const long long base = FILL ? evptr[t] : 0;
-    if (b1 >= 0) {
-        const long long ro = region_off[lo];
-        const int2 rng = ranges[g];
-        const double* P1 = est_P + 6 * g;
-        const float4 m1 = sw_best_depths(M, v1i, b1);
-        bool found = false;
-        long long q = 0;
-        if (rng.x >= 0) {                        // first kept match of this segment in the compact list
-            long long a = 0, b = K;
-            while (a < b) { const long long mid = (a + b) >> 1; if (kx[mid] < ro + rng.x) a = mid + 1; else b = mid; }
-            q = a;
-        }
-        for (; rng.x >= 0 && q < K && kx[q] <= ro + rng.y; ++q) {
-            const long long x = kx[q];
-            if (!flag_slot[q]) continue;
-            const SwEntry me = sw_decode(M.e_val[x], M.pairs, M.row_off, M.num_pairs, M.knn, M.recs);
-            const L3DViewDev* v2 = views + me.tgt_view;
-            const long long gj = v2->seg_off + me.tgt_seg;
-            const long long parent = base + n;
-            if (FILL) { out_i[parent] = g; out_j[parent] = gj; out_w[parent] = sim_slot[q]; out_par[parent] = -1; }
-            ++n; found = true;
-            for (long long q = cptr[gj]; q < cptr[gj + 1]; ++q) {                  // collinear with the target (line3D.cc:1904-1937)
-                const long long g2 = v2->seg_off + cidx[q];
-                const int b2 = est_best[g2];
-                if (b2 < 0) continue;
-                const float s2 = aff_similarity(v1, v2, P1, est_P + 6 * g2, m1, sw_best_depths(M, me.tgt_view, b2), two_sigA_sqr, med_scene_depth_lines);
-                if (s2 > min_affinity) {
-                    if (FILL) { out_i[base + n] = g; out_j[base + n] = g2; out_w[base + n] = s2; out_par[base + n] = (int)parent; }
-                    ++n;
-                }
-            }
-        }
-        if (found)
-            for (long long q = cptr[g]; q < cptr[g + 1]; ++q) {                    // collinear with the source (line3D.cc:1941-1974)
-                const long long g2 = v1->seg_off + cidx[q];
-                const int b2 = est_best[g2];
-                if (b2 < 0) continue;
-                const float s2 = aff_similarity(v1, v1, P1, est_P + 6 * g2, m1, sw_best_depths(M, v1i, b2), two_sigA_sqr, med_scene_depth_lines);
-                if (s2 > min_affinity) {
-                    if (FILL) { out_i[base + n] = g; out_j[base + n] = g2; out_w[base + n] = s2; out_par[base + n] = -2; }
-                    ++n;
-                }
-            }
-    }
-    if (!FILL) evcnt[t] = (int)n;
-}
-
+// Candidates, fill: kept match q writes its events from evptr[q] on, in k_aff_count's order, and with links each one's parent:
+// -1 the direct edge, >= 0 the direct edge a link through the target belongs to, -2 "some direct edge of my source".
+template <bool LINKS>
 __global__ void __launch_bounds__(256)
-k_affinity_compact(long long total, const int* __restrict__ flag, const long long* __restrict__ pos, const float* __restrict__ sim,
-                   const long long* __restrict__ gi, const long long* __restrict__ gj, long long* __restrict__ out_i,
-                   long long* __restrict__ out_j, float* __restrict__ out_w)
+k_aff_fill(const AffArgs a, const float* __restrict__ sim, const int* __restrict__ flag, const long long* __restrict__ gi,
+           const long long* __restrict__ gj, const long long* __restrict__ evptr, long long* __restrict__ out_i, long long* __restrict__ out_j,
+           float* __restrict__ out_w, int* __restrict__ out_par)
 {
-    const long long x = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (x >= total || !flag[x]) return;
-    const long long p = pos[x];
-    out_i[p] = gi[x]; out_j[p] = gj[x]; out_w[p] = sim[x];
+    const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= a.K || (!LINKS && !flag[q])) return;
+    const long long g = gi[q], e0 = evptr[q];
+    long long e = e0;
+    const auto put = [&](long long j, float w, int par) { out_i[e] = g; out_j[e] = j; out_w[e] = w; if (LINKS) out_par[e] = par; ++e; };
+    const auto view_of = [&](long long s) { return last_le(a.V, s, [&](int i) { return a.views[i].seg_off; }); };
+    const int v1 = view_of(g);
+    if (flag[q]) {
+        put(gj[q], sim[q], -1);
+        if (LINKS) aff_links(a, v1, g, view_of(gj[q]), gj[q], [&](long long g2, float s) { put(g2, s, (int)e0); });
+    }
+    if (LINKS && aff_source_links_after(a, q, v1, g, [&](long long p) { return flag[p] != 0; }))
+        aff_links(a, v1, g, v1, g, [&](long long g2, float s) { put(g2, s, -2); });
 }
 
 // ================================================================================================ diffusion
@@ -431,118 +434,170 @@ __global__ void __launch_bounds__(256) k_aff_emit(long long ne, const int* __res
 
 struct KeptFlag { const unsigned char* f; __host__ __device__ int operator()(long long x) const { return (f[x] & SW_KEPT) ? 1 : 0; } };
 
-extern "C" {
-
-// device part shared by l3d_affinity_edges / l3d_affinity_matrix: similarities of all kept matches, then the candidates with
-// sim > min_affinity compacted IN EMISSION ORDER into A.d_aff_oi / oj / ow.  Returns their number (or < 0).
-static long long affinity_candidates(l3d_ctx* c, float two_sigA_sqr, float med_scene_depth_lines, float min_affinity)
+// ---- the steps of l3d_affinity_matrix; l3d_affinity_edges takes the first two ----------------------------------------------------
+// the kept matches (filterMatches survivors) in emission order into A.d_kx: everything below works on this list, not on the whole
+// match store (2.5e9 entries at BASELINE configs[4])
+static int kept_list(l3d_ctx* c, long long* n_kept)
 {
-    SweepState& S = c->sweep;
-    AffinityState& A = c->aff;
-    const long long total = S.total;
-    if (total == 0) return 0;
-    const int V = c->num_views;
-    int rc;
-    DevBuf &d_sim = A.d_aff_sim, &d_flag = A.d_aff_flag, &d_gi = A.d_aff_gi, &d_gj = A.d_aff_gj, &d_pos = A.d_aff_pos;
-    cudaStream_t st = c->stream;
-    // the kept matches (filterMatches survivors), compacted in emission order: everything below works on this list, not on the
-    // whole match store (2.5e9 entries at BASELINE configs[4])
-    const long long BLK = 1ll << 30;
-    long long K = 0;
-    L3D_RESERVE(d_pos, 16, "kept count");
+    SweepState& S = c->sweep; AffinityState& A = c->aff; cudaStream_t st = c->stream; int rc;
+    const long long total = S.total, BLK = 1ll << 30; long long K = 0;
+    DevBuf& d_cnt = A.d_evptr;               // scratch for the counts until the candidates write the event offsets
+    L3D_RESERVE(d_cnt, 16, "kept count");
     std::vector<long long> kept_in_block;
     for (long long base = 0; base < total; base += BLK) {
         const int nblk = (int)std::min(BLK, total - base);
         cub::CountingInputIterator<long long> idx(base);
         cub::TransformInputIterator<int, KeptFlag, cub::CountingInputIterator<long long> > flags(idx, KeptFlag{(const unsigned char*)S.d_eflag.p});
-        if ((rc = l3d_cub(c, "kept count", [&](void* tmp, size_t& bytes) { return cub::DeviceReduce::Sum(tmp, bytes, flags, (int*)d_pos.p, nblk, st); }))) return rc;
+        if ((rc = l3d_cub(c, "kept count", [&](void* tmp, size_t& bytes) { return cub::DeviceReduce::Sum(tmp, bytes, flags, (int*)d_cnt.p, nblk, st); }))) return rc;
         int cnt = 0;
-        L3D_CUDA(c, cudaMemcpyAsync(&cnt, d_pos.p, 4, cudaMemcpyDeviceToHost, st), "kept count");
+        L3D_CUDA(c, cudaMemcpyAsync(&cnt, d_cnt.p, 4, cudaMemcpyDeviceToHost, st), "kept count");
         L3D_CUDA(c, cudaStreamSynchronize(st), "kept count");
         kept_in_block.push_back(cnt); K += cnt;
     }
-    A.n_kept = K;
-    if (K == 0) return 0;
+    *n_kept = K;
+    if (K == 0) return L3D_OK;
     L3D_RESERVE(A.d_kx, 8 * K, "kept list");
-    {
-        long long done = 0; size_t bi = 0;
-        for (long long base = 0; base < total; base += BLK, ++bi) {
-            const int nblk = (int)std::min(BLK, total - base);
-            if (kept_in_block[bi] == 0) continue;
-            cub::CountingInputIterator<long long> idx(base);
-            cub::TransformInputIterator<int, KeptFlag, cub::CountingInputIterator<long long> > flags(idx, KeptFlag{(const unsigned char*)S.d_eflag.p});
-            if ((rc = l3d_cub(c, "kept list", [&](void* tmp, size_t& bytes) {
-                     return cub::DeviceSelect::Flagged(tmp, bytes, idx, flags, (long long*)A.d_kx.p + done, (int*)d_pos.p, nblk, st); }))) return rc;
-            done += kept_in_block[bi];
-        }
-        c->launches += 2 * (long long)kept_in_block.size();
+    long long done = 0; size_t bi = 0;
+    for (long long base = 0; base < total; base += BLK, ++bi) {
+        const int nblk = (int)std::min(BLK, total - base);
+        if (kept_in_block[bi] == 0) continue;
+        cub::CountingInputIterator<long long> idx(base);
+        cub::TransformInputIterator<int, KeptFlag, cub::CountingInputIterator<long long> > flags(idx, KeptFlag{(const unsigned char*)S.d_eflag.p});
+        if ((rc = l3d_cub(c, "kept list", [&](void* tmp, size_t& bytes) {
+                 return cub::DeviceSelect::Flagged(tmp, bytes, idx, flags, (long long*)A.d_kx.p + done, (int*)d_cnt.p, nblk, st); }))) return rc;
+        done += kept_in_block[bi];
     }
-    L3D_RESERVE(d_sim, 4 * K, "affinity sims"); L3D_RESERVE(d_flag, 4 * K, "affinity flags");
-    L3D_RESERVE(d_gi, 8 * K, "affinity gi"); L3D_RESERVE(d_gj, 8 * K, "affinity gj"); L3D_RESERVE(d_pos, 8 * (K + 1), "affinity pos");
-    std::vector<int> rank_of_view(V);
-    for (int i = 0; i < V; ++i) rank_of_view[S.order[i]] = i;
-    L3D_RESERVE(S.d_order, 4 * V, "order"); L3D_RESERVE(A.d_rankofview, 4 * V, "rank of view"); L3D_RESERVE(S.d_region_off, 8 * (V + 1), "region offsets");
+    c->launches += 2 * (long long)kept_in_block.size();
+    return L3D_OK;
+}
+
+// The kept matches with sim > min_affinity and, with collinearity links on, their links (line3D.cc:1904-1974): the candidates in
+// emission order into A.d_aff_oi / oj / ow (and their parents into A.d_aff_par), by count, one scan, fill.  Returns their number (or < 0).
+static long long affinity_candidates(l3d_ctx* c, float two_sigA_sqr, float med_scene_depth_lines, float min_affinity)
+{
+    SweepState& S = c->sweep; AffinityState& A = c->aff; const CollinState& CL = c->collin; cudaStream_t st = c->stream; int rc;
+    const int V = c->num_views; long long K = 0;
+    if ((rc = kept_list(c, &K)) || K == 0) return rc;
+    L3D_RESERVE(A.d_aff_sim, 4 * K, "affinity sims"); L3D_RESERVE(A.d_aff_flag, 4 * K, "affinity flags");
+    L3D_RESERVE(A.d_aff_gi, 8 * K, "affinity gi"); L3D_RESERVE(A.d_aff_gj, 8 * K, "affinity gj"); L3D_RESERVE(A.d_evptr, 8 * K, "event offsets");
+    if (CL.valid) L3D_RESERVE(A.d_aff_cnt, 4 * K, "event counts");
+    L3D_RESERVE(S.d_order, 4 * V, "order"); L3D_RESERVE(S.d_region_off, 8 * (V + 1), "region offsets");
     L3D_CUDA(c, cudaMemcpyAsync(S.d_order.p, S.order.data(), 4 * (size_t)V, cudaMemcpyHostToDevice, st), "order");
-    L3D_CUDA(c, cudaMemcpyAsync(A.d_rankofview.p, rank_of_view.data(), 4 * (size_t)V, cudaMemcpyHostToDevice, st), "rank of view");
     L3D_CUDA(c, cudaMemcpyAsync(S.d_region_off.p, S.region_off.data(), 8 * (size_t)(V + 1), cudaMemcpyHostToDevice, st), "region offsets");
+    const AffArgs a = {c->views(), (const int*)S.d_order.p, (const long long*)S.d_region_off.p, V,
+                       {(const SwView*)S.d_vt.p, (const L3DPairDev*)c->d_pairs.p, (const long long*)S.d_rowoff.p, c->num_pairs, c->knn,
+                        (const l3d_match_rec*)c->d_recs.p, (const unsigned int*)S.d_eval.p, (const unsigned char*)S.d_eflag.p},
+                       (const int*)S.d_est_best.p, (const double*)S.d_est_P.p, (const int2*)S.d_ranges.p, (const long long*)A.d_kx.p, K,
+                       CL.valid ? (const long long*)CL.d_ptr.p : nullptr, CL.valid ? (const int*)CL.d_idx.p : nullptr,
+                       two_sigA_sqr, med_scene_depth_lines, min_affinity};
     const unsigned int nb = (unsigned int)((K + 255) / 256);
-    SwStore M;
-    M.vt = (const SwView*)S.d_vt.p; M.pairs = (const L3DPairDev*)c->d_pairs.p; M.row_off = (const long long*)S.d_rowoff.p; M.num_pairs = c->num_pairs; M.knn = c->knn;
-    M.recs = (const l3d_match_rec*)c->d_recs.p; M.e_val = (const unsigned int*)S.d_eval.p; M.e_flag = (const unsigned char*)S.d_eflag.p;
-    k_affinity<<<nb, 256, 0, st>>>(c->views(), (const long long*)S.d_region_off.p, (const int*)S.d_order.p, V, K, (const long long*)A.d_kx.p, M, (const int*)S.d_est_best.p,
-                                   (const double*)S.d_est_P.p, two_sigA_sqr, med_scene_depth_lines, min_affinity, (float*)d_sim.p, (int*)d_flag.p,
-                                   (long long*)d_gi.p, (long long*)d_gj.p);
-    if (c->collin.valid) {
-        // collinearity links on: events per segment in estimate order (count, scan, fill), each with its parent
-        const CollinState& CL = c->collin;
-        const long long N = c->total_segs;
-        std::vector<long long> segrank_off((size_t)V + 1, 0);
-        for (int i = 0; i < V; ++i) segrank_off[i + 1] = segrank_off[i] + c->h_views[S.order[i]].nseg;
-        L3D_RESERVE(A.d_segrank_off, 8 * (V + 1), "segment rank offsets");
-        L3D_RESERVE(A.d_evcnt, 4 * (N + 1), "event counts"); L3D_RESERVE(A.d_evptr, 8 * (N + 1), "event offsets");
-        L3D_CUDA(c, cudaMemcpyAsync(A.d_segrank_off.p, segrank_off.data(), 8 * ((size_t)V + 1), cudaMemcpyHostToDevice, st), "segment rank offsets");
-        L3D_CUDA(c, cudaMemsetAsync(A.d_evcnt.p, 0, 4 * (size_t)(N + 1), st), "event counts");
-        const unsigned int nbs = (unsigned int)((N + 127) / 128);
-#define EV_ARGS c->views(), (const long long*)S.d_region_off.p, (const int*)S.d_order.p, (const long long*)A.d_segrank_off.p, V, N, M,                      \
-                (const int2*)S.d_ranges.p, (const int*)S.d_est_best.p,                                                                                        \
-                (const double*)S.d_est_P.p, K, (const long long*)A.d_kx.p, (const float*)d_sim.p, (const int*)d_flag.p, (const long long*)CL.d_ptr.p,             \
-                (const int*)CL.d_idx.p, two_sigA_sqr,                                                                                                         \
-                med_scene_depth_lines, min_affinity
-        k_aff_events<false><<<nbs, 128, 0, st>>>(EV_ARGS, (int*)A.d_evcnt.p, nullptr, nullptr, nullptr, nullptr, nullptr);
-        if ((rc = l3d_cub(c, "event scan", [&](void* tmp, size_t& bytes) {
-                 return cub::DeviceScan::ExclusiveSum(tmp, bytes, (const int*)A.d_evcnt.p, (long long*)A.d_evptr.p, N + 1, st); }))) return rc;
-        long long nev = 0;
-        L3D_CUDA(c, cudaMemcpyAsync(&nev, (long long*)A.d_evptr.p + N, 8, cudaMemcpyDeviceToHost, st), "event count");
-        L3D_CUDA(c, cudaStreamSynchronize(st), "affinity events");
-        c->launches += 4;
-        if (nev == 0) return 0;
-        if (nev >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "affinity: more than 2^31 candidate events");
-        L3D_RESERVE(A.d_aff_oi, 8 * nev, "edges i"); L3D_RESERVE(A.d_aff_oj, 8 * nev, "edges j");
-        L3D_RESERVE(A.d_aff_ow, 4 * nev, "edges w"); L3D_RESERVE(A.d_aff_par, 4 * nev, "edge parents");
-        k_aff_events<true><<<nbs, 128, 0, st>>>(EV_ARGS, nullptr, (const long long*)A.d_evptr.p, (long long*)A.d_aff_oi.p, (long long*)A.d_aff_oj.p,
-                                                (float*)A.d_aff_ow.p, (int*)A.d_aff_par.p);
-#undef EV_ARGS
-        ++c->launches;
-        L3D_CUDA(c, cudaGetLastError(), "k_aff_events");
-        A.aff_has_parents = true;
-        return nev;
-    }
-    A.aff_has_parents = false;
-    if (K >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "affinity: more than 2^31 kept matches");
-    ScanTotal t;      // scan over the kept matches; the edge count is pos[K-1] + flag[K-1]
-    if ((rc = l3d_scan_total(c, (const int*)d_flag.p, (long long*)d_pos.p, (int)K, (const int*)d_flag.p, t, "affinity scan"))) return rc;
-    L3D_CUDA(c, cudaStreamSynchronize(st), "affinity");
-    const long long ne = t.last_out + t.last_src;
-    c->launches += 3;
-    if (ne == 0) return 0;
-    DevBuf &o_i = A.d_aff_oi, &o_j = A.d_aff_oj, &o_w = A.d_aff_ow;
-    L3D_RESERVE(o_i, 8 * ne, "edges i"); L3D_RESERVE(o_j, 8 * ne, "edges j"); L3D_RESERVE(o_w, 4 * ne, "edges w");
-    k_affinity_compact<<<nb, 256, 0, st>>>(K, (const int*)d_flag.p, (const long long*)d_pos.p, (const float*)d_sim.p, (const long long*)d_gi.p,
-                                           (const long long*)d_gj.p, (long long*)o_i.p, (long long*)o_j.p, (float*)o_w.p);
+    float* sim = (float*)A.d_aff_sim.p; int* flag = (int*)A.d_aff_flag.p; long long* gi = (long long*)A.d_aff_gi.p; long long* gj = (long long*)A.d_aff_gj.p;
+    int* cnt = CL.valid ? (int*)A.d_aff_cnt.p : flag;        // links off: an event per passing kept match
+    (CL.valid ? k_aff_count<true> : k_aff_count<false>)<<<nb, 256, 0, st>>>(a, sim, flag, gi, gj, cnt);
     ++c->launches;
-    L3D_CUDA(c, cudaGetLastError(), "k_affinity_compact");
+    ScanTotal t;
+    if ((rc = l3d_scan_total(c, (const int*)cnt, (long long*)A.d_evptr.p, K, cnt, t, "event scan"))) return rc;
+    c->launches += 2;
+    L3D_CUDA(c, cudaStreamSynchronize(st), "affinity events");
+    const long long ne = t.last_out + t.last_src;
+    if (ne == 0) return 0;
+    if (ne >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "affinity: more than 2^31 candidate events");
+    L3D_RESERVE(A.d_aff_oi, 8 * ne, "edges i"); L3D_RESERVE(A.d_aff_oj, 8 * ne, "edges j"); L3D_RESERVE(A.d_aff_ow, 4 * ne, "edges w");
+    if (CL.valid) L3D_RESERVE(A.d_aff_par, 4 * ne, "edge parents");
+    (CL.valid ? k_aff_fill<true> : k_aff_fill<false>)<<<nb, 256, 0, st>>>(a, sim, flag, gi, gj, (const long long*)A.d_evptr.p, (long long*)A.d_aff_oi.p,
+                                                                        (long long*)A.d_aff_oj.p, (float*)A.d_aff_ow.p, (int*)A.d_aff_par.p);
+    ++c->launches;
+    L3D_CUDA(c, cudaGetLastError(), "k_aff_fill");
     return ne;
 }
+
+// unused() (line3D.cc:1982-2002) into A.d_keep: the candidates stably sorted by unordered segment pair, then the fixpoint over the
+// conditional events (see k_aff_round)
+static int unused_fixpoint(l3d_ctx* c, long long ne)
+{
+    AffinityState& A = c->aff; const long long N = c->total_segs; cudaStream_t st = c->stream; int rc;
+    const unsigned int nbe = (unsigned int)((ne + 255) / 256); const long long* oi = (const long long*)A.d_aff_oi.p;
+    L3D_RESERVE(A.d_key, 8 * ne, "pair keys"); L3D_RESERVE(A.d_key2, 8 * ne, "pair keys"); L3D_RESERVE(A.d_val, 4 * ne, "pair vals"); L3D_RESERVE(A.d_val2, 4 * ne, "pair vals");
+    L3D_RESERVE(A.d_keep, 4 * ne, "keep flags"); L3D_RESERVE(A.d_keep2, 4 * ne, "keep flags"); L3D_RESERVE(A.d_found, 4 * N, "found flags"); L3D_RESERVE(A.d_changed, 16, "changed flag");
+    k_aff_keys<<<nbe, 256, 0, st>>>(ne, oi, (const long long*)A.d_aff_oj.p, (unsigned long long*)A.d_key.p, (unsigned int*)A.d_val.p);
+    ++c->launches;
+    if ((rc = l3d_cub(c, "pair sort", [&](void* tmp, size_t& bytes) {
+             return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const unsigned long long*)A.d_key.p, (unsigned long long*)A.d_key2.p, (const unsigned int*)A.d_val.p,
+                                                    (unsigned int*)A.d_val2.p, (int)ne, 0, 32 + bits_i64(N), st); }))) return rc;
+    c->launches += 8;
+    // without collinearity links every event is direct: one round, the head of every run of the sort
+    const int* par = c->collin.valid ? (const int*)A.d_aff_par.p : nullptr;
+    L3D_CUDA(c, cudaMemsetAsync(A.d_keep.p, 0, 4 * ne, st), "clear keep");
+    L3D_CUDA(c, cudaMemsetAsync(A.d_found.p, 0, 4 * N, st), "clear found");
+    int* acc_prev = (int*)A.d_keep.p; int* acc_new = (int*)A.d_keep2.p;
+    for (int round = 0;; ++round) {
+        if (round > 100000) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_affinity_matrix: unused() fixpoint did not converge");
+        L3D_CUDA(c, cudaMemsetAsync(A.d_changed.p, 0, 4, st), "clear changed");
+        k_aff_round<<<nbe, 256, 0, st>>>(ne, (const unsigned long long*)A.d_key2.p, (const unsigned int*)A.d_val2.p, par, oi,
+                                         acc_prev, (const int*)A.d_found.p, acc_new, (int*)A.d_changed.p);
+        std::swap(acc_prev, acc_new);
+        ++c->launches;
+        if (!par) break;
+        L3D_CUDA(c, cudaMemsetAsync(A.d_found.p, 0, 4 * N, st), "clear found");
+        k_aff_found<<<nbe, 256, 0, st>>>(ne, par, oi, acc_prev, (int*)A.d_found.p);
+        ++c->launches;
+        int changed = 0;
+        L3D_CUDA(c, cudaMemcpyAsync(&changed, A.d_changed.p, 4, cudaMemcpyDeviceToHost, st), "changed flag");
+        L3D_CUDA(c, cudaStreamSynchronize(st), "affinity fixpoint");
+        if (!changed) break;
+    }
+    if (acc_prev != (int*)A.d_keep.p) L3D_CUDA(c, cudaMemcpyAsync(A.d_keep.p, acc_prev, 4 * ne, cudaMemcpyDeviceToDevice, st), "keep flags");
+    return L3D_OK;
+}
+
+// getLocalID (line3D.cc:2005-2023): A.d_q = position of every accepted candidate among the accepted ones (A.K of them), local ids
+// in order of first appearance, the source of an edge before its target (A.d_idof, A.d_l2g, A.n_ids of them)
+static int local_ids(l3d_ctx* c, long long ne)
+{
+    AffinityState& A = c->aff; const long long N = c->total_segs; cudaStream_t st = c->stream; int rc;
+    const unsigned int nbe = (unsigned int)((ne + 255) / 256), nbn = (unsigned int)((N + 255) / 256);
+    L3D_RESERVE(A.d_q, 8 * (ne + 1), "edge positions"); L3D_RESERVE(A.d_time, 8 * N, "appearance times");
+    L3D_RESERVE(A.d_nflag, 4 * N, "node flags"); L3D_RESERVE(A.d_npos, 8 * (N + 1), "node positions"); L3D_RESERVE(A.d_idof, 4 * N, "id of segment");
+    if ((rc = l3d_cub(c, "edge scan", [&](void* tmp, size_t& bytes) {
+             return cub::DeviceScan::ExclusiveSum(tmp, bytes, (const int*)A.d_keep.p, (long long*)A.d_q.p, ne, st); }))) return rc;
+    c->launches += 2;
+    L3D_CUDA(c, cudaMemsetAsync(A.d_time.p, 0xFF, 8 * N, st), "init times");
+    k_aff_time<<<nbe, 256, 0, st>>>(ne, (const int*)A.d_keep.p, (const long long*)A.d_q.p, (const long long*)A.d_aff_oi.p, (const long long*)A.d_aff_oj.p,
+                                    (unsigned long long*)A.d_time.p);
+    k_aff_nodeflags<<<nbn, 256, 0, st>>>(N, (const unsigned long long*)A.d_time.p, (int*)A.d_nflag.p);
+    c->launches += 2;
+    ScanTotal edges, nodes;         // both totals under one synchronisation
+    if ((rc = l3d_scan_total(c, (const int*)A.d_nflag.p, (long long*)A.d_npos.p, N, (const int*)A.d_nflag.p, nodes, "node scan"))) return rc;
+    c->launches += 2;
+    if ((rc = l3d_read_total(c, (const long long*)A.d_q.p, (const int*)A.d_keep.p, ne, edges, "edge count"))) return rc;
+    L3D_CUDA(c, cudaStreamSynchronize(st), "affinity matrix");
+    A.K = edges.last_out + edges.last_src; A.n_ids = nodes.last_out + nodes.last_src;
+    L3D_RESERVE(A.d_nkey, 8 * A.n_ids, "node keys"); L3D_RESERVE(A.d_nkey2, 8 * A.n_ids, "node keys"); L3D_RESERVE(A.d_nval, 4 * A.n_ids, "node vals");
+    L3D_RESERVE(A.d_nval2, 4 * A.n_ids, "node vals"); L3D_RESERVE(A.d_l2g, 8 * A.n_ids, "local2global");
+    k_aff_nodes<<<nbn, 256, 0, st>>>(N, (const int*)A.d_nflag.p, (const long long*)A.d_npos.p, (const unsigned long long*)A.d_time.p, (unsigned long long*)A.d_nkey.p, (unsigned int*)A.d_nval.p);
+    ++c->launches;
+    if ((rc = l3d_cub(c, "node sort", [&](void* tmp, size_t& bytes) {
+             return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const unsigned long long*)A.d_nkey.p, (unsigned long long*)A.d_nkey2.p, (const unsigned int*)A.d_nval.p,
+                                                    (unsigned int*)A.d_nval2.p, (int)A.n_ids, 0, 64, st); }))) return rc;
+    c->launches += 8;
+    k_aff_ids<<<(unsigned int)((A.n_ids + 255) / 256), 256, 0, st>>>(A.n_ids, (const unsigned int*)A.d_nval2.p, (int*)A.d_idof.p, (long long*)A.d_l2g.p);
+    ++c->launches;
+    return L3D_OK;
+}
+
+// the CLEdge list: (id1, id2, w), (id2, id1, w) per accepted edge, in emission order
+static int emit_edges(l3d_ctx* c, long long ne)
+{
+    AffinityState& A = c->aff; int rc;
+    L3D_RESERVE(A.d_ei, 4 * 2 * A.K, "A i"); L3D_RESERVE(A.d_ej, 4 * 2 * A.K, "A j"); L3D_RESERVE(A.d_ew, 4 * 2 * A.K, "A w");
+    k_aff_emit<<<(unsigned int)((ne + 255) / 256), 256, 0, c->stream>>>(ne, (const int*)A.d_keep.p, (const long long*)A.d_q.p, (const long long*)A.d_aff_oi.p,
+                                                                      (const long long*)A.d_aff_oj.p, (const float*)A.d_aff_ow.p, (const int*)A.d_idof.p,
+                                                                      (int*)A.d_ei.p, (int*)A.d_ej.p, (float*)A.d_ew.p);
+    ++c->launches;
+    return L3D_OK;
+}
+
+extern "C" {
 
 // Affinity edges between segments with 3D estimates, in the reference's emission order (estimate order, then match
 // list order), BEFORE the "unused" de-duplication and local-id assignment (line3D.cc:1881-1900).
@@ -583,69 +638,14 @@ long long l3d_affinity_matrix(l3d_ctx* c, float two_sigA_sqr, float med_scene_de
     if (!c->sweep.valid) return l3d_fail(c, L3D_ERR_STATE, "l3d_affinity_matrix: call l3d_score_sweep first");
     cudaSetDevice(c->device);
     cudaStream_t st = c->stream;
-    int rc;
     if (!cached) {
         const long long ne = affinity_candidates(c, two_sigA_sqr, med_scene_depth_lines, min_affinity);
         if (ne < 0) return ne;
         A.K = 0; A.n_ids = 0;
         if (ne > 0) {
             if (ne >= (1ll << 32) || c->total_segs >= (1ll << 32)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_affinity_matrix: more than 2^32 candidates / segments");
-            const long long N = c->total_segs;
-            L3D_RESERVE(A.d_key, 8 * ne, "pair keys"); L3D_RESERVE(A.d_key2, 8 * ne, "pair keys"); L3D_RESERVE(A.d_val, 4 * ne, "pair vals"); L3D_RESERVE(A.d_val2, 4 * ne, "pair vals");
-            L3D_RESERVE(A.d_keep, 4 * ne, "keep flags"); L3D_RESERVE(A.d_q, 8 * (ne + 1), "edge positions"); L3D_RESERVE(A.d_time, 8 * N, "appearance times");
-            L3D_RESERVE(A.d_nflag, 4 * N, "node flags"); L3D_RESERVE(A.d_npos, 8 * (N + 1), "node positions"); L3D_RESERVE(A.d_idof, 4 * N, "id of segment");
-            const int bseg = bits_i64(N);
-            const unsigned int nbe = (unsigned int)((ne + 255) / 256), nbn = (unsigned int)((N + 255) / 256);
-            const long long* oi = (const long long*)A.d_aff_oi.p; const long long* oj = (const long long*)A.d_aff_oj.p;
-            k_aff_keys<<<nbe, 256, 0, st>>>(ne, oi, oj, (unsigned long long*)A.d_key.p, (unsigned int*)A.d_val.p);
-            if ((rc = l3d_cub(c, "pair sort", [&](void* tmp, size_t& bytes) {
-                     return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const unsigned long long*)A.d_key.p, (unsigned long long*)A.d_key2.p, (const unsigned int*)A.d_val.p,
-                                                            (unsigned int*)A.d_val2.p, (int)ne, 0, 32 + bseg, st); }))) return rc;
-            {   // unused(): fixpoint over the conditional events (one round + one confirming round without collinearity links)
-                const int* par = A.aff_has_parents ? (const int*)A.d_aff_par.p : nullptr;
-                L3D_RESERVE(A.d_keep2, 4 * ne, "keep flags"); L3D_RESERVE(A.d_found, 4 * N, "found flags"); L3D_RESERVE(A.d_changed, 16, "changed flag");
-                L3D_CUDA(c, cudaMemsetAsync(A.d_keep.p, 0, 4 * ne, st), "clear keep");
-                L3D_CUDA(c, cudaMemsetAsync(A.d_found.p, 0, 4 * N, st), "clear found");
-                int* acc_prev = (int*)A.d_keep.p; int* acc_new = (int*)A.d_keep2.p;
-                for (int round = 0;; ++round) {
-                    if (round > 100000) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_affinity_matrix: unused() fixpoint did not converge");
-                    L3D_CUDA(c, cudaMemsetAsync(A.d_changed.p, 0, 4, st), "clear changed");
-                    k_aff_round<<<nbe, 256, 0, st>>>(ne, (const unsigned long long*)A.d_key2.p, (const unsigned int*)A.d_val2.p, par, oi,
-                                                     acc_prev, (const int*)A.d_found.p, acc_new, (int*)A.d_changed.p);
-                    std::swap(acc_prev, acc_new);
-                    ++c->launches;
-                    if (!par) break;                 // all events direct: the head of every run, final after one round
-                    L3D_CUDA(c, cudaMemsetAsync(A.d_found.p, 0, 4 * N, st), "clear found");
-                    k_aff_found<<<nbe, 256, 0, st>>>(ne, par, oi, acc_prev, (int*)A.d_found.p);
-                    int changed = 0;
-                    L3D_CUDA(c, cudaMemcpyAsync(&changed, A.d_changed.p, 4, cudaMemcpyDeviceToHost, st), "changed flag");
-                    L3D_CUDA(c, cudaStreamSynchronize(st), "affinity fixpoint");
-                    ++c->launches;
-                    if (!changed) break;
-                }
-                if (acc_prev != (int*)A.d_keep.p) L3D_CUDA(c, cudaMemcpyAsync(A.d_keep.p, acc_prev, 4 * ne, cudaMemcpyDeviceToDevice, st), "keep flags");
-            }
-            if ((rc = l3d_cub(c, "edge scan", [&](void* tmp, size_t& bytes) {
-                     return cub::DeviceScan::ExclusiveSum(tmp, bytes, (const int*)A.d_keep.p, (long long*)A.d_q.p, ne, st); }))) return rc;
-            L3D_CUDA(c, cudaMemsetAsync(A.d_time.p, 0xFF, 8 * N, st), "init times");
-            k_aff_time<<<nbe, 256, 0, st>>>(ne, (const int*)A.d_keep.p, (const long long*)A.d_q.p, oi, oj, (unsigned long long*)A.d_time.p);
-            k_aff_nodeflags<<<nbn, 256, 0, st>>>(N, (const unsigned long long*)A.d_time.p, (int*)A.d_nflag.p);
-            ScanTotal edges, nodes;         // both totals under one synchronisation
-            if ((rc = l3d_scan_total(c, (const int*)A.d_nflag.p, (long long*)A.d_npos.p, N, (const int*)A.d_nflag.p, nodes, "node scan"))) return rc;
-            if ((rc = l3d_read_total(c, (const long long*)A.d_q.p, (const int*)A.d_keep.p, ne, edges, "edge count"))) return rc;
-            L3D_CUDA(c, cudaStreamSynchronize(st), "affinity matrix");
-            A.K = edges.last_out + edges.last_src; A.n_ids = nodes.last_out + nodes.last_src;
-            L3D_RESERVE(A.d_nkey, 8 * A.n_ids, "node keys"); L3D_RESERVE(A.d_nkey2, 8 * A.n_ids, "node keys"); L3D_RESERVE(A.d_nval, 4 * A.n_ids, "node vals");
-            L3D_RESERVE(A.d_nval2, 4 * A.n_ids, "node vals"); L3D_RESERVE(A.d_l2g, 8 * A.n_ids, "local2global");
-            L3D_RESERVE(A.d_ei, 4 * 2 * A.K, "A i"); L3D_RESERVE(A.d_ej, 4 * 2 * A.K, "A j"); L3D_RESERVE(A.d_ew, 4 * 2 * A.K, "A w");
-            k_aff_nodes<<<nbn, 256, 0, st>>>(N, (const int*)A.d_nflag.p, (const long long*)A.d_npos.p, (const unsigned long long*)A.d_time.p, (unsigned long long*)A.d_nkey.p, (unsigned int*)A.d_nval.p);
-            if ((rc = l3d_cub(c, "node sort", [&](void* tmp, size_t& bytes) {
-                     return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const unsigned long long*)A.d_nkey.p, (unsigned long long*)A.d_nkey2.p, (const unsigned int*)A.d_nval.p,
-                                                            (unsigned int*)A.d_nval2.p, (int)A.n_ids, 0, 64, st); }))) return rc;
-            k_aff_ids<<<(unsigned int)((A.n_ids + 255) / 256), 256, 0, st>>>(A.n_ids, (const unsigned int*)A.d_nval2.p, (int*)A.d_idof.p, (long long*)A.d_l2g.p);
-            k_aff_emit<<<nbe, 256, 0, st>>>(ne, (const int*)A.d_keep.p, (const long long*)A.d_q.p, oi, oj, (const float*)A.d_aff_ow.p, (const int*)A.d_idof.p,
-                                            (int*)A.d_ei.p, (int*)A.d_ej.p, (float*)A.d_ew.p);
-            c->launches += 8 + 30;
+            int rc;
+            if ((rc = unused_fixpoint(c, ne)) || (rc = local_ids(c, ne)) || (rc = emit_edges(c, ne))) return rc;
             L3D_CUDA(c, cudaGetLastError(), "affinity matrix kernels");
         }
         A.valid = true; A.two_sigA_sqr = two_sigA_sqr; A.med = med_scene_depth_lines; A.min_aff = min_affinity;

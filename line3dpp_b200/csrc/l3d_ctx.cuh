@@ -34,14 +34,14 @@ struct SweepState {
     float ms_setup = 0.f, ms_chain = 0.f, ms_filter = 0.f;   // device time of the last sweep's three phases
 };
 
-// device state of the affinity-matrix bookkeeping (l3d_affinity.cu)
+// device state of the affinity matrix (l3d_affinity.cu), by step of l3d_affinity_matrix
 struct AffinityState {
     bool valid = false; float two_sigA_sqr = 0.f, med = 0.f, min_aff = 0.f; long long K = 0, n_ids = 0;
-    // candidate edges of the kept matches (affinity_candidates)
-    DevBuf d_aff_sim, d_aff_flag, d_aff_gi, d_aff_gj, d_aff_pos, d_aff_oi, d_aff_oj, d_aff_ow, d_aff_par, d_kx, d_rankofview, d_segrank_off, d_evcnt, d_evptr;
-    long long n_kept = 0;
-    bool aff_has_parents = false;           // d_aff_par valid: candidates carry parents (collinearity links)
-    DevBuf d_key, d_key2, d_val, d_val2, d_keep, d_keep2, d_found, d_changed, d_q, d_time, d_nflag, d_npos, d_idof, d_nkey, d_nkey2, d_nval, d_nval2, d_l2g, d_ei, d_ej, d_ew;
+    DevBuf d_kx;                                                                    // kept list
+    DevBuf d_aff_sim, d_aff_flag, d_aff_gi, d_aff_gj, d_aff_cnt, d_evptr, d_aff_oi, d_aff_oj, d_aff_ow, d_aff_par;   // candidates
+    DevBuf d_key, d_key2, d_val, d_val2, d_keep, d_keep2, d_found, d_changed;       // unused(): pair sort and fixpoint
+    DevBuf d_q, d_time, d_nflag, d_npos, d_idof, d_nkey, d_nkey2, d_nval, d_nval2, d_l2g;   // appearance times and local ids
+    DevBuf d_ei, d_ej, d_ew;                                                        // the emitted CLEdge list
 };
 
 // per-view lists of potentially collinear segments (l3d_collinear.cu), CSR over the global segment index

@@ -32,8 +32,8 @@ __device__ __forceinline__ D3 dray(const double* M, double x, double y) { return
 
 // Segment3D(P1, P2) (segment3D.h:48-66): a segment whose float length is not above 1e-12 collapses to zero.
 // n2 > 1e-20 already implies (float)sqrt(n2) > 1e-12; testing it first keeps the sqrt off the common path of callers
-// that only need the direction.  Selects rather than if/else: the branching form gave k_aff_events<false> 102 registers
-// instead of 94, one resident CTA less per SM, and made it 20 % slower.
+// that only need the direction.  Selects rather than if/else: the branching form gave the affinity stage's earlier
+// per-segment event kernel 102 registers instead of 94, one resident CTA less per SM, and made it 20 % slower.
 struct Seg3D { D3 P1, P2, dir; float length; };
 __device__ __forceinline__ Seg3D seg3d(D3 P1, D3 P2)
 {
