@@ -30,7 +30,7 @@ def needs_build() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False, defines=(), out: str | None = None) -> str:
-    """defines / out: build a variant (e.g. defines=("MK_RPW=4",), out="libl3d_b200_R4_B3.so") for the tile sweep"""
+    """defines / out: build a variant (e.g. defines=("MK_SLOTS=4",), out="libl3d_b200_S4.so") for the geometry sweep"""
     if out is None and not force and not needs_build():
         return OUT
     target = OUT if out is None else os.path.join(HERE, out)

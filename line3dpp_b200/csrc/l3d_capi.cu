@@ -188,7 +188,7 @@ int l3d_match_pairs(l3d_ctx* c, int num_pairs, const int32_t* pairs, const float
 { return l3d_match_pairs_range(c, num_pairs, pairs, F, epi_overlap, knn, 0, num_pairs); }
 
 struct HostOut { int32_t* counts; l3d_match_rec* recs; int chunks; };
-// Checks the arguments, fills h_pairs and the tiles of the pairs [first_pair, last_pair), uploads both and sizes the result buffers.
+// Checks the arguments, fills h_pairs and the work units of k_match_topk for the pairs [first_pair, last_pair), uploads both and sizes the result buffers.
 // *narcs: the number of level-1 table entries of the matched pairs.
 static int stage_pairs(l3d_ctx* c, int num_pairs, const int32_t* pairs, const float* F, const double* Fd, float epi_overlap, int knn,
                        int first_pair, int last_pair, const HostOut* host, long long* narcs)
@@ -200,9 +200,9 @@ static int stage_pairs(l3d_ctx* c, int num_pairs, const int32_t* pairs, const fl
     if (first_pair < 0 || last_pair < first_pair || last_pair > num_pairs) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs_range: bad pair range");
     if (knn > 32 && host) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs_host: kNN > 32 has no fixed row stride; use l3d_match_pairs + l3d_get_pair_matches");
     cudaSetDevice(c->device);
-    L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync before pair staging");   // h_pairs/h_tiles may still be in flight
+    L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync before pair staging");   // h_pairs/h_units may still be in flight
     c->h_pairs.resize(num_pairs);
-    c->h_tiles.clear();
+    c->h_units.clear();
     long long rows = 0, evals = 0;
     for (int i = 0; i < num_pairs; ++i) {
         int s = pairs[2 * i], t = pairs[2 * i + 1];
@@ -217,21 +217,26 @@ static int stage_pairs(l3d_ctx* c, int num_pairs, const int32_t* pairs, const fl
         if (Nt >= (1 << 24)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: more than 2^24 segments in one view");
         p.arc_off = *narcs;
         if (i >= first_pair && i < last_pair) *narcs += Nt;
-        if (Nt > 0 && i >= first_pair && i < last_pair)
-            for (int r0 = 0; r0 < Ns; r0 += MK_ROWS) c->h_tiles.push_back(make_int2(i, r0));
+        if (Nt > 0 && i >= first_pair && i < last_pair) {     // the pair's rows in even units; several passes keep every row's list in a slot
+            const int most = Nt <= MK_STAGES * MK_TT ? MK_UNIT_ROWS : MK_NSLOT, n = (Ns + most - 1) / most;
+            for (int u = 0; u < n; ++u) {
+                const int r0 = (int)((long long)Ns * u / n), r1 = (int)((long long)Ns * (u + 1) / n);
+                c->h_units.push_back(make_int4(i, r0, r1 - r0, 0));
+            }
+        }
         rows += Ns;
         if (i >= first_pair && i < last_pair) evals += (long long)Ns * Nt;     // evaluated HERE
     }
     c->num_pairs = num_pairs; c->knn = knn; c->epi = epi_overlap; c->total_rows = rows; c->pair_evals = evals;
     int rc;
     L3D_RESERVE(c->d_pairs, sizeof(L3DPairDev) * (size_t)std::max(num_pairs, 1), "pairs");
-    L3D_RESERVE(c->d_tiles, sizeof(int2) * std::max<size_t>(c->h_tiles.size(), 1), "tiles");
+    L3D_RESERVE(c->d_units, sizeof(int4) * std::max<size_t>(c->h_units.size(), 1), "tiles");
     L3D_RESERVE(c->d_arcs, (sizeof(uint4) + sizeof(float4)) * (size_t)std::max<long long>(*narcs, 1), "target arcs");   // arcs, then their segments
     L3D_RESERVE(c->d_basis, sizeof(L3DPairBasis) * (size_t)std::max(num_pairs, 1), "pair bases");
     L3D_RESERVE(c->d_counts, sizeof(int) * (size_t)std::max<long long>(rows, 1), "match counts");
     if (knn > 0 && knn <= 32) L3D_RESERVE(c->d_recs, sizeof(l3d_match_rec) * (size_t)std::max<long long>(rows, 1) * knn, "match records");
     if (num_pairs) L3D_CUDA(c, cudaMemcpyAsync(c->d_pairs.p, c->h_pairs.data(), sizeof(L3DPairDev) * num_pairs, cudaMemcpyHostToDevice, c->stream), "upload pairs");
-    if (!c->h_tiles.empty()) L3D_CUDA(c, cudaMemcpyAsync(c->d_tiles.p, c->h_tiles.data(), sizeof(int2) * c->h_tiles.size(), cudaMemcpyHostToDevice, c->stream), "upload tiles");
+    if (!c->h_units.empty()) L3D_CUDA(c, cudaMemcpyAsync(c->d_units.p, c->h_units.data(), sizeof(int4) * c->h_units.size(), cudaMemcpyHostToDevice, c->stream), "upload tiles");
     if (rows) L3D_CUDA(c, cudaMemsetAsync(c->d_counts.p, 0, sizeof(int) * rows, c->stream), "clear counts");   // rows of pairs with Nt == 0
     return L3D_OK;
 }
@@ -279,10 +284,10 @@ static int build_cache_d(l3d_ctx* c)
     return L3D_OK;
 }
 
-// one launch of k_match_topk<c->semantics, keep> over the tiles [t0, t1)
+// one launch of k_match_topk<c->semantics, keep> over the work units [t0, t1)
 static int launch_match(l3d_ctx* c, Keep keep, MatchArgs a, size_t t0, size_t t1, const char* what)
 {
-    a.tiles += t0;
+    a.units += t0;
     void* args[] = {&a};
     cudaLaunchKernel((const void*)l3d_match_kernels[c->semantics][(int)keep], dim3((unsigned int)(t1 - t0)), dim3(MK_THREADS), args, l3d_match_smem_bytes(), c->stream);
     ++c->launches;
@@ -290,14 +295,14 @@ static int launch_match(l3d_ctx* c, Keep keep, MatchArgs a, size_t t0, size_t t1
     return L3D_OK;
 }
 
-// The kNN best matches of every row: one launch, or (l3d_match_pairs_host) `chunks` launches over contiguous tile ranges with the D2H
+// The kNN best matches of every row: one launch, or (l3d_match_pairs_host) `chunks` launches over contiguous unit ranges with the D2H
 // copy of every finished chunk's rows queued on a second stream, so that the PCIe transfer of chunk k hides behind the arithmetic of
 // chunk k+1.
 static int run_topk(l3d_ctx* c, const MatchArgs& a, const HostOut* host)
 {
     const long long rows = c->total_rows, knn = a.knn;
-    const size_t ntiles = c->h_tiles.size();
-    const int chunks = host ? std::max(1, std::min<int>(host->chunks, (int)std::max<size_t>(ntiles, 1))) : 1;
+    const size_t nunits = c->h_units.size();
+    const int chunks = host ? std::max(1, std::min<int>(host->chunks, (int)std::max<size_t>(nunits, 1))) : 1;
     int rc;
     if (host) {
         if (!c->copy_stream) L3D_CUDA(c, cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking), "copy stream");
@@ -306,13 +311,13 @@ static int run_topk(l3d_ctx* c, const MatchArgs& a, const HostOut* host)
             c->events.push_back(e);
         }
     }
-    auto row_of_tile = [&](size_t t) { return t >= ntiles ? rows : c->h_pairs[c->h_tiles[t].x].row_off + c->h_tiles[t].y; };
+    auto row_of_unit = [&](size_t t) { return t >= nunits ? rows : c->h_pairs[c->h_units[t].x].row_off + c->h_units[t].y; };
     long long row_done = 0;
     for (int k = 0; k < chunks; ++k) {
-        const size_t t0 = ntiles * (size_t)k / chunks, t1 = ntiles * (size_t)(k + 1) / chunks;
+        const size_t t0 = nunits * (size_t)k / chunks, t1 = nunits * (size_t)(k + 1) / chunks;
         if (t1 > t0 && (rc = launch_match(c, Keep::TopK, a, t0, t1, "k_match_topk"))) return rc;
         if (host) {
-            const long long r1 = k == chunks - 1 ? rows : row_of_tile(t1);      // rows [row_done, r1) are final after this launch
+            const long long r1 = k == chunks - 1 ? rows : row_of_unit(t1);      // rows [row_done, r1) are final after this launch
             if (r1 > row_done) {
                 L3D_CUDA(c, cudaEventRecord(c->events[k], c->stream), "event record");
                 L3D_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->events[k], 0), "event wait");
@@ -336,11 +341,11 @@ static int run_topk(l3d_ctx* c, const MatchArgs& a, const HostOut* host)
 static int run_keep_all(l3d_ctx* c, MatchArgs a, int big_k)
 {
     const long long rows = c->total_rows;
-    const size_t ntiles = c->h_tiles.size();
+    const size_t nunits = c->h_units.size();
     int rc, stride = 1;
-    if (ntiles) {
+    if (nunits) {
         a.knn = 0; a.recs = nullptr;
-        if ((rc = launch_match(c, Keep::Count, a, 0, ntiles, "k_match_topk (count)"))) return rc;
+        if ((rc = launch_match(c, Keep::Count, a, 0, nunits, "k_match_topk (count)"))) return rc;
         if (rows > INT_MAX) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: more than 2^31 rows with kNN <= 0");
         L3D_RESERVE(c->d_rowptr, 16, "row max");
         int* d_max = (int*)c->d_rowptr.p;
@@ -353,13 +358,13 @@ static int run_keep_all(l3d_ctx* c, MatchArgs a, int big_k)
     }
     c->knn = stride;
     L3D_RESERVE(c->d_recs, sizeof(l3d_match_rec) * (size_t)std::max<long long>(rows, 1) * stride, "match records");
-    if (ntiles) {
+    if (nunits) {
         const size_t per_warp = sizeof(l3d_match_rec) * (size_t)stride;
         int wpb = 4;
         while (wpb > 1 && per_warp * wpb > 200 * 1024) wpb >>= 1;
         if (per_warp * wpb > 200 * 1024) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: a row with more than 8500 matches (kNN <= 0)");
         a.knn = stride; a.recs = (l3d_match_rec*)c->d_recs.p;
-        if ((rc = launch_match(c, Keep::Store, a, 0, ntiles, "k_match_topk (store)"))) return rc;
+        if ((rc = launch_match(c, Keep::Store, a, 0, nunits, "k_match_topk (store)"))) return rc;
         L3D_CUDA(c, cudaFuncSetAttribute(k_sort_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(per_warp * wpb)), "k_sort_rows smem");
         const long long blocks = std::min<long long>((rows + wpb - 1) / wpb, (long long)c->num_sms * 16);
         k_sort_rows<<<(unsigned int)blocks, wpb * 32, per_warp * wpb, c->stream>>>((int*)c->d_counts.p, (l3d_match_rec*)c->d_recs.p, stride, rows, big_k);
@@ -381,7 +386,7 @@ static int match_impl(l3d_ctx* c, int num_pairs, const int32_t* pairs, const flo
     if (Fd && (rc = build_cache_d(c))) return rc;
     c->semantics = Fd ? L3D_SEM_REF_CPU : L3D_SEM_REF_GPU;
     const MatchArgs a = {c->segs(), (const float4*)c->d_cache.p, Fd ? (const double*)c->d_cache_d.p : nullptr, c->views(), (const L3DPairDev*)c->d_pairs.p,
-                         (const int2*)c->d_tiles.p, (const uint4*)c->d_arcs.p, level1_segs(c, narcs), (const L3DPairBasis*)c->d_basis.p, (int*)c->d_counts.p,
+                         (const int4*)c->d_units.p, (const uint4*)c->d_arcs.p, level1_segs(c, narcs), (const L3DPairBasis*)c->d_basis.p, (int*)c->d_counts.p,
                          (l3d_match_rec*)c->d_recs.p, knn, epi_overlap};
     if ((rc = knn > 0 && knn <= 32 ? run_topk(c, a, host) : run_keep_all(c, a, knn > 32 ? knn : 0))) return rc;
     c->have_matches = true;

@@ -113,8 +113,8 @@ struct l3d_ctx {
     int semantics = 0;                      // L3D_SEM_* of the last match result; the scoring sweep follows it
     long long total_rows = 0, pair_evals = 0;
     std::vector<L3DPairDev> h_pairs;
-    std::vector<int2> h_tiles;
-    DevBuf d_pairs, d_tiles, d_counts, d_recs, d_rowptr, d_csr, d_dense_dep, d_dense_ov, d_dense_jobs, d_arcs, d_basis, d_arcraw, d_arckeys, d_arckeys2, d_arcvals, d_arcvals2;
+    std::vector<int4> h_units;              // k_match_topk work units: (pair, first source row, rows, 0)
+    DevBuf d_pairs, d_units, d_counts, d_recs, d_rowptr, d_csr, d_dense_dep, d_dense_ov, d_dense_jobs, d_arcs, d_basis, d_arcraw, d_arckeys, d_arckeys2, d_arcvals, d_arcvals2;
 
     SweepState sweep;
     RddState rdd;

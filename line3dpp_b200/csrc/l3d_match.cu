@@ -6,9 +6,12 @@
 //   k_pair_arcs,    : level-1 tables of the view pairs of one call (l3d_device.cuh "pencil parameter"): every target segment as an arc of
 //   k_arcs_gather     the epipolar pencil, grouped by arc length and sorted by arc start (one radix sort in between, l3d_capi.cu); the
 //                     table carries each arc's target segment in a parallel array (32 B per pair and target).
-//   k_match_topk    : production kernel.  One CTA = 64 source segments of one view pair; the pair's table (arcs + segments) is staged
-//                     in shared memory by 1-D TMA (cp.async.bulk + mbarrier, 3 stages x 512 entries x 32 B in flight from the first
-//                     instruction; larger target views take several passes); a warp owns 8 rows and, per row, binary-searches the
+//   k_match_topk    : production kernel.  One CTA per SM (24 warps) = one work unit: a view pair and up to 1024 of its source rows.
+//                     The pair's table (arcs + segments) is staged in shared memory by 1-D TMA (cp.async.bulk + mbarrier, 6 stages x
+//                     512 entries x 32 B in flight from the first instruction): a target view of up to 3072 segments is resident in one
+//                     pass, and a warp takes the unit's rows one at a time from a shared counter into one of its 8 row slots (constants,
+//                     key list, score-to-beat), with no CTA barrier; larger target views take several passes over units of at most 192
+//                     rows, each slot bound to one row.  Per row the warp binary-searches the
 //                     window of every arc class and scans only those entries, all windows as one concatenation (full warps): each
 //                     lane runs the arc test (13 integer instructions) and the conservative float filter (27 flop + 2 rcp on the
 //                     staged target segment) on its entry, branch-free, the survivors of both are ballot-compacted into a per-warp
@@ -54,33 +57,63 @@ __global__ void __launch_bounds__(256) k_prep_segments_f64(const float4* __restr
 }
 
 // ------------------------------------------------------------------------------------------------ fused match + top-k
+#ifdef L3D_MATCH_PROBE
+__device__ unsigned long long g_match_probe[MP_N];
+#define MPROBE(...) __VA_ARGS__
+#else
+#define MPROBE(...)
+#endif
+
+// A slot is the state of one source row in flight: key list, score-to-beat, count and the row's filter constants.  Every slot array
+// is indexed by CTA slot (warp * MK_SLOTS + i); slot_row names the unit's row the slot holds.
 struct MatchSmem {
     uint4 stage[MK_STAGES][MK_TT];                   // TMA-staged target arcs in window order (arc_may_match, l3d_device.cuh)
     float4 stage_seg[MK_STAGES][MK_TT];              // their target segments, same order (two arrays: both 16-byte loads of a warp are conflict-free)
-    uint2 rowK[MK_ROWS];                             // pencil parameters of the row's two epipolar lines (l3d_device.cuh)
-    int cls_off[L3D_ARC_NCLS + 2];                   // first sorted entry of every arc class of this view pair, and the end (k_pair_arcs)
-    unsigned char rowall[MK_ROWS];                   // 1: an epipolar line of this row is not a pencil member to within the margins (source point at the epipole): no level 1
-    unsigned long long lists[MK_ROWS][MK_CAP + 1];   // per-row survivor keys (+1: rows start on different banks, lanes that push keys of different rows do not collide)
-    float4 rowA[MK_ROWS];                            // (e1.x, e1.y, e1.z, e2.x)
-    float4 rowB[MK_ROWS];                            // (e2.y, e2.z, g, 0.95 * score-to-beat)
-    float row_thr[MK_ROWS];                          // overlap of the current k-th best survivor (0 until k are known)
-    int list_cnt[MK_ROWS];
-    unsigned int queue[MK_WARPS][96];                // survivors of both filters per warp: (row_local << 24) | position in the ring, evaluated
+    unsigned long long lists[MK_NSLOT][MK_CAP + 1];  // per-slot survivor keys (+1: slots start on different banks, lanes that push keys of different rows do not collide)
+    float4 rowA[MK_NSLOT];                           // (e1.x, e1.y, e1.z, e2.x)
+    float4 rowB[MK_NSLOT];                           // (e2.y, e2.z, g, 0.95 * score-to-beat)
+    uint2 rowK[MK_NSLOT];                            // pencil parameters of the row's two epipolar lines (l3d_device.cuh)
+    float row_thr[MK_NSLOT];                         // overlap of the current k-th best survivor (0 until k are known)
+    int list_cnt[MK_NSLOT];
+    int slot_row[MK_NSLOT];                          // row of the unit (0 .. rows - 1) the slot holds; -1: never used
+    unsigned char rowall[MK_NSLOT];                  // 1: an epipolar line of this row is not a pencil member to within the margins (source point at the epipole): no level 1
+    unsigned int queue[MK_WARPS][96];                // survivors of both filters per warp: (slot << 24) | position in the ring, evaluated
                                                      // exactly 32 at a time (up to 64 pushed per scan step onto at most 31 waiting)
+    L3DPairBasis B;                                  // the pair's pencil basis and the first sorted entry of every arc class, and the end (k_pair_arcs)
+    float F[9];                                      // the pair's float fundamental matrix (row constants)
+    int next_row;                                    // single-pass units: the next row a warp takes
+    int nrows, npass;                                // rows of the unit, passes over the target view (read here, not held in registers across the exact path)
     unsigned long long bars[MK_STAGES];
     // per-CTA constants of the (rarely executed, deliberately out-of-line) exact path
-    const float4* cache;
+    const float4* cache; const float4* ssegs;        // float ray cache; the unit's first source segment
+    const uint4* tarcs; const float4* tasegs;        // the pair's level-1 table (TMA sources of the refills)
     long long src_base, toff;
     float3 Cs, Ct;
     float epi; int knn;
     int cap;                                         // keys a row list collects before it is cut to its k best (and the score-to-beat rises); 16 instead of 32 was measured 7 % slower
     // REF_CPU semantics only: the exact path is matchingCPU's double arithmetic; the float filter stays the same
-    const double* cache_d; const float4* ssegs;
+    const double* cache_d;
     double Fd[9]; D3 Csd, Ctd;
-    // keep-all modes (kNN <= 0, cudawrapper.cu:628-636): output row base / record array; knn then holds the row stride
-    long long R0; l3d_match_rec* recs_out;
+    // output: row base of the unit, per-row counts and records (row stride knn; keep-all modes: knn holds the stride found by Count)
+    long long R0; int* counts_out; l3d_match_rec* recs_out;
+#ifdef L3D_MATCH_PROBE
+    unsigned long long probe[MK_WARPS][MP_N];
+#endif
 };
 size_t l3d_match_smem_bytes() { return sizeof(MatchSmem); }
+
+#ifdef L3D_MATCH_PROBE
+__device__ __forceinline__ void probe_add(MatchSmem& S, int warp, int lane, int k, unsigned long long v) { if (lane == 0) S.probe[warp][k] += v; }
+extern "C" int l3d_match_probe(unsigned long long* out, int reset)
+{
+    if (cudaMemcpyFromSymbol(out, g_match_probe, sizeof(unsigned long long) * MP_N) != cudaSuccess) return -1;
+    if (reset) {
+        static const unsigned long long zero[MP_N] = {};
+        if (cudaMemcpyToSymbol(g_match_probe, zero, sizeof(zero)) != cudaSuccess) return -1;
+    }
+    return MP_N;
+}
+#endif
 
 // rank of lane's key among the n <= 32 keys of a row list (number of larger keys; keys are unique)
 __device__ __forceinline__ int rank_in_row(const unsigned long long* list, int n, unsigned long long k)
@@ -91,12 +124,12 @@ __device__ __forceinline__ int rank_in_row(const unsigned long long* list, int n
 }
 
 // keep the k best keys of a full row list (sorted, best first) and raise the row's score-to-beat
-__device__ __noinline__ void prune_row(MatchSmem& S, int row, int lane)
+__device__ __noinline__ void prune_row(MatchSmem& S, int slot, int lane)
 {
     const int knn = S.knn; const float epi = S.epi;
     __syncwarp();
-    const int n = min(S.list_cnt[row], S.cap);
-    const unsigned long long k = lane < n ? S.lists[row][lane] : 0ull;
+    const int n = min(S.list_cnt[slot], S.cap);
+    const unsigned long long k = lane < n ? S.lists[slot][lane] : 0ull;
     int r;
     if (knn <= 16) {          // k rounds of warp maximum (keys are unique and > 0) instead of ranking all n keys against each other
         bool active = lane < n;
@@ -110,23 +143,23 @@ __device__ __noinline__ void prune_row(MatchSmem& S, int row, int lane)
             if (__popc(bm) > 1) { const unsigned int l = __reduce_max_sync(0xffffffffu, c ? lo : 0u); c = c && lo == l; }
             if (c) { r = i; active = false; }
         }
-    } else r = rank_in_row(S.lists[row], n, k);
+    } else r = rank_in_row(S.lists[slot], n, k);
     __syncwarp();
-    if (lane < n && r < knn) S.lists[row][r] = k;
+    if (lane < n && r < knn) S.lists[slot][r] = k;
     __syncwarp();
     if (lane == 0) {
-        S.list_cnt[row] = min(n, knn);
+        S.list_cnt[slot] = min(n, knn);
         if (n >= knn) {
-            const float kth = key_overlap(S.lists[row][knn - 1]);
-            S.row_thr[row] = kth;
-            S.rowB[row].w = 0.95f * fmaxf(kth, epi);
+            const float kth = key_overlap(S.lists[slot][knn - 1]);
+            S.row_thr[slot] = kth;
+            S.rowB[slot].w = 0.95f * fmaxf(kth, epi);
         }
     }
     __syncwarp();
 }
 
-// depths (d_p1, d_p2, d_q1, d_q2) of target j for row rl, stored as Match stores them (floats, commons.h:186-203); true when all
-// four are in front of the cameras: > 0 in float (REF_GPU, cudawrapper.cu:186-253) or > 1e-12 in double (REF_CPU, line3D.cc:925-1003)
+// depths (d_p1, d_p2, d_q1, d_q2) of target j for the unit's row rl, stored as Match stores them (floats, commons.h:186-203); true when
+// all four are in front of the cameras: > 0 in float (REF_GPU, cudawrapper.cu:186-253) or > 1e-12 in double (REF_CPU, line3D.cc:925-1003)
 template <int SEM>
 __device__ __forceinline__ bool target_depths(const MatchSmem& S, int rl, unsigned int j, float* d)
 {
@@ -142,32 +175,32 @@ __device__ __forceinline__ bool target_depths(const MatchSmem& S, int rl, unsign
     return d[0] > 0.0f && d[1] > 0.0f && d[2] > 0.0f && d[3] > 0.0f;
 }
 
-// exact evaluation of candidate j (target segment q) for row rl (has == false: padding lane, never a match): the overlap must exceed
-// epi and reach the row's current k-th best (below it the candidate can never be selected), and the depths must be positive
-// (target_depths).
+// exact evaluation of candidate j (target segment q) for the row rl held by slot sl (has == false: padding lane, never a match): the
+// overlap must exceed epi and reach the row's current k-th best (below it the candidate can never be selected), and the depths must be
+// positive (target_depths).
 // REF_GPU: K_match_lines' float overlap with the row's cached epipolar lines, inline (the lanes stay converged through it);
 // REF_CPU: matchingCPU's double overlap (line3D.cc:925-1003) with epipolar lines from the double F, out of line.
-template <int SEM> __device__ bool eval_candidate(const MatchSmem& S, int rl, unsigned int j, float4 q, bool has, float* ov, float* d);
-template <> __device__ __forceinline__ bool eval_candidate<L3D_SEM_REF_GPU>(const MatchSmem& S, int rl, unsigned int j, float4 q, bool has, float* ov, float* d)
+template <int SEM> __device__ bool eval_candidate(const MatchSmem& S, int sl, int rl, unsigned int j, float4 q, bool has, float* ov, float* d);
+template <> __device__ __forceinline__ bool eval_candidate<L3D_SEM_REF_GPU>(const MatchSmem& S, int sl, int rl, unsigned int j, float4 q, bool has, float* ov, float* d)
 {
-    const float4 rA = S.rowA[rl], rB = S.rowB[rl];
+    const float4 rA = S.rowA[sl], rB = S.rowB[sl];
     bool inv;
     *ov = exact_overlap(q, make_float3(rA.x, rA.y, rA.z), make_float3(rA.w, rB.x, rB.y), &inv);
-    return has && *ov > S.epi && *ov >= S.row_thr[rl] && target_depths<L3D_SEM_REF_GPU>(S, rl, j, d);
+    return has && *ov > S.epi && *ov >= S.row_thr[sl] && target_depths<L3D_SEM_REF_GPU>(S, rl, j, d);
 }
-template <> __device__ __noinline__ bool eval_candidate<L3D_SEM_REF_CPU>(const MatchSmem& S, int rl, unsigned int j, float4 q, bool has, float* ov, float* d)
+template <> __device__ __noinline__ bool eval_candidate<L3D_SEM_REF_CPU>(const MatchSmem& S, int sl, int rl, unsigned int j, float4 q, bool has, float* ov, float* d)
 {
     if (!has) return false;
     const float4 sp = __ldg(S.ssegs + rl);
     const D3 e1 = dmulmat(S.Fd, d3((double)sp.x, (double)sp.y, 1.0)), e2 = dmulmat(S.Fd, d3((double)sp.z, (double)sp.w, 1.0));
     bool valid;
     *ov = exact_overlap_f64(q, e1, e2, &valid);
-    return valid && *ov > S.epi && *ov >= S.row_thr[rl] && target_depths<L3D_SEM_REF_CPU>(S, rl, j, d);
+    return valid && *ov > S.epi && *ov >= S.row_thr[sl] && target_depths<L3D_SEM_REF_CPU>(S, rl, j, d);
 }
 
 // exact evaluation of up to 32 queued candidates (one per lane).  Out of line on purpose: the hot filter loop must
 // stay inside the instruction cache (the first version inlined this 5x -> 64 KB of SASS, 55 % "no instruction" stalls).
-// A match is kept per KEEP: TopK pushes its key into the row list (cut to the kNN best when full), Count only counts it,
+// A match is kept per KEEP: TopK pushes its key into the slot's list (cut to the kNN best when full), Count only counts it,
 // Store writes its record (row stride S.knn, slot = arrival order; k_sort_rows puts the rows into the reference's
 // ascending-target order afterwards).
 template <int SEM, Keep KEEP>
@@ -176,16 +209,17 @@ __device__ __noinline__ void exact_batch(MatchSmem& S, unsigned int entry, bool 
     const int knn = S.knn;
     bool pending = false;
     unsigned long long key = 0ull;
-    int rl = 0;
+    int sl = 0;
     if (has) {
-        rl = (int)(entry >> 24);
+        sl = (int)(entry >> 24);
+        const int rl = S.slot_row[sl];
         const unsigned int pos = entry & 0xFFFFFFu;                  // position in the resident ring: target index and segment are staged
         const unsigned int j = (&S.stage[0][0])[pos].w;
         float ov = 0.0f, d[4];
-        if (eval_candidate<SEM>(S, rl, j, (&S.stage_seg[0][0])[pos], has, &ov, d)) {
+        if (eval_candidate<SEM>(S, sl, rl, j, (&S.stage_seg[0][0])[pos], has, &ov, d)) {
             if (KEEP == Keep::TopK) { key = make_key(ov, j); pending = true; }
             else {
-                const int slot = atomicAdd(&S.list_cnt[rl], 1);         // a row belongs to one warp: no cross-warp contention
+                const int slot = atomicAdd(&S.list_cnt[sl], 1);         // a row belongs to one warp: no cross-warp contention
                 if (KEEP == Keep::Store && slot < knn) {
                     l3d_match_rec rec;
                     rec.tgt_seg = j; rec.overlap = ov; rec.d_p1 = d[0]; rec.d_p2 = d[1]; rec.d_q1 = d[2]; rec.d_q2 = d[3];
@@ -196,17 +230,17 @@ __device__ __noinline__ void exact_batch(MatchSmem& S, unsigned int entry, bool 
     }
     while (KEEP == Keep::TopK) {
         if (pending) {
-            int slot = atomicAdd(&S.list_cnt[rl], 1);
-            if (slot < S.cap) { S.lists[rl][slot] = key; pending = false; }
+            int slot = atomicAdd(&S.list_cnt[sl], 1);
+            if (slot < S.cap) { S.lists[sl][slot] = key; pending = false; }
         }
         unsigned int pm = __ballot_sync(0xffffffffu, pending);
         if (!pm) break;
         unsigned int todo = pm;                       // a row list is full: keep its k best and retry
         while (todo) {
             int leader = __ffs(todo) - 1;
-            int row = __shfl_sync(0xffffffffu, rl, leader);
+            int row = __shfl_sync(0xffffffffu, sl, leader);
             prune_row(S, row, lane);
-            unsigned int mine = __ballot_sync(0xffffffffu, pending && rl == row);
+            unsigned int mine = __ballot_sync(0xffffffffu, pending && sl == row);
             todo &= ~mine;
             if (knn >= S.cap) {                       // list stays full (k == capacity): fold the pending keys in one by one
                 while (mine) {
@@ -223,32 +257,27 @@ __device__ __noinline__ void exact_batch(MatchSmem& S, unsigned int entry, bool 
     __syncwarp();
 }
 
-// write the match count of each of this warp's rows; TopK also selects the k best survivors and writes their records (once
-// per CTA: out of line)
+// write the match count of the row held by slot sl; TopK also selects its k best survivors and writes their records.  Runs once per
+// row, when the slot is about to be reused or at the end of the unit: out of line.
 template <int SEM, Keep KEEP>
-__device__ __noinline__ void finalize_rows(MatchSmem& S, int warp, int lane, int nrows, long long R0, int* __restrict__ counts_out,
-                                           l3d_match_rec* __restrict__ recs_out)
+__device__ __noinline__ void finalize_row(MatchSmem& S, int sl, int lane)
 {
-    const int knn = S.knn;
-    for (int r = 0; r < MK_RPW; ++r) {
-        const int rl = warp * MK_RPW + r;
-        if (rl >= nrows) break;
-        const long long R = R0 + rl;
-        if (KEEP != Keep::TopK) { if (lane == 0) counts_out[R] = S.list_cnt[rl]; continue; }
-        const int n = min(S.list_cnt[rl], S.cap);
-        if (lane == 0) counts_out[R] = min(n, knn);
-        if (n == 0) continue;
-        const unsigned long long key = lane < n ? S.lists[rl][lane] : 0ull;
-        const int rank = rank_in_row(S.lists[rl], n, key);
-        if (lane < n && rank < knn) {
-            unsigned int j = key_tgt(key);
-            float d[4];
-            target_depths<SEM>(S, rl, j, d);
-            l3d_match_rec rec;
-            rec.tgt_seg = j; rec.overlap = key_overlap(key);
-            rec.d_p1 = d[0]; rec.d_p2 = d[1]; rec.d_q1 = d[2]; rec.d_q2 = d[3];
-            recs_out[R * knn + rank] = rec;
-        }
+    const int knn = S.knn, rl = S.slot_row[sl];
+    const long long R = S.R0 + rl;
+    if (KEEP != Keep::TopK) { if (lane == 0) S.counts_out[R] = S.list_cnt[sl]; return; }
+    const int n = min(S.list_cnt[sl], S.cap);
+    if (lane == 0) S.counts_out[R] = min(n, knn);
+    if (n == 0) return;
+    const unsigned long long key = lane < n ? S.lists[sl][lane] : 0ull;
+    const int rank = rank_in_row(S.lists[sl], n, key);
+    if (lane < n && rank < knn) {
+        unsigned int j = key_tgt(key);
+        float d[4];
+        target_depths<SEM>(S, rl, j, d);
+        l3d_match_rec rec;
+        rec.tgt_seg = j; rec.overlap = key_overlap(key);
+        rec.d_p1 = d[0]; rec.d_p2 = d[1]; rec.d_q1 = d[2]; rec.d_q2 = d[3];
+        S.recs_out[R * knn + rank] = rec;
     }
 }
 
@@ -378,8 +407,9 @@ k_arcs_gather(long long n, const unsigned long long* __restrict__ keys, const un
 
 // thread 0: start the TMA copies of the level-1 entries [base, base + cnt) of a pair into the ring; the arcs and the segments of a
 // stage complete on the stage's barrier together
-__device__ __forceinline__ void stage_entries(MatchSmem& S, const uint4* arcs, const float4* asegs, int base, int cnt)
+__device__ __forceinline__ void stage_entries(MatchSmem& S, int base, int cnt)
 {
+    const uint4* arcs = S.tarcs; const float4* asegs = S.tasegs;
     for (int i = 0; i < MK_STAGES && i * MK_TT < cnt; ++i) {
         const unsigned int bytes = (unsigned int)min(MK_TT, cnt - i * MK_TT) * 16u;
         const size_t o = (size_t)base + (size_t)i * MK_TT;
@@ -410,155 +440,233 @@ __device__ __forceinline__ int flat_entry(int G, int lane, int np, int pE, int p
     return min(G + lane, tot - 1) + __shfl_sync(0xffffffffu, pshift, r);
 }
 
+// the constants of the unit's row rl into slot sl, and an empty key list: the epipolar lines F*p (cudawrapper.cu:216-217), the float
+// filter's scale, the lines' pencil parameters (lanes 0 and 1, one line each) and whether the row skips level 1
+__device__ __forceinline__ void setup_row(MatchSmem& S, int sl, int rl, int lane)
+{
+    const float4 s = __ldg(S.ssegs + rl);
+    const float3 e1 = mulmat_h(S.F, s.x, s.y), e2 = mulmat_h(S.F, s.z, s.w);
+    bool off = false;
+    unsigned int k = 0u;
+    if (lane < 2) k = line_kappa(S.B, lane ? e2 : e1, &off);
+    const unsigned int k2 = __shfl_sync(0xffffffffu, k, 1), offs = __ballot_sync(0xffffffffu, off);
+    if (lane == 0) {
+        const float g = L3D_FILTER_C1 * fmaxf(sqrtf(e1.x * e1.x + e1.y * e1.y), sqrtf(e2.x * e2.x + e2.y * e2.y));
+        S.rowA[sl] = make_float4(e1.x, e1.y, e1.z, e2.x);
+        S.rowB[sl] = make_float4(e2.y, e2.z, g, 0.95f * S.epi);
+        S.rowK[sl] = make_uint2(k, k2);
+        S.rowall[sl] = offs ? 1 : 0;
+        S.list_cnt[sl] = 0;
+        S.row_thr[sl] = 0.0f;
+        S.slot_row[sl] = rl;
+    }
+    __syncwarp();
+}
+
+// evaluate every pending candidate of the warp's queue (qn < 32 of them)
+template <int SEM, Keep KEEP>
+__device__ __forceinline__ void drain_queue(MatchSmem& S, int warp, int lane, int& qn)
+{
+    __syncwarp();
+    if (qn > 0) {
+        MPROBE(const long long t0 = clock64();)
+        const bool has = lane < qn;
+        exact_batch<SEM, KEEP>(S, has ? S.queue[warp][lane] : 0u, has, lane);
+        MPROBE(probe_add(S, warp, lane, MP_EXACT, clock64() - t0); probe_add(S, warp, lane, MP_EVALS, qn);)
+        qn = 0;
+    }
+}
+
+// Scan the window entries of the row in slot sl that lie in the resident ring entries [base, base + cnt) of the pair's level-1 table and
+// queue the survivors of both filters; the queue is evaluated 32 at a time.
+template <int SEM, Keep KEEP>
+__device__ __forceinline__ void scan_row(MatchSmem& S, int sl, int base, int cnt, int warp, int lane, int& qn)
+{
+    MPROBE(const long long t_row = clock64(); long long t_exact = 0;)
+    const unsigned int lt_mask = (1u << lane) - 1u;
+    const uint4* ent = &S.stage[0][0];
+    const int* cls_off = S.B.cls_off;
+    const uint2 kr = S.rowK[sl];
+    const bool rall = S.rowall[sl] != 0;
+    const float4 rA = S.rowA[sl];
+    float4 rB = S.rowB[sl];                     // rB.w: the score-to-beat, re-read after exact batches (a stale value only rejects less)
+    // short arc [ka, kb] between the two kappa values: a target of class c can only match if its arc starts in [ka - 2^(CLS0 + c), kb]
+    const bool fwd = (kr.y - kr.x) < 0x80000000u;
+    const unsigned int ka = fwd ? kr.x : kr.y, kb = fwd ? kr.y : kr.x;
+    // lanes 0 .. 2 * NCLS - 1: lower / upper end of the window of class lane >> 1 inside the resident part of that class (binary search)
+    int res = 0;
+    {
+        const int c = min(lane >> 1, L3D_ARC_NCLS - 1);
+        int lo = min(max(cls_off[c] - base, 0), cnt), hi = min(max(cls_off[c + 1] - base, 0), cnt);
+        const bool upper = lane & 1;
+        const unsigned int key = upper ? kb + 1u : ka - (1u << (L3D_ARC_CLS0 + c));
+        if (lane >= 2 * L3D_ARC_NCLS || rall) hi = lo;                       // no search
+        else if (upper && kb == 0xFFFFFFFFu) lo = hi;
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (ent[mid].x < key) lo = mid + 1; else hi = mid;
+        }
+        res = lo;
+    }
+    // lane p < 2 * NCLS: piece p & 1 of the window of class p >> 1 (two pieces when the window wraps around 2^32); lane 2 * NCLS: the
+    // targets every row looks at.  A row outside the pencil model (rall) takes everything as one piece.
+    int plo = 0, phi = 0;
+    {
+        const int c = min(lane >> 1, L3D_ARC_NCLS - 1);
+        const int i0 = __shfl_sync(0xffffffffu, res, 2 * c), i1 = __shfl_sync(0xffffffffu, res, 2 * c + 1);
+        const int s_c = min(max(cls_off[c] - base, 0), cnt), e_c = min(max(cls_off[c + 1] - base, 0), cnt);
+        const bool wrap = ka - (1u << (L3D_ARC_CLS0 + c)) > kb;
+        if (lane < 2 * L3D_ARC_NCLS) {
+            if (!(lane & 1)) { plo = wrap ? s_c : i0; phi = i1; }
+            else if (wrap) { plo = i0; phi = e_c; }
+        } else if (lane == 2 * L3D_ARC_NCLS) { plo = min(max(cls_off[L3D_ARC_NCLS] - base, 0), cnt); phi = cnt; }
+        if (rall) { plo = 0; phi = lane == 0 ? cnt : 0; }
+    }
+    // The pieces are scanned as one concatenation, so that every step but the row's last fills all 64 lanes: a window piece
+    // averages a few dozen entries.  Lane q < np holds the q-th non-empty piece: its position E in the concatenation and the
+    // shift (first entry - E) that turns a position of that piece into an entry index.
+    const int len = phi - plo;
+    const unsigned int ne = __ballot_sync(0xffffffffu, len > 0);
+    int ex = len;
+    for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, ex, o); if (lane >= o) ex += v; }
+    const int tot = __shfl_sync(0xffffffffu, ex, 31), np = __popc(ne);
+    ex -= len;
+    const int src = lane < np ? (int)__fns(ne, 0u, lane + 1) : 0;
+    const int pE = __shfl_sync(0xffffffffu, ex, src), pshift = __shfl_sync(0xffffffffu, plo - ex, src);
+    MPROBE(probe_add(S, warp, lane, MP_SETUP, clock64() - t_row); const long long t_scan = clock64(); probe_add(S, warp, lane, MP_ENTRIES, tot);)
+    for (int G = 0; G < tot; G += 64) {                 // two entries per lane: half the loop / vote / push overhead per entry
+        const int ia = flat_entry(G, lane, np, pE, pshift, tot), ib = flat_entry(G + 32, lane, np, pE, pshift, tot);
+        const bool pa = entry_may_match(S, ia, kr.x, kr.y, rall, rA, rB) & (G + lane < tot);
+        const bool pb = entry_may_match(S, ib, kr.x, kr.y, rall, rA, rB) & (G + 32 + lane < tot);
+        const unsigned int ba = __ballot_sync(0xffffffffu, pa), bb = __ballot_sync(0xffffffffu, pb);
+        if (ba | bb) {
+            MPROBE(probe_add(S, warp, lane, MP_SURVIVORS, __popc(ba) + __popc(bb));)
+            if (pa) S.queue[warp][qn + __popc(ba & lt_mask)] = ((unsigned int)sl << 24) | (unsigned int)ia;
+            qn += __popc(ba);
+            if (pb) S.queue[warp][qn + __popc(bb & lt_mask)] = ((unsigned int)sl << 24) | (unsigned int)ib;
+            qn += __popc(bb);
+            __syncwarp();
+            if (qn >= 32) {
+                MPROBE(const long long t0 = clock64();)
+                do { qn -= 32; exact_batch<SEM, KEEP>(S, S.queue[warp][qn + lane], true, lane); MPROBE(probe_add(S, warp, lane, MP_EVALS, 32);) } while (qn >= 32);
+                MPROBE(t_exact += clock64() - t0;)
+                rB.w = S.rowB[sl].w;
+            }
+        }
+    }
+    MPROBE(probe_add(S, warp, lane, MP_SCAN, clock64() - t_scan - t_exact); probe_add(S, warp, lane, MP_EXACT, t_exact);)
+}
+
 // One instantiation per semantics (L3D_SEM_*: the exact path's arithmetic; the staging, scan and float filter are the same) and
 // keep policy.  TopK is the production kernel.  kNN <= 0 ("keep all matches", cudawrapper.cu:628-636 / line3D.cc:988-996) runs
 // Count (A.knn unused), then Store with the row stride found by Count in A.knn.
+// One CTA per SM and per work unit (a pair and a range of its source rows, stage_pairs in l3d_capi.cu).  A target view of up to
+// MK_STAGES * MK_TT segments is resident in one pass: a warp takes the unit's rows one at a time from a shared counter as soon as it
+// has a slot, so no warp waits for another until the unit ends.  Larger target views take several passes with a CTA barrier each; their
+// units have at most MK_NSLOT rows, every warp's slots hold fixed rows and keep their lists across the passes.
 // The pair, view and basis records are read with explicit __ldg: pointers taken from a parameter block carry no __restrict__.
 template <int SEM, Keep KEEP>
-__global__ void __launch_bounds__(MK_THREADS, MK_MINB) k_match_topk(const MatchArgs A)
+__global__ void __launch_bounds__(MK_THREADS, 1) k_match_topk(const MatchArgs A)
 {
-    const float4* segs = A.segs;
-    const int knn = A.knn; const float epi = A.epi;
+    MPROBE(const long long t_start = clock64();)
     extern __shared__ __align__(128) unsigned char smem_raw[];
     MatchSmem& S = *reinterpret_cast<MatchSmem*>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int2 tile = __ldg(A.tiles + blockIdx.x);
-    const L3DPairDev* P = A.pairs + tile.x;
-    const L3DPairBasis* PB = A.basis + tile.x;
-    const int row0 = tile.y;
+    const int4 unit = __ldg(A.units + blockIdx.x);
+    const L3DPairDev* P = A.pairs + unit.x;
+    const int row0 = unit.y, nrows = unit.z;
     const L3DViewDev* vs = A.views + __ldg(&P->src);
     const L3DViewDev* vt = A.views + __ldg(&P->tgt);
-    const long long soff = __ldg(&vs->seg_off), toff = __ldg(&vt->seg_off);
-    const int Ns = __ldg(&vs->nseg), Nt = __ldg(&vt->nseg);
-    const long long R0 = __ldg(&P->row_off) + row0;
-    const int nrows = min(MK_ROWS, Ns - row0);
-    const uint4* tarcs = A.arcs + __ldg(&P->arc_off);
-    const float4* tasegs = A.arc_segs + __ldg(&P->arc_off);
+    const int Nt = __ldg(&vt->nseg);
     const int RES = MK_STAGES * MK_TT;                     // entries resident at a time; larger target views take several passes
     const int npass = (Nt + RES - 1) / RES;
     if (tid == 0) {
-        S.cache = A.cache; S.src_base = soff + row0; S.toff = toff; S.epi = epi; S.knn = knn; S.cap = MK_CAP;
+        const long long soff = __ldg(&vs->seg_off);
+        S.cache = A.cache; S.ssegs = A.segs + soff + row0; S.src_base = soff + row0; S.toff = __ldg(&vt->seg_off);
+        S.epi = A.epi; S.knn = A.knn; S.cap = MK_CAP; S.next_row = 0; S.nrows = nrows; S.npass = npass;
+        S.tarcs = A.arcs + __ldg(&P->arc_off); S.tasegs = A.arc_segs + __ldg(&P->arc_off);
         S.Cs = make_float3(__ldg(&vs->C[0]), __ldg(&vs->C[1]), __ldg(&vs->C[2])); S.Ct = make_float3(__ldg(&vt->C[0]), __ldg(&vt->C[1]), __ldg(&vt->C[2]));
-        S.R0 = R0; S.recs_out = A.recs;
+        S.R0 = __ldg(&P->row_off) + row0; S.counts_out = A.counts; S.recs_out = A.recs;
         if (SEM == L3D_SEM_REF_CPU) {
-            S.cache_d = A.cache_d; S.ssegs = segs + soff + row0;
+            S.cache_d = A.cache_d;
             for (int i = 0; i < 9; ++i) S.Fd[i] = __ldg(&P->Fd[i]);
             S.Csd = d3(__ldg(&vs->C_d[0]), __ldg(&vs->C_d[1]), __ldg(&vs->C_d[2])); S.Ctd = d3(__ldg(&vt->C_d[0]), __ldg(&vt->C_d[1]), __ldg(&vt->C_d[2]));
         }
         for (int i = 0; i < MK_STAGES; ++i) mbar_init(&S.bars[i], 1);
         mbar_fence_init();
-        stage_entries(S, tarcs, tasegs, 0, min(RES, Nt));              // the first pass is in flight while the rows are set up
+        stage_entries(S, 0, min(RES, Nt));              // the first pass is in flight while the rows are set up
     }
-    if (tid >= MK_THREADS - (L3D_ARC_NCLS + 2)) S.cls_off[MK_THREADS - 1 - tid] = __ldg(&PB->cls_off[MK_THREADS - 1 - tid]);
-    if (tid < MK_ROWS) {
-        S.list_cnt[tid] = 0;
-        S.row_thr[tid] = 0.0f;
-        if (tid < nrows) {
-            float4 s = __ldg(segs + soff + row0 + tid);
-            float F[9];
-            for (int i = 0; i < 9; ++i) F[i] = __ldg(&P->F[i]);
-            float3 e1 = mulmat_h(F, s.x, s.y), e2 = mulmat_h(F, s.z, s.w);     // epipolar lines F*p (cudawrapper.cu:216-217)
-            float g = L3D_FILTER_C1 * fmaxf(sqrtf(e1.x * e1.x + e1.y * e1.y), sqrtf(e2.x * e2.x + e2.y * e2.y));
-            S.rowA[tid] = make_float4(e1.x, e1.y, e1.z, e2.x);
-            S.rowB[tid] = make_float4(e2.y, e2.z, g, 0.95f * epi);
-            L3DPairBasis B;
-            for (int i = 0; i < 3; ++i) { B.u[i] = __ldg(&PB->u[i]); B.v[i] = __ldg(&PB->v[i]); }
-            bool off1, off2;
-            S.rowK[tid] = make_uint2(line_kappa(B, e1, &off1), line_kappa(B, e2, &off2));
-            S.rowall[tid] = (off1 || off2) ? 1 : 0;
-        }
-    }
+    constexpr int NB = (int)(sizeof(L3DPairBasis) / sizeof(int));
+    static_assert(sizeof(L3DPairBasis) % sizeof(int) == 0 && NB + 9 + 1 <= MK_THREADS, "one word per thread");
+    if (tid < NB) reinterpret_cast<int*>(&S.B)[tid] = __ldg(reinterpret_cast<const int*>(A.basis + unit.x) + tid);
+    else if (tid < NB + 9) S.F[tid - NB] = __ldg(&P->F[tid - NB]);
+    for (int i = tid; i < MK_NSLOT; i += MK_THREADS) S.slot_row[i] = -1;
+    MPROBE(if (tid < MP_N * MK_WARPS) (&S.probe[0][0])[tid] = 0ull; long long t_wait = clock64();)
     __syncthreads();
+    MPROBE(probe_add(S, warp, lane, MP_WAIT, clock64() - t_wait);)
 
-    const unsigned int lt_mask = (1u << lane) - 1u;
-    const uint4* ent = &S.stage[0][0];
-    const int my_rows = min(MK_RPW, nrows - warp * MK_RPW);
     int qn = 0;    // warp-uniform fill of the candidate queue
-
-    for (int pass = 0; pass < npass; ++pass) {
+    for (int pass = 0; pass < S.npass; ++pass) {
         const int base = pass * RES, cnt = min(RES, Nt - base);
+        MPROBE(t_wait = clock64();)
         if (pass > 0) {                                // everybody is done with the resident entries: refill
             __syncthreads();
-            if (tid == 0) stage_entries(S, tarcs, tasegs, base, cnt);
+            if (tid == 0) stage_entries(S, base, cnt);
         }
         for (int i = 0; i < MK_STAGES && i * MK_TT < cnt; ++i) mbar_wait(&S.bars[i], (unsigned int)(pass & 1));
-        for (int r = 0; r < my_rows; ++r) {
-            const int rl = warp * MK_RPW + r;
-            const uint2 kr = S.rowK[rl];
-            const bool rall = S.rowall[rl] != 0;
-            const float4 rA = S.rowA[rl];
-            float4 rB = S.rowB[rl];                     // rB.w: the score-to-beat, re-read after exact batches (a stale value only rejects less)
-            // short arc [ka, kb] between the two kappa values: a target of class c can only match if its arc starts in [ka - 2^(CLS0 + c), kb]
-            const bool fwd = (kr.y - kr.x) < 0x80000000u;
-            const unsigned int ka = fwd ? kr.x : kr.y, kb = fwd ? kr.y : kr.x;
-            // lanes 0 .. 2 * NCLS - 1: lower / upper end of the window of class lane >> 1 inside the resident part of that class (binary search)
-            int res = 0;
-            {
-                const int c = min(lane >> 1, L3D_ARC_NCLS - 1);
-                int lo = min(max(S.cls_off[c] - base, 0), cnt), hi = min(max(S.cls_off[c + 1] - base, 0), cnt);
-                const bool upper = lane & 1;
-                const unsigned int key = upper ? kb + 1u : ka - (1u << (L3D_ARC_CLS0 + c));
-                if (lane >= 2 * L3D_ARC_NCLS || rall) hi = lo;                       // no search
-                else if (upper && kb == 0xFFFFFFFFu) lo = hi;
-                while (lo < hi) {
-                    const int mid = (lo + hi) >> 1;
-                    if (ent[mid].x < key) lo = mid + 1; else hi = mid;
-                }
-                res = lo;
-            }
-            // lane p < 2 * NCLS: piece p & 1 of the window of class p >> 1 (two pieces when the window wraps around 2^32); lane 2 * NCLS: the
-            // targets every row looks at.  A row outside the pencil model (rall) takes everything as one piece.
-            int plo = 0, phi = 0;
-            {
-                const int c = min(lane >> 1, L3D_ARC_NCLS - 1);
-                const int i0 = __shfl_sync(0xffffffffu, res, 2 * c), i1 = __shfl_sync(0xffffffffu, res, 2 * c + 1);
-                const int s_c = min(max(S.cls_off[c] - base, 0), cnt), e_c = min(max(S.cls_off[c + 1] - base, 0), cnt);
-                const bool wrap = ka - (1u << (L3D_ARC_CLS0 + c)) > kb;
-                if (lane < 2 * L3D_ARC_NCLS) {
-                    if (!(lane & 1)) { plo = wrap ? s_c : i0; phi = i1; }
-                    else if (wrap) { plo = i0; phi = e_c; }
-                } else if (lane == 2 * L3D_ARC_NCLS) { plo = min(max(S.cls_off[L3D_ARC_NCLS] - base, 0), cnt); phi = cnt; }
-                if (rall) { plo = 0; phi = lane == 0 ? cnt : 0; }
-            }
-            // The pieces are scanned as one concatenation, so that every step but the row's last fills all 64 lanes: a window piece
-            // averages a few dozen entries.  Lane q < np holds the q-th non-empty piece: its position E in the concatenation and the
-            // shift (first entry - E) that turns a position of that piece into an entry index.
-            const int len = phi - plo;
-            const unsigned int ne = __ballot_sync(0xffffffffu, len > 0);
-            int ex = len;
-            for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, ex, o); if (lane >= o) ex += v; }
-            const int tot = __shfl_sync(0xffffffffu, ex, 31), np = __popc(ne);
-            ex -= len;
-            const int src = lane < np ? (int)__fns(ne, 0u, lane + 1) : 0;
-            const int pE = __shfl_sync(0xffffffffu, ex, src), pshift = __shfl_sync(0xffffffffu, plo - ex, src);
-            for (int G = 0; G < tot; G += 64) {                 // two entries per lane: half the loop / vote / push overhead per entry
-                const int ia = flat_entry(G, lane, np, pE, pshift, tot), ib = flat_entry(G + 32, lane, np, pE, pshift, tot);
-                const bool pa = entry_may_match(S, ia, kr.x, kr.y, rall, rA, rB) & (G + lane < tot);
-                const bool pb = entry_may_match(S, ib, kr.x, kr.y, rall, rA, rB) & (G + 32 + lane < tot);
-                const unsigned int ba = __ballot_sync(0xffffffffu, pa), bb = __ballot_sync(0xffffffffu, pb);
-                if (ba | bb) {
-                    if (pa) S.queue[warp][qn + __popc(ba & lt_mask)] = ((unsigned int)rl << 24) | (unsigned int)ia;
-                    qn += __popc(ba);
-                    if (pb) S.queue[warp][qn + __popc(bb & lt_mask)] = ((unsigned int)rl << 24) | (unsigned int)ib;
-                    qn += __popc(bb);
-                    __syncwarp();
-                    if (qn >= 32) {
-                        do { qn -= 32; exact_batch<SEM, KEEP>(S, S.queue[warp][qn + lane], true, lane); } while (qn >= 32);
-                        rB.w = S.rowB[rl].w;
+        MPROBE(probe_add(S, warp, lane, MP_WAIT, clock64() - t_wait);)
+        for (int taken = 0;; ++taken) {
+            // next row: single pass, the next untaken row of the unit; several passes, the warp's fixed rows
+            int rl = warp * MK_SLOTS + taken;
+            if (S.npass == 1) {
+                if (lane == 0) rl = atomicAdd(&S.next_row, 1);
+                rl = __shfl_sync(0xffffffffu, rl, 0);
+            } else if (taken == MK_SLOTS) break;
+            if (rl >= S.nrows) break;
+            const int sl = warp * MK_SLOTS + taken % MK_SLOTS;
+            if (pass == 0) {
+                if (taken >= MK_SLOTS) {               // the slot's previous row: its queued candidates first (rarely any), then its result
+                    if (__any_sync(0xffffffffu, lane < qn && (S.queue[warp][lane] >> 24) == (unsigned int)sl)) {
+                        MPROBE(probe_add(S, warp, lane, MP_DRAINS, 1);)
+                        drain_queue<SEM, KEEP>(S, warp, lane, qn);
                     }
+                    MPROBE(const long long t0 = clock64();)
+                    finalize_row<SEM, KEEP>(S, sl, lane);
+                    MPROBE(probe_add(S, warp, lane, MP_FINAL, clock64() - t0);)
                 }
+                MPROBE(const long long t0 = clock64();)
+                setup_row(S, sl, rl, lane);
+                MPROBE(probe_add(S, warp, lane, MP_SETUP, clock64() - t0); probe_add(S, warp, lane, MP_ROWS, 1);)
             }
+            scan_row<SEM, KEEP>(S, sl, base, cnt, warp, lane, qn);
         }
-        __syncwarp();
-        if (qn > 0) {                                  // the queue holds ring positions: empty it before the ring is refilled
-            const bool has = lane < qn;
-            exact_batch<SEM, KEEP>(S, has ? S.queue[warp][lane] : 0u, has, lane);
-            qn = 0;
-        }
+        drain_queue<SEM, KEEP>(S, warp, lane, qn);     // the queue holds ring positions: empty it before the ring is refilled
     }
-    __syncwarp();
-
-    finalize_rows<SEM, KEEP>(S, warp, lane, nrows, R0, A.counts, A.recs);
+    MPROBE(const long long t_fin = clock64();)
+    for (int i = 0; i < MK_SLOTS; ++i) {
+        const int sl = warp * MK_SLOTS + i;
+        if (S.slot_row[sl] >= 0) finalize_row<SEM, KEEP>(S, sl, lane);
+    }
+#ifdef L3D_MATCH_PROBE
+    const long long t_done = clock64();
+    probe_add(S, warp, lane, MP_FINAL, t_done - t_fin);
+    __shared__ unsigned long long busy[MK_WARPS];
+    if (lane == 0) busy[warp] = (unsigned long long)(t_done - t_start);
+    __syncthreads();
+    probe_add(S, warp, lane, MP_TAIL, clock64() - t_done);
+    __syncthreads();
+    if (tid == 0) {
+        unsigned long long mx = 0ull, mn = ~0ull, sum = 0ull;
+        for (int w = 0; w < MK_WARPS; ++w) { mx = max(mx, busy[w]); mn = min(mn, busy[w]); sum += busy[w]; }
+        S.probe[0][MP_CTAS] += 1; S.probe[0][MP_BUSY_MAX] += mx; S.probe[0][MP_BUSY_MIN] += mn; S.probe[0][MP_BUSY_SUM] += sum;
+    }
+    __syncthreads();
+    if (tid < MP_N) {
+        unsigned long long v = 0ull;
+        for (int w = 0; w < MK_WARPS; ++w) v += S.probe[w][tid];
+        atomicAdd(&g_match_probe[tid], v);
+    }
+#endif
 }
 
 static_assert(L3D_SEM_REF_GPU == 0 && L3D_SEM_REF_CPU == 1 && (int)Keep::TopK == 0 && (int)Keep::Count == 1 && (int)Keep::Store == 2,

@@ -3,26 +3,26 @@
 #include "l3d_device.cuh"
 #include "../../include/l3d_capi.h"
 
-/* geometry of k_match_topk; every knob can be overridden with -D for the tile sweep (tools/sweep_tiles.py) */
+/* geometry of k_match_topk (one CTA per SM); every knob can be overridden with -D for the sweep (tools/sweep_tiles.py) */
 #ifndef MK_WARPS
-#define MK_WARPS 8
+#define MK_WARPS 24
 #endif
 #define MK_THREADS (32 * MK_WARPS)
-#ifndef MK_RPW
-#define MK_RPW 8                        /* source rows per warp */
+#ifndef MK_SLOTS
+#define MK_SLOTS 8                      /* row slots per warp: key list, threshold, count and constants of a row in flight */
 #endif
-#define MK_ROWS (MK_WARPS * MK_RPW)     /* source rows per CTA  */
+#define MK_NSLOT (MK_WARPS * MK_SLOTS)  /* row slots per CTA; also the most rows of a unit whose target view takes several passes */
+#ifndef MK_UNIT_ROWS
+#define MK_UNIT_ROWS 1024               /* most source rows per work unit (one CTA) of a pair whose target view is resident */
+#endif
 #ifndef MK_TT
 #define MK_TT 512                       /* level-1 entries (target segments) per TMA stage (16 B arc + 16 B segment each: 16 KB) */
 #endif
 #ifndef MK_STAGES
-#define MK_STAGES 3                     /* TMA ring depth: 1536 target segments resident; larger target views take several passes */
+#define MK_STAGES 6                     /* TMA ring depth: 3072 target segments resident; larger target views take several passes */
 #endif
 #ifndef MK_CAP
 #define MK_CAP 32                       /* survivor keys kept per row before pruning to k (<= 32: one key per lane) */
-#endif
-#ifndef MK_MINB
-#define MK_MINB 3                       /* resident CTAs per SM the register budget is tuned for */
 #endif
 
 #define DK_THREADS 256
@@ -45,7 +45,7 @@ __global__ void k_prep_segments(const float4* __restrict__ segs, const L3DViewDe
 // parameters of k_match_topk, passed by value
 struct MatchArgs {
     const float4* segs; const float4* cache; const double* cache_d;       // segments, their float / double ray caches (cache_d: REF_CPU)
-    const L3DViewDev* views; const L3DPairDev* pairs; const int2* tiles;  // tiles: (pair, first source row) of every CTA
+    const L3DViewDev* views; const L3DPairDev* pairs; const int4* units;  // units: (pair, first source row, rows, 0) of every CTA
     const uint4* arcs; const float4* arc_segs;                            // level-1 table (k_arcs_gather): packed arcs and their target segments,
     const L3DPairBasis* basis;                                            // both in window order; the pencil bases (k_pair_arcs)
     int* counts; l3d_match_rec* recs;                                     // per-row match count and records
@@ -55,6 +55,12 @@ struct MatchArgs {
 // what k_match_topk keeps of the matches of a row: the kNN best, only their number, or all of them
 enum class Keep { TopK, Count, Store };
 template <int SEM, Keep KEEP> __global__ void k_match_topk(MatchArgs A);    // SEM: L3D_SEM_REF_GPU / L3D_SEM_REF_CPU
+#ifdef L3D_MATCH_PROBE
+/* probe build only (tools/probe_match_phases.py): clock64 spans of every warp by phase, counters, and per CTA the longest, shortest and
+   summed warp busy time, all summed over the CTAs of the launches since the last reset; read with l3d_match_probe (extern "C") */
+enum { MP_SETUP, MP_SCAN, MP_EXACT, MP_FINAL, MP_WAIT, MP_TAIL, MP_ROWS, MP_ENTRIES, MP_SURVIVORS, MP_EVALS, MP_DRAINS,
+       MP_CTAS, MP_BUSY_MAX, MP_BUSY_MIN, MP_BUSY_SUM, MP_N };
+#endif
 extern void (*const l3d_match_kernels[2][3])(MatchArgs);                   // every instantiation of k_match_topk: [SEM][KEEP]
 // level-1 pre-filter tables: one CTA per view pair of [first_pair, first_pair + gridDim.x): raw arcs + sort keys; after the sort
 // k_arcs_gather writes the packed arcs and, in a parallel array, their target segments, in window order
