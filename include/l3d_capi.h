@@ -128,6 +128,23 @@ int l3d_pair_row_offsets(l3d_ctx* ctx, long long* row_off_out);
 /* pure host helper: contiguous split of n items with the given costs into `parts` ranges of near-equal cost;
  * bounds_out[parts+1], bounds_out[0] = 0, bounds_out[parts] = n. The same split on every rank. */
 int l3d_balanced_split(const long long* cost, int n, int parts, int32_t* bounds_out);
+/* in-process multi-GPU form of the sharded path: gather the rows of contexts that each matched a range of the same pair list into
+ * dst.  Source i (src[i], any device, dst itself allowed) must hold the result of l3d_match_pairs_range / l3d_match_pairs_f64 over
+ * exactly [pair_bounds[i], pair_bounds[i+1]) of the pair list dst matched: the same pairs, matrices, views, semantics, epi_overlap and
+ * kNN.  pair_bounds[n_src+1] is non-decreasing within [0, num_pairs].  Afterwards dst holds what ONE such call over [pair_bounds[0],
+ * pair_bounds[n_src]) would have left (the whole job for 0 and num_pairs): the same counts (0 outside that range), the same records up
+ * to each row's count, the same l3d_match_stride, l3d_match_pair_evals and l3d_match_total_matches.
+ *   1 <= kNN <= 32: the stride is kNN everywhere and rows are copied as they are.  kNN <= 0 or > 32: every source's stride is its own
+ *   longest row; the gathered stride is the largest of them (what one context computes), dst re-lays its own rows if it has to, and
+ *   the sources' rows are copied pitched (no kernel).
+ * Asynchronous: dst's stream waits on an event recorded on every source's stream, so no host synchronisation is needed before the
+ * call; the copies run on dst's stream.  The sources' buffers must stay alive and unchanged (no destroy, no new match call on them)
+ * until dst's stream has passed the copies (l3d_sync(dst)).  Peer access to the sources' devices is enabled where the hardware allows
+ * it (process-local runtime state); otherwise the runtime stages the copies.  Sources on dst's own device are plain device copies.
+ * Errors: L3D_ERR_STATE for a dst or source without a match result, L3D_ERR_INVALID for another pair list or bounds that do not
+ * match what the sources evaluated.  Failed or not, dst's scoring sweep and everything after it are dropped; a failed call also
+ * drops dst's match result. */
+int l3d_match_gather(l3d_ctx* dst, int n_src, l3d_ctx* const* src, const int32_t* pair_bounds);
 /* sizes of the last l3d_match_pairs result */
 long long l3d_match_total_rows(const l3d_ctx* ctx);      /* sum of Ns over pairs */
 long long l3d_match_total_matches(l3d_ctx* ctx);         /* matches of the last result (sum of the row counts), reduced on the device */

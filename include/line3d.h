@@ -136,6 +136,7 @@ struct Line3DStats {
     long long view_pairs, pair_evaluations, matches_after_knn, estimates, affinity_entries, affinity_rows, clusters_total,
         clusters_valid, lines3D, collinear_entries, opt_iterations;
     double ms_match, ms_score, ms_affinity, ms_diffusion, ms_cluster, opt_cost_before, opt_cost_after;
+    double ms_gather;      /* the part of ms_match that gathered the other devices' rows on the first one (device time); 0 on one device */
 };
 
 class Line3D {
@@ -145,6 +146,14 @@ public:
     Line3D(const std::string& output_folder, const bool load_segments = L3D_DEF_LOAD_AND_STORE_SEGMENTS,
            const int max_img_width = L3D_DEF_MAX_IMG_WIDTH, const unsigned int max_line_segments = L3D_DEF_MAX_NUM_SEGMENTS,
            const bool neighbors_by_worldpoints = true, const bool use_GPU = true, const int cuda_device = 0);
+    /* The same on several GPUs (an addition): cuda_devices[0] is the primary, where the scoring sweep, affinity, diffusion, clustering
+     * and bundling run and where the results live.  matchImages splits the view pairs over all listed devices by cost (Ns * Nt), matches
+     * every share from its own host thread and gathers the rows on the primary (l3d_match_gather), so the results, stats included, are
+     * those of one device bit for bit.  A device may be listed more than once (several contexts on one GPU).  Every device holds all
+     * segments and the count / record arrays of the whole job (DESIGN.md §5).  Throws std::invalid_argument for an empty list and
+     * std::runtime_error if a device cannot be used.  The constructor above means {cuda_device}. */
+    Line3D(const std::string& output_folder, const bool load_segments, const int max_img_width, const unsigned int max_line_segments,
+           const bool neighbors_by_worldpoints, const bool use_GPU, const std::vector<int>& cuda_devices);
     ~Line3D();
     Line3D(const Line3D&) = delete;
     Line3D& operator=(const Line3D&) = delete;
@@ -255,7 +264,9 @@ public:
      * `exchange(user, counts_dev, recs_dev, row_bounds, world, knn)`: rank r owns rows [row_bounds[r], row_bounds[r+1]) of
      * counts (int32 per row) and recs (knn * 24 B per row), both DEVICE pointers; on return every rank must hold all rows
      * (an NCCL broadcast per owner; line3dpp_b200/dist.py does it with torch.distributed). Scoring, affinity, diffusion and
-     * clustering then run replicated, so every rank ends with the single-GPU result bit for bit. Return 0 on success. */
+     * clustering then run replicated, so every rank ends with the single-GPU result bit for bit. Return 0 on success.
+     * With several devices per Line3D, they split this rank's share and gather it on the primary before the exchange, which then
+     * sees the primary's buffers. */
     typedef int (*MatchExchangeFn)(void* user, void* counts_dev, void* recs_dev, const long long* row_bounds, int world, int knn);
     void setShard(int rank, int world, MatchExchangeFn exchange, void* user);
     struct Impl;

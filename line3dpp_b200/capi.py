@@ -196,6 +196,16 @@ class Context:
         self._chk(self.L.l3d_match_device_buffers(self.h, C.byref(a), C.byref(b)), "l3d_match_device_buffers")
         return a.value or 0, b.value or 0
 
+    def match_gather(self, sources, pair_bounds):
+        """l3d_match_gather: bring the rows of `sources` (Contexts, this one allowed), source i having matched the pairs
+        [pair_bounds[i], pair_bounds[i+1]) of this context's pair list, into this context; asynchronous on its stream"""
+        b = np.ascontiguousarray(pair_bounds, np.int32)
+        if len(b) != len(sources) + 1:
+            raise ValueError("pair_bounds needs one entry per source + 1")
+        hs = (C.c_void_p * len(sources))(*[s.h.value for s in sources])
+        self._chk(self.L.l3d_match_gather(self.h, len(sources), hs, _p(b)), "l3d_match_gather")
+        self._knn = int(self.L.l3d_match_stride(self.h))
+
     def pair_row_offsets(self, num_pairs):
         out = np.zeros(num_pairs + 1, np.int64)
         self._chk(self.L.l3d_pair_row_offsets(self.h, _p(out)), "l3d_pair_row_offsets")

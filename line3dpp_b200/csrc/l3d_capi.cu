@@ -40,6 +40,9 @@ int DevBuf::reserve(l3d_ctx* c, size_t bytes, const char* what)
 
 struct CastI64 { __host__ __device__ long long operator()(int v) const { return (long long)v; } };
 
+// the most dynamic shared memory k_sort_rows gets (run_keep_all: the rows of the CTA's warps at the keep-all stride)
+static const size_t SORT_SMEM_MAX = 200 * 1024;
+
 extern "C" {
 
 int l3d_ctx_create(int device, l3d_ctx** out)
@@ -61,6 +64,9 @@ int l3d_ctx_create(int device, l3d_ctx** out)
     for (const auto& by_keep : l3d_match_kernels)
         for (auto k : by_keep)
             if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l3d_match_smem_bytes());
+    // once, at the most any launch uses: the attribute is per device, and a per-launch setting would race between contexts that match
+    // on one device from several host threads
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_sort_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SORT_SMEM_MAX);
     if (e != cudaSuccess) { cudaStreamDestroy(c->stream); delete c; return L3D_ERR_CUDA; }
     *out = c;
     return L3D_OK;
@@ -228,6 +234,7 @@ static int stage_pairs(l3d_ctx* c, int num_pairs, const int32_t* pairs, const fl
         if (i >= first_pair && i < last_pair) evals += (long long)Ns * Nt;     // evaluated HERE
     }
     c->num_pairs = num_pairs; c->knn = knn; c->epi = epi_overlap; c->total_rows = rows; c->pair_evals = evals;
+    c->knn_asked = std::max(knn, 0); c->first_pair = first_pair; c->last_pair = last_pair;
     int rc;
     L3D_RESERVE(c->d_pairs, sizeof(L3DPairDev) * (size_t)std::max(num_pairs, 1), "pairs");
     L3D_RESERVE(c->d_units, sizeof(int4) * std::max<size_t>(c->h_units.size(), 1), "tiles");
@@ -361,11 +368,10 @@ static int run_keep_all(l3d_ctx* c, MatchArgs a, int big_k)
     if (nunits) {
         const size_t per_warp = sizeof(l3d_match_rec) * (size_t)stride;
         int wpb = 4;
-        while (wpb > 1 && per_warp * wpb > 200 * 1024) wpb >>= 1;
-        if (per_warp * wpb > 200 * 1024) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: a row with more than 8500 matches (kNN <= 0)");
+        while (wpb > 1 && per_warp * wpb > SORT_SMEM_MAX) wpb >>= 1;
+        if (per_warp * wpb > SORT_SMEM_MAX) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: a row with more than 8500 matches (kNN <= 0)");
         a.knn = stride; a.recs = (l3d_match_rec*)c->d_recs.p;
         if ((rc = launch_match(c, Keep::Store, a, 0, nunits, "k_match_topk (store)"))) return rc;
-        L3D_CUDA(c, cudaFuncSetAttribute(k_sort_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(per_warp * wpb)), "k_sort_rows smem");
         const long long blocks = std::min<long long>((rows + wpb - 1) / wpb, (long long)c->num_sms * 16);
         k_sort_rows<<<(unsigned int)blocks, wpb * 32, per_warp * wpb, c->stream>>>((int*)c->d_counts.p, (l3d_match_rec*)c->d_recs.p, stride, rows, big_k);
         L3D_CUDA(c, cudaGetLastError(), "k_sort_rows");
@@ -440,6 +446,157 @@ int l3d_balanced_split(const long long* cost, int n, int parts, int32_t* bounds)
         before += cost[i];
     }
     while (part < parts) bounds[++part] = n;
+    return L3D_OK;
+}
+
+}   // extern "C"
+
+// ------------------------------------------------------------------------------------------------ gathering match rows
+// whether s holds a match result of the same job as d: the same views' sizes, pairs, matrices, rows, semantics, epi and kNN request
+static bool same_job(const l3d_ctx* d, const l3d_ctx* s)
+{
+    if (s->num_pairs != d->num_pairs || s->total_rows != d->total_rows || s->semantics != d->semantics || s->epi != d->epi ||
+        s->knn_asked != d->knn_asked || s->num_views != d->num_views)
+        return false;
+    for (int v = 0; v < d->num_views; ++v)
+        if (s->h_views[v].nseg != d->h_views[v].nseg) return false;
+    for (int i = 0; i < d->num_pairs; ++i) {
+        const L3DPairDev &a = d->h_pairs[i], &b = s->h_pairs[i];
+        if (a.src != b.src || a.tgt != b.tgt || a.row_off != b.row_off || memcmp(a.F, b.F, sizeof(a.F)) || memcmp(a.Fd, b.Fd, sizeof(a.Fd))) return false;
+    }
+    return true;
+}
+
+static int gather_check(l3d_ctx* d, int n, l3d_ctx* const* src, const int32_t* b)
+{
+    char msg[160];
+    if (n < 1 || !src || !b) return l3d_fail(d, L3D_ERR_INVALID, "l3d_match_gather: bad arguments");
+    if (!d->have_matches) return l3d_fail(d, L3D_ERR_STATE, "l3d_match_gather: the destination has no match result");
+    if (b[0] < 0 || b[n] > d->num_pairs) return l3d_fail(d, L3D_ERR_INVALID, "l3d_match_gather: pair bounds outside the pair list");
+    for (int i = 0; i < n; ++i) {
+        const l3d_ctx* s = src[i];
+        if (!s || b[i + 1] < b[i]) return l3d_fail(d, L3D_ERR_INVALID, "l3d_match_gather: null source or decreasing pair bounds");
+        if (!s->have_matches) {
+            snprintf(msg, sizeof(msg), "l3d_match_gather: source %d has no match result", i);
+            return l3d_fail(d, L3D_ERR_STATE, msg);
+        }
+        if (!same_job(d, s)) {
+            snprintf(msg, sizeof(msg), "l3d_match_gather: source %d matched another pair list, semantics, epi or kNN", i);
+            return l3d_fail(d, L3D_ERR_INVALID, msg);
+        }
+        if (s->first_pair != b[i] || s->last_pair != b[i + 1]) {
+            snprintf(msg, sizeof(msg), "l3d_match_gather: source %d evaluated pairs [%d, %d), not [%d, %d)", i, s->first_pair, s->last_pair, b[i], b[i + 1]);
+            return l3d_fail(d, L3D_ERR_INVALID, msg);
+        }
+    }
+    return L3D_OK;
+}
+
+// the first row of pair p, total_rows for p == num_pairs
+static long long row_of_pair(const l3d_ctx* c, int p) { return p < c->num_pairs ? c->h_pairs[p].row_off : c->total_rows; }
+
+static cudaError_t copy_rows(l3d_ctx* d, void* dp, const l3d_ctx* s, const void* sp, size_t bytes)
+{
+    return s->device == d->device ? cudaMemcpyAsync(dp, sp, bytes, cudaMemcpyDeviceToDevice, d->stream)
+                                  : cudaMemcpyPeerAsync(dp, d->device, sp, s->device, bytes, d->stream);
+}
+
+// `height` rows of `width` bytes from a pitch of spitch to one of dpitch
+static cudaError_t copy_pitched(l3d_ctx* d, void* dp, size_t dpitch, const l3d_ctx* s, const void* sp, size_t spitch, size_t width, size_t height)
+{
+    if (s->device == d->device) return cudaMemcpy2DAsync(dp, dpitch, sp, spitch, width, height, cudaMemcpyDeviceToDevice, d->stream);
+    cudaMemcpy3DPeerParms p = {};
+    p.srcPtr = make_cudaPitchedPtr(const_cast<void*>(sp), spitch, width, height); p.srcDevice = s->device;
+    p.dstPtr = make_cudaPitchedPtr(dp, dpitch, width, height); p.dstDevice = d->device;
+    p.extent = make_cudaExtent(width, height, 1);
+    return cudaMemcpy3DPeerAsync(&p, d->stream);
+}
+
+// direct copies from `peer` where the hardware allows it; otherwise cudaMemcpyPeerAsync stages through the host.  Peer access is state of
+// this process's runtime, not a device setting.  The current device is d's.
+static int enable_peer(l3d_ctx* d, int peer)
+{
+    int can = 0;
+    L3D_CUDA(d, cudaDeviceCanAccessPeer(&can, d->device, peer), "cudaDeviceCanAccessPeer");
+    if (!can) return L3D_OK;
+    const cudaError_t e = cudaDeviceEnablePeerAccess(peer, 0);
+    if (e == cudaErrorPeerAccessAlreadyEnabled) { cudaGetLastError(); return L3D_OK; }
+    L3D_CUDA(d, e, "cudaDeviceEnablePeerAccess");
+    return L3D_OK;
+}
+
+// d's stream waits until s's stream has passed everything enqueued so far (s's match result is complete)
+static int wait_for(l3d_ctx* d, l3d_ctx* s)
+{
+    cudaEvent_t ev;
+    cudaSetDevice(s->device);
+    cudaError_t e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+    if (e == cudaSuccess) {
+        e = cudaEventRecord(ev, s->stream);
+        cudaSetDevice(d->device);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(d->stream, ev, 0);
+        cudaEventDestroy(ev);               // released once the wait has passed it
+    }
+    cudaSetDevice(d->device);
+    L3D_CUDA(d, e, "l3d_match_gather: wait for a source");
+    return L3D_OK;
+}
+
+// The rows [row_of_pair(b[0]), row_of_pair(b[n])) from their sources, at the stride one context matching all those pairs would have
+// chosen: kNN for top-k; for keep-all the longest row, i.e. the largest of the sources' strides.  Rows outside get count 0.
+static int gather_rows(l3d_ctx* d, int n, l3d_ctx* const* src, const int32_t* b)
+{
+    cudaSetDevice(d->device);
+    const size_t REC = sizeof(l3d_match_rec);
+    const bool topk = d->knn_asked >= 1 && d->knn_asked <= 32;
+    int stride = topk ? d->knn_asked : 1, rc;
+    bool d_is_src = false;
+    for (int i = 0; i < n; ++i) { stride = std::max(stride, src[i]->knn); d_is_src |= src[i] == d; }
+    if (!topk && stride != d->knn) {
+        if (d_is_src) {     // re-lay d's own rows at the wider stride (d's stride is one of the maximum's terms, so it is the smaller)
+            const long long a = row_of_pair(d, d->first_pair), z = row_of_pair(d, d->last_pair);
+            DevBuf wide;
+            if ((rc = wide.reserve(d, REC * (size_t)std::max<long long>(d->total_rows, 1) * stride, "gathered match records"))) return rc;
+            if (z > a)
+                L3D_CUDA(d, cudaMemcpy2DAsync((char*)wide.p + REC * a * stride, REC * stride, (const char*)d->d_recs.p + REC * a * d->knn, REC * d->knn,
+                                              REC * d->knn, (size_t)(z - a), cudaMemcpyDeviceToDevice, d->stream), "re-lay match records");
+            L3D_CUDA(d, cudaStreamSynchronize(d->stream), "re-lay match records");   // the old buffer is freed below
+            std::swap(d->d_recs, wide);
+        } else if ((rc = d->d_recs.reserve(d, REC * (size_t)std::max<long long>(d->total_rows, 1) * stride, "gathered match records")))
+            return rc;
+        d->knn = stride;
+    }
+    const long long r0 = row_of_pair(d, b[0]), r1 = row_of_pair(d, b[n]);
+    if (r0 > 0) L3D_CUDA(d, cudaMemsetAsync(d->d_counts.p, 0, sizeof(int) * r0, d->stream), "clear counts");
+    if (r1 < d->total_rows) L3D_CUDA(d, cudaMemsetAsync((int*)d->d_counts.p + r1, 0, sizeof(int) * (d->total_rows - r1), d->stream), "clear counts");
+    for (int i = 0; i < n; ++i) {
+        l3d_ctx* s = src[i];
+        const long long a = row_of_pair(d, b[i]), z = row_of_pair(d, b[i + 1]);
+        if (s == d || z <= a) continue;
+        if (s->device != d->device && (rc = enable_peer(d, s->device))) return rc;
+        if ((rc = wait_for(d, s))) return rc;
+        L3D_CUDA(d, copy_rows(d, (int*)d->d_counts.p + a, s, (const int*)s->d_counts.p + a, sizeof(int) * (size_t)(z - a)), "l3d_match_gather: copy counts");
+        char* dr = (char*)d->d_recs.p + REC * a * stride;
+        const char* sr = (const char*)s->d_recs.p + REC * a * s->knn;
+        L3D_CUDA(d, s->knn == stride ? copy_rows(d, dr, s, sr, REC * stride * (size_t)(z - a))
+                                     : copy_pitched(d, dr, REC * stride, s, sr, REC * s->knn, REC * s->knn, (size_t)(z - a)),
+                 "l3d_match_gather: copy records");
+    }
+    long long evals = 0;
+    for (int p = b[0]; p < b[n]; ++p) evals += (long long)d->h_views[d->h_pairs[p].src].nseg * d->h_views[d->h_pairs[p].tgt].nseg;
+    d->pair_evals = evals; d->first_pair = b[0]; d->last_pair = b[n];
+    return L3D_OK;
+}
+
+extern "C" {
+
+int l3d_match_gather(l3d_ctx* dst, int n_src, l3d_ctx* const* src, const int32_t* pair_bounds)
+{
+    if (!dst) return L3D_ERR_INVALID;
+    int rc = gather_check(dst, n_src, src, pair_bounds);
+    dst->drop(Stage::Matches);              // also on success: the rows change under the sweep and what follows it
+    if (rc || (rc = gather_rows(dst, n_src, src, pair_bounds))) return rc;
+    dst->have_matches = true;
     return L3D_OK;
 }
 

@@ -108,7 +108,9 @@ struct l3d_ctx {
 
     // last match result
     bool have_matches = false;
-    int num_pairs = 0, knn = 0;
+    int num_pairs = 0, knn = 0;             // knn: the row stride of d_recs
+    int knn_asked = 0;                      // the kNN of the call (<= 0 as 0), which picks top-k or keep-all
+    int first_pair = 0, last_pair = 0;      // the pairs evaluated: [first_pair, last_pair)
     float epi = 0.f;
     int semantics = 0;                      // L3D_SEM_* of the last match result; the scoring sweep follows it
     long long total_rows = 0, pair_evals = 0;

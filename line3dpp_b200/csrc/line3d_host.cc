@@ -186,7 +186,8 @@ void Segment3D::translate(const Vector3d& t) { P1_ = P1_ + t; P2_ = P2_ + t; }
 
 // ------------------------------------------------------------------------------------------------ Line3D::Impl
 struct Line3D::Impl {
-    l3d_ctx* ctx = nullptr;
+    l3d_ctx* ctx = nullptr;                               // the primary: ctxs[0]
+    std::vector<l3d_ctx*> ctxs; std::vector<int> devices; // one context per listed device (matchImages splits the pairs over them)
     std::string output_folder, err;
     bool load_segments, by_wps, use_gpu, verbose = false;
     int max_img_width; unsigned int max_line_segments;
@@ -330,15 +331,31 @@ void Line3D::Impl::neighbors_from_wps(unsigned int camID)
 // ------------------------------------------------------------------------------------------------ Line3D
 Line3D::Line3D(const std::string& output_folder, const bool load_segments, const int max_img_width, const unsigned int max_line_segments,
                const bool neighbors_by_worldpoints, const bool use_GPU, const int cuda_device)
-    : p_(new Impl())
+    : Line3D(output_folder, load_segments, max_img_width, max_line_segments, neighbors_by_worldpoints, use_GPU, std::vector<int>(1, cuda_device))
 {
+}
+Line3D::Line3D(const std::string& output_folder, const bool load_segments, const int max_img_width, const unsigned int max_line_segments,
+               const bool neighbors_by_worldpoints, const bool use_GPU, const std::vector<int>& cuda_devices)
+    : p_(nullptr)
+{
+    if (cuda_devices.empty()) throw std::invalid_argument("L3DPP::Line3D: the device list is empty");
+    p_ = new Impl();
     p_->output_folder = output_folder; p_->load_segments = load_segments; p_->max_img_width = max_img_width;
     p_->max_line_segments = max_line_segments; p_->by_wps = neighbors_by_worldpoints; p_->use_gpu = use_GPU;
     memset(&p_->st, 0, sizeof(p_->st));
-    const int rc = l3d_ctx_create(cuda_device, &p_->ctx);
-    if (rc != L3D_OK) { delete p_; p_ = nullptr; throw std::runtime_error("L3DPP::Line3D: no usable CUDA device - this build has no CPU path"); }
+    for (const int dev : cuda_devices) {
+        l3d_ctx* c = nullptr;
+        if (l3d_ctx_create(dev, &c) != L3D_OK) {
+            for (l3d_ctx* x : p_->ctxs) l3d_ctx_destroy(x);
+            delete p_; p_ = nullptr;
+            throw std::runtime_error(cuda_devices.size() == 1 ? std::string("L3DPP::Line3D: no usable CUDA device - this build has no CPU path")
+                                                              : "L3DPP::Line3D: no usable CUDA device " + std::to_string(dev) + " - this build has no CPU path");
+        }
+        p_->ctxs.push_back(c);
+    }
+    p_->ctx = p_->ctxs[0]; p_->devices = cuda_devices;
 }
-Line3D::~Line3D() { if (p_) { l3d_ctx_destroy(p_->ctx); delete p_; } }
+Line3D::~Line3D() { if (p_) { for (l3d_ctx* c : p_->ctxs) l3d_ctx_destroy(c); delete p_; } }
 const Line3DStats& Line3D::stats() const { return p_->st; }
 const char* Line3D::lastError() const { return p_->err.c_str(); }
 void Line3D::setVerbose(bool v) { p_->verbose = v; }
@@ -450,15 +467,57 @@ void Line3D::matchImages(const float sigma_position, const float sigma_angle, co
     bool ok = P.chk(l3d_set_views(P.ctx, (int)d.size(), d.data(), segp.data()), "l3d_set_views");
     // use_GPU selects the reference's semantics, not the processor (line3D.cc:708-757): true = K_match_lines / K_score_matches
     // float arithmetic, false = matchingCPU / scoringCPU double arithmetic.  Both run on the GPU.
-    auto match_range = [&](int first, int last) {
-        return P.use_gpu ? P.chk(l3d_match_pairs_range(P.ctx, npairs, P.pairs.data(), F.data(), P.epi, P.kNN, first, last), "l3d_match_pairs_range")
-                         : P.chk(l3d_match_pairs_f64(P.ctx, npairs, P.pairs.data(), Fdbl.data(), P.epi, P.kNN, first, last), "l3d_match_pairs_f64");
+    const char* match_what = P.use_gpu ? "l3d_match_pairs_range" : "l3d_match_pairs_f64";
+    auto match_on = [&](l3d_ctx* c, int first, int last) {
+        return P.use_gpu ? l3d_match_pairs_range(c, npairs, P.pairs.data(), F.data(), P.epi, P.kNN, first, last)
+                         : l3d_match_pairs_f64(c, npairs, P.pairs.data(), Fdbl.data(), P.epi, P.kNN, first, last);
+    };
+    auto pair_cost = [&](int i) { return (long long)P.vlist[P.pairs[2 * i]]->lines.size() * (long long)P.vlist[P.pairs[2 * i + 1]]->lines.size(); };
+    float ms_gather = 0.0f;
+    // The pairs [first, last) on the primary.  With several devices every one takes a contiguous share balanced by Ns*Nt, uploads the
+    // views and matches its share from its own host thread (keep-all waits on the host between its count and store passes, so one
+    // thread would serialise the devices), and the shares are gathered on the primary's stream.  The threads share no mutable host
+    // state: each works on its own context and writes only its own error slot.
+    auto match_range = [&](int first, int last) -> bool {
+        if (P.ctxs.size() == 1) return P.chk(match_on(P.ctx, first, last), match_what);
+        const int nd = (int)P.ctxs.size();
+        std::vector<long long> cost((size_t)(last - first));
+        for (int i = first; i < last; ++i) cost[i - first] = pair_cost(i);
+        std::vector<int32_t> b((size_t)nd + 1);
+        if (!P.chk(l3d_balanced_split(cost.data(), last - first, nd, b.data()), "l3d_balanced_split")) return false;
+        for (int32_t& x : b) x += first;
+        std::vector<std::string> errs((size_t)nd);
+        auto run = [&](int i) {
+            l3d_ctx* c = P.ctxs[i];
+            const char* what = "l3d_set_views";
+            long long rc = i == 0 ? 0 : l3d_set_views(c, (int)d.size(), d.data(), segp.data());     // the primary has its views already
+            if (rc >= 0) { what = match_what; rc = match_on(c, b[i], b[i + 1]); }
+            if (rc >= 0) { what = "l3d_sync"; rc = l3d_sync(c); }
+            if (rc < 0) errs[i] = "device " + std::to_string(P.devices[i]) + " (#" + std::to_string(i) + "): " + what + ": " + l3d_last_error(c);
+        };
+        std::vector<std::thread> th;
+        for (int i = 1; i < nd; ++i) th.emplace_back(run, i);
+        run(0);
+        for (std::thread& x : th) x.join();
+        for (const std::string& e : errs)
+            if (!e.empty()) { P.fail(e); return false; }
+        cudaSetDevice(P.devices[0]);
+        cudaStream_t s = (cudaStream_t)l3d_stream(P.ctx);
+        cudaEvent_t e0 = nullptr, e1 = nullptr;
+        const bool timed = cudaEventCreate(&e0) == cudaSuccess && cudaEventCreate(&e1) == cudaSuccess && cudaEventRecord(e0, s) == cudaSuccess;
+        bool ok = P.chk(l3d_match_gather(P.ctx, nd, P.ctxs.data(), b.data()), "l3d_match_gather");
+        cudaSetDevice(P.devices[0]);
+        ok = ok && (!timed || cudaEventRecord(e1, s) == cudaSuccess) && P.chk(l3d_sync(P.ctx), "l3d_sync");
+        if (ok && timed) cudaEventElapsedTime(&ms_gather, e0, e1);
+        if (e0) cudaEventDestroy(e0);
+        if (e1) cudaEventDestroy(e1);
+        return ok;
     };
     if (ok && P.shard_world > 1 && (P.kNN <= 0 || P.kNN > 32)) { P.fail("matchImages: kNN <= 0 (keep all matches) or kNN > 32 cannot be sharded: the row stride is only known after matching"); ok = false; }
     if (ok && P.shard_world > 1) {
         // this rank's contiguous share of the pair list, balanced by Ns*Nt; the same split on every rank
         std::vector<long long> cost((size_t)npairs), row_off((size_t)npairs + 1), row_bounds((size_t)P.shard_world + 1);
-        for (int i = 0; i < npairs; ++i) cost[i] = (long long)P.vlist[P.pairs[2 * i]]->lines.size() * (long long)P.vlist[P.pairs[2 * i + 1]]->lines.size();
+        for (int i = 0; i < npairs; ++i) cost[i] = pair_cost(i);
         std::vector<int32_t> bounds((size_t)P.shard_world + 1);
         ok = P.chk(l3d_balanced_split(cost.data(), npairs, P.shard_world, bounds.data()), "l3d_balanced_split") &&
              match_range(bounds[P.shard_rank], bounds[P.shard_rank + 1]) &&
@@ -505,6 +564,7 @@ void Line3D::matchImages(const float sigma_position, const float sigma_angle, co
         P.st.matches_after_knn = l3d_match_total_matches(P.ctx);      // reduced on the device (was: download of the whole count array)
         P.st.ms_match = std::chrono::duration<double, std::milli>(t1 - t0).count();
         P.st.ms_score = std::chrono::duration<double, std::milli>(t2 - t1).count();
+        P.st.ms_gather = ms_gather;
         P.matched = true;
     }
     P.untranslate();
@@ -877,6 +937,15 @@ void* l3dpp_create(int neighbors_by_worldpoints, int use_gpu, int device)
 void* l3dpp_create_in(const char* output_folder, int load_segments, int max_img_width, int neighbors_by_worldpoints, int use_gpu, int device)
 {
     try { return new Line3D(output_folder, load_segments != 0, max_img_width, 3000, neighbors_by_worldpoints != 0, use_gpu != 0, device); } catch (...) { return nullptr; }
+}
+// the device-list constructor; devices[0] is the primary
+void* l3dpp_create_devices(const char* output_folder, int load_segments, int max_img_width, int neighbors_by_worldpoints, int use_gpu, const int* devices,
+                           int num_devices)
+{
+    try {
+        return new Line3D(output_folder, load_segments != 0, max_img_width, 3000, neighbors_by_worldpoints != 0, use_gpu != 0,
+                          std::vector<int>(devices, devices + std::max(num_devices, 0)));
+    } catch (...) { return nullptr; }
 }
 void l3dpp_destroy(void* h) { delete (Line3D*)h; }
 const char* l3dpp_last_error(void* h) { return ((Line3D*)h)->lastError(); }

@@ -16,7 +16,8 @@ RESID_DT = np.dtype([("line", "<i4"), ("cam", "<u4"), ("seg", "<u4")])
 class Stats(C.Structure):
     _fields_ = [(n, C.c_longlong) for n in ("view_pairs", "pair_evaluations", "matches_after_knn", "estimates", "affinity_entries",
                                             "affinity_rows", "clusters_total", "clusters_valid", "lines3D", "collinear_entries", "opt_iterations")] + \
-               [(n, C.c_double) for n in ("ms_match", "ms_score", "ms_affinity", "ms_diffusion", "ms_cluster", "opt_cost_before", "opt_cost_after")]
+               [(n, C.c_double) for n in ("ms_match", "ms_score", "ms_affinity", "ms_diffusion", "ms_cluster", "opt_cost_before", "opt_cost_after",
+                                          "ms_gather")]
 
 
 def _p(a):
@@ -26,9 +27,12 @@ def _p(a):
 class Line3D:
     """addImage / matchImages / reconstruct3Dlines with the reference's argument meaning (line3D.h:80-166)."""
 
-    def __init__(self, neighbors_by_worldpoints=True, use_gpu=True, device=0, output_folder=None, load_segments=True, max_img_width=-1):
+    def __init__(self, neighbors_by_worldpoints=True, use_gpu=True, device=0, output_folder=None, load_segments=True, max_img_width=-1,
+                 devices=None):
         """output_folder / load_segments / max_img_width: the reference's constructor arguments; with an output folder, add_image
-        with no segments reads the segment cache under <output_folder>/L3D++_data/ (segment_cache_path)"""
+        with no segments reads the segment cache under <output_folder>/L3D++_data/ (segment_cache_path).
+        devices: a list of CUDA devices in place of `device` (the first is the primary; repeats allowed): match_images splits the
+        view pairs over them and gathers the matches on the primary, with the single-device result"""
         self.L = capi.lib()
         self.L.l3dpp_create.restype = C.c_void_p
         self.L.l3dpp_create_in.restype = C.c_void_p
@@ -36,14 +40,22 @@ class Line3D:
         self.L.l3dpp_last_error.restype = C.c_char_p
         for n in ("l3dpp_get_affinity", "l3dpp_get_segments3d", "l3dpp_get_residuals", "l3d_get_view_matches", "l3d_get_estimates"):
             getattr(self.L, n).restype = C.c_longlong
-        if output_folder is None:
+        if devices is not None:
+            devs = np.ascontiguousarray([int(d) for d in devices], np.int32)
+            if len(devs) == 0:
+                raise ValueError("devices must name at least one CUDA device")
+            self.L.l3dpp_create_devices.restype = C.c_void_p
+            h = self.L.l3dpp_create_devices(str(output_folder or "").encode(), int(load_segments), int(max_img_width),
+                                            int(neighbors_by_worldpoints), int(use_gpu), _p(devs), len(devs))
+        elif output_folder is None:
             h = self.L.l3dpp_create(int(neighbors_by_worldpoints), int(use_gpu), int(device))
         else:
             h = self.L.l3dpp_create_in(str(output_folder).encode(), int(load_segments), int(max_img_width), int(neighbors_by_worldpoints),
                                        int(use_gpu), int(device))
         self.h = C.c_void_p(h)
         if not self.h:
-            raise capi.L3DError("L3DPP::Line3D: no usable CUDA device (no CPU fallback)")
+            which = "" if devices is None else f" among {list(devices)}"
+            raise capi.L3DError(f"L3DPP::Line3D: no usable CUDA device{which} (no CPU fallback)")
         self.ctx = C.c_void_p(self.L.l3dpp_ctx(self.h))
 
     def close(self):
