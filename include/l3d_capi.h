@@ -228,7 +228,9 @@ long long l3d_affinity_matrix(l3d_ctx* ctx, float two_sigA_sqr, float med_scene_
 /* ---- diffusion: replaces replicator_dynamics_diffusion_GPU (cudawrapper.h:80, cudawrapper.cu:708-766) incl. the
  * SparseMatrix construction it needs (sparsematrix.cc:8-135).  Input: the CLEdge list A_ (clustering.h:47-51) as three
  * arrays and the number of rows n; iters = L3D_DEF_RDD_MAX_ITER (10).  Output: the diffused matrix as row-sorted COO
- * with nnz entries (what the reference downloads from W, line3D.cc:2036-2044).  No ownership transfer. */
+ * with nnz entries (what the reference downloads from W, line3D.cc:2036-2044).  No ownership transfer.
+ * Ids are 0..n-1; an id without entries is allowed.  Each (i, j) may occur once: two equal entries would write one transposed
+ * slot, a race in the reference too.  Weights must be finite and non-negative. */
 int l3d_rdd(l3d_ctx* ctx, int n, long long nnz, const int* ei, const int* ej, const float* ew, int iters, int* out_i,
             int* out_j, float* out_w, float* kernel_ms);
 /* performRDD (line3D.cc:2026-2076) on the affinity matrix that l3d_affinity_matrix left on the device: diffusion + the

@@ -610,9 +610,9 @@ int orc_score_matches_f32(const float* lines, int Ns, const float* matches, int 
     return 0;
 }
 
-// SparseMatrix(A_, n) + replicator_dynamics_diffusion_GPU (cudawrapper.cu:708-766) + download
-int orc_rdd_f32(int nedges, const int* ei, const int* ej, const float* ew, int n, int* out_i, int* out_j,
-                float* out_w, double* wall_ms)
+// SparseMatrix(A_, n) + replicator_dynamics_diffusion_GPU (cudawrapper.cu:708-766) + download, with `iters` iterations
+int orc_rdd_f32_iters(int nedges, const int* ei, const int* ej, const float* ew, int n, int iters, int* out_i, int* out_j,
+                      float* out_w, double* wall_ms)
 {
     auto t0 = std::chrono::steady_clock::now();
     std::list<CLEdge> A;
@@ -626,14 +626,20 @@ int orc_rdd_f32(int nedges, const int* ei, const int* ej, const float* ew, int n
     }
     Pp = P;                                // P_prime = copy of (un-normalised) P  cudawrapper.cu:724
     rdd_row_normalize(P);
-    for (int it = 0; it < RDD_MAX_ITER; ++it) {
+    for (int it = 0; it < iters; ++it) {
         rdd_step(P, W, Pp);
         std::swap(P, Pp);
-        if (it < RDD_MAX_ITER - 1) rdd_row_normalize(P);
+        if (it < iters - 1) rdd_row_normalize(P);
     }
     for (size_t i = 0; i < P.e.size(); ++i) { out_i[i] = (int)P.e[i].x; out_j[i] = (int)P.e[i].y; out_w[i] = P.e[i].z; }
     if (wall_ms) *wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     return 0;
+}
+// the reference's fixed iteration count (L3D_DEF_RDD_MAX_ITER); the signature of ref_rdd (rdd_fn_t)
+int orc_rdd_f32(int nedges, const int* ei, const int* ej, const float* ew, int n, int* out_i, int* out_j,
+                float* out_w, double* wall_ms)
+{
+    return orc_rdd_f32_iters(nedges, ei, ej, ew, n, RDD_MAX_ITER, out_i, out_j, out_w, wall_ms);
 }
 
 int orc_cluster(int nedges, const int* ei, const int* ej, const float* ew, int n, float c, int* labels_out)

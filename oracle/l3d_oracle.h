@@ -48,6 +48,9 @@ int orc_score_matches_f32(const float* lines, int Ns, const float* matches, int 
                           float min_similarity, float* scores_out, float* kernel_ms);
 int orc_rdd_f32(int nedges, const int* ei, const int* ej, const float* ew, int n, int* out_i, int* out_j,
                 float* out_w, double* wall_ms);
+/* the same with `iters` diffusion iterations instead of L3D_DEF_RDD_MAX_ITER (10) */
+int orc_rdd_f32_iters(int nedges, const int* ei, const int* ej, const float* ew, int n, int iters, int* out_i, int* out_j,
+                      float* out_w, double* wall_ms);
 /* find_collinear_segments_GPU + K_collinearity (cudawrapper.cu:370-429, 689-705) / View::findCollinCPU (view.cc:212-263):
  * dense N x N char matrix C[r*N+c] = 1 iff segment c is collinear with segment r (distance threshold dist_t, px) */
 int orc_collinear_f32(const float* lines, int N, float dist_t, unsigned char* C_out, float* kernel_ms);

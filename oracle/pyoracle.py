@@ -112,13 +112,18 @@ def score_matches(fn, lines, matches4, ranges, reg_tgt, RtKinv, Cc, two_sigA_sqr
     return scores, ms.value
 
 
-def rdd(fn, ei, ej, ew, n):
+def rdd(fn, ei, ej, ew, n, iters=None):
+    """fn = lib().orc_rdd_f32 or ref_lib().ref_rdd (10 iterations).  iters (not None): lib().orc_rdd_f32_iters with that many
+    iterations instead of fn.  Returns (out_i, out_j, out_w, wall_ms)."""
     ei, ej = np.ascontiguousarray(ei, np.int32), np.ascontiguousarray(ej, np.int32)
     ew = _f32(ew)
     ne = len(ei)
     oi, oj, ow = np.zeros(ne, np.int32), np.zeros(ne, np.int32), np.zeros(ne, np.float32)
     ms = C.c_double(0)
-    rc = fn(ne, _p(ei), _p(ej), _p(ew), n, _p(oi), _p(oj), _p(ow), C.byref(ms))
+    if iters is None:
+        rc = fn(ne, _p(ei), _p(ej), _p(ew), n, _p(oi), _p(oj), _p(ow), C.byref(ms))
+    else:
+        rc = lib().orc_rdd_f32_iters(ne, _p(ei), _p(ej), _p(ew), n, int(iters), _p(oi), _p(oj), _p(ow), C.byref(ms))
     assert rc == 0, rc
     return oi, oj, ow, ms.value
 
