@@ -481,9 +481,8 @@ static long long affinity_candidates(l3d_ctx* c, float two_sigA_sqr, float med_s
     L3D_RESERVE(A.d_aff_sim, 4 * K, "affinity sims"); L3D_RESERVE(A.d_aff_flag, 4 * K, "affinity flags");
     L3D_RESERVE(A.d_aff_gi, 8 * K, "affinity gi"); L3D_RESERVE(A.d_aff_gj, 8 * K, "affinity gj"); L3D_RESERVE(A.d_evptr, 8 * K, "event offsets");
     if (CL.valid) L3D_RESERVE(A.d_aff_cnt, 4 * K, "event counts");
-    L3D_RESERVE(S.d_order, 4 * V, "order"); L3D_RESERVE(S.d_region_off, 8 * (V + 1), "region offsets");
-    L3D_CUDA(c, cudaMemcpyAsync(S.d_order.p, S.order.data(), 4 * (size_t)V, cudaMemcpyHostToDevice, st), "order");
-    L3D_CUDA(c, cudaMemcpyAsync(S.d_region_off.p, S.region_off.data(), 8 * (size_t)(V + 1), cudaMemcpyHostToDevice, st), "region offsets");
+    // S.d_order and S.d_region_off are the sweep's: it uploads the order and writes the region offsets, and nothing changes them until
+    // the next sweep
     const AffArgs a = {c->views(), (const int*)S.d_order.p, (const long long*)S.d_region_off.p, V,
                        {(const SwView*)S.d_vt.p, (const L3DPairDev*)c->d_pairs.p, (const long long*)S.d_rowoff.p, c->num_pairs, c->knn,
                         (const l3d_match_rec*)c->d_recs.p, (const unsigned int*)S.d_eval.p, (const unsigned char*)S.d_eflag.p},

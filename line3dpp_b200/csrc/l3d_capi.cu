@@ -2,6 +2,7 @@
 // Host C++ only orchestrates: every byte of arithmetic on the hot path runs in the kernels of l3d_match.cu /
 // l3d_pipeline.cu.  There is no CPU fallback: every entry needs a live CUDA context and fails loudly otherwise.
 #include "l3d_cub.cuh"
+#include "l3d_sweep.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_reduce.cuh>
@@ -65,8 +66,11 @@ int l3d_ctx_create(int device, l3d_ctx** out)
         for (auto k : by_keep)
             if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l3d_match_smem_bytes());
     // once, at the most any launch uses: the attribute is per device, and a per-launch setting would race between contexts that match
-    // on one device from several host threads
+    // or score on one device from several host threads
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_sort_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SORT_SMEM_MAX);
+    for (int cpu_sem = 0; cpu_sem < 2; ++cpu_sem)
+        for (auto k : l3d_sw_score_kernels[cpu_sem])
+            if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l3d_sw_score_smem_bytes(cpu_sem));
     if (e != cudaSuccess) { cudaStreamDestroy(c->stream); delete c; return L3D_ERR_CUDA; }
     *out = c;
     return L3D_OK;

@@ -24,7 +24,6 @@ struct DevBuf {
 struct SweepState {
     bool valid = false;
     std::vector<int> order;                 // view indices in processing order (ascending camID)
-    std::vector<int> h_M;                   // per processing rank: number of matches in matches_[view] after scoring (active entries)
     std::vector<long long> region_off;      // per processing rank (+1): first entry of the view's region
     long long total = 0;
     // match store (l3d_sweep.cuh): view table, chunk descriptors, chunk offsets, entries

@@ -284,7 +284,6 @@ __host__ __device__ __forceinline__ SwPtrs sw_carve(unsigned char* base, size_t 
 struct SwChunkInfo { int other, pub; float k; float pad; double Cx, Cy, Cz; };
 struct SwSegInfo { float r1[3], r2[3]; double q1[3], q2[3]; };
 
-template <bool CPU>
 struct SwScoreArgs {
     const float4* cache; const double* rays; const L3DViewDev* views; const l3d_match_rec* recs; int v;
     const SwView* vt; const SwChunkInfo* cinfo; const long long* cstart;
@@ -431,7 +430,7 @@ __device__ __forceinline__ float2 sw_target_reg(const L3DViewDev* V, const SwSeg
 }
 
 template <bool CPU>
-__device__ __forceinline__ void sw_score_range(const SwScoreArgs<CPU>& A, const SwPtrs P, const int* __restrict__ cb, int* __restrict__ cbA,
+__device__ __forceinline__ void sw_score_range(const SwScoreArgs& A,const SwPtrs P, const int* __restrict__ cb, int* __restrict__ cbA,
                                                const SwChunkInfo* __restrict__ cinfo, const SwSegInfo* __restrict__ sinfo, int* __restrict__ wcnt,
                                                int nsegs, long long x0, int n)
 {
@@ -525,6 +524,8 @@ __device__ __forceinline__ void sw_score_range(const SwScoreArgs<CPU>& A, const 
     }
     for (int o = 16; o; o >>= 1) vmax = fmaxf(vmax, __shfl_xor_sync(0xffffffffu, vmax, o));
     if (lane == 0 && vmax > 0.0f) atomicMax(A.view_max_bits + A.v, __float_as_int(vmax));
+    // active entries per view.  Nothing reads them, but without this use of nact ptxas (CUDA 12.9, sm_90a) keeps the count in a
+    // vector register instead of a uniform one and spills vmax in the scoring loop of both REF_GPU instantiations.
     if (threadIdx.x == 0 && nact) atomicAdd(A.M + A.v, nact);
 }
 
@@ -532,7 +533,7 @@ __device__ __forceinline__ void sw_score_range(const SwScoreArgs<CPU>& A, const 
 // such (LDS, not generic loads); otherwise each CTA decides where its tables live.
 template <bool CPU, bool SMEM>
 __global__ void __launch_bounds__(SW_THREADS, CPU ? (SW_THREADS <= 256 ? 3 : 2) : (SW_THREADS <= 256 ? 5 : SW_THREADS <= 320 ? 4 : SW_THREADS <= 384 ? 3 : 2))
-k_sw_score(const SwScoreArgs<CPU> A)
+k_sw_score(const SwScoreArgs A)
 {
     const int CAP = A.cap;
     asm volatile("griddepcontrol.launch_dependents;");       // the next view's kernel may start its independent part
@@ -574,6 +575,12 @@ k_sw_score(const SwScoreArgs<CPU> A)
     __syncthreads();
     sw_score_range<CPU>(A, P, cb, cbA, cinfo, sinfo, wcnt, nsegs, x0, n);
 }
+
+void (*const l3d_sw_score_kernels[2][2])(SwScoreArgs) = {
+    {k_sw_score<false, false>, k_sw_score<false, true>},
+    {k_sw_score<true, false>, k_sw_score<true, true>},
+};
+size_t l3d_sw_score_smem_bytes(bool cpu_sem) { return sw_entry_bytes(cpu_sem) * (cpu_sem ? SW_CAP_MAX_CPU : SW_CAP_MAX); }
 
 // ---------------------------------------------------------------------------------------------- after the chain
 // filterMatches (line3D.cc:1586-1669) for every segment of every view: one thread per global segment
@@ -625,6 +632,15 @@ k_sw_filter(const float4* __restrict__ segs, const L3DViewDev* __restrict__ view
     }
 }
 
+// the L3DPP::Match record of a decoded entry of view v
+__device__ __forceinline__ l3d_match sw_match(const L3DViewDev* __restrict__ views, int v, const SwEntry& e, float score3D)
+{
+    l3d_match m;
+    m.src_cam = views[v].cam_id; m.src_seg = (unsigned int)e.seg; m.tgt_cam = views[e.tgt_view].cam_id; m.tgt_seg = (unsigned int)e.tgt_seg;
+    m.overlap = e.overlap; m.score3D = score3D; m.d_p1 = e.dep.x; m.d_p2 = e.dep.y; m.d_q1 = e.dep.z; m.d_q2 = e.dep.w;
+    return m;
+}
+
 // the matches of one view as L3DPP::Match records (test / dump interface)
 __global__ void __launch_bounds__(256)
 k_sw_export(const L3DViewDev* __restrict__ views, int v, long long ro, int n, const L3DPairDev* __restrict__ pairs,
@@ -638,11 +654,7 @@ k_sw_export(const L3DViewDev* __restrict__ views, int v, long long ro, int n, co
     const bool take = (e_flag[x] & want) == want;
     ok[i] = take ? 1 : 0;
     if (!take) return;
-    const SwEntry e = sw_decode(e_val[x], pairs, row_off, num_pairs, knn, recs);
-    l3d_match m;
-    m.src_cam = views[v].cam_id; m.src_seg = (unsigned int)e.seg; m.tgt_cam = views[e.tgt_view].cam_id; m.tgt_seg = (unsigned int)e.tgt_seg;
-    m.overlap = e.overlap; m.score3D = e_score[x]; m.d_p1 = e.dep.x; m.d_p2 = e.dep.y; m.d_q1 = e.dep.z; m.d_q2 = e.dep.w;
-    out[i] = m;
+    out[i] = sw_match(views, v, sw_decode(e_val[x], pairs, row_off, num_pairs, knn, recs), e_score[x]);
 }
 
 // compact list of the segments that have a 3D estimate: their best match (L3DPP::Match layout) and P1,P2
@@ -659,30 +671,29 @@ k_collect_estimates(const L3DViewDev* __restrict__ views, int V, long long N, co
     const int b = est_best[g];
     if (b < 0) return;
     const int lo = last_le(V, g, [&](int i) { return views[i].seg_off; });
-    const long long x = vt[lo].region_off + b;
-    const SwEntry e = sw_decode(e_val[x], pairs, row_off, num_pairs, knn, recs);
-    l3d_match m;
-    m.src_cam = views[lo].cam_id; m.src_seg = (unsigned int)(g - views[lo].seg_off); m.tgt_cam = views[e.tgt_view].cam_id; m.tgt_seg = (unsigned int)e.tgt_seg;
-    m.overlap = e.overlap; m.score3D = e_score[x]; m.d_p1 = e.dep.x; m.d_p2 = e.dep.y; m.d_q1 = e.dep.z; m.d_q2 = e.dep.w;
+    const long long x = vt[lo].region_off + b;     // an entry of segment g: its decoded segment is g - views[lo].seg_off
     const long long p = pos[g];
-    out_best[p] = m;
+    out_best[p] = sw_match(views, lo, sw_decode(e_val[x], pairs, row_off, num_pairs, knn, recs), e_score[x]);
     for (int i = 0; i < 6; ++i) out_P[6 * p + i] = est_P[6 * g + i];
 }
 
 // ---------------------------------------------------------------------------------------------- host driver
-extern "C" {
+// what the host knows of a sweep's layout that the steps after sweep_layout need
+struct SweepLayout {
+    std::vector<SwView> vt;     // per view: first chunk, chunk descriptors (region_off is written on the device)
+    long long NC = 0;           // chunks of all views
+    long long tab_max = 0;      // most chunk boundaries of one view's CTAs (nseg * np + CTAs): the chunk-table scratch
+    long long nblocks = 0;      // blocks of the record-parallel set-up kernels
+    long long Umax = 1;         // entries of the longest region: the long-list scratch (set by sweep_setup)
+};
 
-int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float min_best_score, float min_best_perc)
+// The processing order, the chunk lists of every view and the tables of the set-up kernels, built on the host and uploaded; the
+// buffers whose sizes follow from them reserved, and those the set-up kernels and the chain accumulate into cleared.
+static int sweep_layout(l3d_ctx* c, SweepLayout& L)
 {
-    if (!c) return L3D_ERR_INVALID;
-    c->drop(Stage::Sweep);
-    if (!c->have_matches) return l3d_fail(c, L3D_ERR_STATE, "l3d_score_sweep: call l3d_match_pairs first");
-    cudaSetDevice(c->device);
-    const int V = c->num_views, NP = c->num_pairs, knn = c->knn;
-    const long long slots = c->total_rows * knn;
-    if (slots >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_score_sweep: more than 2^31 match slots");
-    SweepState& S = c->sweep;
-    const bool cpu_sem = c->semantics == L3D_SEM_REF_CPU;
+    SweepState& S = c->sweep; cudaStream_t st = c->stream; int rc;
+    const int V = c->num_views, NP = c->num_pairs;
+    const long long slots = c->total_rows * c->knn;
     // processing order = ascending camID (std::map iteration, line3D.cc:704)
     S.order.resize(V);
     std::iota(S.order.begin(), S.order.end(), 0);
@@ -699,45 +710,30 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
         chunks[P.src].push_back(SwChunk{p, 0, P.tgt});
         if (rank[P.tgt] > rank[P.src]) chunks[P.tgt].push_back(SwChunk{p, 1, P.src});   // tgt still unprocessed when src stores its inverse matches (line3D.cc:1680)
     }
-    std::vector<SwChunkInfo> cinfo; std::vector<SwView> vt(V); std::vector<int2> pairc(NP, make_int2(-1, -1));
-    long long NC = 0, tab_max = 0;
+    std::vector<SwChunkInfo> cinfo; std::vector<SwView>& vt = L.vt; std::vector<int2> pairc(NP, make_int2(-1, -1));
+    vt.assign(V, SwView{});
     for (int i = 0; i < V; ++i) {
         const int v = S.order[i];
-        std::vector<SwChunk>& L = chunks[v];
-        if (!cpu_sem) std::stable_sort(L.begin(), L.end(), [&](const SwChunk& a, const SwChunk& b) { return rank[a.other] != rank[b.other] ? rank[a.other] < rank[b.other] : a.inv > b.inv; });
-        else std::stable_sort(L.begin(), L.end(), [&](const SwChunk& a, const SwChunk& b) {
+        std::vector<SwChunk>& ch = chunks[v];
+        if (c->semantics != L3D_SEM_REF_CPU) std::stable_sort(ch.begin(), ch.end(), [&](const SwChunk& a, const SwChunk& b) { return rank[a.other] != rank[b.other] ? rank[a.other] < rank[b.other] : a.inv > b.inv; });
+        else std::stable_sort(ch.begin(), ch.end(), [&](const SwChunk& a, const SwChunk& b) {
             if (a.inv != b.inv) return a.inv > b.inv;
             return a.inv ? rank[a.other] < rank[b.other] : a.pair < b.pair; });
-        vt[v].ci_off = (int)cinfo.size(); vt[v].np = (int)L.size(); vt[v].chunk_base = NC; vt[v].region_off = 0;
-        for (int k = 0; k < (int)L.size(); ++k) {
-            if (L[k].inv) pairc[L[k].pair].y = k; else pairc[L[k].pair].x = k;
-            const L3DViewDev& T = c->h_views[L[k].other];
+        vt[v].ci_off = (int)cinfo.size(); vt[v].np = (int)ch.size(); vt[v].chunk_base = L.NC;
+        for (int k = 0; k < (int)ch.size(); ++k) {
+            if (ch[k].inv) pairc[ch[k].pair].y = k; else pairc[ch[k].pair].x = k;
+            const L3DViewDev& T = c->h_views[ch[k].other];
             // a positive score of a direct match is announced to the other view if that holds the inverse match (is processed later)
-            const int pub = !L[k].inv && rank[L[k].other] > i ? L[k].other : -1;
-            cinfo.push_back(SwChunkInfo{L[k].other, pub, T.k, 0.f, T.C_d[0], T.C_d[1], T.C_d[2]});
+            const int pub = !ch[k].inv && rank[ch[k].other] > i ? ch[k].other : -1;
+            cinfo.push_back(SwChunkInfo{ch[k].other, pub, T.k, 0.f, T.C_d[0], T.C_d[1], T.C_d[2]});
         }
         const long long nseg = c->h_views[v].nseg;
-        NC += nseg * (long long)L.size();
-        tab_max = std::max(tab_max, nseg * ((long long)L.size() + 1));     // chunk boundaries of all its CTAs: nseg * np + CTAs
+        L.NC += nseg * (long long)ch.size();
+        L.tab_max = std::max(L.tab_max, nseg * ((long long)ch.size() + 1));
     }
     std::vector<long long> row_off(NP + 1);
     for (int p = 0; p < NP; ++p) row_off[p] = c->h_pairs[p].row_off;
     row_off[NP] = c->total_rows;
-
-    int rc;
-    cudaStream_t st = c->stream;
-    L3D_RESERVE(S.d_vt, sizeof(SwView) * (size_t)V, "view table"); L3D_RESERVE(S.d_cinfo, sizeof(SwChunkInfo) * cinfo.size(), "chunk descriptors");
-    L3D_RESERVE(S.d_rowoff, 8 * (size_t)(NP + 1), "pair row offsets"); L3D_RESERVE(S.d_order, 4 * (size_t)V, "order"); L3D_RESERVE(S.d_region_off, 8 * (size_t)(V + 1), "region offsets");
-    const long long nblocks = (slots + SW_SETUP_THREADS - 1) / SW_SETUP_THREADS;
-    L3D_RESERVE(S.d_pinfo, sizeof(SwPairInfo) * (size_t)(NP + 1), "pair table"); L3D_RESERVE(S.d_bpair, 4 * std::max<long long>(nblocks, 1), "first pair of every block");
-    L3D_RESERVE(S.d_rays, 72 * c->total_segs, "segment rays"); L3D_RESERVE(S.d_rmf, 16 * c->total_segs, "mid-point rays"); L3D_RESERVE(S.d_rflag, slots, "record flags"); L3D_RESERVE(S.d_invpos, 4 * slots, "inverse positions");
-    L3D_RESERVE(S.d_csize, 4 * (NC + 1), "chunk sizes"); L3D_RESERVE(S.d_ccur, 4 * (NC + 1), "chunk cursors"); L3D_RESERVE(S.d_cstart, 8 * (NC + 1), "chunk offsets");
-    L3D_RESERVE(S.d_ranges, 8 * c->total_segs, "ranges"); L3D_RESERVE(S.d_est_best, 4 * c->total_segs, "estimates"); L3D_RESERVE(S.d_est_P, 48 * c->total_segs, "estimate points");
-    L3D_RESERVE(S.d_M, 4 * (size_t)V, "match counts"); L3D_RESERVE(S.d_vmax, 4 * (size_t)V, "view max");
-    L3D_CUDA(c, cudaMemcpyAsync(S.d_vt.p, vt.data(), sizeof(SwView) * (size_t)V, cudaMemcpyHostToDevice, st), "view table");
-    if (!cinfo.empty()) L3D_CUDA(c, cudaMemcpyAsync(S.d_cinfo.p, cinfo.data(), sizeof(SwChunkInfo) * cinfo.size(), cudaMemcpyHostToDevice, st), "chunk descriptors");
-    L3D_CUDA(c, cudaMemcpyAsync(S.d_rowoff.p, row_off.data(), 8 * (size_t)(NP + 1), cudaMemcpyHostToDevice, st), "pair row offsets");
-    L3D_CUDA(c, cudaMemcpyAsync(S.d_order.p, S.order.data(), 4 * (size_t)V, cudaMemcpyHostToDevice, st), "order");
     std::vector<SwPairInfo> pinfo((size_t)NP + 1);
     for (int p = 0; p < NP; ++p) {
         const L3DPairDev& P = c->h_pairs[p];
@@ -748,15 +744,25 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
         q.cx = pairc[p].x; q.cy = pairc[p].y;
     }
     { SwPairInfo& q = pinfo[NP]; std::memset(&q, 0, sizeof(q)); q.row_off = c->total_rows; q.row_end = (1ll << 62); q.cx = q.cy = -1; }   // sentinel
-    std::vector<int> bpair((size_t)std::max<long long>(nblocks, 1), 0);
-    {
-        int p = 0;
-        for (long long b = 0; b < nblocks; ++b) {
-            const long long row = (b * SW_SETUP_THREADS) / knn;
-            while (p < NP && row >= row_off[p + 1]) ++p;          // pairs without rows are skipped
-            bpair[b] = p;
-        }
+    L.nblocks = (slots + SW_SETUP_THREADS - 1) / SW_SETUP_THREADS;
+    std::vector<int> bpair((size_t)std::max<long long>(L.nblocks, 1), 0);
+    for (long long b = 0, p = 0; b < L.nblocks; ++b) {
+        const long long row = (b * SW_SETUP_THREADS) / c->knn;
+        while (p < NP && row >= row_off[p + 1]) ++p;          // pairs without rows are skipped
+        bpair[b] = (int)p;
     }
+    const long long NC = L.NC, N = c->total_segs;
+    L3D_RESERVE(S.d_vt, sizeof(SwView) * (size_t)V, "view table"); L3D_RESERVE(S.d_cinfo, sizeof(SwChunkInfo) * cinfo.size(), "chunk descriptors");
+    L3D_RESERVE(S.d_rowoff, 8 * (size_t)(NP + 1), "pair row offsets"); L3D_RESERVE(S.d_order, 4 * (size_t)V, "order"); L3D_RESERVE(S.d_region_off, 8 * (size_t)(V + 1), "region offsets");
+    L3D_RESERVE(S.d_pinfo, sizeof(SwPairInfo) * (size_t)(NP + 1), "pair table"); L3D_RESERVE(S.d_bpair, 4 * bpair.size(), "first pair of every block");
+    L3D_RESERVE(S.d_rays, 72 * N, "segment rays"); L3D_RESERVE(S.d_rmf, 16 * N, "mid-point rays"); L3D_RESERVE(S.d_rflag, slots, "record flags"); L3D_RESERVE(S.d_invpos, 4 * slots, "inverse positions");
+    L3D_RESERVE(S.d_csize, 4 * (NC + 1), "chunk sizes"); L3D_RESERVE(S.d_ccur, 4 * (NC + 1), "chunk cursors"); L3D_RESERVE(S.d_cstart, 8 * (NC + 1), "chunk offsets");
+    L3D_RESERVE(S.d_ranges, 8 * N, "ranges"); L3D_RESERVE(S.d_est_best, 4 * N, "estimates"); L3D_RESERVE(S.d_est_P, 48 * N, "estimate points");
+    L3D_RESERVE(S.d_M, 4 * (size_t)V, "match counts"); L3D_RESERVE(S.d_vmax, 4 * (size_t)V, "view max");
+    L3D_CUDA(c, cudaMemcpyAsync(S.d_vt.p, vt.data(), sizeof(SwView) * (size_t)V, cudaMemcpyHostToDevice, st), "view table");
+    if (!cinfo.empty()) L3D_CUDA(c, cudaMemcpyAsync(S.d_cinfo.p, cinfo.data(), sizeof(SwChunkInfo) * cinfo.size(), cudaMemcpyHostToDevice, st), "chunk descriptors");
+    L3D_CUDA(c, cudaMemcpyAsync(S.d_rowoff.p, row_off.data(), 8 * (size_t)(NP + 1), cudaMemcpyHostToDevice, st), "pair row offsets");
+    L3D_CUDA(c, cudaMemcpyAsync(S.d_order.p, S.order.data(), 4 * (size_t)V, cudaMemcpyHostToDevice, st), "order");
     L3D_CUDA(c, cudaMemcpyAsync(S.d_pinfo.p, pinfo.data(), sizeof(SwPairInfo) * (size_t)(NP + 1), cudaMemcpyHostToDevice, st), "pair table");
     L3D_CUDA(c, cudaMemcpyAsync(S.d_bpair.p, bpair.data(), 4 * bpair.size(), cudaMemcpyHostToDevice, st), "first pair of every block");
     L3D_CUDA(c, cudaStreamSynchronize(st), "score sweep tables");      // cinfo / pinfo / bpair are locals
@@ -766,20 +772,24 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
     L3D_CUDA(c, cudaMemsetAsync(S.d_invpos.p, 0xFF, 4 * (size_t)slots, st), "init inverse positions");   // "no inverse entry"
     L3D_CUDA(c, cudaMemsetAsync(S.d_M.p, 0, 4 * (size_t)V, st), "init counts");
     L3D_CUDA(c, cudaMemsetAsync(S.d_vmax.p, 0, 4 * (size_t)V, st), "init maxima");
+    return L3D_OK;
+}
 
-    ScopedEvent ev[4];
-    for (ScopedEvent& e : ev) if ((rc = e.create(c))) return rc;
-    cudaEventRecord(ev[0].e, st);
-    const float4* segs = c->segs(); const float4* cache = (const float4*)c->d_cache.p;
-    const L3DViewDev* views = c->views(); const L3DPairDev* pairs = (const L3DPairDev*)c->d_pairs.p;
-    const int* counts = (const int*)c->d_counts.p; const l3d_match_rec* recs = (const l3d_match_rec*)c->d_recs.p;
-    const SwView* d_vt = (const SwView*)S.d_vt.p; const long long* d_rowoff = (const long long*)S.d_rowoff.p;
-    const unsigned int nbs = (unsigned int)nblocks;
-    S.region_off.assign(V + 1, 0); S.total = 0;
-    if (NP > 0 && slots > 0) {
-        k_sw_rays<<<(unsigned int)((c->total_segs + 255) / 256), 256, 0, st>>>(segs, views, V, c->total_segs, (double*)S.d_rays.p, (float4*)S.d_rmf.p);
-        k_sw_flags<<<nbs, SW_SETUP_THREADS, 0, st>>>((const double*)S.d_rays.p, cache, (const float4*)S.d_rmf.p, views, (const SwPairInfo*)S.d_pinfo.p, (const int*)S.d_bpair.p,
-                                                     counts, recs, knn, slots, (unsigned char*)S.d_rflag.p, (int*)S.d_csize.p);
+// The match store: orientation flags of every record and the chunk sizes, chunk offsets and every view's region (downloaded: the
+// chain's geometry and the size of the entry arrays follow from them), then the entries in list order.
+static int sweep_setup(l3d_ctx* c, SweepLayout& L)
+{
+    SweepState& S = c->sweep; cudaStream_t st = c->stream; int rc;
+    const int V = c->num_views, knn = c->knn;
+    const long long slots = c->total_rows * knn, NC = L.NC, N = c->total_segs;
+    const bool cpu_sem = c->semantics == L3D_SEM_REF_CPU;
+    const L3DViewDev* views = c->views(); const l3d_match_rec* recs = (const l3d_match_rec*)c->d_recs.p;
+    const unsigned int nbs = (unsigned int)L.nblocks;
+    S.region_off.assign(V + 1, 0);
+    if (c->num_pairs > 0 && slots > 0) {
+        k_sw_rays<<<(unsigned int)((N + 255) / 256), 256, 0, st>>>(c->segs(), views, V, N, (double*)S.d_rays.p, (float4*)S.d_rmf.p);
+        k_sw_flags<<<nbs, SW_SETUP_THREADS, 0, st>>>((const double*)S.d_rays.p, (const float4*)c->d_cache.p, (const float4*)S.d_rmf.p, views, (const SwPairInfo*)S.d_pinfo.p,
+                                                     (const int*)S.d_bpair.p, (const int*)c->d_counts.p, recs, knn, slots, (unsigned char*)S.d_rflag.p, (int*)S.d_csize.p);
         if ((rc = l3d_cub(c, "chunk scan", [&](void* tmp, size_t& bytes) {
                  return cub::DeviceScan::ExclusiveSum(tmp, bytes, (const int*)S.d_csize.p, (long long*)S.d_cstart.p, NC + 1, st); }))) return rc;
         k_sw_regions<<<(V + 256) / 256, 256, 0, st>>>(V, (SwView*)S.d_vt.p, (const long long*)S.d_cstart.p, NC, (const int*)S.d_order.p, (long long*)S.d_region_off.p);
@@ -790,26 +800,54 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
         L3D_CUDA(c, cudaMemsetAsync(S.d_cstart.p, 0, 8 * (size_t)(NC + 1), st), "chunk offsets");
         L3D_CUDA(c, cudaMemsetAsync(S.d_region_off.p, 0, 8 * (size_t)(V + 1), st), "region offsets");
     }
-    const long long total = S.region_off[V];
-    S.total = total;
-    long long Umax = 1;
-    for (int i = 0; i < V; ++i) Umax = std::max(Umax, S.region_off[i + 1] - S.region_off[i]);
-    if (Umax >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_score_sweep: view with more than 2^31 matches");
+    const long long total = S.total = S.region_off[V];
+    for (int i = 0; i < V; ++i) L.Umax = std::max(L.Umax, S.region_off[i + 1] - S.region_off[i]);
+    if (L.Umax >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_score_sweep: view with more than 2^31 matches");
     L3D_RESERVE(S.d_eval, 4 * total, "entry records"); L3D_RESERVE(S.d_escore, 4 * total, "entry scores"); L3D_RESERVE(S.d_eflag, total, "entry flags");
     L3D_RESERVE(S.d_ekv, 8 * total, "unsorted entries");
     // global scratch of the chain, double-buffered (two kernels may be in flight): staged entries of the longest region, chunk
     // tables of the view with the most chunk boundaries
-    const size_t per_entry = sw_entry_bytes(cpu_sem);
-    L3D_RESERVE(S.d_gstage, 2 * per_entry * Umax, "long-list scratch"); L3D_RESERVE(S.d_gtab, 2 * 2 * 4 * tab_max, "chunk table scratch");
-    unsigned int* e_val = (unsigned int*)S.d_eval.p; float* e_score = (float*)S.d_escore.p; unsigned char* e_flag = (unsigned char*)S.d_eflag.p;
+    L3D_RESERVE(S.d_gstage, 2 * sw_entry_bytes(cpu_sem) * L.Umax, "long-list scratch"); L3D_RESERVE(S.d_gtab, 2 * 2 * 4 * L.tab_max, "chunk table scratch");
     if (total > 0) {
         k_sw_scatter<<<nbs, SW_SETUP_THREADS, 0, st>>>((const SwPairInfo*)S.d_pinfo.p, (const int*)S.d_bpair.p, recs, knn, slots, (const unsigned char*)S.d_rflag.p,
                                                        (const long long*)S.d_cstart.p, (int*)S.d_ccur.p, (uint2*)S.d_ekv.p, cpu_sem ? 1 : 0);
-        k_sw_chunksort<<<(unsigned int)((c->total_segs + CS_WARPS - 1) / CS_WARPS), 32 * CS_WARPS, 0, st>>>(views, V, c->total_segs, d_vt, (const long long*)S.d_cstart.p,
-                                                                                                         (const uint2*)S.d_ekv.p, e_val, e_flag, (unsigned int*)S.d_invpos.p);
+        k_sw_chunksort<<<(unsigned int)((N + CS_WARPS - 1) / CS_WARPS), 32 * CS_WARPS, 0, st>>>(views, V, N, (const SwView*)S.d_vt.p, (const long long*)S.d_cstart.p,
+                                                                                               (const uint2*)S.d_ekv.p, (unsigned int*)S.d_eval.p, (unsigned char*)S.d_eflag.p,
+                                                                                               (unsigned int*)S.d_invpos.p);
         c->launches += 2;
     }
+    return L3D_OK;
+}
 
+// Geometry of one view's chain launch (`entries` in its region, `nseg` segments): the fewest segments per CTA for which all CTAs
+// are resident at once (one wave), or force_segs > 0 of them, and the entries each CTA stages in shared memory.
+struct SwGeometry { int segs, cap; };
+static SwGeometry sw_geometry(bool cpu_sem, long long entries, int nseg, int num_sms, int force_segs)
+{
+    const int cap_max = cpu_sem ? SW_CAP_MAX_CPU : SW_CAP_MAX;
+    const int occ_regs = cpu_sem ? 3 : 5;               // resident CTAs per SM the register budget allows (launch bounds)
+    const double avg = (double)entries / nseg;
+    // staged entries: 45 % + 160 above the mean (a CTA whose range is longer falls back to the slow global-scratch path)
+    auto cap_of = [&](int segs) { return std::min(cap_max, (int)((segs * avg * 1.45 + 160 + 63) / 64) * 64); };
+    if (force_segs > 0) { const int segs = std::min(force_segs, SW_SEGS_MAX); return SwGeometry{segs, cap_of(segs)}; }
+    SwGeometry g = {}; double best = 1e300;
+    for (int segs = 1; segs <= SW_SEGS_MAX; ++segs) {
+        const int cap = cap_of(segs);
+        const int occ = std::max(1, std::min(occ_regs, (int)((227 * 1024) / (sw_entry_bytes(cpu_sem) * cap + 8500))));
+        const long long ctas = (nseg + segs - 1) / segs;
+        const double waves = std::ceil((double)ctas / ((double)num_sms * occ));
+        const double cost = waves * (1.0 + segs * avg / SW_THREADS);      // waves x rounds of work per thread
+        if (cost < best - 1e-9) { best = cost; g = SwGeometry{segs, cap}; }
+    }
+    return g;
+}
+
+// The chain: one k_sw_score launch per view with entries, in processing order.
+static int sweep_chain(l3d_ctx* c, const SweepLayout& L, float two_sigA_sqr, float min_similarity)
+{
+    SweepState& S = c->sweep;
+    if (S.total == 0) return L3D_OK;
+    const bool cpu_sem = c->semantics == L3D_SEM_REF_CPU;
     // shortcut thresholds of sw_score_gpu (see there); disabled (never true) when sim_t <= 0 or the margins do not apply
     float q_thr = INFINITY, cos_thr = -1.0f;
     if (min_similarity > 0.0f && min_similarity < 1.0f) {
@@ -817,102 +855,95 @@ int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float 
         const double ang = std::sqrt((double)q_thr * (double)two_sigA_sqr);           // degrees
         cos_thr = ang < 89.0 ? (float)(std::cos(ang * L3D_PI_D / 180.0) * (1.0 - 1e-4)) : -1.0f;
     }
-    cudaEventRecord(ev[1].e, st);
-    // ---- the chain: one launch per view, ascending camID
-    if (total > 0) {
-        SwScoreArgs<false> A;
-        A.cache = cache; A.rays = (const double*)S.d_rays.p; A.views = views; A.recs = recs; A.v = 0;
-        A.vt = d_vt; A.cinfo = (const SwChunkInfo*)S.d_cinfo.p; A.cstart = (const long long*)S.d_cstart.p;
-        A.e_val = e_val; A.e_score = e_score; A.e_flag = e_flag; A.invpos = (const unsigned int*)S.d_invpos.p;
-        A.view_max_bits = (int*)S.d_vmax.p; A.M = (int*)S.d_M.p;
-        int launched = 0;
-        A.angle_reg = two_sigA_sqr; A.sim_t = min_similarity; A.q_thr = q_thr; A.cos_thr = cos_thr;
-        SwScoreArgs<true> B;
-        static_assert(sizeof(SwScoreArgs<true>) == sizeof(SwScoreArgs<false>), "same layout");
-        std::memcpy((void*)&B, (const void*)&A, sizeof(A));
-        for (auto kern : {k_sw_score<false, true>, k_sw_score<false, false>})
-            L3D_CUDA(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sw_entry_bytes(false) * SW_CAP_MAX)), "k_sw_score shared memory");
-        for (auto kern : {k_sw_score<true, true>, k_sw_score<true, false>})
-            L3D_CUDA(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sw_entry_bytes(true) * SW_CAP_MAX_CPU)), "k_sw_score shared memory");
-        const int cap_max = cpu_sem ? SW_CAP_MAX_CPU : SW_CAP_MAX;
-        const int occ_regs = cpu_sem ? 3 : 5;               // resident CTAs per SM the register budget allows (launch bounds)
-        const int force_segs = getenv("L3D_SW_SEGS") ? atoi(getenv("L3D_SW_SEGS")) : 0;      // tools/sweep_score.py: override the geometry choice
-        for (int i = 0; i < V; ++i) {
-            const int v = S.order[i];
-            const int nseg = c->h_views[v].nseg;
-            if (nseg == 0 || S.region_off[i + 1] == S.region_off[i]) continue;
-            // geometry of this view's launch: the fewest segments per CTA for which all CTAs are resident at once (one wave)
-            const double avg = (double)(S.region_off[i + 1] - S.region_off[i]) / nseg;
-            int segs = 1, cap = 64; double best = 1e300;
-            for (int sgs = 1; sgs <= SW_SEGS_MAX; ++sgs) {
-                // staged entries: 45 % + 160 above the mean (a CTA whose range is longer falls back to the slow global-scratch path)
-                const int cp = std::min(cap_max, (int)((sgs * avg * 1.45 + 160 + 63) / 64) * 64);
-                const int occ = std::max(1, std::min(occ_regs, (int)((227 * 1024) / (per_entry * cp + 8500))));
-                const long long ctas = (nseg + sgs - 1) / sgs;
-                const double waves = std::ceil((double)ctas / ((double)c->num_sms * occ));
-                const double cost = waves * (1.0 + sgs * avg / SW_THREADS);      // waves x rounds of work per thread
-                if (cost < best - 1e-9) { best = cost; segs = sgs; cap = cp; }
-            }
-            if (force_segs > 0) { segs = std::min(force_segs, SW_SEGS_MAX); cap = std::min(cap_max, (int)((segs * avg * 1.45 + 160 + 63) / 64) * 64); }
-            const size_t smem = per_entry * (size_t)cap;
-            A.segs = B.segs = segs; A.cap = B.cap = cap;
-            const unsigned int nb = (unsigned int)((nseg + segs - 1) / segs);
-            cudaLaunchConfig_t cfg = {};
-            cfg.gridDim = dim3(nb); cfg.blockDim = dim3(SW_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-            cudaLaunchAttribute attr[1];
-            attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = 1;
-            // programmatic dependent launch: this view's kernel may stage its lists while the previous view's kernel is still scoring
-            // (it waits before it reads the bits that kernel publishes).  The first one follows ordinary kernels: plain stream order.
-            cfg.attrs = attr; cfg.numAttrs = launched ? 1 : 0;
-            A.gstage = B.gstage = (unsigned char*)S.d_gstage.p + (launched & 1) * per_entry * Umax;     // double-buffered scratch
-            A.gtab = B.gtab = (int*)S.d_gtab.p + (launched & 1) * 2 * tab_max;
-            ++launched;
-            const bool smem_tables = vt[v].np <= SW_MAXNP && segs * vt[v].np <= SW_MAXCH;
-            if (cpu_sem) { B.v = v; L3D_CUDA(c, cudaLaunchKernelEx(&cfg, smem_tables ? k_sw_score<true, true> : k_sw_score<true, false>, B), "k_sw_score"); }
-            else { A.v = v; L3D_CUDA(c, cudaLaunchKernelEx(&cfg, smem_tables ? k_sw_score<false, true> : k_sw_score<false, false>, A), "k_sw_score"); }
-            ++c->launches;
-        }
-        L3D_CUDA(c, cudaGetLastError(), "score sweep launch");
+    SwScoreArgs A = {};
+    A.cache = (const float4*)c->d_cache.p; A.rays = (const double*)S.d_rays.p; A.views = c->views(); A.recs = (const l3d_match_rec*)c->d_recs.p;
+    A.vt = (const SwView*)S.d_vt.p; A.cinfo = (const SwChunkInfo*)S.d_cinfo.p; A.cstart = (const long long*)S.d_cstart.p;
+    A.e_val = (const unsigned int*)S.d_eval.p; A.e_score = (float*)S.d_escore.p; A.e_flag = (unsigned char*)S.d_eflag.p; A.invpos = (const unsigned int*)S.d_invpos.p;
+    A.view_max_bits = (int*)S.d_vmax.p; A.M = (int*)S.d_M.p;
+    A.angle_reg = two_sigA_sqr; A.sim_t = min_similarity; A.q_thr = q_thr; A.cos_thr = cos_thr;
+    const size_t per_entry = sw_entry_bytes(cpu_sem);
+    const int force_segs = getenv("L3D_SW_SEGS") ? atoi(getenv("L3D_SW_SEGS")) : 0;      // tools/sweep_score.py: override the geometry choice
+    // programmatic dependent launch: a view's kernel may stage its lists while the previous view's kernel is still scoring (it waits
+    // before it reads the bits that kernel publishes).  The first one follows ordinary kernels: plain stream order.
+    cudaLaunchAttribute pdl;
+    pdl.id = cudaLaunchAttributeProgrammaticStreamSerialization; pdl.val.programmaticStreamSerializationAllowed = 1;
+    int launched = 0;
+    for (int i = 0; i < c->num_views; ++i) {
+        const int v = S.order[i], nseg = c->h_views[v].nseg;
+        const long long entries = S.region_off[i + 1] - S.region_off[i];
+        if (nseg == 0 || entries == 0) continue;
+        const SwGeometry g = sw_geometry(cpu_sem, entries, nseg, c->num_sms, force_segs);
+        A.v = v; A.segs = g.segs; A.cap = g.cap;
+        A.gstage = (unsigned char*)S.d_gstage.p + (launched & 1) * per_entry * L.Umax;     // double-buffered scratch
+        A.gtab = (int*)S.d_gtab.p + (launched & 1) * 2 * L.tab_max;
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3((unsigned int)((nseg + g.segs - 1) / g.segs)); cfg.blockDim = dim3(SW_THREADS); cfg.dynamicSmemBytes = per_entry * (size_t)g.cap;
+        cfg.stream = c->stream; cfg.attrs = &pdl; cfg.numAttrs = launched ? 1 : 0;
+        const bool smem_tables = L.vt[v].np <= SW_MAXNP && g.segs * L.vt[v].np <= SW_MAXCH;
+        L3D_CUDA(c, cudaLaunchKernelEx(&cfg, l3d_sw_score_kernels[cpu_sem][smem_tables], A), "k_sw_score");
+        ++launched; ++c->launches;
     }
-    cudaEventRecord(ev[2].e, st);
-    // ---- filterMatches + best estimates for all views
-    {
-        const long long N = c->total_segs;
-        if (N > 0) {
-            k_sw_filter<<<(unsigned int)((N + 255) / 256), 256, 0, st>>>(segs, views, V, N, d_vt, (const long long*)S.d_cstart.p, e_val, e_score, e_flag, recs,
-                                                                        (const int*)S.d_vmax.p, min_best_score, min_best_perc, (int2*)S.d_ranges.p,
-                                                                        (int*)S.d_est_best.p, (double*)S.d_est_P.p);
-            ++c->launches;
-            L3D_CUDA(c, cudaGetLastError(), "k_sw_filter");
-        }
-        std::vector<int> M(V);
-        L3D_CUDA(c, cudaMemcpyAsync(M.data(), S.d_M.p, 4 * (size_t)V, cudaMemcpyDeviceToHost, st), "download counts");
-        // compact the estimates on the device: flags -> exclusive scan -> gather (best match record + P1,P2)
-        S.n_est = 0;
-        if (N > 0) {
-            L3D_RESERVE(S.d_est_pos, 8 * (size_t)(N + 1), "estimate positions");
-            cub::TransformInputIterator<long long, HasEstimate, const int*> flags((const int*)S.d_est_best.p, HasEstimate());
-            ScanTotal t;
-            if ((rc = l3d_scan_total(c, flags, (long long*)S.d_est_pos.p, N, (const int*)S.d_est_best.p, t, "estimate scan"))) return rc;
-            L3D_CUDA(c, cudaStreamSynchronize(st), "score sweep");
-            S.n_est = t.last_out + HasEstimate()(t.last_src);
-            L3D_RESERVE(S.d_est_out_best, sizeof(l3d_match) * (size_t)std::max<long long>(S.n_est, 1), "estimate records");
-            L3D_RESERVE(S.d_est_out_P, 48 * (size_t)std::max<long long>(S.n_est, 1), "estimate points");
-            if (S.n_est > 0) {
-                k_collect_estimates<<<(unsigned int)((N + 255) / 256), 256, 0, st>>>(views, V, N, d_vt, (const int*)S.d_est_best.p, (const long long*)S.d_est_pos.p, pairs,
-                                                                                   d_rowoff, NP, knn, recs, e_val, e_score, (const double*)S.d_est_P.p,
-                                                                                   (l3d_match*)S.d_est_out_best.p, (double*)S.d_est_out_P.p);
-                c->launches += 3;
-                L3D_CUDA(c, cudaGetLastError(), "k_collect_estimates");
-            }
-        }
-        cudaEventRecord(ev[3].e, st);
-        L3D_CUDA(c, cudaStreamSynchronize(st), "score sweep");
-        cudaEventElapsedTime(&S.ms_setup, ev[0].e, ev[1].e); cudaEventElapsedTime(&S.ms_chain, ev[1].e, ev[2].e); cudaEventElapsedTime(&S.ms_filter, ev[2].e, ev[3].e);
-        if (getenv("L3D_SWEEP_TIMING")) fprintf(stderr, "[l3d] score sweep: set-up %.3f ms, chain %.3f ms (%d views), filter+estimates %.3f ms\n", S.ms_setup, S.ms_chain, V, S.ms_filter);
-        S.h_M.resize(V);
-        for (int i = 0; i < V; ++i) S.h_M[i] = M[S.order[i]];
+    L3D_CUDA(c, cudaGetLastError(), "score sweep launch");
+    return L3D_OK;
+}
+
+// filterMatches and the best 3D estimate of every segment for all views, then the estimates compacted on the device: flags ->
+// exclusive scan -> gather (best match record + P1,P2)
+static int sweep_filter(l3d_ctx* c, float min_best_score, float min_best_perc)
+{
+    SweepState& S = c->sweep; cudaStream_t st = c->stream; int rc;
+    const int V = c->num_views; const long long N = c->total_segs;
+    const SwView* vt = (const SwView*)S.d_vt.p; const l3d_match_rec* recs = (const l3d_match_rec*)c->d_recs.p;
+    const unsigned int* e_val = (const unsigned int*)S.d_eval.p; const float* e_score = (const float*)S.d_escore.p;
+    S.n_est = 0;
+    if (N == 0) return L3D_OK;
+    const unsigned int nb = (unsigned int)((N + 255) / 256);
+    k_sw_filter<<<nb, 256, 0, st>>>(c->segs(), c->views(), V, N, vt, (const long long*)S.d_cstart.p, e_val, e_score, (unsigned char*)S.d_eflag.p, recs,
+                                    (const int*)S.d_vmax.p, min_best_score, min_best_perc, (int2*)S.d_ranges.p, (int*)S.d_est_best.p, (double*)S.d_est_P.p);
+    ++c->launches;
+    L3D_CUDA(c, cudaGetLastError(), "k_sw_filter");
+    L3D_RESERVE(S.d_est_pos, 8 * (size_t)(N + 1), "estimate positions");
+    cub::TransformInputIterator<long long, HasEstimate, const int*> flags((const int*)S.d_est_best.p, HasEstimate());
+    ScanTotal t;
+    if ((rc = l3d_scan_total(c, flags, (long long*)S.d_est_pos.p, N, (const int*)S.d_est_best.p, t, "estimate scan"))) return rc;
+    L3D_CUDA(c, cudaStreamSynchronize(st), "score sweep");
+    S.n_est = t.last_out + HasEstimate()(t.last_src);
+    L3D_RESERVE(S.d_est_out_best, sizeof(l3d_match) * (size_t)std::max<long long>(S.n_est, 1), "estimate records");
+    L3D_RESERVE(S.d_est_out_P, 48 * (size_t)std::max<long long>(S.n_est, 1), "estimate points");
+    if (S.n_est > 0) {
+        k_collect_estimates<<<nb, 256, 0, st>>>(c->views(), V, N, vt, (const int*)S.d_est_best.p, (const long long*)S.d_est_pos.p, (const L3DPairDev*)c->d_pairs.p,
+                                                (const long long*)S.d_rowoff.p, c->num_pairs, c->knn, recs, e_val, e_score, (const double*)S.d_est_P.p,
+                                                (l3d_match*)S.d_est_out_best.p, (double*)S.d_est_out_P.p);
+        c->launches += 3;
+        L3D_CUDA(c, cudaGetLastError(), "k_collect_estimates");
     }
+    return L3D_OK;
+}
+
+extern "C" {
+
+int l3d_score_sweep(l3d_ctx* c, float two_sigA_sqr, float min_similarity, float min_best_score, float min_best_perc)
+{
+    if (!c) return L3D_ERR_INVALID;
+    c->drop(Stage::Sweep);
+    if (!c->have_matches) return l3d_fail(c, L3D_ERR_STATE, "l3d_score_sweep: call l3d_match_pairs first");
+    cudaSetDevice(c->device);
+    if (c->total_rows * c->knn >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_score_sweep: more than 2^31 match slots");
+    SweepState& S = c->sweep; SweepLayout L; int rc;
+    if ((rc = sweep_layout(c, L))) return rc;
+    // device time of the three phases: set-up, chain, filter + estimates
+    ScopedEvent ev[4];
+    for (ScopedEvent& e : ev) if ((rc = e.create(c))) return rc;
+    cudaEventRecord(ev[0].e, c->stream);
+    if ((rc = sweep_setup(c, L))) return rc;
+    cudaEventRecord(ev[1].e, c->stream);
+    if ((rc = sweep_chain(c, L, two_sigA_sqr, min_similarity))) return rc;
+    cudaEventRecord(ev[2].e, c->stream);
+    if ((rc = sweep_filter(c, min_best_score, min_best_perc))) return rc;
+    cudaEventRecord(ev[3].e, c->stream);
+    L3D_CUDA(c, cudaStreamSynchronize(c->stream), "score sweep");
+    cudaEventElapsedTime(&S.ms_setup, ev[0].e, ev[1].e); cudaEventElapsedTime(&S.ms_chain, ev[1].e, ev[2].e); cudaEventElapsedTime(&S.ms_filter, ev[2].e, ev[3].e);
+    if (getenv("L3D_SWEEP_TIMING")) fprintf(stderr, "[l3d] score sweep: set-up %.3f ms, chain %.3f ms (%d views), filter+estimates %.3f ms\n", S.ms_setup, S.ms_chain, c->num_views, S.ms_filter);
     S.valid = true;
     return L3D_OK;
 }

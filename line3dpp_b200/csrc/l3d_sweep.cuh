@@ -52,3 +52,7 @@ __device__ __forceinline__ float4 sw_depths(unsigned int val, const l3d_match_re
     const l3d_match_rec rec = recs[val & ~SW_INV];
     return (val & SW_INV) ? make_float4(rec.d_q1, rec.d_q2, rec.d_p1, rec.d_p2) : make_float4(rec.d_p1, rec.d_p2, rec.d_q1, rec.d_q2);
 }
+
+struct SwScoreArgs;
+extern void (*const l3d_sw_score_kernels[2][2])(SwScoreArgs);     // every instantiation of the chain kernel k_sw_score: [REF_CPU][tables in shared memory]
+size_t l3d_sw_score_smem_bytes(bool cpu_sem);                     // the most dynamic shared memory a k_sw_score launch uses
