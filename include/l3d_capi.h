@@ -13,7 +13,7 @@
  * 0 on success or a negative l3d_status; l3d_last_error() gives the message (the reference prints CUDA errors to
  * cerr and carries on, dataArray.h:198-237).  A call that fails leaves its stage (views, matches, score sweep,
  * collinear lists, affinity matrix), and every stage computed from it, without a result: later calls that need one
- * return L3D_ERR_STATE.  The image calls (l3d_undistort_u8, l3d_undistort_map, l3d_remap_u8) and the tie-point calls
+ * return L3D_ERR_STATE.  The image calls (l3d_undistort_u8, l3d_undistort_map, l3d_remap_u8, l3d_prepare_gray_u8) and the tie-point calls
  * (l3d_triangulate_points, l3d_median_depths) are not part of that chain: whether
  * they succeed or fail, every stage and its result stay as they were.  A context is single-owner (not thread-safe), one per GPU, and runs
  * on its own non-default stream.  There is NO CPU fallback: without a usable CUDA device l3d_ctx_create fails.
@@ -282,6 +282,29 @@ int l3d_undistort_u8(l3d_ctx* ctx, int n, const l3d_undistort_desc* descs, int o
 int l3d_undistort_map(l3d_ctx* ctx, const l3d_undistort_desc* desc, int16_t* map_xy, uint16_t* map_frac, int on_device);
 /* cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) of one image with caller-given maps in that layout (the camera is not used) */
 int l3d_remap_u8(l3d_ctx* ctx, const l3d_undistort_desc* desc, const int16_t* map_xy, const uint16_t* map_frac, int on_device);
+
+/* ---- image preparation for line detection: what the reference's detectLineSegments (line3D.cc:249-289) does to an image before LSD
+ * sees it.  cvtColor(CV_RGB2GRAY) for 3 channels (channel 0 is R; OpenCV's 15-bit fixed point) or the grey pixels as they are, then,
+ * when max_img_width > 0 and the larger side exceeds it, cv::resize(gray, out, Size(), s, s) with INTER_LINEAR and
+ * s = float(max_img_width) / float(max(width, height)); OpenCV turns a source step of exactly 2 into the 2x2 INTER_AREA mean.  Bit-exact
+ * to OpenCV 4.13's x86 build (DESIGN.md §4b).  One fused kernel per call: no grey intermediate is stored.
+ * out_width / out_height must be what l3d_image_prep_size returns for width, height and max_img_width (the caller sizes dst with it).
+ * Rejected with L3D_ERR_INVALID: width or height outside [1, 32767], channels other than 1 or 3, out_width / out_height other than
+ * l3d_image_prep_size's, a src pitch below width*channels or a dst pitch below out_width, null pointers, src == dst.
+ * on_device as for l3d_undistort_u8.  Not part of the pipeline chain: every stage and its result stay as they were. */
+typedef struct {
+    int32_t width, height, channels;   /* source image; channels 1 or 3, interleaved */
+    int32_t max_img_width;             /* the Line3D constructor's argument; <= 0: no resize */
+    int64_t src_pitch, dst_pitch;      /* row strides in bytes */
+    const uint8_t* src;
+    uint8_t* dst;                      /* out_height rows of out_width grey bytes */
+    int32_t out_width, out_height;     /* from l3d_image_prep_size */
+} l3d_image_prep_desc;
+/* the size of the prepared image (the rounding of the segment cache's file name, segmentCachePath); returns 1 if the image is resized,
+ * 0 if not, L3D_ERR_INVALID for a size outside [1, 32767] or a null output pointer.  Needs no context and no GPU. */
+int l3d_image_prep_size(int width, int height, int max_img_width, int32_t* out_width, int32_t* out_height);
+/* prepare n images in one launch; sizes, channel counts and max_img_width may all differ */
+int l3d_prepare_gray_u8(l3d_ctx* ctx, int n, const l3d_image_prep_desc* descs, int on_device);
 
 /* ---- tie-point triangulation: linearHomTriangulation of the reference's Pix4D frontend (main_pix4d.cpp:34-70, 354-372) for every point
  * in one launch.  Point i has the observations [obs_ptr[i], obs_ptr[i+1]) (obs_ptr[0] = 0): camera obs_cam[o] in [0, n_cams) and image

@@ -11,12 +11,15 @@
  *     Eigen::Matrix3d, Eigen::Vector3d, std::vector<cv::Vec4f>) is available as an inline overload that converts and
  *     forwards; tests/test_cpu.py compiles it against the header stand-ins of oracle/ref_shim.  get3Dlines() returns the POD
  *     types (P1().x is a member, not Eigen's x()): a frontend that reads the result lines needs that one-character change.
- *   - addImage takes the image SIZE and the 2D segments (the reference's own line_segments argument, line3D.h:102-108).  With no
- *     segments it reads the reference's segment cache <output_folder>/L3D++_data/segments_L3D++_<camID>_<w>x<h>_3000.bin
- *     (line3D.cc:295-309; segmentCachePath in include/line3d_io.h) when load_segments is true and the file exists, so a
- *     folder the reference has run on gives it exactly the segments the reference used.  LSD detection inside addImage
- *     (line3D.cc:249-372) is outside this library (SURVEY.md §2 row 13): without segments and without a cache file the view is
- *     rejected and lastError() names the file that was looked for.
+ *   - addImage takes the image (an Image8u, or its size alone) and the 2D segments (the reference's own line_segments argument,
+ *     line3D.h:102-108).  With no segments it reads the reference's segment cache
+ *     <output_folder>/L3D++_data/segments_L3D++_<camID>_<w>x<h>_3000.bin (line3D.cc:295-309; segmentCachePath in include/line3d_io.h)
+ *     when load_segments is true and the file exists, so a folder the reference has run on gives it exactly the segments the reference
+ *     used.  Otherwise the image overload does what the reference's detectLineSegments (line3D.cc:249-372) does around its LSD call:
+ *     grey conversion and the max_img_width resize on the GPU (l3d_prepare_gray_u8, bit-exact to OpenCV), then the detector the
+ *     caller registered with setSegmentDetector, then the upscale, length filter, longest-first order and max_line_segments cut, and
+ *     the segment cache is written.  The detector itself (LSD) is outside this library (SURVEY.md §2 row 13): without one, and without
+ *     segments or a cache file, the view is rejected and lastError() names the file that was looked for.
  *   - undistortImage (line3D.h:119-122) takes the owning Image8u and the POD vectors; with Eigen / OpenCV headers the reference's
  *     cv::Mat signature is an inline overload for CV_8UC1 / CV_8UC3.  It runs on the GPU and its map is defined by an explicit
  *     formula, which OpenCV builds reproduce to within one 1/32-px step (DESIGN.md §4a).
@@ -60,6 +63,31 @@ struct Image8u {
     Image8u() : cols(0), rows(0), channels(1) {}
     Image8u(int r, int c, int ch) : cols(c), rows(r), channels(ch), data((size_t)(r > 0 ? r : 0) * (c > 0 ? c : 0) * (ch > 0 ? ch : 0)) {}
 };
+
+#ifdef L3DPP_WITH_EIGEN_OPENCV
+namespace detail {
+/* the pixels of a cv::Mat as an Image8u, honouring its row step; a type other than CV_8UC1 / CV_8UC3 gives 0 channels, which
+ * addImage rejects as the reference does (line3D.cc:251-266) */
+template <class M>
+auto imageOf(const M& m, int) -> decltype((void)m.data, (void)m.step, Image8u())
+{
+    const bool ok = m.type() == CV_8UC1 || m.type() == CV_8UC3;
+    Image8u img(m.rows, m.cols, ok ? m.channels() : 0);
+    const size_t row = (size_t)m.cols * img.channels, step = static_cast<size_t>(m.step);
+    for (int r = 0; r < m.rows && row; ++r) std::memcpy(img.data.data() + r * row, m.data + r * step, row);
+    return img;
+}
+/* a cv::Mat stand-in that carries no pixels (the header stand-ins of the verbatim reference build) gives its size and no pixels:
+ * addImage can still use the segment cache, and rejects the view if it would have to prepare the image */
+template <class M>
+Image8u imageOf(const M& m, long)
+{
+    Image8u img;
+    img.rows = m.rows; img.cols = m.cols; img.channels = m.channels();
+    return img;
+}
+}  // namespace detail
+#endif
 
 /* defaults: commons.h:41-69 */
 const int L3D_DEF_MAX_IMG_WIDTH = -1;
@@ -141,8 +169,8 @@ struct Line3DStats {
 
 class Line3D {
 public:
-    /* line3D.h:80-85.  output_folder / load_segments / max_img_width only matter for the segment cache (addImage without
-     * segments) and the output filename (createOutputFilename); max_line_segments is stored and not used (it bounds detection). */
+    /* line3D.h:80-85.  output_folder / load_segments / max_img_width / max_line_segments only matter for addImage without segments
+     * (segment cache, image preparation, the cut of the detections) and the output filename (createOutputFilename). */
     Line3D(const std::string& output_folder, const bool load_segments = L3D_DEF_LOAD_AND_STORE_SEGMENTS,
            const int max_img_width = L3D_DEF_MAX_IMG_WIDTH, const unsigned int max_line_segments = L3D_DEF_MAX_NUM_SEGMENTS,
            const bool neighbors_by_worldpoints = true, const bool use_GPU = true, const int cuda_device = 0);
@@ -166,10 +194,25 @@ public:
                   const Vector3d& t, const float median_depth, const std::list<unsigned int>& wps_or_neighbors,
                   const std::vector<Vec4f>& line_segments);
 
+    /* line3D.h:104-108 with an Image8u (1 or 3 channels, channel 0 is R).  In the reference's order (line3D.cc:116-186, 249-372): the
+     * size check and the camera-ID check (an ID is reserved while its image is prepared, so a repeated ID never reaches the detector)
+     * come first.  Given segments are used as they are.  Otherwise the segment cache is read as above; on a miss the image is
+     * prepared on the GPU (grey, and resized when its larger side exceeds max_img_width: l3d_prepare_gray_u8), handed to the
+     * setSegmentDetector function, and its detections are scaled back to the image's size, kept when longer than
+     * 0.005 * the image diagonal, ordered longest first by the reference's std::priority_queue and cut at max_line_segments; when
+     * load_segments is true and a segment survives, they are written to the segment cache (the L3D++_data folder is created if
+     * needed; a cache that cannot be written is only reported in verbose mode, the view is still added).  Rejected with lastError() set: no detector and no cache file (the message names the file), a detector that returns
+     * false, no detection longer than the threshold, an image that is not 8-bit grey or RGB.  Thread-safe: the GPU step of concurrent
+     * calls is serialised on the primary device; the detector runs on the calling thread outside every lock. */
+    bool addImage(const unsigned int camID, const Image8u& image, const Matrix3d& K, const Matrix3d& R, const Vector3d& t,
+                  const float median_depth, const std::list<unsigned int>& wps_or_neighbors,
+                  const std::vector<Vec4f>& line_segments = std::vector<Vec4f>());
+
 #ifdef L3DPP_WITH_EIGEN_OPENCV
-    /* The reference's exact signature (line3D.h:104-108).  The image only contributes its size.  With an empty list (the frontends'
-     * call, main_vsfm.cpp:306) the segments come from the segment cache as above; line detection is outside this library
-     * (SURVEY.md §2 row 13), so without a cache file the call fails like any other rejected view. */
+    /* The reference's exact signature (line3D.h:104-108) for CV_8UC1 / CV_8UC3 images of any row step: the image overload above.
+     * With segments given only the image's size is used.  A template only so that this header also compiles against cv::Mat
+     * stand-ins that carry no pixels; calls are written as for the reference. */
+    template <class MatT = cv::Mat>
     bool addImage(const unsigned int camID, cv::Mat& image, const Eigen::Matrix3d& K, const Eigen::Matrix3d& R, const Eigen::Vector3d& t,
                   const float median_depth, const std::list<unsigned int>& wps_or_neighbors,
                   const std::vector<cv::Vec4f>& line_segments = std::vector<cv::Vec4f>())
@@ -178,9 +221,19 @@ public:
         for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) { Kp(r, c) = K(r, c); Rp(r, c) = R(r, c); }
         std::vector<Vec4f> segs(line_segments.size());
         for (size_t i = 0; i < line_segments.size(); ++i) for (int k = 0; k < 4; ++k) segs[i].v[k] = line_segments[i](k);
-        return addImage(camID, image.cols, image.rows, Kp, Rp, Vector3d(t(0), t(1), t(2)), median_depth, wps_or_neighbors, segs);
+        const Vector3d tp(t(0), t(1), t(2));
+        const MatT& img = image;
+        if (!segs.empty()) return addImage(camID, img.cols, img.rows, Kp, Rp, tp, median_depth, wps_or_neighbors, segs);
+        return addImage(camID, detail::imageOf(img, 0), Kp, Rp, tp, median_depth, wps_or_neighbors, segs);
     }
 #endif
+
+    /* The line detector addImage calls on the prepared grey image (what the reference does with
+     * cv::createLineSegmentDetector(cv::LSD_REFINE_ADV)->detect, line3D.cc:311-317): fill `detections` with (x1, y1, x2, y2) in the
+     * coordinates of `gray` and return true, or return false to reject the view.  Called from the thread that called addImage, with
+     * no lock held: concurrent addImage calls run it concurrently, so it must be thread-safe.  nullptr: no detector. */
+    typedef bool (*SegmentDetectorFn)(void* user, const Image8u& gray, std::vector<Vec4f>& detections);
+    void setSegmentDetector(SegmentDetectorFn detector, void* user);
 
     /* line3D.h:140-145 */
     void matchImages(const float sigma_position = L3D_DEF_SCORING_POS_REGULARIZER, const float sigma_angle = L3D_DEF_SCORING_ANG_REGULARIZER,

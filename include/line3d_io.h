@@ -90,9 +90,14 @@ bool write3DLinesBIN(const std::string& path, const std::vector<FinalLine3D>& li
 bool readSegmentCache(const std::string& path, std::vector<Vec4f>& segments, std::string* error = 0);
 bool writeSegmentCache(const std::string& path, const std::vector<Vec4f>& segments, std::string* error = 0);
 
-/* <output_folder>/L3D++_data/segments_L3D++_<camID>_<w>x<h>_3000.bin (line3D.cc:271-300).  <w>x<h> is the image size, or the size
- * cv::resize(img, out, Size(), s, s) gives with s = float(max_img_width) / float(max(w, h)) when max_img_width > 0 and the larger
- * side exceeds it.  The suffix is L3D_DEF_MAX_NUM_SEGMENTS, whatever max_line_segments is. */
+/* The size of the image detectLineSegments hands to line detection (line3D.cc:271-289): out = (w, h), or the size
+ * cv::resize(img, out, Size(), s, s) gives with s = float(max_img_width) / float(max(w, h)) when max_img_width > 0 and the larger side
+ * exceeds it.  Returns whether the image is resized; *scale (optional) = s, or 1.  The one place this rounding is decided: the
+ * segment cache's file name and the GPU image preparation (l3d_image_prep_size) both call it. */
+bool preparedImageSize(int w, int h, int max_img_width, int& out_w, int& out_h, float* scale = 0);
+
+/* <output_folder>/L3D++_data/segments_L3D++_<camID>_<w>x<h>_3000.bin (line3D.cc:271-300).  <w>x<h> is preparedImageSize's.  The
+ * suffix is L3D_DEF_MAX_NUM_SEGMENTS, whatever max_line_segments is. */
 std::string segmentCachePath(const std::string& output_folder, unsigned int camID, int image_width, int image_height, int max_img_width);
 
 }  // namespace L3DPP

@@ -42,6 +42,34 @@ def make_undistort_desc(width, height, channels, K, radial=(0, 0, 0), tangential
     return d
 
 
+class ImagePrepDesc(C.Structure):
+    """l3d_image_prep_desc: one 8-bit image, its max_img_width and the grey output"""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("channels", C.c_int32), ("max_img_width", C.c_int32),
+                ("src_pitch", C.c_int64), ("dst_pitch", C.c_int64), ("src", C.c_void_p), ("dst", C.c_void_p),
+                ("out_width", C.c_int32), ("out_height", C.c_int32)]
+
+
+def image_prep_size(width, height, max_img_width):
+    """(out_width, out_height, resized) of l3d_image_prep_size: the size of the image line detection sees"""
+    w, h = C.c_int32(), C.c_int32()
+    rc = lib().l3d_image_prep_size(int(width), int(height), int(max_img_width), C.byref(w), C.byref(h))
+    if rc < 0:
+        raise L3DError(f"l3d_image_prep_size({width}, {height}, {max_img_width}) failed ({rc})")
+    return w.value, h.value, bool(rc)
+
+
+def make_image_prep_desc(width, height, channels, max_img_width, src=0, src_pitch=None, dst=0, dst_pitch=None):
+    """src / dst: addresses; pitches in bytes (default packed); the output size is l3d_image_prep_size's"""
+    ow, oh, _ = image_prep_size(width, height, max_img_width)
+    d = ImagePrepDesc()
+    d.width, d.height, d.channels, d.max_img_width = int(width), int(height), int(channels), int(max_img_width)
+    d.src_pitch = int(width) * int(channels) if src_pitch is None else int(src_pitch)
+    d.dst_pitch = ow if dst_pitch is None else int(dst_pitch)
+    d.src, d.dst = int(src) or None, int(dst) or None
+    d.out_width, d.out_height = ow, oh
+    return d
+
+
 def _image_rows(a):
     """(array, row pitch in bytes) of a uint8 HxW / HxWx3 image whose pixels are packed within each row; other layouts are copied"""
     a = np.asarray(a)
@@ -349,6 +377,28 @@ class Context:
             outs.append(o)
         self._chk(self.L.l3d_undistort_u8(self.h, n, descs, 0), "l3d_undistort_u8")
         return outs
+
+    # ---- image preparation for line detection (stateless: no pipeline stage changes)
+    def prepare_gray(self, images, max_img_width):
+        """l3d_prepare_gray_u8 for a list of uint8 HxW / HxWx3 images in ONE batched call; max_img_width: one value for all images or
+        one per image.  Returns the grey uint8 [out_h, out_w] arrays."""
+        n = len(images)
+        mws = [max_img_width] * n if np.ndim(max_img_width) == 0 else list(max_img_width)
+        descs, keep, outs = (ImagePrepDesc * n)(), [], []
+        for i, img in enumerate(images):
+            a, sp = _image_rows(img)
+            c = 1 if a.ndim == 2 else 3
+            ow, oh, _ = image_prep_size(a.shape[1], a.shape[0], mws[i])
+            o = np.empty((oh, ow), np.uint8)
+            keep += [a, o]
+            descs[i] = make_image_prep_desc(a.shape[1], a.shape[0], c, mws[i], a.ctypes.data, sp, o.ctypes.data, ow)
+            outs.append(o)
+        self._chk(self.L.l3d_prepare_gray_u8(self.h, n, descs, 0), "l3d_prepare_gray_u8")
+        return outs
+
+    def prepare_gray_device(self, descs):
+        """l3d_prepare_gray_u8 on device addresses (a ctypes array of ImagePrepDesc); asynchronous on the context's stream"""
+        self._chk(self.L.l3d_prepare_gray_u8(self.h, len(descs), descs, 1), "l3d_prepare_gray_u8")
 
     def undistort_device(self, descs):
         """l3d_undistort_u8 on device addresses (a ctypes array of UndistortDesc); asynchronous on the context's stream"""

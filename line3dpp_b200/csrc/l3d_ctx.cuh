@@ -77,6 +77,22 @@ struct UndistortState {
     DevBuf d_imgs, d_src, d_dst, d_map_xy, d_map_frac;   // d_src .. d_map_frac: host-mode staging
 };
 
+// per-image parameters of k_prepare_gray_u8 (l3d_image_prep.cu): source (width x height, 1 or 3 channels) -> grey out_w x out_h
+struct L3DPrepImage {
+    const unsigned char* src;
+    unsigned char* dst;
+    long long src_pitch, dst_pitch, tile0;   // tile0: first tile of this image in the batch grid
+    int width, height, channels, out_w, out_h, tiles_x;
+    int mode;                                // L3D_PREP_COPY / L3D_PREP_LINEAR / L3D_PREP_AREA2
+    double scale;                            // source step 1 / (double)s of the resize (OpenCV's scale_x = scale_y)
+};
+
+// buffers of the image preparation calls: not a pipeline stage, nothing else reads them
+struct ImagePrepState {
+    std::vector<L3DPrepImage> h_imgs;
+    DevBuf d_imgs, d_src, d_dst;                         // d_src, d_dst: host-mode staging
+};
+
 // buffers of the triangulation and median-depth calls (l3d_triangulate.cu): not a pipeline stage either; the d_* of host mode
 // stage the caller's arrays
 struct TriangulateState {
@@ -123,6 +139,7 @@ struct l3d_ctx {
     CollinState collin;
     OptState opt;
     UndistortState undist;
+    ImagePrepState prep;
     TriangulateState tri;
 
     const float4* segs() const { return segs_ext ? segs_ext : (const float4*)d_segs.p; }

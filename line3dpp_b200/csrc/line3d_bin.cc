@@ -233,16 +233,24 @@ bool writeSegmentCache(const std::string& path, const std::vector<Vec4f>& segmen
     return o.save(path, error);
 }
 
+bool preparedImageSize(int w, int h, int max_img_width, int& out_w, int& out_h, float* scale)
+{
+    out_w = w; out_h = h;
+    if (scale) *scale = 1.0f;
+    const int max_dim = std::max(w, h);
+    if (!(max_img_width > 0 && max_dim > max_img_width)) return false;
+    // cv::resize(img, out, Size(), s, s): Size(saturate_cast<int>(cols * s), saturate_cast<int>(rows * s)) in double, rounded to nearest even
+    const float s = float(max_img_width) / float(max_dim);
+    out_w = (int)std::llrint((double)w * (double)s);
+    out_h = (int)std::llrint((double)h * (double)s);
+    if (scale) *scale = s;
+    return true;
+}
+
 std::string segmentCachePath(const std::string& output_folder, unsigned int camID, int w, int h, int max_img_width)
 {
-    long long nw = w, nh = h;
-    const int max_dim = std::max(w, h);
-    if (max_img_width > 0 && max_dim > max_img_width) {
-        // cv::resize(img, out, Size(), s, s): Size(saturate_cast<int>(cols * s), saturate_cast<int>(rows * s)) in double, rounded to nearest even
-        const float s = float(max_img_width) / float(max_dim);
-        nw = std::llrint((double)w * (double)s);
-        nh = std::llrint((double)h * (double)s);
-    }
+    int nw, nh;
+    preparedImageSize(w, h, max_img_width, nw, nh);
     std::stringstream p;
     p << output_folder << "/L3D++_data/segments_L3D++_" << camID << "_" << nw << "x" << nh << "_" << L3D_DEF_MAX_NUM_SEGMENTS << ".bin";
     return p.str();

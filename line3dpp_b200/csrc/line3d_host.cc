@@ -22,12 +22,14 @@
 #include <iostream>
 #include <map>
 #include <mutex>
+#include <queue>
 #include <set>
 #include <sstream>
 #include <stdexcept>
 #include <thread>
 #include <unordered_map>
 #include <unordered_set>
+#include <sys/stat.h>                  // mkdir: the segment cache's folder
 
 namespace L3DPP {
 
@@ -205,6 +207,11 @@ struct Line3D::Impl {
     bool fixed3Dreg = false, perform_RDD = false, matched = false;
     Vector3d translation;
     int shard_rank = 0, shard_world = 1; Line3D::MatchExchangeFn exchange = nullptr; void* exchange_user = nullptr;
+    // addImage with an image: the detector, the camera IDs whose image is being prepared, and the lock of the GPU step on ctx
+    Line3D::SegmentDetectorFn detector = nullptr; void* detector_user = nullptr;
+    std::set<unsigned int> reserved;
+    std::mutex prep_mtx;
+    struct { int (*fn)(void*, const unsigned char*, int, int, void*); void* user; } c_detector{nullptr, nullptr};   // l3dpp_set_segment_detector
     // index maps (rebuilt at matchImages)
     std::vector<HostView*> vlist;                         // by view index (ascending camID)
     std::map<unsigned int, int> index_of;
@@ -280,6 +287,8 @@ struct Line3D::Impl {
         const size_t e = est_of_gseg.at(v->seg_off + s.segID());
         return Segment3D(Vector3d(est_P[6 * e], est_P[6 * e + 1], est_P[6 * e + 2]), Vector3d(est_P[6 * e + 3], est_P[6 * e + 4], est_P[6 * e + 5]));
     }
+    bool segments_from_image(unsigned int camID, const Image8u& image, Line3D::SegmentDetectorFn fn, void* user, std::vector<Vec4f>& segs,
+                             std::string& why);
     bool line_from_cluster(const std::list<Segment2D>& cluster, LineCluster3D& out) const;
     Segment3D project_onto_line(const Segment2D& s2, const Segment3D& s3, bool& ok) const;
     std::list<Segment3D> collinear_segments(const LineCluster3D& cl) const;
@@ -407,6 +416,126 @@ bool Line3D::addImage(const unsigned int camID, const int w, const int h, const 
     P.visual_neighbors[camID];
     P.views_avg_depths.push_back((float)std::fmax((double)median_depth, EPS));
     return true;
+}
+
+// the post-processing of detectLineSegments (line3D.cc:320-360, commons.h:135-156): detections in the prepared (w_p x h_p) image are
+// scaled to the image's (w x h), their float length must exceed 0.005 * the image diagonal, std::priority_queue orders them longest
+// first (equal lengths in the heap's order) and at most max_segments are kept
+struct SegmentData2D { float p1x_, p1y_, p2x_, p2y_, length_; };
+struct SegmentData2D_comparison { bool operator()(const SegmentData2D& a, const SegmentData2D& b) const { return a.length_ < b.length_; } };
+static std::vector<Vec4f> filter_detections(const std::vector<Vec4f>& detections, int w, int h, int w_p, int h_p, unsigned int max_segments)
+{
+    const float upscale_x = float(w) / float(w_p), upscale_y = float(h) / float(h_p);
+    const float min_len = sqrtf(float(h * h) + float(w * w)) * 0.005f;                   // L3D_DEF_MIN_LINE_LENGTH_FACTOR
+    std::priority_queue<SegmentData2D, std::vector<SegmentData2D>, SegmentData2D_comparison> sorted;
+    for (const Vec4f& d : detections) {
+        SegmentData2D s;
+        s.p1x_ = d.v[0] * upscale_x; s.p1y_ = d.v[1] * upscale_y; s.p2x_ = d.v[2] * upscale_x; s.p2y_ = d.v[3] * upscale_y;
+        const float dx = s.p1x_ - s.p2x_, dy = s.p1y_ - s.p2y_;
+        s.length_ = sqrtf(dx * dx + dy * dy);
+        if (s.length_ > min_len) sorted.push(s);
+    }
+    std::vector<Vec4f> out;
+    out.reserve(std::min<size_t>(sorted.size(), max_segments));
+    while (!sorted.empty() && out.size() < max_segments) {
+        const SegmentData2D& s = sorted.top();
+        out.push_back(Vec4f{{s.p1x_, s.p1y_, s.p2x_, s.p2y_}});
+        sorted.pop();
+    }
+    return out;
+}
+
+// the segments of an image without given segments (detectLineSegments line3D.cc:249-372): the segment cache, or the prepared image
+// through the detector and the post-processing, then the cache is written.  false with `why` set if the view has to be rejected.
+bool Line3D::Impl::segments_from_image(unsigned int camID, const Image8u& image, Line3D::SegmentDetectorFn fn, void* user, std::vector<Vec4f>& segs,
+                                       std::string& why)
+{
+    const int w = image.cols, h = image.rows;
+    if (image.channels != 1 && image.channels != 3) {                                                     // line3D.cc:251-266
+        why = "image type not supported: " + std::to_string(image.channels) + " channels (8-bit grey or RGB images only)";
+        return false;
+    }
+    const std::string path = segmentCachePath(output_folder, camID, w, h, max_img_width);
+    if (load_segments && std::ifstream(path.c_str(), std::ios::binary)) {                                 // line3D.cc:295-309
+        std::string e;
+        if (!readSegmentCache(path, segs, &e)) { why = "unreadable segment cache " + e; return false; }
+        if (segs.empty()) { why = "the segment cache " + path + " holds no segments"; return false; }
+        return true;
+    }
+    if (!fn) {
+        why = load_segments ? "no line segments given and no segment cache " + path + " (line detection is outside this library)"
+                            : "no line segments given, and load_segments is off so the segment cache " + path + " was not read";
+        return false;
+    }
+    if (image.data.size() != (size_t)w * h * image.channels) { why = "the pixel buffer does not match rows x cols x channels"; return false; }
+    int w_p, h_p;
+    preparedImageSize(w, h, max_img_width, w_p, h_p);
+    Image8u gray(h_p, w_p, 1);
+    {
+        // the primary context is single-owner: one preparation at a time
+        std::lock_guard<std::mutex> g(prep_mtx);
+        l3d_image_prep_desc d;
+        std::memset(&d, 0, sizeof(d));
+        d.width = w; d.height = h; d.channels = image.channels; d.max_img_width = max_img_width;
+        d.src_pitch = (int64_t)w * image.channels; d.dst_pitch = w_p;
+        d.src = image.data.data(); d.dst = gray.data.data();
+        d.out_width = w_p; d.out_height = h_p;
+        if (l3d_prepare_gray_u8(ctx, 1, &d, 0) != L3D_OK) { why = std::string("image preparation: ") + l3d_last_error(ctx); return false; }
+    }
+    std::vector<Vec4f> detections;
+    if (!fn(user, gray, detections)) { why = "the segment detector failed"; return false; }
+    segs = filter_detections(detections, w, h, w_p, h_p, max_line_segments);
+    if (segs.empty()) {
+        why = "none of the " + std::to_string(detections.size()) + " detected segments is longer than 0.005 * the image diagonal";
+        return false;
+    }
+    if (load_segments) {                                                                                  // line3D.cc:363-366
+        std::string e;
+        mkdir((output_folder + "/L3D++_data").c_str(), 0777);     // the reference's constructor creates it (line3D.cc:59-61)
+        if (!writeSegmentCache(path, segs, &e)) log("WARNING: segment cache not written: " + e);
+    }
+    return true;
+}
+
+bool Line3D::addImage(const unsigned int camID, const Image8u& image, const Matrix3d& K, const Matrix3d& R, const Vector3d& t,
+                      const float median_depth, const std::list<unsigned int>& wps_or_neighbors, const std::vector<Vec4f>& line_segments)
+{
+    Impl& P = *p_;
+    const int w = image.cols, h = image.rows;
+    if (!line_segments.empty()) return addImage(camID, w, h, K, R, t, median_depth, wps_or_neighbors, line_segments);
+    // line3D.cc:116-155: the size, the camera ID (reserved until the view is added or rejected) and the world points, before any
+    // image work
+    Line3D::SegmentDetectorFn fn;
+    void* user;
+    {
+        std::lock_guard<std::mutex> g(P.mtx);
+        auto failed = [&](const std::string& what) { P.fail("addImage [" + std::to_string(camID) + "]: " + what); return false; };
+        if (std::max(w, h) < 800) return failed("image is too small for reliable results (larger side should be >= 800px)");
+        if (P.views.count(camID) || P.reserved.count(camID)) return failed("camera ID already in use");
+        if (wps_or_neighbors.empty()) return failed(P.by_wps ? "view has no worldpoints" : "view has no visual neighbors");
+        P.reserved.insert(camID);
+        fn = P.detector; user = P.detector_user;
+    }
+    struct Release {
+        Impl& P; unsigned int id;
+        ~Release() { std::lock_guard<std::mutex> g(P.mtx); P.reserved.erase(id); }
+    } release{P, camID};
+    std::vector<Vec4f> segs;
+    std::string why;
+    if (!P.segments_from_image(camID, image, fn, user, segs, why)) {
+        std::lock_guard<std::mutex> g(P.mtx);
+        P.fail("addImage [" + std::to_string(camID) + "]: " + why);
+        return false;
+    }
+    return addImage(camID, w, h, K, R, t, median_depth, wps_or_neighbors, segs);
+}
+
+void Line3D::setSegmentDetector(SegmentDetectorFn detector, void* user)
+{
+    Impl& P = *p_;
+    std::lock_guard<std::mutex> g(P.mtx);
+    P.err.clear();
+    P.detector = detector; P.detector_user = user;
 }
 
 void Line3D::matchImages(const float sigma_position, const float sigma_angle, const unsigned int num_neighbors, const float epipolar_overlap,
@@ -1058,6 +1187,72 @@ int l3dpp_set_lines(void* h, int nlines, const int* nseg, const double* segs6, c
 }
 int l3dpp_save_txt(void* h, const char* folder) { Line3D* L = (Line3D*)h; L->save3DLinesAsTXT(folder); return L->lastError()[0] ? -1 : 0; }
 int l3dpp_save_bin(void* h, const char* folder) { Line3D* L = (Line3D*)h; L->save3DLinesAsBIN(folder); return L->lastError()[0] ? -1 : 0; }
+// the full constructor with max_line_segments
+void* l3dpp_create_full(const char* output_folder, int load_segments, int max_img_width, unsigned int max_line_segments, int neighbors_by_worldpoints,
+                        int use_gpu, int device)
+{
+    try { return new Line3D(output_folder, load_segments != 0, max_img_width, max_line_segments, neighbors_by_worldpoints != 0, use_gpu != 0, device); }
+    catch (...) { return nullptr; }
+}
+// addImage with an image: rows x cols, 1 or 3 channels, row step in bytes; nseg == 0: no segments given
+int l3dpp_add_image_pixels(void* h, unsigned int cam, const unsigned char* pixels, int rows, int cols, int channels, long long step, const double* K,
+                           const double* R, const double* t, float median_depth, const unsigned int* list, int nlist, const float* segs, int nseg)
+{
+    Image8u img(rows, cols, channels);
+    const size_t row = (size_t)std::max(cols, 0) * std::max(channels, 0);
+    for (int r = 0; r < rows && row; ++r) memcpy(img.data.data() + r * row, pixels + r * step, row);
+    Matrix3d Km, Rm; memcpy(Km.m, K, 72); memcpy(Rm.m, R, 72);
+    std::vector<Vec4f> s(nseg); if (nseg) memcpy(s.data(), segs, 16 * (size_t)nseg);
+    Line3D* L = (Line3D*)h;
+    return L->addImage(cam, img, Km, Rm, Vector3d(t[0], t[1], t[2]), median_depth, std::list<unsigned int>(list, list + nlist), s) ? 0 : -1;
+}
+// detector in C terms: fn(user, gray, rows, cols, out) returns non-zero on success and hands its detections over with
+// l3dpp_push_detections(out, xy4, n) (any number of calls)
+typedef int (*l3dpp_detect_fn)(void* user, const unsigned char* gray, int rows, int cols, void* out);
+void l3dpp_push_detections(void* out, const float* xy4, long long n)
+{
+    std::vector<Vec4f>& v = *(std::vector<Vec4f>*)out;
+    const size_t k = v.size();
+    v.resize(k + (size_t)std::max(n, 0ll));
+    if (n > 0) memcpy(v.data() + k, xy4, 16 * (size_t)n);
+}
+static bool l3dpp_detect_trampoline(void* user, const Image8u& gray, std::vector<Vec4f>& detections)
+{
+    const Line3D::Impl& P = *(const Line3D::Impl*)user;
+    return P.c_detector.fn(P.c_detector.user, gray.data.data(), gray.rows, gray.cols, &detections) != 0;
+}
+int l3dpp_set_segment_detector(void* h, l3dpp_detect_fn fn, void* user)
+{
+    Line3D* L = (Line3D*)h;
+    Line3D::Impl& P = *L->impl();
+    { std::lock_guard<std::mutex> g(P.mtx); P.c_detector.fn = fn; P.c_detector.user = user; }
+    L->setSegmentDetector(fn ? l3dpp_detect_trampoline : nullptr, &P);
+    return 0;
+}
+// the 2D segments of a view through getSegmentCoords2D: out[cap * 4]; returns the view's segment count (-1 for an unknown camID)
+long long l3dpp_view_segments(void* h, unsigned int cam, float* out, long long cap)
+{
+    Line3D* L = (Line3D*)h;
+    long long n;
+    {
+        Line3D::Impl& P = *L->impl();
+        std::lock_guard<std::mutex> g(P.mtx);
+        auto it = P.views.find(cam);
+        if (it == P.views.end()) return -1;
+        n = (long long)it->second.lines.size();
+    }
+    for (long long i = 0; i < n && i < cap; ++i) memcpy(out + 4 * i, L->getSegmentCoords2D(cam, (unsigned int)i).v, 16);
+    return n;
+}
+// detectLineSegments' post-processing alone (no GPU): out[cap * 4]; returns the number of segments kept (even if > cap)
+long long l3dpp_filter_detections(const float* det, long long n, int w, int h, int w_p, int h_p, unsigned int max_segments, float* out, long long cap)
+{
+    std::vector<Vec4f> d((size_t)std::max(n, 0ll));
+    if (n > 0) memcpy(d.data(), det, 16 * (size_t)n);
+    const std::vector<Vec4f> r = filter_detections(d, w, h, w_p, h_p, max_segments);
+    if ((long long)r.size() <= cap && !r.empty()) memcpy(out, r.data(), 16 * r.size());
+    return (long long)r.size();
+}
 // Line3D::undistortImage on a packed image; K row-major, radial[3], tangential[2].  0, -1 (std::invalid_argument) or -2 (std::runtime_error)
 int l3dpp_undistort_image(const unsigned char* src, unsigned char* dst, int rows, int cols, int channels, const double* radial, const double* tangential,
                           const double* K)

@@ -5,6 +5,8 @@ Used by the tests and tools; the arithmetic is all in libl3d_b200.so (GPU) — n
 from __future__ import annotations
 
 import ctypes as C
+import threading
+
 import numpy as np
 
 from . import capi
@@ -24,13 +26,18 @@ def _p(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
 
 
+# Line3D::SegmentDetectorFn in C terms (l3dpp_set_segment_detector): (user, gray pixels, rows, cols, detections handle) -> non-zero on success
+DETECT_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_uint8), C.c_int, C.c_int, C.c_void_p)
+
+
 class Line3D:
     """addImage / matchImages / reconstruct3Dlines with the reference's argument meaning (line3D.h:80-166)."""
 
     def __init__(self, neighbors_by_worldpoints=True, use_gpu=True, device=0, output_folder=None, load_segments=True, max_img_width=-1,
-                 devices=None):
-        """output_folder / load_segments / max_img_width: the reference's constructor arguments; with an output folder, add_image
-        with no segments reads the segment cache under <output_folder>/L3D++_data/ (segment_cache_path).
+                 devices=None, max_line_segments=3000):
+        """output_folder / load_segments / max_img_width / max_line_segments: the reference's constructor arguments; with an output
+        folder, add_image with no segments reads the segment cache under <output_folder>/L3D++_data/ (segment_cache_path), and
+        add_image_pixels also writes it.
         devices: a list of CUDA devices in place of `device` (the first is the primary; repeats allowed): match_images splits the
         view pairs over them and gathers the matches on the primary, with the single-device result"""
         self.L = capi.lib()
@@ -47,6 +54,10 @@ class Line3D:
             self.L.l3dpp_create_devices.restype = C.c_void_p
             h = self.L.l3dpp_create_devices(str(output_folder or "").encode(), int(load_segments), int(max_img_width),
                                             int(neighbors_by_worldpoints), int(use_gpu), _p(devs), len(devs))
+        elif max_line_segments != 3000:
+            self.L.l3dpp_create_full.restype = C.c_void_p
+            h = self.L.l3dpp_create_full(str(output_folder or "").encode(), int(load_segments), int(max_img_width), C.c_uint(int(max_line_segments)),
+                                         int(neighbors_by_worldpoints), int(use_gpu), int(device))
         elif output_folder is None:
             h = self.L.l3dpp_create(int(neighbors_by_worldpoints), int(use_gpu), int(device))
         else:
@@ -78,6 +89,56 @@ class Line3D:
         f64 = lambda a: np.ascontiguousarray(a, np.float64)
         self._chk(self.L.l3dpp_add_image(self.h, C.c_uint(int(cam)), int(width), int(height), _p(f64(K)), _p(f64(R)), _p(f64(t)),
                                          C.c_float(float(median_depth)), _p(lst), len(lst), _p(segs), len(segs)), "addImage")
+
+    def add_image_pixels(self, cam, img, K, R, t, median_depth, wps_or_neighbors, segs=()):
+        """addImage with the image itself: img uint8 HxW (grey) or HxWx3 (channel 0 is R), any row stride.  Without segs the segment
+        cache is read, or the image is prepared on the GPU and handed to the set_segment_detector function.  An exception raised by
+        the detector is raised here again."""
+        a, sp = capi._image_rows(img)
+        lst = np.ascontiguousarray(wps_or_neighbors, np.uint32)
+        segs = np.ascontiguousarray(segs, np.float32).reshape(-1, 4)
+        f64 = lambda v: np.ascontiguousarray(v, np.float64)
+        errors = self.__dict__.setdefault("_detector_errors", {})      # per calling thread: the detector runs on it
+        errors.pop(threading.get_ident(), None)
+        rc = self.L.l3dpp_add_image_pixels(self.h, C.c_uint(int(cam)), C.c_void_p(a.ctypes.data), a.shape[0], a.shape[1], 1 if a.ndim == 2 else 3,
+                                           C.c_longlong(sp), _p(f64(K)), _p(f64(R)), _p(f64(t)), C.c_float(float(median_depth)), _p(lst), len(lst),
+                                           _p(segs), len(segs))
+        err = errors.pop(threading.get_ident(), None)
+        if err is not None:
+            raise err
+        self._chk(rc, "addImage")
+
+    def set_segment_detector(self, fn):
+        """fn(gray uint8 [rows, cols]) -> detections float32 [n, 4] (x1, y1, x2, y2 in gray's coordinates), or None / False to reject
+        the view; None: no detector.  It runs on the thread that called add_image_pixels, possibly on several at once."""
+        if fn is None:
+            cb = None
+        else:
+            def call(_user, gray, rows, cols, out):
+                try:
+                    det = fn(np.ctypeslib.as_array(gray, shape=(rows, cols)).copy())
+                    if det is None or det is False:
+                        return 0
+                    det = np.ascontiguousarray(det, np.float32).reshape(-1, 4)
+                    self.L.l3dpp_push_detections(C.c_void_p(out), _p(det), C.c_longlong(len(det)))
+                    return 1
+                except BaseException as e:      # noqa: BLE001 - handed back to add_image_pixels
+                    self.__dict__.setdefault("_detector_errors", {})[threading.get_ident()] = e
+                    return 0
+            cb = DETECT_FN(call)
+        self._detector = cb                     # the library keeps the pointer: keep the callback alive
+        self.L.l3dpp_set_segment_detector.argtypes = [C.c_void_p, DETECT_FN, C.c_void_p]
+        self.L.l3dpp_set_segment_detector(self.h, cb, None)
+
+    def view_segments(self, cam):
+        """float32 [n, 4]: the view's 2D segments as getSegmentCoords2D returns them"""
+        self.L.l3dpp_view_segments.restype = C.c_longlong
+        n = self.L.l3dpp_view_segments(self.h, C.c_uint(int(cam)), None, C.c_longlong(0))
+        if n < 0:
+            raise KeyError(cam)
+        out = np.zeros((n, 4), np.float32)
+        self.L.l3dpp_view_segments(self.h, C.c_uint(int(cam)), _p(out), C.c_longlong(n))
+        return out
 
     def add_scene(self, scene):
         for i in range(scene.num_views):
