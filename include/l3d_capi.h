@@ -244,7 +244,8 @@ long long l3d_rdd_affinity(l3d_ctx* ctx, int iters, int32_t* out_i, int32_t* out
  * Levenberg-Marquardt solves and the candidate costs run on the device for all lines at once; the host plays Ceres'
  * trust-region controller (one radius, its default tolerances).  Ceres itself is not needed.
  *   p1p2        6 doubles per line: the cluster's 3D segment in the working (translated) frame   optimization.cc:36-39
- *   res_ptr     num_lines+1 offsets into the residual arrays
+ *   res_ptr     num_lines+1 offsets into the residual arrays: res_ptr[0] == 0 and non-decreasing (else L3D_ERR_INVALID,
+ *               checked before anything is uploaded); line i owns residuals res_ptr[i] .. res_ptr[i+1]-1
  *   res_cam     per residual: index into cams
  *   res_xy      per residual: x1 y1 x2 y2 of the observed 2D segment (View::getLineSegment2D)     optimization.cc:155-166
  *   cams        16 doubles per camera: R (row-major), C (working frame), fx, fy, px, py           optimization.cc:108-141
@@ -252,7 +253,8 @@ long long l3d_rdd_affinity(l3d_ctx* ctx, int iters, int32_t* out_i, int32_t* out
  *   p1p2_out    updated segments (unit direction around the old mid point, optimization.cc:259-277); may alias p1p2
  *   valid_out   0 where the reference drops the cluster (optimization.cc:293-298)
  *   summary     optional, 8 doubles: iterations, initial cost, final cost, termination (0 convergence, 1 max_iter reached,
- *               2 failure), successful steps, free lines, final trust-region radius, kernels launched */
+ *               2 failure), successful steps, free lines, final trust-region radius, kernels launched.  Both costs are 0
+ *               when the first evaluation fails (a residual block with omega or the projected line's norm below 1e-12). */
 int l3d_optimize_lines(l3d_ctx* ctx, int num_lines, const double* p1p2, const long long* res_ptr, const int32_t* res_cam,
                        const double* res_xy, int num_cams, const double* cams, int max_iter, double* p1p2_out, int32_t* valid_out,
                        double* summary);

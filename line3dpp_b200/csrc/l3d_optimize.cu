@@ -324,8 +324,11 @@ int l3d_optimize_lines(l3d_ctx* c, int num_lines, const double* p1p2, const long
     if (summary) for (int k = 0; k < 8; ++k) summary[k] = 0.0;
     if (num_lines == 0) return L3D_OK;
     const int L = num_lines;
+    if (res_ptr[0] != 0) return l3d_fail(c, L3D_ERR_INVALID, "l3d_optimize_lines: res_ptr[0] must be 0");
+    for (int i = 0; i < L; ++i)
+        if (res_ptr[i + 1] < res_ptr[i]) return l3d_fail(c, L3D_ERR_INVALID, "l3d_optimize_lines: res_ptr must not decrease");
     const long long NR = res_ptr[L];
-    if (NR < 0 || (NR && (!res_cam || !res_xy || !cams || num_cams == 0))) return l3d_fail(c, L3D_ERR_INVALID, "l3d_optimize_lines: bad residual arrays");
+    if (NR && (!res_cam || !res_xy || !cams || num_cams == 0)) return l3d_fail(c, L3D_ERR_INVALID, "l3d_optimize_lines: bad residual arrays");
     for (long long r = 0; r < NR; ++r) if (res_cam[r] < 0 || res_cam[r] >= num_cams) return l3d_fail(c, L3D_ERR_INVALID, "l3d_optimize_lines: camera index out of range");
     cudaSetDevice(c->device);
     OptState& O = c->opt;
@@ -375,9 +378,9 @@ int l3d_optimize_lines(l3d_ctx* c, int num_lines, const double* p1p2, const long
     double cost = 0.0, cost0 = 0.0, radius = 1e4;
     if (max_iter >= 0) {
         if ((rc = linearize())) return rc;
-        cost = cost0 = h[0];
-        if (h[2] > 0.0) term = 2;                                    // initial evaluation failed: nothing is changed
+        if (h[2] > 0.0) term = 2;                                    // initial evaluation failed: nothing is changed, no cost reported
         else {
+            cost = cost0 = h[0];
             k_opt_scale<<<nbl, 128, 0, st>>>(L, isfree, (const double*)O.d_H.p, (double*)O.d_S.p); ++launches;
             double decrease_factor = 2.0; bool reuse_diagonal = false; int invalid = 0;
             bool done = h[1] <= 1e-10;                               // gradient tolerance at iteration zero
