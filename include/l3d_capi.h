@@ -210,7 +210,10 @@ long long l3d_get_collinear(l3d_ctx* ctx, int view, long long* row_ptr_out, int3
  * "unused" de-duplication and local-id assignment stay on the host (line3D.cc:1881-1900, 1982-2023).  Needs
  * views[].median_depth to be current (l3d_update_view_params).  Returns the number of edges (even if > cap).
  * With collinearity links on (l3d_find_collinear) the list also holds the collinear candidates, each of which only
- * counts if its parent edge passed unused(): use l3d_affinity_matrix, which resolves that on the device. */
+ * counts if its parent edge passed unused(): use l3d_affinity_matrix, which resolves that on the device.
+ * min_affinity must be >= 0 (the reference's constant is 0.5): a segment without an estimate has similarity 0, and below 0 the
+ * reference's loop would accept it, which the device does not model.  A negative or NaN min_affinity is rejected with
+ * L3D_ERR_INVALID by this call and by l3d_affinity_matrix, and the rejected call drops any affinity matrix the context held. */
 long long l3d_affinity_edges(l3d_ctx* ctx, float two_sigA_sqr, float med_scene_depth_lines, float min_affinity,
                              long long* out_gi, long long* out_gj, float* out_w, long long cap);
 

@@ -605,6 +605,7 @@ long long l3d_affinity_edges(l3d_ctx* c, float two_sigA_sqr, float med_scene_dep
                              long long* out_gi, long long* out_gj, float* out_w, long long cap)
 {
     if (!c) return L3D_ERR_INVALID;
+    if (!(min_affinity >= 0.0f)) { c->drop(Stage::Affinity); return l3d_fail(c, L3D_ERR_INVALID, "l3d_affinity_edges: min_affinity must be >= 0"); }
     if (!c->sweep.valid) return l3d_fail(c, L3D_ERR_STATE, "l3d_affinity_edges: call l3d_score_sweep first");
     cudaSetDevice(c->device);
     const AffinityState& A = c->aff;
@@ -631,6 +632,7 @@ long long l3d_affinity_matrix(l3d_ctx* c, float two_sigA_sqr, float med_scene_de
 {
     if (!c) return L3D_ERR_INVALID;
     AffinityState& A = c->aff;
+    if (!(min_affinity >= 0.0f)) { c->drop(Stage::Affinity); return l3d_fail(c, L3D_ERR_INVALID, "l3d_affinity_matrix: min_affinity must be >= 0"); }
     const bool cached = A.valid && A.two_sigA_sqr == two_sigA_sqr && A.med == med_scene_depth_lines && A.min_aff == min_affinity;
     if (!cached) c->drop(Stage::Affinity);
     if (!num_ids) return L3D_ERR_INVALID;
