@@ -6,11 +6,11 @@
 //   k_pair_arcs,    : level-1 tables of the view pairs of one call (l3d_device.cuh "pencil parameter"): every target segment as an arc of
 //   k_arcs_gather     the epipolar pencil, grouped by arc length and sorted by arc start (one radix sort in between, l3d_capi.cu); the
 //                     table carries each arc's target segment in a parallel array (32 B per pair and target).
-//   k_match_topk    : production kernel.  One CTA per SM (24 warps) = one work unit: a view pair and up to 1024 of its source rows.
+//   k_match_topk    : production kernel.  One CTA per SM (32 warps) = one work unit: a view pair and up to 1024 of its source rows.
 //                     The pair's table (arcs + segments) is staged in shared memory by 1-D TMA (cp.async.bulk + mbarrier, 6 stages x
 //                     512 entries x 32 B in flight from the first instruction): a target view of up to 3072 segments is resident in one
 //                     pass, and a warp takes the unit's rows one at a time from a shared counter into one of its 8 row slots (constants,
-//                     key list, score-to-beat), with no CTA barrier; larger target views take several passes over units of at most 192
+//                     key list, score-to-beat), with no CTA barrier; larger target views take several passes over units of at most 256
 //                     rows, each slot bound to one row.  Per row the warp binary-searches the
 //                     window of every arc class and scans only those entries, all windows as one concatenation (full warps): each
 //                     lane runs the arc test (13 integer instructions) and the conservative float filter (27 flop + 2 rcp on the
@@ -82,7 +82,8 @@ struct MatchSmem {
     L3DPairBasis B;                                  // the pair's pencil basis and the first sorted entry of every arc class, and the end (k_pair_arcs)
     float F[9];                                      // the pair's float fundamental matrix (row constants)
     int next_row;                                    // single-pass units: the next row a warp takes
-    int nrows, npass;                                // rows of the unit, passes over the target view (read here, not held in registers across the exact path)
+    int nrows, nt, npass, pass;                      // rows of the unit, target segments, passes over the target view and the current pass
+                                                     // (read here, not held in registers across the exact path)
     unsigned long long bars[MK_STAGES];
     // per-CTA constants of the (rarely executed, deliberately out-of-line) exact path
     const float4* cache; const float4* ssegs;        // float ray cache; the unit's first source segment
@@ -405,14 +406,15 @@ k_arcs_gather(long long n, const unsigned long long* __restrict__ keys, const un
     out_segs[i] = segs[views[P->tgt].seg_off + j];
 }
 
-// thread 0: start the TMA copies of the level-1 entries [base, base + cnt) of a pair into the ring; the arcs and the segments of a
-// stage complete on the stage's barrier together
-__device__ __forceinline__ void stage_entries(MatchSmem& S, int base, int cnt)
+// thread 0: start the TMA copies of the level-1 entries of pass `pass` of a pair into the ring; the arcs and the segments of a stage
+// complete on the stage's barrier together
+__device__ __forceinline__ void stage_entries(MatchSmem& S, int pass)
 {
     const uint4* arcs = S.tarcs; const float4* asegs = S.tasegs;
-    for (int i = 0; i < MK_STAGES && i * MK_TT < cnt; ++i) {
-        const unsigned int bytes = (unsigned int)min(MK_TT, cnt - i * MK_TT) * 16u;
-        const size_t o = (size_t)base + (size_t)i * MK_TT;
+    for (int i = 0; i < MK_STAGES; ++i) {
+        const int o = (pass * MK_STAGES + i) * MK_TT, n = min(MK_TT, S.nt - o);
+        if (n <= 0) break;
+        const unsigned int bytes = (unsigned int)n * 16u;
         mbar_expect_tx(&S.bars[i], 2u * bytes);
         tma_load_1d(S.stage[i], arcs + o, bytes, &S.bars[i]);
         tma_load_1d(S.stage_seg[i], asegs + o, bytes, &S.bars[i]);
@@ -477,19 +479,22 @@ __device__ __forceinline__ void drain_queue(MatchSmem& S, int warp, int lane, in
     }
 }
 
-// Scan the window entries of the row in slot sl that lie in the resident ring entries [base, base + cnt) of the pair's level-1 table and
-// queue the survivors of both filters; the queue is evaluated 32 at a time.
+// Scan the window entries of the row in slot sl that lie in the ring entries [base, base + cnt) of the pair's level-1 table resident in
+// the current pass, and queue the survivors of both filters; the queue is evaluated 32 at a time.
 template <int SEM, Keep KEEP>
-__device__ __forceinline__ void scan_row(MatchSmem& S, int sl, int base, int cnt, int warp, int lane, int& qn)
+__device__ __forceinline__ void scan_row(MatchSmem& S, int sl, int warp, int lane, int& qn)
 {
+    const int base = S.pass * (MK_STAGES * MK_TT), cnt = min(MK_STAGES * MK_TT, S.nt - base);
     MPROBE(const long long t_row = clock64(); long long t_exact = 0;)
     const unsigned int lt_mask = (1u << lane) - 1u;
     const uint4* ent = &S.stage[0][0];
     const int* cls_off = S.B.cls_off;
-    const uint2 kr = S.rowK[sl];
-    const bool rall = S.rowall[sl] != 0;
-    const float4 rA = S.rowA[sl];
-    float4 rB = S.rowB[sl];                     // rB.w: the score-to-beat, re-read after exact batches (a stale value only rejects less)
+    // the row's constants, re-read from shared memory after exact batches instead of held across them (register budget of 32 warps);
+    // rB.w: the score-to-beat, which the batches may raise (a stale value only rejects less)
+    uint2 kr = S.rowK[sl];
+    bool rall = S.rowall[sl] != 0;
+    float4 rA = S.rowA[sl];
+    float4 rB = S.rowB[sl];
     // short arc [ka, kb] between the two kappa values: a target of class c can only match if its arc starts in [ka - 2^(CLS0 + c), kb]
     const bool fwd = (kr.y - kr.x) < 0x80000000u;
     const unsigned int ka = fwd ? kr.x : kr.y, kb = fwd ? kr.y : kr.x;
@@ -550,7 +555,7 @@ __device__ __forceinline__ void scan_row(MatchSmem& S, int sl, int base, int cnt
                 MPROBE(const long long t0 = clock64();)
                 do { qn -= 32; exact_batch<SEM, KEEP>(S, S.queue[warp][qn + lane], true, lane); MPROBE(probe_add(S, warp, lane, MP_EVALS, 32);) } while (qn >= 32);
                 MPROBE(t_exact += clock64() - t0;)
-                rB.w = S.rowB[sl].w;
+                kr = S.rowK[sl]; rall = S.rowall[sl] != 0; rA = S.rowA[sl]; rB = S.rowB[sl];
             }
         }
     }
@@ -583,7 +588,7 @@ __global__ void __launch_bounds__(MK_THREADS, 1) k_match_topk(const MatchArgs A)
     if (tid == 0) {
         const long long soff = __ldg(&vs->seg_off);
         S.cache = A.cache; S.ssegs = A.segs + soff + row0; S.src_base = soff + row0; S.toff = __ldg(&vt->seg_off);
-        S.epi = A.epi; S.knn = A.knn; S.cap = MK_CAP; S.next_row = 0; S.nrows = nrows; S.npass = npass;
+        S.epi = A.epi; S.knn = A.knn; S.cap = MK_CAP; S.next_row = 0; S.nrows = nrows; S.nt = Nt; S.npass = npass; S.pass = 0;
         S.tarcs = A.arcs + __ldg(&P->arc_off); S.tasegs = A.arc_segs + __ldg(&P->arc_off);
         S.Cs = make_float3(__ldg(&vs->C[0]), __ldg(&vs->C[1]), __ldg(&vs->C[2])); S.Ct = make_float3(__ldg(&vt->C[0]), __ldg(&vt->C[1]), __ldg(&vt->C[2]));
         S.R0 = __ldg(&P->row_off) + row0; S.counts_out = A.counts; S.recs_out = A.recs;
@@ -594,7 +599,7 @@ __global__ void __launch_bounds__(MK_THREADS, 1) k_match_topk(const MatchArgs A)
         }
         for (int i = 0; i < MK_STAGES; ++i) mbar_init(&S.bars[i], 1);
         mbar_fence_init();
-        stage_entries(S, 0, min(RES, Nt));              // the first pass is in flight while the rows are set up
+        stage_entries(S, 0);                            // the first pass is in flight while the rows are set up
     }
     constexpr int NB = (int)(sizeof(L3DPairBasis) / sizeof(int));
     static_assert(sizeof(L3DPairBasis) % sizeof(int) == 0 && NB + 9 + 1 <= MK_THREADS, "one word per thread");
@@ -606,26 +611,20 @@ __global__ void __launch_bounds__(MK_THREADS, 1) k_match_topk(const MatchArgs A)
     MPROBE(probe_add(S, warp, lane, MP_WAIT, clock64() - t_wait);)
 
     int qn = 0;    // warp-uniform fill of the candidate queue
-    for (int pass = 0; pass < S.npass; ++pass) {
-        const int base = pass * RES, cnt = min(RES, Nt - base);
-        MPROBE(t_wait = clock64();)
-        if (pass > 0) {                                // everybody is done with the resident entries: refill
-            __syncthreads();
-            if (tid == 0) stage_entries(S, base, cnt);
-        }
-        for (int i = 0; i < MK_STAGES && i * MK_TT < cnt; ++i) mbar_wait(&S.bars[i], (unsigned int)(pass & 1));
+    MPROBE(t_wait = clock64();)
+    while (S.pass < S.npass) {                         // passes over the target view
+        for (int i = 0; i < MK_STAGES && (S.pass * MK_STAGES + i) * MK_TT < S.nt; ++i) mbar_wait(&S.bars[i], (unsigned int)(S.pass & 1));
         MPROBE(probe_add(S, warp, lane, MP_WAIT, clock64() - t_wait);)
-        for (int taken = 0;; ++taken) {
-            // next row: single pass, the next untaken row of the unit; several passes, the warp's fixed rows
-            int rl = warp * MK_SLOTS + taken;
+        for (int sl = warp * MK_SLOTS;;) {
+            // next row: single pass, the next untaken row of the unit; several passes, the warp's fixed rows (slot sl holds row sl)
+            int rl = sl;
             if (S.npass == 1) {
                 if (lane == 0) rl = atomicAdd(&S.next_row, 1);
                 rl = __shfl_sync(0xffffffffu, rl, 0);
-            } else if (taken == MK_SLOTS) break;
+            }
             if (rl >= S.nrows) break;
-            const int sl = warp * MK_SLOTS + taken % MK_SLOTS;
-            if (pass == 0) {
-                if (taken >= MK_SLOTS) {               // the slot's previous row: its queued candidates first (rarely any), then its result
+            if (S.pass == 0) {
+                if (S.slot_row[sl] >= 0) {             // the slot's previous row: its queued candidates first (rarely any), then its result
                     if (__any_sync(0xffffffffu, lane < qn && (S.queue[warp][lane] >> 24) == (unsigned int)sl)) {
                         MPROBE(probe_add(S, warp, lane, MP_DRAINS, 1);)
                         drain_queue<SEM, KEEP>(S, warp, lane, qn);
@@ -638,9 +637,18 @@ __global__ void __launch_bounds__(MK_THREADS, 1) k_match_topk(const MatchArgs A)
                 setup_row(S, sl, rl, lane);
                 MPROBE(probe_add(S, warp, lane, MP_SETUP, clock64() - t0); probe_add(S, warp, lane, MP_ROWS, 1);)
             }
-            scan_row<SEM, KEEP>(S, sl, base, cnt, warp, lane, qn);
+            scan_row<SEM, KEEP>(S, sl, warp, lane, qn);
+            if (++sl == (warp + 1) * MK_SLOTS) {       // the warp's slots hold its rows in turn; several passes: one row per slot
+                if (S.npass > 1) break;
+                sl = warp * MK_SLOTS;
+            }
         }
         drain_queue<SEM, KEEP>(S, warp, lane, qn);     // the queue holds ring positions: empty it before the ring is refilled
+        MPROBE(t_wait = clock64();)
+        if (S.pass + 1 == S.npass) break;
+        __syncthreads();                               // everybody is done with the resident entries: refill
+        if (tid == 0) { ++S.pass; stage_entries(S, S.pass); }
+        __syncthreads();                               // the new pass index is visible to every warp
     }
     MPROBE(const long long t_fin = clock64();)
     for (int i = 0; i < MK_SLOTS; ++i) {

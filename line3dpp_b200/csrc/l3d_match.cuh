@@ -5,13 +5,14 @@
 
 /* geometry of k_match_topk (one CTA per SM); every knob can be overridden with -D for the sweep (tools/sweep_tiles.py) */
 #ifndef MK_WARPS
-#define MK_WARPS 24
+#define MK_WARPS 32
 #endif
 #define MK_THREADS (32 * MK_WARPS)
 #ifndef MK_SLOTS
 #define MK_SLOTS 8                      /* row slots per warp: key list, threshold, count and constants of a row in flight */
 #endif
 #define MK_NSLOT (MK_WARPS * MK_SLOTS)  /* row slots per CTA; also the most rows of a unit whose target view takes several passes */
+static_assert(MK_NSLOT <= 256, "a queue entry is (slot << 24) | ring position: 8 bits of slot");
 #ifndef MK_UNIT_ROWS
 #define MK_UNIT_ROWS 1024               /* most source rows per work unit (one CTA) of a pair whose target view is resident */
 #endif
