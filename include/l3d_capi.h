@@ -99,7 +99,8 @@ int l3d_match_pairs(l3d_ctx* ctx, int num_pairs, const int32_t* pairs, const flo
 /* sharded form (SURVEY.md 8e: view pairs are independent given all segment lists): the whole pair list is staged, so
  * row offsets and buffer sizes are those of the full job, but only pairs [first_pair, last_pair) are evaluated here;
  * the rows of the other pairs are filled in by the caller (l3d_match_device_buffers + a broadcast from their owner)
- * before l3d_score_sweep. l3d_match_pairs == the range [0, num_pairs). */
+ * before l3d_score_sweep; for kNN <= 0 or > 32 the counts first, then l3d_match_restride(ctx, 0), then the records at that stride.
+ * l3d_match_pairs == the range [0, num_pairs). */
 int l3d_match_pairs_range(l3d_ctx* ctx, int num_pairs, const int32_t* pairs, const float* F, float epi_overlap, int knn,
                           int first_pair, int last_pair);
 /* l3d_match_pairs + download in ONE call, overlapped (the shape of match_lines_GPU, which returns host lists): the pair
@@ -145,6 +146,15 @@ int l3d_balanced_split(const long long* cost, int n, int parts, int32_t* bounds_
  * match what the sources evaluated.  Failed or not, dst's scoring sweep and everything after it are dropped; a failed call also
  * drops dst's match result. */
 int l3d_match_gather(l3d_ctx* dst, int n_src, l3d_ctx* const* src, const int32_t* pair_bounds);
+/* re-lay the record array of the current match result at `stride` slots per row, wider or narrower; the counts and every row's records
+ * up to its count stay as they are.  stride <= 0: the largest entry of the current count array (at least 1), reduced on the device.
+ * This is how ranks that matched disjoint shares of a keep-all (kNN <= 0) or kNN > 32 job agree on one stride without another
+ * collective: exchange the counts, call this with 0 (every rank now reduces the same counts), then exchange the records at the stride it
+ * returns.  Returns the stride chosen, or L3D_ERR_STATE without a match result, L3D_ERR_INVALID for a stride below some row's count or
+ * total_rows * stride >= 2^31 (the scoring sweep indexes slots in 32 bits).  Waits for the copy.  The buffer l3d_match_device_buffers
+ * returned before is freed: ask again.  Failed or not, the scoring sweep and everything after it are dropped; a failed call also drops
+ * the match result. */
+int l3d_match_restride(l3d_ctx* ctx, int stride);
 /* sizes of the last l3d_match_pairs result */
 long long l3d_match_total_rows(const l3d_ctx* ctx);      /* sum of Ns over pairs */
 long long l3d_match_total_matches(l3d_ctx* ctx);         /* matches of the last result (sum of the row counts), reduced on the device */

@@ -315,9 +315,15 @@ public:
     /* Multi-GPU matching (SURVEY.md 8e). One Line3D per GPU / process, every one fed the same images. With world > 1
      * matchImages evaluates only this rank's contiguous, cost-balanced share of the view pairs and then calls
      * `exchange(user, counts_dev, recs_dev, row_bounds, world, knn)`: rank r owns rows [row_bounds[r], row_bounds[r+1]) of
-     * counts (int32 per row) and recs (knn * 24 B per row), both DEVICE pointers; on return every rank must hold all rows
-     * (an NCCL broadcast per owner; line3dpp_b200/dist.py does it with torch.distributed). Scoring, affinity, diffusion and
-     * clustering then run replicated, so every rank ends with the single-GPU result bit for bit. Return 0 on success.
+     * counts (int32 per row) and recs (knn * 24 B per row: `knn` is the row stride of recs_dev), both DEVICE pointers; on return
+     * every rank must hold all rows (an NCCL broadcast per owner; line3dpp_b200/dist.py does it with torch.distributed). Scoring,
+     * affinity, diffusion and clustering then run replicated, so every rank ends with the single-GPU result bit for bit. Return 0
+     * on success.
+     * 1 <= kNN <= 32: one call, knn = kNN.  kNN <= 0 (keep all matches) and kNN > 32: the stride is only known once every row's
+     * count is, so there are two calls.  The first has knn = 0 and moves only the counts (recs is 0 B per row).  Every rank then
+     * re-lays its rows at the longest row of the whole job (after the cut to kNN when kNN > 32), and the second call has knn = that
+     * stride and a recs_dev that may differ from the first call's; it must move the records (the counts may move again).  A non-zero return
+     * from either call fails matchImages.
      * With several devices per Line3D, they split this rank's share and gather it on the primary before the exchange, which then
      * sees the primary's buffers. */
     typedef int (*MatchExchangeFn)(void* user, void* counts_dev, void* recs_dev, const long long* row_bounds, int world, int knn);

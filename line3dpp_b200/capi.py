@@ -234,6 +234,11 @@ class Context:
         self._chk(self.L.l3d_match_gather(self.h, len(sources), hs, _p(b)), "l3d_match_gather")
         self._knn = int(self.L.l3d_match_stride(self.h))
 
+    def match_restride(self, stride=0) -> int:
+        """l3d_match_restride: re-lay the records at `stride` slots per row (<= 0: the longest row); returns the stride"""
+        self._knn = int(self._chk(self.L.l3d_match_restride(self.h, int(stride)), "l3d_match_restride"))
+        return self._knn
+
     def pair_row_offsets(self, num_pairs):
         out = np.zeros(num_pairs + 1, np.int64)
         self._chk(self.L.l3d_pair_row_offsets(self.h, _p(out)), "l3d_pair_row_offsets")

@@ -346,6 +346,42 @@ static int run_topk(l3d_ctx* c, const MatchArgs& a, const HostOut* host)
     return L3D_OK;
 }
 
+// *out = the largest entry of the count array, at least 1 (the smallest stride a record array can have).  Waits for the stream.
+static int row_max(l3d_ctx* c, int* out)
+{
+    const long long rows = c->total_rows;
+    int rc, m = 0;
+    if (rows > 0) {
+        if (rows > INT_MAX) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: more than 2^31 rows with kNN <= 0");
+        L3D_RESERVE(c->d_rowptr, 16, "row max");
+        int* d_max = (int*)c->d_rowptr.p;
+        if ((rc = l3d_cub(c, "row maximum", [&](void* tmp, size_t& bytes) {
+                 return cub::DeviceReduce::Max(tmp, bytes, (const int*)c->d_counts.p, d_max, (int)rows, c->stream); }))) return rc;
+        c->launches += 1;
+        L3D_CUDA(c, cudaMemcpyAsync(&m, d_max, sizeof(int), cudaMemcpyDeviceToHost, c->stream), "row maximum");
+        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync");
+    }
+    *out = std::max(m, 1);
+    return L3D_OK;
+}
+
+// The record array at `stride` slots per row in a new buffer: rows [a, z) are copied pitched (the first min(old, new) slots of each,
+// no kernel), the others are left unset.  Waits for the copy, because the old buffer is freed on return.
+static int relay_recs(l3d_ctx* c, int stride, long long a, long long z)
+{
+    const size_t REC = sizeof(l3d_match_rec);
+    int rc;
+    DevBuf out;
+    if ((rc = out.reserve(c, REC * (size_t)std::max<long long>(c->total_rows, 1) * stride, "re-laid match records"))) return rc;
+    if (z > a)
+        L3D_CUDA(c, cudaMemcpy2DAsync((char*)out.p + REC * a * stride, REC * stride, (const char*)c->d_recs.p + REC * a * c->knn, REC * c->knn,
+                                      REC * std::min(stride, c->knn), (size_t)(z - a), cudaMemcpyDeviceToDevice, c->stream), "re-lay match records");
+    L3D_CUDA(c, cudaStreamSynchronize(c->stream), "re-lay match records");
+    std::swap(c->d_recs, out);
+    c->knn = stride;
+    return L3D_OK;
+}
+
 // "Keep all matches" (kNN <= 0, cudawrapper.cu:628-636, line3D.cc:988-996): count pass -> row stride = largest row -> store pass ->
 // rows sorted.  big_k > 0 (kNN > 32 exceeds the fused kernel's per-row key list): the same passes, and every row is cut to its big_k
 // best afterwards (same matches as the reference's priority queue, line3D.cc:999-1006 / cudawrapper.cu:637-645).
@@ -357,15 +393,7 @@ static int run_keep_all(l3d_ctx* c, MatchArgs a, int big_k)
     if (nunits) {
         a.knn = 0; a.recs = nullptr;
         if ((rc = launch_match(c, Keep::Count, a, 0, nunits, "k_match_topk (count)"))) return rc;
-        if (rows > INT_MAX) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: more than 2^31 rows with kNN <= 0");
-        L3D_RESERVE(c->d_rowptr, 16, "row max");
-        int* d_max = (int*)c->d_rowptr.p;
-        if ((rc = l3d_cub(c, "row maximum", [&](void* tmp, size_t& bytes) {
-                 return cub::DeviceReduce::Max(tmp, bytes, (const int*)c->d_counts.p, d_max, (int)rows, c->stream); }))) return rc;
-        c->launches += 1;
-        L3D_CUDA(c, cudaMemcpyAsync(&stride, d_max, sizeof(int), cudaMemcpyDeviceToHost, c->stream), "row maximum");
-        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync");
-        stride = std::max(stride, 1);
+        if ((rc = row_max(c, &stride))) return rc;
     }
     c->knn = stride;
     L3D_RESERVE(c->d_recs, sizeof(l3d_match_rec) * (size_t)std::max<long long>(rows, 1) * stride, "match records");
@@ -558,17 +586,11 @@ static int gather_rows(l3d_ctx* d, int n, l3d_ctx* const* src, const int32_t* b)
     for (int i = 0; i < n; ++i) { stride = std::max(stride, src[i]->knn); d_is_src |= src[i] == d; }
     if (!topk && stride != d->knn) {
         if (d_is_src) {     // re-lay d's own rows at the wider stride (d's stride is one of the maximum's terms, so it is the smaller)
-            const long long a = row_of_pair(d, d->first_pair), z = row_of_pair(d, d->last_pair);
-            DevBuf wide;
-            if ((rc = wide.reserve(d, REC * (size_t)std::max<long long>(d->total_rows, 1) * stride, "gathered match records"))) return rc;
-            if (z > a)
-                L3D_CUDA(d, cudaMemcpy2DAsync((char*)wide.p + REC * a * stride, REC * stride, (const char*)d->d_recs.p + REC * a * d->knn, REC * d->knn,
-                                              REC * d->knn, (size_t)(z - a), cudaMemcpyDeviceToDevice, d->stream), "re-lay match records");
-            L3D_CUDA(d, cudaStreamSynchronize(d->stream), "re-lay match records");   // the old buffer is freed below
-            std::swap(d->d_recs, wide);
-        } else if ((rc = d->d_recs.reserve(d, REC * (size_t)std::max<long long>(d->total_rows, 1) * stride, "gathered match records")))
-            return rc;
-        d->knn = stride;
+            if ((rc = relay_recs(d, stride, row_of_pair(d, d->first_pair), row_of_pair(d, d->last_pair)))) return rc;
+        } else {
+            if ((rc = d->d_recs.reserve(d, REC * (size_t)std::max<long long>(d->total_rows, 1) * stride, "gathered match records"))) return rc;
+            d->knn = stride;
+        }
     }
     const long long r0 = row_of_pair(d, b[0]), r1 = row_of_pair(d, b[n]);
     if (r0 > 0) L3D_CUDA(d, cudaMemsetAsync(d->d_counts.p, 0, sizeof(int) * r0, d->stream), "clear counts");
@@ -602,6 +624,35 @@ int l3d_match_gather(l3d_ctx* dst, int n_src, l3d_ctx* const* src, const int32_t
     if (rc || (rc = gather_rows(dst, n_src, src, pair_bounds))) return rc;
     dst->have_matches = true;
     return L3D_OK;
+}
+
+static int restride(l3d_ctx* c, int stride)
+{
+    cudaSetDevice(c->device);
+    const long long SLOTS = 1ll << 31;      // the scoring sweep indexes record slots in 32 bits (l3d_score_sweep)
+    const char* too_many = "l3d_match_restride: 2^31 or more record slots";
+    if (c->total_rows >= SLOTS) return l3d_fail(c, L3D_ERR_INVALID, too_many);
+    int longest, rc;
+    if ((rc = row_max(c, &longest))) return rc;
+    if (stride <= 0) stride = longest;
+    if (stride < longest) {
+        char msg[128];
+        snprintf(msg, sizeof(msg), "l3d_match_restride: stride %d is below the longest row (%d matches)", stride, longest);
+        return l3d_fail(c, L3D_ERR_INVALID, msg);
+    }
+    if (c->total_rows * stride >= SLOTS) return l3d_fail(c, L3D_ERR_INVALID, too_many);
+    return stride == c->knn ? L3D_OK : relay_recs(c, stride, 0, c->total_rows);
+}
+
+int l3d_match_restride(l3d_ctx* c, int stride)
+{
+    if (!c) return L3D_ERR_INVALID;
+    if (!c->have_matches) return l3d_fail(c, L3D_ERR_STATE, "l3d_match_restride: no match result");
+    c->drop(Stage::Matches);                // the rows move under the sweep and what follows it
+    const int rc = restride(c, stride);
+    if (rc) return rc;
+    c->have_matches = true;
+    return c->knn;
 }
 
 int l3d_match_stride(const l3d_ctx* c) { return c && c->have_matches ? c->knn : L3D_ERR_STATE; }

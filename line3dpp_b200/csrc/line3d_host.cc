@@ -642,7 +642,6 @@ void Line3D::matchImages(const float sigma_position, const float sigma_angle, co
         if (e1) cudaEventDestroy(e1);
         return ok;
     };
-    if (ok && P.shard_world > 1 && (P.kNN <= 0 || P.kNN > 32)) { P.fail("matchImages: kNN <= 0 (keep all matches) or kNN > 32 cannot be sharded: the row stride is only known after matching"); ok = false; }
     if (ok && P.shard_world > 1) {
         // this rank's contiguous share of the pair list, balanced by Ns*Nt; the same split on every rank
         std::vector<long long> cost((size_t)npairs), row_off((size_t)npairs + 1), row_bounds((size_t)P.shard_world + 1);
@@ -655,7 +654,19 @@ void Line3D::matchImages(const float sigma_position, const float sigma_angle, co
         ok = ok && P.chk(l3d_match_device_buffers(P.ctx, &dc, &dr), "l3d_match_device_buffers");
         if (ok) {
             for (int r = 0; r <= P.shard_world; ++r) row_bounds[r] = row_off[bounds[r]];
-            if (P.exchange(P.exchange_user, dc, dr, row_bounds.data(), P.shard_world, P.kNN) != 0) { P.fail("matchImages: the match exchange callback failed"); ok = false; }
+            auto exchange = [&](int knn, const char* what) {
+                if (P.exchange(P.exchange_user, dc, dr, row_bounds.data(), P.shard_world, knn) == 0) return true;
+                P.fail(std::string("matchImages: the match exchange callback failed") + what);
+                return false;
+            };
+            if (P.kNN >= 1 && P.kNN <= 32) ok = exchange(P.kNN, "");
+            else {
+                // Keep-all and kNN > 32: every rank laid out its records at the longest row of its own share.  Once the counts are
+                // exchanged, every rank reduces the same counts to the same stride and re-lays its rows at it; then the records move.
+                int stride = 0;
+                ok = exchange(0, " (row counts)") && P.chk(stride = l3d_match_restride(P.ctx, 0), "l3d_match_restride") &&
+                     P.chk(l3d_match_device_buffers(P.ctx, &dc, &dr), "l3d_match_device_buffers") && exchange(stride, " (records)");
+            }
         }
     } else
         ok = ok && match_range(0, npairs) && P.chk(l3d_sync(P.ctx), "l3d_sync");

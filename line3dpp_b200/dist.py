@@ -4,11 +4,13 @@ Every rank holds all images, matches its contiguous, cost-balanced share of the 
 (computeMatches order, line3D.cc:704-741) with `l3d_match_pairs_range`, and then needs the rows of the other ranks before
 the order-dependent scoring sweep (storeInverseMatches, line3D.cc:1672-1699) can run replicated.  The rows live in two
 device arrays with the layout of the FULL job (counts int32[rows], recs 24·knn B per row), so the exchange is one
-broadcast per owner over NCCL/NVLink, in place, no packing.  Nothing else is communicated.
+broadcast per owner over NCCL/NVLink, in place, no packing.  Nothing else is communicated.  Keep-all (kNN <= 0) and
+kNN > 32 exchange twice: the counts alone, which give every rank the same row stride, then the rows at that stride.
 """
 from __future__ import annotations
 
 import ctypes as C
+import time
 
 import numpy as np
 import torch
@@ -46,7 +48,8 @@ def balanced_split(cost, parts: int) -> np.ndarray:
 
 def exchange_rows(counts: torch.Tensor, recs: torch.Tensor, row_bounds, knn: int, group=None) -> None:
     """counts: uint8 view of int32[rows]; recs: uint8 view of rows*knn records.  Rank r owns rows
-    [row_bounds[r], row_bounds[r+1]); after the call every rank holds every row.  Works on CPU tensors (gloo) as well."""
+    [row_bounds[r], row_bounds[r+1]); after the call every rank holds every row.  knn = 0 (the first of the two calls of
+    keep-all and kNN > 32, include/line3d.h) moves only the counts.  Works on CPU tensors (gloo) as well."""
     world = dist.get_world_size(group)
     assert len(row_bounds) == world + 1
     for r in range(world):
@@ -55,7 +58,8 @@ def exchange_rows(counts: torch.Tensor, recs: torch.Tensor, row_bounds, knn: int
             continue
         src = dist.get_global_rank(group, r) if group is not None else r
         dist.broadcast(counts[4 * a:4 * b], src=src, group=group)
-        dist.broadcast(recs[REC_BYTES * knn * a:REC_BYTES * knn * b], src=src, group=group)
+        if knn > 0:
+            dist.broadcast(recs[REC_BYTES * knn * a:REC_BYTES * knn * b], src=src, group=group)
 
 
 _EXCHANGE_T = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_longlong), C.c_int, C.c_int)
@@ -63,9 +67,11 @@ _EXCHANGE_T = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER
 
 def attach(line3d, device: int, group=None):
     """Make `line3d` (line3dpp_b200.line3d.Line3D) a member of the process group: matching sharded, the rest replicated.
-    Returns the callback object, which the caller must keep alive as long as the Line3D is used."""
+    Returns the callback object, which the caller must keep alive as long as the Line3D is used.
+    line3d._exchange_state["exchanges"] gets one entry per callback (knn, ms, count_bytes, record_bytes: what every rank holds
+    after it); the caller may clear the list."""
     rank, world = dist.get_rank(group), dist.get_world_size(group)
-    state = {"error": None}
+    state = {"error": None, "exchanges": []}
 
     def _exchange(_user, counts_dev, recs_dev, row_bounds, w, knn):
         try:
@@ -74,11 +80,12 @@ def attach(line3d, device: int, group=None):
             counts = device_bytes(counts_dev, 4 * rows, device)
             recs = device_bytes(recs_dev, REC_BYTES * knn * rows, device)
             torch.cuda.synchronize(device)                     # the match kernel ran on the context's own stream
-            import time
             t0 = time.perf_counter()
             exchange_rows(counts, recs, rb, knn, group)
             torch.cuda.synchronize(device)
-            state["exchange_ms"] = (time.perf_counter() - t0) * 1e3     # includes waiting for the slowest rank's matching
+            ms = (time.perf_counter() - t0) * 1e3              # the first call includes waiting for the slowest rank's matching
+            state["exchange_ms"] = ms
+            state["exchanges"].append({"knn": knn, "ms": ms, "count_bytes": 4 * rows, "record_bytes": REC_BYTES * knn * rows})
             return 0
         except Exception as e:  # noqa: BLE001 — must not unwind through the C frame
             state["error"] = e
