@@ -13,12 +13,12 @@
 #include <cuda_runtime_api.h>          // cudaGetDevice: undistortImage runs on the caller's current device
 
 #include <algorithm>
+#include <cassert>
 #include <chrono>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <fstream>
-#include <iomanip>
 #include <iostream>
 #include <map>
 #include <mutex>
@@ -27,8 +27,6 @@
 #include <sstream>
 #include <stdexcept>
 #include <thread>
-#include <unordered_map>
-#include <unordered_set>
 #include <sys/stat.h>                  // mkdir: the segment cache's folder
 
 namespace L3DPP {
@@ -63,6 +61,8 @@ inline Matrix3d matmul(const Matrix3d& a, const Matrix3d& b)
 { Matrix3d r; for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) { double s = 0; for (int k = 0; k < 3; ++k) s += a(i, k) * b(k, j); r(i, j) = s; } return r; }
 inline Vector3d matvec(const Matrix3d& a, const Vector3d& v)
 { return Vector3d(a(0, 0) * v.x + a(0, 1) * v.y + a(0, 2) * v.z, a(1, 0) * v.x + a(1, 1) * v.y + a(1, 2) * v.z, a(2, 0) * v.x + a(2, 1) * v.y + a(2, 2) * v.z); }
+template <class T> T median_of(std::vector<T>& v, T if_empty)   // sorts v; the reference's median is the element at size / 2
+{ if (v.empty()) return if_empty; std::sort(v.begin(), v.end()); return v[v.size() / 2]; }
 inline Matrix3d transposed(const Matrix3d& a) { Matrix3d r; for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) r(i, j) = a(j, i); return r; }
 Matrix3d inverted(const Matrix3d& a)   // adjugate / determinant
 {
@@ -97,7 +97,7 @@ struct HostView {
     }
 };
 
-struct Edge { int i, j; float w; };   // CLEdge clustering.h:47-51
+struct Affinity { std::vector<int> i, j; std::vector<float> w; };   // the CLEdges (clustering.h:47-51) as l3d_affinity_matrix fills them
 
 // Felzenszwalb-Huttenlocher graph segmentation as used by the reference (clustering.cc:6-48, universe.h:49-104):
 // edges visited by ascending weight (stable), components merge while w <= both thresholds, threshold = w + c/|C|.
@@ -117,25 +117,25 @@ private:
     std::vector<int> parent_, rank_, size_;
 };
 
-// `order` (optional): indices of `edges` by ascending weight, ties in list order (from l3d_argsort_f32 for big lists)
-std::vector<int> segment_graph(const std::vector<Edge>& edges, int n, float c, const std::vector<unsigned int>* order)
+// `order` (optional): indices of the edges by ascending weight, ties in list order (from l3d_argsort_f32 for big lists)
+std::vector<int> segment_graph(const Affinity& A, int n, float c, const std::vector<unsigned int>* order)
 {
     std::vector<unsigned int> local;
     if (!order) {
-        local.resize(edges.size());
+        local.resize(A.w.size());
         for (size_t i = 0; i < local.size(); ++i) local[i] = (unsigned int)i;
-        std::stable_sort(local.begin(), local.end(), [&](unsigned int a, unsigned int b) { return edges[a].w < edges[b].w; });
+        std::stable_sort(local.begin(), local.end(), [&](unsigned int a, unsigned int b) { return A.w[a] < A.w[b]; });
         order = &local;
     }
     DisjointSets u(n);
     std::vector<float> thr(n, c);
     for (unsigned int idx : *order) {
-        const Edge& e = edges[idx];
-        int a = u.find(e.i), b = u.find(e.j);
-        if (a == b || !(e.w <= thr[a] && e.w <= thr[b])) continue;
+        const float w = A.w[idx];
+        int a = u.find(A.i[idx]), b = u.find(A.j[idx]);
+        if (a == b || !(w <= thr[a] && w <= thr[b])) continue;
         u.unite(a, b);
         a = u.find(a);
-        thr[a] = e.w + c / (float)u.size(a);
+        thr[a] = w + c / (float)u.size(a);
     }
     std::vector<int> label(n);
     for (int i = 0; i < n; ++i) label[i] = u.find(i);
@@ -215,15 +215,15 @@ struct Line3D::Impl {
     // index maps (rebuilt at matchImages)
     std::vector<HostView*> vlist;                         // by view index (ascending camID)
     std::map<unsigned int, int> index_of;
-    std::vector<int32_t> pairs;                           // (src idx, tgt idx) in match order
+    std::vector<int32_t> pairs; std::vector<float> F; std::vector<double> F_d;   // (src idx, tgt idx) in match order, 9 entries of F per pair
     // results
-    std::vector<l3d_match> est_best; std::vector<double> est_P; std::vector<long long> est_gseg;
-    std::unordered_map<long long, size_t> est_of_gseg;
-    std::vector<Edge> A, A_raw; std::vector<long long> local2global;
+    std::vector<l3d_match> est_best; std::vector<double> est_P; std::vector<int> est_index;   // est_index: est_best's entry by global segment, or -1
+    Affinity A, A_raw; std::vector<long long> local2global;
     std::vector<FinalLine3D> lines3D;
     Line3DStats st;
 
     void fail(const std::string& what) { err = what; if (verbose) std::cerr << "[L3D++] ERROR: " << what << std::endl; }
+    bool reject(unsigned int camID, const std::string& what) { fail("addImage [" + std::to_string(camID) + "]: " + what); return false; }
     bool chk(long long rc, const char* what) { if (rc < 0) { fail(std::string(what) + ": " + l3d_last_error(ctx)); return false; } return true; }
     void log(const std::string& s) { if (verbose) std::cout << "[L3D++] " << s << std::endl; }
 
@@ -235,26 +235,29 @@ struct Line3D::Impl {
             L.underlyingCluster_.translate(d);
         }
     }
-    void translate()                                      // line3D.cc:500-536
-    {
-        if (views.empty()) return;
-        double tr[3] = {0, 0, 0};
-        for (int a = 0; a < 3; ++a) {
-            std::vector<double> c;
-            for (auto& kv : views) { const double v = a == 0 ? kv.second.C.x : (a == 1 ? kv.second.C.y : kv.second.C.z); if (std::fabs(v) > EPS) c.push_back(v); }
-            if (!c.empty()) { std::sort(c.begin(), c.end()); tr[a] = c[c.size() / 2]; }
+    struct Translated {                                   // translate (line3D.cc:500-536) for one scope, untranslate (539-545) at its end:
+        Impl& P;                                          // the 3D lines made meanwhile move back with the views
+        explicit Translated(Impl& p) : P(p)
+        {
+            if (P.views.empty()) return;
+            double tr[3] = {0, 0, 0};
+            for (int a = 0; a < 3; ++a) {
+                std::vector<double> c;
+                for (auto& kv : P.views) { const double v = a == 0 ? kv.second.C.x : (a == 1 ? kv.second.C.y : kv.second.C.z); if (std::fabs(v) > EPS) c.push_back(v); }
+                tr[a] = median_of(c, 0.0);
+            }
+            P.translation = Vector3d(tr[0], tr[1], tr[2]);
+            P.shift_all(P.translation * -1.0);
         }
-        translation = Vector3d(tr[0], tr[1], tr[2]);
-        shift_all(translation * -1.0);
-    }
-    void untranslate() { shift_all(translation); }        // line3D.cc:539-545
+        ~Translated() { P.shift_all(P.translation); }
+    };
 
     float spatial_reg(const HostView& v, float r) const   // View::getSpecificSpatialReg view.cc:307-314
     {
         const Vector3d a = v.ray(v.pp.x, v.pp.y), b = v.ray(v.pp.x + r, v.pp.y);
         return (float)std::sin(std::acos(std::fmin(std::fmax(dot(a, b), -1.0), 1.0)));
     }
-    void neighbors_from_wps(unsigned int camID);
+    void find_visual_neighbors(unsigned int camID);
     Matrix3d fundamental(const HostView& s, const HostView& t) const   // getFundamentalMatrix line3D.cc:874-892
     {
         const Matrix3d R = matmul(t.R, transposed(s.R));
@@ -262,11 +265,12 @@ struct Line3D::Impl {
         Matrix3d T; T(0, 0) = 0; T(0, 1) = -tt.z; T(0, 2) = tt.y; T(1, 0) = tt.z; T(1, 1) = 0; T(1, 2) = -tt.x; T(2, 0) = -tt.y; T(2, 1) = tt.x; T(2, 2) = 0;
         return matmul(matmul(inverted(transposed(t.K)), matmul(T, R)), inverted(s.K));
     }
-    std::vector<l3d_view_desc> descs() const
+    std::vector<l3d_view_desc> descs(std::vector<const float*>* segp = nullptr) const   // segp: each view's segments, for l3d_set_views
     {
         std::vector<l3d_view_desc> d(vlist.size());
         for (size_t i = 0; i < vlist.size(); ++i) {
             const HostView& v = *vlist[i];
+            if (segp) segp->push_back(&v.lines[0].v[0]);
             d[i].cam_id = v.id; d[i].width = v.width; d[i].height = v.height; d[i].nseg = (int32_t)v.lines.size();
             memcpy(d[i].RtKinv, v.RtKinv_f, sizeof(v.RtKinv_f)); memcpy(d[i].C, v.C_f3, sizeof(v.C_f3));
             memcpy(d[i].RtKinv_d, v.RtKinv.m, sizeof(v.RtKinv.m));
@@ -283,8 +287,8 @@ struct Line3D::Impl {
     }
     const Segment3D estimate(const Segment2D& s) const
     {
-        const HostView* v = vlist[index_of.at(s.camID())];
-        const size_t e = est_of_gseg.at(v->seg_off + s.segID());
+        const int e = est_index[vlist[index_of.at(s.camID())]->seg_off + s.segID()];
+        assert(e >= 0);                                   // cluster members come from the affinity matrix: all have an estimate
         return Segment3D(Vector3d(est_P[6 * e], est_P[6 * e + 1], est_P[6 * e + 2]), Vector3d(est_P[6 * e + 3], est_P[6 * e + 4], est_P[6 * e + 5]));
     }
     bool segments_from_image(unsigned int camID, const Image8u& image, Line3D::SegmentDetectorFn fn, void* user, std::vector<Vec4f>& segs,
@@ -292,14 +296,282 @@ struct Line3D::Impl {
     bool line_from_cluster(const std::list<Segment2D>& cluster, LineCluster3D& out) const;
     Segment3D project_onto_line(const Segment2D& s2, const Segment3D& s3, bool& ok) const;
     std::list<Segment3D> collinear_segments(const LineCluster3D& cl) const;
+    // addImage's checks under mtx.  Image overload (no_segments null): size, camera ID in views or reservations, world points (line3D.cc:116-155).
+    // Segments overload: size, world points, segments (no_segments: why none), then the ID in views only (the image overload calls it reserved).
+    bool check_view(unsigned int camID, int w, int h, const std::list<unsigned int>& wps_or_neighbors, const std::string* no_segments)
+    {
+        const bool in_use = views.count(camID) || (!no_segments && reserved.count(camID));
+        const bool rest_ok = !wps_or_neighbors.empty() && (!no_segments || no_segments->empty());
+        if (std::max(w, h) < 800) return reject(camID, "image is too small for reliable results (larger side should be >= 800px)");
+        if (in_use && (!no_segments || rest_ok)) return reject(camID, "camera ID already in use");
+        if (wps_or_neighbors.empty()) return reject(camID, by_wps ? "view has no worldpoints" : "view has no visual neighbors");
+        return rest_ok || reject(camID, *no_segments);
+    }
+    // the view's segment cache, used as stored (detectLineSegments line3D.cc:295-309): true if it was read, with `why` set if the view
+    // cannot use what it holds; false with `why` saying why it was not read.  Reads only what is fixed at construction: needs no lock.
+    bool read_segment_cache(unsigned int camID, int w, int h, std::vector<Vec4f>& segs, std::string& why) const
+    {
+        const std::string path = segmentCachePath(output_folder, camID, w, h, max_img_width);
+        if (!load_segments) { why = "no line segments given, and load_segments is off so the segment cache " + path + " was not read"; return false; }
+        if (!std::ifstream(path.c_str(), std::ios::binary)) { why = "no line segments given and no segment cache " + path + " (line detection is outside this library)"; return false; }
+        std::string e;
+        if (!readSegmentCache(path, segs, &e)) why = "unreadable segment cache " + e;
+        else if (segs.empty()) why = "the segment cache " + path + " holds no segments";
+        return true;
+    }
+    void index_views()                                    // vlist, index_of and every view's global index of its segment 0
+    {
+        vlist.clear(); index_of.clear();
+        long long off = 0;
+        for (auto& kv : views) {
+            HostView& v = kv.second;
+            v.seg_off = off; off += (long long)v.lines.size();
+            index_of[v.id] = (int)vlist.size(); vlist.push_back(&v);
+        }
+    }
+    // the view pairs in the reference's order (computeMatches line3D.cc:704-741), F in float and double (861-897, 2775-2781)
+    void list_pairs()
+    {
+        pairs.clear(); F.clear(); F_d.clear();
+        std::set<std::pair<unsigned int, unsigned int> > done;
+        for (auto& kv : visual_neighbors)
+            for (unsigned int n : kv.second) {
+                const unsigned int s = kv.first;
+                if (n == s || !done.insert(std::make_pair(std::min(s, n), std::max(s, n))).second) continue;
+                pairs.push_back(index_of[s]); pairs.push_back(index_of[n]);
+                const Matrix3d Fd = fundamental(views[s], views[n]);
+                for (int i = 0; i < 9; ++i) { F.push_back((float)Fd.m[i]); F_d.push_back(Fd.m[i]); }
+            }
+    }
+    // the pairs [first, last) in `parts` contiguous shares balanced by Ns*Nt: share p is [bounds[p], bounds[p + 1])
+    bool split_pairs(int first, int last, int parts, std::vector<int32_t>& bounds)
+    {
+        std::vector<long long> cost((size_t)(last - first));
+        for (int i = first; i < last; ++i) cost[i - first] = (long long)vlist[pairs[2 * i]]->lines.size() * (long long)vlist[pairs[2 * i + 1]]->lines.size();
+        bounds.resize((size_t)parts + 1);
+        if (!chk(l3d_balanced_split(cost.data(), last - first, parts, bounds.data()), "l3d_balanced_split")) return false;
+        for (int32_t& b : bounds) b += first;
+        return true;
+    }
+    // the upload, this rank's share of the pairs (all without setShard) matched on this Line3D's devices, the exchange with the others
+    bool match(const std::vector<l3d_view_desc>& d, const std::vector<const float*>& segp, float& ms_gather)
+    {
+        if (!chk(l3d_set_views(ctx, (int)d.size(), d.data(), segp.data()), "l3d_set_views")) return false;
+        const int npairs = (int)(pairs.size() / 2);
+        if (shard_world == 1) return match_on_devices(0, npairs, d, segp, ms_gather) && chk(l3d_sync(ctx), "l3d_sync");
+        std::vector<int32_t> bounds;
+        return split_pairs(0, npairs, shard_world, bounds) && match_on_devices(bounds[shard_rank], bounds[shard_rank + 1], d, segp, ms_gather) &&
+               chk(l3d_sync(ctx), "l3d_sync") && exchange_matches(bounds);
+    }
+    // The pairs [first, last) on the primary, or every device's share (split_pairs) uploaded and matched from its own host thread (keep-all
+    // waits on the host between its count and store passes, so one thread would serialise the devices), then gathered on the primary's
+    // stream.  The threads share no mutable host state: each works on its own context and writes only its own error slot.
+    bool match_on_devices(int first, int last, const std::vector<l3d_view_desc>& d, const std::vector<const float*>& segp, float& ms_gather)
+    {
+        // use_GPU selects the reference's semantics, not the processor (line3D.cc:708-757): true = K_match_lines / K_score_matches
+        // float arithmetic, false = matchingCPU / scoringCPU double arithmetic.  Both run on the GPU.
+        const char* match_what = use_gpu ? "l3d_match_pairs_range" : "l3d_match_pairs_f64";
+        const int npairs = (int)(pairs.size() / 2);
+        auto match_on = [&](l3d_ctx* c, int f, int l) {
+            return use_gpu ? l3d_match_pairs_range(c, npairs, pairs.data(), F.data(), epi, kNN, f, l)
+                           : l3d_match_pairs_f64(c, npairs, pairs.data(), F_d.data(), epi, kNN, f, l);
+        };
+        if (ctxs.size() == 1) return chk(match_on(ctx, first, last), match_what);
+        const int nd = (int)ctxs.size();
+        std::vector<int32_t> b;
+        if (!split_pairs(first, last, nd, b)) return false;
+        std::vector<std::string> errs((size_t)nd);
+        auto run = [&](int i) {
+            l3d_ctx* c = ctxs[i];
+            const char* what = "l3d_set_views";
+            long long rc = i == 0 ? 0 : l3d_set_views(c, (int)d.size(), d.data(), segp.data());     // the primary has its views already
+            if (rc >= 0) { what = match_what; rc = match_on(c, b[i], b[i + 1]); }
+            if (rc >= 0) { what = "l3d_sync"; rc = l3d_sync(c); }
+            if (rc < 0) errs[i] = "device " + std::to_string(devices[i]) + " (#" + std::to_string(i) + "): " + what + ": " + l3d_last_error(c);
+        };
+        std::vector<std::thread> th;
+        for (int i = 1; i < nd; ++i) th.emplace_back(run, i);
+        run(0);
+        for (std::thread& x : th) x.join();
+        for (const std::string& e : errs)
+            if (!e.empty()) { fail(e); return false; }
+        cudaSetDevice(devices[0]);
+        cudaStream_t s = (cudaStream_t)l3d_stream(ctx);
+        cudaEvent_t e0 = nullptr, e1 = nullptr;
+        const bool timed = cudaEventCreate(&e0) == cudaSuccess && cudaEventCreate(&e1) == cudaSuccess && cudaEventRecord(e0, s) == cudaSuccess;
+        bool ok = chk(l3d_match_gather(ctx, nd, ctxs.data(), b.data()), "l3d_match_gather");
+        cudaSetDevice(devices[0]);
+        ok = ok && (!timed || cudaEventRecord(e1, s) == cudaSuccess) && chk(l3d_sync(ctx), "l3d_sync");
+        if (ok && timed) cudaEventElapsedTime(&ms_gather, e0, e1);
+        if (e0) cudaEventDestroy(e0);
+        if (e1) cudaEventDestroy(e1);
+        return ok;
+    }
+    bool exchange_matches(const std::vector<int32_t>& bounds)   // every rank's rows of the match buffers to every rank; bounds: the ranks' shares
+    {
+        std::vector<long long> row_off(pairs.size() / 2 + 1), row_bounds((size_t)shard_world + 1);
+        void *dc = nullptr, *dr = nullptr;
+        if (!chk(l3d_pair_row_offsets(ctx, row_off.data()), "l3d_pair_row_offsets") || !chk(l3d_match_device_buffers(ctx, &dc, &dr), "l3d_match_device_buffers")) return false;
+        for (int r = 0; r <= shard_world; ++r) row_bounds[r] = row_off[bounds[r]];
+        auto send = [&](int knn, const char* what) {
+            if (exchange(exchange_user, dc, dr, row_bounds.data(), shard_world, knn) == 0) return true;
+            fail(std::string("matchImages: the match exchange callback failed") + what);
+            return false;
+        };
+        if (kNN >= 1 && kNN <= 32) return send(kNN, "");
+        // Keep-all and kNN > 32: every rank laid out its records at the longest row of its own share.  Once the counts are exchanged,
+        // every rank reduces the same counts to the same stride and re-lays its rows at it; then the records move.
+        int stride = 0;
+        return send(0, " (row counts)") && chk(stride = l3d_match_restride(ctx, 0), "l3d_match_restride") &&
+               chk(l3d_match_device_buffers(ctx, &dc, &dr), "l3d_match_device_buffers") && send(stride, " (records)");
+    }
+    // every segment's best estimate, then filterMatches' tail (line3D.cc:1657-1668): every view's median depth of them
+    bool download_estimates()
+    {
+        const long long ne = l3d_get_estimates(ctx, nullptr, nullptr, 0);
+        if (!chk(ne, "l3d_get_estimates")) return false;
+        est_best.resize(ne); est_P.resize(6 * (size_t)ne);
+        if (ne && !chk(l3d_get_estimates(ctx, est_best.data(), est_P.data(), ne), "l3d_get_estimates")) return false;
+        std::map<unsigned int, std::vector<float> > depths;
+        est_index.assign((size_t)(vlist.back()->seg_off + (long long)vlist.back()->lines.size()), -1);
+        for (size_t e = 0; e < est_best.size(); ++e) {
+            const l3d_match& m = est_best[e];
+            depths[m.src_cam].push_back(m.d_p1); depths[m.src_cam].push_back(m.d_p2);
+            est_index[views[m.src_cam].seg_off + m.src_seg] = (int)e;
+        }
+        for (auto& kv : views) {
+            kv.second.median_depth = median_of(depths[kv.first], (float)EPS);          // update_median_depth view.h:108-121
+            if (fixed3Dreg) kv.second.k = sigma_p / med_scene_depth;
+        }
+        return true;
+    }
+    // findCollinearSegments and computingAffinityMatrix (line3D.cc:1751-1756, 1827-1979) on the device; collin_t <= eps: no collinearity
+    bool affinity_matrix(const std::vector<l3d_view_desc>& d)
+    {
+        bool ok = chk(l3d_update_view_params(ctx, (int)d.size(), d.data()), "l3d_update_view_params") &&
+                  chk(l3d_find_collinear(ctx, collin_t > EPS ? collin_t : 0.0f, use_gpu ? L3D_SEM_REF_GPU : L3D_SEM_REF_CPU), "l3d_find_collinear");
+        st.collinear_entries = ok ? l3d_collinear_total(ctx) : 0;
+        long long nids = 0;
+        const long long nA = ok ? l3d_affinity_matrix(ctx, two_sigA_sqr, med_scene_depth_lines, MIN_AFFINITY, nullptr, nullptr, nullptr, 0, nullptr, 0, &nids) : -1;
+        ok = ok && chk(nA, "l3d_affinity_matrix");
+        A = Affinity(); local2global.clear();
+        if (ok && nA > 0) {
+            A.i.resize((size_t)nA); A.j.resize((size_t)nA); A.w.resize((size_t)nA); local2global.resize((size_t)nids);
+            ok = chk(l3d_affinity_matrix(ctx, two_sigA_sqr, med_scene_depth_lines, MIN_AFFINITY, A.i.data(), A.j.data(), A.w.data(), nA,
+                                         local2global.data(), nids, &nids), "l3d_affinity_matrix");
+        }
+        if (!ok) return false;
+        A_raw = A;
+        st.affinity_entries = (long long)A.w.size(); st.affinity_rows = (long long)local2global.size();
+        return true;
+    }
+    // performRDD (line3D.cc:2026-2076) on the device; one download in the (i, j) order the reference's std::map rebuilds A_ in (2039-2071)
+    bool diffuse()
+    {
+        Affinity D{std::vector<int>(A.w.size()), std::vector<int>(A.w.size()), std::vector<float>(A.w.size())};
+        if (!chk(l3d_rdd_affinity(ctx, RDD_MAX_ITER, D.i.data(), D.j.data(), D.w.data(), (long long)D.w.size()), "l3d_rdd_affinity")) return false;
+        A = std::move(D);
+        return true;
+    }
+    bool cluster_segments(std::vector<LineCluster3D>& clusters)   // clusterSegments line3D.cc:2079-2152
+    {
+        st.clusters_total = 0;
+        const int n = (int)local2global.size();           // 0 without edges: then there is nothing to cluster
+        std::vector<unsigned int> worder;
+        if (A.w.size() > (1u << 20)) {          // big list: sort the weights on the device (stable, like std::list::sort)
+            worder.resize(A.w.size());
+            if (!chk(l3d_argsort_f32(ctx, (long long)A.w.size(), A.w.data(), worder.data()), "l3d_argsort_f32")) return false;
+        }
+        const std::vector<int> label = segment_graph(A, n, 3.0f, worder.empty() ? nullptr : &worder);
+        std::map<int, std::list<Segment2D> > members; std::map<int, std::set<unsigned int> > cams; std::vector<int> order;
+        for (int id = 0; id < n; ++id) {
+            const int cl = label[id];
+            if (!members.count(cl)) order.push_back(cl);
+            const Segment2D s = seg_of(local2global[id]);
+            members[cl].push_back(s); cams[cl].insert(s.camID());
+        }
+        st.clusters_total = (long long)order.size();
+        std::vector<const std::list<Segment2D>*> todo;
+        for (int cl : order) if (cams[cl].size() >= visibility_t) todo.push_back(&members[cl]);
+        std::vector<LineCluster3D> fitted(todo.size()); std::vector<unsigned char> good(todo.size(), 0);
+        parallel_for(todo.size(), [&](size_t i) { good[i] = line_from_cluster(*todo[i], fitted[i]) ? 1 : 0; });
+        for (size_t i = 0; i < todo.size(); ++i) if (good[i]) clusters.push_back(fitted[i]);
+        st.clusters_valid = (long long)clusters.size();
+        return true;
+    }
+    // optimizeClusters (line3D.cc:1800-1805, 2269-2275): bundle the cluster lines against their 2D residuals and drop the invalid ones.
+    // The reference needs Ceres for this (optimization.cc); here the same problem is minimised on the GPU (l3d_optimize_lines).
+    bool optimize_clusters(std::vector<LineCluster3D>& clusters, bool use_CERES, unsigned int max_iter)
+    {
+        st.opt_iterations = 0; st.opt_cost_before = st.opt_cost_after = 0.0;
+        if (!use_CERES || clusters.empty()) return true;
+        const int Lc = (int)clusters.size(), nc = (int)vlist.size();
+        std::vector<double> p((size_t)6 * Lc), cams((size_t)16 * nc), xy;
+        std::vector<long long> ptr((size_t)Lc + 1, 0);
+        std::vector<int> rcam;
+        for (int v = 0; v < nc; ++v) {
+            const HostView& hv = *vlist[v];
+            double* cm = &cams[(size_t)16 * v];
+            for (int r = 0; r < 3; ++r) for (int c2 = 0; c2 < 3; ++c2) cm[3 * r + c2] = hv.R(r, c2);
+            cm[9] = hv.C.x; cm[10] = hv.C.y; cm[11] = hv.C.z;
+            cm[12] = hv.K(0, 0); cm[13] = hv.K(1, 1); cm[14] = hv.K(0, 2); cm[15] = hv.K(1, 2);
+        }
+        for (int i = 0; i < Lc; ++i) {
+            const Segment3D s3 = clusters[i].seg3D();
+            p[6 * i] = s3.P1().x; p[6 * i + 1] = s3.P1().y; p[6 * i + 2] = s3.P1().z; p[6 * i + 3] = s3.P2().x; p[6 * i + 4] = s3.P2().y; p[6 * i + 5] = s3.P2().z;
+            for (const Segment2D& s2 : *clusters[i].residuals()) {
+                const int vi = index_of.at(s2.camID());
+                const Vec4f& ln = vlist[vi]->lines[s2.segID()];
+                rcam.push_back(vi);
+                for (int k = 0; k < 4; ++k) xy.push_back((double)ln.v[k]);
+            }
+            ptr[i + 1] = (long long)rcam.size();
+        }
+        std::vector<int> valid((size_t)Lc);
+        double summ[8];
+        if (!chk(l3d_optimize_lines(ctx, Lc, p.data(), ptr.data(), rcam.data(), xy.data(), nc, cams.data(), (int)max_iter, p.data(), valid.data(), summ),
+                 "l3d_optimize_lines")) return false;
+        std::vector<LineCluster3D> kept;
+        for (int i = 0; i < Lc; ++i) {
+            if (!valid[i]) continue;                        // optimization.cc:293-298
+            clusters[i].update3Dline(Segment3D(Vector3d(p[6 * i], p[6 * i + 1], p[6 * i + 2]), Vector3d(p[6 * i + 3], p[6 * i + 4], p[6 * i + 5])));
+            kept.push_back(clusters[i]);
+        }
+        clusters.swap(kept);
+        st.opt_iterations = (long long)summ[0]; st.opt_cost_before = summ[1]; st.opt_cost_after = summ[2];
+        return true;
+    }
+    void final_segments(const std::vector<LineCluster3D>& clusters)   // computeFinal3Dsegments + filterTinySegments (line3D.cc:2278-2339)
+    {
+        std::vector<std::list<Segment3D> > kept_segs(clusters.size());
+        parallel_for(clusters.size(), [&](size_t i) {
+            const LineCluster3D& cl = clusters[i];
+            std::list<Segment3D> col = collinear_segments(cl);
+            if (col.empty()) return;
+            const HostView& rv = *vlist[index_of.at(cl.reference_view())];
+            for (const Segment3D& s : col) {
+                double u1, v1, u2, v2; rv.project(s.P1(), u1, v1); rv.project(s.P2(), u2, v2);
+                if (std::sqrt((u1 - u2) * (u1 - u2) + (v1 - v2) * (v1 - v2)) > rv.min_line_length) kept_segs[i].push_back(s);  // projectedLongEnough view.cc:423-428
+            }
+        });
+        for (size_t i = 0; i < clusters.size(); ++i) {
+            if (kept_segs[i].empty()) continue;
+            FinalLine3D f; f.collinear3Dsegments_ = kept_segs[i]; f.underlyingCluster_ = clusters[i];
+            lines3D.push_back(f);
+        }
+    }
 };
 
-// findVisualNeighborsFromWPs (line3D.cc:578-699)
-void Line3D::Impl::neighbors_from_wps(unsigned int camID)
+// visual neighbours (line3D.cc:463-485): the given ones that were added, or findVisualNeighborsFromWPs (578-699)
+void Line3D::Impl::find_visual_neighbors(unsigned int camID)
 {
     std::set<unsigned int>& out = visual_neighbors[camID];
-    out.clear();
     HostView& v = views[camID];
+    if (!by_wps) {
+        if (out.empty()) for (unsigned int n : v.wps_or_neighbors) if (views.count(n)) out.insert(n);
+        return;
+    }
+    out.clear();
     std::map<unsigned int, unsigned int> common;
     for (unsigned int wp : v.wps_or_neighbors)
         for (unsigned int other : wps2views[wp]) if (other != camID) ++common[other];
@@ -385,17 +657,8 @@ bool Line3D::addImage(const unsigned int camID, const int w, const int h, const 
     // everything that needs no shared state first (the reference's frontends call addImage from an OpenMP loop) ...
     HostView v;
     v.id = camID; v.width = w; v.height = h; v.K = K; v.R = R; v.t = t; v.lines = line_segments; v.wps_or_neighbors = wps_or_neighbors;
-    // no segments given: the reference's segment cache, used as stored (detectLineSegments line3D.cc:295-309).  output_folder,
-    // load_segments and max_img_width are fixed at construction, so this needs no lock either.
     std::string no_segments;
-    if (line_segments.empty()) {
-        const std::string path = segmentCachePath(P.output_folder, camID, w, h, P.max_img_width);
-        std::string e;
-        if (!P.load_segments) no_segments = "no line segments given, and load_segments is off so the segment cache " + path + " was not read";
-        else if (!std::ifstream(path.c_str(), std::ios::binary)) no_segments = "no line segments given and no segment cache " + path + " (line detection is outside this library)";
-        else if (!readSegmentCache(path, v.lines, &e)) no_segments = "unreadable segment cache " + e;
-        else if (v.lines.empty()) no_segments = "the segment cache " + path + " holds no segments";
-    }
+    if (line_segments.empty()) P.read_segment_cache(camID, w, h, v.lines, no_segments);
     v.min_line_length = std::sqrt(float((unsigned)w * (unsigned)w + (unsigned)h * (unsigned)h)) * 0.005f;                           // view.cc:17-18
     v.pp = Vector3d(K(0, 2), K(1, 2), 1.0);
     const Matrix3d Rt = transposed(R);
@@ -406,11 +669,7 @@ bool Line3D::addImage(const unsigned int camID, const int w, const int h, const 
     // ... then one critical section for the checks, the insertion and the error string.  A failure is reported through the return
     // value AND stays in lastError() (a later successful addImage does not clear it) until the next non-addImage call.
     std::lock_guard<std::mutex> g(P.mtx);
-    auto failed = [&](const std::string& what) { P.fail("addImage [" + std::to_string(camID) + "]: " + what); return false; };
-    if (std::max(w, h) < 800) return failed("image is too small for reliable results (larger side should be >= 800px)");   // line3D.cc:119
-    if (wps_or_neighbors.empty()) return failed(P.by_wps ? "view has no worldpoints" : "view has no visual neighbors");    // line3D.cc:154
-    if (v.lines.empty()) return failed(no_segments);
-    if (P.views.count(camID)) return failed("camera ID already in use");                                                     // line3D.cc:130
+    if (!P.check_view(camID, w, h, wps_or_neighbors, &no_segments)) return false;
     if (P.by_wps) for (unsigned int wp : wps_or_neighbors) P.wps2views[wp].push_back(camID);
     P.views[camID] = v;
     P.visual_neighbors[camID];
@@ -455,18 +714,8 @@ bool Line3D::Impl::segments_from_image(unsigned int camID, const Image8u& image,
         why = "image type not supported: " + std::to_string(image.channels) + " channels (8-bit grey or RGB images only)";
         return false;
     }
-    const std::string path = segmentCachePath(output_folder, camID, w, h, max_img_width);
-    if (load_segments && std::ifstream(path.c_str(), std::ios::binary)) {                                 // line3D.cc:295-309
-        std::string e;
-        if (!readSegmentCache(path, segs, &e)) { why = "unreadable segment cache " + e; return false; }
-        if (segs.empty()) { why = "the segment cache " + path + " holds no segments"; return false; }
-        return true;
-    }
-    if (!fn) {
-        why = load_segments ? "no line segments given and no segment cache " + path + " (line detection is outside this library)"
-                            : "no line segments given, and load_segments is off so the segment cache " + path + " was not read";
-        return false;
-    }
+    if (read_segment_cache(camID, w, h, segs, why)) return why.empty();        // a cache that exists decides, usable or not
+    if (!fn) return false;
     if (image.data.size() != (size_t)w * h * image.channels) { why = "the pixel buffer does not match rows x cols x channels"; return false; }
     int w_p, h_p;
     preparedImageSize(w, h, max_img_width, w_p, h_p);
@@ -492,7 +741,7 @@ bool Line3D::Impl::segments_from_image(unsigned int camID, const Image8u& image,
     if (load_segments) {                                                                                  // line3D.cc:363-366
         std::string e;
         mkdir((output_folder + "/L3D++_data").c_str(), 0777);     // the reference's constructor creates it (line3D.cc:59-61)
-        if (!writeSegmentCache(path, segs, &e)) log("WARNING: segment cache not written: " + e);
+        if (!writeSegmentCache(segmentCachePath(output_folder, camID, w, h, max_img_width), segs, &e)) log("WARNING: segment cache not written: " + e);
     }
     return true;
 }
@@ -503,16 +752,12 @@ bool Line3D::addImage(const unsigned int camID, const Image8u& image, const Matr
     Impl& P = *p_;
     const int w = image.cols, h = image.rows;
     if (!line_segments.empty()) return addImage(camID, w, h, K, R, t, median_depth, wps_or_neighbors, line_segments);
-    // line3D.cc:116-155: the size, the camera ID (reserved until the view is added or rejected) and the world points, before any
-    // image work
+    // the checks before any image work; the camera ID stays reserved until the view is added or rejected
     Line3D::SegmentDetectorFn fn;
     void* user;
     {
         std::lock_guard<std::mutex> g(P.mtx);
-        auto failed = [&](const std::string& what) { P.fail("addImage [" + std::to_string(camID) + "]: " + what); return false; };
-        if (std::max(w, h) < 800) return failed("image is too small for reliable results (larger side should be >= 800px)");
-        if (P.views.count(camID) || P.reserved.count(camID)) return failed("camera ID already in use");
-        if (wps_or_neighbors.empty()) return failed(P.by_wps ? "view has no worldpoints" : "view has no visual neighbors");
+        if (!P.check_view(camID, w, h, wps_or_neighbors, nullptr)) return false;
         P.reserved.insert(camID);
         fn = P.detector; user = P.detector_user;
     }
@@ -524,8 +769,7 @@ bool Line3D::addImage(const unsigned int camID, const Image8u& image, const Matr
     std::string why;
     if (!P.segments_from_image(camID, image, fn, user, segs, why)) {
         std::lock_guard<std::mutex> g(P.mtx);
-        P.fail("addImage [" + std::to_string(camID) + "]: " + why);
-        return false;
+        return P.reject(camID, why);
     }
     return addImage(camID, w, h, K, R, t, median_depth, wps_or_neighbors, segs);
 }
@@ -552,162 +796,31 @@ void Line3D::matchImages(const float sigma_position, const float sigma_angle, co
     P.epi = std::fmin(std::fabs(epipolar_overlap), 0.99f); P.kNN = kNN; P.const_reg_depth = const_regularization_depth;
     if (P.sigma_p < 0.0f) { P.fixed3Dreg = true; P.sigma_p = std::fabs(P.sigma_p); } else { P.fixed3Dreg = false; P.sigma_p = std::fmax(0.1f, P.sigma_p); }
     P.med_scene_depth = const_regularization_depth;
-    if (const_regularization_depth < 0.0f && P.fixed3Dreg && !P.views_avg_depths.empty()) {
-        std::sort(P.views_avg_depths.begin(), P.views_avg_depths.end());
-        P.med_scene_depth = P.views_avg_depths[P.views_avg_depths.size() / 2];
-    }
-    P.matched = false; P.est_best.clear(); P.est_P.clear(); P.est_gseg.clear(); P.est_of_gseg.clear();
-    P.translate();
-    P.vlist.clear(); P.index_of.clear();
-    long long off = 0;
-    for (auto& kv : P.views) {
-        HostView& v = kv.second;
-        v.k = P.fixed3Dreg ? P.sigma_p / P.med_scene_depth : P.spatial_reg(v, P.sigma_p);
-        v.seg_off = off; off += (long long)v.lines.size();
-        P.index_of[v.id] = (int)P.vlist.size(); P.vlist.push_back(&v);
-    }
-    // visual neighbours (line3D.cc:463-485)
-    for (auto& kv : P.views) {
-        if (!P.by_wps) {
-            std::set<unsigned int>& vn = P.visual_neighbors[kv.first];
-            if (vn.empty()) for (unsigned int n : kv.second.wps_or_neighbors) if (P.views.count(n)) vn.insert(n);
-        } else P.neighbors_from_wps(kv.first);
-    }
-    // view pairs in the reference's order (computeMatches line3D.cc:704-741) + float fundamental matrices
-    P.pairs.clear();
-    std::vector<float> F; std::vector<double> Fdbl;
-    std::set<std::pair<unsigned int, unsigned int> > done;
-    for (auto& kv : P.visual_neighbors)
-        for (unsigned int n : kv.second) {
-            const unsigned int s = kv.first;
-            if (n == s || done.count(std::make_pair(std::min(s, n), std::max(s, n)))) continue;
-            done.insert(std::make_pair(std::min(s, n), std::max(s, n)));
-            P.pairs.push_back(P.index_of[s]); P.pairs.push_back(P.index_of[n]);
-            const Matrix3d Fd = P.fundamental(P.views[s], P.views[n]);
-            for (int i = 0; i < 9; ++i) { F.push_back((float)Fd.m[i]); Fdbl.push_back(Fd.m[i]); }   // eigen2dataArray line3D.cc:2775-2781
-        }
-    const int npairs = (int)(P.pairs.size() / 2);
-    // ---- device: upload, match all pairs, scoring sweep
-    std::vector<l3d_view_desc> d = P.descs();
-    std::vector<const float*> segp(P.vlist.size());
-    for (size_t i = 0; i < P.vlist.size(); ++i) segp[i] = &P.vlist[i]->lines[0].v[0];
-    auto t0 = std::chrono::steady_clock::now();
-    nvtxRangePushA("l3d:set_views+match");
-    bool ok = P.chk(l3d_set_views(P.ctx, (int)d.size(), d.data(), segp.data()), "l3d_set_views");
-    // use_GPU selects the reference's semantics, not the processor (line3D.cc:708-757): true = K_match_lines / K_score_matches
-    // float arithmetic, false = matchingCPU / scoringCPU double arithmetic.  Both run on the GPU.
-    const char* match_what = P.use_gpu ? "l3d_match_pairs_range" : "l3d_match_pairs_f64";
-    auto match_on = [&](l3d_ctx* c, int first, int last) {
-        return P.use_gpu ? l3d_match_pairs_range(c, npairs, P.pairs.data(), F.data(), P.epi, P.kNN, first, last)
-                         : l3d_match_pairs_f64(c, npairs, P.pairs.data(), Fdbl.data(), P.epi, P.kNN, first, last);
-    };
-    auto pair_cost = [&](int i) { return (long long)P.vlist[P.pairs[2 * i]]->lines.size() * (long long)P.vlist[P.pairs[2 * i + 1]]->lines.size(); };
+    if (const_regularization_depth < 0.0f && P.fixed3Dreg) P.med_scene_depth = median_of(P.views_avg_depths, P.med_scene_depth);
+    for (auto& kv : P.views) kv.second.k = P.fixed3Dreg ? P.sigma_p / P.med_scene_depth : P.spatial_reg(kv.second, P.sigma_p);   // view.cc:301-314
+    P.matched = false; P.est_best.clear(); P.est_P.clear(); P.est_index.clear();
+    const Impl::Translated frame(P);
+    P.index_views();
+    for (auto& kv : P.views) P.find_visual_neighbors(kv.first);
+    P.list_pairs();
     float ms_gather = 0.0f;
-    // The pairs [first, last) on the primary.  With several devices every one takes a contiguous share balanced by Ns*Nt, uploads the
-    // views and matches its share from its own host thread (keep-all waits on the host between its count and store passes, so one
-    // thread would serialise the devices), and the shares are gathered on the primary's stream.  The threads share no mutable host
-    // state: each works on its own context and writes only its own error slot.
-    auto match_range = [&](int first, int last) -> bool {
-        if (P.ctxs.size() == 1) return P.chk(match_on(P.ctx, first, last), match_what);
-        const int nd = (int)P.ctxs.size();
-        std::vector<long long> cost((size_t)(last - first));
-        for (int i = first; i < last; ++i) cost[i - first] = pair_cost(i);
-        std::vector<int32_t> b((size_t)nd + 1);
-        if (!P.chk(l3d_balanced_split(cost.data(), last - first, nd, b.data()), "l3d_balanced_split")) return false;
-        for (int32_t& x : b) x += first;
-        std::vector<std::string> errs((size_t)nd);
-        auto run = [&](int i) {
-            l3d_ctx* c = P.ctxs[i];
-            const char* what = "l3d_set_views";
-            long long rc = i == 0 ? 0 : l3d_set_views(c, (int)d.size(), d.data(), segp.data());     // the primary has its views already
-            if (rc >= 0) { what = match_what; rc = match_on(c, b[i], b[i + 1]); }
-            if (rc >= 0) { what = "l3d_sync"; rc = l3d_sync(c); }
-            if (rc < 0) errs[i] = "device " + std::to_string(P.devices[i]) + " (#" + std::to_string(i) + "): " + what + ": " + l3d_last_error(c);
-        };
-        std::vector<std::thread> th;
-        for (int i = 1; i < nd; ++i) th.emplace_back(run, i);
-        run(0);
-        for (std::thread& x : th) x.join();
-        for (const std::string& e : errs)
-            if (!e.empty()) { P.fail(e); return false; }
-        cudaSetDevice(P.devices[0]);
-        cudaStream_t s = (cudaStream_t)l3d_stream(P.ctx);
-        cudaEvent_t e0 = nullptr, e1 = nullptr;
-        const bool timed = cudaEventCreate(&e0) == cudaSuccess && cudaEventCreate(&e1) == cudaSuccess && cudaEventRecord(e0, s) == cudaSuccess;
-        bool ok = P.chk(l3d_match_gather(P.ctx, nd, P.ctxs.data(), b.data()), "l3d_match_gather");
-        cudaSetDevice(P.devices[0]);
-        ok = ok && (!timed || cudaEventRecord(e1, s) == cudaSuccess) && P.chk(l3d_sync(P.ctx), "l3d_sync");
-        if (ok && timed) cudaEventElapsedTime(&ms_gather, e0, e1);
-        if (e0) cudaEventDestroy(e0);
-        if (e1) cudaEventDestroy(e1);
-        return ok;
-    };
-    if (ok && P.shard_world > 1) {
-        // this rank's contiguous share of the pair list, balanced by Ns*Nt; the same split on every rank
-        std::vector<long long> cost((size_t)npairs), row_off((size_t)npairs + 1), row_bounds((size_t)P.shard_world + 1);
-        for (int i = 0; i < npairs; ++i) cost[i] = pair_cost(i);
-        std::vector<int32_t> bounds((size_t)P.shard_world + 1);
-        ok = P.chk(l3d_balanced_split(cost.data(), npairs, P.shard_world, bounds.data()), "l3d_balanced_split") &&
-             match_range(bounds[P.shard_rank], bounds[P.shard_rank + 1]) &&
-             P.chk(l3d_sync(P.ctx), "l3d_sync") && P.chk(l3d_pair_row_offsets(P.ctx, row_off.data()), "l3d_pair_row_offsets");
-        void *dc = nullptr, *dr = nullptr;
-        ok = ok && P.chk(l3d_match_device_buffers(P.ctx, &dc, &dr), "l3d_match_device_buffers");
-        if (ok) {
-            for (int r = 0; r <= P.shard_world; ++r) row_bounds[r] = row_off[bounds[r]];
-            auto exchange = [&](int knn, const char* what) {
-                if (P.exchange(P.exchange_user, dc, dr, row_bounds.data(), P.shard_world, knn) == 0) return true;
-                P.fail(std::string("matchImages: the match exchange callback failed") + what);
-                return false;
-            };
-            if (P.kNN >= 1 && P.kNN <= 32) ok = exchange(P.kNN, "");
-            else {
-                // Keep-all and kNN > 32: every rank laid out its records at the longest row of its own share.  Once the counts are
-                // exchanged, every rank reduces the same counts to the same stride and re-lays its rows at it; then the records move.
-                int stride = 0;
-                ok = exchange(0, " (row counts)") && P.chk(stride = l3d_match_restride(P.ctx, 0), "l3d_match_restride") &&
-                     P.chk(l3d_match_device_buffers(P.ctx, &dc, &dr), "l3d_match_device_buffers") && exchange(stride, " (records)");
-            }
-        }
-    } else
-        ok = ok && match_range(0, npairs) && P.chk(l3d_sync(P.ctx), "l3d_sync");
-    auto t1 = std::chrono::steady_clock::now();
+    std::vector<const float*> segp;
+    const std::vector<l3d_view_desc> d = P.descs(&segp);
+    const auto t0 = std::chrono::steady_clock::now();
+    nvtxRangePushA("l3d:set_views+match");
+    bool ok = P.match(d, segp, ms_gather);
+    const auto t1 = std::chrono::steady_clock::now();
     nvtxRangePop(); nvtxRangePushA("l3d:score_sweep");
     ok = ok && P.chk(l3d_score_sweep(P.ctx, P.two_sigA_sqr, MIN_SIMILARITY_3D, MIN_BEST_SCORE_3D, MIN_BEST_SCORE_PERC), "l3d_score_sweep");
     nvtxRangePop();
-    auto t2 = std::chrono::steady_clock::now();
-    if (ok) {
-        const long long ne = l3d_get_estimates(P.ctx, nullptr, nullptr, 0);
-        ok = P.chk(ne, "l3d_get_estimates");
-        if (ok) {
-            P.est_best.resize(ne); P.est_P.resize(6 * (size_t)ne);
-            if (ne) ok = P.chk(l3d_get_estimates(P.ctx, P.est_best.data(), P.est_P.data(), ne), "l3d_get_estimates");
-        }
-    }
-    if (ok) {
-        // filterMatches' tail (line3D.cc:1657-1668): per-view median of the best matches' depths
-        std::map<unsigned int, std::vector<float> > depths;
-        P.est_gseg.resize(P.est_best.size());
-        for (size_t e = 0; e < P.est_best.size(); ++e) {
-            const l3d_match& m = P.est_best[e];
-            depths[m.src_cam].push_back(m.d_p1); depths[m.src_cam].push_back(m.d_p2);
-            P.est_gseg[e] = P.views[m.src_cam].seg_off + m.src_seg;
-            P.est_of_gseg[P.est_gseg[e]] = e;
-        }
-        for (auto& kv : P.views) {
-            float med = (float)EPS;
-            std::vector<float>& dv = depths[kv.first];
-            if (!dv.empty()) { std::sort(dv.begin(), dv.end()); med = dv[dv.size() / 2]; }
-            kv.second.median_depth = med;                                               // update_median_depth view.h:108-121
-            if (P.fixed3Dreg) kv.second.k = P.sigma_p / P.med_scene_depth;
-        }
-        P.st.view_pairs = npairs; P.st.pair_evaluations = l3d_match_pair_evals(P.ctx); P.st.estimates = (long long)P.est_best.size();
-        P.st.matches_after_knn = l3d_match_total_matches(P.ctx);      // reduced on the device (was: download of the whole count array)
-        P.st.ms_match = std::chrono::duration<double, std::milli>(t1 - t0).count();
-        P.st.ms_score = std::chrono::duration<double, std::milli>(t2 - t1).count();
-        P.st.ms_gather = ms_gather;
-        P.matched = true;
-    }
-    P.untranslate();
+    const auto t2 = std::chrono::steady_clock::now();
+    if (!ok || !P.download_estimates()) return;
+    P.st.view_pairs = (long long)(P.pairs.size() / 2); P.st.pair_evaluations = l3d_match_pair_evals(P.ctx); P.st.estimates = (long long)P.est_best.size();
+    P.st.matches_after_knn = l3d_match_total_matches(P.ctx);      // reduced on the device (was: download of the whole count array)
+    P.st.ms_match = std::chrono::duration<double, std::milli>(t1 - t0).count();
+    P.st.ms_score = std::chrono::duration<double, std::milli>(t2 - t1).count();
+    P.st.ms_gather = ms_gather;
+    P.matched = true;
 }
 
 // get3DlineFromCluster (line3D.cc:2155-2218)
@@ -797,136 +910,25 @@ void Line3D::reconstruct3Dlines(const unsigned int visibility_t, const bool perf
     P.visibility_t = (unsigned int)std::max(int(visibility_t), 3);
     P.lines3D.clear(); P.collin_t = collinearity_t;
     P.perform_RDD = perform_diffusion && P.use_gpu;                                       // line3D.cc:1729
-    P.translate();
-    // median scene depth for lines (line3D.cc:1759-1774)
-    std::vector<float> sd;
+    const Impl::Translated frame(P);
+    std::vector<float> sd;                                // median scene depth for lines (line3D.cc:1759-1774)
     for (auto& kv : P.views) if (kv.second.median_depth > EPS) sd.push_back(kv.second.median_depth);
-    if (!sd.empty()) { std::sort(sd.begin(), sd.end()); P.med_scene_depth_lines = sd[sd.size() / 2]; } else P.med_scene_depth_lines = 0.0f;
-    std::vector<l3d_view_desc> d = P.descs();
-    auto t0 = std::chrono::steady_clock::now();
-    bool ok = P.chk(l3d_update_view_params(P.ctx, (int)d.size(), d.data()), "l3d_update_view_params");
-    // potentially collinear segments of every view (findCollinearSegments line3D.cc:1751-1756, 1827-1849); the affinity matrix
-    // below then adds the collinearity links (line3D.cc:1904-1974).  collinearity_t <= eps switches them off.
-    ok = ok && P.chk(l3d_find_collinear(P.ctx, collinearity_t > EPS ? collinearity_t : 0.0f, P.use_gpu ? L3D_SEM_REF_GPU : L3D_SEM_REF_CPU), "l3d_find_collinear");
-    P.st.collinear_entries = ok ? l3d_collinear_total(P.ctx) : 0;
-    // affinity matrix incl. the "unused" pair filter and first-come local ids (line3D.cc:1881-1900, 1982-2023), on the device
-    long long nids = 0;
-    long long nA = ok ? l3d_affinity_matrix(P.ctx, P.two_sigA_sqr, P.med_scene_depth_lines, MIN_AFFINITY, nullptr, nullptr, nullptr, 0, nullptr, 0, &nids) : -1;
-    ok = ok && P.chk(nA, "l3d_affinity_matrix");
-    P.A.clear(); P.local2global.clear();
-    if (ok && nA > 0) {
-        std::vector<int> ai((size_t)nA), aj((size_t)nA); std::vector<float> aw((size_t)nA);
-        P.local2global.resize((size_t)nids);
-        ok = P.chk(l3d_affinity_matrix(P.ctx, P.two_sigA_sqr, P.med_scene_depth_lines, MIN_AFFINITY, ai.data(), aj.data(), aw.data(), nA,
-                                       P.local2global.data(), nids, &nids), "l3d_affinity_matrix");
-        P.A.resize((size_t)nA);
-        for (long long e = 0; e < nA; ++e) { P.A[e].i = ai[e]; P.A[e].j = aj[e]; P.A[e].w = aw[e]; }
-    }
-    if (!ok) { P.untranslate(); return; }
-    P.A_raw = P.A;
-    auto t1 = std::chrono::steady_clock::now();
-    const int n = (int)P.local2global.size();
-    P.st.affinity_entries = (long long)P.A.size(); P.st.affinity_rows = n;
-    // diffusion (performRDD line3D.cc:2026-2076)
-    if (P.perform_RDD && !P.A.empty()) {
-        // the matrix is still on the device (l3d_affinity_matrix): diffusion + min(w12, w21) there, one download of the result in the
-        // (i, j) order the reference's std::map rebuilds A_ in (line3D.cc:2039-2071)
-        const long long nnz = (long long)P.A.size();
-        std::vector<int> oi(nnz), oj(nnz); std::vector<float> ow(nnz);
-        if (!P.chk(l3d_rdd_affinity(P.ctx, RDD_MAX_ITER, oi.data(), oj.data(), ow.data(), nnz), "l3d_rdd_affinity")) { P.untranslate(); return; }
-        for (long long e = 0; e < nnz; ++e) { P.A[e].i = oi[e]; P.A[e].j = oj[e]; P.A[e].w = ow[e]; }
-    }
-    auto t2 = std::chrono::steady_clock::now();
-    // clustering (clusterSegments line3D.cc:2079-2152)
+    P.med_scene_depth_lines = median_of(sd, 0.0f);
+    const std::vector<l3d_view_desc> d = P.descs();
+    const auto t0 = std::chrono::steady_clock::now();
+    if (!P.affinity_matrix(d)) return;
+    const auto t1 = std::chrono::steady_clock::now();
+    if (P.perform_RDD && !P.A.w.empty() && !P.diffuse()) return;
+    const auto t2 = std::chrono::steady_clock::now();
     std::vector<LineCluster3D> clusters;
-    P.st.clusters_total = 0;
-    if (!P.A.empty()) {
-        std::vector<unsigned int> worder;
-        if (P.A.size() > (1u << 20)) {          // big list: sort the weights on the device (stable, like std::list::sort)
-            std::vector<float> w(P.A.size());
-            for (size_t e = 0; e < w.size(); ++e) w[e] = P.A[e].w;
-            worder.resize(w.size());
-            if (!P.chk(l3d_argsort_f32(P.ctx, (long long)w.size(), w.data(), worder.data()), "l3d_argsort_f32")) { P.untranslate(); return; }
-        }
-        const std::vector<int> label = segment_graph(P.A, n, 3.0f, worder.empty() ? nullptr : &worder);
-        std::map<int, std::list<Segment2D> > members; std::map<int, std::set<unsigned int> > cams; std::vector<int> order;
-        for (int id = 0; id < n; ++id) {
-            const int cl = label[id];
-            if (!members.count(cl)) order.push_back(cl);
-            const Segment2D s = P.seg_of(P.local2global[id]);
-            members[cl].push_back(s); cams[cl].insert(s.camID());
-        }
-        P.st.clusters_total = (long long)order.size();
-        std::vector<const std::list<Segment2D>*> todo;
-        for (int cl : order) if (cams[cl].size() >= P.visibility_t) todo.push_back(&members[cl]);
-        std::vector<LineCluster3D> fitted(todo.size()); std::vector<unsigned char> good(todo.size(), 0);
-        parallel_for(todo.size(), [&](size_t i) { good[i] = P.line_from_cluster(*todo[i], fitted[i]) ? 1 : 0; });
-        for (size_t i = 0; i < todo.size(); ++i) if (good[i]) clusters.push_back(fitted[i]);
-    }
-    P.st.clusters_valid = (long long)clusters.size();
-    // optimizeClusters (line3D.cc:1800-1805, 2269-2275): bundle the cluster lines against their 2D residuals.  The reference
-    // needs Ceres for this (optimization.cc); here the same problem is minimised on the GPU (l3d_optimize_lines).
-    P.st.opt_iterations = 0; P.st.opt_cost_before = P.st.opt_cost_after = 0.0;
-    if (use_CERES && !clusters.empty()) {
-        const int Lc = (int)clusters.size(), nc = (int)P.vlist.size();
-        std::vector<double> p((size_t)6 * Lc), cams((size_t)16 * nc), xy;
-        std::vector<long long> ptr((size_t)Lc + 1, 0);
-        std::vector<int> rcam;
-        for (int v = 0; v < nc; ++v) {
-            const HostView& hv = *P.vlist[v];
-            double* cm = &cams[(size_t)16 * v];
-            for (int r = 0; r < 3; ++r) for (int c2 = 0; c2 < 3; ++c2) cm[3 * r + c2] = hv.R(r, c2);
-            cm[9] = hv.C.x; cm[10] = hv.C.y; cm[11] = hv.C.z;
-            cm[12] = hv.K(0, 0); cm[13] = hv.K(1, 1); cm[14] = hv.K(0, 2); cm[15] = hv.K(1, 2);
-        }
-        for (int i = 0; i < Lc; ++i) {
-            const Segment3D s3 = clusters[i].seg3D();
-            p[6 * i] = s3.P1().x; p[6 * i + 1] = s3.P1().y; p[6 * i + 2] = s3.P1().z; p[6 * i + 3] = s3.P2().x; p[6 * i + 4] = s3.P2().y; p[6 * i + 5] = s3.P2().z;
-            for (const Segment2D& s2 : *clusters[i].residuals()) {
-                const int vi = P.index_of.at(s2.camID());
-                const Vec4f& ln = P.vlist[vi]->lines[s2.segID()];
-                rcam.push_back(vi);
-                for (int k = 0; k < 4; ++k) xy.push_back((double)ln.v[k]);
-            }
-            ptr[i + 1] = (long long)rcam.size();
-        }
-        std::vector<int> valid((size_t)Lc);
-        double summ[8];
-        if (!P.chk(l3d_optimize_lines(P.ctx, Lc, p.data(), ptr.data(), rcam.data(), xy.data(), nc, cams.data(), (int)max_iter_CERES, p.data(), valid.data(), summ),
-                   "l3d_optimize_lines")) { P.untranslate(); return; }
-        std::vector<LineCluster3D> kept;
-        for (int i = 0; i < Lc; ++i) {
-            if (!valid[i]) continue;                        // optimization.cc:293-298
-            clusters[i].update3Dline(Segment3D(Vector3d(p[6 * i], p[6 * i + 1], p[6 * i + 2]), Vector3d(p[6 * i + 3], p[6 * i + 4], p[6 * i + 5])));
-            kept.push_back(clusters[i]);
-        }
-        clusters.swap(kept);
-        P.st.opt_iterations = (long long)summ[0]; P.st.opt_cost_before = summ[1]; P.st.opt_cost_after = summ[2];
-    }
+    if (!P.cluster_segments(clusters) || !P.optimize_clusters(clusters, use_CERES, max_iter_CERES)) return;
     P.use_ceres = use_CERES;
-    // computeFinal3Dsegments + filterTinySegments (line3D.cc:2278-2339)
-    std::vector<std::list<Segment3D> > kept_segs(clusters.size());
-    parallel_for(clusters.size(), [&](size_t i) {
-        const LineCluster3D& cl = clusters[i];
-        std::list<Segment3D> col = P.collinear_segments(cl);
-        if (col.empty()) return;
-        const HostView& rv = *P.vlist[P.index_of.at(cl.reference_view())];
-        for (const Segment3D& s : col) {
-            double u1, v1, u2, v2; rv.project(s.P1(), u1, v1); rv.project(s.P2(), u2, v2);
-            if (std::sqrt((u1 - u2) * (u1 - u2) + (v1 - v2) * (v1 - v2)) > rv.min_line_length) kept_segs[i].push_back(s);  // projectedLongEnough view.cc:423-428
-        }
-    });
-    for (size_t i = 0; i < clusters.size(); ++i) {
-        if (kept_segs[i].empty()) continue;
-        FinalLine3D f; f.collinear3Dsegments_ = kept_segs[i]; f.underlyingCluster_ = clusters[i];
-        P.lines3D.push_back(f);
-    }
-    auto t3 = std::chrono::steady_clock::now();
+    P.final_segments(clusters);
+    const auto t3 = std::chrono::steady_clock::now();
     P.st.lines3D = (long long)P.lines3D.size();
     P.st.ms_affinity = std::chrono::duration<double, std::milli>(t1 - t0).count();
     P.st.ms_diffusion = std::chrono::duration<double, std::milli>(t2 - t1).count();
     P.st.ms_cluster = std::chrono::duration<double, std::milli>(t3 - t2).count();
-    P.untranslate();
 }
 
 void Line3D::get3Dlines(std::vector<FinalLine3D>& result) { std::lock_guard<std::mutex> g(p_->mtx); result = p_->lines3D; }
@@ -1113,10 +1115,7 @@ int l3dpp_view_index(void* h, unsigned int cam) { auto& m = ((Line3D*)h)->impl()
 int l3dpp_collinear_from_cluster(void* h, const double* p1p2, int nres, const unsigned int* cams, const unsigned int* segs, double* out6, int cap)
 {
     Line3D::Impl& P = *((Line3D*)h)->impl();
-    if (P.vlist.size() != P.views.size()) {                       // views are indexed at the start of matchImages: do it here too
-        P.vlist.clear(); P.index_of.clear();
-        for (auto& kv : P.views) { P.index_of[kv.first] = (int)P.vlist.size(); P.vlist.push_back(&kv.second); }
-    }
+    if (P.vlist.size() != P.views.size()) { P.index_views(); P.matched = false; }   // as matchImages does, which outdates its results
     std::list<Segment2D> res;
     for (int i = 0; i < nres; ++i) res.push_back(Segment2D(cams[i], segs[i]));
     const LineCluster3D cl(Segment3D(Vector3d(p1p2[0], p1p2[1], p1p2[2]), Vector3d(p1p2[3], p1p2[4], p1p2[5])), res, nres ? cams[0] : 0);
@@ -1139,9 +1138,9 @@ int l3dpp_get_pairs(void* h, int* out, int cap)   // (src cam, tgt cam) in match
 long long l3dpp_get_affinity(void* h, int raw, int* ei, int* ej, float* ew, long long cap)
 {
     Line3D::Impl* P = ((Line3D*)h)->impl();
-    const std::vector<L3DPP::Edge>& A = raw ? P->A_raw : P->A;
-    for (size_t e = 0; e < A.size() && (long long)e < cap; ++e) { ei[e] = A[e].i; ej[e] = A[e].j; ew[e] = A[e].w; }
-    return (long long)A.size();
+    const L3DPP::Affinity& A = raw ? P->A_raw : P->A;
+    for (size_t e = 0; e < A.w.size() && (long long)e < cap; ++e) { ei[e] = A.i[e]; ej[e] = A.j[e]; ew[e] = A.w[e]; }
+    return (long long)A.w.size();
 }
 int l3dpp_get_local2global(void* h, unsigned int* cam_seg, int cap)
 {

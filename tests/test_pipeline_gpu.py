@@ -10,7 +10,7 @@ The oracle's host logic (oracle/l3d_oracle.cc) is driven twice:
 import numpy as np
 import pytest
 
-from line3dpp_b200 import synth, line3d
+from line3dpp_b200 import capi, synth, line3d
 from tests import util
 
 pytestmark = pytest.mark.gpu
@@ -279,4 +279,31 @@ def test_add_image_and_writer_errors_are_reported(tmp_path):
     assert "cannot open" in str(e.value)
     L.save_txt(str(tmp_path))
     assert any(f.name.endswith(".txt") for f in tmp_path.iterdir())
+    L.close()
+
+
+def test_add_image_reports_the_first_failed_check_in_each_overloads_order(tmp_path):
+    """a call that fails several checks reports the first: the segments overload checks the size, the neighbours, the segments and
+    then the camera ID; the image overload the size, the camera ID and then the neighbours (line3D.cc:116-155)"""
+    sc = synth.make_scene(6, 200, 3, "ring2")
+    L = line3d.Line3D(neighbors_by_worldpoints=False, use_gpu=True, output_folder=str(tmp_path), load_segments=False)
+    L.add_scene(sc)
+    K, R, t, nb, sg = sc.K[0], sc.R[0], sc.t[0], sc.neighbors[0], sc.segs[0]
+
+    def error(add):
+        with pytest.raises(capi.L3DError) as e:
+            add()
+        return str(e.value)
+    assert "too small" in error(lambda: L.add_image(0, 100, 75, K, R, t, 4.0, [], ()))
+    assert "no visual neighbors" in error(lambda: L.add_image(0, 3072, 2304, K, R, t, 4.0, [], sg))
+    assert "load_segments is off" in error(lambda: L.add_image(0, 3072, 2304, K, R, t, 4.0, nb, ()))
+    assert "no visual neighbors" in error(lambda: L.add_image(77, 3072, 2304, K, R, t, 4.0, [], ()))
+    assert "already in use" in error(lambda: L.add_image(0, 3072, 2304, K, R, t, 4.0, nb, sg))
+    img = np.zeros((900, 1200), np.uint8)
+    assert "too small" in error(lambda: L.add_image_pixels(0, img[:700, :700], K, R, t, 4.0, [], ()))
+    assert "already in use" in error(lambda: L.add_image_pixels(0, img, K, R, t, 4.0, [], ()))
+    assert "no visual neighbors" in error(lambda: L.add_image_pixels(77, img, K, R, t, 4.0, [], ()))
+    with pytest.raises(KeyError):                                                          # nothing was added ...
+        L.view_segments(77)
+    assert L.view_segments(0).tobytes() == np.ascontiguousarray(sg, np.float32).tobytes()   # ... or replaced
     L.close()
