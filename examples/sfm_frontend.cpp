@@ -1,12 +1,14 @@
-// examples/sfm_frontend.cpp — the reference's mavmap, OpenMVG and Pix4D frontends (main_mavmap.cpp, main_openmvg.cpp, main_pix4d.cpp) on
+// examples/sfm_frontend.cpp — the reference's mavmap, OpenMVG, Pix4D and COLMAP frontends (main_mavmap.cpp, main_openmvg.cpp, main_pix4d.cpp,
+// main_colmap.cpp) on
 // top of include/line3d.h + include/line3d_io.h: read the model, hand every camera its 2D segments, match, reconstruct, save.  Like
 // examples/vsfm_frontend.cpp it is deliberately small: no option parser, and the 2D segments come from text files because line
 // detection is outside this library.  The images are not loaded either, so lens distortion is only reported: the segments are expected
-// in the undistorted image (Line3D::undistortImage with the camera's coefficients gives that image).
+// in the undistorted image (Line3D::undistortImage with the camera's coefficients, or with its LensDistortion, gives that image).
 //
 //   sfm_frontend mavmap  <result.txt>     <segments_dir> <output_dir> [const_reg_depth]
 //   sfm_frontend openmvg <sfm_data.json>  <segments_dir> <output_dir>
 //   sfm_frontend pix4d   <params_folder>  <segments_dir> <output_dir> <project_prefix>
+//   sfm_frontend colmap  <sparse folder>  <segments_dir> <output_dir>      (text or binary model; prints every camera's lens)
 //   <segments_dir>/<image file name>.txt :  first line "width height", then one "x1 y1 x2 y2" per line
 //
 // build:  g++ -std=c++17 examples/sfm_frontend.cpp -Iinclude -Lline3dpp_b200 -ll3d_b200 -Wl,-rpath,$PWD/line3dpp_b200 -o sfm_frontend
@@ -30,8 +32,8 @@ static bool read_segments(const std::string& path, int& w, int& h, std::vector<L
 int main(int argc, char** argv)
 {
     const std::string fmt = argc > 1 ? argv[1] : "";
-    if (argc < 5 || (fmt != "mavmap" && fmt != "openmvg" && fmt != "pix4d") || (fmt == "pix4d" && argc < 6)) {
-        std::fprintf(stderr, "usage: %s mavmap|openmvg|pix4d <model> <segments_dir> <output_dir> [const_reg_depth | project_prefix]\n", argv[0]);
+    if (argc < 5 || (fmt != "mavmap" && fmt != "openmvg" && fmt != "pix4d" && fmt != "colmap") || (fmt == "pix4d" && argc < 6)) {
+        std::fprintf(stderr, "usage: %s mavmap|openmvg|pix4d|colmap <model> <segments_dir> <output_dir> [const_reg_depth | project_prefix]\n", argv[0]);
         return 2;
     }
     const std::string model = argv[2], segdir = argv[3], outdir = argv[4];
@@ -39,12 +41,20 @@ int main(int argc, char** argv)
     const float const_reg_depth = mavmap && argc > 5 ? (float)std::atof(argv[5]) : -1.0f;
 
     std::vector<L3DPP::SfMCamera> cams;
+    std::vector<L3DPP::LensDistortion> lenses;
     std::string err;
     bool ok;
     if (mavmap) ok = L3DPP::readMavmap(model, cams, &err);
     else if (fmt == "openmvg") ok = L3DPP::readOpenMVG(model, cams, &err);
+    else if (fmt == "colmap") ok = L3DPP::readColmap(model, cams, &err, &lenses);   // cameras/images/points3D .txt, or else .bin
     else ok = L3DPP::readPix4D(model, argv[5], cams, &err);             // triangulates the tie points on GPU 0
     if (!ok) { std::fprintf(stderr, "%s\n", err.c_str()); return 1; }
+    for (size_t i = 0; i < lenses.size(); ++i) {
+        const L3DPP::LensDistortion& l = lenses[i];
+        const bool fe = l.model == L3DPP::LensDistortion::FISHEYE;
+        std::printf("camera %u (%s): %s lens, k = %g %g %g %g %g %g, p = %g %g\n", cams[i].id, cams[i].image.c_str(), fe ? "fisheye" : "radtan", l.k[0],
+                    l.k[1], l.k[2], l.k[3], l.k[4], l.k[5], l.p[0], l.p[1]);
+    }
 
     try {
         // mavmap has no world points: explicit neighbour lists and a constant regularisation depth (main_mavmap.cpp:150-151, 309-326)
@@ -57,7 +67,9 @@ int main(int argc, char** argv)
             int w = 0, h = 0;
             std::vector<L3DPP::Vec4f> segs;
             if (!read_segments(segdir + "/" + name + ".txt", w, h, segs)) { std::fprintf(stderr, "no segments for %s, skipped\n", name.c_str()); continue; }
-            if (c.radial[0] != 0.0 || c.radial[1] != 0.0 || c.radial[2] != 0.0 || c.tangential[0] != 0.0 || c.tangential[1] != 0.0)
+            bool distorted = c.radial[0] != 0.0 || c.radial[1] != 0.0 || c.radial[2] != 0.0 || c.tangential[0] != 0.0 || c.tangential[1] != 0.0;
+            for (int k = 0; k < 6 && i < lenses.size(); ++k) distorted = distorted || lenses[i].k[k] != 0.0;
+            if (distorted)
                 std::fprintf(stderr, "note: %s is distorted; segments are expected in the undistorted image\n", name.c_str());
             const std::list<unsigned int> list = mavmap ? L3DPP::sequentialNeighbors((unsigned int)i, (unsigned int)cams.size(), L3DPP::L3D_DEF_MATCHING_NEIGHBORS)
                                                         : c.worldpoints;

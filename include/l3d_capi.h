@@ -272,14 +272,20 @@ int l3d_optimize_lines(l3d_ctx* ctx, int num_lines, const double* p1p2, const lo
                        const double* res_xy, int num_cams, const double* cams, int max_iter, double* p1p2_out, int32_t* valid_out,
                        double* summary);
 
+#define L3D_LENS_RADTAN 0       /* OpenCV's standard model: k1 k2 p1 p2 k3 [k4 k5 k6] */
+#define L3D_LENS_FISHEYE 1      /* OpenCV's fisheye (equidistant) model: k1..k4 */
 /* ---- lens undistortion of 8-bit images: Line3D::undistortImage (line3D.cc:83-109), i.e. OpenCV's initUndistortRectifyMap with
  * fixed-point maps (CV_16SC2 pixel + CV_16UC1 1/32-px fraction) followed by remap(INTER_LINEAR, BORDER_CONSTANT 0), output the size
  * and type of the input, K unchanged.  The camera matrix is [[fx,0,cx],[0,fy,cy],[0,0,1]] (skew is ignored, as in the reference);
- * the distortion vector is (k1, k2, p1, p2, k3) = (radial[0], radial[1], tangential[0], tangential[1], radial[2]).  The map is
- * defined by the formula of DESIGN.md §4a, which OpenCV builds reproduce to within one 1/32-px step; the remap is bit-exact to
- * OpenCV's.  Pixels are interleaved (channels 1 or 3); pitches are row strides in bytes.
+ * the distortion vector is (k1, k2, p1, p2, k3, k4, k5, k6) = (radial[0], radial[1], tangential[0], tangential[1], radial[2],
+ * rational[0..2]).  model = L3D_LENS_FISHEYE instead is cv::fisheye::initUndistortRectifyMap(K, fisheye[0..3], I, K) with the same
+ * fixed-point maps; radial, tangential and rational must then be zero.  The maps are defined by the formulas of DESIGN.md §4a,
+ * which OpenCV builds reproduce to within one 1/32-px step (radtan: exactly, for the rational terms too, up to OpenCV's accumulation
+ * order; fisheye: up to the last ulp of atan); the remap is bit-exact to OpenCV's.  Pixels are interleaved (channels 1 or 3);
+ * pitches are row strides in bytes.
  * Rejected with L3D_ERR_INVALID: width or height outside [1, 32767], channels other than 1 or 3, a pitch below width*channels,
- * null pointers, src == dst, fx or fy zero or not finite, a principal point or coefficient that is not finite.
+ * null pointers, src == dst, fx or fy zero or not finite, a principal point or coefficient that is not finite, an unknown model,
+ * a fisheye descriptor with a nonzero radial, tangential or rational term.
  * on_device != 0: every pointer is a device address on this GPU and the call is asynchronous on the context's stream;
  * on_device == 0: host buffers, staged through the context's own device buffers, and the call returns when the output is written. */
 typedef struct {
@@ -289,6 +295,10 @@ typedef struct {
     uint8_t* dst;
     double fx, fy, cx, cy;
     double radial[3], tangential[2];
+    /* lens model; a zero-initialised tail is the model above (L3D_LENS_RADTAN without rational terms) */
+    int32_t model;                 /* L3D_LENS_RADTAN or L3D_LENS_FISHEYE */
+    double rational[3];            /* L3D_LENS_RADTAN: k4, k5, k6 (the denominator of OpenCV's 8-coefficient model) */
+    double fisheye[4];             /* L3D_LENS_FISHEYE: k1..k4 of theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 + k4 theta^8) */
 } l3d_undistort_desc;
 /* undistort n images in one launch; images, sizes, channel counts and cameras may all differ */
 int l3d_undistort_u8(l3d_ctx* ctx, int n, const l3d_undistort_desc* descs, int on_device);

@@ -64,6 +64,15 @@ struct Image8u {
     Image8u(int r, int c, int ch) : cols(c), rows(r), channels(ch), data((size_t)(r > 0 ? r : 0) * (c > 0 ? c : 0) * (ch > 0 ? ch : 0)) {}
 };
 
+/* a camera's lens distortion as OpenCV models it (include/l3d_capi.h l3d_undistort_desc).  RADTAN: k = k1..k6 (OpenCV's
+ * (k1, k2, p1, p2, k3, k4, k5, k6); k4..k6 = 0 is the 5-coefficient model), p = p1, p2.  FISHEYE: cv::fisheye's k1..k4 in k[0..3],
+ * the rest zero.  Zero-initialised: no distortion. */
+struct LensDistortion {
+    enum Model { RADTAN = 0, FISHEYE = 1 };
+    int model;
+    double k[6], p[2];
+};
+
 #ifdef L3DPP_WITH_EIGEN_OPENCV
 namespace detail {
 /* the pixels of a cv::Mat as an Image8u, honouring its row step; a type other than CV_8UC1 / CV_8UC3 gives 0 channels, which
@@ -285,6 +294,9 @@ public:
      * the call.  Throws std::invalid_argument for an image or camera l3d_undistort_u8 rejects, std::runtime_error on a CUDA failure
      * or without a usable device. */
     static void undistortImage(const Image8u& in, Image8u& out, const Vector3d& radial_coeffs, const Vector2d& tangential_coeffs, const Matrix3d& K);
+    /* the same for any lens l3d_undistort_u8 takes (the overload above is lens = {RADTAN, {k1, k2, k3, 0, 0, 0}, {p1, p2}});
+     * std::invalid_argument also for an unknown model and a fisheye lens with k[4], k[5], p[0] or p[1] nonzero */
+    static void undistortImage(const Image8u& in, Image8u& out, const LensDistortion& lens, const Matrix3d& K);
 
 #ifdef L3DPP_WITH_EIGEN_OPENCV
     /* The reference's exact signature for CV_8UC1 / CV_8UC3 images; honours the row step of inImg and create()s outImg.  A template
@@ -302,6 +314,23 @@ public:
         Matrix3d Kp;
         for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) Kp(r, c) = K(r, c);
         undistortImage(a, b, Vector3d(radial_coeffs(0), radial_coeffs(1), radial_coeffs(2)), Vector2d(tangential_coeffs(0), tangential_coeffs(1)), Kp);
+        out.create(in.rows, in.cols, in.type());
+        const size_t out_step = static_cast<size_t>(out.step);
+        for (int r = 0; r < b.rows; ++r) std::memcpy(out.data + r * out_step, b.data.data() + r * row, row);
+    }
+    /* the cv::Mat form of the LensDistortion overload (e.g. with readColmap's lenses) */
+    template <class MatT = cv::Mat>
+    static void undistortImage(const cv::Mat& inImg, cv::Mat& outImg, const LensDistortion& lens, const Eigen::Matrix3d& K)
+    {
+        const MatT& in = inImg;
+        MatT& out = outImg;
+        if (in.type() != CV_8UC1 && in.type() != CV_8UC3) throw std::invalid_argument("undistortImage: only CV_8UC1 and CV_8UC3 images");
+        Image8u a(in.rows, in.cols, in.channels()), b;
+        const size_t row = (size_t)in.cols * in.channels(), in_step = static_cast<size_t>(in.step);
+        for (int r = 0; r < in.rows; ++r) std::memcpy(a.data.data() + r * row, in.data + r * in_step, row);
+        Matrix3d Kp;
+        for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) Kp(r, c) = K(r, c);
+        undistortImage(a, b, lens, Kp);
         out.create(in.rows, in.cols, in.type());
         const size_t out_step = static_cast<size_t>(out.step);
         for (int r = 0; r < b.rows; ++r) std::memcpy(out.data + r * out_step, b.data.data() + r * row, row);

@@ -42,9 +42,18 @@ struct SfMCamera {
  * flipped (Bundler looks down -z). */
 bool readBundler(const std::string& bundle_file, const std::string& image_list_file, std::vector<SfMCamera>& cameras, std::string* error = 0);
 
-/* cameras.txt / images.txt / points3D.txt of a COLMAP text model like main_colmap.cpp:140-349 (models SIMPLE_PINHOLE, PINHOLE,
- * SIMPLE_RADIAL, RADIAL, OPENCV, FULL_OPENCV; images whose camera is unknown are dropped).  Cameras are returned in file order. */
-bool readColmap(const std::string& sfm_folder, std::vector<SfMCamera>& cameras, std::string* error = 0);
+/* A COLMAP model like main_colmap.cpp:140-349: cameras.txt / images.txt / points3D.txt when all three exist, otherwise COLMAP's default
+ * output cameras.bin / images.bin / points3D.bin (its documented little-endian layout; a point3D_id of 2^64 - 1 is "none", like -1 in
+ * the text file).  Both give the same cameras, field for field: images in file order, those whose camera is unknown dropped,
+ * worldpoints in observation order, the float median depth.
+ * Models: SIMPLE_PINHOLE, PINHOLE, SIMPLE_RADIAL, RADIAL, OPENCV, FULL_OPENCV (radial / tangential as the reference sets them:
+ * FULL_OPENCV's k4..k6 are not among them) and OPENCV_FISHEYE, SIMPLE_RADIAL_FISHEYE, RADIAL_FISHEYE (radial / tangential zero).
+ * With lenses, (*lenses)[i] is camera i's full lens (LensDistortion, for Line3D::undistortImage), FULL_OPENCV's k4..k6 included;
+ * without it a fisheye camera is rejected, since its distortion has nowhere to go.  FOV, THIN_PRISM_FISHEYE,
+ * RAD_TAN_THIN_PRISM_FISHEYE and unknown models are rejected with an error naming the model and the camera.  Like the readers below,
+ * a truncated or malformed binary file returns false with *error naming the file and the problem, never crashes the reader and never
+ * makes it allocate more than the file's size warrants; ids that do not fit unsigned int are rejected. */
+bool readColmap(const std::string& sfm_folder, std::vector<SfMCamera>& cameras, std::string* error = 0, std::vector<LensDistortion>* lenses = 0);
 
 /* The mavmap, OpenMVG and Pix4D models (csrc/line3d_sfm.cc, DESIGN.md §6b).  Like the readers above: false with *error naming the
  * file, the line or JSON path and the problem on malformed input, which never crashes the reader and never makes it allocate more

@@ -24,11 +24,17 @@ class UndistortDesc(C.Structure):
     """l3d_undistort_desc: one 8-bit image and its camera"""
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("channels", C.c_int32), ("src_pitch", C.c_int64), ("dst_pitch", C.c_int64),
                 ("src", C.c_void_p), ("dst", C.c_void_p), ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
-                ("radial", C.c_double * 3), ("tangential", C.c_double * 2)]
+                ("radial", C.c_double * 3), ("tangential", C.c_double * 2), ("model", C.c_int32), ("rational", C.c_double * 3),
+                ("fisheye", C.c_double * 4)]
 
 
-def make_undistort_desc(width, height, channels, K, radial=(0, 0, 0), tangential=(0, 0), src=0, src_pitch=None, dst=0, dst_pitch=None):
-    """K: 3x3 camera matrix (fx, fy, cx, cy are read, skew is ignored); src / dst: addresses; pitches in bytes (default packed)"""
+LENS_RADTAN, LENS_FISHEYE = 0, 1     # l3d_undistort_desc::model
+
+
+def make_undistort_desc(width, height, channels, K, radial=(0, 0, 0), tangential=(0, 0), src=0, src_pitch=None, dst=0, dst_pitch=None,
+                        model=LENS_RADTAN, rational=(0, 0, 0), fisheye=(0, 0, 0, 0)):
+    """K: 3x3 camera matrix (fx, fy, cx, cy are read, skew is ignored); src / dst: addresses; pitches in bytes (default packed);
+    model: LENS_RADTAN (radial k1 k2 k3, tangential p1 p2, rational k4 k5 k6) or LENS_FISHEYE (fisheye k1..k4)"""
     K = np.asarray(K, np.float64).reshape(3, 3)
     row = int(width) * int(channels)
     d = UndistortDesc()
@@ -39,7 +45,20 @@ def make_undistort_desc(width, height, channels, K, radial=(0, 0, 0), tangential
     d.fx, d.fy, d.cx, d.cy = float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2])
     d.radial[:] = [float(v) for v in radial]
     d.tangential[:] = [float(v) for v in tangential]
+    d.model = int(model)
+    d.rational[:] = [float(v) for v in rational]
+    d.fisheye[:] = [float(v) for v in fisheye]
     return d
+
+
+def lens_desc_args(lens):
+    """the make_undistort_desc keywords of a lens dict {"model": 0 | 1, "k": k1..k6 (radtan) or k1..k4 (fisheye), "p": p1, p2}, the
+    layout of L3DPP::LensDistortion"""
+    k = [float(v) for v in lens.get("k", ())] + [0.0] * 6
+    p = [float(v) for v in lens.get("p", ())] + [0.0] * 2
+    if int(lens.get("model", LENS_RADTAN)) == LENS_FISHEYE:     # k5, k6, p1, p2 go where l3d_undistort_u8 rejects them if nonzero
+        return dict(model=LENS_FISHEYE, fisheye=k[:4], radial=k[4:6] + [0.0], tangential=p[:2])
+    return dict(model=int(lens.get("model", LENS_RADTAN)), radial=k[:3], tangential=p[:2], rational=k[3:6])
 
 
 class ImagePrepDesc(C.Structure):
@@ -363,12 +382,14 @@ class Context:
         return cnt, med
 
     # ---- lens undistortion (stateless: no pipeline stage changes)
-    def undistort(self, images, K, radial=(0, 0, 0), tangential=(0, 0), out=None):
+    def undistort(self, images, K, radial=(0, 0, 0), tangential=(0, 0), out=None, lens=None):
         """Line3D::undistortImage for a list of uint8 HxW / HxWx3 images in ONE batched call.  K, radial, tangential: one camera for
-        all images or one per image.  out: optional list of preallocated outputs (any row pitch).  Returns the output arrays."""
+        all images or one per image.  lens: instead of radial / tangential, one lens dict (lens_desc_args) or a list with one per image.
+        out: optional list of preallocated outputs (any row pitch).  Returns the output arrays."""
         n = len(images)
         per = lambda v, nd: [v] * n if np.ndim(v) == nd else list(v)
         Ks, rads, tans = per(K, 2), per(radial, 1), per(tangential, 1)
+        lenses = [None] * n if lens is None else [lens] * n if isinstance(lens, dict) else list(lens)
         descs, keep = (UndistortDesc * n)(), []
         outs = []
         for i, img in enumerate(images):
@@ -377,8 +398,9 @@ class Context:
             if o.shape != a.shape or o.dtype != np.uint8 or o.strides[1:] != a.strides[1:]:
                 raise ValueError("output must be a uint8 array of the input's shape with packed rows")
             keep += [a, o]
-            descs[i] = make_undistort_desc(a.shape[1], a.shape[0], 1 if a.ndim == 2 else 3, Ks[i], rads[i], tans[i], a.ctypes.data, sp,
-                                           o.ctypes.data, o.strides[0])
+            lk = dict(radial=rads[i], tangential=tans[i]) if lenses[i] is None else lens_desc_args(lenses[i])
+            descs[i] = make_undistort_desc(a.shape[1], a.shape[0], 1 if a.ndim == 2 else 3, Ks[i], src=a.ctypes.data, src_pitch=sp,
+                                           dst=o.ctypes.data, dst_pitch=o.strides[0], **lk)
             outs.append(o)
         self._chk(self.L.l3d_undistort_u8(self.h, n, descs, 0), "l3d_undistort_u8")
         return outs
@@ -409,9 +431,10 @@ class Context:
         """l3d_undistort_u8 on device addresses (a ctypes array of UndistortDesc); asynchronous on the context's stream"""
         self._chk(self.L.l3d_undistort_u8(self.h, len(descs), descs, 1), "l3d_undistort_u8")
 
-    def undistort_map(self, width, height, K, radial=(0, 0, 0), tangential=(0, 0)):
-        """the fixed-point maps cv::remap takes: (map_xy int16 [h, w, 2], map_frac uint16 [h, w])"""
-        d = make_undistort_desc(width, height, 1, K, radial, tangential)
+    def undistort_map(self, width, height, K, radial=(0, 0, 0), tangential=(0, 0), lens=None):
+        """the fixed-point maps cv::remap takes: (map_xy int16 [h, w, 2], map_frac uint16 [h, w]); lens as in undistort"""
+        lk = dict(radial=radial, tangential=tangential) if lens is None else lens_desc_args(lens)
+        d = make_undistort_desc(width, height, 1, K, **lk)
         xy = np.empty((height, width, 2), np.int16)
         fr = np.empty((height, width), np.uint16)
         self._chk(self.L.l3d_undistort_map(self.h, C.byref(d), _p(xy), _p(fr), 0), "l3d_undistort_map")

@@ -65,16 +65,20 @@ struct RddState {
 struct L3DUndistImage {
     const unsigned char* src;
     unsigned char* dst;
+    const double* xcol;                      // fisheye: x of every column (OpenCV's accumulated sum), in UndistortState::d_cols
     long long src_pitch, dst_pitch, tile0;   // tile0: first tile of this image in the batch grid
     int width, height, channels, tiles_x;
+    int kind;                                // lens kind of l3d_undistort.cu: radtan, radtan with k4..k6 (rational), fisheye
     int full_radial, tangential;             // 0: k2 = k3 = 0, resp. p1 = p2 = 0 (those terms are skipped)
-    double ir0, ir2, ir4, ir5, fx, fy, cx, cy, k1, k2, k3, p1, p2;
+    double ir0, ir2, ir4, ir5, fx, fy, cx, cy;
+    double k1, k2, k3, k4, k5, k6, p1, p2;   // radtan: k1..k6, p1, p2; fisheye: k1..k4 are the theta coefficients
 };
 
 // buffers of the undistortion calls: not a pipeline stage, nothing else reads them
 struct UndistortState {
     std::vector<L3DUndistImage> h_imgs;
-    DevBuf d_imgs, d_src, d_dst, d_map_xy, d_map_frac;   // d_src .. d_map_frac: host-mode staging
+    std::vector<double> h_cols;                          // fisheye column tables, one per distinct (ir0, ir2)
+    DevBuf d_imgs, d_cols, d_src, d_dst, d_map_xy, d_map_frac;   // d_src .. d_map_frac: host-mode staging
 };
 
 // per-image parameters of k_prepare_gray_u8 (l3d_image_prep.cu): source (width x height, 1 or 3 channels) -> grey out_w x out_h

@@ -1,16 +1,23 @@
 // l3d_undistort.cu — lens undistortion of 8-bit images: what Line3D::undistortImage computes with OpenCV (line3D.cc:83-109,
 // initUndistortRectifyMap with fixed-point CV_16SC2 + CV_16UC1 maps, then remap INTER_LINEAR / BORDER_CONSTANT 0), and the three
-// C-ABI entry points declared in include/l3d_capi.h.  The arithmetic contract is DESIGN.md §4a; tests/undistort_model.py restates it.
+// C-ABI entry points declared in include/l3d_capi.h.  Two lens models: OpenCV's standard one with up to 8 coefficients (radtan) and
+// cv::fisheye's.  The arithmetic contract is DESIGN.md §4a; tests/undistort_model.py and tests/lens_model.py restate it.
 //
 // None of these calls belongs to the pipeline: they never drop a stage and touch only the buffers of UndistortState.
 #include "l3d_ctx.cuh"
 
+#include <algorithm>
 #include <climits>
 #include <cmath>
 #include <cstring>
+#include <vector>
 
 #define UD_TW 128       // columns per tile of k_undistort_u8 (one per thread)
 #define UD_TH 16        // rows per tile
+
+// the kernels' lens kinds (L3DUndistImage::kind): radtan without and with the rational denominator, fisheye.  Each has its own
+// instance of k_undistort_u8, so the pinhole kernel keeps its 48 registers (a double division or atan in the same kernel costs 16 / 24).
+enum { UD_RADTAN = 0, UD_RATIONAL = 1, UD_FISHEYE = 2, UD_KINDS = 3 };
 
 // cvRound(t * 32) as OpenCV's x86 build does it: round half to even; a value that is not finite or does not fit int32 gives INT_MIN
 __device__ __forceinline__ int ud_fix(double t)
@@ -23,10 +30,12 @@ __device__ __forceinline__ int ud_fix(double t)
 // (the zero entries of ir only add signed zeros).  x2 = x*x and y2 = y*y come from the caller so that a tile computes them once
 // per column / row.  Terms whose coefficients are zero are skipped: that changes at most the sign of a zero, which the rounding
 // erases.  Plain IEEE double operations in the reference's order (the library is compiled with -fmad=false).
+template <bool RATIONAL>
 __device__ __forceinline__ void ud_map_point(const L3DUndistImage& d, double x, double x2, double y, double y2, int& iu, int& iv)
 {
     const double r2 = x2 + y2;
-    const double kr = 1.0 + (d.full_radial ? ((d.k3 * r2 + d.k2) * r2 + d.k1) : d.k1) * r2;
+    double kr = 1.0 + (d.full_radial ? ((d.k3 * r2 + d.k2) * r2 + d.k1) : d.k1) * r2;
+    if (RATIONAL) kr = kr / (1.0 + ((d.k6 * r2 + d.k5) * r2 + d.k4) * r2);
     double xd = x * kr, yd = y * kr;
     if (d.tangential) {
         const double _2xy = 2.0 * x * y;
@@ -37,13 +46,47 @@ __device__ __forceinline__ void ud_map_point(const L3DUndistImage& d, double x, 
     iv = ud_fix(d.fy * yd + d.cy);
 }
 
+// The same for cv::fisheye::initUndistortRectifyMap with R = I, newK = K: x comes from the column table (OpenCV's loop accumulates it),
+// r = |(x, y)|, theta = atan(r), theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 + k4 theta^8), u = fx x (theta_d / r) + cx.
+// Everything but atan is IEEE; atan may differ from the host's in the last ulp (the fisheye contract is one step, DESIGN.md §4a).
+__device__ __forceinline__ void ud_fisheye_point(const L3DUndistImage& d, double x, double x2, double y, double y2, int& iu, int& iv)
+{
+    const double r = sqrt(x2 + y2);
+    const double th = atan(r);
+    const double t2 = th * th, t4 = t2 * t2, t6 = t4 * t2, t8 = t4 * t4;
+    const double thd = th * (1.0 + d.k1 * t2 + d.k2 * t4 + d.k3 * t6 + d.k4 * t8);
+    const double scale = r == 0.0 ? 1.0 : thd / r;
+    iu = ud_fix(d.fx * x * scale + d.cx);
+    iv = ud_fix(d.fy * y * scale + d.cy);
+}
+
 __device__ __forceinline__ short ud_sat16(int v) { return (short)max(-32768, min(32767, v)); }
 
-// OpenCV's map entry: integer pixel (saturated to int16) and the 1/32-px fractions packed as ty*32 + tx
+// OpenCV's map entry: integer pixel and the 1/32-px fractions packed as ty*32 + tx.  The pixel is saturated to int16 by
+// initUndistortRectifyMap and truncated (wraps) by the fisheye loop's (short) cast.
+template <int KIND>
 __device__ __forceinline__ void ud_entry(int iu, int iv, short2& xy, unsigned short& frac)
 {
-    xy = make_short2(ud_sat16(iu >> 5), ud_sat16(iv >> 5));
+    if (KIND == UD_FISHEYE) xy = make_short2((short)(iu >> 5), (short)(iv >> 5));
+    else xy = make_short2(ud_sat16(iu >> 5), ud_sat16(iv >> 5));
     frac = (unsigned short)(((iv & 31) << 5) + (iu & 31));
+}
+
+// source position and map entry of one destination pixel under the image's model
+template <int KIND>
+__device__ __forceinline__ void ud_map_entry(const L3DUndistImage& d, double x, double x2, double y, double y2, short2& xy, unsigned short& frac)
+{
+    int iu, iv;
+    if (KIND == UD_FISHEYE) ud_fisheye_point(d, x, x2, y, y2, iu, iv);
+    else ud_map_point<KIND == UD_RATIONAL>(d, x, x2, y, y2, iu, iv);
+    ud_entry<KIND>(iu, iv, xy, frac);
+}
+
+// x of column j: j*ir0 + ir2 (radtan) or the fisheye column table
+template <int KIND>
+__device__ __forceinline__ double ud_column_x(const L3DUndistImage& d, int j)
+{
+    return KIND == UD_FISHEYE ? d.xcol[j] : (double)j * d.ir0 + d.ir2;
 }
 
 // remap's bilinear tap sum for one destination pixel: weights (32-tx|tx)*(32-ty|ty)*32 sum to 32768; a tap outside the image
@@ -71,15 +114,15 @@ __device__ __forceinline__ void ud_tap_sum(const unsigned char* __restrict__ src
 }
 
 // the maps of one image, OpenCV's layout: map_xy short2[H*W], map_frac ushort[H*W], rows packed
+template <int KIND>
 __global__ void __launch_bounds__(UD_TW) k_undistort_map(L3DUndistImage d, short2* __restrict__ map_xy, unsigned short* __restrict__ map_frac)
 {
     const int j = blockIdx.x * UD_TW + threadIdx.x, i = blockIdx.y;
     if (j >= d.width) return;
-    const double x = (double)j * d.ir0 + d.ir2, y = (double)i * d.ir4 + d.ir5;
-    int iu, iv;
-    ud_map_point(d, x, x * x, y, y * y, iu, iv);
+    const double y = (double)i * d.ir4 + d.ir5;
     const long long o = (long long)i * d.width + j;
-    ud_entry(iu, iv, map_xy[o], map_frac[o]);
+    const double x = ud_column_x<KIND>(d, j);
+    ud_map_entry<KIND>(d, x, x * x, y, y * y, map_xy[o], map_frac[o]);
 }
 
 // remap of one image with caller-given maps (same layout)
@@ -92,21 +135,22 @@ __global__ void __launch_bounds__(UD_TW) k_remap_u8(L3DUndistImage d, const shor
     ud_tap_sum<C>(d.src, d.src_pitch, d.width, d.height, map_xy[o], map_frac[o], d.dst + (long long)i * d.dst_pitch + (long long)j * C);
 }
 
-template <int C>
-__device__ __forceinline__ void ud_tile_rows(const L3DUndistImage& d, int j, int i0, int rows, double x, double x2, const double2* s_y)
+template <int KIND, int C>
+__device__ __forceinline__ void ud_tile_rows(const L3DUndistImage& d, int j, int i0, int rows, const double2* s_y)
 {
+    const double x = ud_column_x<KIND>(d, j), x2 = x * x;
     unsigned char* out = d.dst + (long long)i0 * d.dst_pitch + (long long)j * C;
     for (int r = 0; r < rows; ++r, out += d.dst_pitch) {
-        int iu, iv;
-        ud_map_point(d, x, x2, s_y[r].x, s_y[r].y, iu, iv);
         short2 xy; unsigned short frac;
-        ud_entry(iu, iv, xy, frac);
+        ud_map_entry<KIND>(d, x, x2, s_y[r].x, s_y[r].y, xy, frac);
         ud_tap_sum<C>(d.src, d.src_pitch, d.width, d.height, xy, frac, out);
     }
 }
 
 // The fused hot path over a batch: map entries in registers, never stored.  One CTA = UD_TW columns x UD_TH rows of one image;
-// the tiles of all images form one grid (image found by binary search over tile0), grey and RGB images alike.
+// the tiles of all images of one model form one grid (image found by binary search over tile0), grey and RGB images alike.  One
+// instance per lens kind (UD_RADTAN ..), each over its own images.
+template <int KIND>
 __global__ void __launch_bounds__(UD_TW) k_undistort_u8(const L3DUndistImage* __restrict__ imgs, int n)
 {
     __shared__ double2 s_y[UD_TH];          // (y, y*y) of the tile's rows
@@ -119,10 +163,9 @@ __global__ void __launch_bounds__(UD_TW) k_undistort_u8(const L3DUndistImage* __
     }
     __syncthreads();
     if (j >= d.width) return;
-    const double x = (double)j * d.ir0 + d.ir2;
     const int rows = min(UD_TH, d.height - i0);
-    if (d.channels == 3) ud_tile_rows<3>(d, j, i0, rows, x, x * x, s_y);
-    else ud_tile_rows<1>(d, j, i0, rows, x, x * x, s_y);
+    if (d.channels == 3) ud_tile_rows<KIND, 3>(d, j, i0, rows, s_y);
+    else ud_tile_rows<KIND, 1>(d, j, i0, rows, s_y);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -141,10 +184,13 @@ static int ud_check(l3d_ctx* c, const l3d_undistort_desc& u, bool image, bool ca
     }
     if (camera) {
         if (!std::isfinite(u.fx) || !std::isfinite(u.fy) || u.fx == 0.0 || u.fy == 0.0) return bad("fx and fy must be finite and non-zero");
-        bool finite = std::isfinite(u.cx) && std::isfinite(u.cy);
-        for (int k = 0; k < 3; ++k) finite = finite && std::isfinite(u.radial[k]);
-        for (int k = 0; k < 2; ++k) finite = finite && std::isfinite(u.tangential[k]);
+        bool finite = std::isfinite(u.cx) && std::isfinite(u.cy), zero = true;
+        for (int k = 0; k < 3; ++k) { finite = finite && std::isfinite(u.radial[k]) && std::isfinite(u.rational[k]); zero = zero && u.radial[k] == 0.0 && u.rational[k] == 0.0; }
+        for (int k = 0; k < 2; ++k) { finite = finite && std::isfinite(u.tangential[k]); zero = zero && u.tangential[k] == 0.0; }
+        for (int k = 0; k < 4; ++k) finite = finite && std::isfinite(u.fisheye[k]);
         if (!finite) return bad("principal point and coefficients must be finite");
+        if (u.model != L3D_LENS_RADTAN && u.model != L3D_LENS_FISHEYE) return bad("unknown lens model");
+        if (u.model == L3D_LENS_FISHEYE && !zero) return bad("a fisheye lens takes no radial, tangential or rational coefficients");
     }
     return L3D_OK;
 }
@@ -160,10 +206,50 @@ static L3DUndistImage ud_image(const l3d_undistort_desc& u, const unsigned char*
     const double det = u.fx * u.fy, id = 1.0 / det;
     d.ir0 = u.fy * id; d.ir2 = -(u.cx * u.fy) * id; d.ir4 = u.fx * id; d.ir5 = -(u.fx * u.cy) * id;
     d.fx = u.fx; d.fy = u.fy; d.cx = u.cx; d.cy = u.cy;
+    if (u.model == L3D_LENS_FISHEYE) {
+        d.kind = UD_FISHEYE;
+        d.k1 = u.fisheye[0]; d.k2 = u.fisheye[1]; d.k3 = u.fisheye[2]; d.k4 = u.fisheye[3];
+        return d;
+    }
     d.k1 = u.radial[0]; d.k2 = u.radial[1]; d.k3 = u.radial[2]; d.p1 = u.tangential[0]; d.p2 = u.tangential[1];
+    d.k4 = u.rational[0]; d.k5 = u.rational[1]; d.k6 = u.rational[2];
     d.full_radial = d.k2 != 0.0 || d.k3 != 0.0;
     d.tangential = d.p1 != 0.0 || d.p2 != 0.0;
+    d.kind = d.k4 != 0.0 || d.k5 != 0.0 || d.k6 != 0.0 ? UD_RATIONAL : UD_RADTAN;
     return d;
+}
+
+// The column tables of the fisheye images among imgs[0, n): x_0 = ir2, x_{j+1} = x_j + ir0, summed in order as OpenCV's loop does.
+// Images whose (ir0, ir2) agree share one table (its prefixes are the same), as long as the widest of them.  Sets every fisheye
+// image's xcol; the tables are uploaded on the context's stream.
+static int ud_column_tables(l3d_ctx* c, UndistortState& s, L3DUndistImage* imgs, int n)
+{
+    struct Key { double ir0, ir2; int width; size_t off; };
+    std::vector<Key> keys;
+    std::vector<int> which(n, -1);
+    for (int i = 0; i < n; ++i) {
+        if (imgs[i].kind != UD_FISHEYE) continue;
+        size_t k = 0;
+        while (k < keys.size() && !(keys[k].ir0 == imgs[i].ir0 && keys[k].ir2 == imgs[i].ir2)) ++k;
+        if (k == keys.size()) keys.push_back(Key{imgs[i].ir0, imgs[i].ir2, 0, 0});
+        keys[k].width = std::max(keys[k].width, imgs[i].width);
+        which[i] = (int)k;
+    }
+    if (keys.empty()) return L3D_OK;
+    size_t total = 0;
+    for (Key& k : keys) { k.off = total; total += (size_t)k.width; }
+    s.h_cols.resize(total);
+    for (const Key& k : keys) {
+        double x = k.ir2;
+        for (int j = 0; j < k.width; ++j) { s.h_cols[k.off + j] = x; x = x + k.ir0; }
+    }
+    int rc;
+    L3D_RESERVE(s.d_cols, sizeof(double) * total, "fisheye column tables");
+    // pageable host memory: staged before the call returns, like the descriptors
+    L3D_CUDA(c, cudaMemcpyAsync(s.d_cols.p, s.h_cols.data(), sizeof(double) * total, cudaMemcpyHostToDevice, c->stream), "upload column tables");
+    for (int i = 0; i < n; ++i)
+        if (which[i] >= 0) imgs[i].xcol = (const double*)s.d_cols.p + keys[which[i]].off;
+    return L3D_OK;
 }
 
 static dim3 ud_grid(const l3d_undistort_desc& u) { return dim3((unsigned)((u.width + UD_TW - 1) / UD_TW), (unsigned)u.height); }
@@ -189,7 +275,6 @@ int l3d_undistort_u8(l3d_ctx* c, int n, const l3d_undistort_desc* descs, int on_
         L3D_RESERVE(s.d_dst, staged, "undistort output staging");
     }
     s.h_imgs.resize(n);
-    long long tiles = 0;
     size_t off = 0;
     for (int i = 0; i < n; ++i) {
         const l3d_undistort_desc& u = descs[i];
@@ -201,16 +286,31 @@ int l3d_undistort_u8(l3d_ctx* c, int n, const l3d_undistort_desc* descs, int on_
             s.h_imgs[i] = ud_image(u, src, row, (unsigned char*)s.d_dst.p + off, row);
             off += (size_t)row * u.height;
         }
-        s.h_imgs[i].tile0 = tiles;
-        tiles += (long long)s.h_imgs[i].tiles_x * ((u.height + UD_TH - 1) / UD_TH);
     }
-    if (tiles >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_undistort_u8: more than 2^31 tiles in one call");
+    // the images grouped by lens kind: one grid per kind, each numbering its tiles from 0
+    std::stable_sort(s.h_imgs.begin(), s.h_imgs.end(), [](const L3DUndistImage& a, const L3DUndistImage& b) { return a.kind < b.kind; });
+    long long tiles[UD_KINDS] = {};
+    int first[UD_KINDS + 1] = {};
+    for (int i = 0; i < n; ++i) {
+        L3DUndistImage& d = s.h_imgs[i];
+        d.tile0 = tiles[d.kind];
+        tiles[d.kind] += (long long)d.tiles_x * ((d.height + UD_TH - 1) / UD_TH);
+        if (tiles[d.kind] >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_undistort_u8: more than 2^31 tiles in one call");
+        first[d.kind + 1] = i + 1;
+    }
+    for (int k = 1; k <= UD_KINDS; ++k) first[k] = std::max(first[k], first[k - 1]);
+    if ((rc = ud_column_tables(c, s, s.h_imgs.data(), n))) return rc;
     L3D_RESERVE(s.d_imgs, sizeof(L3DUndistImage) * (size_t)n, "undistort descriptors");
     // pageable host memory: the copy is staged before the call returns, so h_imgs may be rewritten by the next call right away
     L3D_CUDA(c, cudaMemcpyAsync(s.d_imgs.p, s.h_imgs.data(), sizeof(L3DUndistImage) * n, cudaMemcpyHostToDevice, c->stream), "upload descriptors");
-    k_undistort_u8<<<(unsigned int)tiles, UD_TW, 0, c->stream>>>((const L3DUndistImage*)s.d_imgs.p, n);
-    ++c->launches;
-    L3D_CUDA(c, cudaGetLastError(), "k_undistort_u8");
+    const L3DUndistImage* d_imgs = (const L3DUndistImage*)s.d_imgs.p;
+    void (*const kernels[UD_KINDS])(const L3DUndistImage*, int) = {k_undistort_u8<UD_RADTAN>, k_undistort_u8<UD_RATIONAL>, k_undistort_u8<UD_FISHEYE>};
+    for (int k = 0; k < UD_KINDS; ++k) {
+        if (first[k + 1] == first[k]) continue;
+        kernels[k]<<<(unsigned int)tiles[k], UD_TW, 0, c->stream>>>(d_imgs + first[k], first[k + 1] - first[k]);
+        ++c->launches;
+        L3D_CUDA(c, cudaGetLastError(), "k_undistort_u8");
+    }
     if (!on_device) {
         off = 0;
         for (int i = 0; i < n; ++i) {
@@ -241,7 +341,11 @@ int l3d_undistort_map(l3d_ctx* c, const l3d_undistort_desc* desc, int16_t* map_x
         L3D_RESERVE(s.d_map_frac, 2 * px, "undistort map fractions");
         xy = (short2*)s.d_map_xy.p; fr = (unsigned short*)s.d_map_frac.p;
     }
-    k_undistort_map<<<ud_grid(*desc), UD_TW, 0, c->stream>>>(ud_image(*desc, nullptr, 0, nullptr, 0), xy, fr);
+    L3DUndistImage d = ud_image(*desc, nullptr, 0, nullptr, 0);
+    if ((rc = ud_column_tables(c, s, &d, 1))) return rc;
+    void (*const kernels[UD_KINDS])(L3DUndistImage, short2*, unsigned short*) = {k_undistort_map<UD_RADTAN>, k_undistort_map<UD_RATIONAL>,
+                                                                                 k_undistort_map<UD_FISHEYE>};
+    kernels[d.kind]<<<ud_grid(*desc), UD_TW, 0, c->stream>>>(d, xy, fr);
     ++c->launches;
     L3D_CUDA(c, cudaGetLastError(), "k_undistort_map");
     if (!on_device) {

@@ -1043,6 +1043,15 @@ Matrix3d Line3D::rotationFromQ(const double Qw, const double Qx, const double Qy
 
 void Line3D::undistortImage(const Image8u& in, Image8u& out, const Vector3d& radial, const Vector2d& tangential, const Matrix3d& K)
 {
+    LensDistortion lens;
+    std::memset(&lens, 0, sizeof(lens));
+    lens.model = LensDistortion::RADTAN;
+    lens.k[0] = radial.x; lens.k[1] = radial.y; lens.k[2] = radial.z; lens.p[0] = tangential.x; lens.p[1] = tangential.y;
+    undistortImage(in, out, lens, K);
+}
+
+void Line3D::undistortImage(const Image8u& in, Image8u& out, const LensDistortion& lens, const Matrix3d& K)
+{
     if (in.data.size() != (size_t)in.rows * in.cols * in.channels || in.rows < 0 || in.cols < 0)
         throw std::invalid_argument("undistortImage: the pixel buffer does not match rows x cols x channels");
     int dev = 0;
@@ -1056,8 +1065,14 @@ void Line3D::undistortImage(const Image8u& in, Image8u& out, const Vector3d& rad
     d.src_pitch = d.dst_pitch = (int64_t)in.cols * in.channels;
     d.src = in.data.data(); d.dst = res.data.data();
     d.fx = K(0, 0); d.fy = K(1, 1); d.cx = K(0, 2); d.cy = K(1, 2);
-    d.radial[0] = radial.x; d.radial[1] = radial.y; d.radial[2] = radial.z;
-    d.tangential[0] = tangential.x; d.tangential[1] = tangential.y;
+    d.model = lens.model;
+    d.tangential[0] = lens.p[0]; d.tangential[1] = lens.p[1];
+    if (lens.model == LensDistortion::FISHEYE) {   // k[4], k[5] go where l3d_undistort_u8 rejects them if nonzero
+        for (int k = 0; k < 4; ++k) d.fisheye[k] = lens.k[k];
+        d.radial[0] = lens.k[4]; d.radial[1] = lens.k[5];
+    } else {
+        for (int k = 0; k < 3; ++k) { d.radial[k] = lens.k[k]; d.rational[k] = lens.k[3 + k]; }
+    }
     const int rc = l3d_undistort_u8(ctx, 1, &d, 0);
     const std::string msg = std::string("undistortImage: ") + l3d_last_error(ctx);
     l3d_ctx_destroy(ctx);
@@ -1272,6 +1287,26 @@ int l3dpp_undistort_image(const unsigned char* src, unsigned char* dst, int rows
     Matrix3d Km; memcpy(Km.m, K, 72);
     try {
         Line3D::undistortImage(in, out, Vector3d(radial[0], radial[1], radial[2]), Vector2d(tangential[0], tangential[1]), Km);
+    } catch (const std::invalid_argument&) { return -1; } catch (const std::exception&) { return -2; }
+    memcpy(dst, out.data.data(), out.data.size());
+    return 0;
+}
+// the LensDistortion overload on CUDA device `device` (the thread's current device is restored); lens = model, k[6], p[2] as 9 doubles
+int l3dpp_undistort_image_lens(const unsigned char* src, unsigned char* dst, int rows, int cols, int channels, const double* lens9, const double* K,
+                               int device)
+{
+    int prev = 0;
+    if (cudaGetDevice(&prev) != cudaSuccess || cudaSetDevice(device) != cudaSuccess) return -2;
+    struct Restore { int d; ~Restore() { cudaSetDevice(d); } } restore{prev};
+    Image8u in(rows, cols, channels), out;
+    if (!in.data.empty()) memcpy(in.data.data(), src, in.data.size());
+    Matrix3d Km; memcpy(Km.m, K, 72);
+    LensDistortion lens;
+    lens.model = (int)lens9[0];
+    for (int k = 0; k < 6; ++k) lens.k[k] = lens9[1 + k];
+    lens.p[0] = lens9[7]; lens.p[1] = lens9[8];
+    try {
+        Line3D::undistortImage(in, out, lens, Km);
     } catch (const std::invalid_argument&) { return -1; } catch (const std::exception&) { return -2; }
     memcpy(dst, out.data.data(), out.data.size());
     return 0;

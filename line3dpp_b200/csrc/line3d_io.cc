@@ -1,11 +1,15 @@
-// line3d_io.cc — .nvm reader for frontends built on include/line3d.h (restates main_vsfm.cpp:143-310; host only)
+// line3d_io.cc — .nvm, Bundler and COLMAP (text and binary) readers for frontends built on include/line3d.h (restates main_vsfm.cpp:143-310,
+// main_bundler.cpp, main_colmap.cpp; host only)
 #include "../../include/line3d_io.h"
+#include "l3d_sfm_handle.h"
 
 #include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <cstdlib>
+#include <cstdint>
 #include <fstream>
+#include <iterator>
 #include <map>
 #include <sstream>
 
@@ -139,68 +143,213 @@ bool readBundler(const std::string& bundle_file, const std::string& image_list_f
     return true;
 }
 
-bool readColmap(const std::string& folder, std::vector<SfMCamera>& cams, std::string* error)
+// COLMAP's camera models (colmap/sensor/models.h): name, model_id, number of parameters.  `lens` 0: not undistortable here (rejected),
+// 1: radtan, 2: fisheye.
+struct ColmapModel { const char* name; int id, num_params, lens; };
+static const ColmapModel kColmapModels[] = {
+    {"SIMPLE_PINHOLE", 0, 3, 1}, {"PINHOLE", 1, 4, 1}, {"SIMPLE_RADIAL", 2, 4, 1}, {"RADIAL", 3, 5, 1}, {"OPENCV", 4, 8, 1},
+    {"OPENCV_FISHEYE", 5, 8, 2}, {"FULL_OPENCV", 6, 12, 1}, {"FOV", 7, 5, 0}, {"SIMPLE_RADIAL_FISHEYE", 8, 4, 2}, {"RADIAL_FISHEYE", 9, 5, 2},
+    {"THIN_PRISM_FISHEYE", 10, 12, 0}, {"RAD_TAN_THIN_PRISM_FISHEYE", 11, 16, 0},
+};
+
+struct ColmapIntr { Matrix3d K; double radial[3], tangential[2]; LensDistortion lens; };
+
+// K, the radial / tangential pair of main_colmap.cpp:160-234 and the full lens of one camera from its parameters in COLMAP's order
+static bool colmap_intrinsics(const ColmapModel* m, const std::string& model, unsigned int cam, const double* q, bool want_lens, ColmapIntr& in,
+                              std::string* error)
+{
+    if (!m || m->lens == 0) { if (error) *error = "camera model " + model + " unknown! (camera " + std::to_string(cam) + ")"; return false; }
+    if (m->lens == 2 && !want_lens) {
+        if (error) *error = "camera " + std::to_string(cam) + " uses the fisheye model " + model + ": its distortion has no place in radial / tangential, "
+                            "read the model with the lenses argument of readColmap";
+        return false;
+    }
+    double fx = 0, fy = 0, cx = 0, cy = 0;
+    std::memset(&in.lens, 0, sizeof(in.lens));
+    double* k = in.lens.k; double* p = in.lens.p;
+    switch (m->id) {
+    case 0: fx = fy = q[0]; cx = q[1]; cy = q[2]; break;                                                     // f cx cy
+    case 1: fx = q[0]; fy = q[1]; cx = q[2]; cy = q[3]; break;                                               // fx fy cx cy
+    case 2: fx = fy = q[0]; cx = q[1]; cy = q[2]; k[0] = q[3]; break;                                        // f cx cy k
+    case 3: fx = fy = q[0]; cx = q[1]; cy = q[2]; k[0] = q[3]; k[1] = q[4]; break;                           // f cx cy k1 k2
+    case 4: fx = q[0]; fy = q[1]; cx = q[2]; cy = q[3]; k[0] = q[4]; k[1] = q[5]; p[0] = q[6]; p[1] = q[7]; break;   // .. k1 k2 p1 p2
+    case 6: fx = q[0]; fy = q[1]; cx = q[2]; cy = q[3]; k[0] = q[4]; k[1] = q[5]; p[0] = q[6]; p[1] = q[7];          // .. k3 k4 k5 k6
+        k[2] = q[8]; k[3] = q[9]; k[4] = q[10]; k[5] = q[11]; break;
+    case 5: fx = q[0]; fy = q[1]; cx = q[2]; cy = q[3]; for (int j = 0; j < 4; ++j) k[j] = q[4 + j]; break;  // fx fy cx cy k1..k4
+    case 8: fx = fy = q[0]; cx = q[1]; cy = q[2]; k[0] = q[3]; break;                                        // f cx cy k
+    case 9: fx = fy = q[0]; cx = q[1]; cy = q[2]; k[0] = q[3]; k[1] = q[4]; break;                           // f cx cy k1 k2
+    }
+    in.lens.model = m->lens == 2 ? LensDistortion::FISHEYE : LensDistortion::RADTAN;
+    std::memset(in.K.m, 0, sizeof(in.K.m));
+    in.K(0, 0) = fx; in.K(0, 2) = cx; in.K(1, 1) = fy; in.K(1, 2) = cy; in.K(2, 2) = 1.0;
+    const bool radtan = m->lens == 1;                                   // FULL_OPENCV's k4..k6 only reach the lens (main_colmap.cpp:210)
+    in.radial[0] = radtan ? k[0] : 0.0; in.radial[1] = radtan ? k[1] : 0.0; in.radial[2] = radtan ? k[2] : 0.0;
+    in.tangential[0] = radtan ? p[0] : 0.0; in.tangential[1] = radtan ? p[1] : 0.0;
+    return true;
+}
+
+// bounds-checked little-endian reads of one COLMAP binary file, loaded whole (its size bounds every allocation)
+struct ColmapBin {
+    std::string path;
+    std::vector<unsigned char> b;
+    size_t pos = 0;
+    std::string* error;
+    bool fail(const std::string& why) { if (error) *error = path + ": " + why; return false; }
+    bool open()
+    {
+        std::ifstream f(path.c_str(), std::ios::binary);
+        if (!f) return fail("cannot open");
+        b.assign(std::istreambuf_iterator<char>(f), std::istreambuf_iterator<char>());
+        return true;
+    }
+    template <class T> bool get(T& v, const char* what)
+    {
+        if (b.size() - pos < sizeof(T)) return fail(std::string("truncated at byte ") + std::to_string(pos) + " (" + what + ")");
+        std::memcpy(&v, b.data() + pos, sizeof(T)); pos += sizeof(T);
+        return true;
+    }
+    bool skip(size_t n, const char* what)
+    {
+        if (b.size() - pos < n) return fail(std::string("truncated at byte ") + std::to_string(pos) + " (" + what + ")");
+        pos += n;
+        return true;
+    }
+    // a record count: each record takes at least min_bytes, so a count the rest of the file cannot hold is malformed
+    bool count(uint64_t& n, size_t min_bytes, const char* what)
+    {
+        if (!get(n, what)) return false;
+        if (n > (b.size() - pos) / min_bytes) return fail(std::string(what) + " " + std::to_string(n) + " exceeds what the file holds");
+        return true;
+    }
+    bool name(std::string& s)
+    {
+        const void* z = std::memchr(b.data() + pos, 0, b.size() - pos);
+        if (!z) return fail("unterminated image name at byte " + std::to_string(pos));
+        const size_t n = (const unsigned char*)z - (b.data() + pos);
+        s.assign((const char*)b.data() + pos, n); pos += n + 1;
+        return true;
+    }
+    bool id32(uint64_t v, unsigned int& out, const char* what)
+    {
+        if (v > 0xFFFFFFFFull) return fail(std::string(what) + " " + std::to_string(v) + " does not fit unsigned int");
+        out = (unsigned int)v;
+        return true;
+    }
+};
+
+static bool file_exists(const std::string& p) { std::ifstream f(p.c_str()); return (bool)f; }
+
+bool readColmap(const std::string& folder, std::vector<SfMCamera>& cams, std::string* error, std::vector<LensDistortion>* lenses)
 {
     cams.clear();
-    std::ifstream fc((folder + "/cameras.txt").c_str()), fi((folder + "/images.txt").c_str()), fp((folder + "/points3D.txt").c_str());
-    if (!fc || !fi || !fp) { if (error) *error = "at least one of the colmap result files does not exist in sfm folder: " + folder; return false; }
-    struct Intr { Matrix3d K; double radial[3], tangential[2]; };
-    std::map<unsigned int, Intr> intr;
-    std::string line;
-    while (std::getline(fc, line)) {             // main_colmap.cpp:160-234
-        if (line.empty() || line[0] == '#') continue;
-        std::stringstream s(line);
-        unsigned int cam = 0, w = 0, h = 0; std::string model;
-        s >> cam >> model >> w >> h;
-        double fx = 0, fy = 0, cx = 0, cy = 0, k1 = 0, k2 = 0, k3 = 0, p1 = 0, p2 = 0;
-        if (model == "SIMPLE_PINHOLE") { s >> fx >> cx >> cy; fy = fx; }
-        else if (model == "PINHOLE") s >> fx >> fy >> cx >> cy;
-        else if (model == "SIMPLE_RADIAL") { s >> fx >> cx >> cy >> k1; fy = fx; }
-        else if (model == "RADIAL") { s >> fx >> cx >> cy >> k1 >> k2; fy = fx; }
-        else if (model == "OPENCV") s >> fx >> fy >> cx >> cy >> k1 >> k2 >> p1 >> p2;
-        else if (model == "FULL_OPENCV") s >> fx >> fy >> cx >> cy >> k1 >> k2 >> p1 >> p2 >> k3;
-        else { if (error) *error = "camera model " + model + " unknown!"; return false; }
-        Intr in; std::memset(in.K.m, 0, sizeof(in.K.m));
-        in.K(0, 0) = fx; in.K(0, 2) = cx; in.K(1, 1) = fy; in.K(1, 2) = cy; in.K(2, 2) = 1.0;
-        in.radial[0] = k1; in.radial[1] = k2; in.radial[2] = k3; in.tangential[0] = p1; in.tangential[1] = p2;
-        intr[cam] = in;
-    }
-    std::map<unsigned int, Vector3d> wps;        // world points referenced by a kept image; (0,0,0) until points3D.txt fills them in
-    bool first = true, keep = false;
-    while (std::getline(fi, line)) {             // main_colmap.cpp:252-321: two lines per image
-        if (!line.empty() && line[0] == '#') continue;
-        std::stringstream s(line);
-        if (first) {
-            unsigned int img = 0, cam = 0; double qw = 1, qx = 0, qy = 0, qz = 0, tx = 0, ty = 0, tz = 0; std::string name;
-            s >> img >> qw >> qx >> qy >> qz >> tx >> ty >> tz >> cam >> name;
-            keep = intr.count(cam) != 0;
-            if (keep) {
-                SfMCamera c;
-                c.id = img; c.image = name; c.has_K = true; c.K = intr[cam].K; c.focal = 0.0f; c.median_depth = 0.0f;
-                for (int k = 0; k < 3; ++k) c.radial[k] = intr[cam].radial[k];
-                c.tangential[0] = intr[cam].tangential[0]; c.tangential[1] = intr[cam].tangential[1];
-                c.R = Line3D::rotationFromQ(qw, qx, qy, qz); c.t = Vector3d(tx, ty, tz); c.C = center_of(c.R, c.t);
-                cams.push_back(c);
-            }
-            first = false;
-        } else {
-            if (keep) {
-                double x, y; std::string id;
-                while (s >> x >> y >> id) {
-                    const int wp = std::atoi(id.c_str());
-                    if (wp >= 0) { cams.back().worldpoints.push_back((unsigned int)wp); wps[(unsigned int)wp] = Vector3d(0, 0, 0); }
-                }
-            }
-            first = true;
+    if (lenses) lenses->clear();
+    const bool text = file_exists(folder + "/cameras.txt") && file_exists(folder + "/images.txt") && file_exists(folder + "/points3D.txt");
+    const bool binary = file_exists(folder + "/cameras.bin") && file_exists(folder + "/images.bin") && file_exists(folder + "/points3D.bin");
+    if (!text && !binary) { if (error) *error = "at least one of the colmap result files does not exist in sfm folder: " + folder; return false; }
+    std::map<unsigned int, ColmapIntr> intr;
+    std::map<unsigned int, Vector3d> wps;        // world points referenced by a kept image; (0,0,0) until points3D fills them in
+    // one image of images.txt / .bin: kept (and its camera's lens recorded) when its camera is known
+    auto add_image = [&](unsigned int img, double qw, double qx, double qy, double qz, double tx, double ty, double tz, unsigned int cam,
+                         const std::string& name) {
+        std::map<unsigned int, ColmapIntr>::const_iterator it = intr.find(cam);
+        if (it == intr.end()) return false;
+        SfMCamera c;
+        c.id = img; c.image = name; c.has_K = true; c.K = it->second.K; c.focal = 0.0f; c.median_depth = 0.0f;
+        for (int k = 0; k < 3; ++k) c.radial[k] = it->second.radial[k];
+        c.tangential[0] = it->second.tangential[0]; c.tangential[1] = it->second.tangential[1];
+        c.R = Line3D::rotationFromQ(qw, qx, qy, qz); c.t = Vector3d(tx, ty, tz); c.C = center_of(c.R, c.t);
+        cams.push_back(c);
+        if (lenses) lenses->push_back(it->second.lens);
+        return true;
+    };
+    auto add_observation = [&](unsigned int wp) { cams.back().worldpoints.push_back(wp); wps[wp] = Vector3d(0, 0, 0); };
+    if (text) {
+        std::ifstream fc((folder + "/cameras.txt").c_str()), fi((folder + "/images.txt").c_str()), fp((folder + "/points3D.txt").c_str());
+        std::string line;
+        while (std::getline(fc, line)) {         // main_colmap.cpp:160-234
+            if (line.empty() || line[0] == '#') continue;
+            std::stringstream s(line);
+            unsigned int cam = 0, w = 0, h = 0; std::string model;
+            s >> cam >> model >> w >> h;
+            const ColmapModel* m = nullptr;
+            for (const ColmapModel& e : kColmapModels) if (model == e.name) m = &e;
+            double q[16] = {0};
+            for (int k = 0; m && k < m->num_params; ++k) s >> q[k];
+            ColmapIntr in;
+            if (!colmap_intrinsics(m, model, cam, q, lenses != nullptr, in, error)) return false;
+            intr[cam] = in;
         }
-    }
-    while (std::getline(fp, line)) {             // main_colmap.cpp:330-349
-        if (line.empty() || line[0] == '#') continue;
-        std::stringstream s(line);
-        unsigned int id = 0; double X = 0, Y = 0, Z = 0;
-        s >> id >> X >> Y >> Z;
-        std::map<unsigned int, Vector3d>::iterator it = wps.find(id);
-        if (s && it != wps.end()) it->second = Vector3d(X, Y, Z);
+        bool first = true, keep = false;
+        while (std::getline(fi, line)) {         // main_colmap.cpp:252-321: two lines per image
+            if (!line.empty() && line[0] == '#') continue;
+            std::stringstream s(line);
+            if (first) {
+                unsigned int img = 0, cam = 0; double qw = 1, qx = 0, qy = 0, qz = 0, tx = 0, ty = 0, tz = 0; std::string name;
+                s >> img >> qw >> qx >> qy >> qz >> tx >> ty >> tz >> cam >> name;
+                keep = add_image(img, qw, qx, qy, qz, tx, ty, tz, cam, name);
+                first = false;
+            } else {
+                if (keep) {
+                    double x, y; std::string id;
+                    while (s >> x >> y >> id) {
+                        const int wp = std::atoi(id.c_str());
+                        if (wp >= 0) add_observation((unsigned int)wp);
+                    }
+                }
+                first = true;
+            }
+        }
+        while (std::getline(fp, line)) {         // main_colmap.cpp:330-349
+            if (line.empty() || line[0] == '#') continue;
+            std::stringstream s(line);
+            unsigned int id = 0; double X = 0, Y = 0, Z = 0;
+            s >> id >> X >> Y >> Z;
+            std::map<unsigned int, Vector3d>::iterator it = wps.find(id);
+            if (s && it != wps.end()) it->second = Vector3d(X, Y, Z);
+        }
+    } else {                                     // COLMAP's binary model (colmap/scene/reconstruction_io.cc), little-endian
+        ColmapBin fc{folder + "/cameras.bin", {}, 0, error}, fi{folder + "/images.bin", {}, 0, error}, fp{folder + "/points3D.bin", {}, 0, error};
+        if (!fc.open() || !fi.open() || !fp.open()) return false;
+        uint64_t n = 0;
+        if (!fc.count(n, 24, "camera count")) return false;
+        for (uint64_t i = 0; i < n; ++i) {       // u32 camera_id, i32 model_id, u64 width, u64 height, f64 params[num_params]
+            uint32_t cam = 0; int32_t mid = 0; uint64_t w = 0, h = 0;
+            if (!fc.get(cam, "camera_id") || !fc.get(mid, "model_id") || !fc.get(w, "width") || !fc.get(h, "height")) return false;
+            const ColmapModel* m = nullptr;
+            for (const ColmapModel& e : kColmapModels) if (mid == e.id) m = &e;
+            if (!m) return fc.fail("camera model id " + std::to_string(mid) + " of camera " + std::to_string(cam) + " unknown!");
+            double q[16] = {0};
+            for (int k = 0; k < m->num_params; ++k) if (!fc.get(q[k], "camera parameters")) return false;
+            ColmapIntr in;
+            if (!colmap_intrinsics(m, m->name, cam, q, lenses != nullptr, in, error)) return false;
+            intr[cam] = in;
+        }
+        if (!fi.count(n, 4 + 56 + 4 + 1 + 8, "image count")) return false;
+        for (uint64_t i = 0; i < n; ++i) {       // u32 image_id, f64 qw qx qy qz tx ty tz, u32 camera_id, name\0, u64 n2d, n2d x (f64 x, f64 y, u64 id)
+            uint32_t img = 0, cam = 0; double v[7]; std::string name; uint64_t n2d = 0;
+            if (!fi.get(img, "image_id")) return false;
+            for (int k = 0; k < 7; ++k) if (!fi.get(v[k], "image pose")) return false;
+            if (!fi.get(cam, "camera_id") || !fi.name(name) || !fi.count(n2d, 24, "point count")) return false;
+            const bool keep = add_image(img, v[0], v[1], v[2], v[3], v[4], v[5], v[6], cam, name);
+            for (uint64_t j = 0; j < n2d; ++j) {
+                uint64_t id = 0;
+                if (!fi.skip(16, "point xy") || !fi.get(id, "point3D_id")) return false;
+                unsigned int wp = 0;
+                if (id == ~0ull) continue;       // no 3D point (-1 in images.txt)
+                if (!fi.id32(id, wp, "point3D_id")) return false;
+                if (keep) add_observation(wp);
+            }
+        }
+        if (!fp.count(n, 8 + 24 + 3 + 8 + 8, "point count")) return false;
+        for (uint64_t i = 0; i < n; ++i) {       // u64 id, f64 xyz, u8 rgb, f64 error, u64 track_len, track_len x (u32 image_id, u32 point2D_idx)
+            uint64_t id = 0, track = 0; double X = 0, Y = 0, Z = 0;
+            unsigned int wp = 0;
+            if (!fp.get(id, "point3D_id") || !fp.id32(id, wp, "point3D_id") || !fp.get(X, "xyz") || !fp.get(Y, "xyz") || !fp.get(Z, "xyz") ||
+                !fp.skip(3 + 8, "colour and error") || !fp.count(track, 8, "track length") || !fp.skip(8 * (size_t)track, "track"))
+                return false;
+            std::map<unsigned int, Vector3d>::iterator it = wps.find(wp);
+            if (it != wps.end()) it->second = Vector3d(X, Y, Z);
+        }
     }
     for (size_t i = 0; i < cams.size(); ++i) {   // main_colmap.cpp:386-401
         std::vector<float> d;
@@ -211,7 +360,7 @@ bool readColmap(const std::string& folder, std::vector<SfMCamera>& cams, std::st
         }
         cams[i].median_depth = median_of(d);
     }
-    if (cams.empty()) { if (error) *error = "no usable image in " + folder; return false; }
+    if (cams.empty()) { if (lenses) lenses->clear(); if (error) *error = "no usable image in " + folder; return false; }
     return true;
 }
 
@@ -254,20 +403,30 @@ int l3dpp_nvm_worldpoints(void* h, int i, unsigned int* out, int cap)
     for (unsigned int w : v[i].worldpoints) { if (n < cap) out[n] = w; ++n; }
     return n;
 }
-void* l3dpp_sfm_open(int kind /*0 bundler, 1 colmap*/, const char* path, const char* aux, char* err, int errcap)
+void* l3dpp_sfm_open(int kind /*0 bundler, 1 colmap, 5 colmap with lenses*/, const char* path, const char* aux, char* err, int errcap)
 {
-    std::vector<L3DPP::SfMCamera>* v = new std::vector<L3DPP::SfMCamera>();
+    L3DSfMHandle* v = new L3DSfMHandle();
     std::string e;
-    const bool ok = kind == 0 ? L3DPP::readBundler(path, aux ? aux : "", *v, &e) : L3DPP::readColmap(path, *v, &e);
+    const bool ok = kind == 0 ? L3DPP::readBundler(path, aux ? aux : "", v->cams, &e)
+                              : L3DPP::readColmap(path, v->cams, &e, kind == 5 ? &v->lenses : nullptr);
     if (!ok) { if (err && errcap > 0) { std::strncpy(err, e.c_str(), errcap - 1); err[errcap - 1] = 0; } delete v; return nullptr; }
     return v;
 }
-void l3dpp_sfm_close(void* h) { delete (std::vector<L3DPP::SfMCamera>*)h; }
-int l3dpp_sfm_num_cameras(void* h) { return (int)((std::vector<L3DPP::SfMCamera>*)h)->size(); }
-/* out: id, has_K, focal, median_depth, num_wps as 5 doubles; K R 9 each; t C 3 each; dist = radial[3] + tangential[2] */
+void l3dpp_sfm_close(void* h) { delete (L3DSfMHandle*)h; }
+int l3dpp_sfm_num_cameras(void* h) { return (int)((L3DSfMHandle*)h)->cams.size(); }
+/* lens of camera i as model, k[6], p[2] (9 doubles); -1 when i is out of range or the model was read without lenses */
+int l3dpp_sfm_lens(void* h, int i, double* lens9)
+{
+    const std::vector<L3DPP::LensDistortion>& v = ((L3DSfMHandle*)h)->lenses;
+    if (i < 0 || i >= (int)v.size()) return -1;
+    lens9[0] = v[i].model;
+    for (int k = 0; k < 6; ++k) lens9[1 + k] = v[i].k[k];
+    lens9[7] = v[i].p[0]; lens9[8] = v[i].p[1];
+    return 0;
+}
 int l3dpp_sfm_camera(void* h, int i, double* head5, double* K9, double* R9, double* t3, double* C3, double* dist5, char* name, int namecap)
 {
-    const std::vector<L3DPP::SfMCamera>& v = *(std::vector<L3DPP::SfMCamera>*)h;
+    const std::vector<L3DPP::SfMCamera>& v = ((L3DSfMHandle*)h)->cams;
     if (i < 0 || i >= (int)v.size()) return -1;
     const L3DPP::SfMCamera& c = v[i];
     head5[0] = c.id; head5[1] = c.has_K; head5[2] = c.focal; head5[3] = c.median_depth; head5[4] = (double)c.worldpoints.size();
@@ -280,7 +439,7 @@ int l3dpp_sfm_camera(void* h, int i, double* head5, double* K9, double* R9, doub
 }
 int l3dpp_sfm_worldpoints(void* h, int i, unsigned int* out, int cap)
 {
-    const std::vector<L3DPP::SfMCamera>& v = *(std::vector<L3DPP::SfMCamera>*)h;
+    const std::vector<L3DPP::SfMCamera>& v = ((L3DSfMHandle*)h)->cams;
     if (i < 0 || i >= (int)v.size()) return -1;
     int n = 0;
     for (unsigned int w : v[i].worldpoints) { if (n < cap) out[n] = w; ++n; }

@@ -8,6 +8,7 @@
 // path and the problem; nothing is allocated beyond what the bytes read justify; JSON nesting is capped at JSON_MAX_DEPTH.
 #include "../../include/line3d_io.h"
 #include "../../include/l3d_capi.h"
+#include "l3d_sfm_handle.h"
 
 #include <algorithm>
 #include <cmath>
@@ -667,12 +668,12 @@ extern "C" {
  * GPU that triangulates) */
 void* l3dpp_sfm_read(int kind, const char* path, const char* aux, int device, char* err, int errcap)
 {
-    std::vector<L3DPP::SfMCamera>* v = new std::vector<L3DPP::SfMCamera>();
+    L3DSfMHandle* v = new L3DSfMHandle();
     std::string e;
     bool ok = false;
-    if (kind == 2) ok = L3DPP::readMavmap(path, *v, &e);
-    else if (kind == 3) ok = L3DPP::readOpenMVG(path, *v, &e);
-    else if (kind == 4) ok = L3DPP::readPix4D(path, aux ? aux : "", *v, &e, device);
+    if (kind == 2) ok = L3DPP::readMavmap(path, v->cams, &e);
+    else if (kind == 3) ok = L3DPP::readOpenMVG(path, v->cams, &e);
+    else if (kind == 4) ok = L3DPP::readPix4D(path, aux ? aux : "", v->cams, &e, device);
     else e = "unknown model kind";
     if (!ok) { if (err && errcap > 0) { std::strncpy(err, e.c_str(), errcap - 1); err[errcap - 1] = 0; } delete v; return nullptr; }
     return v;

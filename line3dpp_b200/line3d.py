@@ -331,8 +331,9 @@ def segment_cache_path(output_folder, cam, width, height, max_img_width=-1):
 
 
 # ---- SfM models (include/line3d_io.h, csrc/line3d_io.cc + csrc/line3d_sfm.cc); host only except read_pix4d, which triangulates on a GPU
-def _sfm_cameras(L, h):
-    """the cameras of an l3dpp_sfm_* handle as dicts (id, image, K, R, t, C, radial, tangential, median_depth, worldpoints); closes it"""
+def _sfm_cameras(L, h, lenses=False):
+    """the cameras of an l3dpp_sfm_* handle as dicts (id, image, K, R, t, C, radial, tangential, median_depth, worldpoints, and with
+    lenses the lens dict {model, k[6], p[2]} of L3DPP::LensDistortion); closes it"""
     p = lambda a: a.ctypes.data_as(C.c_void_p)
     cams = []
     try:
@@ -344,6 +345,11 @@ def _sfm_cameras(L, h):
             L.l3dpp_sfm_worldpoints(h, i, p(w), int(head[4]))
             cams.append(dict(id=int(head[0]), image=name.value.decode(errors="replace"), K=K.reshape(3, 3), R=R.reshape(3, 3), t=t, C=Cc,
                              radial=dist[:3].copy(), tangential=dist[3:].copy(), median_depth=np.float32(head[3]), worldpoints=w[:int(head[4])]))
+            if lenses:
+                lens = np.zeros(9)
+                if L.l3dpp_sfm_lens(h, i, p(lens)) != 0:
+                    raise capi.L3DError(f"no lens for camera {i}")
+                cams[-1]["lens"] = dict(model=int(lens[0]), k=lens[1:7].copy(), p=lens[7:9].copy())
     finally:
         L.l3dpp_sfm_close(h)
     return cams
@@ -357,6 +363,37 @@ def _read_sfm(kind, path, aux="", device=0):
     if not h:
         raise capi.L3DError(err.value.decode(errors="replace"))
     return _sfm_cameras(L, C.c_void_p(h))
+
+
+def read_colmap(sfm_folder):
+    """readColmap with lenses: the cameras of a COLMAP model (cameras/images/points3D .txt, or else .bin), each with a `lens` dict
+    {model: capi.LENS_RADTAN | capi.LENS_FISHEYE, k: k1..k6, p: p1, p2} for undistort_image.  Raises L3DError on a malformed model."""
+    L = capi.lib()
+    L.l3dpp_sfm_open.restype = C.c_void_p
+    err = C.create_string_buffer(4096)
+    h = L.l3dpp_sfm_open(5, str(sfm_folder).encode(), b"", err, 4096)
+    if not h:
+        raise capi.L3DError(err.value.decode(errors="replace"))
+    return _sfm_cameras(L, C.c_void_p(h), lenses=True)
+
+
+def undistort_image(img, K, lens, device=0):
+    """Line3D::undistortImage(in, out, lens, K) of a uint8 HxW / HxWx3 image on GPU `device`; lens as read_colmap gives it"""
+    a = np.ascontiguousarray(img, np.uint8)
+    if a.ndim not in (2, 3) or (a.ndim == 3 and a.shape[2] != 3):
+        raise ValueError("image must be uint8 HxW or HxWx3")
+    Kd = np.ascontiguousarray(K, np.float64).reshape(9)
+    k = [float(v) for v in lens.get("k", ())] + [0.0] * 6
+    pp = [float(v) for v in lens.get("p", ())] + [0.0] * 2
+    l9 = np.array([float(lens.get("model", capi.LENS_RADTAN))] + k[:6] + pp[:2], np.float64)
+    out = np.empty_like(a)
+    L = capi.lib()
+    rc = L.l3dpp_undistort_image_lens(_p(a), _p(out), a.shape[0], a.shape[1], 1 if a.ndim == 2 else 3, _p(l9), _p(Kd), int(device))
+    if rc == -1:
+        raise ValueError("undistort_image: an image or lens l3d_undistort_u8 rejects")
+    if rc != 0:
+        raise capi.L3DError("undistort_image: no usable CUDA device or a CUDA failure")
+    return out
 
 
 def read_mavmap(path):
