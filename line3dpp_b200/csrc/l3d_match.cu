@@ -12,7 +12,8 @@
 //                     pass, and a warp takes the unit's rows one at a time from a shared counter into one of its 8 row slots (constants,
 //                     key list, score-to-beat), with no CTA barrier; larger target views take several passes over units of at most 256
 //                     rows, each slot bound to one row.  Per row the warp binary-searches the
-//                     window of every arc class and scans only those entries, all windows as one concatenation (full warps): each
+//                     window of every arc class and scans only those entries, all windows as one concatenation (full warps), the
+//                     class nearest the row's own span first so that its score-to-beat rises early: each
 //                     lane runs the arc test (13 integer instructions) and the conservative float filter (27 flop + 2 rcp on the
 //                     staged target segment) on its entry, branch-free, the survivors of both are ballot-compacted into a per-warp
 //                     queue of ring positions (emptied before every refill) and evaluated 32 at a time on the staged segment with the
@@ -91,7 +92,7 @@ struct MatchSmem {
     long long src_base, toff;
     float3 Cs, Ct;
     float epi; int knn;
-    int cap;                                         // keys a row list collects before it is cut to its k best (and the score-to-beat rises); 16 instead of 32 was measured 7 % slower
+    int cap;                                         // keys a row list collects before it is cut to its k best (and the score-to-beat rises); a list holds at most cap keys, so the kNN <= 32 this kernel serves need 32 (smaller caps: sweep builds for kNN 10 only, DESIGN.md section 8)
     // REF_CPU semantics only: the exact path is matchingCPU's double arithmetic; the float filter stays the same
     const double* cache_d;
     double Fd[9]; D3 Csd, Ctd;
@@ -498,10 +499,22 @@ __device__ __forceinline__ void scan_row(MatchSmem& S, int sl, int warp, int lan
     // short arc [ka, kb] between the two kappa values: a target of class c can only match if its arc starts in [ka - 2^(CLS0 + c), kb]
     const bool fwd = (kr.y - kr.x) < 0x80000000u;
     const unsigned int ka = fwd ? kr.x : kr.y, kb = fwd ? kr.y : kr.x;
-    // lanes 0 .. 2 * NCLS - 1: lower / upper end of the window of class lane >> 1 inside the resident part of that class (binary search)
+    // Lanes 2i and 2i + 1 (i < NCLS) work on class c, the i-th class of the row's scan order.  The best overlaps come from targets
+    // whose arc is about as long as the row's own span kb - ka, so the class of that span goes first, then the classes on either
+    // side of it by distance (the smaller class first on a tie): the row's score-to-beat rises after fewer exact evaluations.  The
+    // order only changes when candidates arrive, not which of them are kept.
+    int c = min(lane >> 1, L3D_ARC_NCLS - 1);
+#if MK_SCAN_ORDER
+    {
+        const int rc = min(arc_class(kb - ka), L3D_ARC_NCLS - 1), m = min(rc, L3D_ARC_NCLS - 1 - rc);   // m classes on both sides
+        const int d = c <= 2 * m ? (c + 1) >> 1 : c - m;
+        const bool below = c <= 2 * m ? (c & 1) != 0 : 2 * rc > L3D_ARC_NCLS - 1;
+        c = below ? rc - d : rc + d;
+    }
+#endif
+    // lanes 0 .. 2 * NCLS - 1: lower / upper end of the window of class c inside the resident part of that class (binary search)
     int res = 0;
     {
-        const int c = min(lane >> 1, L3D_ARC_NCLS - 1);
         int lo = min(max(cls_off[c] - base, 0), cnt), hi = min(max(cls_off[c + 1] - base, 0), cnt);
         const bool upper = lane & 1;
         const unsigned int key = upper ? kb + 1u : ka - (1u << (L3D_ARC_CLS0 + c));
@@ -513,12 +526,11 @@ __device__ __forceinline__ void scan_row(MatchSmem& S, int sl, int warp, int lan
         }
         res = lo;
     }
-    // lane p < 2 * NCLS: piece p & 1 of the window of class p >> 1 (two pieces when the window wraps around 2^32); lane 2 * NCLS: the
-    // targets every row looks at.  A row outside the pencil model (rall) takes everything as one piece.
+    // lane p < 2 * NCLS: piece p & 1 of the window of class c (two pieces when the window wraps around 2^32); lane 2 * NCLS: the
+    // targets every row looks at, last.  A row outside the pencil model (rall) takes everything as one piece.
     int plo = 0, phi = 0;
     {
-        const int c = min(lane >> 1, L3D_ARC_NCLS - 1);
-        const int i0 = __shfl_sync(0xffffffffu, res, 2 * c), i1 = __shfl_sync(0xffffffffu, res, 2 * c + 1);
+        const int i0 = __shfl_sync(0xffffffffu, res, lane & ~1), i1 = __shfl_sync(0xffffffffu, res, lane | 1);
         const int s_c = min(max(cls_off[c] - base, 0), cnt), e_c = min(max(cls_off[c + 1] - base, 0), cnt);
         const bool wrap = ka - (1u << (L3D_ARC_CLS0 + c)) > kb;
         if (lane < 2 * L3D_ARC_NCLS) {

@@ -25,6 +25,10 @@ static_assert(MK_NSLOT <= 256, "a queue entry is (slot << 24) | ring position: 8
 #ifndef MK_CAP
 #define MK_CAP 32                       /* survivor keys kept per row before pruning to k (<= 32: one key per lane) */
 #endif
+#ifndef MK_SCAN_ORDER
+#define MK_SCAN_ORDER 1                 /* order of a row's window pieces: 1 = arc class nearest the row's own span first, 0 = class
+                                           order 0 .. NCLS - 1 (A/B builds only; the matches are the same either way) */
+#endif
 
 #define DK_THREADS 256
 #ifndef DK_MINB

@@ -1,7 +1,8 @@
 """Where the warps of k_match_topk spend their cycles, on the benchmark's workload (ring +-5, 3000 segments per view, kNN 10; the
 first V views, 5 V view pairs).
 
-    python tools/probe_match_phases.py build          # no GPU needed: line3dpp_b200/libl3d_b200_probe.so (-DL3D_MATCH_PROBE)
+    python tools/probe_match_phases.py build [O0]     # no GPU needed: line3dpp_b200/libl3d_b200_probe.so (-DL3D_MATCH_PROBE); O0:
+                                                      # libl3d_b200_probe_O0.so, window pieces in class order (MK_SCAN_ORDER=0)
     python tools/probe_match_phases.py run [V]        # on the GPU (default V = 100); L3D_LIB=<.so> runs another probe build
 
 The probe build adds clock64() spans per warp (l3d_match.cuh, MP_*); without the define none of it is compiled.  Shares are of all
@@ -56,6 +57,7 @@ def run(V):
 if __name__ == "__main__":
     if sys.argv[1] == "build":
         from line3dpp_b200 import build
-        print(build.build(defines=["L3D_MATCH_PROBE"], out=SO))
+        o0 = sys.argv[2:] == ["O0"]
+        print(build.build(defines=["L3D_MATCH_PROBE"] + (["MK_SCAN_ORDER=0"] if o0 else []), out=SO.replace(".so", "_O0.so") if o0 else SO))
     elif sys.argv[1] == "run":
         run(int(sys.argv[2]) if len(sys.argv) > 2 else 100)

@@ -10,8 +10,9 @@ import json, os, subprocess, sys
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, ROOT)
 BASE = "base"
-# warps per CTA (one CTA per SM), row slots per warp, most rows per work unit, TMA ring depth (6 x 512: 3072 resident); the base is
-# l3d_match.cuh's default: 32 warps x 8 slots, 1024-row units
+# warps per CTA (one CTA per SM), row slots per warp, most rows per work unit, TMA ring depth (6 x 512: 3072 resident), keys per row
+# before the first prune, order of a row's window pieces; the base is l3d_match.cuh's default: 32 warps x 8 slots, 1024-row units,
+# 32 keys, nearest arc class first
 VARIANTS = {
     BASE: [],
     "U512": ["MK_UNIT_ROWS=512"],
@@ -22,6 +23,9 @@ VARIANTS = {
     "W16": ["MK_WARPS=16"],
     "W24": ["MK_WARPS=24"],
     "W28": ["MK_WARPS=28"],
+    "C16": ["MK_CAP=16"],
+    "C24": ["MK_CAP=24"],
+    "O0": ["MK_SCAN_ORDER=0"],
 }
 args = sys.argv[2:]
 reps = 1
