@@ -25,7 +25,7 @@ def needs_build() -> bool:
     if not os.path.exists(OUT):
         return True
     t = os.path.getmtime(OUT)
-    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "l3d_capi.h")]
+    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", h) for h in ("l3d_capi.h", "l3dpp_capi.h")]
     return any(os.path.getmtime(d) > t for d in deps)
 
 

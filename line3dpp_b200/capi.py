@@ -1,17 +1,20 @@
-"""ctypes binding of libl3d_b200.so (include/l3d_capi.h).  Thin: no arithmetic happens in Python.
+"""ctypes binding of libl3d_b200.so (include/l3d_capi.h, include/l3dpp_capi.h).  Thin: no arithmetic happens in Python.
 
 The library is REQUIRED: importing this module builds it if the .so is missing and raises if that fails; creating a
 context raises if there is no usable CUDA device.  There is no CPU fallback anywhere in this package.
+Every function the two headers declare gets its argtypes / restype from its declaration when the library is loaded.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
+import re
 import numpy as np
 
 from . import build as _build
 
 HERE = os.path.dirname(os.path.abspath(__file__))
+HEADERS = [os.path.join(os.path.dirname(HERE), "include", h) for h in ("l3d_capi.h", "l3dpp_capi.h")]
 
 
 class ViewDesc(C.Structure):
@@ -113,17 +116,56 @@ class L3DError(RuntimeError):
     pass
 
 
+_VALUE_TYPES = {"int": C.c_int, "int32_t": C.c_int, "unsigned int": C.c_uint, "uint32_t": C.c_uint, "long long": C.c_longlong,
+                "int64_t": C.c_longlong, "size_t": C.c_size_t, "float": C.c_float, "double": C.c_double}
+
+
+def declarations(path):
+    """{name: (restype, argtypes)} of the file-scope declarations `ret name(params);` of l3d_* / l3dpp_* functions in a C header.
+    Every pointer (function-pointer typedefs of the header and `T* const*` included) is c_void_p, a `const char*` result c_char_p,
+    the other types those of _VALUE_TYPES; any other spelling raises, naming the declaration."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", open(path).read(), flags=re.S)
+    text = re.sub(r"^[ \t]*#.*$", " ", text, flags=re.M)
+    text = re.sub(r'extern\s*"C"\s*\{|\}', " ", text)
+    fn_ptrs, out = set(), {}
+
+    def c_type(spelling, decl, result=False):
+        t = " ".join(spelling.replace("*", " * ").split())
+        if result and t in ("void", "const char *"):
+            return None if t == "void" else C.c_char_p
+        if "*" in t or t in fn_ptrs:
+            return C.c_void_p
+        if t not in _VALUE_TYPES:
+            raise L3DError(f"{os.path.basename(path)}: no ctypes type for `{spelling}` in `{decl};`")
+        return _VALUE_TYPES[t]
+
+    for decl in (" ".join(s.split()) for s in text.split(";")):
+        if decl.startswith("typedef"):
+            fn_ptrs.update(re.findall(r"\(\s*\*\s*(\w+)\s*\)\s*\(", decl))
+        elif re.search(r"\bl3d(pp)?_\w+\s*\(", decl):
+            m = re.fullmatch(r"([\w ]+?\**) ?(l3d(?:pp)?_\w+) ?\(([^()]*)\)", decl)
+            if m is None:
+                raise L3DError(f"{os.path.basename(path)}: `{decl};` is not a declaration `ret name(params);`")
+            params = [] if m.group(3).strip() == "void" else [p.replace("*", "* ").split() for p in m.group(3).split(",")]
+            # a parameter's last word is its name, unless the words are a type on their own or end a pointer type
+            types = [w if len(w) <= 1 or " ".join(w) in _VALUE_TYPES or w[-1].endswith("*") else w[:-1] for w in params]
+            out[m.group(2)] = (c_type(m.group(1), decl, result=True), [c_type(" ".join(w), decl) for w in types])
+    return out
+
+
+def bind(L, headers=HEADERS):
+    """L (a CDLL) with the argtypes / restype of every function the headers declare; raises if L lacks one"""
+    for h in headers:
+        for name, (restype, argtypes) in declarations(h).items():
+            f = getattr(L, name)
+            f.restype, f.argtypes = restype, argtypes
+    return L
+
+
 def lib():
     global _lib
     if _lib is None:
-        path = os.environ.get("L3D_LIB") or _build.build()     # L3D_LIB: load a tile-sweep variant instead
-        L = C.CDLL(path)
-        L.l3d_last_error.restype = C.c_char_p
-        L.l3d_stream.restype = C.c_void_p
-        for n in ("l3d_launch_count", "l3d_match_total_rows", "l3d_match_pair_evals", "l3d_get_match_counts",
-                  "l3d_get_matches_csr", "l3d_collinear_total", "l3d_get_collinear"):
-            getattr(L, n).restype = C.c_longlong
-        _lib = L
+        _lib = bind(C.CDLL(os.environ.get("L3D_LIB") or _build.build()))     # L3D_LIB: load a tile-sweep variant instead
     return _lib
 
 
@@ -194,7 +236,7 @@ class Context:
 
     def set_views_flat(self, descs, segs_flat_ptr: int, on_device: bool):
         self._keep = [descs]
-        self._chk(self.L.l3d_set_views_flat(self.h, len(descs), descs, C.c_void_p(segs_flat_ptr), int(on_device)),
+        self._chk(self.L.l3d_set_views_flat(self.h, len(descs), descs, segs_flat_ptr, int(on_device)),
                   "l3d_set_views_flat")
 
     def update_view_params(self, descs):
@@ -205,7 +247,7 @@ class Context:
         pairs = np.ascontiguousarray(pairs, np.int32).reshape(-1, 2)
         F = np.ascontiguousarray(F, np.float32).reshape(-1, 9)
         assert len(pairs) == len(F)
-        self._chk(self.L.l3d_match_pairs(self.h, len(pairs), _p(pairs), _p(F), C.c_float(epi_overlap), int(knn)),
+        self._chk(self.L.l3d_match_pairs(self.h, len(pairs), _p(pairs), _p(F), epi_overlap, int(knn)),
                   "l3d_match_pairs")
         self._knn = int(self.L.l3d_match_stride(self.h))
 
@@ -214,7 +256,7 @@ class Context:
         pairs = np.ascontiguousarray(pairs, np.int32).reshape(-1, 2)
         F = np.ascontiguousarray(F, np.float32).reshape(-1, 9)
         assert len(pairs) == len(F)
-        self._chk(self.L.l3d_match_pairs_range(self.h, len(pairs), _p(pairs), _p(F), C.c_float(epi_overlap), int(knn), int(first), int(last)),
+        self._chk(self.L.l3d_match_pairs_range(self.h, len(pairs), _p(pairs), _p(F), epi_overlap, int(knn), int(first), int(last)),
                   "l3d_match_pairs_range")
         self._knn = int(self.L.l3d_match_stride(self.h))
 
@@ -224,7 +266,7 @@ class Context:
         Fd = np.ascontiguousarray(Fd, np.float64).reshape(-1, 9)
         assert len(pairs) == len(Fd)
         last = len(pairs) if last is None else last
-        self._chk(self.L.l3d_match_pairs_f64(self.h, len(pairs), _p(pairs), _p(Fd), C.c_float(epi_overlap), int(knn), int(first), int(last)),
+        self._chk(self.L.l3d_match_pairs_f64(self.h, len(pairs), _p(pairs), _p(Fd), epi_overlap, int(knn), int(first), int(last)),
                   "l3d_match_pairs_f64")
         self._knn = int(self.L.l3d_match_stride(self.h))
 
@@ -233,8 +275,8 @@ class Context:
         pairs = np.ascontiguousarray(pairs, np.int32).reshape(-1, 2)
         F = np.ascontiguousarray(F, np.float32).reshape(-1, 9)
         assert len(pairs) == len(F)
-        self._chk(self.L.l3d_match_pairs_host(self.h, len(pairs), _p(pairs), _p(F), C.c_float(epi_overlap), int(knn),
-                                              C.c_void_p(counts_ptr), C.c_void_p(recs_ptr), int(chunks)), "l3d_match_pairs_host")
+        self._chk(self.L.l3d_match_pairs_host(self.h, len(pairs), _p(pairs), _p(F), epi_overlap, int(knn), counts_ptr, recs_ptr, int(chunks)),
+                  "l3d_match_pairs_host")
         self._knn = int(knn)
 
     def match_device_buffers(self):
@@ -285,39 +327,38 @@ class Context:
         if row_ptr is None:
             row_ptr = np.zeros(rows + 1, np.int64)
         cap = 0 if recs is None else len(recs)
-        total = self._chk(self.L.l3d_get_matches_csr(self.h, _p(row_ptr), _p(recs), C.c_longlong(cap)),
+        total = self._chk(self.L.l3d_get_matches_csr(self.h, _p(row_ptr), _p(recs), cap),
                           "l3d_get_matches_csr")
         if recs is None or total > cap:
             recs = np.zeros(total, REC_DT)
-            total = self._chk(self.L.l3d_get_matches_csr(self.h, _p(row_ptr), _p(recs), C.c_longlong(len(recs))),
+            total = self._chk(self.L.l3d_get_matches_csr(self.h, _p(row_ptr), _p(recs), len(recs)),
                               "l3d_get_matches_csr")
         return row_ptr, recs[:total]
 
     def matches_csr_raw(self, row_ptr_ptr: int, recs_ptr: int, capacity: int) -> int:
-        return int(self._chk(self.L.l3d_get_matches_csr(self.h, C.c_void_p(row_ptr_ptr), C.c_void_p(recs_ptr),
-                                                        C.c_longlong(capacity)), "l3d_get_matches_csr"))
+        return int(self._chk(self.L.l3d_get_matches_csr(self.h, row_ptr_ptr, recs_ptr, capacity), "l3d_get_matches_csr"))
 
     def rdd(self, n, ei, ej, ew, iters=10):
         """l3d_rdd: returns (out_i, out_j, out_w, device ms of the diffusion iterations)"""
         ei = np.ascontiguousarray(ei, np.int32); ej = np.ascontiguousarray(ej, np.int32); ew = np.ascontiguousarray(ew, np.float32)
         oi, oj, ow = np.empty_like(ei), np.empty_like(ej), np.empty_like(ew)
         ms = C.c_float(0)
-        self._chk(self.L.l3d_rdd(self.h, int(n), C.c_longlong(len(ei)), _p(ei), _p(ej), _p(ew), int(iters), _p(oi), _p(oj), _p(ow),
+        self._chk(self.L.l3d_rdd(self.h, int(n), len(ei), _p(ei), _p(ej), _p(ew), int(iters), _p(oi), _p(oj), _p(ow),
                                  C.byref(ms)), "l3d_rdd")
         return oi, oj, ow, ms.value
 
     def find_collinear(self, dist_t: float, semantics: int = 0):
         """l3d_find_collinear for all views (semantics 0 = REF_GPU float kernel, 1 = REF_CPU); dist_t <= 0 switches the links off"""
-        self._chk(self.L.l3d_find_collinear(self.h, C.c_float(dist_t), int(semantics)), "l3d_find_collinear")
+        self._chk(self.L.l3d_find_collinear(self.h, dist_t, int(semantics)), "l3d_find_collinear")
         return int(self.L.l3d_collinear_total(self.h))
 
     def collinear(self, view: int, nseg: int):
         """View::collin_ of one view as CSR (row_ptr[nseg+1], idx)"""
         row_ptr = np.zeros(nseg + 1, np.int64)
-        n = self._chk(self.L.l3d_get_collinear(self.h, int(view), _p(row_ptr), None, C.c_longlong(0)), "l3d_get_collinear")
+        n = self._chk(self.L.l3d_get_collinear(self.h, int(view), _p(row_ptr), None, 0), "l3d_get_collinear")
         idx = np.zeros(max(int(n), 1), np.int32)
         if n > 0:
-            self._chk(self.L.l3d_get_collinear(self.h, int(view), _p(row_ptr), _p(idx), C.c_longlong(int(n))), "l3d_get_collinear")
+            self._chk(self.L.l3d_get_collinear(self.h, int(view), _p(row_ptr), _p(idx), n), "l3d_get_collinear")
         return row_ptr, idx[:int(n)]
 
     def optimize_lines(self, p1p2, res_ptr, res_cam, res_xy, cams, max_iter=250):
@@ -342,7 +383,7 @@ class Context:
         F = np.ascontiguousarray(F, np.float32).reshape(-1, 9)
         dp = (C.c_void_p * len(pairs))(*[int(x) for x in depth_ptrs])
         op = (C.c_void_p * len(pairs))(*[int(x) for x in overlap_ptrs])
-        self._chk(self.L.l3d_match_dense_pairs(self.h, len(pairs), _p(pairs), _p(F), C.c_float(epi_overlap), dp, op), "l3d_match_dense_pairs")
+        self._chk(self.L.l3d_match_dense_pairs(self.h, len(pairs), _p(pairs), _p(F), epi_overlap, dp, op), "l3d_match_dense_pairs")
 
     # ---- tie points (stateless: no pipeline stage changes)
     def triangulate_points(self, obs_ptr, obs_cam, obs_xy, P):
@@ -356,14 +397,14 @@ class Context:
         if n < 0 or len(cam) != len(xy) or (n >= 0 and ptr[-1] != len(cam)):
             raise ValueError("obs_ptr must have n+1 entries ending at the number of observations")
         X = np.zeros((n, 3), np.float64); valid = np.zeros(n, np.int32)
-        self._chk(self.L.l3d_triangulate_points(self.h, C.c_longlong(n), _p(ptr), _p(cam), _p(xy), len(P), _p(P), _p(X), _p(valid), 0),
+        self._chk(self.L.l3d_triangulate_points(self.h, n, _p(ptr), _p(cam), _p(xy), len(P), _p(P), _p(X), _p(valid), 0),
                   "l3d_triangulate_points")
         return X, valid
 
     def triangulate_points_device(self, n, obs_ptr, obs_cam, obs_xy, n_cams, P, X_out, valid_out):
         """l3d_triangulate_points on device addresses; asynchronous on the context's stream"""
-        a = [C.c_void_p(int(x)) for x in (obs_ptr, obs_cam, obs_xy, P, X_out, valid_out)]
-        self._chk(self.L.l3d_triangulate_points(self.h, C.c_longlong(n), a[0], a[1], a[2], int(n_cams), a[3], a[4], a[5], 1), "l3d_triangulate_points")
+        self._chk(self.L.l3d_triangulate_points(self.h, n, int(obs_ptr), int(obs_cam), int(obs_xy), int(n_cams), int(P), int(X_out), int(valid_out), 1),
+                  "l3d_triangulate_points")
 
     def median_depths(self, list_ptr, list_pts, X, valid, centres):
         """l3d_median_depths on host arrays: per camera the points list_pts[list_ptr[c]:list_ptr[c+1]] and its centre.  Returns
@@ -377,7 +418,7 @@ class Context:
         if nc != len(Cs) or len(valid) != len(X) or lptr[-1] != len(lpts):
             raise ValueError("list_ptr needs one entry per camera + 1 and must end at len(list_pts); valid needs one flag per point")
         cnt = np.zeros(nc, np.int32); med = np.zeros(nc, np.float32)
-        self._chk(self.L.l3d_median_depths(self.h, nc, _p(lptr), _p(lpts), C.c_longlong(len(X)), _p(X), _p(valid), _p(Cs), _p(cnt), _p(med), 0),
+        self._chk(self.L.l3d_median_depths(self.h, nc, _p(lptr), _p(lpts), len(X), _p(X), _p(valid), _p(Cs), _p(cnt), _p(med), 0),
                   "l3d_median_depths")
         return cnt, med
 
@@ -456,11 +497,10 @@ class Context:
         F = np.ascontiguousarray(F, np.float32).reshape(9)
         fn = self.L.l3d_match_dense_nofilter if nofilter else self.L.l3d_match_dense
         if dev_ptrs is not None:
-            self._chk(fn(self.h, int(src_view), int(tgt_view), _p(F), C.c_float(epi_overlap), C.c_void_p(dev_ptrs[0]),
-                         C.c_void_p(dev_ptrs[1]), 1), "l3d_match_dense")
+            self._chk(fn(self.h, int(src_view), int(tgt_view), _p(F), epi_overlap, dev_ptrs[0], dev_ptrs[1], 1), "l3d_match_dense")
             return None
         dep = np.empty((ns, nt, 4), np.float32)
         ov = np.empty((ns, nt), np.float32)
-        self._chk(fn(self.h, int(src_view), int(tgt_view), _p(F), C.c_float(epi_overlap), _p(dep), _p(ov), 0),
+        self._chk(fn(self.h, int(src_view), int(tgt_view), _p(F), epi_overlap, _p(dep), _p(ov), 0),
                   "l3d_match_dense")
         return dep, ov

@@ -3,6 +3,8 @@
 // this file reads and writes exactly the types they hold, in the order of the reference's serialize() methods.  Byte layout:
 // DESIGN.md §6a.  Host only.
 #include "../../include/line3d_io.h"
+#include "../../include/l3dpp_capi.h"
+#include "l3dpp_wrap.h"
 
 #include <algorithm>
 #include <cmath>
@@ -258,16 +260,8 @@ std::string segmentCachePath(const std::string& output_folder, unsigned int camI
 
 }  // namespace L3DPP
 
-// C wrapper (tests / Python), handles like l3dpp_nvm_*.  No GPU is involved.
+// C wrapper (include/l3dpp_capi.h), handles like l3dpp_nvm_*.  No GPU is involved.
 extern "C" {
-struct l3dpp_bin_line { int nseg, nres; unsigned int reference_view; int pad; };
-struct l3dpp_bin_seg { int line, valid; float length; int pad; double p1[3], p2[3], dir[3]; };
-struct l3dpp_bin_res { int line; unsigned int cam, seg; };
-
-static void l3dpp_copy_err(const std::string& e, char* err, int errcap)
-{
-    if (err && errcap > 0) { std::strncpy(err, e.c_str(), errcap - 1); err[errcap - 1] = 0; }
-}
 static void l3dpp_seg_out(const L3DPP::Segment3D& s, int line, l3dpp_bin_seg& o)
 {
     o.line = line; o.valid = s.valid() ? 1 : 0; o.length = s.length(); o.pad = 0;
@@ -285,7 +279,7 @@ void* l3dpp_bin_open(const char* path, char* err, int errcap)
 {
     std::vector<L3DPP::FinalLine3D>* v = new std::vector<L3DPP::FinalLine3D>();
     std::string e;
-    if (!L3DPP::read3DLinesBIN(path, *v, &e)) { l3dpp_copy_err(e, err, errcap); delete v; return nullptr; }
+    if (!L3DPP::read3DLinesBIN(path, *v, &e)) { l3dpp_copy_str(e, err, errcap); delete v; return nullptr; }
     return v;
 }
 void l3dpp_bin_close(void* h) { delete (std::vector<L3DPP::FinalLine3D>*)h; }
@@ -295,7 +289,6 @@ void l3dpp_bin_sizes(void* h, long long* nlines, long long* nsegs, long long* nr
     *nlines = (long long)v.size(); *nsegs = *nres = 0;
     for (const L3DPP::FinalLine3D& L : v) { *nsegs += (long long)L.collinear3Dsegments_.size(); *nres += (long long)L.underlyingCluster_.size(); }
 }
-/* arrays sized by l3dpp_bin_sizes: lines[nlines], clusters[nlines] (the cluster's line), segs[nsegs], res[nres] */
 void l3dpp_bin_get(void* h, l3dpp_bin_line* lines, l3dpp_bin_seg* clusters, l3dpp_bin_seg* segs, l3dpp_bin_res* res)
 {
     const std::vector<L3DPP::FinalLine3D>& v = *(std::vector<L3DPP::FinalLine3D>*)h;
@@ -309,14 +302,13 @@ void l3dpp_bin_get(void* h, l3dpp_bin_line* lines, l3dpp_bin_seg* clusters, l3dp
         for (const L3DPP::Segment2D& r : *L.underlyingCluster_.residuals()) { res[ro].line = (int)i; res[ro].cam = r.camID(); res[ro].seg = r.segID(); ++ro; }
     }
 }
-/* the inverse of l3dpp_bin_get: lines[i].nseg / nres consecutive entries of segs / res belong to line i (their `line` field is not read) */
 int l3dpp_bin_write(const char* path, long long nlines, const l3dpp_bin_line* lines, const l3dpp_bin_seg* clusters, const l3dpp_bin_seg* segs,
                     const l3dpp_bin_res* res, char* err, int errcap)
 {
     std::vector<L3DPP::FinalLine3D> v;
     size_t so = 0, ro = 0;
     for (long long i = 0; i < nlines; ++i) {
-        if (lines[i].nseg < 0 || lines[i].nres < 0) { l3dpp_copy_err("negative segment or residual count", err, errcap); return -1; }
+        if (lines[i].nseg < 0 || lines[i].nres < 0) { l3dpp_copy_str("negative segment or residual count", err, errcap); return -1; }
         std::list<L3DPP::Segment3D> s;
         for (int k = 0; k < lines[i].nseg; ++k) s.push_back(l3dpp_seg_in(segs[so++]));
         std::list<L3DPP::Segment2D> r;
@@ -324,7 +316,7 @@ int l3dpp_bin_write(const char* path, long long nlines, const l3dpp_bin_line* li
         v.push_back(L3DPP::FinalLine3D{s, L3DPP::LineCluster3D(l3dpp_seg_in(clusters[i]), r, lines[i].reference_view)});
     }
     std::string e;
-    if (!L3DPP::write3DLinesBIN(path, v, &e)) { l3dpp_copy_err(e, err, errcap); return -1; }
+    if (!L3DPP::write3DLinesBIN(path, v, &e)) { l3dpp_copy_str(e, err, errcap); return -1; }
     return 0;
 }
 
@@ -332,7 +324,7 @@ void* l3dpp_segcache_open(const char* path, char* err, int errcap)
 {
     std::vector<L3DPP::Vec4f>* v = new std::vector<L3DPP::Vec4f>();
     std::string e;
-    if (!L3DPP::readSegmentCache(path, *v, &e)) { l3dpp_copy_err(e, err, errcap); delete v; return nullptr; }
+    if (!L3DPP::readSegmentCache(path, *v, &e)) { l3dpp_copy_str(e, err, errcap); delete v; return nullptr; }
     return v;
 }
 void l3dpp_segcache_close(void* h) { delete (std::vector<L3DPP::Vec4f>*)h; }
@@ -344,14 +336,13 @@ void l3dpp_segcache_get(void* h, float* xy4)
 }
 int l3dpp_segcache_write(const char* path, const float* xy4, long long n, char* err, int errcap)
 {
-    if (n < 0) { l3dpp_copy_err("negative segment count", err, errcap); return -1; }
+    if (n < 0) { l3dpp_copy_str("negative segment count", err, errcap); return -1; }
     std::vector<L3DPP::Vec4f> v((size_t)n);
     if (n) std::memcpy(v.data(), xy4, (size_t)n * sizeof(L3DPP::Vec4f));
     std::string e;
-    if (!L3DPP::writeSegmentCache(path, v, &e)) { l3dpp_copy_err(e, err, errcap); return -1; }
+    if (!L3DPP::writeSegmentCache(path, v, &e)) { l3dpp_copy_str(e, err, errcap); return -1; }
     return 0;
 }
-/* segmentCachePath into buf; returns its length, or -1 if it does not fit */
 int l3dpp_segcache_path(const char* folder, unsigned int cam, int w, int h, int max_img_width, char* buf, int cap)
 {
     const std::string s = L3DPP::segmentCachePath(folder, cam, w, h, max_img_width);

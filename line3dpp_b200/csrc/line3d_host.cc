@@ -10,12 +10,14 @@
 #include "../../include/line3d_io.h"   // segment cache + .bin writer (csrc/line3d_bin.cc)
 #include <nvtx3/nvToolsExt.h>      // header-only; ranges show up in nsys / ncu timelines
 #include "../../include/l3d_capi.h"
+#include "../../include/l3dpp_capi.h"
 #include <cuda_runtime_api.h>          // cudaGetDevice: undistortImage runs on the caller's current device
 
 #include <algorithm>
 #include <cassert>
 #include <chrono>
 #include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstring>
 #include <fstream>
@@ -27,6 +29,7 @@
 #include <sstream>
 #include <stdexcept>
 #include <thread>
+#include <type_traits>
 #include <sys/stat.h>                  // mkdir: the segment cache's folder
 
 namespace L3DPP {
@@ -211,7 +214,7 @@ struct Line3D::Impl {
     Line3D::SegmentDetectorFn detector = nullptr; void* detector_user = nullptr;
     std::set<unsigned int> reserved;
     std::mutex prep_mtx;
-    struct { int (*fn)(void*, const unsigned char*, int, int, void*); void* user; } c_detector{nullptr, nullptr};   // l3dpp_set_segment_detector
+    struct { l3dpp_detect_fn fn; void* user; } c_detector{nullptr, nullptr};   // l3dpp_set_segment_detector
     // index maps (rebuilt at matchImages)
     std::vector<HostView*> vlist;                         // by view index (ascending camID)
     std::map<unsigned int, int> index_of;
@@ -1083,24 +1086,26 @@ void Line3D::undistortImage(const Image8u& in, Image8u& out, const LensDistortio
 
 }  // namespace L3DPP
 
-// ================================================================================================ C wrapper (tests / Python)
+// ================================================================================================ C wrapper (include/l3dpp_capi.h)
+// The header spells Line3D's C++ types in C: check that they are the same.
+static_assert(std::is_same<L3DPP::Line3D::MatchExchangeFn, l3dpp_exchange_fn>::value, "l3dpp_exchange_fn differs from Line3D::MatchExchangeFn");
+static_assert(sizeof(l3dpp_stats_block) == sizeof(L3DPP::Line3DStats), "l3dpp_stats_block differs from Line3DStats");
+#define L3DPP_SAME_STAT(f) static_assert(offsetof(l3dpp_stats_block, f) == offsetof(L3DPP::Line3DStats, f) && \
+                                         std::is_same<decltype(l3dpp_stats_block::f), decltype(L3DPP::Line3DStats::f)>::value, "l3dpp_stats_block::" #f);
+L3DPP_SAME_STAT(view_pairs) L3DPP_SAME_STAT(pair_evaluations) L3DPP_SAME_STAT(matches_after_knn) L3DPP_SAME_STAT(estimates)
+L3DPP_SAME_STAT(affinity_entries) L3DPP_SAME_STAT(affinity_rows) L3DPP_SAME_STAT(clusters_total) L3DPP_SAME_STAT(clusters_valid)
+L3DPP_SAME_STAT(lines3D) L3DPP_SAME_STAT(collinear_entries) L3DPP_SAME_STAT(opt_iterations) L3DPP_SAME_STAT(ms_match) L3DPP_SAME_STAT(ms_score)
+L3DPP_SAME_STAT(ms_affinity) L3DPP_SAME_STAT(ms_diffusion) L3DPP_SAME_STAT(ms_cluster) L3DPP_SAME_STAT(opt_cost_before)
+L3DPP_SAME_STAT(opt_cost_after) L3DPP_SAME_STAT(ms_gather)
+#undef L3DPP_SAME_STAT
+
 extern "C" {
 using namespace L3DPP;
-void* l3dpp_create(int neighbors_by_worldpoints, int use_gpu, int device)
-{
-    try { return new Line3D("", true, -1, 3000, neighbors_by_worldpoints != 0, use_gpu != 0, device); } catch (...) { return nullptr; }
-}
-// the full constructor: output folder, segment cache switch and max_img_width as Line3D takes them
-void* l3dpp_create_in(const char* output_folder, int load_segments, int max_img_width, int neighbors_by_worldpoints, int use_gpu, int device)
-{
-    try { return new Line3D(output_folder, load_segments != 0, max_img_width, 3000, neighbors_by_worldpoints != 0, use_gpu != 0, device); } catch (...) { return nullptr; }
-}
-// the device-list constructor; devices[0] is the primary
-void* l3dpp_create_devices(const char* output_folder, int load_segments, int max_img_width, int neighbors_by_worldpoints, int use_gpu, const int* devices,
-                           int num_devices)
+void* l3dpp_create(const char* output_folder, int load_segments, int max_img_width, unsigned int max_line_segments, int neighbors_by_worldpoints,
+                   int use_gpu, const int* devices, int num_devices)
 {
     try {
-        return new Line3D(output_folder, load_segments != 0, max_img_width, 3000, neighbors_by_worldpoints != 0, use_gpu != 0,
+        return new Line3D(output_folder, load_segments != 0, max_img_width, max_line_segments, neighbors_by_worldpoints != 0, use_gpu != 0,
                           std::vector<int>(devices, devices + std::max(num_devices, 0)));
     } catch (...) { return nullptr; }
 }
@@ -1117,16 +1122,12 @@ int l3dpp_add_image(void* h, unsigned int cam, int w, int hgt, const double* K, 
 }
 int l3dpp_match_images(void* h, float sp, float sa, unsigned int nn, float epi, int knn, float crd)
 { Line3D* L = (Line3D*)h; L->matchImages(sp, sa, nn, epi, knn, crd); return L->lastError()[0] ? -1 : 0; }
-int l3dpp_reconstruct(void* h, unsigned int vis, int diffusion, float collin)
-{ Line3D* L = (Line3D*)h; L->reconstruct3Dlines(vis, diffusion != 0, collin, false, 0); return L->lastError()[0] ? -1 : 0; }
 int l3dpp_reconstruct_opt(void* h, unsigned int vis, int diffusion, float collin, int use_ceres, unsigned int max_iter)
 { Line3D* L = (Line3D*)h; L->reconstruct3Dlines(vis, diffusion != 0, collin, use_ceres != 0, max_iter); return L->lastError()[0] ? -1 : 0; }
-int l3dpp_set_shard(void* h, int rank, int world, Line3D::MatchExchangeFn fn, void* user)
+int l3dpp_set_shard(void* h, int rank, int world, l3dpp_exchange_fn fn, void* user)
 { Line3D* L = (Line3D*)h; L->setShard(rank, world, fn, user); return L->lastError()[0] ? -1 : 0; }
-int l3dpp_stats(void* h, Line3DStats* out) { *out = ((Line3D*)h)->stats(); return 0; }
+int l3dpp_stats(void* h, l3dpp_stats_block* out) { memcpy(out, &((Line3D*)h)->stats(), sizeof(*out)); return 0; }
 int l3dpp_view_index(void* h, unsigned int cam) { auto& m = ((Line3D*)h)->impl()->index_of; auto it = m.find(cam); return it == m.end() ? -1 : it->second; }
-// test hook for the cluster -> 3D segment tail: findCollinearSegments(cluster) (line3D.cc:2342-2452) on an explicit cluster
-// (line end points + (camID, segID) residuals of views added with addImage).  Returns the number of 3D segments.
 int l3dpp_collinear_from_cluster(void* h, const double* p1p2, int nres, const unsigned int* cams, const unsigned int* segs, double* out6, int cap)
 {
     Line3D::Impl& P = *((Line3D*)h)->impl();
@@ -1143,7 +1144,7 @@ int l3dpp_collinear_from_cluster(void* h, const double* p1p2, int nres, const un
 }
 int l3dpp_view_info(void* h, unsigned int cam, float* k, float* md)
 { auto& v = ((Line3D*)h)->impl()->views; auto it = v.find(cam); if (it == v.end()) return -1; *k = it->second.k; *md = it->second.median_depth; return 0; }
-int l3dpp_get_pairs(void* h, int* out, int cap)   // (src cam, tgt cam) in match order
+int l3dpp_get_pairs(void* h, int* out, int cap)
 {
     Line3D::Impl* P = ((Line3D*)h)->impl();
     const int n = (int)(P->pairs.size() / 2);
@@ -1163,8 +1164,6 @@ int l3dpp_get_local2global(void* h, unsigned int* cam_seg, int cap)
     for (size_t i = 0; i < P->local2global.size() && (int)i < cap; ++i) { const Segment2D s = P->seg_of(P->local2global[i]); cam_seg[2 * i] = s.camID(); cam_seg[2 * i + 1] = s.segID(); }
     return (int)P->local2global.size();
 }
-struct l3dpp_seg3d { int line; int pad; double p1[3], p2[3]; };
-struct l3dpp_residual { int line; unsigned int cam, seg; };
 long long l3dpp_get_segments3d(void* h, l3dpp_seg3d* out, long long cap)
 {
     std::vector<FinalLine3D> L; ((Line3D*)h)->get3Dlines(L);
@@ -1184,13 +1183,11 @@ long long l3dpp_get_residuals(void* h, l3dpp_residual* out, long long cap)
         for (const Segment2D& s : *L[i].underlyingCluster_.residuals()) { if (out && n < cap) { out[n].line = (int)i; out[n].cam = s.camID(); out[n].seg = s.segID(); } ++n; }
     return n;
 }
-// get3Dlines() as a handle of the l3dpp_bin_* functions (csrc/line3d_bin.cc): every field, for comparison with a .bin file
 void* l3dpp_lines_handle(void* h) { std::vector<FinalLine3D>* v = new std::vector<FinalLine3D>(); ((Line3D*)h)->get3Dlines(*v); return v; }
 int l3dpp_save_obj(void* h, const char* folder) { Line3D* L = (Line3D*)h; L->saveResultAsOBJ(folder); return L->lastError()[0] ? -1 : 0; }
 int l3dpp_save_stl(void* h, const char* folder) { Line3D* L = (Line3D*)h; L->saveResultAsSTL(folder); return L->lastError()[0] ? -1 : 0; }
 int l3dpp_output_filename(void* h, char* buf, int cap)
 { const std::string s = ((Line3D*)h)->createOutputFilename(); if ((int)s.size() + 1 > cap) return -1; memcpy(buf, s.c_str(), s.size() + 1); return (int)s.size(); }
-// test hook for the writers: replace the result by explicit lines (segments: 6 doubles each; residuals: camID, segID of added views)
 int l3dpp_set_lines(void* h, int nlines, const int* nseg, const double* segs6, const int* nres, const unsigned int* res_cam, const unsigned int* res_seg)
 {
     Line3D::Impl& P = *((Line3D*)h)->impl();
@@ -1212,14 +1209,6 @@ int l3dpp_set_lines(void* h, int nlines, const int* nseg, const double* segs6, c
 }
 int l3dpp_save_txt(void* h, const char* folder) { Line3D* L = (Line3D*)h; L->save3DLinesAsTXT(folder); return L->lastError()[0] ? -1 : 0; }
 int l3dpp_save_bin(void* h, const char* folder) { Line3D* L = (Line3D*)h; L->save3DLinesAsBIN(folder); return L->lastError()[0] ? -1 : 0; }
-// the full constructor with max_line_segments
-void* l3dpp_create_full(const char* output_folder, int load_segments, int max_img_width, unsigned int max_line_segments, int neighbors_by_worldpoints,
-                        int use_gpu, int device)
-{
-    try { return new Line3D(output_folder, load_segments != 0, max_img_width, max_line_segments, neighbors_by_worldpoints != 0, use_gpu != 0, device); }
-    catch (...) { return nullptr; }
-}
-// addImage with an image: rows x cols, 1 or 3 channels, row step in bytes; nseg == 0: no segments given
 int l3dpp_add_image_pixels(void* h, unsigned int cam, const unsigned char* pixels, int rows, int cols, int channels, long long step, const double* K,
                            const double* R, const double* t, float median_depth, const unsigned int* list, int nlist, const float* segs, int nseg)
 {
@@ -1231,9 +1220,6 @@ int l3dpp_add_image_pixels(void* h, unsigned int cam, const unsigned char* pixel
     Line3D* L = (Line3D*)h;
     return L->addImage(cam, img, Km, Rm, Vector3d(t[0], t[1], t[2]), median_depth, std::list<unsigned int>(list, list + nlist), s) ? 0 : -1;
 }
-// detector in C terms: fn(user, gray, rows, cols, out) returns non-zero on success and hands its detections over with
-// l3dpp_push_detections(out, xy4, n) (any number of calls)
-typedef int (*l3dpp_detect_fn)(void* user, const unsigned char* gray, int rows, int cols, void* out);
 void l3dpp_push_detections(void* out, const float* xy4, long long n)
 {
     std::vector<Vec4f>& v = *(std::vector<Vec4f>*)out;
@@ -1254,7 +1240,6 @@ int l3dpp_set_segment_detector(void* h, l3dpp_detect_fn fn, void* user)
     L->setSegmentDetector(fn ? l3dpp_detect_trampoline : nullptr, &P);
     return 0;
 }
-// the 2D segments of a view through getSegmentCoords2D: out[cap * 4]; returns the view's segment count (-1 for an unknown camID)
 long long l3dpp_view_segments(void* h, unsigned int cam, float* out, long long cap)
 {
     Line3D* L = (Line3D*)h;
@@ -1269,7 +1254,6 @@ long long l3dpp_view_segments(void* h, unsigned int cam, float* out, long long c
     for (long long i = 0; i < n && i < cap; ++i) memcpy(out + 4 * i, L->getSegmentCoords2D(cam, (unsigned int)i).v, 16);
     return n;
 }
-// detectLineSegments' post-processing alone (no GPU): out[cap * 4]; returns the number of segments kept (even if > cap)
 long long l3dpp_filter_detections(const float* det, long long n, int w, int h, int w_p, int h_p, unsigned int max_segments, float* out, long long cap)
 {
     std::vector<Vec4f> d((size_t)std::max(n, 0ll));
@@ -1278,7 +1262,6 @@ long long l3dpp_filter_detections(const float* det, long long n, int w, int h, i
     if ((long long)r.size() <= cap && !r.empty()) memcpy(out, r.data(), 16 * r.size());
     return (long long)r.size();
 }
-// Line3D::undistortImage on a packed image; K row-major, radial[3], tangential[2].  0, -1 (std::invalid_argument) or -2 (std::runtime_error)
 int l3dpp_undistort_image(const unsigned char* src, unsigned char* dst, int rows, int cols, int channels, const double* radial, const double* tangential,
                           const double* K)
 {
@@ -1291,7 +1274,6 @@ int l3dpp_undistort_image(const unsigned char* src, unsigned char* dst, int rows
     memcpy(dst, out.data.data(), out.data.size());
     return 0;
 }
-// the LensDistortion overload on CUDA device `device` (the thread's current device is restored); lens = model, k[6], p[2] as 9 doubles
 int l3dpp_undistort_image_lens(const unsigned char* src, unsigned char* dst, int rows, int cols, int channels, const double* lens9, const double* K,
                                int device)
 {

@@ -1,7 +1,8 @@
 // line3d_io.cc — .nvm, Bundler and COLMAP (text and binary) readers for frontends built on include/line3d.h (restates main_vsfm.cpp:143-310,
 // main_bundler.cpp, main_colmap.cpp; host only)
 #include "../../include/line3d_io.h"
-#include "l3d_sfm_handle.h"
+#include "../../include/l3dpp_capi.h"
+#include "l3dpp_wrap.h"
 
 #include <algorithm>
 #include <cmath>
@@ -373,13 +374,13 @@ Matrix3d intrinsicsFromFocal(float focal, int w, int h)
 
 }  // namespace L3DPP
 
-// C wrapper (tests / Python): flat arrays.  R, t: 9 + 3 doubles per camera; returns the number of cameras or -1.
+// C wrapper (include/l3dpp_capi.h): flat arrays
 extern "C" {
 void* l3dpp_nvm_open(const char* path, char* err, int errcap)
 {
     std::vector<L3DPP::NVMCamera>* v = new std::vector<L3DPP::NVMCamera>();
     std::string e;
-    if (!L3DPP::readNVM(path, *v, &e)) { if (err && errcap > 0) { std::strncpy(err, e.c_str(), errcap - 1); err[errcap - 1] = 0; } delete v; return nullptr; }
+    if (!L3DPP::readNVM(path, *v, &e)) { l3dpp_copy_str(e, err, errcap); delete v; return nullptr; }
     return v;
 }
 void l3dpp_nvm_close(void* h) { delete (std::vector<L3DPP::NVMCamera>*)h; }
@@ -392,7 +393,7 @@ int l3dpp_nvm_camera(void* h, int i, double* R9, double* t3, double* C3, float* 
     for (int k = 0; k < 9; ++k) R9[k] = c.R.m[k];
     t3[0] = c.t.x; t3[1] = c.t.y; t3[2] = c.t.z; C3[0] = c.C.x; C3[1] = c.C.y; C3[2] = c.C.z;
     *focal = c.focal; *distortion = c.distortion; *median_depth = c.median_depth; *num_wps = (int)c.worldpoints.size();
-    if (name && namecap > 0) { std::strncpy(name, c.image.c_str(), namecap - 1); name[namecap - 1] = 0; }
+    l3dpp_copy_str(c.image, name, namecap);
     return 0;
 }
 int l3dpp_nvm_worldpoints(void* h, int i, unsigned int* out, int cap)
@@ -403,18 +404,26 @@ int l3dpp_nvm_worldpoints(void* h, int i, unsigned int* out, int cap)
     for (unsigned int w : v[i].worldpoints) { if (n < cap) out[n] = w; ++n; }
     return n;
 }
-void* l3dpp_sfm_open(int kind /*0 bundler, 1 colmap, 5 colmap with lenses*/, const char* path, const char* aux, char* err, int errcap)
+void* l3dpp_sfm_open(int kind, const char* path, const char* aux, char* err, int errcap)
 {
     L3DSfMHandle* v = new L3DSfMHandle();
+    const std::string a = aux ? aux : "";
     std::string e;
-    const bool ok = kind == 0 ? L3DPP::readBundler(path, aux ? aux : "", v->cams, &e)
-                              : L3DPP::readColmap(path, v->cams, &e, kind == 5 ? &v->lenses : nullptr);
-    if (!ok) { if (err && errcap > 0) { std::strncpy(err, e.c_str(), errcap - 1); err[errcap - 1] = 0; } delete v; return nullptr; }
+    bool ok = false;
+    switch (kind) {
+    case L3DPP_SFM_BUNDLER: ok = L3DPP::readBundler(path, a, v->cams, &e); break;
+    case L3DPP_SFM_COLMAP: ok = L3DPP::readColmap(path, v->cams, &e); break;
+    case L3DPP_SFM_COLMAP_LENSES: ok = L3DPP::readColmap(path, v->cams, &e, &v->lenses); break;
+    case L3DPP_SFM_MAVMAP: ok = L3DPP::readMavmap(path, v->cams, &e); break;
+    case L3DPP_SFM_OPENMVG: ok = L3DPP::readOpenMVG(path, v->cams, &e); break;
+    case L3DPP_SFM_PIX4D: ok = L3DPP::readPix4D(path, a, v->cams, &e); break;
+    default: e = "unknown model kind " + std::to_string(kind);
+    }
+    if (!ok) { l3dpp_copy_str(e, err, errcap); delete v; return nullptr; }
     return v;
 }
 void l3dpp_sfm_close(void* h) { delete (L3DSfMHandle*)h; }
 int l3dpp_sfm_num_cameras(void* h) { return (int)((L3DSfMHandle*)h)->cams.size(); }
-/* lens of camera i as model, k[6], p[2] (9 doubles); -1 when i is out of range or the model was read without lenses */
 int l3dpp_sfm_lens(void* h, int i, double* lens9)
 {
     const std::vector<L3DPP::LensDistortion>& v = ((L3DSfMHandle*)h)->lenses;
@@ -434,7 +443,7 @@ int l3dpp_sfm_camera(void* h, int i, double* head5, double* K9, double* R9, doub
     t3[0] = c.t.x; t3[1] = c.t.y; t3[2] = c.t.z; C3[0] = c.C.x; C3[1] = c.C.y; C3[2] = c.C.z;
     for (int k = 0; k < 3; ++k) dist5[k] = c.radial[k];
     dist5[3] = c.tangential[0]; dist5[4] = c.tangential[1];
-    if (name && namecap > 0) { std::strncpy(name, c.image.c_str(), namecap - 1); name[namecap - 1] = 0; }
+    l3dpp_copy_str(c.image, name, namecap);
     return 0;
 }
 int l3dpp_sfm_worldpoints(void* h, int i, unsigned int* out, int cap)

@@ -8,7 +8,7 @@
 // path and the problem; nothing is allocated beyond what the bytes read justify; JSON nesting is capped at JSON_MAX_DEPTH.
 #include "../../include/line3d_io.h"
 #include "../../include/l3d_capi.h"
-#include "l3d_sfm_handle.h"
+#include "../../include/l3dpp_capi.h"
 
 #include <algorithm>
 #include <cmath>
@@ -662,22 +662,8 @@ bool readPix4D(const std::string& params_folder, const std::string& project_pref
 
 }  // namespace L3DPP
 
-// C wrapper (tests / Python); the cameras are read back with l3dpp_sfm_camera / l3dpp_sfm_worldpoints / l3dpp_sfm_close (line3d_io.cc)
+// C wrapper (include/l3dpp_capi.h); l3dpp_sfm_open, which reads these models too, is in line3d_io.cc
 extern "C" {
-/* kind 2 mavmap (path = the file), 3 OpenMVG (path = sfm_data.json), 4 Pix4D (path = params folder, aux = project prefix, device = the
- * GPU that triangulates) */
-void* l3dpp_sfm_read(int kind, const char* path, const char* aux, int device, char* err, int errcap)
-{
-    L3DSfMHandle* v = new L3DSfMHandle();
-    std::string e;
-    bool ok = false;
-    if (kind == 2) ok = L3DPP::readMavmap(path, v->cams, &e);
-    else if (kind == 3) ok = L3DPP::readOpenMVG(path, v->cams, &e);
-    else if (kind == 4) ok = L3DPP::readPix4D(path, aux ? aux : "", v->cams, &e, device);
-    else e = "unknown model kind";
-    if (!ok) { if (err && errcap > 0) { std::strncpy(err, e.c_str(), errcap - 1); err[errcap - 1] = 0; } delete v; return nullptr; }
-    return v;
-}
 void l3dpp_rotation_from_rpy(double roll, double pitch, double yaw, double* R9)
 {
     const L3DPP::Matrix3d R = L3DPP::Line3D::rotationFromRPY(roll, pitch, yaw);

@@ -26,7 +26,7 @@ def _p(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
 
 
-# Line3D::SegmentDetectorFn in C terms (l3dpp_set_segment_detector): (user, gray pixels, rows, cols, detections handle) -> non-zero on success
+# l3dpp_detect_fn (include/l3dpp_capi.h): (user, gray pixels, rows, cols, detections handle) -> non-zero on success
 DETECT_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_uint8), C.c_int, C.c_int, C.c_void_p)
 
 
@@ -41,28 +41,11 @@ class Line3D:
         devices: a list of CUDA devices in place of `device` (the first is the primary; repeats allowed): match_images splits the
         view pairs over them and gathers the matches on the primary, with the single-device result"""
         self.L = capi.lib()
-        self.L.l3dpp_create.restype = C.c_void_p
-        self.L.l3dpp_create_in.restype = C.c_void_p
-        self.L.l3dpp_ctx.restype = C.c_void_p
-        self.L.l3dpp_last_error.restype = C.c_char_p
-        for n in ("l3dpp_get_affinity", "l3dpp_get_segments3d", "l3dpp_get_residuals", "l3d_get_view_matches", "l3d_get_estimates"):
-            getattr(self.L, n).restype = C.c_longlong
-        if devices is not None:
-            devs = np.ascontiguousarray([int(d) for d in devices], np.int32)
-            if len(devs) == 0:
-                raise ValueError("devices must name at least one CUDA device")
-            self.L.l3dpp_create_devices.restype = C.c_void_p
-            h = self.L.l3dpp_create_devices(str(output_folder or "").encode(), int(load_segments), int(max_img_width),
-                                            int(neighbors_by_worldpoints), int(use_gpu), _p(devs), len(devs))
-        elif max_line_segments != 3000:
-            self.L.l3dpp_create_full.restype = C.c_void_p
-            h = self.L.l3dpp_create_full(str(output_folder or "").encode(), int(load_segments), int(max_img_width), C.c_uint(int(max_line_segments)),
-                                         int(neighbors_by_worldpoints), int(use_gpu), int(device))
-        elif output_folder is None:
-            h = self.L.l3dpp_create(int(neighbors_by_worldpoints), int(use_gpu), int(device))
-        else:
-            h = self.L.l3dpp_create_in(str(output_folder).encode(), int(load_segments), int(max_img_width), int(neighbors_by_worldpoints),
-                                       int(use_gpu), int(device))
+        devs = np.ascontiguousarray([int(d) for d in ([device] if devices is None else devices)], np.int32)
+        if len(devs) == 0:
+            raise ValueError("devices must name at least one CUDA device")
+        h = self.L.l3dpp_create(str(output_folder or "").encode(), int(load_segments), int(max_img_width), int(max_line_segments),
+                                int(neighbors_by_worldpoints), int(use_gpu), _p(devs), len(devs))
         self.h = C.c_void_p(h)
         if not self.h:
             which = "" if devices is None else f" among {list(devices)}"
@@ -87,8 +70,8 @@ class Line3D:
         lst = np.ascontiguousarray(wps_or_neighbors, np.uint32)
         segs = np.ascontiguousarray(segs, np.float32).reshape(-1, 4)
         f64 = lambda a: np.ascontiguousarray(a, np.float64)
-        self._chk(self.L.l3dpp_add_image(self.h, C.c_uint(int(cam)), int(width), int(height), _p(f64(K)), _p(f64(R)), _p(f64(t)),
-                                         C.c_float(float(median_depth)), _p(lst), len(lst), _p(segs), len(segs)), "addImage")
+        self._chk(self.L.l3dpp_add_image(self.h, int(cam), int(width), int(height), _p(f64(K)), _p(f64(R)), _p(f64(t)), float(median_depth),
+                                         _p(lst), len(lst), _p(segs), len(segs)), "addImage")
 
     def add_image_pixels(self, cam, img, K, R, t, median_depth, wps_or_neighbors, segs=()):
         """addImage with the image itself: img uint8 HxW (grey) or HxWx3 (channel 0 is R), any row stride.  Without segs the segment
@@ -100,9 +83,8 @@ class Line3D:
         f64 = lambda v: np.ascontiguousarray(v, np.float64)
         errors = self.__dict__.setdefault("_detector_errors", {})      # per calling thread: the detector runs on it
         errors.pop(threading.get_ident(), None)
-        rc = self.L.l3dpp_add_image_pixels(self.h, C.c_uint(int(cam)), C.c_void_p(a.ctypes.data), a.shape[0], a.shape[1], 1 if a.ndim == 2 else 3,
-                                           C.c_longlong(sp), _p(f64(K)), _p(f64(R)), _p(f64(t)), C.c_float(float(median_depth)), _p(lst), len(lst),
-                                           _p(segs), len(segs))
+        rc = self.L.l3dpp_add_image_pixels(self.h, int(cam), a.ctypes.data, a.shape[0], a.shape[1], 1 if a.ndim == 2 else 3, sp, _p(f64(K)),
+                                           _p(f64(R)), _p(f64(t)), float(median_depth), _p(lst), len(lst), _p(segs), len(segs))
         err = errors.pop(threading.get_ident(), None)
         if err is not None:
             raise err
@@ -120,24 +102,22 @@ class Line3D:
                     if det is None or det is False:
                         return 0
                     det = np.ascontiguousarray(det, np.float32).reshape(-1, 4)
-                    self.L.l3dpp_push_detections(C.c_void_p(out), _p(det), C.c_longlong(len(det)))
+                    self.L.l3dpp_push_detections(out, _p(det), len(det))
                     return 1
                 except BaseException as e:      # noqa: BLE001 - handed back to add_image_pixels
                     self.__dict__.setdefault("_detector_errors", {})[threading.get_ident()] = e
                     return 0
             cb = DETECT_FN(call)
         self._detector = cb                     # the library keeps the pointer: keep the callback alive
-        self.L.l3dpp_set_segment_detector.argtypes = [C.c_void_p, DETECT_FN, C.c_void_p]
         self.L.l3dpp_set_segment_detector(self.h, cb, None)
 
     def view_segments(self, cam):
         """float32 [n, 4]: the view's 2D segments as getSegmentCoords2D returns them"""
-        self.L.l3dpp_view_segments.restype = C.c_longlong
-        n = self.L.l3dpp_view_segments(self.h, C.c_uint(int(cam)), None, C.c_longlong(0))
+        n = self.L.l3dpp_view_segments(self.h, int(cam), None, 0)
         if n < 0:
             raise KeyError(cam)
         out = np.zeros((n, 4), np.float32)
-        self.L.l3dpp_view_segments(self.h, C.c_uint(int(cam)), _p(out), C.c_longlong(n))
+        self.L.l3dpp_view_segments(self.h, int(cam), _p(out), n)
         return out
 
     def add_scene(self, scene):
@@ -146,12 +126,11 @@ class Line3D:
                            scene.neighbors[i], scene.segs[i])
 
     def match_images(self, sigma_p=2.5, sigma_a=10.0, num_neighbors=10, epi_overlap=0.25, knn=10, const_reg_depth=-1.0):
-        self._chk(self.L.l3dpp_match_images(self.h, C.c_float(sigma_p), C.c_float(sigma_a), C.c_uint(num_neighbors), C.c_float(epi_overlap),
-                                            C.c_int(knn), C.c_float(const_reg_depth)), "matchImages")
+        self._chk(self.L.l3dpp_match_images(self.h, sigma_p, sigma_a, num_neighbors, epi_overlap, knn, const_reg_depth), "matchImages")
 
     def reconstruct_3d_lines(self, visibility_t=3, perform_diffusion=False, collinearity_t=-1.0, use_ceres=False, max_iter_ceres=250):
-        self._chk(self.L.l3dpp_reconstruct_opt(self.h, C.c_uint(visibility_t), int(perform_diffusion), C.c_float(collinearity_t),
-                                               int(use_ceres), C.c_uint(max_iter_ceres)), "reconstruct3Dlines")
+        self._chk(self.L.l3dpp_reconstruct_opt(self.h, visibility_t, int(perform_diffusion), collinearity_t, int(use_ceres), max_iter_ceres),
+                  "reconstruct3Dlines")
 
     # ---- dumps
     def stats(self):
@@ -167,43 +146,42 @@ class Line3D:
 
     def view_info(self, cam):
         k, md = C.c_float(0), C.c_float(0)
-        self.L.l3dpp_view_info(self.h, C.c_uint(int(cam)), C.byref(k), C.byref(md))
+        self.L.l3dpp_view_info(self.h, int(cam), C.byref(k), C.byref(md))
         return k.value, md.value
 
     def view_matches(self, cam, kept_only):
-        vi = self.L.l3dpp_view_index(self.h, C.c_uint(int(cam)))
-        n = self.L.l3d_get_view_matches(self.ctx, vi, int(kept_only), None, C.c_longlong(0))
+        vi = self.L.l3dpp_view_index(self.h, int(cam))
+        n = self.L.l3d_get_view_matches(self.ctx, vi, int(kept_only), None, 0)
         if n < 0:
             raise capi.L3DError("l3d_get_view_matches failed")
         a = np.zeros(n, capi.MATCH_DT)
         if n:
-            self.L.l3d_get_view_matches(self.ctx, vi, int(kept_only), _p(a), C.c_longlong(n))
+            self.L.l3d_get_view_matches(self.ctx, vi, int(kept_only), _p(a), n)
         return a
 
     def estimates(self):
-        n = self.L.l3d_get_estimates(self.ctx, None, None, C.c_longlong(0))
+        n = self.L.l3d_get_estimates(self.ctx, None, None, 0)
         best, p = np.zeros(max(n, 0), capi.MATCH_DT), np.zeros((max(n, 0), 6), np.float64)
         if n > 0:
-            self.L.l3d_get_estimates(self.ctx, _p(best), _p(p), C.c_longlong(n))
+            self.L.l3d_get_estimates(self.ctx, _p(best), _p(p), n)
         return best, p
 
     def ctx_collinear(self, view_index, nseg):
         """View::collin_ of the view_index-th added view as CSR (row_ptr, idx), straight from the C ABI"""
         row_ptr = np.zeros(nseg + 1, np.int64)
-        self.L.l3d_get_collinear.restype = C.c_longlong
-        n = self.L.l3d_get_collinear(self.ctx, int(view_index), _p(row_ptr), None, C.c_longlong(0))
+        n = self.L.l3d_get_collinear(self.ctx, int(view_index), _p(row_ptr), None, 0)
         if n < 0:
             raise capi.L3DError("l3d_get_collinear failed")
         idx = np.zeros(max(int(n), 1), np.int32)
         if n > 0:
-            self.L.l3d_get_collinear(self.ctx, int(view_index), _p(row_ptr), _p(idx), C.c_longlong(int(n)))
+            self.L.l3d_get_collinear(self.ctx, int(view_index), _p(row_ptr), _p(idx), n)
         return row_ptr, idx[:int(n)]
 
     def affinity(self, raw=False):
-        n = self.L.l3dpp_get_affinity(self.h, int(raw), None, None, None, C.c_longlong(0))
+        n = self.L.l3dpp_get_affinity(self.h, int(raw), None, None, None, 0)
         ei, ej, ew = np.zeros(n, np.int32), np.zeros(n, np.int32), np.zeros(n, np.float32)
         if n:
-            self.L.l3dpp_get_affinity(self.h, int(raw), _p(ei), _p(ej), _p(ew), C.c_longlong(n))
+            self.L.l3dpp_get_affinity(self.h, int(raw), _p(ei), _p(ej), _p(ew), n)
         return ei, ej, ew
 
     def local2global(self):
@@ -214,17 +192,17 @@ class Line3D:
         return a
 
     def segments3d(self):
-        n = self.L.l3dpp_get_segments3d(self.h, None, C.c_longlong(0))
+        n = self.L.l3dpp_get_segments3d(self.h, None, 0)
         a = np.zeros(n, SEG3D_DT)
         if n:
-            self.L.l3dpp_get_segments3d(self.h, _p(a), C.c_longlong(n))
+            self.L.l3dpp_get_segments3d(self.h, _p(a), n)
         return a
 
     def residuals(self):
-        n = self.L.l3dpp_get_residuals(self.h, None, C.c_longlong(0))
+        n = self.L.l3dpp_get_residuals(self.h, None, 0)
         a = np.zeros(n, RESID_DT)
         if n:
-            self.L.l3dpp_get_residuals(self.h, _p(a), C.c_longlong(n))
+            self.L.l3dpp_get_residuals(self.h, _p(a), n)
         return a
 
     def save_txt(self, folder):
@@ -232,8 +210,7 @@ class Line3D:
 
     def lines(self):
         """get3Dlines() with every field, in the layout read_lines_bin returns"""
-        self.L.l3dpp_lines_handle.restype = C.c_void_p
-        return _lines_from_handle(_io_lib(), C.c_void_p(self.L.l3dpp_lines_handle(self.h)))
+        return _lines_from_handle(self.L, self.L.l3dpp_lines_handle(self.h))
 
     def save_bin(self, folder):
         """save3DLinesAsBIN: <folder>/<createOutputFilename()>.bin; nothing is written (and L3DError is raised) without 3D lines"""
@@ -251,24 +228,16 @@ BIN_SEG_DT = np.dtype([("line", "<i4"), ("valid", "<i4"), ("length", "<f4"), ("_
                        ("dir", "<f8", 3)])
 
 
-def _io_lib():
-    L = capi.lib()
-    for n in ("l3dpp_bin_open", "l3dpp_segcache_open"):
-        getattr(L, n).restype = C.c_void_p
-    L.l3dpp_segcache_count.restype = C.c_longlong
-    return L
-
-
 def read_lines_bin(path):
     """read3DLinesBIN: a .bin result file as numpy arrays.  Returns dict(lines: LINE_DT [L] (segment / residual counts, reference
     view), clusters: BIN_SEG_DT [L] (each cluster's own 3D line), segments: BIN_SEG_DT [S], residuals: RESID_DT [R]); segments and
     residuals of line i are consecutive and carry line = i.  Raises L3DError with the reader's message on a malformed file."""
-    L = _io_lib()
+    L = capi.lib()
     err = C.create_string_buffer(1024)
     h = L.l3dpp_bin_open(str(path).encode(), err, 1024)
     if not h:
         raise capi.L3DError(err.value.decode())
-    return _lines_from_handle(L, C.c_void_p(h))
+    return _lines_from_handle(L, h)
 
 
 def _lines_from_handle(L, h):
@@ -293,18 +262,17 @@ def write_lines_bin(path, d):
     if len(clusters) != len(lines) or lines["nseg"].sum() != len(segs) or lines["nres"].sum() != len(res):
         raise ValueError("clusters must have one entry per line, and the per-line counts must add up to the segment / residual arrays")
     err = C.create_string_buffer(1024)
-    if _io_lib().l3dpp_bin_write(str(path).encode(), C.c_longlong(len(lines)), _p(lines), _p(clusters), _p(segs), _p(res), err, 1024) != 0:
+    if capi.lib().l3dpp_bin_write(str(path).encode(), len(lines), _p(lines), _p(clusters), _p(segs), _p(res), err, 1024) != 0:
         raise capi.L3DError(err.value.decode())
 
 
 def read_segment_cache(path):
     """readSegmentCache: a view's cached 2D segments as float32 [n, 4] (x1, y1, x2, y2)"""
-    L = _io_lib()
+    L = capi.lib()
     err = C.create_string_buffer(1024)
     h = L.l3dpp_segcache_open(str(path).encode(), err, 1024)
     if not h:
         raise capi.L3DError(err.value.decode())
-    h = C.c_void_p(h)
     try:
         out = np.zeros((L.l3dpp_segcache_count(h), 4), np.float32)
         L.l3dpp_segcache_get(h, _p(out))
@@ -317,14 +285,14 @@ def write_segment_cache(path, segs):
     """writeSegmentCache of float32 [n, 4] segments"""
     segs = np.ascontiguousarray(segs, np.float32).reshape(-1, 4)
     err = C.create_string_buffer(1024)
-    if _io_lib().l3dpp_segcache_write(str(path).encode(), _p(segs), C.c_longlong(len(segs)), err, 1024) != 0:
+    if capi.lib().l3dpp_segcache_write(str(path).encode(), _p(segs), len(segs), err, 1024) != 0:
         raise capi.L3DError(err.value.decode())
 
 
 def segment_cache_path(output_folder, cam, width, height, max_img_width=-1):
     """segmentCachePath: <output_folder>/L3D++_data/segments_L3D++_<cam>_<w>x<h>_3000.bin"""
     buf = C.create_string_buffer(4096)
-    n = _io_lib().l3dpp_segcache_path(str(output_folder).encode(), C.c_uint(int(cam)), int(width), int(height), int(max_img_width), buf, 4096)
+    n = capi.lib().l3dpp_segcache_path(str(output_folder).encode(), int(cam), int(width), int(height), int(max_img_width), buf, 4096)
     if n < 0:
         raise ValueError("path too long")
     return buf.value.decode()
@@ -355,26 +323,23 @@ def _sfm_cameras(L, h, lenses=False):
     return cams
 
 
-def _read_sfm(kind, path, aux="", device=0):
+# the model kinds of l3dpp_sfm_open (L3DPP_SFM_* of include/l3dpp_capi.h)
+SFM_BUNDLER, SFM_COLMAP, SFM_MAVMAP, SFM_OPENMVG, SFM_PIX4D, SFM_COLMAP_LENSES = range(6)
+
+
+def _read_sfm(kind, path, aux=""):
     L = capi.lib()
-    L.l3dpp_sfm_read.restype = C.c_void_p
     err = C.create_string_buffer(4096)
-    h = L.l3dpp_sfm_read(int(kind), str(path).encode(), str(aux).encode(), int(device), err, 4096)
+    h = L.l3dpp_sfm_open(int(kind), str(path).encode(), str(aux).encode(), err, 4096)
     if not h:
         raise capi.L3DError(err.value.decode(errors="replace"))
-    return _sfm_cameras(L, C.c_void_p(h))
+    return _sfm_cameras(L, h, lenses=kind == SFM_COLMAP_LENSES)
 
 
 def read_colmap(sfm_folder):
     """readColmap with lenses: the cameras of a COLMAP model (cameras/images/points3D .txt, or else .bin), each with a `lens` dict
     {model: capi.LENS_RADTAN | capi.LENS_FISHEYE, k: k1..k6, p: p1, p2} for undistort_image.  Raises L3DError on a malformed model."""
-    L = capi.lib()
-    L.l3dpp_sfm_open.restype = C.c_void_p
-    err = C.create_string_buffer(4096)
-    h = L.l3dpp_sfm_open(5, str(sfm_folder).encode(), b"", err, 4096)
-    if not h:
-        raise capi.L3DError(err.value.decode(errors="replace"))
-    return _sfm_cameras(L, C.c_void_p(h), lenses=True)
+    return _read_sfm(SFM_COLMAP_LENSES, sfm_folder)
 
 
 def undistort_image(img, K, lens, device=0):
@@ -398,30 +363,30 @@ def undistort_image(img, K, lens, device=0):
 
 def read_mavmap(path):
     """readMavmap: the cameras of a mavmap result file (no world points; see sequential_neighbors).  Raises L3DError on malformed input."""
-    return _read_sfm(2, path)
+    return _read_sfm(SFM_MAVMAP, path)
 
 
 def read_openmvg(sfm_data_json):
     """readOpenMVG: the cameras of an OpenMVG sfm_data.json with world-point lists and median depths"""
-    return _read_sfm(3, sfm_data_json)
+    return _read_sfm(SFM_OPENMVG, sfm_data_json)
 
 
-def read_pix4d(params_folder, project_prefix, device=0):
-    """readPix4D: the cameras of a Pix4D project; its tie points are triangulated on GPU `device` (L3DError without one)"""
-    return _read_sfm(4, params_folder, project_prefix, device)
+def read_pix4d(params_folder, project_prefix):
+    """readPix4D: the cameras of a Pix4D project; its tie points are triangulated on CUDA device 0 (L3DError without one)"""
+    return _read_sfm(SFM_PIX4D, params_folder, project_prefix)
 
 
 def sequential_neighbors(i, n_cams, num_neighbors):
     """sequentialNeighbors: the mavmap frontend's neighbour list of camera i"""
     out = np.zeros(max(int(num_neighbors), 1), np.uint32)
-    n = capi.lib().l3dpp_sequential_neighbors(C.c_uint(int(i)), C.c_uint(int(n_cams)), C.c_uint(int(num_neighbors)), _p(out), len(out))
+    n = capi.lib().l3dpp_sequential_neighbors(int(i), int(n_cams), int(num_neighbors), _p(out), len(out))
     return out[:n].tolist()
 
 
 def rotation_from_rpy(roll, pitch, yaw):
     """Line3D::rotationFromRPY"""
     R = np.zeros(9)
-    capi.lib().l3dpp_rotation_from_rpy(C.c_double(roll), C.c_double(pitch), C.c_double(yaw), _p(R))
+    capi.lib().l3dpp_rotation_from_rpy(roll, pitch, yaw, _p(R))
     return R.reshape(3, 3)
 
 

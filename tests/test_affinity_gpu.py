@@ -23,7 +23,6 @@ def _scored_context(sc):
     descs = capi.make_view_descs(sc.cam_ids, [sc.width] * V, [sc.height] * V, [len(s) for s in sc.segs], RtKinv, Cw, Cw, k, sc.median_depth)
     pairs = synth.view_pairs(sc.neighbors, sc.cam_ids)
     ctx = capi.Context(0)
-    ctx.L.l3d_affinity_edges.restype = ctx.L.l3d_affinity_matrix.restype = C.c_longlong
     ctx.set_views(descs, sc.segs)
     ctx.match_pairs(pairs, util.pair_F(sc, pairs))
     assert ctx.L.l3d_score_sweep(ctx.h, C.c_float(TWO_SIGA_SQR), C.c_float(.5), C.c_float(.75), C.c_float(.1)) == 0

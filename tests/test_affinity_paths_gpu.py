@@ -55,8 +55,6 @@ class Run:
                                                       self.k[o], md[o])
         ctx = self.ctx = capi.Context(0)
         L = ctx.L
-        for f in ("l3d_affinity_edges", "l3d_affinity_matrix", "l3d_get_view_matches", "l3d_get_estimates", "l3d_rdd_affinity"):
-            getattr(L, f).restype = C.c_longlong
         ctx.set_views(self.descs(self.md), [sc.segs[v] for v in o])
         pairs = synth.view_pairs(sc.neighbors, sc.cam_ids)                       # camIDs == scene indices
         idx = np.array([[self.pos[int(s)], self.pos[int(t)]] for s, t in pairs], np.int32).reshape(-1, 2)

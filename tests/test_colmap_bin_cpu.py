@@ -1,6 +1,5 @@
 """L3DPP::readColmap on COLMAP's binary model (cameras.bin / images.bin / points3D.bin) and on every lens model it reads, against an
 independent writer of both formats (COLMAP's documented layouts, written here with struct.pack / text formatting)."""
-import ctypes
 import struct
 
 import numpy as np
@@ -97,14 +96,11 @@ def write_bin(folder, cameras, images, pts):
 
 
 def read_plain(folder):
-    """readColmap without lenses (l3dpp_sfm_open kind 1): (cameras as dicts, '') or (None, error)"""
-    L = capi.lib()
-    L.l3dpp_sfm_open.restype = ctypes.c_void_p
-    err = ctypes.create_string_buffer(1024)
-    h = L.l3dpp_sfm_open(1, str(folder).encode(), b"", err, 1024)
-    if not h:
-        return None, err.value.decode()
-    return line3d._sfm_cameras(L, ctypes.c_void_p(h)), ""
+    """readColmap without lenses (L3DPP_SFM_COLMAP): (cameras as dicts, '') or (None, error)"""
+    try:
+        return line3d._read_sfm(line3d.SFM_COLMAP, folder), ""
+    except capi.L3DError as e:
+        return None, str(e)
 
 
 def read_lenses(folder):

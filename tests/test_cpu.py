@@ -351,9 +351,8 @@ def test_oracle_cluster_tail_reproduces_the_reference_result_file(oracle):
 
 # ---------------------------------------------------------------------------------------------- .nvm input format (SURVEY §8f-2)
 def _read_nvm_product(path):
-    from line3dpp_b200 import build
-    L = ctypes.CDLL(build.build())
-    L.l3dpp_nvm_open.restype = ctypes.c_void_p
+    from line3dpp_b200 import capi
+    L = capi.lib()
     err = ctypes.create_string_buffer(256)
     h = L.l3dpp_nvm_open(str(path).encode(), err, 256)
     if not h:
@@ -427,8 +426,8 @@ def test_nvm_reader_on_the_reference_test_data(tmp_path):
     _, wps, depths = read_nvm(path)
     cams, err = _read_nvm_product(path)
     assert cams is not None and len(cams) == inp["V"], err
-    from line3dpp_b200 import build
-    L = ctypes.CDLL(build.build())
+    from line3dpp_b200 import capi
+    L = capi.lib()
     for i, c in enumerate(cams):
         np.testing.assert_allclose(c["R"], inp["R"][i], atol=1e-15)
         np.testing.assert_allclose(c["t"], inp["t"][i], atol=1e-13)
@@ -438,19 +437,6 @@ def test_nvm_reader_on_the_reference_test_data(tmp_path):
         L.l3dpp_intrinsics_from_focal(ctypes.c_float(c["f"]), int(inp["wh"][i][0]), int(inp["wh"][i][1]), K.ctypes.data_as(ctypes.c_void_p))
         assert np.array_equal(K.reshape(3, 3), inp["K"][i])
     assert sum(len(c["wps"]) for c in cams) > 10000
-
-# ---------------------------------------------------------------------------------------------- product library surface
-def test_capi_library_loads_and_exports_every_declared_symbol():
-    from line3dpp_b200 import build
-    so = build.build()
-    lib = ctypes.CDLL(so)
-    hdr = open(os.path.join(ROOT, "include", "l3d_capi.h")).read()
-    names = sorted(set(re.findall(r"\b(l3d_[a-z0-9_]+)\s*\(", hdr)))
-    assert len(names) >= 20
-    for n in names:
-        assert hasattr(lib, n), f"{n} declared in include/l3d_capi.h but not exported"
-    for n in ("l3dpp_create", "l3dpp_add_image", "l3dpp_match_images", "l3dpp_reconstruct", "l3dpp_save_txt"):
-        assert hasattr(lib, n)
 
 
 def test_nvm_reader_rejects_truncated_camera_list(tmp_path):
@@ -465,9 +451,8 @@ def test_nvm_reader_rejects_truncated_camera_list(tmp_path):
 
 
 def _read_sfm_product(kind, path, aux=""):
-    from line3dpp_b200 import build
-    L = ctypes.CDLL(build.build())
-    L.l3dpp_sfm_open.restype = ctypes.c_void_p
+    from line3dpp_b200 import capi
+    L = capi.lib()
     err = ctypes.create_string_buffer(256)
     h = L.l3dpp_sfm_open(kind, str(path).encode(), str(aux).encode(), err, 256)
     if not h:

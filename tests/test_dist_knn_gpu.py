@@ -260,7 +260,6 @@ def _sweep(c):
 
 
 def _estimates(c):
-    c.L.l3d_get_estimates.restype = C.c_longlong
     n = c.L.l3d_get_estimates(c.h, None, None, C.c_longlong(0))
     if n < 0:
         return n

@@ -170,7 +170,6 @@ def test_postprocess_restatement_equals_priority_queue(pq_exe, case):
     model = pm.postprocess(det, w, h, wp, hp, mx)
     assert model.tobytes() == ref.tobytes()
     L = capi.lib()
-    L.l3dpp_filter_detections.restype = C.c_longlong
     lib_out = np.zeros((max(len(det), 1), 4), np.float32)
     n = L.l3dpp_filter_detections(det.ctypes.data_as(C.c_void_p), C.c_longlong(len(det)), w, h, wp, hp, C.c_uint(mx),
                                   lib_out.ctypes.data_as(C.c_void_p), C.c_longlong(len(lib_out)))

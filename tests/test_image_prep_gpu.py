@@ -178,11 +178,12 @@ def test_detector_sees_the_prepared_image_and_the_cache_is_written(inp, image, g
 
 
 def test_cut_at_max_line_segments(inp, image, tmp_path):
-    L = line3d.Line3D(True, True, output_folder=str(tmp_path), load_segments=False, max_img_width=MW, max_line_segments=500)
-    L.set_segment_detector(lambda g: detections(inp, 1))
-    _add(L, inp, 1, image)
-    assert L.view_segments(1).tobytes() == expected(inp, 1, 500).tobytes()
-    L.close()
+    for devices in (None, [0]):                  # the device-list constructor takes max_line_segments as well
+        L = line3d.Line3D(True, True, output_folder=str(tmp_path), load_segments=False, max_img_width=MW, max_line_segments=500, devices=devices)
+        L.set_segment_detector(lambda g: detections(inp, 1))
+        _add(L, inp, 1, image)
+        assert L.view_segments(1).tobytes() == expected(inp, 1, 500).tobytes(), devices
+        L.close()
 
 
 def test_without_load_segments_nothing_is_written(inp, image, tmp_path):

@@ -373,7 +373,6 @@ def test_new_match_drops_affinity(rematch):
     F = util.pair_F(sc, pairs)
     ctx = capi.Context(0)
     L = ctx.L
-    L.l3d_affinity_matrix.restype = L.l3d_rdd_affinity.restype = C.c_longlong
     ctx.set_views(descs, sc.segs)
     ctx.match_pairs(pairs, F)
     assert L.l3d_score_sweep(ctx.h, C.c_float(200), C.c_float(.5), C.c_float(.75), C.c_float(.1)) == 0

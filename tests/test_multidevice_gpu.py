@@ -117,7 +117,6 @@ def _job(sc):
 
 def _ctx(sc, descs):
     c = capi.Context(0)
-    c.L.l3d_match_total_matches.restype = C.c_longlong
     c.set_views(descs, sc.segs)
     return c
 

@@ -80,7 +80,6 @@ def affinity_ctx(request):
     else:
         ctx, med = _scored_context(synth.make_scene(12, 500, 93, "ring3", collinear=True))
         assert ctx.find_collinear(2.0, 0) > 1000
-    ctx.L.l3d_rdd_affinity.restype = C.c_longlong
     ei, ej, ew, l2g = affinity_matrix(ctx, med)
     yield ctx, ei, ej, ew, len(l2g)
     ctx.close()

@@ -171,7 +171,6 @@ def test_undistort_calls_leave_the_pipeline_results_alone(gold):
     pairs = synth.view_pairs(sc.neighbors, sc.cam_ids)
     ctx = capi.Context(0)
     L = ctx.L
-    L.l3d_affinity_matrix.restype = L.l3d_rdd_affinity.restype = L.l3d_get_view_matches.restype = C.c_longlong
     p = lambda a: a.ctypes.data_as(C.c_void_p)
     ctx.set_views(descs, sc.segs)
     ctx.match_pairs(pairs, util.pair_F(sc, pairs))

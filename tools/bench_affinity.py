@@ -53,8 +53,6 @@ def scored_context(sc):
     pairs = synth.view_pairs(sc.neighbors, sc.cam_ids)
     F = np.stack([synth.fundamental(sc.K[s], sc.R[s], sc.t[s], sc.K[t], sc.R[t], sc.t[t]).astype(np.float32).reshape(9) for s, t in pairs])
     ctx = capi.Context(0)
-    for f in ("l3d_affinity_edges", "l3d_affinity_matrix", "l3d_rdd_affinity"):
-        getattr(ctx.L, f).restype = C.c_longlong
     ctx.set_views(descs, sc.segs)
     ctx.match_pairs(pairs, F, EPI, KNN)
     ctx._chk(ctx.L.l3d_score_sweep(ctx.h, C.c_float(TWO_SIGA_SQR), C.c_float(.5), C.c_float(.75), C.c_float(.1)), "l3d_score_sweep")

@@ -41,8 +41,8 @@ class ParentDesc(C.Structure):
 class Lib:
     """one library's context: create, undistort on device, stream"""
     def __init__(self, path, desc_type):
-        self.L = C.CDLL(path)
-        self.L.l3d_stream.restype = C.c_void_p
+        from line3dpp_b200 import capi
+        self.L = capi.bind(C.CDLL(path), capi.HEADERS[:1])      # include/l3d_capi.h: the ABI both builds export
         self.h = C.c_void_p()
         assert self.L.l3d_ctx_create(0, C.byref(self.h)) == 0, path
         self.desc_type = desc_type

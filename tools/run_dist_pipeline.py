@@ -12,7 +12,6 @@ matches_after_knn x 24 B).
         tools/run_dist_pipeline.py --views 1000 --segs 3000 --ring 5 --diffusion 1 [--knn 10] [--check-views 60] [--reps 2]
 """
 import argparse
-import ctypes
 import hashlib
 import json
 import os
@@ -106,7 +105,6 @@ def main():
         if best is None or cur["matchImages_s"] + cur["reconstruct_s"] < best["matchImages_s"] + best["reconstruct_s"]:
             best = cur
     st = L.stats()
-    L.L.l3d_match_total_rows.restype = ctypes.c_longlong
     stride, rows = int(L.L.l3d_match_stride(L.ctx)), int(L.L.l3d_match_total_rows(L.ctx))
     free1, _ = torch.cuda.mem_get_info()
     keys = sorted(best)
