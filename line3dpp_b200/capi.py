@@ -422,6 +422,12 @@ class Context:
                   "l3d_median_depths")
         return cnt, med
 
+    def median_depths_device(self, n_cams, list_ptr, list_pts, n_points, X, valid, centres, count_out, median_out):
+        """l3d_median_depths on device addresses; asynchronous on the context's stream apart from reading list_ptr[n_cams] (a point id
+        outside [0, n_points) counts as invalid)"""
+        self._chk(self.L.l3d_median_depths(self.h, int(n_cams), int(list_ptr), int(list_pts), int(n_points), int(X), int(valid), int(centres),
+                                           int(count_out), int(median_out), 1), "l3d_median_depths")
+
     # ---- lens undistortion (stateless: no pipeline stage changes)
     def undistort(self, images, K, radial=(0, 0, 0), tangential=(0, 0), out=None, lens=None):
         """Line3D::undistortImage for a list of uint8 HxW / HxWx3 images in ONE batched call.  K, radial, tangential: one camera for
