@@ -93,7 +93,7 @@ int l3dpp_undistort_image(const unsigned char* src, unsigned char* dst, int rows
 int l3dpp_undistort_image_lens(const unsigned char* src, unsigned char* dst, int rows, int cols, int channels, const double* lens9, const double* K,
                                int device);
 
-/* ---- .nvm models (csrc/line3d_io.cc) */
+/* ---- .nvm models (csrc/line3d_sfm.cc) */
 void* l3dpp_nvm_open(const char* path, char* err, int errcap);
 void l3dpp_nvm_close(void* h);
 int l3dpp_nvm_num_cameras(void* h);
@@ -102,7 +102,7 @@ int l3dpp_nvm_camera(void* h, int i, double* R9, double* t3, double* C3, float* 
 int l3dpp_nvm_worldpoints(void* h, int i, unsigned int* out, int cap);
 void l3dpp_intrinsics_from_focal(float focal, int w, int h, double* K9);
 
-/* ---- the other SfM models (csrc/line3d_io.cc, csrc/line3d_sfm.cc) */
+/* ---- the other SfM models (csrc/line3d_sfm.cc) */
 #define L3DPP_SFM_BUNDLER 0         /* path = the bundle file, aux = the image list */
 #define L3DPP_SFM_COLMAP 1          /* path = the sparse model folder (.txt, or else .bin) */
 #define L3DPP_SFM_MAVMAP 2          /* path = the result file */

@@ -1,6 +1,7 @@
 /* include/line3d_io.h — input formats of the reference's six frontends (SURVEY.md §8f-2): what main_*.cpp read from an SfM model
  * before they call Line3D::addImage, as library functions so that a frontend built on include/line3d.h needs no parsing code of its
- * own; and the reference's binary result file and segment cache.  Host code; readPix4D triangulates through include/l3d_capi.h. */
+ * own (csrc/line3d_sfm.cc, DESIGN.md §6b); and the reference's binary result file and segment cache (csrc/line3d_bin.cc).  Host
+ * code; readPix4D triangulates through include/l3d_capi.h. */
 #ifndef L3DPP_LINE3D_IO_H_
 #define L3DPP_LINE3D_IO_H_
 #include "line3d.h"
@@ -22,7 +23,8 @@ struct NVMCamera {
     float median_depth;                    /* median distance of those points to C; 0 if there are none (camera is skipped) */
 };
 
-/* Reads an NVM_V3 file like main_vsfm.cpp:143-250.  Returns false and sets *error on an unreadable or empty model. */
+/* Reads an NVM_V3 file like main_vsfm.cpp:143-250.  Returns false and sets *error on an unreadable, empty or malformed model; a
+ * header that claims more cameras than the file holds is a truncated camera list. */
 bool readNVM(const std::string& path, std::vector<NVMCamera>& cameras, std::string* error = 0);
 
 /* one camera of a Bundler, COLMAP, mavmap, OpenMVG or Pix4D model, ready for Line3D::addImage.  Bundler has no K in the file (focal
@@ -55,9 +57,9 @@ bool readBundler(const std::string& bundle_file, const std::string& image_list_f
  * makes it allocate more than the file's size warrants; ids that do not fit unsigned int are rejected. */
 bool readColmap(const std::string& sfm_folder, std::vector<SfMCamera>& cameras, std::string* error = 0, std::vector<LensDistortion>* lenses = 0);
 
-/* The mavmap, OpenMVG and Pix4D models (csrc/line3d_sfm.cc, DESIGN.md §6b).  Like the readers above: false with *error naming the
- * file, the line or JSON path and the problem on malformed input, which never crashes the reader and never makes it allocate more
- * than the input's size warrants.  Every camera has has_K set. */
+/* The mavmap, OpenMVG and Pix4D models.  Like the readers above: false with *error naming the file, the line or JSON path and the
+ * problem on malformed input, which never crashes the reader and never makes it allocate more than the input's size warrants.
+ * Every camera has has_K set. */
 
 /* mavmap's result file like main_mavmap.cpp:153-250: leading '#' lines skipped, a line shorter than 28 characters ends the list, every
  * field carries a trailing comma, only the PINHOLE model; R = rotationFromRPY(roll, pitch, yaw) and [R|t] inverted (R^T, -R^T t),

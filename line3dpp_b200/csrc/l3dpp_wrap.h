@@ -1,18 +1,9 @@
-// l3dpp_wrap.h — what the C wrappers of the host files share (include/l3dpp_capi.h; line3d_io.cc, line3d_bin.cc): the object behind an
-// l3dpp_sfm_* handle, and the copy of a message into a caller's buffer.  Host only, header only.
+// l3dpp_wrap.h — what the C wrappers of the host files share (include/l3dpp_capi.h; line3d_sfm.cc, line3d_bin.cc): the copy of a
+// message into a caller's buffer.  Host only, header only.
 #ifndef L3DPP_WRAP_H_
 #define L3DPP_WRAP_H_
-#include "../../include/line3d_io.h"
-
 #include <cstring>
 #include <string>
-#include <vector>
-
-// the cameras of any SfM reader, and the lenses readColmap returns when asked for them
-struct L3DSfMHandle {
-    std::vector<L3DPP::SfMCamera> cams;
-    std::vector<L3DPP::LensDistortion> lenses;
-};
 
 // s into buf[cap], NUL-terminated and cut to fit; nothing for a null buffer or cap <= 0
 inline void l3dpp_copy_str(const std::string& s, char* buf, int cap)

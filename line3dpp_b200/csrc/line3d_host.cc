@@ -1033,17 +1033,6 @@ void Line3D::saveResultAsSTL(const std::string& folder)
     f << "endsolid lineModel" << std::endl;
 }
 
-Matrix3d Line3D::rotationFromQ(const double Qw, const double Qx, const double Qy, const double Qz)   // line3D.cc:2737-2754
-{
-    const double n = std::sqrt(Qw * Qw + Qx * Qx + Qy * Qy + Qz * Qz);
-    const double w = Qw / n, x = Qx / n, y = Qy / n, z = Qz / n;
-    Matrix3d R;
-    R(0, 0) = 1 - 2 * y * y - 2 * z * z; R(0, 1) = 2 * x * y - 2 * z * w; R(0, 2) = 2 * x * z + 2 * y * w;
-    R(1, 0) = 2 * x * y + 2 * z * w; R(1, 1) = 1 - 2 * x * x - 2 * z * z; R(1, 2) = 2 * y * z - 2 * x * w;
-    R(2, 0) = 2 * x * z - 2 * y * w; R(2, 1) = 2 * y * z + 2 * x * w; R(2, 2) = 1 - 2 * x * x - 2 * y * y;
-    return R;
-}
-
 void Line3D::undistortImage(const Image8u& in, Image8u& out, const Vector3d& radial, const Vector2d& tangential, const Matrix3d& K)
 {
     LensDistortion lens;

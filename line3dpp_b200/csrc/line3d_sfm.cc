@@ -1,32 +1,85 @@
-// line3d_sfm.cc — the input side of the reference's mavmap, OpenMVG and Pix4D frontends (main_mavmap.cpp:153-321,
-// main_openmvg.cpp:136-410, main_pix4d.cpp:163-420) as library readers, and the two static helpers only these frontends use
-// (Line3D::rotationFromRPY, Line3D::decomposeProjectionMatrix).  Host code; the Pix4D reader triangulates its tie points and computes
-// the median depths through the C ABI (l3d_triangulate_points, l3d_median_depths).  The file needs no CUDA header, so it builds
-// alone (with stand-ins for those two entries) for the sanitizer test.
+// line3d_sfm.cc — the input side of the reference's six frontends as library readers: NVM (main_vsfm.cpp:143-310), Bundler
+// (main_bundler.cpp:143-286), COLMAP text and binary (main_colmap.cpp:140-401), mavmap (main_mavmap.cpp:153-321), OpenMVG
+// (main_openmvg.cpp:136-410) and Pix4D (main_pix4d.cpp:163-420); the static helpers only these frontends use (Line3D::rotationFromQ,
+// rotationFromRPY, decomposeProjectionMatrix); and their C wrappers.  Host code; the Pix4D reader triangulates its tie points and
+// computes the median depths through the C ABI (l3d_triangulate_points, l3d_median_depths).  The file needs no CUDA header, so it
+// builds alone (with stand-ins for those two entries) for the sanitizer test.
 //
-// Every reader takes input from outside the program: a malformed file returns false with *error naming the file, the line or JSON
-// path and the problem; nothing is allocated beyond what the bytes read justify; JSON nesting is capped at JSON_MAX_DEPTH.
+// Every reader takes input from outside the program: a malformed file returns false with *error naming the file and the problem
+// (the line or JSON path where the format has them); nothing is allocated beyond what the bytes read justify, whatever count a header
+// claims; JSON nesting is capped at JSON_MAX_DEPTH.
 #include "../../include/line3d_io.h"
 #include "../../include/l3d_capi.h"
 #include "../../include/l3dpp_capi.h"
+#include "l3dpp_wrap.h"
 
 #include <algorithm>
 #include <cmath>
+#include <cstdint>
 #include <cstdlib>
 #include <cstring>
 #include <fstream>
+#include <iterator>
 #include <map>
 #include <sstream>
 
 namespace L3DPP {
 
+// ------------------------------------------------------------------------------------------------ camera algebra
+// Every product sums left to right.  The negations come after the sums: -(a + b) is -0 where (-a) + (-b) is +0, so the two spellings
+// are not interchangeable when a component cancels exactly.
+static Matrix3d zero3() { Matrix3d m; std::memset(m.m, 0, sizeof(m.m)); return m; }
+static Vector3d neg(const Vector3d& v) { return Vector3d(-v.x, -v.y, -v.z); }
+static Vector3d mul(const Matrix3d& R, const Vector3d& v)
+{
+    return Vector3d(R(0, 0) * v.x + R(0, 1) * v.y + R(0, 2) * v.z, R(1, 0) * v.x + R(1, 1) * v.y + R(1, 2) * v.z,
+                    R(2, 0) * v.x + R(2, 1) * v.y + R(2, 2) * v.z);
+}
+static Vector3d mul_transposed(const Matrix3d& R, const Vector3d& v)      // R^T v
+{
+    return Vector3d(R(0, 0) * v.x + R(1, 0) * v.y + R(2, 0) * v.z, R(0, 1) * v.x + R(1, 1) * v.y + R(2, 1) * v.z,
+                    R(0, 2) * v.x + R(1, 2) * v.y + R(2, 2) * v.z);
+}
+static Vector3d translation_of(const Matrix3d& R, const Vector3d& C) { return neg(mul(R, C)); }           // t = -R C
+static Vector3d center_of(const Matrix3d& R, const Vector3d& t) { return neg(mul_transposed(R, t)); }    // C = -R^T t
+
+// |C - X| rounded to float: the reference keeps depths in float vectors (main_vsfm.cpp:228, main_colmap.cpp:386-401)
+static float point_depth(const Vector3d& C, const Vector3d& X)
+{
+    const double dx = C.x - X.x, dy = C.y - X.y, dz = C.z - X.z;
+    return (float)std::sqrt(dx * dx + dy * dy + dz * dz);
+}
+
+// element size/2 of the sorted depths; 0 for none
+static float median_of(std::vector<float>& d)
+{
+    if (d.empty()) return 0.0f;
+    std::sort(d.begin(), d.end());
+    return d[d.size() / 2];
+}
+
 // ------------------------------------------------------------------------------------------------ helpers on Line3D
+// the rotation of a unit quaternion (line3D.cc:2737-2754 after its normalisation; main_vsfm.cpp:193-203 uses it as stored)
+static Matrix3d quaternion_matrix(double w, double x, double y, double z)
+{
+    Matrix3d R;
+    R(0, 0) = 1.0 - 2.0 * y * y - 2.0 * z * z; R(0, 1) = 2.0 * x * y - 2.0 * z * w; R(0, 2) = 2.0 * x * z + 2.0 * y * w;
+    R(1, 0) = 2.0 * x * y + 2.0 * z * w; R(1, 1) = 1.0 - 2.0 * x * x - 2.0 * z * z; R(1, 2) = 2.0 * y * z - 2.0 * x * w;
+    R(2, 0) = 2.0 * x * z - 2.0 * y * w; R(2, 1) = 2.0 * y * z + 2.0 * x * w; R(2, 2) = 1.0 - 2.0 * x * x - 2.0 * y * y;
+    return R;
+}
+
+Matrix3d Line3D::rotationFromQ(const double Qw, const double Qx, const double Qy, const double Qz)   // line3D.cc:2737-2754
+{
+    const double n = std::sqrt(Qw * Qw + Qx * Qx + Qy * Qy + Qz * Qz);
+    return quaternion_matrix(Qw / n, Qx / n, Qy / n, Qz / n);
+}
+
 // Eigen's AngleAxisd(angle, axis).toRotationMatrix() for a unit axis e_k: the diagonal entry of the axis is (1 - c) + c
 static Matrix3d axis_rotation(double angle, int k)
 {
     const double s = std::sin(angle), c = std::cos(angle);
-    Matrix3d R;
-    std::memset(R.m, 0, sizeof(R.m));
+    Matrix3d R = zero3();
     const int i = (k + 1) % 3, j = (k + 2) % 3;
     R(k, k) = (1.0 - c) + c;
     R(i, i) = c; R(j, j) = c;
@@ -53,8 +106,7 @@ void Line3D::decomposeProjectionMatrix(const double P[12], Matrix3d& K, Matrix3d
     for (int r = 0; r < 3; ++r)
         for (int c = 0; c < 3; ++c) K(r, c) = P[4 * r + c];
     auto givens = [](int a, int b, double s, double c) {      // identity with c at (a,a), (b,b); -s at (a,b); s at (b,a)
-        Matrix3d G;
-        std::memset(G.m, 0, sizeof(G.m));
+        Matrix3d G = zero3();
         G(3 - a - b, 3 - a - b) = 1.0;
         G(a, a) = c; G(b, b) = c; G(a, b) = -s; G(b, a) = s;
         return G;
@@ -68,8 +120,7 @@ void Line3D::decomposeProjectionMatrix(const double P[12], Matrix3d& K, Matrix3d
     h = std::sqrt(K(1, 0) * K(1, 0) + K(1, 1) * K(1, 1));
     const Matrix3d Rz = givens(0, 1, K(1, 0) / h, -K(1, 1) / h);
     K = mul(K, Rz);
-    Matrix3d Sign;
-    std::memset(Sign.m, 0, sizeof(Sign.m));
+    Matrix3d Sign = zero3();
     for (int i = 0; i < 3; ++i) Sign(i, i) = K(i, i) < 0 ? -1.0 : 1.0;
     K = mul(K, Sign);                                      // change the sign of columns
     const Matrix3d Rt = mul(mul(mul(Rx, Ry), Rz), Sign);
@@ -84,9 +135,7 @@ void Line3D::decomposeProjectionMatrix(const double P[12], Matrix3d& K, Matrix3d
     Matrix3d Ki;
     for (int r = 0; r < 3; ++r)
         for (int c = 0; c < 3; ++c) Ki(r, c) = cof(c, r) * invdet;
-    const double p4[3] = {P[3], P[7], P[11]};
-    t = Vector3d(Ki(0, 0) * p4[0] + Ki(0, 1) * p4[1] + Ki(0, 2) * p4[2], Ki(1, 0) * p4[0] + Ki(1, 1) * p4[1] + Ki(1, 2) * p4[2],
-                 Ki(2, 0) * p4[0] + Ki(2, 1) * p4[1] + Ki(2, 2) * p4[2]);
+    t = mul(Ki, Vector3d(P[3], P[7], P[11]));
     const double n = 1.0 / K(2, 2);                        // normalise so that K(2,2) = 1
     for (int i = 0; i < 9; ++i) K.m[i] *= n;
 }
@@ -100,8 +149,15 @@ std::list<unsigned int> sequentialNeighbors(unsigned int i, unsigned int n_cams,
     return nb;
 }
 
+Matrix3d intrinsicsFromFocal(float focal, int w, int h)
+{
+    Matrix3d K = zero3();
+    K(0, 0) = focal; K(1, 1) = focal; K(0, 2) = float(w) / 2.0f; K(1, 2) = float(h) / 2.0f; K(2, 2) = 1.0;
+    return K;
+}
+
 // ------------------------------------------------------------------------------------------------ shared parsing helpers
-static bool fail(std::string* error, const std::string& msg) { if (error) *error = msg; return false; }
+static bool fail(std::string* error, const std::string& msg) { if (error) error->assign(msg); return false; }
 
 // the whole token must be a number (strtod: correctly rounded, like the reference's stream extraction)
 static bool to_double(const std::string& tok, double& v)
@@ -122,7 +178,8 @@ static bool read_numbers(const std::string& line, double* out, int n)
     return true;
 }
 
-static Matrix3d zero3() { Matrix3d m; std::memset(m.m, 0, sizeof(m.m)); return m; }
+// a camera's K, the radial / tangential distortion the frontend undistorts with and (COLMAP only) its full lens
+struct Intrinsics { Matrix3d K; double radial[3], tangential[2]; LensDistortion lens; };
 
 static SfMCamera empty_camera(unsigned int id)
 {
@@ -130,6 +187,334 @@ static SfMCamera empty_camera(unsigned int id)
     c.id = id; c.has_K = true; c.K = zero3(); c.focal = 0.0f; c.R = zero3(); c.median_depth = 0.0f;
     c.radial[0] = c.radial[1] = c.radial[2] = 0.0; c.tangential[0] = c.tangential[1] = 0.0;
     return c;
+}
+
+// ------------------------------------------------------------------------------------------------ NVM
+// the view list "n  cam feature x y  ..." of point i at X in an NVM or Bundler file: each camera it names gets the point and its depth;
+// false when the list is cut short or names a camera that does not exist
+template <class Cam> static bool add_views(std::istream& s, unsigned int i, const Vector3d& X, std::vector<Cam>& cams, std::vector<std::vector<float> >& depths)
+{
+    unsigned int nviews = 0;
+    s >> nviews;
+    for (unsigned int j = 0; j < nviews; ++j) {
+        unsigned int cam = 0, sift = 0; float x, y;
+        s >> cam >> sift >> x >> y;
+        if (!s || cam >= cams.size()) return false;
+        cams[cam].worldpoints.push_back(i);
+        depths[cam].push_back(point_depth(cams[cam].C, X));
+    }
+    return true;
+}
+
+bool readNVM(const std::string& path, std::vector<NVMCamera>& cams, std::string* error)
+{
+    cams.clear();
+    std::ifstream f(path.c_str());
+    if (!f) return fail(error, "cannot open " + path);
+    std::string line;
+    std::getline(f, line);                       // "NVM_V3"
+    std::getline(f, line);                       // empty
+    std::getline(f, line);
+    unsigned int num_cams = 0;
+    { std::stringstream s(line); s >> num_cams; }
+    if (num_cams == 0) return fail(error, "No aligned cameras in NVM file!");     // main_vsfm.cpp:157-161
+    for (unsigned int i = 0; i < num_cams; ++i) {   // appended as read: a count the file does not hold allocates nothing
+        // a truncated or malformed camera line must not become a default camera (the reference has the same hole, main_vsfm.cpp:168-190)
+        if (!std::getline(f, line)) return fail(error, "unexpected end of file in the camera list of " + path + " (camera " + std::to_string(i) + ")");
+        std::stringstream s(line);
+        NVMCamera c;
+        double focal = 0, qw = 1, qx = 0, qy = 0, qz = 0, Cx = 0, Cy = 0, Cz = 0, dist = 0;
+        if (!(s >> c.image >> focal >> qw >> qx >> qy >> qz >> Cx >> Cy >> Cz >> dist)) return fail(error, "malformed camera line " + std::to_string(i) + " in " + path);
+        c.focal = (float)focal; c.distortion = (float)dist;
+        c.R = quaternion_matrix(qw, qx, qy, qz);   // main_vsfm.cpp:193-203 (the quaternion is used as stored, not re-normalised)
+        c.C = Vector3d(Cx, Cy, Cz);
+        c.t = translation_of(c.R, c.C);
+        c.median_depth = 0.0f;
+        cams.push_back(c);
+    }
+    std::getline(f, line);                       // empty
+    std::getline(f, line);
+    unsigned int num_points = 0;
+    { std::stringstream s(line); s >> num_points; }
+    std::vector<std::vector<float> > depths(cams.size());
+    for (unsigned int i = 0; i < num_points; ++i) {
+        if (!std::getline(f, line)) break;
+        std::istringstream s(line);
+        double px = 0, py = 0, pz = 0, cr, cg, cb;
+        s >> px >> py >> pz >> cr >> cg >> cb;
+        if (!add_views(s, i, Vector3d(px, py, pz), cams, depths)) return fail(error, "malformed measurement list in " + path);
+    }
+    for (size_t i = 0; i < cams.size(); ++i) cams[i].median_depth = median_of(depths[i]);     // main_vsfm.cpp:301-303
+    return true;
+}
+
+// ------------------------------------------------------------------------------------------------ Bundler
+bool readBundler(const std::string& bundle_file, const std::string& image_list_file, std::vector<SfMCamera>& cams, std::string* error)
+{
+    cams.clear();
+    std::ifstream f(bundle_file.c_str());
+    if (!f) return fail(error, "cannot open " + bundle_file);
+    std::string line;
+    std::getline(f, line);                       // "# Bundle file v0.3"
+    std::getline(f, line);
+    unsigned int num_cams = 0, num_points = 0;
+    { std::stringstream s(line); s >> num_cams >> num_points; }
+    if (num_cams == 0 || num_points == 0) return fail(error, "No cameras and/or points in bundle file!");   // main_bundler.cpp:159-163
+    for (unsigned int i = 0; i < num_cams; ++i) {   // appended as read, like the NVM cameras
+        SfMCamera c = empty_camera(i);
+        c.has_K = false;
+        double focal = 0, d1 = 0, d2 = 0;
+        bool good = (bool)std::getline(f, line);
+        if (good) { std::stringstream s(line); good = (bool)(s >> focal >> d1 >> d2); }
+        c.focal = (float)focal;
+        c.radial[0] = (float)d1; c.radial[1] = (float)d2;                                                               // float pair, main_bundler.cpp:170, 183
+        for (int j = 0; j < 3 && good; ++j) { good = (bool)std::getline(f, line); std::stringstream s(line); good = good && (bool)(s >> c.R(j, 0) >> c.R(j, 1) >> c.R(j, 2)); }
+        for (int k = 0; k < 3; ++k) { c.R(1, k) *= -1.0; c.R(2, k) *= -1.0; }                                           // main_bundler.cpp:196-198
+        good = good && (bool)std::getline(f, line);
+        if (good) { std::stringstream s(line); good = (bool)(s >> c.t.x >> c.t.y >> c.t.z); }
+        if (!good) return fail(error, "truncated or malformed camera " + std::to_string(i) + " in " + bundle_file);
+        c.t.y *= -1.0; c.t.z *= -1.0;                                                                                    // main_bundler.cpp:210-212
+        c.C = center_of(c.R, c.t);
+        cams.push_back(c);
+    }
+    std::vector<std::vector<float> > depths(cams.size());
+    for (unsigned int i = 0; i < num_points; ++i) {
+        if (!std::getline(f, line)) break;
+        double px = 0, py = 0, pz = 0;
+        { std::istringstream s(line); s >> px >> py >> pz; }
+        std::getline(f, line);                   // colour
+        std::getline(f, line);                   // view list
+        std::istringstream s(line);
+        if (!add_views(s, i, Vector3d(px, py, pz), cams, depths)) return fail(error, "malformed view list in " + bundle_file);
+    }
+    for (size_t i = 0; i < cams.size(); ++i) cams[i].median_depth = median_of(depths[i]);
+    if (!image_list_file.empty()) {              // main_bundler.cpp:264-286: the first token of line i names image i
+        std::ifstream l(image_list_file.c_str());
+        size_t id = 0;
+        while (std::getline(l, line)) {
+            std::stringstream s(line);
+            std::string fname;
+            s >> fname;
+            if (!fname.empty() && id < cams.size()) cams[id].image = fname;
+            ++id;
+        }
+    }
+    return true;
+}
+
+// ------------------------------------------------------------------------------------------------ COLMAP
+// COLMAP's camera models (colmap/sensor/models.h): name, model_id, number of parameters.  `lens` 0: not undistortable here (rejected),
+// 1: radtan, 2: fisheye.
+struct ColmapModel { const char* name; int id, num_params, lens; };
+static const ColmapModel kColmapModels[] = {
+    {"SIMPLE_PINHOLE", 0, 3, 1}, {"PINHOLE", 1, 4, 1}, {"SIMPLE_RADIAL", 2, 4, 1}, {"RADIAL", 3, 5, 1}, {"OPENCV", 4, 8, 1},
+    {"OPENCV_FISHEYE", 5, 8, 2}, {"FULL_OPENCV", 6, 12, 1}, {"FOV", 7, 5, 0}, {"SIMPLE_RADIAL_FISHEYE", 8, 4, 2}, {"RADIAL_FISHEYE", 9, 5, 2},
+    {"THIN_PRISM_FISHEYE", 10, 12, 0}, {"RAD_TAN_THIN_PRISM_FISHEYE", 11, 16, 0},
+};
+
+
+// K, the radial / tangential pair of main_colmap.cpp:160-234 and the full lens of one camera from its parameters in COLMAP's order
+static bool colmap_intrinsics(const ColmapModel* m, const std::string& model, unsigned int cam, const double* q, bool want_lens, Intrinsics& in,
+                              std::string* error)
+{
+    if (!m || m->lens == 0) return fail(error, "camera model " + model + " unknown! (camera " + std::to_string(cam) + ")");
+    if (m->lens == 2 && !want_lens)
+        return fail(error, "camera " + std::to_string(cam) + " uses the fisheye model " + model + ": its distortion has no place in radial / tangential, "
+                           "read the model with the lenses argument of readColmap");
+    double fx = 0, fy = 0, cx = 0, cy = 0;
+    std::memset(&in.lens, 0, sizeof(in.lens));
+    double* k = in.lens.k; double* p = in.lens.p;
+    switch (m->id) {
+    case 0: fx = fy = q[0]; cx = q[1]; cy = q[2]; break;                                                     // f cx cy
+    case 1: fx = q[0]; fy = q[1]; cx = q[2]; cy = q[3]; break;                                               // fx fy cx cy
+    case 2: fx = fy = q[0]; cx = q[1]; cy = q[2]; k[0] = q[3]; break;                                        // f cx cy k
+    case 3: fx = fy = q[0]; cx = q[1]; cy = q[2]; k[0] = q[3]; k[1] = q[4]; break;                           // f cx cy k1 k2
+    case 4: fx = q[0]; fy = q[1]; cx = q[2]; cy = q[3]; k[0] = q[4]; k[1] = q[5]; p[0] = q[6]; p[1] = q[7]; break;   // .. k1 k2 p1 p2
+    case 6: fx = q[0]; fy = q[1]; cx = q[2]; cy = q[3]; k[0] = q[4]; k[1] = q[5]; p[0] = q[6]; p[1] = q[7];          // .. k3 k4 k5 k6
+        k[2] = q[8]; k[3] = q[9]; k[4] = q[10]; k[5] = q[11]; break;
+    case 5: fx = q[0]; fy = q[1]; cx = q[2]; cy = q[3]; for (int j = 0; j < 4; ++j) k[j] = q[4 + j]; break;  // fx fy cx cy k1..k4
+    case 8: fx = fy = q[0]; cx = q[1]; cy = q[2]; k[0] = q[3]; break;                                        // f cx cy k
+    case 9: fx = fy = q[0]; cx = q[1]; cy = q[2]; k[0] = q[3]; k[1] = q[4]; break;                           // f cx cy k1 k2
+    }
+    in.lens.model = m->lens == 2 ? LensDistortion::FISHEYE : LensDistortion::RADTAN;
+    in.K = zero3();
+    in.K(0, 0) = fx; in.K(0, 2) = cx; in.K(1, 1) = fy; in.K(1, 2) = cy; in.K(2, 2) = 1.0;
+    const bool radtan = m->lens == 1;                                   // FULL_OPENCV's k4..k6 only reach the lens (main_colmap.cpp:210)
+    in.radial[0] = radtan ? k[0] : 0.0; in.radial[1] = radtan ? k[1] : 0.0; in.radial[2] = radtan ? k[2] : 0.0;
+    in.tangential[0] = radtan ? p[0] : 0.0; in.tangential[1] = radtan ? p[1] : 0.0;
+    return true;
+}
+
+// bounds-checked little-endian reads of one COLMAP binary file, loaded whole (its size bounds every allocation)
+struct ColmapBin {
+    std::string path;
+    std::vector<unsigned char> b;
+    size_t pos = 0;
+    std::string* error;
+    bool bad(const std::string& why) { return fail(error, path + ": " + why); }
+    bool open()
+    {
+        std::ifstream f(path.c_str(), std::ios::binary);
+        if (!f) return bad("cannot open");
+        b.assign(std::istreambuf_iterator<char>(f), std::istreambuf_iterator<char>());
+        return true;
+    }
+    template <class T> bool get(T& v, const char* what)
+    {
+        if (b.size() - pos < sizeof(T)) return bad(std::string("truncated at byte ") + std::to_string(pos) + " (" + what + ")");
+        std::memcpy(&v, b.data() + pos, sizeof(T)); pos += sizeof(T);
+        return true;
+    }
+    bool skip(size_t n, const char* what)
+    {
+        if (b.size() - pos < n) return bad(std::string("truncated at byte ") + std::to_string(pos) + " (" + what + ")");
+        pos += n;
+        return true;
+    }
+    // a record count: each record takes at least min_bytes, so a count the rest of the file cannot hold is malformed
+    bool count(uint64_t& n, size_t min_bytes, const char* what)
+    {
+        if (!get(n, what)) return false;
+        if (n > (b.size() - pos) / min_bytes) return bad(std::string(what) + " " + std::to_string(n) + " exceeds what the file holds");
+        return true;
+    }
+    bool name(std::string& s)
+    {
+        const void* z = std::memchr(b.data() + pos, 0, b.size() - pos);
+        if (!z) return bad("unterminated image name at byte " + std::to_string(pos));
+        const size_t n = (const unsigned char*)z - (b.data() + pos);
+        s.assign((const char*)b.data() + pos, n); pos += n + 1;
+        return true;
+    }
+    bool id32(uint64_t v, unsigned int& out, const char* what)
+    {
+        if (v > 0xFFFFFFFFull) return bad(std::string(what) + " " + std::to_string(v) + " does not fit unsigned int");
+        out = (unsigned int)v;
+        return true;
+    }
+};
+
+static bool file_exists(const std::string& p) { std::ifstream f(p.c_str()); return (bool)f; }
+
+bool readColmap(const std::string& folder, std::vector<SfMCamera>& cams, std::string* error, std::vector<LensDistortion>* lenses)
+{
+    cams.clear();
+    if (lenses) lenses->clear();
+    const bool text = file_exists(folder + "/cameras.txt") && file_exists(folder + "/images.txt") && file_exists(folder + "/points3D.txt");
+    const bool binary = file_exists(folder + "/cameras.bin") && file_exists(folder + "/images.bin") && file_exists(folder + "/points3D.bin");
+    if (!text && !binary) return fail(error, "at least one of the colmap result files does not exist in sfm folder: " + folder);
+    std::map<unsigned int, Intrinsics> intr;
+    std::map<unsigned int, Vector3d> wps;        // world points referenced by a kept image; (0,0,0) until points3D fills them in
+    // one image of images.txt / .bin: kept (and its camera's lens recorded) when its camera is known
+    auto add_image = [&](unsigned int img, double qw, double qx, double qy, double qz, double tx, double ty, double tz, unsigned int cam,
+                         const std::string& name) {
+        std::map<unsigned int, Intrinsics>::const_iterator it = intr.find(cam);
+        if (it == intr.end()) return false;
+        SfMCamera c = empty_camera(img);
+        c.image = name; c.K = it->second.K;
+        for (int k = 0; k < 3; ++k) c.radial[k] = it->second.radial[k];
+        c.tangential[0] = it->second.tangential[0]; c.tangential[1] = it->second.tangential[1];
+        c.R = Line3D::rotationFromQ(qw, qx, qy, qz); c.t = Vector3d(tx, ty, tz); c.C = center_of(c.R, c.t);
+        cams.push_back(c);
+        if (lenses) lenses->push_back(it->second.lens);
+        return true;
+    };
+    auto add_observation = [&](unsigned int wp) { cams.back().worldpoints.push_back(wp); wps[wp] = Vector3d(0, 0, 0); };
+    if (text) {
+        std::ifstream fc((folder + "/cameras.txt").c_str()), fi((folder + "/images.txt").c_str()), fp((folder + "/points3D.txt").c_str());
+        std::string line;
+        while (std::getline(fc, line)) {         // main_colmap.cpp:160-234
+            if (line.empty() || line[0] == '#') continue;
+            std::stringstream s(line);
+            unsigned int cam = 0, w = 0, h = 0; std::string model;
+            s >> cam >> model >> w >> h;
+            const ColmapModel* m = nullptr;
+            for (const ColmapModel& e : kColmapModels) if (model == e.name) m = &e;
+            double q[16] = {0};
+            for (int k = 0; m && k < m->num_params; ++k) s >> q[k];
+            Intrinsics in;
+            if (!colmap_intrinsics(m, model, cam, q, lenses != nullptr, in, error)) return false;
+            intr[cam] = in;
+        }
+        bool first = true, keep = false;
+        while (std::getline(fi, line)) {         // main_colmap.cpp:252-321: two lines per image
+            if (!line.empty() && line[0] == '#') continue;
+            std::stringstream s(line);
+            if (first) {
+                unsigned int img = 0, cam = 0; double qw = 1, qx = 0, qy = 0, qz = 0, tx = 0, ty = 0, tz = 0; std::string name;
+                s >> img >> qw >> qx >> qy >> qz >> tx >> ty >> tz >> cam >> name;
+                keep = add_image(img, qw, qx, qy, qz, tx, ty, tz, cam, name);
+                first = false;
+            } else {
+                if (keep) {
+                    double x, y; std::string id;
+                    while (s >> x >> y >> id) {
+                        const int wp = std::atoi(id.c_str());
+                        if (wp >= 0) add_observation((unsigned int)wp);
+                    }
+                }
+                first = true;
+            }
+        }
+        while (std::getline(fp, line)) {         // main_colmap.cpp:330-349
+            if (line.empty() || line[0] == '#') continue;
+            std::stringstream s(line);
+            unsigned int id = 0; double X = 0, Y = 0, Z = 0;
+            s >> id >> X >> Y >> Z;
+            std::map<unsigned int, Vector3d>::iterator it = wps.find(id);
+            if (s && it != wps.end()) it->second = Vector3d(X, Y, Z);
+        }
+    } else {                                     // COLMAP's binary model (colmap/scene/reconstruction_io.cc), little-endian
+        ColmapBin fc{folder + "/cameras.bin", {}, 0, error}, fi{folder + "/images.bin", {}, 0, error}, fp{folder + "/points3D.bin", {}, 0, error};
+        if (!fc.open() || !fi.open() || !fp.open()) return false;
+        uint64_t n = 0;
+        if (!fc.count(n, 24, "camera count")) return false;
+        for (uint64_t i = 0; i < n; ++i) {       // u32 camera_id, i32 model_id, u64 width, u64 height, f64 params[num_params]
+            uint32_t cam = 0; int32_t mid = 0; uint64_t w = 0, h = 0;
+            if (!fc.get(cam, "camera_id") || !fc.get(mid, "model_id") || !fc.get(w, "width") || !fc.get(h, "height")) return false;
+            const ColmapModel* m = nullptr;
+            for (const ColmapModel& e : kColmapModels) if (mid == e.id) m = &e;
+            if (!m) return fc.bad("camera model id " + std::to_string(mid) + " of camera " + std::to_string(cam) + " unknown!");
+            double q[16] = {0};
+            for (int k = 0; k < m->num_params; ++k) if (!fc.get(q[k], "camera parameters")) return false;
+            Intrinsics in;
+            if (!colmap_intrinsics(m, m->name, cam, q, lenses != nullptr, in, error)) return false;
+            intr[cam] = in;
+        }
+        if (!fi.count(n, 4 + 56 + 4 + 1 + 8, "image count")) return false;
+        for (uint64_t i = 0; i < n; ++i) {       // u32 image_id, f64 qw qx qy qz tx ty tz, u32 camera_id, name\0, u64 n2d, n2d x (f64 x, f64 y, u64 id)
+            uint32_t img = 0, cam = 0; double v[7]; std::string name; uint64_t n2d = 0;
+            if (!fi.get(img, "image_id")) return false;
+            for (int k = 0; k < 7; ++k) if (!fi.get(v[k], "image pose")) return false;
+            if (!fi.get(cam, "camera_id") || !fi.name(name) || !fi.count(n2d, 24, "point count")) return false;
+            const bool keep = add_image(img, v[0], v[1], v[2], v[3], v[4], v[5], v[6], cam, name);
+            for (uint64_t j = 0; j < n2d; ++j) {
+                uint64_t id = 0;
+                if (!fi.skip(16, "point xy") || !fi.get(id, "point3D_id")) return false;
+                unsigned int wp = 0;
+                if (id == ~0ull) continue;       // no 3D point (-1 in images.txt)
+                if (!fi.id32(id, wp, "point3D_id")) return false;
+                if (keep) add_observation(wp);
+            }
+        }
+        if (!fp.count(n, 8 + 24 + 3 + 8 + 8, "point count")) return false;
+        for (uint64_t i = 0; i < n; ++i) {       // u64 id, f64 xyz, u8 rgb, f64 error, u64 track_len, track_len x (u32 image_id, u32 point2D_idx)
+            uint64_t id = 0, track = 0; double X = 0, Y = 0, Z = 0;
+            unsigned int wp = 0;
+            if (!fp.get(id, "point3D_id") || !fp.id32(id, wp, "point3D_id") || !fp.get(X, "xyz") || !fp.get(Y, "xyz") || !fp.get(Z, "xyz") ||
+                !fp.skip(3 + 8, "colour and error") || !fp.count(track, 8, "track length") || !fp.skip(8 * (size_t)track, "track"))
+                return false;
+            std::map<unsigned int, Vector3d>::iterator it = wps.find(wp);
+            if (it != wps.end()) it->second = Vector3d(X, Y, Z);
+        }
+    }
+    for (SfMCamera& c : cams) {                  // main_colmap.cpp:386-401
+        std::vector<float> d;
+        for (unsigned int w : c.worldpoints) d.push_back(point_depth(c.C, wps[w]));
+        c.median_depth = median_of(d);
+    }
+    if (cams.empty()) { if (lenses) lenses->clear(); return fail(error, "no usable image in " + folder); }
+    return true;
 }
 
 // ------------------------------------------------------------------------------------------------ mavmap
@@ -162,12 +547,10 @@ bool readMavmap(const std::string& path, std::vector<SfMCamera>& out, std::strin
         SfMCamera c = empty_camera((unsigned int)cams.size());
         c.image = strip(tok[0]);
         const Matrix3d R = Line3D::rotationFromRPY(v[1], v[2], v[3]);
-        const Vector3d t(v[8], v[9], v[10]);
         for (int r = 0; r < 3; ++r)               // [R|t]^-1 = [R^T | -R^T t]  (main_mavmap.cpp:214-223)
             for (int k = 0; k < 3; ++k) c.R(r, k) = R(k, r);
-        c.t = Vector3d(-(R(0, 0) * t.x + R(1, 0) * t.y + R(2, 0) * t.z), -(R(0, 1) * t.x + R(1, 1) * t.y + R(2, 1) * t.z),
-                       -(R(0, 2) * t.x + R(1, 2) * t.y + R(2, 2) * t.z));
-        c.C = t;                                  // mavmap stores the camera centre
+        c.C = Vector3d(v[8], v[9], v[10]);        // mavmap stores the camera centre
+        c.t = translation_of(c.R, c.C);
         c.K(0, 0) = v[13]; c.K(1, 1) = v[14]; c.K(0, 2) = v[15]; c.K(1, 2) = v[16]; c.K(2, 2) = 1.0;     // main_mavmap.cpp:290-296
         cams.push_back(c);
     }
@@ -354,7 +737,7 @@ struct JsonReader {
     bool ok = true;
     bool fail_at(const JV& v, const std::string& what)
     {
-        if (ok && error) *error = file + ": " + v.path + ": " + (v.p ? what : "missing");
+        if (ok) fail(error, file + ": " + v.path + ": " + (v.p ? what : "missing"));
         ok = false;
         return false;
     }
@@ -429,8 +812,7 @@ bool readOpenMVG(const std::string& path, std::vector<SfMCamera>& cams, std::str
 
     // intrinsics (main_openmvg.cpp:201-277).  cam_model lives outside the loop in the reference: an entry without polymorphic_name
     // keeps the model of the entry before it (none before the first: no distortion)
-    struct Intr { Matrix3d K; double radial[3], tangential[2]; };
-    std::map<unsigned int, Intr> intr;
+    std::map<unsigned int, Intrinsics> intr;
     if (!rd.array(root["intrinsics"], arr)) return false;
     if (arr.empty()) return fail(error, path + ": No intrinsics in json file!");
     std::string model;
@@ -439,7 +821,7 @@ bool readOpenMVG(const std::string& path, std::vector<SfMCamera>& cams, std::str
         if (val["polymorphic_name"].p && !rd.string(val["polymorphic_name"], model)) return false;
         unsigned int key = 0;
         double focal = 0, px = 0, py = 0;
-        Intr in;
+        Intrinsics in;
         std::memset(&in, 0, sizeof(in));
         if (!rd.uint(el["key"], key) || !rd.dbl(d["focal_length"], focal) || !rd.dbl_at(d["principal_point"], 0, px) || !rd.dbl_at(d["principal_point"], 1, py))
             return false;
@@ -471,9 +853,7 @@ bool readOpenMVG(const std::string& path, std::vector<SfMCamera>& cams, std::str
             for (int c = 0; c < 3; ++c) if (!rd.dbl_at(row, c, ps.R(r, c))) return false;
         }
         if (!rd.dbl_at(val["center"], 0, ps.C.x) || !rd.dbl_at(val["center"], 1, ps.C.y) || !rd.dbl_at(val["center"], 2, ps.C.z)) return false;
-        const Matrix3d& R = ps.R;
-        ps.t = Vector3d(-(R(0, 0) * ps.C.x + R(0, 1) * ps.C.y + R(0, 2) * ps.C.z), -(R(1, 0) * ps.C.x + R(1, 1) * ps.C.y + R(1, 2) * ps.C.z),
-                        -(R(2, 0) * ps.C.x + R(2, 1) * ps.C.y + R(2, 2) * ps.C.z));
+        ps.t = translation_of(ps.R, ps.C);
         poses[it->second] = ps;
     }
 
@@ -485,26 +865,25 @@ bool readOpenMVG(const std::string& path, std::vector<SfMCamera>& cams, std::str
     std::vector<JV> obs;
     for (const JV& el : arr) {
         unsigned int id = 0;
-        double X[3];
+        Vector3d X;
         const JV val = el["value"];
         if (!rd.uint(el["key"], id)) return false;
-        for (int k = 0; k < 3; ++k) if (!rd.dbl_at(val["X"], k, X[k])) return false;
+        if (!rd.dbl_at(val["X"], 0, X.x) || !rd.dbl_at(val["X"], 1, X.y) || !rd.dbl_at(val["X"], 2, X.z)) return false;
         if (!rd.array(val["observations"], obs)) return false;
         for (const JV& o : obs) {
             unsigned int view = 0;
             if (!rd.uint(o["key"], view)) return false;
             std::map<unsigned int, Pose>::const_iterator it = poses.find(view);
             if (it == poses.end()) continue;
-            const double dx = it->second.C.x - X[0], dy = it->second.C.y - X[1], dz = it->second.C.z - X[2];
             wps[view].push_back(id);
-            depths[view].push_back((float)std::sqrt(dx * dx + dy * dy + dz * dz));
+            depths[view].push_back(point_depth(it->second.C, X));
         }
     }
 
     // cameras in view order (main_openmvg.cpp:367-409)
     for (const View& v : views) {
         if (!wps.count(v.id) || !intr.count(v.intr)) continue;
-        const Intr& in = intr[v.intr];
+        const Intrinsics& in = intr[v.intr];
         const Pose& ps = poses[v.id];
         SfMCamera c = empty_camera(v.id);
         c.image = v.file; c.K = in.K;
@@ -512,9 +891,7 @@ bool readOpenMVG(const std::string& path, std::vector<SfMCamera>& cams, std::str
         c.tangential[0] = in.tangential[0]; c.tangential[1] = in.tangential[1];
         c.R = ps.R; c.t = ps.t; c.C = ps.C;
         c.worldpoints = wps[v.id];
-        std::vector<float>& d = depths[v.id];
-        std::sort(d.begin(), d.end());
-        c.median_depth = d[d.size() / 2];
+        c.median_depth = median_of(depths[v.id]);
         cams.push_back(c);
     }
     if (cams.empty()) return fail(error, path + ": no view has both intrinsics and world points");
@@ -564,11 +941,8 @@ bool readPix4D(const std::string& params_folder, const std::string& project_pref
         const Vector3d centre(v[0], v[1], v[2]);
         for (int r = 0; r < 3; ++r) { if (!next(3, "R row")) return false; for (int k = 0; k < 3; ++k) c.R(r, k) = v[k]; }
         const Matrix3d& R = c.R;
-        c.t = Vector3d(-(R(0, 0) * centre.x + R(0, 1) * centre.y + R(0, 2) * centre.z), -(R(1, 0) * centre.x + R(1, 1) * centre.y + R(1, 2) * centre.z),
-                       -(R(2, 0) * centre.x + R(2, 1) * centre.y + R(2, 2) * centre.z));
-        // C = R^T (-t) as main_pix4d.cpp:391-392 forms it
-        c.C = Vector3d(R(0, 0) * -c.t.x + R(1, 0) * -c.t.y + R(2, 0) * -c.t.z, R(0, 1) * -c.t.x + R(1, 1) * -c.t.y + R(2, 1) * -c.t.z,
-                       R(0, 2) * -c.t.x + R(1, 2) * -c.t.y + R(2, 2) * -c.t.z);
+        c.t = translation_of(R, centre);
+        c.C = mul_transposed(R, neg(c.t));        // R^T (-t) as main_pix4d.cpp:391-392 forms it, not center_of's -(R^T t)
         const double Rt[12] = {R(0, 0), R(0, 1), R(0, 2), c.t.x, R(1, 0), R(1, 1), R(1, 2), c.t.y, R(2, 0), R(2, 1), R(2, 2), c.t.z};
         for (int r = 0; r < 3; ++r)
             for (int k = 0; k < 4; ++k) P.push_back(c.K(r, 0) * Rt[k] + c.K(r, 1) * Rt[4 + k] + c.K(r, 2) * Rt[8 + k]);
@@ -660,10 +1034,92 @@ bool readPix4D(const std::string& params_folder, const std::string& project_pref
     return true;
 }
 
+// ------------------------------------------------------------------------------------------------ what the C wrappers share
+// element i of a handle's list; nullptr when i is out of range
+template <class T> static const T* item(const std::vector<T>& v, int i) { return i >= 0 && i < (int)v.size() ? &v[i] : nullptr; }
+
+// a list of ids (world points, neighbours) into out[cap]: its length, even when it exceeds cap
+static int copy_ids(const std::list<unsigned int>& ids, unsigned int* out, int cap)
+{
+    int n = 0;
+    for (unsigned int w : ids) { if (n < cap) out[n] = w; ++n; }
+    return n;
+}
+
 }  // namespace L3DPP
 
-// C wrapper (include/l3dpp_capi.h); l3dpp_sfm_open, which reads these models too, is in line3d_io.cc
+// the object behind an l3dpp_sfm_* handle: the cameras of any reader, and the lenses readColmap returns when asked for them
+struct L3DSfMHandle {
+    std::vector<L3DPP::SfMCamera> cams;
+    std::vector<L3DPP::LensDistortion> lenses;
+};
+typedef std::vector<L3DPP::NVMCamera> L3DNVMHandle;
+
+// C wrapper (include/l3dpp_capi.h): flat arrays
 extern "C" {
+void* l3dpp_nvm_open(const char* path, char* err, int errcap)
+{
+    L3DNVMHandle* v = new L3DNVMHandle();
+    std::string e;
+    if (!L3DPP::readNVM(path, *v, &e)) { l3dpp_copy_str(e, err, errcap); delete v; return nullptr; }
+    return v;
+}
+void l3dpp_nvm_close(void* h) { delete (L3DNVMHandle*)h; }
+int l3dpp_nvm_num_cameras(void* h) { return (int)((L3DNVMHandle*)h)->size(); }
+int l3dpp_nvm_camera(void* h, int i, double* R9, double* t3, double* C3, float* focal, float* distortion, float* median_depth, int* num_wps, char* name, int namecap)
+{
+    const L3DPP::NVMCamera* c = L3DPP::item(*(L3DNVMHandle*)h, i);
+    if (!c) return -1;
+    for (int k = 0; k < 9; ++k) R9[k] = c->R.m[k];
+    t3[0] = c->t.x; t3[1] = c->t.y; t3[2] = c->t.z; C3[0] = c->C.x; C3[1] = c->C.y; C3[2] = c->C.z;
+    *focal = c->focal; *distortion = c->distortion; *median_depth = c->median_depth; *num_wps = (int)c->worldpoints.size();
+    l3dpp_copy_str(c->image, name, namecap);
+    return 0;
+}
+int l3dpp_nvm_worldpoints(void* h, int i, unsigned int* out, int cap) { const L3DPP::NVMCamera* c = L3DPP::item(*(L3DNVMHandle*)h, i); return c ? L3DPP::copy_ids(c->worldpoints, out, cap) : -1; }
+void l3dpp_intrinsics_from_focal(float focal, int w, int h, double* K9) { const L3DPP::Matrix3d K = L3DPP::intrinsicsFromFocal(focal, w, h); for (int k = 0; k < 9; ++k) K9[k] = K.m[k]; }
+void* l3dpp_sfm_open(int kind, const char* path, const char* aux, char* err, int errcap)
+{
+    L3DSfMHandle* v = new L3DSfMHandle();
+    const std::string a = aux ? aux : "";
+    std::string e;
+    bool ok = false;
+    switch (kind) {
+    case L3DPP_SFM_BUNDLER: ok = L3DPP::readBundler(path, a, v->cams, &e); break;
+    case L3DPP_SFM_COLMAP: ok = L3DPP::readColmap(path, v->cams, &e); break;
+    case L3DPP_SFM_COLMAP_LENSES: ok = L3DPP::readColmap(path, v->cams, &e, &v->lenses); break;
+    case L3DPP_SFM_MAVMAP: ok = L3DPP::readMavmap(path, v->cams, &e); break;
+    case L3DPP_SFM_OPENMVG: ok = L3DPP::readOpenMVG(path, v->cams, &e); break;
+    case L3DPP_SFM_PIX4D: ok = L3DPP::readPix4D(path, a, v->cams, &e); break;
+    default: e = "unknown model kind " + std::to_string(kind);
+    }
+    if (!ok) { l3dpp_copy_str(e, err, errcap); delete v; return nullptr; }
+    return v;
+}
+void l3dpp_sfm_close(void* h) { delete (L3DSfMHandle*)h; }
+int l3dpp_sfm_num_cameras(void* h) { return (int)((L3DSfMHandle*)h)->cams.size(); }
+int l3dpp_sfm_lens(void* h, int i, double* lens9)
+{
+    const L3DPP::LensDistortion* l = L3DPP::item(((L3DSfMHandle*)h)->lenses, i);
+    if (!l) return -1;
+    lens9[0] = l->model;
+    for (int k = 0; k < 6; ++k) lens9[1 + k] = l->k[k];
+    lens9[7] = l->p[0]; lens9[8] = l->p[1];
+    return 0;
+}
+int l3dpp_sfm_camera(void* h, int i, double* head5, double* K9, double* R9, double* t3, double* C3, double* dist5, char* name, int namecap)
+{
+    const L3DPP::SfMCamera* c = L3DPP::item(((L3DSfMHandle*)h)->cams, i);
+    if (!c) return -1;
+    head5[0] = c->id; head5[1] = c->has_K; head5[2] = c->focal; head5[3] = c->median_depth; head5[4] = (double)c->worldpoints.size();
+    for (int k = 0; k < 9; ++k) { K9[k] = c->K.m[k]; R9[k] = c->R.m[k]; }
+    t3[0] = c->t.x; t3[1] = c->t.y; t3[2] = c->t.z; C3[0] = c->C.x; C3[1] = c->C.y; C3[2] = c->C.z;
+    for (int k = 0; k < 3; ++k) dist5[k] = c->radial[k];
+    dist5[3] = c->tangential[0]; dist5[4] = c->tangential[1];
+    l3dpp_copy_str(c->image, name, namecap);
+    return 0;
+}
+int l3dpp_sfm_worldpoints(void* h, int i, unsigned int* out, int cap) { const L3DPP::SfMCamera* c = L3DPP::item(((L3DSfMHandle*)h)->cams, i); return c ? L3DPP::copy_ids(c->worldpoints, out, cap) : -1; }
 void l3dpp_rotation_from_rpy(double roll, double pitch, double yaw, double* R9)
 {
     const L3DPP::Matrix3d R = L3DPP::Line3D::rotationFromRPY(roll, pitch, yaw);
@@ -678,8 +1134,6 @@ void l3dpp_decompose_projection(const double* P12, double* K9, double* R9, doubl
 }
 int l3dpp_sequential_neighbors(unsigned int i, unsigned int n_cams, unsigned int num_neighbors, unsigned int* out, int cap)
 {
-    int n = 0;
-    for (unsigned int j : L3DPP::sequentialNeighbors(i, n_cams, num_neighbors)) { if (n < cap) out[n] = j; ++n; }
-    return n;
+    return L3DPP::copy_ids(L3DPP::sequentialNeighbors(i, n_cams, num_neighbors), out, cap);
 }
 }

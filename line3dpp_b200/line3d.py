@@ -298,24 +298,54 @@ def segment_cache_path(output_folder, cam, width, height, max_img_width=-1):
     return buf.value.decode()
 
 
-# ---- SfM models (include/line3d_io.h, csrc/line3d_io.cc + csrc/line3d_sfm.cc); host only except read_pix4d, which triangulates on a GPU
+# ---- SfM models (include/line3d_io.h, csrc/line3d_sfm.cc); host only except read_pix4d, which triangulates on a GPU
+def _worldpoints(get, h, i, n):
+    """the n world point ids of camera i through l3dpp_nvm_worldpoints / l3dpp_sfm_worldpoints"""
+    w = np.zeros(max(n, 1), np.uint32)
+    if get(h, i, _p(w), n) != n:
+        raise capi.L3DError(f"world point count of camera {i} changed")
+    return w[:n]
+
+
+def read_nvm(path):
+    """readNVM: the cameras of an NVM_V3 file as dicts (image, focal, distortion, R, t, C, median_depth, worldpoints).  Raises L3DError
+    on a malformed model."""
+    L = capi.lib()
+    err = C.create_string_buffer(4096)
+    h = L.l3dpp_nvm_open(str(path).encode(), err, 4096)
+    if not h:
+        raise capi.L3DError(err.value.decode(errors="replace"))
+    cams = []
+    try:
+        for i in range(L.l3dpp_nvm_num_cameras(h)):
+            R, t, Cc = np.zeros(9), np.zeros(3), np.zeros(3)
+            f, d, md, nw = C.c_float(), C.c_float(), C.c_float(), C.c_int()
+            name = C.create_string_buffer(4096)
+            if L.l3dpp_nvm_camera(h, i, _p(R), _p(t), _p(Cc), C.byref(f), C.byref(d), C.byref(md), C.byref(nw), name, 4096) != 0:
+                raise capi.L3DError(f"no camera {i}")
+            cams.append(dict(image=name.value.decode(errors="replace"), focal=np.float32(f.value), distortion=np.float32(d.value), R=R.reshape(3, 3),
+                             t=t, C=Cc, median_depth=np.float32(md.value), worldpoints=_worldpoints(L.l3dpp_nvm_worldpoints, h, i, nw.value)))
+    finally:
+        L.l3dpp_nvm_close(h)
+    return cams
+
+
 def _sfm_cameras(L, h, lenses=False):
-    """the cameras of an l3dpp_sfm_* handle as dicts (id, image, K, R, t, C, radial, tangential, median_depth, worldpoints, and with
-    lenses the lens dict {model, k[6], p[2]} of L3DPP::LensDistortion); closes it"""
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
+    """the cameras of an l3dpp_sfm_* handle as dicts (id, image, has_K, K, focal, R, t, C, radial, tangential, median_depth, worldpoints,
+    and with lenses the lens dict {model, k[6], p[2]} of L3DPP::LensDistortion); closes it"""
     cams = []
     try:
         for i in range(L.l3dpp_sfm_num_cameras(h)):
             head, K, R, t, Cc, dist = np.zeros(5), np.zeros(9), np.zeros(9), np.zeros(3), np.zeros(3), np.zeros(5)
             name = C.create_string_buffer(4096)
-            L.l3dpp_sfm_camera(h, i, p(head), p(K), p(R), p(t), p(Cc), p(dist), name, 4096)
-            w = np.zeros(max(int(head[4]), 1), np.uint32)
-            L.l3dpp_sfm_worldpoints(h, i, p(w), int(head[4]))
-            cams.append(dict(id=int(head[0]), image=name.value.decode(errors="replace"), K=K.reshape(3, 3), R=R.reshape(3, 3), t=t, C=Cc,
-                             radial=dist[:3].copy(), tangential=dist[3:].copy(), median_depth=np.float32(head[3]), worldpoints=w[:int(head[4])]))
+            if L.l3dpp_sfm_camera(h, i, _p(head), _p(K), _p(R), _p(t), _p(Cc), _p(dist), name, 4096) != 0:
+                raise capi.L3DError(f"no camera {i}")
+            cams.append(dict(id=int(head[0]), image=name.value.decode(errors="replace"), has_K=bool(head[1]), K=K.reshape(3, 3),
+                             focal=np.float32(head[2]), R=R.reshape(3, 3), t=t, C=Cc, radial=dist[:3].copy(), tangential=dist[3:].copy(),
+                             median_depth=np.float32(head[3]), worldpoints=_worldpoints(L.l3dpp_sfm_worldpoints, h, i, int(head[4]))))
             if lenses:
                 lens = np.zeros(9)
-                if L.l3dpp_sfm_lens(h, i, p(lens)) != 0:
+                if L.l3dpp_sfm_lens(h, i, _p(lens)) != 0:
                     raise capi.L3DError(f"no lens for camera {i}")
                 cams[-1]["lens"] = dict(model=int(lens[0]), k=lens[1:7].copy(), p=lens[7:9].copy())
     finally:
@@ -336,10 +366,17 @@ def _read_sfm(kind, path, aux=""):
     return _sfm_cameras(L, h, lenses=kind == SFM_COLMAP_LENSES)
 
 
-def read_colmap(sfm_folder):
-    """readColmap with lenses: the cameras of a COLMAP model (cameras/images/points3D .txt, or else .bin), each with a `lens` dict
-    {model: capi.LENS_RADTAN | capi.LENS_FISHEYE, k: k1..k6, p: p1, p2} for undistort_image.  Raises L3DError on a malformed model."""
-    return _read_sfm(SFM_COLMAP_LENSES, sfm_folder)
+def read_bundler(bundle_file, image_list=""):
+    """readBundler: the cameras of a bundle.rd.out (focal only, has_K False; names from the optional image list).  Raises L3DError on
+    a malformed model."""
+    return _read_sfm(SFM_BUNDLER, bundle_file, image_list)
+
+
+def read_colmap(sfm_folder, lenses=True):
+    """readColmap: the cameras of a COLMAP model (cameras/images/points3D .txt, or else .bin).  With lenses each has a `lens` dict
+    {model: capi.LENS_RADTAN | capi.LENS_FISHEYE, k: k1..k6, p: p1, p2} for undistort_image; without, fisheye cameras are rejected.
+    Raises L3DError on a malformed model."""
+    return _read_sfm(SFM_COLMAP_LENSES if lenses else SFM_COLMAP, sfm_folder)
 
 
 def undistort_image(img, K, lens, device=0):

@@ -95,17 +95,10 @@ def write_bin(folder, cameras, images, pts):
     (folder / "points3D.bin").write_bytes(bin_points(pts))
 
 
-def read_plain(folder):
-    """readColmap without lenses (L3DPP_SFM_COLMAP): (cameras as dicts, '') or (None, error)"""
+def read(folder, lenses=True):
+    """readColmap with or without lenses: (cameras as dicts, '') or (None, error)"""
     try:
-        return line3d._read_sfm(line3d.SFM_COLMAP, folder), ""
-    except capi.L3DError as e:
-        return None, str(e)
-
-
-def read_lenses(folder):
-    try:
-        return line3d.read_colmap(folder), ""
+        return line3d.read_colmap(folder, lenses), ""
     except capi.L3DError as e:
         return None, str(e)
 
@@ -181,9 +174,9 @@ def every_model(tmp_path):
 
 def test_binary_equals_text_field_for_field(every_model):
     t, b, both, images, pts = every_model
-    ct, e1 = read_lenses(t)
-    cb, e2 = read_lenses(b)
-    cboth, e3 = read_lenses(both)
+    ct, e1 = read(t)
+    cb, e2 = read(b)
+    cboth, e3 = read(both)
     assert ct is not None and cb is not None and cboth is not None, (e1, e2, e3)
     assert len(ct) == len(CAMERAS) and len(ct) == len(cb)
     for a, c, d in zip(ct, cb, cboth):
@@ -196,9 +189,9 @@ def test_old_models_read_as_before_with_or_without_lenses(tmp_path, fmt):
     cams6 = {cid: v for cid, v in CAMERAS.items() if v[0] in OLD_SIX}
     images, pts = _scene(cams6, seed=2)
     (write_text if fmt == "txt" else write_bin)(tmp_path, cams6, images, pts)
-    plain, err = read_plain(tmp_path)
+    plain, err = read(tmp_path, lenses=False)
     assert plain is not None, err
-    lensed, err = read_lenses(tmp_path)
+    lensed, err = read(tmp_path)
     assert lensed is not None, err
     exp = _expected(cams6, images, pts)
     _check_against_expected(plain, exp, pts, with_lens=False)
@@ -211,7 +204,7 @@ def test_old_models_read_as_before_with_or_without_lenses(tmp_path, fmt):
 def test_lens_contents_per_model(tmp_path, fmt):
     images, pts = _scene(CAMERAS, seed=3)
     (write_text if fmt == "txt" else write_bin)(tmp_path, CAMERAS, images, pts)
-    cams, err = read_lenses(tmp_path)
+    cams, err = read(tmp_path)
     assert cams is not None, err
     by_cam = {im[0]: im[3] for im in images}
     seen = set()
@@ -242,9 +235,9 @@ def test_rejections(tmp_path, fmt):
         cams = {1: CAMERAS[1], 5: next(v for v in CAMERAS.values() if v[0] == model)}
         images, pts = _scene(cams, seed=4)
         write(d, cams, images, pts)
-        bad, err = read_plain(d)
+        bad, err = read(d, lenses=False)
         assert bad is None and "fisheye model " + model in err and "lenses" in err, err
-        ok, err = read_lenses(d)
+        ok, err = read(d)
         assert ok is not None, err
     for model, prm in (("FOV", [500, 500, 320, 240, 0.9]), ("THIN_PRISM_FISHEYE", [500, 500, 320, 240] + [0.01] * 8)):
         d = tmp_path / f"rej_{model}"
@@ -252,67 +245,61 @@ def test_rejections(tmp_path, fmt):
         cams = {1: CAMERAS[1], 3: (model, 640, 480, prm)}
         images, pts = _scene(cams, seed=5)
         write(d, cams, images, pts)
-        for reader in (read_plain, read_lenses):
-            bad, err = reader(d)
+        for lenses in (False, True):
+            bad, err = read(d, lenses)
             assert bad is None and f"camera model {model} unknown! (camera 3)" in err, err
 
 
-def _small(tmp_path):
+def _small():
     cams = {4: CAMERAS[5]}
     images = [(7, [1, 0, 0, 0], [0.5, 0, 2], 4, "a.png", [(1.0, 2.0, 11), (3.0, 4.0, NONE)])]
     pts = {11: np.array([0.1, 0.2, 5.0])}
     return cams, images, pts
 
 
-def test_malformed_binary_files_fail_cleanly(tmp_path):
-    cams, images, pts = _small(tmp_path)
+def malformed_binary_models():
+    """a small binary model's files and every malformed variant of them: (good files, [(name, replaced files, check)]), where
+    check(error) holds for the message readColmap must give"""
+    cams, images, pts = _small()
     good = {"cameras.bin": bin_cameras(cams), "images.bin": bin_images(images), "points3D.bin": bin_points(pts)}
-    d = tmp_path / "m"
-    d.mkdir()
-
-    def put(**over):
-        for k, v in good.items():
-            (d / k).write_bytes(over.get(k.replace(".", "_"), v))
-
-    put()
-    ok, err = read_lenses(d)
-    assert ok is not None and len(ok) == 1 and ok[0]["worldpoints"].tolist() == [11], err
-    checked = 0
+    out = []
     for name, data in good.items():
         for cut in range(len(data)):
-            put(**{name.replace(".", "_"): data[:cut]})
-            bad, err = read_lenses(d)
-            assert bad is None and name in err and ("truncated" in err or "exceeds" in err), (name, cut, err)
-            checked += 1
-    assert checked == sum(len(v) for v in good.values())
-    for name in good:                                             # a count the file cannot hold: no allocation of that size
-        data = good[name]
-        put(**{name.replace(".", "_"): struct.pack("<Q", 2 ** 60) + data[8:]})
-        bad, err = read_lenses(d)
-        assert bad is None and name in err and "exceeds" in err, err
-    put(cameras_bin=struct.pack("<Q", 2 ** 60) + b"\0" * 32)      # 40 bytes
-    bad, err = read_lenses(d)
-    assert bad is None and "cameras.bin" in err
-    im = bin_images(images)
+            out.append((f"{name}_cut{cut}", {name: data[:cut]}, lambda e, name=name: name in e and ("truncated" in e or "exceeds" in e)))
+    for name, data in good.items():                               # a count the file cannot hold: no allocation of that size
+        out.append((f"{name}_count", {name: struct.pack("<Q", 2 ** 60) + data[8:]}, lambda e, name=name: name in e and "exceeds" in e))
+    out.append(("cameras_40_bytes", {"cameras.bin": struct.pack("<Q", 2 ** 60) + b"\0" * 32}, lambda e: "cameras.bin" in e))
     name_at = 8 + 4 + 56 + 4
-    put(images_bin=im[:name_at] + b"x" * 40)                      # the name never ends
-    bad, err = read_lenses(d)
-    assert bad is None and "images.bin" in err and "unterminated" in err, err
-    put(cameras_bin=bin_cameras(cams, model_id=42))
-    bad, err = read_lenses(d)
-    assert bad is None and "cameras.bin" in err and "42" in err and "unknown" in err, err
-    put(cameras_bin=bin_cameras(cams, model_id=-1))
-    bad, err = read_lenses(d)
-    assert bad is None and "unknown" in err, err
+    out.append(("unterminated_name", {"images.bin": good["images.bin"][:name_at] + b"x" * 40},   # the name never ends
+                lambda e: "images.bin" in e and "unterminated" in e))
+    out.append(("model_42", {"cameras.bin": bin_cameras(cams, model_id=42)}, lambda e: "cameras.bin" in e and "42" in e and "unknown" in e))
+    out.append(("model_-1", {"cameras.bin": bin_cameras(cams, model_id=-1)}, lambda e: "unknown" in e))
     big = [(7, [1, 0, 0, 0], [0.5, 0, 2], 4, "a.png", [(1.0, 2.0, 2 ** 33)])]
-    put(images_bin=bin_images(big))
-    bad, err = read_lenses(d)
-    assert bad is None and "images.bin" in err and "unsigned int" in err, err
-    put(points3D_bin=bin_points({2 ** 32: np.zeros(3)}))
-    bad, err = read_lenses(d)
-    assert bad is None and "points3D.bin" in err and "unsigned int" in err, err
+    out.append(("image_point_id", {"images.bin": bin_images(big)}, lambda e: "images.bin" in e and "unsigned int" in e))
+    out.append(("point_id", {"points3D.bin": bin_points({2 ** 32: np.zeros(3)})}, lambda e: "points3D.bin" in e and "unsigned int" in e))
+    return good, out
+
+
+def write_files(d, good, replaced):
+    for k, v in good.items():
+        (d / k).write_bytes(replaced.get(k, v))
+
+
+def test_malformed_binary_files_fail_cleanly(tmp_path):
+    good, variants = malformed_binary_models()
+    d = tmp_path / "m"
+    d.mkdir()
+    write_files(d, good, {})
+    ok, err = read(d)
+    assert ok is not None and len(ok) == 1 and ok[0]["worldpoints"].tolist() == [11], err
+    for name, replaced, check in variants:
+        write_files(d, good, replaced)
+        bad, err = read(d)
+        assert bad is None and check(err), (name, err)
+    assert sum(1 for name, _, _ in variants if "_cut" in name) == sum(len(v) for v in good.values())
+    write_files(d, good, {})
     (d / "points3D.bin").unlink()
-    bad, err = read_lenses(d)
+    bad, err = read(d)
     assert bad is None and "does not exist" in err
 
 

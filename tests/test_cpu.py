@@ -349,220 +349,6 @@ def test_oracle_cluster_tail_reproduces_the_reference_result_file(oracle):
     assert extra <= 0.02 * total, extra
 
 
-# ---------------------------------------------------------------------------------------------- .nvm input format (SURVEY §8f-2)
-def _read_nvm_product(path):
-    from line3dpp_b200 import capi
-    L = capi.lib()
-    err = ctypes.create_string_buffer(256)
-    h = L.l3dpp_nvm_open(str(path).encode(), err, 256)
-    if not h:
-        return None, err.value.decode()
-    h = ctypes.c_void_p(h)
-    cams = []
-    for i in range(L.l3dpp_nvm_num_cameras(h)):
-        R, t, Cc = np.zeros(9), np.zeros(3), np.zeros(3)
-        f, d, md, nw = ctypes.c_float(), ctypes.c_float(), ctypes.c_float(), ctypes.c_int()
-        name = ctypes.create_string_buffer(512)
-        p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-        assert L.l3dpp_nvm_camera(h, i, p(R), p(t), p(Cc), ctypes.byref(f), ctypes.byref(d), ctypes.byref(md), ctypes.byref(nw), name, 512) == 0
-        w = np.zeros(max(nw.value, 1), np.uint32)
-        assert L.l3dpp_nvm_worldpoints(h, i, p(w), nw.value) == nw.value
-        cams.append(dict(R=R.reshape(3, 3), t=t, C=Cc, f=f.value, dist=d.value, md=md.value, wps=w[:nw.value], name=name.value.decode()))
-    L.l3dpp_nvm_close(h)
-    return cams, ""
-
-
-def test_nvm_reader_round_trip(tmp_path):
-    """L3DPP::readNVM (include/line3d_io.h; restates main_vsfm.cpp:143-310) on a synthetic NVM_V3 model"""
-    rng = np.random.default_rng(3)
-    V, NP = 5, 40
-    q = rng.normal(size=(V, 4)); q /= np.linalg.norm(q, axis=1, keepdims=True)
-    Cc = rng.uniform(-3, 3, (V, 3)); f = rng.uniform(800, 2500, V); d = np.array([0, 0.01, 0, -0.02, 0])
-    pts = rng.uniform(-1, 1, (NP, 3))
-    vis = [sorted(rng.choice(V, size=rng.integers(2, V + 1), replace=False).tolist()) for _ in range(NP)]
-    lines = ["NVM_V3", "", str(V)]
-    for i in range(V):
-        lines.append(f"dir/img{i}.jpg\t{f[i]:.10f} {q[i,0]:.12f} {q[i,1]:.12f} {q[i,2]:.12f} {q[i,3]:.12f} {Cc[i,0]:.12f} {Cc[i,1]:.12f} {Cc[i,2]:.12f} {d[i]:.6f} 0")
-    lines += ["", str(NP)]
-    for j in range(NP):
-        meas = " ".join(f"{c} {7 * j + c} {10.5 + c} {-3.25 + j}" for c in vis[j])
-        lines.append(f"{pts[j,0]:.12f} {pts[j,1]:.12f} {pts[j,2]:.12f} 255 128 0 {len(vis[j])} {meas}")
-    path = tmp_path / "model.nvm"
-    path.write_text("\n".join(lines) + "\n0\n")
-    cams, err = _read_nvm_product(path)
-    assert cams is not None, err
-    assert len(cams) == V
-    for i, c in enumerate(cams):
-        qw, qx, qy, qz = [float(f"{v:.12f}") for v in q[i]]
-        R = np.array([[1 - 2 * qy * qy - 2 * qz * qz, 2 * qx * qy - 2 * qz * qw, 2 * qx * qz + 2 * qy * qw],
-                      [2 * qx * qy + 2 * qz * qw, 1 - 2 * qx * qx - 2 * qz * qz, 2 * qy * qz - 2 * qx * qw],
-                      [2 * qx * qz - 2 * qy * qw, 2 * qy * qz + 2 * qx * qw, 1 - 2 * qx * qx - 2 * qy * qy]])
-        Ci = np.array([float(f"{v:.12f}") for v in Cc[i]])
-        np.testing.assert_allclose(c["R"], R, atol=1e-14)
-        np.testing.assert_allclose(c["t"], -R @ Ci, atol=1e-13)
-        assert c["name"] == f"dir/img{i}.jpg" and abs(c["f"] - np.float32(f[i])) < 1e-3 and abs(c["dist"] - d[i]) < 1e-7
-        mine = [j for j in range(NP) if i in vis[j]]
-        assert c["wps"].tolist() == mine
-        dep = np.sort(np.array([np.float32(np.linalg.norm(np.array([float(f"{v:.12f}") for v in pts[j]]) - Ci)) for j in mine], np.float32))
-        assert c["md"] == (dep[len(dep) // 2] if len(dep) else 0.0)
-    bad, err = _read_nvm_product(tmp_path / "missing.nvm")
-    assert bad is None and "cannot open" in err
-    (tmp_path / "empty.nvm").write_text("NVM_V3\n\n0\n")
-    bad, err = _read_nvm_product(tmp_path / "empty.nvm")
-    assert bad is None and "No aligned cameras" in err
-
-
-def test_nvm_reader_on_the_reference_test_data(tmp_path):
-    """readNVM on the reference's own testdata/vsfm_result.nvm (every camera, the first 4500 points: tests/golden/vsfm_result_head.nvm.gz)
-    equals the committed inputs of the nvm configuration (cameras) and the numpy reader of tests/golden/make_nvm_inputs.py
-    (world-point lists, median depths)"""
-    import gzip
-    path = tmp_path / "vsfm_result.nvm"
-    path.write_bytes(gzip.decompress(open(os.path.join(ROOT, "tests", "golden", "vsfm_result_head.nvm.gz"), "rb").read()))
-    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
-    from make_nvm_inputs import read_nvm
-    from tests import nvm_util as nu
-    inp = nu.load_inputs()
-    _, wps, depths = read_nvm(path)
-    cams, err = _read_nvm_product(path)
-    assert cams is not None and len(cams) == inp["V"], err
-    from line3dpp_b200 import capi
-    L = capi.lib()
-    for i, c in enumerate(cams):
-        np.testing.assert_allclose(c["R"], inp["R"][i], atol=1e-15)
-        np.testing.assert_allclose(c["t"], inp["t"][i], atol=1e-13)
-        d = np.sort(np.array(depths[i], np.float32))
-        assert len(d) > 0 and c["md"] == d[len(d) // 2] and np.array_equal(c["wps"], np.array(wps[i], np.uint32))
-        K = np.zeros(9)
-        L.l3dpp_intrinsics_from_focal(ctypes.c_float(c["f"]), int(inp["wh"][i][0]), int(inp["wh"][i][1]), K.ctypes.data_as(ctypes.c_void_p))
-        assert np.array_equal(K.reshape(3, 3), inp["K"][i])
-    assert sum(len(c["wps"]) for c in cams) > 10000
-
-
-def test_nvm_reader_rejects_truncated_camera_list(tmp_path):
-    """ADVICE r1: a truncated camera section must be an error, not a default camera"""
-    f = tmp_path / "t.nvm"
-    f.write_text("NVM_V3\n\n3\nimg0.jpg 1000 1 0 0 0 0 0 0 0 0\nimg1.jpg 1000 1 0 0 0\n")
-    cams, err = _read_nvm_product(f)
-    assert cams is None and "camera" in err
-    f.write_text("NVM_V3\n\n2\nimg0.jpg 1000 1 0 0 0 0 0 0 0 0\n")
-    cams, err = _read_nvm_product(f)
-    assert cams is None and "end of file" in err
-
-
-def _read_sfm_product(kind, path, aux=""):
-    from line3dpp_b200 import capi
-    L = capi.lib()
-    err = ctypes.create_string_buffer(256)
-    h = L.l3dpp_sfm_open(kind, str(path).encode(), str(aux).encode(), err, 256)
-    if not h:
-        return None, err.value.decode()
-    h = ctypes.c_void_p(h)
-    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    cams = []
-    for i in range(L.l3dpp_sfm_num_cameras(h)):
-        head, K, R, t, Cc, dist = np.zeros(5), np.zeros(9), np.zeros(9), np.zeros(3), np.zeros(3), np.zeros(5)
-        name = ctypes.create_string_buffer(512)
-        assert L.l3dpp_sfm_camera(h, i, p(head), p(K), p(R), p(t), p(Cc), p(dist), name, 512) == 0
-        w = np.zeros(max(int(head[4]), 1), np.uint32)
-        assert L.l3dpp_sfm_worldpoints(h, i, p(w), int(head[4])) == int(head[4])
-        cams.append(dict(id=int(head[0]), has_K=bool(head[1]), f=head[2], md=np.float32(head[3]), wps=w[:int(head[4])], K=K.reshape(3, 3), R=R.reshape(3, 3),
-                         t=t, C=Cc, dist=dist, name=name.value.decode()))
-    L.l3dpp_sfm_close(h)
-    return cams, ""
-
-
-def _rot(rng):
-    q = rng.normal(size=4); q /= np.linalg.norm(q)
-    w, x, y, z = q
-    return q, np.array([[1 - 2 * y * y - 2 * z * z, 2 * x * y - 2 * z * w, 2 * x * z + 2 * y * w], [2 * x * y + 2 * z * w, 1 - 2 * x * x - 2 * z * z, 2 * y * z - 2 * x * w],
-                        [2 * x * z - 2 * y * w, 2 * y * z + 2 * x * w, 1 - 2 * x * x - 2 * y * y]])
-
-
-def test_bundler_reader(tmp_path):
-    """L3DPP::readBundler (include/line3d_io.h; restates main_bundler.cpp:143-286) on a synthetic bundle.rd.out"""
-    rng = np.random.default_rng(5)
-    V, NP = 4, 30
-    Rs = [_rot(rng)[1] for _ in range(V)]; ts = rng.uniform(-2, 2, (V, 3)); f = rng.uniform(500, 2000, V); k = rng.uniform(-0.1, 0.1, (V, 2))
-    pts = rng.uniform(-1, 1, (NP, 3))
-    vis = [sorted(rng.choice(V, size=rng.integers(2, V + 1), replace=False).tolist()) for _ in range(NP)]
-    L = ["# Bundle file v0.3", f"{V} {NP}"]
-    for i in range(V):
-        L.append(f"{f[i]:.10f} {k[i,0]:.10f} {k[i,1]:.10f}")
-        L += [" ".join(f"{v:.12f}" for v in Rs[i][r]) for r in range(3)]
-        L.append(" ".join(f"{v:.12f}" for v in ts[i]))
-    for j in range(NP):
-        L += [" ".join(f"{v:.12f}" for v in pts[j]), "255 0 0", f"{len(vis[j])} " + " ".join(f"{c} {j} 1.5 -2.5" for c in vis[j])]
-    (tmp_path / "bundle.rd.out").write_text("\n".join(L) + "\n")
-    (tmp_path / "list.txt").write_text("a.jpg 0 123\nb.jpg\n\nd.jpg 1 2\n")
-    cams, err = _read_sfm_product(0, tmp_path / "bundle.rd.out", tmp_path / "list.txt")
-    assert cams is not None and len(cams) == V, err
-    rd = lambda a: np.array([float(f"{v:.12f}") for v in np.ravel(a)]).reshape(np.shape(a))
-    for i, c in enumerate(cams):
-        R = rd(Rs[i]); R[1:] *= -1
-        t = rd(ts[i]); t[1:] *= -1
-        np.testing.assert_allclose(c["R"], R, atol=1e-15); np.testing.assert_allclose(c["t"], t, atol=1e-15)
-        Ci = -R.T @ t
-        np.testing.assert_allclose(c["C"], Ci, atol=1e-14)
-        assert c["id"] == i and not c["has_K"] and abs(c["f"] - np.float32(float(f"{f[i]:.10f}"))) < 1e-3
-        np.testing.assert_allclose(c["dist"][:2], np.float32(rd(k[i])), atol=1e-9); assert not c["dist"][2:].any()
-        mine = [j for j in range(NP) if i in vis[j]]
-        assert c["wps"].tolist() == mine
-        dep = np.sort(np.array([np.float32(np.linalg.norm(rd(pts[j]) - c["C"])) for j in mine], np.float32))
-        assert c["md"] == (dep[len(dep) // 2] if len(dep) else np.float32(0))
-    assert [c["name"] for c in cams] == ["a.jpg", "b.jpg", "", "d.jpg"]
-    (tmp_path / "empty.out").write_text("# Bundle file v0.3\n0 0\n")
-    bad, err = _read_sfm_product(0, tmp_path / "empty.out")
-    assert bad is None and "No cameras" in err
-
-
-def test_colmap_reader(tmp_path):
-    """L3DPP::readColmap (include/line3d_io.h; restates main_colmap.cpp:140-401) on a synthetic text model"""
-    rng = np.random.default_rng(6)
-    cam_lines = ["# Camera list", "1 SIMPLE_PINHOLE 640 480 500.5 320 240", "2 PINHOLE 640 480 500 510 321 239", "3 SIMPLE_RADIAL 640 480 400 300 200 0.01",
-                 "4 RADIAL 640 480 410 310 210 0.02 -0.03", "5 OPENCV 800 600 700 710 400 300 0.1 0.2 0.001 0.002",
-                 "6 FULL_OPENCV 800 600 701 711 401 301 0.11 0.21 0.0011 0.0021 0.31 0 0 0"]
-    (tmp_path / "cameras.txt").write_text("\n".join(cam_lines) + "\n")
-    NP = 25
-    pts = rng.uniform(-1, 1, (NP, 3))
-    imgs, L = [], ["# Image list with two lines of data per image:"]
-    for n, (img_id, cam_id) in enumerate([(10, 1), (11, 2), (12, 3), (13, 4), (14, 5), (15, 6), (16, 99)]):
-        q, R = _rot(rng)
-        q = q * 1.7                                   # rotationFromQ normalises (line3D.cc:2737-2754)
-        t = rng.uniform(-2, 2, 3)
-        seen = sorted(rng.choice(NP, size=8, replace=False).tolist())
-        obs = " ".join(f"{1.0 + j} {2.0 + j} {(-1 if k % 3 == 0 else p)}" for k, (j, p) in enumerate(zip(range(8), seen)))
-        L += [f"{img_id} {q[0]:.12f} {q[1]:.12f} {q[2]:.12f} {q[3]:.12f} {t[0]:.12f} {t[1]:.12f} {t[2]:.12f} {cam_id} im{img_id}.png", obs]
-        imgs.append((img_id, cam_id, q, t, [p for k, p in enumerate(seen) if k % 3 != 0]))
-    (tmp_path / "images.txt").write_text("\n".join(L) + "\n")
-    (tmp_path / "points3D.txt").write_text("# 3D point list\n" + "\n".join(f"{j} {pts[j,0]:.12f} {pts[j,1]:.12f} {pts[j,2]:.12f} 1 2 3 0.5 10 1" for j in range(NP) if j != 7) + "\n")
-    cams, err = _read_sfm_product(1, tmp_path)
-    assert cams is not None, err
-    assert [c["id"] for c in cams] == [10, 11, 12, 13, 14, 15]                     # image 16 uses an unknown camera: dropped
-    expK = {1: (500.5, 500.5, 320, 240), 2: (500, 510, 321, 239), 3: (400, 400, 300, 200), 4: (410, 410, 310, 210), 5: (700, 710, 400, 300), 6: (701, 711, 401, 301)}
-    expD = {1: (0, 0, 0, 0, 0), 2: (0, 0, 0, 0, 0), 3: (0.01, 0, 0, 0, 0), 4: (0.02, -0.03, 0, 0, 0), 5: (0.1, 0.2, 0, 0.001, 0.002), 6: (0.11, 0.21, 0.31, 0.0011, 0.0021)}
-    rd = lambda a: np.array([float(f"{v:.12f}") for v in np.ravel(a)])
-    for c, (img_id, cam_id, q, t, seen) in zip(cams, imgs):
-        fx, fy, cx, cy = expK[cam_id]
-        assert np.array_equal(c["K"], np.array([[fx, 0, cx], [0, fy, cy], [0, 0, 1.0]])) and c["has_K"]
-        np.testing.assert_allclose(c["dist"], expD[cam_id], atol=1e-15)
-        qq = rd(q); qq = qq / np.linalg.norm(qq); w, x, y, z = qq
-        R = np.array([[1 - 2 * y * y - 2 * z * z, 2 * x * y - 2 * z * w, 2 * x * z + 2 * y * w], [2 * x * y + 2 * z * w, 1 - 2 * x * x - 2 * z * z, 2 * y * z - 2 * x * w],
-                      [2 * x * z - 2 * y * w, 2 * y * z + 2 * x * w, 1 - 2 * x * x - 2 * y * y]])
-        np.testing.assert_allclose(c["R"], R, atol=1e-14); np.testing.assert_allclose(c["t"], rd(t), atol=1e-15)
-        np.testing.assert_allclose(c["C"], -R.T @ rd(t), atol=1e-13)
-        assert c["wps"].tolist() == seen and c["name"] == f"im{img_id}.png"
-        P = np.array([rd(pts[j]) if j != 7 else np.zeros(3) for j in seen])       # a point missing from points3D.txt stays at the origin
-        dep = np.sort(np.array([np.float32(np.linalg.norm(c["C"] - p)) for p in P], np.float32))
-        assert c["md"] == dep[len(dep) // 2]
-    bad, err = _read_sfm_product(1, tmp_path / "nowhere")
-    assert bad is None and "does not exist" in err
-    (tmp_path / "cameras.txt").write_text("1 FISHEYE 10 10 1 2 3\n")
-    bad, err = _read_sfm_product(1, tmp_path)
-    assert bad is None and "FISHEYE unknown" in err
-
-
-
 def test_cpp_frontend_compiles_against_the_public_headers(tmp_path):
     """the drop-in boundary is plain C++: examples/vsfm_frontend.cpp (the reference's main_vsfm.cpp flow on include/line3d.h +
     include/line3d_io.h) must compile warning-free with g++ alone, link against the in-tree library and - without a GPU - fail
