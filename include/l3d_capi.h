@@ -299,13 +299,23 @@ typedef struct {
     int32_t model;                 /* L3D_LENS_RADTAN or L3D_LENS_FISHEYE */
     double rational[3];            /* L3D_LENS_RADTAN: k4, k5, k6 (the denominator of OpenCV's 8-coefficient model) */
     double fisheye[4];             /* L3D_LENS_FISHEYE: k1..k4 of theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 + k4 theta^8) */
+    /* OpenCV's newCameraMatrix and newImageSize; a zero-initialised tail is the camera's own K and the source size, as above.
+     * With them the maps are initUndistortRectifyMap(K, D, I, newK, newSize) (fisheye: cv::fisheye's, with P = newK): the output
+     * pixel (j, i) is taken back through inv(newK) (by cofactors, as above), distorted and projected with the camera's fx, fy, cx, cy.
+     * The output is out_height x out_width: l3d_undistort_u8 writes that many rows to dst with dst_pitch >= out_width * channels;
+     * l3d_undistort_map returns maps of that size; l3d_remap_u8 reads a width x height source with maps of the output size.
+     * Rejected with L3D_ERR_INVALID: a new K that is not all zero and has new_fx or new_fy zero or not finite, or new_cx or new_cy
+     * not finite; an output size other than (0, 0) with a value outside [1, 32767].  Skew is ignored here too.  DESIGN.md §4a. */
+    double new_fx, new_fy, new_cx, new_cy;   /* all four 0: the camera's own K */
+    int32_t out_width, out_height;           /* both 0: the source size */
 } l3d_undistort_desc;
 /* undistort n images in one launch; images, sizes, channel counts and cameras may all differ */
 int l3d_undistort_u8(l3d_ctx* ctx, int n, const l3d_undistort_desc* descs, int on_device);
-/* the fixed-point maps of one image (src, dst and the pitches are not used): map_xy int16[height*width*2] (x, y per pixel),
- * map_frac uint16[height*width] = (v & 31) * 32 + (u & 31); rows packed.  What cv::remap takes as its two maps. */
+/* the fixed-point maps of one image (src, dst and the pitches are not used): map_xy int16[out_height*out_width*2] (x, y per pixel),
+ * map_frac uint16[out_height*out_width] = (v & 31) * 32 + (u & 31); rows packed.  What cv::remap takes as its two maps. */
 int l3d_undistort_map(l3d_ctx* ctx, const l3d_undistort_desc* desc, int16_t* map_xy, uint16_t* map_frac, int on_device);
-/* cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) of one image with caller-given maps in that layout (the camera is not used) */
+/* cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) of one image with caller-given maps in that layout, of the output size (the camera and
+ * the new K are not used) */
 int l3d_remap_u8(l3d_ctx* ctx, const l3d_undistort_desc* desc, const int16_t* map_xy, const uint16_t* map_frac, int on_device);
 
 /* ---- image preparation for line detection: what the reference's detectLineSegments (line3D.cc:249-289) does to an image before LSD

@@ -92,6 +92,16 @@ int l3dpp_undistort_image(const unsigned char* src, unsigned char* dst, int rows
 /* the LensDistortion overload on CUDA device `device` (the thread's current device is restored); lens = model, k[6], p[2] as 9 doubles */
 int l3dpp_undistort_image_lens(const unsigned char* src, unsigned char* dst, int rows, int cols, int channels, const double* lens9, const double* K,
                                int device);
+/* the overload with a new camera matrix (newK row-major, all zero: K) and output size (out_rows = out_cols = 0: rows x cols); dst holds
+ * out_rows x out_cols x channels (rows x cols x channels for 0, 0).  Same returns */
+int l3dpp_undistort_image_newk(const unsigned char* src, unsigned char* dst, int rows, int cols, int channels, const double* lens9, const double* K,
+                               const double* newK, int out_rows, int out_cols, int device);
+/* Line3D::getOptimalNewCameraMatrix: newK[9] row-major, roi[4] = x, y, width, height.  0, or -1 (std::invalid_argument); no GPU used */
+int l3dpp_optimal_new_camera_matrix(const double* K, const double* lens9, int width, int height, double alpha, int new_width, int new_height,
+                                    int center_principal_point, double* newK, int* roi);
+/* Line3D::estimateNewCameraMatrixForUndistortRectify: newK[9] row-major.  0, or -1 (std::invalid_argument); no GPU used */
+int l3dpp_fisheye_new_camera_matrix(const double* K, const double* lens9, int width, int height, double balance, int new_width, int new_height,
+                                    double fov_scale, double* newK);
 
 /* ---- .nvm models (csrc/line3d_sfm.cc) */
 void* l3dpp_nvm_open(const char* path, char* err, int errcap);

@@ -297,6 +297,24 @@ public:
     /* the same for any lens l3d_undistort_u8 takes (the overload above is lens = {RADTAN, {k1, k2, k3, 0, 0, 0}, {p1, p2}});
      * std::invalid_argument also for an unknown model and a fisheye lens with k[4], k[5], p[0] or p[1] nonzero */
     static void undistortImage(const Image8u& in, Image8u& out, const LensDistortion& lens, const Matrix3d& K);
+    /* the same into a chosen camera matrix and size: OpenCV's initUndistortRectifyMap(K, D, I, newK, Size(out_width, out_height)) (or
+     * cv::fisheye's with P = newK) + remap.  Uses newK(0,0), newK(1,1), newK(0,2), newK(1,2); those four all zero: K.  out_width and
+     * out_height both 0: the size of in; out gets out_height x out_width and the channels of in.  With newK zero and the size 0 (or
+     * newK = K and the size of in) this is the overload above, byte for byte.  std::invalid_argument also for a new K or size
+     * l3d_undistort_u8 rejects (include/l3d_capi.h). */
+    static void undistortImage(const Image8u& in, Image8u& out, const LensDistortion& lens, const Matrix3d& K, const Matrix3d& newK, int out_width,
+                               int out_height);
+    /* cv::getOptimalNewCameraMatrix(K, D, Size(width, height), alpha, Size(new_width, new_height), validPixROI, centerPrincipalPoint) for
+     * a RADTAN lens (5 or 8 coefficients), restated in double on the host as OpenCV 4.13 computes it (DESIGN.md §4a).  new_width /
+     * new_height 0: the image size.  validPixROI (optional): x, y, width, height of the all-valid pixels in the new image.  Skew is
+     * taken as zero.  std::invalid_argument for a fisheye lens, a size below 1, or fx / fy zero or not finite. */
+    static Matrix3d getOptimalNewCameraMatrix(const Matrix3d& K, const LensDistortion& lens, int width, int height, double alpha, int new_width = 0,
+                                              int new_height = 0, int validPixROI[4] = nullptr, bool centerPrincipalPoint = false);
+    /* cv::fisheye::estimateNewCameraMatrixForUndistortRectify(K, D, Size(width, height), I, P, balance, Size(new_width, new_height),
+     * fov_scale) for a FISHEYE lens, restated in double on the host (DESIGN.md §4a); R is the identity.  Same exceptions, for a
+     * radtan lens instead. */
+    static Matrix3d estimateNewCameraMatrixForUndistortRectify(const Matrix3d& K, const LensDistortion& lens, int width, int height, double balance = 0.0,
+                                                               int new_width = 0, int new_height = 0, double fov_scale = 1.0);
 
 #ifdef L3DPP_WITH_EIGEN_OPENCV
     /* The reference's exact signature for CV_8UC1 / CV_8UC3 images; honours the row step of inImg and create()s outImg.  A template
@@ -334,6 +352,25 @@ public:
         out.create(in.rows, in.cols, in.type());
         const size_t out_step = static_cast<size_t>(out.step);
         for (int r = 0; r < b.rows; ++r) std::memcpy(out.data + r * out_step, b.data.data() + r * row, row);
+    }
+    /* the cv::Mat form of the overload with a new camera matrix and size; outImg is create()d out_height x out_width (the size of
+     * inImg when both are 0) */
+    template <class MatT = cv::Mat>
+    static void undistortImage(const cv::Mat& inImg, cv::Mat& outImg, const LensDistortion& lens, const Eigen::Matrix3d& K, const Eigen::Matrix3d& newK,
+                               int out_width, int out_height)
+    {
+        const MatT& in = inImg;
+        MatT& out = outImg;
+        if (in.type() != CV_8UC1 && in.type() != CV_8UC3) throw std::invalid_argument("undistortImage: only CV_8UC1 and CV_8UC3 images");
+        Image8u a(in.rows, in.cols, in.channels()), b;
+        const size_t row = (size_t)in.cols * in.channels(), in_step = static_cast<size_t>(in.step);
+        for (int r = 0; r < in.rows; ++r) std::memcpy(a.data.data() + r * row, in.data + r * in_step, row);
+        Matrix3d Kp, nKp;
+        for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) { Kp(r, c) = K(r, c); nKp(r, c) = newK(r, c); }
+        undistortImage(a, b, lens, Kp, nKp, out_width, out_height);
+        out.create(b.rows, b.cols, in.type());
+        const size_t out_row = (size_t)b.cols * b.channels, out_step = static_cast<size_t>(out.step);
+        for (int r = 0; r < b.rows; ++r) std::memcpy(out.data + r * out_step, b.data.data() + r * out_row, out_row);
     }
 #endif
 

@@ -28,22 +28,28 @@ class UndistortDesc(C.Structure):
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("channels", C.c_int32), ("src_pitch", C.c_int64), ("dst_pitch", C.c_int64),
                 ("src", C.c_void_p), ("dst", C.c_void_p), ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
                 ("radial", C.c_double * 3), ("tangential", C.c_double * 2), ("model", C.c_int32), ("rational", C.c_double * 3),
-                ("fisheye", C.c_double * 4)]
+                ("fisheye", C.c_double * 4), ("new_fx", C.c_double), ("new_fy", C.c_double), ("new_cx", C.c_double), ("new_cy", C.c_double),
+                ("out_width", C.c_int32), ("out_height", C.c_int32)]
 
 
 LENS_RADTAN, LENS_FISHEYE = 0, 1     # l3d_undistort_desc::model
 
 
 def make_undistort_desc(width, height, channels, K, radial=(0, 0, 0), tangential=(0, 0), src=0, src_pitch=None, dst=0, dst_pitch=None,
-                        model=LENS_RADTAN, rational=(0, 0, 0), fisheye=(0, 0, 0, 0)):
-    """K: 3x3 camera matrix (fx, fy, cx, cy are read, skew is ignored); src / dst: addresses; pitches in bytes (default packed);
-    model: LENS_RADTAN (radial k1 k2 k3, tangential p1 p2, rational k4 k5 k6) or LENS_FISHEYE (fisheye k1..k4)"""
+                        model=LENS_RADTAN, rational=(0, 0, 0), fisheye=(0, 0, 0, 0), new_K=None, out_size=None):
+    """K: 3x3 camera matrix (fx, fy, cx, cy are read, skew is ignored); src / dst: addresses; pitches in bytes (default packed, dst
+    at the output width); model: LENS_RADTAN (radial k1 k2 k3, tangential p1 p2, rational k4 k5 k6) or LENS_FISHEYE (fisheye k1..k4);
+    new_K: the output's 3x3 camera matrix (None: K); out_size: the output's (width, height) (None: the source size)"""
     K = np.asarray(K, np.float64).reshape(3, 3)
-    row = int(width) * int(channels)
+    ow, oh = (0, 0) if out_size is None else (int(out_size[0]), int(out_size[1]))
     d = UndistortDesc()
     d.width, d.height, d.channels = int(width), int(height), int(channels)
-    d.src_pitch = row if src_pitch is None else int(src_pitch)
-    d.dst_pitch = row if dst_pitch is None else int(dst_pitch)
+    d.src_pitch = int(width) * int(channels) if src_pitch is None else int(src_pitch)
+    d.dst_pitch = (ow or int(width)) * int(channels) if dst_pitch is None else int(dst_pitch)
+    if new_K is not None:
+        nK = np.asarray(new_K, np.float64).reshape(3, 3)
+        d.new_fx, d.new_fy, d.new_cx, d.new_cy = float(nK[0, 0]), float(nK[1, 1]), float(nK[0, 2]), float(nK[1, 2])
+    d.out_width, d.out_height = ow, oh
     d.src, d.dst = int(src) or None, int(dst) or None
     d.fx, d.fy, d.cx, d.cy = float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2])
     d.radial[:] = [float(v) for v in radial]
@@ -52,6 +58,19 @@ def make_undistort_desc(width, height, channels, K, radial=(0, 0, 0), tangential
     d.rational[:] = [float(v) for v in rational]
     d.fisheye[:] = [float(v) for v in fisheye]
     return d
+
+
+def _one_or_per_image(v, n, nd):
+    """[v] * n when v is None or one numeric value of nd dimensions (a 3x3 matrix, a (width, height) pair, as a list, tuple or array),
+    else v's entries, one per image (None entries allowed)"""
+    if v is None:
+        return [None] * n
+    try:
+        a = np.asarray(v)
+        single = a.ndim == nd and a.dtype != object
+    except ValueError:                  # ragged: a list of per-image entries
+        single = False
+    return [v] * n if single else list(v)
 
 
 def lens_desc_args(lens):
@@ -429,25 +448,29 @@ class Context:
                                            int(count_out), int(median_out), 1), "l3d_median_depths")
 
     # ---- lens undistortion (stateless: no pipeline stage changes)
-    def undistort(self, images, K, radial=(0, 0, 0), tangential=(0, 0), out=None, lens=None):
+    def undistort(self, images, K, radial=(0, 0, 0), tangential=(0, 0), out=None, lens=None, new_K=None, out_size=None):
         """Line3D::undistortImage for a list of uint8 HxW / HxWx3 images in ONE batched call.  K, radial, tangential: one camera for
         all images or one per image.  lens: instead of radial / tangential, one lens dict (lens_desc_args) or a list with one per image.
-        out: optional list of preallocated outputs (any row pitch).  Returns the output arrays."""
+        new_K: the output camera matrix (3x3) for all images, or one per image (None entries: the image's K).  out_size: (width,
+        height) for all images, or one per image (None entries: the source size); told apart by np.ndim, as K is.  out: optional list of
+        preallocated outputs of the output size (any row pitch).  Returns the output arrays."""
         n = len(images)
         per = lambda v, nd: [v] * n if np.ndim(v) == nd else list(v)
         Ks, rads, tans = per(K, 2), per(radial, 1), per(tangential, 1)
         lenses = [None] * n if lens is None else [lens] * n if isinstance(lens, dict) else list(lens)
+        newKs, sizes = _one_or_per_image(new_K, n, 2), _one_or_per_image(out_size, n, 1)
         descs, keep = (UndistortDesc * n)(), []
         outs = []
         for i, img in enumerate(images):
             a, sp = _image_rows(img)
-            o = np.empty_like(a) if out is None else out[i]
-            if o.shape != a.shape or o.dtype != np.uint8 or o.strides[1:] != a.strides[1:]:
-                raise ValueError("output must be a uint8 array of the input's shape with packed rows")
+            shape = a.shape if sizes[i] is None else (int(sizes[i][1]), int(sizes[i][0])) + a.shape[2:]
+            o = np.empty(shape, np.uint8) if out is None else out[i]
+            if o.shape != shape or o.dtype != np.uint8 or o.strides[1:] != a.strides[1:]:
+                raise ValueError("output must be a uint8 array of the output's shape with packed rows")
             keep += [a, o]
             lk = dict(radial=rads[i], tangential=tans[i]) if lenses[i] is None else lens_desc_args(lenses[i])
             descs[i] = make_undistort_desc(a.shape[1], a.shape[0], 1 if a.ndim == 2 else 3, Ks[i], src=a.ctypes.data, src_pitch=sp,
-                                           dst=o.ctypes.data, dst_pitch=o.strides[0], **lk)
+                                           dst=o.ctypes.data, dst_pitch=o.strides[0], new_K=newKs[i], out_size=sizes[i], **lk)
             outs.append(o)
         self._chk(self.L.l3d_undistort_u8(self.h, n, descs, 0), "l3d_undistort_u8")
         return outs
@@ -478,24 +501,29 @@ class Context:
         """l3d_undistort_u8 on device addresses (a ctypes array of UndistortDesc); asynchronous on the context's stream"""
         self._chk(self.L.l3d_undistort_u8(self.h, len(descs), descs, 1), "l3d_undistort_u8")
 
-    def undistort_map(self, width, height, K, radial=(0, 0, 0), tangential=(0, 0), lens=None):
-        """the fixed-point maps cv::remap takes: (map_xy int16 [h, w, 2], map_frac uint16 [h, w]); lens as in undistort"""
+    def undistort_map(self, width, height, K, radial=(0, 0, 0), tangential=(0, 0), lens=None, new_K=None, out_size=None):
+        """the fixed-point maps cv::remap takes: (map_xy int16 [oh, ow, 2], map_frac uint16 [oh, ow]) over the output grid (out_size
+        = (ow, oh), default the source's width x height); lens, new_K as in undistort"""
         lk = dict(radial=radial, tangential=tangential) if lens is None else lens_desc_args(lens)
-        d = make_undistort_desc(width, height, 1, K, **lk)
-        xy = np.empty((height, width, 2), np.int16)
-        fr = np.empty((height, width), np.uint16)
+        d = make_undistort_desc(width, height, 1, K, new_K=new_K, out_size=out_size, **lk)
+        ow, oh = (width, height) if out_size is None else (int(out_size[0]), int(out_size[1]))
+        xy = np.empty((oh, ow, 2), np.int16)
+        fr = np.empty((oh, ow), np.uint16)
         self._chk(self.L.l3d_undistort_map(self.h, C.byref(d), _p(xy), _p(fr), 0), "l3d_undistort_map")
         return xy, fr
 
     def remap(self, image, map_xy, map_frac):
-        """cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) of a uint8 HxW / HxWx3 image with fixed-point maps"""
+        """cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) of a uint8 HxW / HxWx3 image with fixed-point maps; the output has the maps'
+        size (the source's unless they are another size)"""
         a, sp = _image_rows(image)
         xy = np.ascontiguousarray(map_xy, np.int16)
         fr = np.ascontiguousarray(map_frac, np.uint16)
-        if xy.shape != a.shape[:2] + (2,) or fr.shape != a.shape[:2]:
-            raise ValueError("maps must be [h, w, 2] int16 and [h, w] uint16")
-        o = np.empty(a.shape, np.uint8)
-        d = make_undistort_desc(a.shape[1], a.shape[0], 1 if a.ndim == 2 else 3, np.eye(3), src=a.ctypes.data, src_pitch=sp, dst=o.ctypes.data)
+        if xy.ndim != 3 or xy.shape[2] != 2 or fr.shape != xy.shape[:2]:
+            raise ValueError("maps must be [oh, ow, 2] int16 and [oh, ow] uint16")
+        o = np.empty(fr.shape + a.shape[2:], np.uint8)
+        size = None if fr.shape == a.shape[:2] else (fr.shape[1], fr.shape[0])
+        d = make_undistort_desc(a.shape[1], a.shape[0], 1 if a.ndim == 2 else 3, np.eye(3), src=a.ctypes.data, src_pitch=sp, dst=o.ctypes.data,
+                                out_size=size)
         self._chk(self.L.l3d_remap_u8(self.h, C.byref(d), _p(xy), _p(fr), 0), "l3d_remap_u8")
         return o
 

@@ -61,17 +61,18 @@ struct RddState {
 };
 
 // per-image parameters of the undistortion kernels (l3d_undistort.cu); ir0, ir2, ir4, ir5 = the non-trivial entries of
-// inv([[fx,0,cx],[0,fy,cy],[0,0,1]])
+// inv([[fx',0,cx'],[0,fy',cy'],[0,0,1]]) of the new camera matrix (the camera's own K unless one is given); fx .. cy are the camera's
 struct L3DUndistImage {
     const unsigned char* src;
     unsigned char* dst;
-    const double* xcol;                      // fisheye: x of every column (OpenCV's accumulated sum), in UndistortState::d_cols
+    const double* xcol;                      // fisheye: x of every output column (OpenCV's accumulated sum), in UndistortState::d_cols
     long long src_pitch, dst_pitch, tile0;   // tile0: first tile of this image in the batch grid
-    int width, height, channels, tiles_x;
+    int width, height, channels, tiles_x;    // width, height: the source (bounds the taps); tiles_x: of the output
     int kind;                                // lens kind of l3d_undistort.cu: radtan, radtan with k4..k6 (rational), fisheye
     int full_radial, tangential;             // 0: k2 = k3 = 0, resp. p1 = p2 = 0 (those terms are skipped)
     double ir0, ir2, ir4, ir5, fx, fy, cx, cy;
     double k1, k2, k3, k4, k5, k6, p1, p2;   // radtan: k1..k6, p1, p2; fisheye: k1..k4 are the theta coefficients
+    int out_width, out_height;               // the output grid (the source size unless one is given)
 };
 
 // buffers of the undistortion calls: not a pipeline stage, nothing else reads them

@@ -1,7 +1,7 @@
 // l3d_undistort.cu — lens undistortion of 8-bit images: what Line3D::undistortImage computes with OpenCV (line3D.cc:83-109,
 // initUndistortRectifyMap with fixed-point CV_16SC2 + CV_16UC1 maps, then remap INTER_LINEAR / BORDER_CONSTANT 0), and the three
 // C-ABI entry points declared in include/l3d_capi.h.  Two lens models: OpenCV's standard one with up to 8 coefficients (radtan) and
-// cv::fisheye's.  The arithmetic contract is DESIGN.md §4a; tests/undistort_model.py and tests/lens_model.py restate it.
+// cv::fisheye's.  The output may have its own camera matrix and size (OpenCV's newCameraMatrix / newImageSize).  The arithmetic contract is DESIGN.md §4a; tests/undistort_model.py and tests/lens_model.py restate it.
 //
 // None of these calls belongs to the pipeline: they never drop a stage and touch only the buffers of UndistortState.
 #include "l3d_ctx.cuh"
@@ -26,8 +26,8 @@ __device__ __forceinline__ int ud_fix(double t)
     return (r >= -2147483648.0 && r <= 2147483647.0) ? (int)r : INT_MIN;
 }
 
-// Fixed-point source position (u*32, v*32) of the pixel whose normalised coordinates are x = ir2 + j*ir0, y = i*ir4 + ir5
-// (the zero entries of ir only add signed zeros).  x2 = x*x and y2 = y*y come from the caller so that a tile computes them once
+// Fixed-point source position (u*32, v*32) of the output pixel whose normalised coordinates are x = ir2 + j*ir0, y = i*ir4 + ir5
+// (ir: the inverse of the new camera matrix; its zero entries only add signed zeros), projected with the camera's fx, fy, cx, cy.  x2 = x*x and y2 = y*y come from the caller so that a tile computes them once
 // per column / row.  Terms whose coefficients are zero are skipped: that changes at most the sign of a zero, which the rounding
 // erases.  Plain IEEE double operations in the reference's order (the library is compiled with -fmad=false).
 template <bool RATIONAL>
@@ -46,7 +46,7 @@ __device__ __forceinline__ void ud_map_point(const L3DUndistImage& d, double x, 
     iv = ud_fix(d.fy * yd + d.cy);
 }
 
-// The same for cv::fisheye::initUndistortRectifyMap with R = I, newK = K: x comes from the column table (OpenCV's loop accumulates it),
+// The same for cv::fisheye::initUndistortRectifyMap with R = I, P = newK: x comes from the column table (OpenCV's loop accumulates it),
 // r = |(x, y)|, theta = atan(r), theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 + k4 theta^8), u = fx x (theta_d / r) + cx.
 // Everything but atan is IEEE; atan may differ from the host's in the last ulp (the fisheye contract is one step, DESIGN.md §4a).
 __device__ __forceinline__ void ud_fisheye_point(const L3DUndistImage& d, double x, double x2, double y, double y2, int& iu, int& iv)
@@ -113,25 +113,25 @@ __device__ __forceinline__ void ud_tap_sum(const unsigned char* __restrict__ src
     for (int c = 0; c < C; ++c) out[c] = (unsigned char)max(0, min(255, (acc[c] + 16384) >> 15));
 }
 
-// the maps of one image, OpenCV's layout: map_xy short2[H*W], map_frac ushort[H*W], rows packed
+// the maps of one image, OpenCV's layout: map_xy short2[oH*oW], map_frac ushort[oH*oW] over the output grid, rows packed
 template <int KIND>
 __global__ void __launch_bounds__(UD_TW) k_undistort_map(L3DUndistImage d, short2* __restrict__ map_xy, unsigned short* __restrict__ map_frac)
 {
     const int j = blockIdx.x * UD_TW + threadIdx.x, i = blockIdx.y;
-    if (j >= d.width) return;
+    if (j >= d.out_width) return;
     const double y = (double)i * d.ir4 + d.ir5;
-    const long long o = (long long)i * d.width + j;
+    const long long o = (long long)i * d.out_width + j;
     const double x = ud_column_x<KIND>(d, j);
     ud_map_entry<KIND>(d, x, x * x, y, y * y, map_xy[o], map_frac[o]);
 }
 
-// remap of one image with caller-given maps (same layout)
+// remap of one image with caller-given maps (same layout, output grid); the taps are bounded by the source size
 template <int C>
 __global__ void __launch_bounds__(UD_TW) k_remap_u8(L3DUndistImage d, const short2* __restrict__ map_xy, const unsigned short* __restrict__ map_frac)
 {
     const int j = blockIdx.x * UD_TW + threadIdx.x, i = blockIdx.y;
-    if (j >= d.width) return;
-    const long long o = (long long)i * d.width + j;
+    if (j >= d.out_width) return;
+    const long long o = (long long)i * d.out_width + j;
     ud_tap_sum<C>(d.src, d.src_pitch, d.width, d.height, map_xy[o], map_frac[o], d.dst + (long long)i * d.dst_pitch + (long long)j * C);
 }
 
@@ -147,14 +147,10 @@ __device__ __forceinline__ void ud_tile_rows(const L3DUndistImage& d, int j, int
     }
 }
 
-// The fused hot path over a batch: map entries in registers, never stored.  One CTA = UD_TW columns x UD_TH rows of one image;
-// the tiles of all images of one model form one grid (image found by binary search over tile0), grey and RGB images alike.  One
-// instance per lens kind (UD_RADTAN ..), each over its own images.
+// One CTA's work of k_undistort_u8: UD_TW output columns x UD_TH output rows of the image d (the taps are bounded by its source size)
 template <int KIND>
-__global__ void __launch_bounds__(UD_TW) k_undistort_u8(const L3DUndistImage* __restrict__ imgs, int n)
+__device__ __forceinline__ void ud_tile(const L3DUndistImage& d, double2* s_y)
 {
-    __shared__ double2 s_y[UD_TH];          // (y, y*y) of the tile's rows
-    const L3DUndistImage d = imgs[last_le(n, (long long)blockIdx.x, [&](int i) { return imgs[i].tile0; })];
     const long long t = (long long)blockIdx.x - d.tile0;
     const int i0 = (int)(t / d.tiles_x) * UD_TH, j = (int)(t % d.tiles_x) * UD_TW + threadIdx.x;
     if (threadIdx.x < UD_TH) {
@@ -162,10 +158,32 @@ __global__ void __launch_bounds__(UD_TW) k_undistort_u8(const L3DUndistImage* __
         s_y[threadIdx.x] = make_double2(y, y * y);
     }
     __syncthreads();
-    if (j >= d.width) return;
-    const int rows = min(UD_TH, d.height - i0);
+    if (j >= d.out_width) return;
+    const int rows = min(UD_TH, d.out_height - i0);
     if (d.channels == 3) ud_tile_rows<KIND, 3>(d, j, i0, rows, s_y);
     else ud_tile_rows<KIND, 1>(d, j, i0, rows, s_y);
+}
+
+// The fused hot path over a batch: map entries in registers, never stored.  One CTA = UD_TW columns x UD_TH rows of one image's
+// output grid; the tiles of all images of one model form one grid (image found by binary search over tile0), grey and RGB images
+// alike.  One instance per lens kind (UD_RADTAN ..), each over its own images.  The pinhole and fisheye instances hold the descriptor
+// in registers (48 and 55).  The rational one would need 72 that way; it reads the descriptor from a shared-memory copy instead, which
+// the compiler reloads where it is used (the output may alias it as far as the compiler knows), and stays below 64.
+template <int KIND>
+__global__ void __launch_bounds__(UD_TW) k_undistort_u8(const L3DUndistImage* __restrict__ imgs, int n)
+{
+    __shared__ double2 s_y[UD_TH];          // (y, y*y) of the tile's rows
+    const L3DUndistImage* g = imgs + last_le(n, (long long)blockIdx.x, [&](int i) { return imgs[i].tile0; });
+    if (KIND == UD_RATIONAL) {
+        __shared__ L3DUndistImage s_d;
+        static_assert(sizeof(L3DUndistImage) % 8 == 0 && sizeof(L3DUndistImage) / 8 <= UD_TW, "descriptor staging");
+        if (threadIdx.x < sizeof(L3DUndistImage) / 8) ((long long*)&s_d)[threadIdx.x] = __ldg((const long long*)g + threadIdx.x);
+        __syncthreads();
+        ud_tile<KIND>(s_d, s_y);
+    } else {
+        const L3DUndistImage d = *g;
+        ud_tile<KIND>(d, s_y);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -176,9 +194,11 @@ static int ud_check(l3d_ctx* c, const l3d_undistort_desc& u, bool image, bool ca
     auto bad = [&](const char* why) { snprintf(buf, sizeof(buf), "%s: %s", what, why); return l3d_fail(c, L3D_ERR_INVALID, buf); };
     if (u.width < 1 || u.width > 32767 || u.height < 1 || u.height > 32767) return bad("width and height must lie in [1, 32767]");
     if (u.channels != 1 && u.channels != 3) return bad("channels must be 1 or 3");
+    if ((u.out_width != 0 || u.out_height != 0) && (u.out_width < 1 || u.out_width > 32767 || u.out_height < 1 || u.out_height > 32767))
+        return bad("out_width and out_height must both be 0 or lie in [1, 32767]");
     if (image) {
-        const long long row = (long long)u.width * u.channels;
-        if (u.src_pitch < row || u.dst_pitch < row) return bad("row pitch below width * channels");
+        if (u.src_pitch < (long long)u.width * u.channels) return bad("row pitch below width * channels");
+        if (u.dst_pitch < (long long)(u.out_width ? u.out_width : u.width) * u.channels) return bad("dst row pitch below out_width * channels");
         if (!u.src || !u.dst) return bad("null image pointer");
         if (u.src == u.dst) return bad("src == dst (no in-place undistortion)");
     }
@@ -191,20 +211,32 @@ static int ud_check(l3d_ctx* c, const l3d_undistort_desc& u, bool image, bool ca
         if (!finite) return bad("principal point and coefficients must be finite");
         if (u.model != L3D_LENS_RADTAN && u.model != L3D_LENS_FISHEYE) return bad("unknown lens model");
         if (u.model == L3D_LENS_FISHEYE && !zero) return bad("a fisheye lens takes no radial, tangential or rational coefficients");
+        const bool new_k = u.new_fx != 0.0 || u.new_fy != 0.0 || u.new_cx != 0.0 || u.new_cy != 0.0;
+        if (new_k && (!std::isfinite(u.new_fx) || !std::isfinite(u.new_fy) || u.new_fx == 0.0 || u.new_fy == 0.0))
+            return bad("new_fx and new_fy must be finite and non-zero");
+        if (new_k && (!std::isfinite(u.new_cx) || !std::isfinite(u.new_cy))) return bad("new_cx and new_cy must be finite");
     }
     return L3D_OK;
 }
 
-// kernel parameters of one image; the inverse camera matrix is formed like OpenCV's 3x3 inversion (cofactors / determinant)
+static int ud_out_width(const l3d_undistort_desc& u) { return u.out_width ? u.out_width : u.width; }
+static int ud_out_height(const l3d_undistort_desc& u) { return u.out_height ? u.out_height : u.height; }
+
+// kernel parameters of one image; the inverse of the new camera matrix (the camera's own K when new_fx .. new_cy are all zero) is
+// formed like OpenCV's 3x3 inversion (cofactors / determinant).  cv::fisheye inverts by SVD instead, which can differ in the last
+// bits; DESIGN.md §4a counts what that costs.
 static L3DUndistImage ud_image(const l3d_undistort_desc& u, const unsigned char* src, long long src_pitch, unsigned char* dst, long long dst_pitch)
 {
     L3DUndistImage d;
     memset(&d, 0, sizeof(d));
     d.src = src; d.dst = dst; d.src_pitch = src_pitch; d.dst_pitch = dst_pitch;
     d.width = u.width; d.height = u.height; d.channels = u.channels;
-    d.tiles_x = (u.width + UD_TW - 1) / UD_TW;
-    const double det = u.fx * u.fy, id = 1.0 / det;
-    d.ir0 = u.fy * id; d.ir2 = -(u.cx * u.fy) * id; d.ir4 = u.fx * id; d.ir5 = -(u.fx * u.cy) * id;
+    d.out_width = ud_out_width(u); d.out_height = ud_out_height(u);
+    d.tiles_x = (d.out_width + UD_TW - 1) / UD_TW;
+    const bool new_k = u.new_fx != 0.0 || u.new_fy != 0.0 || u.new_cx != 0.0 || u.new_cy != 0.0;
+    const double nfx = new_k ? u.new_fx : u.fx, nfy = new_k ? u.new_fy : u.fy, ncx = new_k ? u.new_cx : u.cx, ncy = new_k ? u.new_cy : u.cy;
+    const double det = nfx * nfy, id = 1.0 / det;
+    d.ir0 = nfy * id; d.ir2 = -(ncx * nfy) * id; d.ir4 = nfx * id; d.ir5 = -(nfx * ncy) * id;
     d.fx = u.fx; d.fy = u.fy; d.cx = u.cx; d.cy = u.cy;
     if (u.model == L3D_LENS_FISHEYE) {
         d.kind = UD_FISHEYE;
@@ -220,7 +252,7 @@ static L3DUndistImage ud_image(const l3d_undistort_desc& u, const unsigned char*
 }
 
 // The column tables of the fisheye images among imgs[0, n): x_0 = ir2, x_{j+1} = x_j + ir0, summed in order as OpenCV's loop does.
-// Images whose (ir0, ir2) agree share one table (its prefixes are the same), as long as the widest of them.  Sets every fisheye
+// Images whose (ir0, ir2) agree share one table (its prefixes are the same), as long as the widest output among them.  Sets every fisheye
 // image's xcol; the tables are uploaded on the context's stream.
 static int ud_column_tables(l3d_ctx* c, UndistortState& s, L3DUndistImage* imgs, int n)
 {
@@ -232,7 +264,7 @@ static int ud_column_tables(l3d_ctx* c, UndistortState& s, L3DUndistImage* imgs,
         size_t k = 0;
         while (k < keys.size() && !(keys[k].ir0 == imgs[i].ir0 && keys[k].ir2 == imgs[i].ir2)) ++k;
         if (k == keys.size()) keys.push_back(Key{imgs[i].ir0, imgs[i].ir2, 0, 0});
-        keys[k].width = std::max(keys[k].width, imgs[i].width);
+        keys[k].width = std::max(keys[k].width, imgs[i].out_width);
         which[i] = (int)k;
     }
     if (keys.empty()) return L3D_OK;
@@ -252,7 +284,8 @@ static int ud_column_tables(l3d_ctx* c, UndistortState& s, L3DUndistImage* imgs,
     return L3D_OK;
 }
 
-static dim3 ud_grid(const l3d_undistort_desc& u) { return dim3((unsigned)((u.width + UD_TW - 1) / UD_TW), (unsigned)u.height); }
+// one CTA row per output row, UD_TW output columns per CTA
+static dim3 ud_grid(const l3d_undistort_desc& u) { return dim3((unsigned)((ud_out_width(u) + UD_TW - 1) / UD_TW), (unsigned)ud_out_height(u)); }
 
 extern "C" {
 
@@ -268,23 +301,27 @@ int l3d_undistort_u8(l3d_ctx* c, int n, const l3d_undistort_desc* descs, int on_
     cudaSetDevice(c->device);
     UndistortState& s = c->undist;
     int rc;
-    size_t staged = 0;                      // host mode: packed copies of every image on the device
+    size_t staged_src = 0, staged_dst = 0;  // host mode: packed copies of every source and output on the device
     if (!on_device) {
-        for (int i = 0; i < n; ++i) staged += (size_t)descs[i].width * descs[i].channels * descs[i].height;
-        L3D_RESERVE(s.d_src, staged, "undistort source staging");
-        L3D_RESERVE(s.d_dst, staged, "undistort output staging");
+        for (int i = 0; i < n; ++i) {
+            staged_src += (size_t)descs[i].width * descs[i].channels * descs[i].height;
+            staged_dst += (size_t)ud_out_width(descs[i]) * descs[i].channels * ud_out_height(descs[i]);
+        }
+        L3D_RESERVE(s.d_src, staged_src, "undistort source staging");
+        L3D_RESERVE(s.d_dst, staged_dst, "undistort output staging");
     }
     s.h_imgs.resize(n);
-    size_t off = 0;
+    size_t off = 0, off_dst = 0;
     for (int i = 0; i < n; ++i) {
         const l3d_undistort_desc& u = descs[i];
-        const long long row = (long long)u.width * u.channels;
+        const long long row = (long long)u.width * u.channels, out_row = (long long)ud_out_width(u) * u.channels;
         if (on_device) s.h_imgs[i] = ud_image(u, u.src, u.src_pitch, u.dst, u.dst_pitch);
         else {
             unsigned char* src = (unsigned char*)s.d_src.p + off;
             L3D_CUDA(c, cudaMemcpy2DAsync(src, row, u.src, u.src_pitch, row, u.height, cudaMemcpyHostToDevice, c->stream), "upload image");
-            s.h_imgs[i] = ud_image(u, src, row, (unsigned char*)s.d_dst.p + off, row);
+            s.h_imgs[i] = ud_image(u, src, row, (unsigned char*)s.d_dst.p + off_dst, out_row);
             off += (size_t)row * u.height;
+            off_dst += (size_t)out_row * ud_out_height(u);
         }
     }
     // the images grouped by lens kind: one grid per kind, each numbering its tiles from 0
@@ -294,7 +331,7 @@ int l3d_undistort_u8(l3d_ctx* c, int n, const l3d_undistort_desc* descs, int on_
     for (int i = 0; i < n; ++i) {
         L3DUndistImage& d = s.h_imgs[i];
         d.tile0 = tiles[d.kind];
-        tiles[d.kind] += (long long)d.tiles_x * ((d.height + UD_TH - 1) / UD_TH);
+        tiles[d.kind] += (long long)d.tiles_x * ((d.out_height + UD_TH - 1) / UD_TH);
         if (tiles[d.kind] >= (1ll << 31)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_undistort_u8: more than 2^31 tiles in one call");
         first[d.kind + 1] = i + 1;
     }
@@ -315,10 +352,10 @@ int l3d_undistort_u8(l3d_ctx* c, int n, const l3d_undistort_desc* descs, int on_
         off = 0;
         for (int i = 0; i < n; ++i) {
             const l3d_undistort_desc& u = descs[i];
-            const size_t row = (size_t)u.width * u.channels;
-            L3D_CUDA(c, cudaMemcpy2DAsync(u.dst, u.dst_pitch, (const unsigned char*)s.d_dst.p + off, row, row, u.height, cudaMemcpyDeviceToHost, c->stream),
-                     "download image");
-            off += row * u.height;
+            const size_t row = (size_t)ud_out_width(u) * u.channels;
+            L3D_CUDA(c, cudaMemcpy2DAsync(u.dst, u.dst_pitch, (const unsigned char*)s.d_dst.p + off, row, row, ud_out_height(u), cudaMemcpyDeviceToHost,
+                                          c->stream), "download image");
+            off += row * ud_out_height(u);
         }
         L3D_CUDA(c, cudaStreamSynchronize(c->stream), "l3d_undistort_u8");
     }
@@ -334,7 +371,7 @@ int l3d_undistort_map(l3d_ctx* c, const l3d_undistort_desc* desc, int16_t* map_x
     if (rc) return rc;
     cudaSetDevice(c->device);
     UndistortState& s = c->undist;
-    const size_t px = (size_t)desc->width * desc->height;
+    const size_t px = (size_t)ud_out_width(*desc) * ud_out_height(*desc);
     short2* xy = (short2*)map_xy; unsigned short* fr = map_frac;
     if (!on_device) {
         L3D_RESERVE(s.d_map_xy, 4 * px, "undistort map");
@@ -366,18 +403,18 @@ int l3d_remap_u8(l3d_ctx* c, const l3d_undistort_desc* desc, const int16_t* map_
     cudaSetDevice(c->device);
     UndistortState& s = c->undist;
     const l3d_undistort_desc& u = *desc;
-    const size_t px = (size_t)u.width * u.height, row = (size_t)u.width * u.channels;
+    const size_t px = (size_t)ud_out_width(u) * ud_out_height(u), row = (size_t)u.width * u.channels, out_row = (size_t)ud_out_width(u) * u.channels;
     L3DUndistImage d = ud_image(u, u.src, u.src_pitch, u.dst, u.dst_pitch);
     const short2* xy = (const short2*)map_xy; const unsigned short* fr = map_frac;
     if (!on_device) {
         L3D_RESERVE(s.d_src, row * u.height, "remap source staging");
-        L3D_RESERVE(s.d_dst, row * u.height, "remap output staging");
+        L3D_RESERVE(s.d_dst, out_row * ud_out_height(u), "remap output staging");
         L3D_RESERVE(s.d_map_xy, 4 * px, "remap map");
         L3D_RESERVE(s.d_map_frac, 2 * px, "remap map fractions");
         L3D_CUDA(c, cudaMemcpy2DAsync(s.d_src.p, row, u.src, u.src_pitch, row, u.height, cudaMemcpyHostToDevice, c->stream), "upload image");
         L3D_CUDA(c, cudaMemcpyAsync(s.d_map_xy.p, map_xy, 4 * px, cudaMemcpyHostToDevice, c->stream), "upload map");
         L3D_CUDA(c, cudaMemcpyAsync(s.d_map_frac.p, map_frac, 2 * px, cudaMemcpyHostToDevice, c->stream), "upload map fractions");
-        d.src = (const unsigned char*)s.d_src.p; d.dst = (unsigned char*)s.d_dst.p; d.src_pitch = d.dst_pitch = (long long)row;
+        d.src = (const unsigned char*)s.d_src.p; d.dst = (unsigned char*)s.d_dst.p; d.src_pitch = (long long)row; d.dst_pitch = (long long)out_row;
         xy = (const short2*)s.d_map_xy.p; fr = (const unsigned short*)s.d_map_frac.p;
     }
     if (u.channels == 3) k_remap_u8<3><<<ud_grid(u), UD_TW, 0, c->stream>>>(d, xy, fr);
@@ -385,7 +422,8 @@ int l3d_remap_u8(l3d_ctx* c, const l3d_undistort_desc* desc, const int16_t* map_
     ++c->launches;
     L3D_CUDA(c, cudaGetLastError(), "k_remap_u8");
     if (!on_device) {
-        L3D_CUDA(c, cudaMemcpy2DAsync(u.dst, u.dst_pitch, s.d_dst.p, row, row, u.height, cudaMemcpyDeviceToHost, c->stream), "download image");
+        L3D_CUDA(c, cudaMemcpy2DAsync(u.dst, u.dst_pitch, s.d_dst.p, out_row, out_row, ud_out_height(u), cudaMemcpyDeviceToHost, c->stream),
+                 "download image");
         L3D_CUDA(c, cudaStreamSynchronize(c->stream), "l3d_remap_u8");
     }
     return L3D_OK;

@@ -1044,19 +1044,33 @@ void Line3D::undistortImage(const Image8u& in, Image8u& out, const Vector3d& rad
 
 void Line3D::undistortImage(const Image8u& in, Image8u& out, const LensDistortion& lens, const Matrix3d& K)
 {
+    Matrix3d none;
+    std::memset(&none, 0, sizeof(none));
+    undistortImage(in, out, lens, K, none, 0, 0);
+}
+
+void Line3D::undistortImage(const Image8u& in, Image8u& out, const LensDistortion& lens, const Matrix3d& K, const Matrix3d& newK, int out_width,
+                            int out_height)
+{
     if (in.data.size() != (size_t)in.rows * in.cols * in.channels || in.rows < 0 || in.cols < 0)
         throw std::invalid_argument("undistortImage: the pixel buffer does not match rows x cols x channels");
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) throw std::runtime_error("undistortImage: no usable CUDA device");
     l3d_ctx* ctx = nullptr;
     if (l3d_ctx_create(dev, &ctx) != L3D_OK) throw std::runtime_error("undistortImage: no usable CUDA device");
-    Image8u res(in.rows, in.cols, in.channels);       // a separate buffer: in and out may be the same image
+    // a separate buffer: in and out may be the same image.  A size l3d_undistort_u8 rejects gets an empty one; the call fails.
+    const bool size_ok = (out_width == 0 && out_height == 0) || (out_width >= 1 && out_width <= 32767 && out_height >= 1 && out_height <= 32767);
+    const int ow = out_width == 0 && out_height == 0 ? in.cols : out_width, oh = out_width == 0 && out_height == 0 ? in.rows : out_height;
+    Image8u res(size_ok ? oh : 0, size_ok ? ow : 0, in.channels);
     l3d_undistort_desc d;
     std::memset(&d, 0, sizeof(d));
     d.width = in.cols; d.height = in.rows; d.channels = in.channels;
-    d.src_pitch = d.dst_pitch = (int64_t)in.cols * in.channels;
+    d.src_pitch = (int64_t)in.cols * in.channels;
+    d.dst_pitch = (int64_t)(size_ok ? ow : in.cols) * in.channels;
     d.src = in.data.data(); d.dst = res.data.data();
     d.fx = K(0, 0); d.fy = K(1, 1); d.cx = K(0, 2); d.cy = K(1, 2);
+    d.new_fx = newK(0, 0); d.new_fy = newK(1, 1); d.new_cx = newK(0, 2); d.new_cy = newK(1, 2);
+    d.out_width = out_width; d.out_height = out_height;
     d.model = lens.model;
     d.tangential[0] = lens.p[0]; d.tangential[1] = lens.p[1];
     if (lens.model == LensDistortion::FISHEYE) {   // k[4], k[5] go where l3d_undistort_u8 rejects them if nonzero
@@ -1266,18 +1280,24 @@ int l3dpp_undistort_image(const unsigned char* src, unsigned char* dst, int rows
 int l3dpp_undistort_image_lens(const unsigned char* src, unsigned char* dst, int rows, int cols, int channels, const double* lens9, const double* K,
                                int device)
 {
+    const double zero[9] = {};
+    return l3dpp_undistort_image_newk(src, dst, rows, cols, channels, lens9, K, zero, 0, 0, device);
+}
+int l3dpp_undistort_image_newk(const unsigned char* src, unsigned char* dst, int rows, int cols, int channels, const double* lens9, const double* K,
+                               const double* newK, int out_rows, int out_cols, int device)
+{
     int prev = 0;
     if (cudaGetDevice(&prev) != cudaSuccess || cudaSetDevice(device) != cudaSuccess) return -2;
     struct Restore { int d; ~Restore() { cudaSetDevice(d); } } restore{prev};
     Image8u in(rows, cols, channels), out;
     if (!in.data.empty()) memcpy(in.data.data(), src, in.data.size());
-    Matrix3d Km; memcpy(Km.m, K, 72);
+    Matrix3d Km, nKm; memcpy(Km.m, K, 72); memcpy(nKm.m, newK, 72);
     LensDistortion lens;
     lens.model = (int)lens9[0];
     for (int k = 0; k < 6; ++k) lens.k[k] = lens9[1 + k];
     lens.p[0] = lens9[7]; lens.p[1] = lens9[8];
     try {
-        Line3D::undistortImage(in, out, lens, Km);
+        Line3D::undistortImage(in, out, lens, Km, nKm, out_cols, out_rows);
     } catch (const std::invalid_argument&) { return -1; } catch (const std::exception&) { return -2; }
     memcpy(dst, out.data.data(), out.data.size());
     return 0;

@@ -379,23 +379,56 @@ def read_colmap(sfm_folder, lenses=True):
     return _read_sfm(SFM_COLMAP_LENSES if lenses else SFM_COLMAP, sfm_folder)
 
 
-def undistort_image(img, K, lens, device=0):
-    """Line3D::undistortImage(in, out, lens, K) of a uint8 HxW / HxWx3 image on GPU `device`; lens as read_colmap gives it"""
+def _lens9(lens):
+    """a lens dict as L3DPP::LensDistortion's 9 doubles: model, k[6], p[2]"""
+    k = [float(v) for v in lens.get("k", ())] + [0.0] * 6
+    pp = [float(v) for v in lens.get("p", ())] + [0.0] * 2
+    return np.array([float(lens.get("model", capi.LENS_RADTAN))] + k[:6] + pp[:2], np.float64)
+
+
+def undistort_image(img, K, lens, new_K=None, out_size=None, device=0):
+    """Line3D::undistortImage(in, out, lens, K[, newK, out_width, out_height]) of a uint8 HxW / HxWx3 image on GPU `device`; lens as
+    read_colmap gives it.  new_K: the output's camera matrix (None: K), e.g. from optimal_new_camera_matrix or
+    fisheye_new_camera_matrix; out_size: the output's (width, height) (None: the image's)"""
     a = np.ascontiguousarray(img, np.uint8)
     if a.ndim not in (2, 3) or (a.ndim == 3 and a.shape[2] != 3):
         raise ValueError("image must be uint8 HxW or HxWx3")
     Kd = np.ascontiguousarray(K, np.float64).reshape(9)
-    k = [float(v) for v in lens.get("k", ())] + [0.0] * 6
-    pp = [float(v) for v in lens.get("p", ())] + [0.0] * 2
-    l9 = np.array([float(lens.get("model", capi.LENS_RADTAN))] + k[:6] + pp[:2], np.float64)
-    out = np.empty_like(a)
+    nK = np.zeros(9) if new_K is None else np.ascontiguousarray(new_K, np.float64).reshape(9)
+    ow, oh = (0, 0) if out_size is None else (int(out_size[0]), int(out_size[1]))
+    out = np.empty(((oh, ow) if out_size is not None and ow >= 1 and oh >= 1 else a.shape[:2]) + a.shape[2:], np.uint8)
     L = capi.lib()
-    rc = L.l3dpp_undistort_image_lens(_p(a), _p(out), a.shape[0], a.shape[1], 1 if a.ndim == 2 else 3, _p(l9), _p(Kd), int(device))
+    rc = L.l3dpp_undistort_image_newk(_p(a), _p(out), a.shape[0], a.shape[1], 1 if a.ndim == 2 else 3, _p(_lens9(lens)), _p(Kd), _p(nK), oh, ow,
+                                      int(device))
     if rc == -1:
-        raise ValueError("undistort_image: an image or lens l3d_undistort_u8 rejects")
+        raise ValueError("undistort_image: an image, lens, new K or size l3d_undistort_u8 rejects")
     if rc != 0:
         raise capi.L3DError("undistort_image: no usable CUDA device or a CUDA failure")
     return out
+
+
+def optimal_new_camera_matrix(K, lens, image_size, alpha, new_size=None, center_principal_point=False):
+    """Line3D::getOptimalNewCameraMatrix, i.e. cv2.getOptimalNewCameraMatrix(K, D, image_size, alpha, new_size, centerPrincipalPoint)
+    for a radtan lens dict: (new K 3x3, valid-pixel ROI (x, y, width, height)).  Sizes are (width, height); host only"""
+    newK, roi = np.zeros(9), np.zeros(4, np.int32)
+    nw, nh = (0, 0) if new_size is None else (int(new_size[0]), int(new_size[1]))
+    rc = capi.lib().l3dpp_optimal_new_camera_matrix(_p(np.ascontiguousarray(K, np.float64).reshape(9)), _p(_lens9(lens)), int(image_size[0]),
+                                                    int(image_size[1]), float(alpha), nw, nh, int(bool(center_principal_point)), _p(newK), _p(roi))
+    if rc != 0:
+        raise ValueError("optimal_new_camera_matrix: a fisheye lens, a size below 1 or a bad camera matrix")
+    return newK.reshape(3, 3), tuple(int(v) for v in roi)
+
+
+def fisheye_new_camera_matrix(K, lens, image_size, balance=0.0, new_size=None, fov_scale=1.0):
+    """Line3D::estimateNewCameraMatrixForUndistortRectify, i.e. cv2.fisheye.estimateNewCameraMatrixForUndistortRectify(K, D,
+    image_size, I, balance=, new_size=, fov_scale=) for a fisheye lens dict: the new K 3x3.  Sizes are (width, height); host only"""
+    newK = np.zeros(9)
+    nw, nh = (0, 0) if new_size is None else (int(new_size[0]), int(new_size[1]))
+    rc = capi.lib().l3dpp_fisheye_new_camera_matrix(_p(np.ascontiguousarray(K, np.float64).reshape(9)), _p(_lens9(lens)), int(image_size[0]),
+                                                    int(image_size[1]), float(balance), nw, nh, float(fov_scale), _p(newK))
+    if rc != 0:
+        raise ValueError("fisheye_new_camera_matrix: a radtan lens, a size below 1 or a bad camera matrix")
+    return newK.reshape(3, 3)
 
 
 def read_mavmap(path):
