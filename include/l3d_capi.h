@@ -13,7 +13,7 @@
  * 0 on success or a negative l3d_status; l3d_last_error() gives the message (the reference prints CUDA errors to
  * cerr and carries on, dataArray.h:198-237).  A call that fails leaves its stage (views, matches, score sweep,
  * collinear lists, affinity matrix), and every stage computed from it, without a result: later calls that need one
- * return L3D_ERR_STATE.  The image calls (l3d_undistort_u8, l3d_undistort_map, l3d_remap_u8, l3d_prepare_gray_u8) and the tie-point calls
+ * return L3D_ERR_STATE.  The image calls (l3d_undistort_u8, l3d_undistort_map, l3d_remap_u8, l3d_prepare_gray_u8, l3d_decode_jpeg_gray_u8) and the tie-point calls
  * (l3d_triangulate_points, l3d_median_depths) are not part of that chain: whether
  * they succeed or fail, every stage and its result stay as they were.  A context is single-owner (not thread-safe), one per GPU, and runs
  * on its own non-default stream.  There is NO CPU fallback: without a usable CUDA device l3d_ctx_create fails.
@@ -341,7 +341,35 @@ int l3d_image_prep_size(int width, int height, int max_img_width, int32_t* out_w
 /* prepare n images in one launch; sizes, channel counts and max_img_width may all differ */
 int l3d_prepare_gray_u8(l3d_ctx* ctx, int n, const l3d_image_prep_desc* descs, int on_device);
 
-/* ---- tie-point triangulation: linearHomTriangulation of the reference's Pix4D frontend (main_pix4d.cpp:34-70, 354-372) for every point
+/* ---- JPEG decoding: the first step of every frontend's image loop (main_vsfm.cpp:267-306 and its five siblings), cv::imread(path,
+ * IMREAD_GRAYSCALE), byte for byte as OpenCV 4.13 returns it on x86: the Y component of a baseline or extended-sequential Huffman JPEG
+ * (no colour conversion, no upsampling), libjpeg-turbo's accurate integer IDCT as its SIMD code computes it, then OpenCV's EXIF
+ * orientation (1..8; any other value, a missing or a broken EXIF block: none).  DESIGN.md §4c.
+ * Supported: SOF0 / SOF1 with 8-bit samples, 8- or 16-bit DQT, one component or three (YCbCr) with Y at the largest sampling factors,
+ * interleaved and non-interleaved scans, restart intervals, APPn / COM / fill bytes.  Rejected with a message that names the reason:
+ * progressive, lossless, hierarchical and arithmetic-coded files, 12-bit samples, DNL, 2 or 4 components, RGB (Adobe transform 0, or
+ * component ids 'R' 'G' 'B' without JFIF), Y below the largest sampling factors, a side outside [1, 32767], a missing table, EOI or
+ * component scan, and corrupt or truncated data (no attempt is made at libjpeg's recovery).
+ * Not part of the pipeline chain: every stage and its result stay as they were. */
+/* size of imread(IMREAD_GRAYSCALE)'s output (after EXIF orientation); needs no context and no GPU.  L3D_OK, or L3D_ERR_INVALID for a
+ * file outside the subset above (readJPEGSize of include/line3d_io.h gives the reason) or a null pointer */
+int l3d_jpeg_info(const uint8_t* data, int64_t size, int32_t* out_width, int32_t* out_height);
+typedef struct {
+    const uint8_t* data; int64_t size;   /* the file's bytes, always HOST memory (the headers are parsed on the host) */
+    uint8_t* dst; int64_t dst_pitch;     /* out_height rows of out_width grey bytes */
+    int32_t out_width, out_height;       /* from l3d_jpeg_info */
+} l3d_jpeg_desc;
+/* decode n files in two launches (Huffman decoding: one thread per entropy-coded segment; IDCT and store: one thread per 8x8 block);
+ * sizes, sampling, restart intervals and orientations may all differ.  on_device != 0: dst (only) is a device address on this GPU;
+ * on_device == 0: dst is host memory, staged through the context's own device buffers.  Either way only the coded bytes of Y's scan
+ * are uploaded, and the call returns when its result is known: bytes of dst beyond each row's out_width stay untouched.
+ * A descriptor with no data, a file outside the subset, a null dst, an out size other than l3d_jpeg_info's or a dst_pitch below
+ * out_width is rejected (L3D_ERR_INVALID, l3d_last_error naming the first bad index and the reason) before anything is launched.
+ * Corrupt entropy-coded data (no Huffman code matches, AC coefficients past index 63, a segment that ends early) is found on the GPU:
+ * L3D_ERR_INVALID naming the first such image; host dst buffers are then untouched, device ones hold undefined bytes. */
+int l3d_decode_jpeg_gray_u8(l3d_ctx* ctx, int n, const l3d_jpeg_desc* descs, int on_device);
+
+/* ---- tie-point triangulation:linearHomTriangulation of the reference's Pix4D frontend (main_pix4d.cpp:34-70, 354-372) for every point
  * in one launch.  Point i has the observations [obs_ptr[i], obs_ptr[i+1]) (obs_ptr[0] = 0): camera obs_cam[o] in [0, n_cams) and image
  * point (obs_xy[2o], obs_xy[2o+1]); P: the 3x4 projection matrix of every camera, 12 doubles row-major.  A point with fewer than three
  * observations is invalid with X = 0, as the reference skips it.  Otherwise A^T A (4x4, double) is accumulated from the rows Sx P[cam]

@@ -103,6 +103,15 @@ int l3dpp_optimal_new_camera_matrix(const double* K, const double* lens9, int wi
 int l3dpp_fisheye_new_camera_matrix(const double* K, const double* lens9, int width, int height, double balance, int new_width, int new_height,
                                     double fov_scale, double* newK);
 
+/* ---- JPEG files (csrc/line3d_jpeg.cc) */
+/* readJPEGSize: imread(IMREAD_GRAYSCALE)'s size; 0, or -1 with the reason in err.  No GPU */
+int l3dpp_jpeg_size(const char* path, int* width, int* height, char* err, int errcap);
+/* readJPEGsGray of n files on CUDA device cuda_device: a handle for l3dpp_jpegs_image (never NULL; failures are per file) */
+void* l3dpp_jpegs_read(const char* const* paths, int n, int cuda_device);
+void l3dpp_jpegs_close(void* h);
+/* file i of the batch: its size, and its packed grey pixels into out[cap] when cap >= width * height; -1 with the file's error in err */
+int l3dpp_jpegs_image(void* h, int i, int* width, int* height, unsigned char* out, long long cap, char* err, int errcap);
+
 /* ---- .nvm models (csrc/line3d_sfm.cc) */
 void* l3dpp_nvm_open(const char* path, char* err, int errcap);
 void l3dpp_nvm_close(void* h);

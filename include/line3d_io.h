@@ -85,6 +85,16 @@ bool readOpenMVG(const std::string& sfm_data_json, std::vector<SfMCamera>& camer
 bool readPix4D(const std::string& params_folder, const std::string& project_prefix, std::vector<SfMCamera>& cameras, std::string* error = 0,
                int cuda_device = 0);
 
+/* The first step of the frontends' image loop, cv::imread(path, IMREAD_GRAYSCALE) (main_vsfm.cpp:267-306), for JPEG files: OpenCV 4.13's
+ * grey bytes, decoded on the GPU (l3d_decode_jpeg_gray_u8 of include/l3d_capi.h; the subset and the rejections are listed there).
+ * readJPEGSize reads the headers only (no GPU): the size after EXIF orientation.  readJPEGGray decodes one file into a 1-channel
+ * image on device cuda_device.  readJPEGsGray decodes every readable file of the list in one batch; a file that cannot be read,
+ * parsed or decoded leaves its image empty and its own message in (*errors)[i] (empty for the others), and makes the function return
+ * false.  All three return false with *error set on failure; a context lives for the call, as in readPix4D. */
+bool readJPEGSize(const std::string& path, int& width, int& height, std::string* error = 0);
+bool readJPEGGray(const std::string& path, Image8u& image, std::string* error = 0, int cuda_device = 0);
+bool readJPEGsGray(const std::vector<std::string>& paths, std::vector<Image8u>& images, std::vector<std::string>* errors = 0, int cuda_device = 0);
+
 /* K of main_vsfm.cpp:266-278: focal on the diagonal, principal point at the image centre (float arithmetic like the reference) */
 Matrix3d intrinsicsFromFocal(float focal, int image_width, int image_height);
 

@@ -111,6 +111,34 @@ def make_image_prep_desc(width, height, channels, max_img_width, src=0, src_pitc
     return d
 
 
+class JpegDesc(C.Structure):
+    """l3d_jpeg_desc: one JPEG file (host bytes) and its grey output"""
+    _fields_ = [("data", C.c_void_p), ("size", C.c_int64), ("dst", C.c_void_p), ("dst_pitch", C.c_int64), ("out_width", C.c_int32),
+                ("out_height", C.c_int32)]
+
+
+def jpeg_info(data):
+    """(width, height) of imread(IMREAD_GRAYSCALE)'s output for a JPEG file's bytes (l3d_jpeg_info; after EXIF orientation).  Raises
+    L3DError for a file outside the supported subset (line3d.jpeg_size names the reason)."""
+    b = bytes(data)
+    w, h = C.c_int32(), C.c_int32()
+    rc = lib().l3d_jpeg_info(b, len(b), C.byref(w), C.byref(h))
+    if rc < 0:
+        raise L3DError(f"l3d_jpeg_info failed ({rc}): not a JPEG file l3d_decode_jpeg_gray_u8 reads")
+    return w.value, h.value
+
+
+def _device_rows(o):
+    """(address, row pitch in bytes, (rows, cols)) of a 2-D uint8 array in GPU memory that exposes __cuda_array_interface__"""
+    ai = o.__cuda_array_interface__
+    if ai["typestr"] != "|u1" or len(ai["shape"]) != 2:
+        raise ValueError("device output must be a 2-D uint8 array")
+    strides = ai.get("strides") or (ai["shape"][1], 1)
+    if strides[1] != 1:
+        raise ValueError("device output rows must be packed")
+    return int(ai["data"][0]), int(strides[0]), tuple(ai["shape"])
+
+
 def _image_rows(a):
     """(array, row pitch in bytes) of a uint8 HxW / HxWx3 image whose pixels are packed within each row; other layouts are copied"""
     a = np.asarray(a)
@@ -492,6 +520,40 @@ class Context:
             outs.append(o)
         self._chk(self.L.l3d_prepare_gray_u8(self.h, n, descs, 0), "l3d_prepare_gray_u8")
         return outs
+
+    # ---- JPEG decoding (stateless: no pipeline stage changes)
+    def decode_jpeg_gray(self, files, out=None):
+        """l3d_decode_jpeg_gray_u8: imread(IMREAD_GRAYSCALE) of a list of JPEG files (bytes) in ONE batched call.  out=None: returns
+        new uint8 [h, w] host arrays.  out: one output per file, all host numpy arrays or all GPU arrays exposing
+        __cuda_array_interface__ (e.g. torch CUDA tensors) of shape [h, w] with packed rows and any row pitch; GPU outputs are written
+        in place (on_device=1), ready for undistort_device / prepare_gray_device.  Returns the outputs."""
+        n = len(files)
+        data = [bytes(f) for f in files]
+        sizes = [jpeg_info(d) for d in data]
+        device = out is not None and n > 0 and hasattr(out[0], "__cuda_array_interface__")
+        outs = [np.empty((h, w), np.uint8) for w, h in sizes] if out is None else list(out)
+        if len(outs) != n:
+            raise ValueError("out needs one array per file")
+        descs = (JpegDesc * n)()
+        for i, (d, (w, h)) in enumerate(zip(data, sizes)):
+            if device:
+                addr, pitch, shape = _device_rows(outs[i])
+            else:
+                o = outs[i]
+                if not isinstance(o, np.ndarray) or o.dtype != np.uint8 or o.ndim != 2 or o.strides[1] != 1:
+                    raise ValueError("host output must be a uint8 [h, w] array with packed rows")
+                addr, pitch, shape = o.ctypes.data, o.strides[0], o.shape
+            if shape != (h, w):
+                raise ValueError(f"output {i} has shape {shape}, the file decodes to {(h, w)}")
+            descs[i].data = C.cast(C.c_char_p(d), C.c_void_p).value
+            descs[i].size, descs[i].dst, descs[i].dst_pitch = len(d), addr, pitch
+            descs[i].out_width, descs[i].out_height = w, h
+        self._chk(self.L.l3d_decode_jpeg_gray_u8(self.h, n, descs, int(device)), "l3d_decode_jpeg_gray_u8")
+        return outs
+
+    def decode_jpeg_gray_descs(self, descs, on_device):
+        """l3d_decode_jpeg_gray_u8 on a ctypes array of JpegDesc as given (for tests of the checks)"""
+        self._chk(self.L.l3d_decode_jpeg_gray_u8(self.h, len(descs), descs, int(on_device)), "l3d_decode_jpeg_gray_u8")
 
     def prepare_gray_device(self, descs):
         """l3d_prepare_gray_u8 on device addresses (a ctypes array of ImagePrepDesc); asynchronous on the context's stream"""

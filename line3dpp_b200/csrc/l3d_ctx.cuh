@@ -3,6 +3,7 @@
 #include "l3d_match.cuh"
 
 #include <algorithm>
+#include <cstddef>
 #include <memory>
 #include <string>
 #include <utility>
@@ -98,6 +99,42 @@ struct ImagePrepState {
     DevBuf d_imgs, d_src, d_dst;                         // d_src, d_dst: host-mode staging
 };
 
+// a Huffman table as k_jpeg_entropy reads it (l3d_jpeg.cu): a 9-bit lookahead (length << 8 | symbol, 0 for a longer code), then
+// libjpeg's canonical decode for lengths 10..16: a code c of length l is valid when c <= maxcode[l], its symbol vals[c + valoff[l]]
+struct L3DJpegTable {
+    unsigned short look[512];
+    int maxcode[18], valoff[18];
+    unsigned char vals[256];
+};
+
+// per-image parameters of the JPEG kernels (l3d_jpeg.cu)
+struct L3DJpegImage {
+    unsigned char* dst;
+    long long dst_pitch, coef0, tile0;       // coef0: Y's first block in the coefficient buffer; tile0: first IDCT block in the batch grid
+    int width, height, blocks_x;             // the coded frame; blocks_x: 8x8 blocks per row holding image pixels (ceil(width / 8))
+    int yblocks_x;                           // Y's coded grid (MCU-padded in an interleaved scan)
+    int ns, y_in_scan, mcus_x;               // Y's scan: components, Y's position, MCUs per row
+    int bh[4], bv[4];                        // blocks of scan component k per MCU
+    int ryy, ryx, ry0, rxy, rxx, rx0;        // EXIF orientation: the pixel (y, x) goes to row ryy*y + ryx*x + ry0, column rxy*y + rxx*x + rx0
+    alignas(16) unsigned short q[64];        // Y's quantisation table, natural order (k_jpeg_idct reads it as uint4)
+};
+static_assert(offsetof(L3DJpegImage, q) % 16 == 0 && sizeof(L3DJpegImage) % 16 == 0, "L3DJpegImage::q is read as uint4");
+
+// one entropy-coded segment: bytes [first, end) of the staged data, MCUs [mcu0, mcu1) of image `image`
+struct L3DJpegSeg {
+    long long first, end;
+    int image, mcu0, mcu1, pad;
+};
+
+// buffers of the JPEG decode: not a pipeline stage, nothing else reads them
+struct JpegState {
+    std::vector<L3DJpegImage> h_imgs;
+    std::vector<L3DJpegSeg> h_segs;
+    std::vector<L3DJpegTable> h_tabs;                    // 8 per image: DC, AC of each component of Y's scan
+    std::vector<int> h_status;
+    DevBuf d_imgs, d_segs, d_tabs, d_bytes, d_coefs, d_status, d_dst;   // d_dst: host-mode staging
+};
+
 // buffers of the triangulation and median-depth calls (l3d_triangulate.cu): not a pipeline stage either; the d_* of host mode
 // stage the caller's arrays
 struct TriangulateState {
@@ -145,6 +182,7 @@ struct l3d_ctx {
     OptState opt;
     UndistortState undist;
     ImagePrepState prep;
+    JpegState jpeg;
     TriangulateState tri;
 
     const float4* segs() const { return segs_ext ? segs_ext : (const float4*)d_segs.p; }

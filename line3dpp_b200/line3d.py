@@ -431,6 +431,47 @@ def fisheye_new_camera_matrix(K, lens, image_size, balance=0.0, new_size=None, f
     return newK.reshape(3, 3)
 
 
+def jpeg_size(path):
+    """readJPEGSize: (width, height) of imread(path, IMREAD_GRAYSCALE)'s output, after EXIF orientation; headers only, no GPU.  Raises
+    L3DError naming the reason for a file that cannot be read or is outside the supported subset."""
+    w, h = C.c_int(), C.c_int()
+    err = C.create_string_buffer(4096)
+    if capi.lib().l3dpp_jpeg_size(str(path).encode(), C.byref(w), C.byref(h), err, 4096) != 0:
+        raise capi.L3DError(err.value.decode(errors="replace"))
+    return w.value, h.value
+
+
+def read_jpeg_gray(path_or_paths, device=0, errors=None):
+    """readJPEGGray / readJPEGsGray: imread(path, IMREAD_GRAYSCALE) as uint8 [h, w], decoded on GPU `device`; a list of paths is one
+    batched decode and gives a list.  A file that fails raises L3DError with its message, unless a list `errors` is given: then every
+    failed file's entry is None, and errors receives one message per file ("" for the decoded ones)."""
+    single = isinstance(path_or_paths, (str, bytes)) or hasattr(path_or_paths, "__fspath__")
+    paths = [path_or_paths] if single else list(path_or_paths)
+    L = capi.lib()
+    arr = (C.c_char_p * len(paths))(*[str(p).encode() for p in paths])
+    h = L.l3dpp_jpegs_read(arr, len(paths), int(device))
+    outs, msgs = [], []
+    try:
+        for i in range(len(paths)):
+            w, ht = C.c_int(), C.c_int()
+            err = C.create_string_buffer(4096)
+            if L.l3dpp_jpegs_image(h, i, C.byref(w), C.byref(ht), None, 0, err, 4096) != 0:
+                outs.append(None)
+                msgs.append(err.value.decode(errors="replace"))
+                continue
+            o = np.empty((ht.value, w.value), np.uint8)
+            L.l3dpp_jpegs_image(h, i, C.byref(w), C.byref(ht), _p(o), o.size, err, 4096)
+            outs.append(o)
+            msgs.append("")
+    finally:
+        L.l3dpp_jpegs_close(h)
+    if errors is not None:
+        errors[:] = msgs
+    elif any(msgs):
+        raise capi.L3DError("; ".join(m for m in msgs if m))
+    return outs[0] if single else outs
+
+
 def read_mavmap(path):
     """readMavmap: the cameras of a mavmap result file (no world points; see sequential_neighbors).  Raises L3DError on malformed input."""
     return _read_sfm(SFM_MAVMAP, path)
