@@ -124,6 +124,13 @@ int l3d_match_stride(const l3d_ctx* ctx);
 int l3d_match_semantics(const l3d_ctx* ctx);
 /* device addresses of the last match result: counts int32[total_rows], recs l3d_match_rec[total_rows*knn] (fixed slots) */
 int l3d_match_device_buffers(l3d_ctx* ctx, void** counts_dev, void** recs_dev);
+/* what the window scan of the matching kernel starts from for pair `pair`, one of the pairs the context's own last match call evaluated
+ * (DESIGN.md section 2): windows_out[Ns * 20], per source row the pencil parameters k1, k2 of its two epipolar lines, 1 if the row
+ * skips level 1, 0, then for every arc class c < 8 the first entry of the pair's sorted table inside class c whose arc start is not below
+ * ka - 2^(21 + c) and the first whose start is above kb (pair-relative, over the whole class); basis_out[6] the pencil basis u, v;
+ * class_off_out[10] the first sorted entry of every class and the end; arc_starts_out[Nt] the arc start of every sorted entry.  NULL
+ * skips an output; a pair whose target view has no segments writes none. */
+int l3d_match_row_windows(l3d_ctx* ctx, int pair, uint32_t* windows_out, double* basis_out, int32_t* class_off_out, uint32_t* arc_starts_out);
 /* row_off_out[num_pairs+1]: first row of every pair in those buffers (prefix sum of Ns), last = total_rows */
 int l3d_pair_row_offsets(l3d_ctx* ctx, long long* row_off_out);
 /* pure host helper: contiguous split of n items with the given costs into `parts` ranges of near-equal cost;

@@ -347,6 +347,14 @@ class Context:
         self._knn = int(self._chk(self.L.l3d_match_restride(self.h, int(stride)), "l3d_match_restride"))
         return self._knn
 
+    def row_windows(self, pair, ns, nt):
+        """l3d_match_row_windows: (windows uint32[ns, 20], basis float64[2, 3] (u, v), class offsets int32[10], arc starts uint32[nt])
+        of a pair the last match call evaluated here (ns / nt: the sizes of its source and target views)"""
+        win, basis = np.zeros((ns, 20), np.uint32), np.zeros((2, 3), np.float64)
+        off, starts = np.zeros(10, np.int32), np.zeros(nt, np.uint32)
+        self._chk(self.L.l3d_match_row_windows(self.h, int(pair), _p(win), _p(basis), _p(off), _p(starts)), "l3d_match_row_windows")
+        return win, basis, off, starts
+
     def pair_row_offsets(self, num_pairs):
         out = np.zeros(num_pairs + 1, np.int64)
         self._chk(self.L.l3d_pair_row_offsets(self.h, _p(out)), "l3d_pair_row_offsets")

@@ -259,6 +259,7 @@ static float4* level1_segs(l3d_ctx* c, long long narcs) { return (float4*)((uint
 // segments in window order.  Below epi_overlap 0.01 the extended arcs would span the whole line: everything is then handed to the float filter.
 static int build_level1(l3d_ctx* c, int first_pair, int last_pair, long long narcs, float epi_overlap)
 {
+    c->level1_first = c->level1_last = 0;
     if (last_pair <= first_pair || narcs <= 0) return L3D_OK;
     if (narcs >= (1ll << 31) - 2) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: more than 2^31 (pair, target segment) combinations in one call");
     const int npr = last_pair - first_pair;
@@ -280,6 +281,19 @@ static int build_level1(l3d_ctx* c, int first_pair, int last_pair, long long nar
                                                                              first_pair, (uint4*)c->d_arcs.p, level1_segs(c, narcs));
     L3D_CUDA(c, cudaGetLastError(), "k_arcs_gather");
     c->launches += 2 + 8;
+    // the row windows of every work unit, read by each k_match_topk launch of the call (all chunks of l3d_match_pairs_host)
+    const long long row0 = c->h_pairs[first_pair].row_off, row1 = last_pair < c->num_pairs ? c->h_pairs[last_pair].row_off : c->total_rows;
+    int stage = 0;
+    for (int i = first_pair; i < last_pair; ++i) stage = std::max(stage, std::min(c->h_views[c->h_pairs[i].tgt].nseg, L3D_RW_STAGE));
+    L3D_RESERVE(c->d_rowwin, 4 * L3D_RW_WORDS * (size_t)std::max<long long>(row1 - row0, 1), "row windows");
+    if (!c->h_units.empty()) {
+        k_row_windows<<<(unsigned int)c->h_units.size(), 256, sizeof(unsigned int) * (size_t)stage, c->stream>>>(
+            c->segs(), c->views(), (const L3DPairDev*)c->d_pairs.p, (const int4*)c->d_units.p, (const L3DPairBasis*)c->d_basis.p,
+            (const uint4*)c->d_arcs.p, row0, (uint4*)c->d_rowwin.p);
+        ++c->launches;
+        L3D_CUDA(c, cudaGetLastError(), "k_row_windows");
+    }
+    c->level1_first = first_pair; c->level1_last = last_pair;
     return L3D_OK;
 }
 
@@ -424,7 +438,8 @@ static int match_impl(l3d_ctx* c, int num_pairs, const int32_t* pairs, const flo
     if (Fd && (rc = build_cache_d(c))) return rc;
     c->semantics = Fd ? L3D_SEM_REF_CPU : L3D_SEM_REF_GPU;
     const MatchArgs a = {c->segs(), (const float4*)c->d_cache.p, Fd ? (const double*)c->d_cache_d.p : nullptr, c->views(), (const L3DPairDev*)c->d_pairs.p,
-                         (const int4*)c->d_units.p, (const uint4*)c->d_arcs.p, level1_segs(c, narcs), (const L3DPairBasis*)c->d_basis.p, (int*)c->d_counts.p,
+                         (const int4*)c->d_units.p, (const uint4*)c->d_arcs.p, level1_segs(c, narcs), (const L3DPairBasis*)c->d_basis.p,
+                         (const uint4*)c->d_rowwin.p, first_pair < num_pairs ? c->h_pairs[first_pair].row_off : 0, (int*)c->d_counts.p,
                          (l3d_match_rec*)c->d_recs.p, knn, epi_overlap};
     if ((rc = knn > 0 && knn <= 32 ? run_topk(c, a, host) : run_keep_all(c, a, knn > 32 ? knn : 0))) return rc;
     c->have_matches = true;
@@ -450,6 +465,29 @@ int l3d_match_device_buffers(l3d_ctx* c, void** counts_dev, void** recs_dev)
     if (!c->have_matches) return l3d_fail(c, L3D_ERR_STATE, "l3d_match_device_buffers: no match result");
     *counts_dev = c->d_counts.p; *recs_dev = c->d_recs.p;
     c->drop(Stage::Sweep);                  // the caller may overwrite rows
+    return L3D_OK;
+}
+
+int l3d_match_row_windows(l3d_ctx* c, int pair, uint32_t* windows_out, double* basis_out, int32_t* class_off_out, uint32_t* arc_starts_out)
+{
+    if (!c) return L3D_ERR_INVALID;
+    if (!c->have_matches) return l3d_fail(c, L3D_ERR_STATE, "l3d_match_row_windows: no match result");
+    if (pair < c->level1_first || pair >= c->level1_last) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_row_windows: pair not evaluated by the last match call");
+    cudaSetDevice(c->device);
+    const L3DPairDev& p = c->h_pairs[pair];
+    const int Ns = c->h_views[p.src].nseg, Nt = c->h_views[p.tgt].nseg;
+    if (Nt == 0) return L3D_OK;             // no level-1 table and no windows: the pair has no candidates
+    L3DPairBasis B;
+    L3D_CUDA(c, cudaMemcpyAsync(&B, (const L3DPairBasis*)c->d_basis.p + pair, sizeof(B), cudaMemcpyDeviceToHost, c->stream), "download pair basis");
+    if (windows_out && Ns)
+        L3D_CUDA(c, cudaMemcpyAsync(windows_out, (const uint32_t*)c->d_rowwin.p + (p.row_off - c->h_pairs[c->level1_first].row_off) * L3D_RW_WORDS,
+                                    4 * L3D_RW_WORDS * (size_t)Ns, cudaMemcpyDeviceToHost, c->stream), "download row windows");
+    if (arc_starts_out)     // x of every packed entry (uint4) of the pair's sorted table
+        L3D_CUDA(c, cudaMemcpy2DAsync(arc_starts_out, 4, (const uint4*)c->d_arcs.p + p.arc_off, sizeof(uint4), 4, (size_t)Nt, cudaMemcpyDeviceToHost, c->stream),
+                 "download arc starts");
+    L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync");
+    if (basis_out) for (int i = 0; i < 3; ++i) { basis_out[i] = B.u[i]; basis_out[3 + i] = B.v[i]; }
+    if (class_off_out) for (int i = 0; i < L3D_ARC_NCLS + 2; ++i) class_off_out[i] = B.cls_off[i];
     return L3D_OK;
 }
 

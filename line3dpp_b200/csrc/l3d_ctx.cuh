@@ -174,6 +174,8 @@ struct l3d_ctx {
     std::vector<L3DPairDev> h_pairs;
     std::vector<int4> h_units;              // k_match_topk work units: (pair, first source row, rows, 0)
     DevBuf d_pairs, d_units, d_counts, d_recs, d_rowptr, d_csr, d_dense_dep, d_dense_ov, d_dense_jobs, d_arcs, d_basis, d_arcraw, d_arckeys, d_arckeys2, d_arcvals, d_arcvals2;
+    DevBuf d_rowwin;                        // row windows of the rows of [level1_first, level1_last) (k_row_windows, L3D_RW_WORDS words per row)
+    int level1_first = 0, level1_last = 0;  // the pairs whose level-1 tables, bases and row windows the context holds (its own last match call)
 
     SweepState sweep;
     RddState rdd;

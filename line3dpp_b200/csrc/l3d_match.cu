@@ -6,13 +6,16 @@
 //   k_pair_arcs,    : level-1 tables of the view pairs of one call (l3d_device.cuh "pencil parameter"): every target segment as an arc of
 //   k_arcs_gather     the epipolar pencil, grouped by arc length and sorted by arc start (one radix sort in between, l3d_capi.cu); the
 //                     table carries each arc's target segment in a parallel array (32 B per pair and target).
+//   k_row_windows   : per source row of every work unit, before k_match_topk: the pencil parameters of its epipolar lines (FP64) and
+//                     the two ends of its window in every arc class (binary searches of the sorted table), 80 B per row, so that
+//                     k_match_topk's row set-up is one load instead of a dependent FP64 chain and 16 searches on 16 of 32 lanes.
 //   k_match_topk    : production kernel.  One CTA per SM (32 warps) = one work unit: a view pair and up to 1024 of its source rows.
 //                     The pair's table (arcs + segments) is staged in shared memory by 1-D TMA (cp.async.bulk + mbarrier, 6 stages x
 //                     512 entries x 32 B in flight from the first instruction): a target view of up to 3072 segments is resident in one
 //                     pass, and a warp takes the unit's rows one at a time from a shared counter into one of its 8 row slots (constants,
 //                     key list, score-to-beat), with no CTA barrier; larger target views take several passes over units of at most 256
-//                     rows, each slot bound to one row.  Per row the warp binary-searches the
-//                     window of every arc class and scans only those entries, all windows as one concatenation (full warps), the
+//                     rows, each slot bound to one row.  Per row the warp clips the window of every arc class (k_row_windows) to the
+//                     resident entries and scans only those entries, all windows as one concatenation (full warps), the
 //                     class nearest the row's own span first so that its score-to-beat rises early: each
 //                     lane runs the arc test (13 integer instructions) and the conservative float filter (27 flop + 2 rcp on the
 //                     staged target segment) on its entry, branch-free, the survivors of both are ballot-compacted into a per-warp
@@ -73,7 +76,7 @@ struct MatchSmem {
     unsigned long long lists[MK_NSLOT][MK_CAP + 1];  // per-slot survivor keys (+1: slots start on different banks, lanes that push keys of different rows do not collide)
     float4 rowA[MK_NSLOT];                           // (e1.x, e1.y, e1.z, e2.x)
     float4 rowB[MK_NSLOT];                           // (e2.y, e2.z, g, 0.95 * score-to-beat)
-    uint2 rowK[MK_NSLOT];                            // pencil parameters of the row's two epipolar lines (l3d_device.cuh)
+    uint2 rowK[MK_NSLOT];                            // pencil parameters of the row's two epipolar lines (l3d_device.cuh, k_row_windows)
     float row_thr[MK_NSLOT];                         // overlap of the current k-th best survivor (0 until k are known)
     int list_cnt[MK_NSLOT];
     int slot_row[MK_NSLOT];                          // row of the unit (0 .. rows - 1) the slot holds; -1: never used
@@ -89,6 +92,7 @@ struct MatchSmem {
     // per-CTA constants of the (rarely executed, deliberately out-of-line) exact path
     const float4* cache; const float4* ssegs;        // float ray cache; the unit's first source segment
     const uint4* tarcs; const float4* tasegs;        // the pair's level-1 table (TMA sources of the refills)
+    const unsigned int* wins;                        // row windows of the unit's rows (k_row_windows), L3D_RW_WORDS words per row
     long long src_base, toff;
     float3 Cs, Ct;
     float epi; int knn;
@@ -407,6 +411,63 @@ k_arcs_gather(long long n, const unsigned long long* __restrict__ keys, const un
     out_segs[i] = segs[views[P->tgt].seg_off + j];
 }
 
+// One CTA per work unit of k_match_topk: the row windows of its rows (l3d_match.cuh), one row per thread.  This is the arithmetic
+// k_match_topk's row set-up needs before a row's scan, the same operations on the same values: the float epipolar lines F*p
+// (mulmat_h), their pencil parameters (line_kappa, double) and per arc class the lower bounds of the two window keys in the sorted
+// table (a row outside the pencil model, rall, needs none: the class start).  The arc starts of classes 0 .. NCLS - 1 are staged in
+// shared memory when there are at most L3D_RW_STAGE of them (the launch sizes the dynamic shared memory), searched in the table otherwise.
+__global__ void __launch_bounds__(256)
+k_row_windows(const float4* __restrict__ segs, const L3DViewDev* __restrict__ views, const L3DPairDev* __restrict__ pairs,
+              const int4* __restrict__ units, const L3DPairBasis* __restrict__ basis, const uint4* __restrict__ arcs, long long win_row0,
+              uint4* __restrict__ wins)
+{
+    extern __shared__ unsigned int rw_starts[];
+    __shared__ L3DPairBasis B;
+    __shared__ float F[9];
+    const int4 unit = units[blockIdx.x];
+    const L3DPairDev* P = pairs + unit.x;
+    constexpr int NB = (int)(sizeof(L3DPairBasis) / sizeof(int));
+    static_assert(L3D_RW_WORDS == 4 + 2 * L3D_ARC_NCLS && NB + 9 <= 256, "row window layout; one word of the pair per thread");
+    if (threadIdx.x < NB) reinterpret_cast<int*>(&B)[threadIdx.x] = reinterpret_cast<const int*>(basis + unit.x)[threadIdx.x];
+    else if (threadIdx.x < NB + 9) F[threadIdx.x - NB] = P->F[threadIdx.x - NB];
+    __syncthreads();
+    const uint4* tab = arcs + P->arc_off;
+    const bool staged = B.cls_off[L3D_ARC_NCLS] <= L3D_RW_STAGE;
+    if (staged)
+        for (int i = threadIdx.x; i < B.cls_off[L3D_ARC_NCLS]; i += blockDim.x) rw_starts[i] = tab[i].x;
+    __syncthreads();
+    const float4* ssegs = segs + views[P->src].seg_off + unit.y;
+    uint4* out = wins + (P->row_off + unit.y - win_row0) * (L3D_RW_WORDS / 4);
+    for (int r = threadIdx.x; r < unit.z; r += blockDim.x) {
+        const float4 s = ssegs[r];
+        const float3 e1 = mulmat_h(F, s.x, s.y), e2 = mulmat_h(F, s.z, s.w);
+        bool off1, off2;
+        const unsigned int k1 = line_kappa(B, e1, &off1), k2 = line_kappa(B, e2, &off2);
+        const bool rall = off1 || off2;
+        const bool fwd = (k2 - k1) < 0x80000000u;
+        const unsigned int ka = fwd ? k1 : k2, kb = fwd ? k2 : k1;
+        unsigned int pos[2 * L3D_ARC_NCLS];
+#pragma unroll
+        for (int i = 0; i < 2 * L3D_ARC_NCLS; ++i) {
+            const int c = i >> 1;
+            const bool upper = i & 1;
+            int lo = B.cls_off[c], hi = B.cls_off[c + 1];
+            const unsigned int key = upper ? kb + 1u : ka - (1u << (L3D_ARC_CLS0 + c));
+            if (rall) hi = lo;
+            else if (upper && kb == 0xFFFFFFFFu) lo = hi;
+            while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                if ((staged ? rw_starts[mid] : __ldg(&tab[mid].x)) < key) lo = mid + 1; else hi = mid;
+            }
+            pos[i] = (unsigned int)lo;
+        }
+        uint4* o = out + (size_t)r * (L3D_RW_WORDS / 4);
+        o[0] = make_uint4(k1, k2, rall ? 1u : 0u, 0u);
+#pragma unroll
+        for (int i = 0; i < L3D_ARC_NCLS / 2; ++i) o[1 + i] = make_uint4(pos[4 * i], pos[4 * i + 1], pos[4 * i + 2], pos[4 * i + 3]);
+    }
+}
+
 // thread 0: start the TMA copies of the level-1 entries of pass `pass` of a pair into the ring; the arcs and the segments of a stage
 // complete on the stage's barrier together
 __device__ __forceinline__ void stage_entries(MatchSmem& S, int pass)
@@ -443,27 +504,28 @@ __device__ __forceinline__ int flat_entry(int G, int lane, int np, int pE, int p
     return min(G + lane, tot - 1) + __shfl_sync(0xffffffffu, pshift, r);
 }
 
-// the constants of the unit's row rl into slot sl, and an empty key list: the epipolar lines F*p (cudawrapper.cu:216-217), the float
-// filter's scale, the lines' pencil parameters (lanes 0 and 1, one line each) and whether the row skips level 1
-__device__ __forceinline__ void setup_row(MatchSmem& S, int sl, int rl, int lane)
+// the row windows of the unit's row rl (k_row_windows), one word per lane: the pencil parameters, the level-1 flag and the window
+// positions of every arc class
+__device__ __forceinline__ unsigned int row_window(const MatchSmem& S, int rl, int lane)
+{ return lane < L3D_RW_WORDS ? __ldg(S.wins + (size_t)rl * L3D_RW_WORDS + lane) : 0u; }
+
+// the constants of the unit's row rl into slot sl, and an empty key list: the epipolar lines F*p (cudawrapper.cu:216-217) and the float
+// filter's scale.  Returns the row's windows (row_window), loaded together with its segment so that the two loads overlap.
+__device__ __forceinline__ unsigned int setup_row(MatchSmem& S, int sl, int rl, int lane)
 {
+    const unsigned int rw = row_window(S, rl, lane);
     const float4 s = __ldg(S.ssegs + rl);
     const float3 e1 = mulmat_h(S.F, s.x, s.y), e2 = mulmat_h(S.F, s.z, s.w);
-    bool off = false;
-    unsigned int k = 0u;
-    if (lane < 2) k = line_kappa(S.B, lane ? e2 : e1, &off);
-    const unsigned int k2 = __shfl_sync(0xffffffffu, k, 1), offs = __ballot_sync(0xffffffffu, off);
     if (lane == 0) {
         const float g = L3D_FILTER_C1 * fmaxf(sqrtf(e1.x * e1.x + e1.y * e1.y), sqrtf(e2.x * e2.x + e2.y * e2.y));
         S.rowA[sl] = make_float4(e1.x, e1.y, e1.z, e2.x);
         S.rowB[sl] = make_float4(e2.y, e2.z, g, 0.95f * S.epi);
-        S.rowK[sl] = make_uint2(k, k2);
-        S.rowall[sl] = offs ? 1 : 0;
         S.list_cnt[sl] = 0;
         S.row_thr[sl] = 0.0f;
         S.slot_row[sl] = rl;
     }
     __syncwarp();
+    return rw;
 }
 
 // evaluate every pending candidate of the warp's queue (qn < 32 of them)
@@ -480,20 +542,20 @@ __device__ __forceinline__ void drain_queue(MatchSmem& S, int warp, int lane, in
     }
 }
 
-// Scan the window entries of the row in slot sl that lie in the ring entries [base, base + cnt) of the pair's level-1 table resident in
-// the current pass, and queue the survivors of both filters; the queue is evaluated 32 at a time.
+// Scan the window entries of the row in slot sl (its row windows rw, row_window) that lie in the ring entries [base, base + cnt) of the
+// pair's level-1 table resident in the current pass, and queue the survivors of both filters; the queue is evaluated 32 at a time.
 template <int SEM, Keep KEEP>
-__device__ __forceinline__ void scan_row(MatchSmem& S, int sl, int warp, int lane, int& qn)
+__device__ __forceinline__ void scan_row(MatchSmem& S, int sl, unsigned int rw, int warp, int lane, int& qn)
 {
     const int base = S.pass * (MK_STAGES * MK_TT), cnt = min(MK_STAGES * MK_TT, S.nt - base);
     MPROBE(const long long t_row = clock64(); long long t_exact = 0;)
     const unsigned int lt_mask = (1u << lane) - 1u;
-    const uint4* ent = &S.stage[0][0];
     const int* cls_off = S.B.cls_off;
     // the row's constants, re-read from shared memory after exact batches instead of held across them (register budget of 32 warps);
     // rB.w: the score-to-beat, which the batches may raise (a stale value only rejects less)
-    uint2 kr = S.rowK[sl];
-    bool rall = S.rowall[sl] != 0;
+    uint2 kr = make_uint2(__shfl_sync(0xffffffffu, rw, 0), __shfl_sync(0xffffffffu, rw, 1));
+    bool rall = __shfl_sync(0xffffffffu, rw, 2) != 0u;
+    if (lane == 0) { S.rowK[sl] = kr; S.rowall[sl] = rall ? 1 : 0; }
     float4 rA = S.rowA[sl];
     float4 rB = S.rowB[sl];
     // short arc [ka, kb] between the two kappa values: a target of class c can only match if its arc starts in [ka - 2^(CLS0 + c), kb]
@@ -512,20 +574,11 @@ __device__ __forceinline__ void scan_row(MatchSmem& S, int sl, int warp, int lan
         c = below ? rc - d : rc + d;
     }
 #endif
-    // lanes 0 .. 2 * NCLS - 1: lower / upper end of the window of class c inside the resident part of that class (binary search)
-    int res = 0;
-    {
-        int lo = min(max(cls_off[c] - base, 0), cnt), hi = min(max(cls_off[c + 1] - base, 0), cnt);
-        const bool upper = lane & 1;
-        const unsigned int key = upper ? kb + 1u : ka - (1u << (L3D_ARC_CLS0 + c));
-        if (lane >= 2 * L3D_ARC_NCLS || rall) hi = lo;                       // no search
-        else if (upper && kb == 0xFFFFFFFFu) lo = hi;
-        while (lo < hi) {
-            const int mid = (lo + hi) >> 1;
-            if (ent[mid].x < key) lo = mid + 1; else hi = mid;
-        }
-        res = lo;
-    }
+    // lanes 0 .. 2 * NCLS - 1: lower / upper end of the window of class c inside the resident part of that class.  The row's window
+    // position over the whole class, clipped to the resident entries [base, base + cnt): a class is sorted, so that is the first resident
+    // entry of the class at or after the key, as a search of the resident part would find it.
+    const int res = min(max((int)__shfl_sync(0xffffffffu, rw, 4 + 2 * c + (lane & 1)) - base, 0), cnt);
+    MPROBE(const long long t_win = clock64(); probe_add(S, warp, lane, MP_WINDOW, t_win - t_row);)
     // lane p < 2 * NCLS: piece p & 1 of the window of class c (two pieces when the window wraps around 2^32); lane 2 * NCLS: the
     // targets every row looks at, last.  A row outside the pencil model (rall) takes everything as one piece.
     int plo = 0, phi = 0;
@@ -550,7 +603,7 @@ __device__ __forceinline__ void scan_row(MatchSmem& S, int sl, int warp, int lan
     ex -= len;
     const int src = lane < np ? (int)__fns(ne, 0u, lane + 1) : 0;
     const int pE = __shfl_sync(0xffffffffu, ex, src), pshift = __shfl_sync(0xffffffffu, plo - ex, src);
-    MPROBE(probe_add(S, warp, lane, MP_SETUP, clock64() - t_row); const long long t_scan = clock64(); probe_add(S, warp, lane, MP_ENTRIES, tot);)
+    MPROBE(probe_add(S, warp, lane, MP_PIECES, clock64() - t_win); const long long t_scan = clock64(); probe_add(S, warp, lane, MP_ENTRIES, tot);)
     for (int G = 0; G < tot; G += 64) {                 // two entries per lane: half the loop / vote / push overhead per entry
         const int ia = flat_entry(G, lane, np, pE, pshift, tot), ib = flat_entry(G + 32, lane, np, pE, pshift, tot);
         const bool pa = entry_may_match(S, ia, kr.x, kr.y, rall, rA, rB) & (G + lane < tot);
@@ -604,6 +657,7 @@ __global__ void __launch_bounds__(MK_THREADS, 1) k_match_topk(const MatchArgs A)
         S.tarcs = A.arcs + __ldg(&P->arc_off); S.tasegs = A.arc_segs + __ldg(&P->arc_off);
         S.Cs = make_float3(__ldg(&vs->C[0]), __ldg(&vs->C[1]), __ldg(&vs->C[2])); S.Ct = make_float3(__ldg(&vt->C[0]), __ldg(&vt->C[1]), __ldg(&vt->C[2]));
         S.R0 = __ldg(&P->row_off) + row0; S.counts_out = A.counts; S.recs_out = A.recs;
+        S.wins = reinterpret_cast<const unsigned int*>(A.wins + (S.R0 - A.win_row0) * (L3D_RW_WORDS / 4));
         if (SEM == L3D_SEM_REF_CPU) {
             S.cache_d = A.cache_d;
             for (int i = 0; i < 9; ++i) S.Fd[i] = __ldg(&P->Fd[i]);
@@ -635,6 +689,7 @@ __global__ void __launch_bounds__(MK_THREADS, 1) k_match_topk(const MatchArgs A)
                 rl = __shfl_sync(0xffffffffu, rl, 0);
             }
             if (rl >= S.nrows) break;
+            unsigned int rw;
             if (S.pass == 0) {
                 if (S.slot_row[sl] >= 0) {             // the slot's previous row: its queued candidates first (rarely any), then its result
                     if (__any_sync(0xffffffffu, lane < qn && (S.queue[warp][lane] >> 24) == (unsigned int)sl)) {
@@ -646,10 +701,10 @@ __global__ void __launch_bounds__(MK_THREADS, 1) k_match_topk(const MatchArgs A)
                     MPROBE(probe_add(S, warp, lane, MP_FINAL, clock64() - t0);)
                 }
                 MPROBE(const long long t0 = clock64();)
-                setup_row(S, sl, rl, lane);
+                rw = setup_row(S, sl, rl, lane);
                 MPROBE(probe_add(S, warp, lane, MP_SETUP, clock64() - t0); probe_add(S, warp, lane, MP_ROWS, 1);)
-            }
-            scan_row<SEM, KEEP>(S, sl, warp, lane, qn);
+            } else rw = row_window(S, rl, lane);
+            scan_row<SEM, KEEP>(S, sl, rw, warp, lane, qn);
             if (++sl == (warp + 1) * MK_SLOTS) {       // the warp's slots hold its rows in turn; several passes: one row per slot
                 if (S.npass > 1) break;
                 sl = warp * MK_SLOTS;

@@ -53,6 +53,7 @@ struct MatchArgs {
     const L3DViewDev* views; const L3DPairDev* pairs; const int4* units;  // units: (pair, first source row, rows, 0) of every CTA
     const uint4* arcs; const float4* arc_segs;                            // level-1 table (k_arcs_gather): packed arcs and their target segments,
     const L3DPairBasis* basis;                                            // both in window order; the pencil bases (k_pair_arcs)
+    const uint4* wins; long long win_row0;                                // row windows (k_row_windows) of the rows from win_row0 on
     int* counts; l3d_match_rec* recs;                                     // per-row match count and records
     int knn;                                                              // TopK: k; Store: row stride; Count: unused
     float epi;
@@ -61,9 +62,10 @@ struct MatchArgs {
 enum class Keep { TopK, Count, Store };
 template <int SEM, Keep KEEP> __global__ void k_match_topk(MatchArgs A);    // SEM: L3D_SEM_REF_GPU / L3D_SEM_REF_CPU
 #ifdef L3D_MATCH_PROBE
-/* probe build only (tools/probe_match_phases.py): clock64 spans of every warp by phase, counters, and per CTA the longest, shortest and
+/* probe build only (tools/probe_match_phases.py): clock64 spans (a row's set-up: its constants, its window positions, the concatenation
+   of its window pieces) of every warp by phase, counters, and per CTA the longest, shortest and
    summed warp busy time, all summed over the CTAs of the launches since the last reset; read with l3d_match_probe (extern "C") */
-enum { MP_SETUP, MP_SCAN, MP_EXACT, MP_FINAL, MP_WAIT, MP_TAIL, MP_ROWS, MP_ENTRIES, MP_SURVIVORS, MP_EVALS, MP_DRAINS,
+enum { MP_SETUP, MP_WINDOW, MP_PIECES, MP_SCAN, MP_EXACT, MP_FINAL, MP_WAIT, MP_TAIL, MP_ROWS, MP_ENTRIES, MP_SURVIVORS, MP_EVALS, MP_DRAINS,
        MP_CTAS, MP_BUSY_MAX, MP_BUSY_MIN, MP_BUSY_SUM, MP_N };
 #endif
 extern void (*const l3d_match_kernels[2][3])(MatchArgs);                   // every instantiation of k_match_topk: [SEM][KEEP]
@@ -75,6 +77,17 @@ __global__ void k_pair_arcs(const float4* __restrict__ segs, const L3DViewDev* _
 __global__ void k_arcs_gather(long long n, const unsigned long long* __restrict__ keys, const unsigned int* __restrict__ vals,
                               const uint4* __restrict__ raw, const float4* __restrict__ segs, const L3DViewDev* __restrict__ views,
                               const L3DPairDev* __restrict__ pairs, int first_pair, uint4* __restrict__ out, float4* __restrict__ out_segs);
+// row windows of the work units of one call (k_match_topk reads them): L3D_RW_WORDS words per row, 16-byte aligned, row r of the
+// call (counted from win_row0) at wins + r * (L3D_RW_WORDS / 4):
+//   word 0, 1: the pencil parameters k1, k2 of the row's two epipolar lines (line_kappa); word 2: 1 if the row skips level 1; word 3: 0;
+//   word 4 + 2c, 5 + 2c (arc class c < L3D_ARC_NCLS): the first entry of the pair's sorted table inside class c whose arc start is not
+//   below ka - 2^(L3D_ARC_CLS0 + c), resp. above kb (the class end when kb = 2^32 - 1); pair-relative, over the whole class
+#define L3D_RW_WORDS 20
+#define L3D_RW_STAGE 12000      /* most arc starts of a pair k_row_windows stages in shared memory: 47 KB, plus its static shared memory within
+                                   the 48 KB a launch gets without opting in; larger tables are searched in place */
+__global__ void k_row_windows(const float4* __restrict__ segs, const L3DViewDev* __restrict__ views, const L3DPairDev* __restrict__ pairs,
+                              const int4* __restrict__ units, const L3DPairBasis* __restrict__ basis, const uint4* __restrict__ arcs,
+                              long long win_row0, uint4* __restrict__ wins);
 __global__ void k_sort_rows(int* __restrict__ counts, l3d_match_rec* __restrict__ recs, int stride, long long rows, int topk);
 __global__ void k_prep_segments_f64(const float4* __restrict__ segs, const L3DViewDev* __restrict__ views, int num_views,
                                     long long total, double* __restrict__ cache);

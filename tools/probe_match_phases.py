@@ -5,7 +5,8 @@ first V views, 5 V view pairs).
                                                       # libl3d_b200_probe_O0.so, window pieces in class order (MK_SCAN_ORDER=0)
     python tools/probe_match_phases.py run [V]        # on the GPU (default V = 100); L3D_LIB=<.so> runs another probe build
 
-The probe build adds clock64() spans per warp (l3d_match.cuh, MP_*); without the define none of it is compiled.  Shares are of all
+The probe build adds clock64() spans per warp (l3d_match.cuh, MP_*); without the define none of it is compiled.  A row's set-up is three
+phases: "setup" (setup_row: its constants), "window" (its window positions in every arc class) and "pieces" (their concatenation).  Shares are of all
 warp-cycles of the launch: every warp's time from its first instruction to the end of its CTA.  "other" is the busy time no phase
 covers (the CTA prologue before its barrier).  The spread compares, per CTA, the longest and the shortest warp busy time.
 """
@@ -16,7 +17,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 
-PHASES = ["setup", "scan", "exact", "finalize", "wait", "tail"]
+PHASES = ["setup", "window", "pieces", "scan", "exact", "finalize", "wait", "tail"]
 KEYS = PHASES + ["rows", "entries", "survivors", "evals", "drains", "ctas", "busy_max", "busy_min", "busy_sum"]
 SO = "libl3d_b200_probe.so"
 
@@ -46,6 +47,7 @@ def run(V):
     print("| phase | share of warp-cycles |\n|---|---|")
     for k in PHASES:
         print(f"| {k} | {p[k] / total:.1%} |")
+    print(f"| row set-up (setup + window + pieces) | {sum(p[k] for k in PHASES[:3]) / total:.1%} |")
     print(f"| other | {(p['busy_sum'] - sum(p[k] for k in PHASES[:-1])) / total:.1%} |")
     print(f"warp busy time inside a CTA, summed over CTAs: shortest / longest {p['busy_min'] / p['busy_max']:.3f}, "
           f"mean / longest {p['busy_sum'] / total:.3f}")
