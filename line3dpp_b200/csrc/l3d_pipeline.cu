@@ -85,7 +85,9 @@ __device__ __forceinline__ bool sw_orientation_ok(const L3DViewDev* V, const Seg
     const double n2 = ddot(d, d);
     if (n2 > 1e-20) {
         const double c = ddot(q.rm, d) / sqrt(n2);
-        const double c1 = 0.99518472667, c2 = -0.99518472667;       // cos(pi/32), cos(31 pi/32)
+        // the cosines of the thresholds the reference compares acos with, (double)L3D_PI_1_32_F and (double)L3D_PI_31_32_F: the two
+        // float constants are not symmetric about pi/2, so c2 != -c1
+        const double c1 = 0.99518472640441780, c2 = -0.99518473132192450;
         if (c < c1 - 1e-9 && c > c2 + 1e-9) return true;
         if (c > c1 + 1e-9 || c < c2 - 1e-9) return false;
     }

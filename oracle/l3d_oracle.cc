@@ -962,6 +962,7 @@ struct FinalLine {
 struct orc_ctx {
     bool by_wps, use_gpu;
     match_lines_fn_t match_fn; score_matches_fn_t score_fn; rdd_fn_t rdd_fn; collinear_fn_t collin_fn;
+    orc_match_source_fn match_source;     // set: hands over every pair's match lists in place of matching, in both semantics
     std::map<uint32_t, View*> views; std::vector<uint32_t> view_order;
     std::map<uint32_t, std::vector<std::list<orc_match_t> > > matches;
     std::map<uint32_t, std::vector<orc_match_t> > scored;    // dump: flattened matches right after scoring
@@ -1076,7 +1077,9 @@ void matching(orc_ctx* c, uint32_t src, uint32_t tgt, const M3& F)   // matching
     int cap = c->kNN > 0 ? c->kNN : Nt;
     std::vector<int> counts(Ns); std::vector<orc_match_t> out((size_t)Ns * cap);
     long long n;
-    if (c->use_gpu) {
+    if (c->match_source) {
+        n = c->match_source(src, tgt, Ns, Nt, c->kNN, &counts[0], &out[0], cap);
+    } else if (c->use_gpu) {
         float Ff[9]; for (int i = 0; i < 9; ++i) Ff[i] = (float)F.m[i];   // eigen2dataArray line3D.cc:2775-2781
         n = c->match_fn(&v1->lines[0].x, Ns, &v2->lines[0].x, Nt, Ff, v1->RtKinv_f, v2->RtKinv_f, v1->C_f3, v2->C_f3,
                         src, tgt, c->epi, c->kNN, &counts[0], &out[0], cap, NULL);
@@ -1512,7 +1515,7 @@ orc_ctx* orc_create(int neighbors_by_worldpoints, int use_gpu)
     orc_ctx* c = new orc_ctx();
     c->by_wps = neighbors_by_worldpoints != 0; c->use_gpu = use_gpu != 0;
     c->match_fn = (match_lines_fn_t)orc_match_lines_f32; c->score_fn = (score_matches_fn_t)orc_score_matches_f32; c->rdd_fn = (rdd_fn_t)orc_rdd_f32;
-    c->collin_fn = (collinear_fn_t)orc_collinear_f32;
+    c->collin_fn = (collinear_fn_t)orc_collinear_f32; c->match_source = NULL;
     c->num_lines_total = 0; c->pair_evals = 0; c->collin_t = -1.0f; c->localID = 0;
     c->translation = V(0, 0, 0); c->med_scene_depth = -1.0f; c->med_scene_depth_lines = 0.0f;
     c->fixed3Dreg = false; c->perform_RDD = false; c->visibility_t = 3; c->num_neighbors = 10; c->kNN = 10;
@@ -1530,6 +1533,7 @@ void orc_set_backend(orc_ctx* c, void* m, void* s, void* r)
     if (s) c->score_fn = (score_matches_fn_t)s;
     if (r) c->rdd_fn = (rdd_fn_t)r;
 }
+void orc_set_match_source(orc_ctx* c, orc_match_source_fn fn) { c->match_source = fn; }
 void orc_set_collinear_backend(orc_ctx* c, void* f) { c->collin_fn = f ? (collinear_fn_t)f : (collinear_fn_t)orc_collinear_f32; }
 
 int orc_add_view(orc_ctx* c, uint32_t cam_id, int width, int height, const double* K, const double* R, const double* t,

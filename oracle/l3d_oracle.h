@@ -76,6 +76,11 @@ void orc_set_backend(orc_ctx*, void* match_lines_fn, void* score_matches_fn, voi
 void orc_set_threads(int n);
 /* same for find_collinear_segments_GPU (signature of ref_collinear / orc_collinear_f32); NULL restores the CPU emulation */
 void orc_set_collinear_backend(orc_ctx*, void* collinear_fn);
+/* optional: the match lists of every view pair from fn instead of from matching (matchingGPU / matchingCPU), so that hand-built
+ * lists reach the orientation check, scoring and filter of either semantics.  fn(src cam, tgt cam, Ns, Nt, kNN, counts[Ns],
+ * out[Ns * cap], cap) fills row r's counts[r] <= cap matches at out[r * cap] and returns their total.  NULL: matching again. */
+typedef long long (*orc_match_source_fn)(uint32_t src_cam, uint32_t tgt_cam, int Ns, int Nt, int kNN, int* counts, orc_match_t* out, int cap);
+void orc_set_match_source(orc_ctx*, orc_match_source_fn fn);
 /* addImage with explicit line segments (line3D.cc:112-226); image itself is not needed */
 int orc_add_view(orc_ctx*, uint32_t cam_id, int width, int height, const double* K, const double* R, const double* t,
                  float median_depth, const uint32_t* wps_or_neighbors, int n_list, const float* segs, int nseg);

@@ -148,12 +148,32 @@ def cluster(fn, ei, ej, ew, n, c=3.0):
 
 
 # ------------------------------------------------------------------------------------------- pipeline wrapper
+_MATCH_SOURCE_T = C.CFUNCTYPE(C.c_longlong, C.c_uint32, C.c_uint32, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int)
+
 class OraclePipeline:
     """Restatement of L3DPP::Line3D (addImage / matchImages / reconstruct3Dlines) on explicit segments."""
 
-    def __init__(self, neighbors_by_worldpoints=False, use_gpu=True, backend=None):
+    def __init__(self, neighbors_by_worldpoints=False, use_gpu=True, backend=None, match_source=None):
+        """match_source: fn(src_cam, tgt_cam, Ns, Nt, kNN, cap) -> (counts int32[Ns], matches MATCH_DT[Ns, cap]) in place of
+        matching every view pair (orc_set_match_source); its rows must obey what the matcher guarantees"""
         self.L = lib()
         self.ctx = C.c_void_p(self.L.orc_create(int(neighbors_by_worldpoints), int(use_gpu)))
+        if match_source is not None:
+            def source(src, tgt, Ns, Nt, knn, counts, out, cap):
+                try:
+                    cnt, m = match_source(int(src), int(tgt), int(Ns), int(Nt), int(knn), int(cap))
+                    cnt = np.ascontiguousarray(cnt, np.int32)
+                    m = np.ascontiguousarray(m, MATCH_DT)
+                    assert cnt.shape == (Ns,) and m.shape == (Ns, cap) and (cnt >= 0).all() and (cnt <= cap).all()
+                    C.memmove(counts, cnt.ctypes.data, cnt.nbytes)
+                    C.memmove(out, m.ctypes.data, m.nbytes)
+                    return int(cnt.sum())
+                except Exception as e:  # noqa: BLE001 - must not unwind through the C frame; raised again by match_images
+                    self._source_error = e
+                    return 0
+            self._source_error = None
+            self._source = _MATCH_SOURCE_T(source)       # the library keeps the pointer: keep the callback alive
+            self.L.orc_set_match_source(self.ctx, self._source)
         if backend is not None:   # verbatim reference kernels (oracle/_ref) instead of the CPU emulation
             g = lambda n: C.cast(getattr(backend, n), C.c_void_p)
             self.L.orc_set_backend(self.ctx, g("ref_match_lines"), g("ref_score_matches"), g("ref_rdd"))
@@ -179,8 +199,11 @@ class OraclePipeline:
             assert rc == 0, rc
 
     def match_images(self, sigma_p=2.5, sigma_a=10.0, num_neighbors=10, epi_overlap=0.25, knn=10, const_reg_depth=-1.0):
-        return self.L.orc_match_images(self.ctx, C.c_float(sigma_p), C.c_float(sigma_a), C.c_uint(num_neighbors),
-                                       C.c_float(epi_overlap), C.c_int(knn), C.c_float(const_reg_depth))
+        rc = self.L.orc_match_images(self.ctx, C.c_float(sigma_p), C.c_float(sigma_a), C.c_uint(num_neighbors),
+                                     C.c_float(epi_overlap), C.c_int(knn), C.c_float(const_reg_depth))
+        if getattr(self, "_source_error", None) is not None:
+            raise self._source_error
+        return rc
 
     def reconstruct(self, visibility_t=3, perform_diffusion=False, collinearity_t=-1.0, use_ceres=False, max_iter_ceres=250):
         return self.L.orc_reconstruct_opt(self.ctx, C.c_uint(visibility_t), int(perform_diffusion),
