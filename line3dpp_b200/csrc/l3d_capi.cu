@@ -62,9 +62,9 @@ int l3d_ctx_create(int device, l3d_ctx** out)
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, device);
     c->num_sms = prop.multiProcessorCount;
-    for (const auto& by_keep : l3d_match_kernels)
-        for (auto k : by_keep)
-            if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l3d_match_smem_bytes());
+    for (int sem = 0; sem < 2; ++sem)
+        for (auto k : l3d_match_kernels[sem])
+            if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l3d_match_smem_bytes(sem));
     // once, at the most any launch uses: the attribute is per device, and a per-launch setting would race between contexts that match
     // or score on one device from several host threads
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_sort_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SORT_SMEM_MAX);
@@ -314,7 +314,7 @@ static int launch_match(l3d_ctx* c, Keep keep, MatchArgs a, size_t t0, size_t t1
 {
     a.units += t0;
     void* args[] = {&a};
-    cudaLaunchKernel((const void*)l3d_match_kernels[c->semantics][(int)keep], dim3((unsigned int)(t1 - t0)), dim3(MK_THREADS), args, l3d_match_smem_bytes(), c->stream);
+    cudaLaunchKernel((const void*)l3d_match_kernels[c->semantics][(int)keep], dim3((unsigned int)(t1 - t0)), dim3(MK_THREADS), args, l3d_match_smem_bytes(c->semantics), c->stream);
     ++c->launches;
     L3D_CUDA(c, cudaGetLastError(), what);
     return L3D_OK;

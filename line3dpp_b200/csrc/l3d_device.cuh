@@ -110,6 +110,14 @@ __device__ __forceinline__ SegRays load_rays(const float4* __restrict__ cache, l
     s.n = make_float3(b.z, b.w, c.x);
     return s;
 }
+// the same three float4 from shared memory
+__device__ __forceinline__ SegRays rays_from_smem(const float4* p)
+{
+    const float4 a = p[0], b = p[1], c = p[2];
+    SegRays s;
+    s.r1 = make_float3(a.x, a.y, a.z); s.r2 = make_float3(a.w, b.x, b.y); s.n = make_float3(b.z, b.w, c.x);
+    return s;
+}
 
 // =============================================================================== exact section (reference op order)
 __device__ __forceinline__ float dot3(float3 a, float3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
@@ -177,6 +185,9 @@ __device__ __forceinline__ float exact_overlap(float4 q, float3 e1, float3 e2, b
     return any ? r : 0.0f;
 }
 
+// numerator of the depths on the plane through camera centre Ca with normal n, seen from camera centre Cb
+__device__ __forceinline__ float depth_num(float3 n, float3 Ca, float3 Cb) { return dot3(Ca, n) - dot3(n, Cb); }
+
 // The two D_triangulate_depth calls of K_match_lines (cudawrapper.cu:139-164, 237-242) from cached rays / normals.
 //   d[0],d[1]: depths of the src endpoints on the plane (C_tgt, tgt segment)
 //   d[2],d[3]: depths of the tgt endpoints on the plane (C_src, src segment)
@@ -186,17 +197,31 @@ __device__ __forceinline__ void exact_depths(const SegRays& s, const SegRays& t,
     {
         float dp1 = dot3(t.n, s.r1), dp2 = dot3(t.n, s.r2);
         if (!(fabsf(dp1) < L3D_EPS_F || fabsf(dp2) < L3D_EPS_F)) {
-            float num = dot3(Ct, t.n) - dot3(t.n, Cs);
+            float num = depth_num(t.n, Ct, Cs);
             d[0] = num / dp1; d[1] = num / dp2;
         }
     }
     {
         float dq1 = dot3(s.n, t.r1), dq2 = dot3(s.n, t.r2);
         if (!(fabsf(dq1) < L3D_EPS_F || fabsf(dq2) < L3D_EPS_F)) {
-            float num = dot3(Cs, s.n) - dot3(s.n, Ct);
+            float num = depth_num(s.n, Cs, Ct);
             d[2] = num / dq1; d[3] = num / dq2;
         }
     }
+}
+
+// True exactly when exact_depths(s, t, Cs, Ct, d) makes all four d > 0, without its four divisions; num_s = depth_num(s.n, Cs, Ct).
+// Each depth is num / dp with |dp| >= L3D_EPS_F (else -1), and |dp| <= 1 + 1e-6: both factors are unit vectors normalised with
+// rsqrtf, or NaN.  Denormals are kept (no -ftz), so a finite num != 0 gives a quotient of magnitude at least 2^-149 / (1 + 1e-6)
+// before rounding, above the 2^-150 midpoint: it never rounds to 0, and num / dp > 0 exactly when num and dp are nonzero with the
+// same sign.  NaN fails both forms; an infinite quotient passes both when the signs agree.
+__device__ __forceinline__ bool same_sign(float a, float b) { return (a > 0.0f && b > 0.0f) || (a < 0.0f && b < 0.0f); }
+__device__ __forceinline__ bool depths_in_front(const SegRays& s, const SegRays& t, float3 Cs, float3 Ct, float num_s)
+{
+    const float dp1 = dot3(t.n, s.r1), dp2 = dot3(t.n, s.r2), dq1 = dot3(s.n, t.r1), dq2 = dot3(s.n, t.r2);
+    if (fabsf(dp1) < L3D_EPS_F || fabsf(dp2) < L3D_EPS_F || fabsf(dq1) < L3D_EPS_F || fabsf(dq2) < L3D_EPS_F) return false;
+    const float num_t = depth_num(t.n, Ct, Cs);
+    return same_sign(num_t, dp1) && same_sign(num_t, dp2) && same_sign(num_s, dq1) && same_sign(num_s, dq2);
 }
 
 // =============================================================================== conservative pre-filter

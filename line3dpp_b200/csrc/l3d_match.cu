@@ -105,8 +105,11 @@ struct MatchSmem {
 #ifdef L3D_MATCH_PROBE
     unsigned long long probe[MK_WARPS][MP_N];
 #endif
+    // REF_GPU only, last: REF_CPU launches without them (l3d_match_smem_bytes), which leaves it 32 KB more L1 (DESIGN.md section 8)
+    float4 srays[MK_NSLOT][3];                       // the row's cached rays and plane normal (k_prep_segments), for its depths
+    float snum[MK_NSLOT];                            // the row's depth numerator depth_num(n, Cs, Ct) (depths_in_front)
 };
-size_t l3d_match_smem_bytes() { return sizeof(MatchSmem); }
+size_t l3d_match_smem_bytes(int sem) { return sem == L3D_SEM_REF_GPU ? sizeof(MatchSmem) : offsetof(MatchSmem, srays); }
 
 #ifdef L3D_MATCH_PROBE
 __device__ __forceinline__ void probe_add(MatchSmem& S, int warp, int lane, int k, unsigned long long v) { if (lane == 0) S.probe[warp][k] += v; }
@@ -129,27 +132,31 @@ __device__ __forceinline__ int rank_in_row(const unsigned long long* list, int n
     return r;
 }
 
+// the same rank when lane's key is one of the `rounds` best keys of the active lanes, 64 otherwise: `rounds` rounds of warp maximum
+// (keys are unique and > 0) instead of ranking all keys against each other.  rounds is warp-uniform.
+__device__ __forceinline__ int top_rank(unsigned long long k, bool active, int rounds)
+{
+    const unsigned int hi = (unsigned int)(k >> 32), lo = (unsigned int)k;
+    int r = 64;
+    for (int i = 0; i < rounds; ++i) {
+        const unsigned int m = __reduce_max_sync(0xffffffffu, active ? hi : 0u);
+        bool c = active && hi == m;
+        unsigned int bm = __ballot_sync(0xffffffffu, c);
+        if (__popc(bm) > 1) { const unsigned int l = __reduce_max_sync(0xffffffffu, c ? lo : 0u); c = c && lo == l; }
+        if (c) { r = i; active = false; }
+    }
+    return r;
+}
+
 // keep the k best keys of a full row list (sorted, best first) and raise the row's score-to-beat
 __device__ __noinline__ void prune_row(MatchSmem& S, int slot, int lane)
 {
     const int knn = S.knn; const float epi = S.epi;
+    MPROBE(probe_add(S, threadIdx.x >> 5, lane, MP_PRUNES, 1);)
     __syncwarp();
     const int n = min(S.list_cnt[slot], S.cap);
     const unsigned long long k = lane < n ? S.lists[slot][lane] : 0ull;
-    int r;
-    if (knn <= 16) {          // k rounds of warp maximum (keys are unique and > 0) instead of ranking all n keys against each other
-        bool active = lane < n;
-        const unsigned int hi = (unsigned int)(k >> 32), lo = (unsigned int)k;
-        r = 64;
-        const int rounds = min(knn, n);
-        for (int i = 0; i < rounds; ++i) {
-            const unsigned int m = __reduce_max_sync(0xffffffffu, active ? hi : 0u);
-            bool c = active && hi == m;
-            unsigned int bm = __ballot_sync(0xffffffffu, c);
-            if (__popc(bm) > 1) { const unsigned int l = __reduce_max_sync(0xffffffffu, c ? lo : 0u); c = c && lo == l; }
-            if (c) { r = i; active = false; }
-        }
-    } else r = rank_in_row(S.lists[slot], n, k);
+    const int r = knn <= 16 ? top_rank(k, lane < n, min(knn, n)) : rank_in_row(S.lists[slot], n, k);
     __syncwarp();
     if (lane < n && r < knn) S.lists[slot][r] = k;
     __syncwarp();
@@ -164,10 +171,11 @@ __device__ __noinline__ void prune_row(MatchSmem& S, int slot, int lane)
     __syncwarp();
 }
 
-// depths (d_p1, d_p2, d_q1, d_q2) of target j for the unit's row rl, stored as Match stores them (floats, commons.h:186-203); true when
-// all four are in front of the cameras: > 0 in float (REF_GPU, cudawrapper.cu:186-253) or > 1e-12 in double (REF_CPU, line3D.cc:925-1003)
+// depths (d_p1, d_p2, d_q1, d_q2) of target j for the unit's row rl in slot sl, stored as Match stores them (floats, commons.h:186-203);
+// true when all four are in front of the cameras: > 0 in float (REF_GPU, cudawrapper.cu:186-253; the row's rays from its slot) or
+// > 1e-12 in double (REF_CPU, line3D.cc:925-1003)
 template <int SEM>
-__device__ __forceinline__ bool target_depths(const MatchSmem& S, int rl, unsigned int j, float* d)
+__device__ __forceinline__ bool target_depths(const MatchSmem& S, int sl, int rl, unsigned int j, float* d)
 {
     if (SEM == L3D_SEM_REF_CPU) {
         const SegRaysD s = load_rays_d(S.cache_d, S.src_base + rl), t = load_rays_d(S.cache_d, S.toff + j);
@@ -176,35 +184,35 @@ __device__ __forceinline__ bool target_depths(const MatchSmem& S, int rl, unsign
         d[0] = (float)dd[0]; d[1] = (float)dd[1]; d[2] = (float)dd[2]; d[3] = (float)dd[3];
         return dd[0] > L3D_EPS_D && dd[1] > L3D_EPS_D && dd[2] > L3D_EPS_D && dd[3] > L3D_EPS_D;
     }
-    const SegRays s = load_rays(S.cache, S.src_base + rl), t = load_rays(S.cache, S.toff + j);
+    const SegRays s = rays_from_smem(S.srays[sl]), t = load_rays(S.cache, S.toff + j);
     exact_depths(s, t, S.Cs, S.Ct, d);
     return d[0] > 0.0f && d[1] > 0.0f && d[2] > 0.0f && d[3] > 0.0f;
 }
 
-// exact evaluation of candidate j (target segment q) for the row rl held by slot sl (has == false: padding lane, never a match): the
-// overlap must exceed epi and reach the row's current k-th best (below it the candidate can never be selected), and the depths must be
-// positive (target_depths).
-// REF_GPU: K_match_lines' float overlap with the row's cached epipolar lines, inline (the lanes stay converged through it);
-// REF_CPU: matchingCPU's double overlap (line3D.cc:925-1003) with epipolar lines from the double F, out of line.
-template <int SEM> __device__ bool eval_candidate(const MatchSmem& S, int sl, int rl, unsigned int j, float4 q, bool has, float* ov, float* d);
-template <> __device__ __forceinline__ bool eval_candidate<L3D_SEM_REF_GPU>(const MatchSmem& S, int sl, int rl, unsigned int j, float4 q, bool has, float* ov, float* d)
+// REF_GPU: the overlap test of a candidate (target segment q) for the row held by slot sl (has == false: padding lane, never a match),
+// K_match_lines' float overlap with the row's cached epipolar lines: it must exceed epi and reach the row's current k-th best (below it
+// the candidate can never be selected).  Inline: the lanes stay converged through it.
+__device__ __forceinline__ bool overlap_pass(const MatchSmem& S, int sl, float4 q, bool has, float* ov)
 {
     const float4 rA = S.rowA[sl], rB = S.rowB[sl];
     bool inv;
     *ov = exact_overlap(q, make_float3(rA.x, rA.y, rA.z), make_float3(rA.w, rB.x, rB.y), &inv);
-    return has && *ov > S.epi && *ov >= S.row_thr[sl] && target_depths<L3D_SEM_REF_GPU>(S, rl, j, d);
+    return has && *ov > S.epi && *ov >= S.row_thr[sl];
 }
-template <> __device__ __noinline__ bool eval_candidate<L3D_SEM_REF_CPU>(const MatchSmem& S, int sl, int rl, unsigned int j, float4 q, bool has, float* ov, float* d)
+// REF_CPU: the same test with matchingCPU's double overlap (line3D.cc:925-1003) and epipolar lines from the double F, then the depth
+// test; out of line, so that its double values are not live in exact_batch
+__device__ __noinline__ bool eval_candidate_f64(const MatchSmem& S, int sl, int rl, unsigned int j, float4 q, bool has, float* ov, float* d)
 {
     if (!has) return false;
     const float4 sp = __ldg(S.ssegs + rl);
     const D3 e1 = dmulmat(S.Fd, d3((double)sp.x, (double)sp.y, 1.0)), e2 = dmulmat(S.Fd, d3((double)sp.z, (double)sp.w, 1.0));
     bool valid;
     *ov = exact_overlap_f64(q, e1, e2, &valid);
-    return valid && *ov > S.epi && *ov >= S.row_thr[sl] && target_depths<L3D_SEM_REF_CPU>(S, rl, j, d);
+    return valid && *ov > S.epi && *ov >= S.row_thr[sl] && target_depths<L3D_SEM_REF_CPU>(S, sl, rl, j, d);
 }
 
-// exact evaluation of up to 32 queued candidates (one per lane).  Out of line on purpose: the hot filter loop must
+// exact evaluation of up to 32 queued candidates (one per lane): REF_GPU the overlap test (overlap_pass), then the depth test on the
+// lanes that passed it; REF_CPU both in eval_candidate_f64.  Out of line on purpose: the hot filter loop must
 // stay inside the instruction cache (the first version inlined this 5x -> 64 KB of SASS, 55 % "no instruction" stalls).
 // A match is kept per KEEP: TopK pushes its key into the slot's list (cut to the kNN best when full), Count only counts it,
 // Store writes its record (row stride S.knn, slot = arrival order; k_sort_rows puts the rows into the reference's
@@ -213,32 +221,45 @@ template <int SEM, Keep KEEP>
 __device__ __noinline__ void exact_batch(MatchSmem& S, unsigned int entry, bool has, int lane)
 {
     const int knn = S.knn;
-    bool pending = false;
-    unsigned long long key = 0ull;
-    int sl = 0;
-    if (has) {
-        sl = (int)(entry >> 24);
-        const int rl = S.slot_row[sl];
-        const unsigned int pos = entry & 0xFFFFFFu;                  // position in the resident ring: target index and segment are staged
-        const unsigned int j = (&S.stage[0][0])[pos].w;
-        float ov = 0.0f, d[4];
-        if (eval_candidate<SEM>(S, sl, rl, j, (&S.stage_seg[0][0])[pos], has, &ov, d)) {
-            if (KEEP == Keep::TopK) { key = make_key(ov, j); pending = true; }
-            else {
-                const int slot = atomicAdd(&S.list_cnt[sl], 1);         // a row belongs to one warp: no cross-warp contention
-                if (KEEP == Keep::Store && slot < knn) {
-                    l3d_match_rec rec;
-                    rec.tgt_seg = j; rec.overlap = ov; rec.d_p1 = d[0]; rec.d_p2 = d[1]; rec.d_q1 = d[2]; rec.d_q2 = d[3];
-                    S.recs_out[(S.R0 + rl) * knn + slot] = rec;
-                }
+    MPROBE(const int warp = threadIdx.x >> 5;)
+    const int sl = has ? (int)(entry >> 24) : 0;
+    const int rl = S.slot_row[sl];
+    const unsigned int pos = entry & 0xFFFFFFu;                      // position in the resident ring: target index and segment are staged
+    const unsigned int j = (&S.stage[0][0])[pos].w;
+    float ov = 0.0f, d[4];
+    const float4 q = (&S.stage_seg[0][0])[pos];
+    bool pending;
+    if (SEM == L3D_SEM_REF_CPU) pending = eval_candidate_f64(S, sl, rl, j, q, has, &ov, d);
+    else {
+        // TopK and Count only need the depth test's outcome: a sign test without the divisions (depths_in_front), on the target's rays
+        // loaded before the overlap arithmetic, which hides their L2 latency (Store holds the depths too and would spill with them)
+        const SegRays t = KEEP != Keep::Store ? load_rays(S.cache, S.toff + j) : SegRays{};
+        pending = overlap_pass(S, sl, q, has, &ov);
+        MPROBE(probe_add(S, warp, lane, MP_OVERLAP_PASS, __popc(__ballot_sync(0xffffffffu, pending)));)
+        if (pending)
+            pending = KEEP == Keep::Store ? target_depths<SEM>(S, sl, rl, j, d) : depths_in_front(rays_from_smem(S.srays[sl]), t, S.Cs, S.Ct, S.snum[sl]);
+    }
+    MPROBE(probe_add(S, warp, lane, MP_DEPTH_PASS, __popc(__ballot_sync(0xffffffffu, pending)));)
+    if (KEEP != Keep::TopK) {
+        if (pending) {
+            const int slot = atomicAdd(&S.list_cnt[sl], 1);             // a row belongs to one warp: no cross-warp contention
+            if (KEEP == Keep::Store && slot < knn) {
+                l3d_match_rec rec;
+                rec.tgt_seg = j; rec.overlap = ov; rec.d_p1 = d[0]; rec.d_p2 = d[1]; rec.d_q1 = d[2]; rec.d_q2 = d[3];
+                S.recs_out[(S.R0 + rl) * knn + slot] = rec;
             }
         }
+        __syncwarp();
+        return;
     }
-    while (KEEP == Keep::TopK) {
+    const unsigned long long key = make_key(ov, j);
+    while (true) {
+        MPROBE(bool pushed = false;)
         if (pending) {
             int slot = atomicAdd(&S.list_cnt[sl], 1);
-            if (slot < S.cap) { S.lists[sl][slot] = key; pending = false; }
+            if (slot < S.cap) { S.lists[sl][slot] = key; pending = false; MPROBE(pushed = true;) }
         }
+        MPROBE(probe_add(S, warp, lane, MP_PUSHED, __popc(__ballot_sync(0xffffffffu, pushed)));)
         unsigned int pm = __ballot_sync(0xffffffffu, pending);
         if (!pm) break;
         unsigned int todo = pm;                       // a row list is full: keep its k best and retry
@@ -275,11 +296,16 @@ __device__ __noinline__ void finalize_row(MatchSmem& S, int sl, int lane)
     if (lane == 0) S.counts_out[R] = min(n, knn);
     if (n == 0) return;
     const unsigned long long key = lane < n ? S.lists[sl][lane] : 0ull;
-    const int rank = rank_in_row(S.lists[sl], n, key);
+    const unsigned int j = key_tgt(key);
+    // REF_GPU: the target's rays loaded before the ranking, which hides their latency
+    const SegRays t = SEM == L3D_SEM_REF_GPU ? load_rays(S.cache, S.toff + (lane < n ? j : 0u)) : SegRays{};
+    // REF_GPU kNN <= 16: prune_row's selection; REF_CPU ranks by counting (the selection makes its finalize_row spill, 18 % slower on
+    // the benchmark's first 500 view pairs, H100 80GB HBM3, 700 W)
+    const int rank = SEM == L3D_SEM_REF_GPU && knn <= 16 ? top_rank(key, lane < n, min(knn, n)) : rank_in_row(S.lists[sl], n, key);
     if (lane < n && rank < knn) {
-        unsigned int j = key_tgt(key);
         float d[4];
-        target_depths<SEM>(S, rl, j, d);
+        if (SEM == L3D_SEM_REF_GPU) exact_depths(rays_from_smem(S.srays[sl]), t, S.Cs, S.Ct, d);
+        else target_depths<SEM>(S, sl, rl, j, d);
         l3d_match_rec rec;
         rec.tgt_seg = j; rec.overlap = key_overlap(key);
         rec.d_p1 = d[0]; rec.d_p2 = d[1]; rec.d_q1 = d[2]; rec.d_q2 = d[3];
@@ -510,11 +536,19 @@ __device__ __forceinline__ unsigned int row_window(const MatchSmem& S, int rl, i
 { return lane < L3D_RW_WORDS ? __ldg(S.wins + (size_t)rl * L3D_RW_WORDS + lane) : 0u; }
 
 // the constants of the unit's row rl into slot sl, and an empty key list: the epipolar lines F*p (cudawrapper.cu:216-217) and the float
-// filter's scale.  Returns the row's windows (row_window), loaded together with its segment so that the two loads overlap.
+// filter's scale; REF_GPU also its cached rays (lanes 0 .. 2, one float4 each) and their depth numerator, which every depth test of
+// the row uses.  Returns the row's windows (row_window), loaded together with its segment and rays so that the loads overlap.
+template <int SEM>
 __device__ __forceinline__ unsigned int setup_row(MatchSmem& S, int sl, int rl, int lane)
 {
     const unsigned int rw = row_window(S, rl, lane);
     const float4 s = __ldg(S.ssegs + rl);
+    if (SEM == L3D_SEM_REF_GPU) {
+        const float4 ray = lane < 3 ? __ldg(S.cache + 3 * (S.src_base + rl) + lane) : make_float4(0.f, 0.f, 0.f, 0.f);
+        const float nz = __shfl_sync(0xffffffffu, ray.x, 2);                 // n = (c1.z, c1.w, c2.x), rays_from_smem
+        if (lane < 3) S.srays[sl][lane] = ray;
+        if (lane == 1) S.snum[sl] = depth_num(make_float3(ray.z, ray.w, nz), S.Cs, S.Ct);
+    }
     const float3 e1 = mulmat_h(S.F, s.x, s.y), e2 = mulmat_h(S.F, s.z, s.w);
     if (lane == 0) {
         const float g = L3D_FILTER_C1 * fmaxf(sqrtf(e1.x * e1.x + e1.y * e1.y), sqrtf(e2.x * e2.x + e2.y * e2.y));
@@ -701,7 +735,7 @@ __global__ void __launch_bounds__(MK_THREADS, 1) k_match_topk(const MatchArgs A)
                     MPROBE(probe_add(S, warp, lane, MP_FINAL, clock64() - t0);)
                 }
                 MPROBE(const long long t0 = clock64();)
-                rw = setup_row(S, sl, rl, lane);
+                rw = setup_row<SEM>(S, sl, rl, lane);
                 MPROBE(probe_add(S, warp, lane, MP_SETUP, clock64() - t0); probe_add(S, warp, lane, MP_ROWS, 1);)
             } else rw = row_window(S, rl, lane);
             scan_row<SEM, KEEP>(S, sl, rw, warp, lane, qn);
@@ -810,14 +844,6 @@ int l3d_dense_rows_per_cta(int Ns, int Nt, int num_sms)
         if (eff > best_eff + 1e-9 || (eff > best_eff - 1e-9 && R > best)) { best_eff = eff; best = R; }
     }
     return best;
-}
-
-__device__ __forceinline__ SegRays rays_from_smem(const float4* p)
-{
-    const float4 a = p[0], b = p[1], c = p[2];
-    SegRays s;
-    s.r1 = make_float3(a.x, a.y, a.z); s.r2 = make_float3(a.w, b.x, b.y); s.n = make_float3(b.z, b.w, c.x);
-    return s;
 }
 
 __device__ __noinline__ void dense_exact_batch(DenseSmem& S, unsigned int entry, bool has, int warp, int x0)

@@ -42,7 +42,7 @@ static_assert(MK_NSLOT <= 256, "a queue entry is (slot << 24) | ring position: 8
 
 struct L3DMat3 { float m[9]; };
 
-size_t l3d_match_smem_bytes();
+size_t l3d_match_smem_bytes(int sem);        // dynamic shared memory of k_match_topk<sem, *>
 size_t l3d_dense_smem_bytes();
 
 __global__ void k_prep_segments(const float4* __restrict__ segs, const L3DViewDev* __restrict__ views, int num_views,
@@ -63,10 +63,11 @@ enum class Keep { TopK, Count, Store };
 template <int SEM, Keep KEEP> __global__ void k_match_topk(MatchArgs A);    // SEM: L3D_SEM_REF_GPU / L3D_SEM_REF_CPU
 #ifdef L3D_MATCH_PROBE
 /* probe build only (tools/probe_match_phases.py): clock64 spans (a row's set-up: its constants, its window positions, the concatenation
-   of its window pieces) of every warp by phase, counters, and per CTA the longest, shortest and
+   of its window pieces) of every warp by phase, counters (exact evaluations, those that pass the overlap test (REF_GPU), then the depth test, keys
+   pushed into row lists, prune_row calls), and per CTA the longest, shortest and
    summed warp busy time, all summed over the CTAs of the launches since the last reset; read with l3d_match_probe (extern "C") */
 enum { MP_SETUP, MP_WINDOW, MP_PIECES, MP_SCAN, MP_EXACT, MP_FINAL, MP_WAIT, MP_TAIL, MP_ROWS, MP_ENTRIES, MP_SURVIVORS, MP_EVALS, MP_DRAINS,
-       MP_CTAS, MP_BUSY_MAX, MP_BUSY_MIN, MP_BUSY_SUM, MP_N };
+       MP_OVERLAP_PASS, MP_DEPTH_PASS, MP_PUSHED, MP_PRUNES, MP_CTAS, MP_BUSY_MAX, MP_BUSY_MIN, MP_BUSY_SUM, MP_N };
 #endif
 extern void (*const l3d_match_kernels[2][3])(MatchArgs);                   // every instantiation of k_match_topk: [SEM][KEEP]
 // level-1 pre-filter tables: one CTA per view pair of [first_pair, first_pair + gridDim.x): raw arcs + sort keys; after the sort

@@ -8,7 +8,9 @@ first V views, 5 V view pairs).
 The probe build adds clock64() spans per warp (l3d_match.cuh, MP_*); without the define none of it is compiled.  A row's set-up is three
 phases: "setup" (setup_row: its constants), "window" (its window positions in every arc class) and "pieces" (their concatenation).  Shares are of all
 warp-cycles of the launch: every warp's time from its first instruction to the end of its CTA.  "other" is the busy time no phase
-covers (the CTA prologue before its barrier).  The spread compares, per CTA, the longest and the shortest warp busy time.
+covers (the CTA prologue before its barrier).  The spread compares, per CTA, the longest and the shortest warp busy time.  The
+counters split the exact evaluations by the test that stops them (overlap, then depths) and count the keys pushed into row lists and
+the prune_row calls that cut a full list to its k best.
 """
 import os
 import sys
@@ -18,7 +20,8 @@ import numpy as np
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 
 PHASES = ["setup", "window", "pieces", "scan", "exact", "finalize", "wait", "tail"]
-KEYS = PHASES + ["rows", "entries", "survivors", "evals", "drains", "ctas", "busy_max", "busy_min", "busy_sum"]
+KEYS = PHASES + ["rows", "entries", "survivors", "evals", "drains", "overlap_pass", "depth_pass", "pushed", "prunes", "ctas", "busy_max",
+                 "busy_min", "busy_sum"]
 SO = "libl3d_b200_probe.so"
 
 
@@ -54,6 +57,10 @@ def run(V):
     rows = max(p["rows"], 1.0)
     print(f"per row set-up: {p['entries'] / rows:.1f} window entries, {p['survivors'] / rows:.1f} survivors of both filters, "
           f"{p['evals'] / rows:.1f} exact evaluations; early queue drains {int(p['drains'])}")
+    ev = max(p["evals"], 1.0)
+    print(f"exact evaluations {int(p['evals'])}: {int(p['overlap_pass'])} pass the overlap test ({p['overlap_pass'] / ev:.1%}, "
+          f"{32 * p['overlap_pass'] / ev:.1f} of 32 lanes per batch), {int(p['depth_pass'])} the depth test too ({p['depth_pass'] / ev:.1%}); "
+          f"{int(p['pushed'])} keys pushed, {int(p['prunes'])} prune_row calls ({p['prunes'] / rows:.2f} per row)")
 
 
 if __name__ == "__main__":
