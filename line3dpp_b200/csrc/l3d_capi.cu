@@ -39,6 +39,48 @@ int DevBuf::reserve(l3d_ctx* c, size_t bytes, const char* what)
     return L3D_OK;
 }
 
+// the packed bytes of the blocks, each starting on a 16-byte boundary (k_remap_u8 reads its maps as short2 / ushort behind an image
+// of any width, triangulation stages doubles, l3d_match_dense writes float4); with a base, also each block's dev
+static size_t stage_layout(HostBlock* b, int n, char* base)
+{
+    size_t off = 0;
+    for (int i = 0; i < n; ++i) {
+        off = (off + 15) & ~(size_t)15;
+        if (base) b[i].dev = base + off;
+        off += b[i].row_bytes * b[i].rows;
+    }
+    return off;
+}
+
+int l3d_stage_host(l3d_ctx* c, HostBlock* in, int n_in, HostBlock* out, int n_out)
+{
+    int rc;
+    L3D_RESERVE(c->stage_in, stage_layout(in, n_in, nullptr), "host-mode input staging");
+    L3D_RESERVE(c->stage_out, stage_layout(out, n_out, nullptr), "host-mode output staging");
+    stage_layout(in, n_in, (char*)c->stage_in.p);
+    stage_layout(out, n_out, (char*)c->stage_out.p);
+    for (int i = 0; i < n_in; ++i) {
+        const HostBlock& b = in[i];
+        if (b.row_bytes * b.rows == 0) continue;
+        if (b.pitch == b.row_bytes) L3D_CUDA(c, cudaMemcpyAsync(b.dev, b.host, b.row_bytes * b.rows, cudaMemcpyHostToDevice, c->stream), "host-mode upload");
+        else L3D_CUDA(c, cudaMemcpy2DAsync(b.dev, b.row_bytes, b.host, b.pitch, b.row_bytes, b.rows, cudaMemcpyHostToDevice, c->stream), "host-mode upload");
+    }
+    return L3D_OK;
+}
+
+int l3d_unstage_host(l3d_ctx* c, const HostBlock* out, int n_out, const char* what)
+{
+    for (int i = 0; i < n_out; ++i) {
+        const HostBlock& b = out[i];
+        void* host = const_cast<void*>(b.host);     // the caller's output array, writable
+        if (b.row_bytes * b.rows == 0) continue;
+        if (b.pitch == b.row_bytes) L3D_CUDA(c, cudaMemcpyAsync(host, b.dev, b.row_bytes * b.rows, cudaMemcpyDeviceToHost, c->stream), "host-mode download");
+        else L3D_CUDA(c, cudaMemcpy2DAsync(host, b.pitch, b.dev, b.row_bytes, b.row_bytes, b.rows, cudaMemcpyDeviceToHost, c->stream), "host-mode download");
+    }
+    L3D_CUDA(c, cudaStreamSynchronize(c->stream), what);
+    return L3D_OK;
+}
+
 struct CastI64 { __host__ __device__ long long operator()(int v) const { return (long long)v; } };
 
 // the most dynamic shared memory k_sort_rows gets (run_keep_all: the rows of the CTA's warps at the keep-all stride)
@@ -805,11 +847,11 @@ static int match_dense_impl(l3d_ctx* c, int sv, int tv, const float* F, float ep
     if (Ns == 0 || Nt == 0) return L3D_OK;
     const size_t cells = (size_t)Ns * Nt;
     float4* d_dep = (float4*)depths; float* d_ov = overlaps;
+    HostBlock out[2] = {host_array(depths, sizeof(float4) * cells), host_array(overlaps, sizeof(float) * cells)};
+    int rc;
     if (!on_dev) {
-        int rc;
-        L3D_RESERVE(c->d_dense_dep, sizeof(float4) * cells, "dense depths");
-        L3D_RESERVE(c->d_dense_ov, sizeof(float) * cells, "dense overlaps");
-        d_dep = (float4*)c->d_dense_dep.p; d_ov = (float*)c->d_dense_ov.p;
+        if ((rc = l3d_stage_host(c, nullptr, 0, out, 2))) return rc;
+        d_dep = (float4*)out[0].dev; d_ov = (float*)out[1].dev;
     }
     const L3DDenseJob J = dense_job(c, sv, tv, F, d_dep, d_ov, l3d_dense_rows_per_cta(Ns, Nt, c->num_sms));
     if (filter)
@@ -818,11 +860,7 @@ static int match_dense_impl(l3d_ctx* c, int sv, int tv, const float* F, float ep
         k_match_dense_nofilter<<<dim3((Nt + DK_THREADS - 1) / DK_THREADS, (Ns + DKN_ROWS - 1) / DKN_ROWS), DK_THREADS, 0, c->stream>>>(J, epi);
     ++c->launches;
     L3D_CUDA(c, cudaGetLastError(), "k_match_dense");
-    if (!on_dev) {
-        L3D_CUDA(c, cudaMemcpyAsync(depths, d_dep, sizeof(float4) * cells, cudaMemcpyDeviceToHost, c->stream), "download dense depths");
-        L3D_CUDA(c, cudaMemcpyAsync(overlaps, d_ov, sizeof(float) * cells, cudaMemcpyDeviceToHost, c->stream), "download dense overlaps");
-        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync");
-    }
+    if (!on_dev && (rc = l3d_unstage_host(c, out, 2, "sync"))) return rc;
     return L3D_OK;
 }
 

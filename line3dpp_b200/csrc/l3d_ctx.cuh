@@ -21,6 +21,22 @@ struct DevBuf {
     int reserve(l3d_ctx* c, size_t bytes, const char* what);
 };
 
+// One caller array of a host-mode call: `rows` rows of `row_bytes` bytes, `pitch` bytes apart in host memory (a 1-D array is one
+// row).  l3d_stage_host sets `dev` to the block's device copy: its rows packed (pitch row_bytes), starting on a 16-byte boundary.
+struct HostBlock {
+    const void* host;                       // an output block's array is written by l3d_unstage_host
+    size_t pitch, row_bytes, rows;
+    void* dev = nullptr;
+};
+inline HostBlock host_array(const void* p, size_t bytes) { return HostBlock{p, bytes, bytes, 1}; }
+
+// Host mode of the calls that are not pipeline stages: packs the `in` blocks into the context's stage_in and the `out` blocks into
+// its stage_out, uploads `in` on the context's stream and sets every block's dev.  l3d_unstage_host then downloads `out` and waits
+// for the stream.  Two calls, so that a call may still fail in between and leave the caller's outputs untouched (the JPEG decode
+// does when the coded data turns out corrupt).
+int l3d_stage_host(l3d_ctx* c, HostBlock* in, int n_in, HostBlock* out, int n_out);
+int l3d_unstage_host(l3d_ctx* c, const HostBlock* out, int n_out, const char* what);
+
 // state of the per-view scoring sweep (l3d_pipeline.cu)
 struct SweepState {
     bool valid = false;
@@ -80,7 +96,7 @@ struct L3DUndistImage {
 struct UndistortState {
     std::vector<L3DUndistImage> h_imgs;
     std::vector<double> h_cols;                          // fisheye column tables, one per distinct (ir0, ir2)
-    DevBuf d_imgs, d_cols, d_src, d_dst, d_map_xy, d_map_frac;   // d_src .. d_map_frac: host-mode staging
+    DevBuf d_imgs, d_cols;
 };
 
 // per-image parameters of k_prepare_gray_u8 (l3d_image_prep.cu): source (width x height, 1 or 3 channels) -> grey out_w x out_h
@@ -96,7 +112,7 @@ struct L3DPrepImage {
 // buffers of the image preparation calls: not a pipeline stage, nothing else reads them
 struct ImagePrepState {
     std::vector<L3DPrepImage> h_imgs;
-    DevBuf d_imgs, d_src, d_dst;                         // d_src, d_dst: host-mode staging
+    DevBuf d_imgs;
 };
 
 // a Huffman table as k_jpeg_entropy reads it (l3d_jpeg.cu): a 9-bit lookahead (length << 8 | symbol, 0 for a longer code), then
@@ -132,13 +148,12 @@ struct JpegState {
     std::vector<L3DJpegSeg> h_segs;
     std::vector<L3DJpegTable> h_tabs;                    // 8 per image: DC, AC of each component of Y's scan
     std::vector<int> h_status;
-    DevBuf d_imgs, d_segs, d_tabs, d_bytes, d_coefs, d_status, d_dst;   // d_dst: host-mode staging
+    DevBuf d_imgs, d_segs, d_tabs, d_bytes, d_coefs, d_status;
 };
 
-// buffers of the triangulation and median-depth calls (l3d_triangulate.cu): not a pipeline stage either; the d_* of host mode
-// stage the caller's arrays
+// buffers of the median-depth call (l3d_triangulate.cu): not a pipeline stage either
 struct TriangulateState {
-    DevBuf d_ptr, d_cam, d_xy, d_P, d_X, d_valid, d_lptr, d_lpts, d_C, d_cnt, d_med, d_keys, d_keys2;
+    DevBuf d_keys, d_keys2;
 };
 
 // The results a context holds, each computed from the ones before it:
@@ -152,6 +167,7 @@ struct l3d_ctx {
     std::string err;
     long long launches = 0;
     DevBuf cub_tmp;                         // temporary storage of every cub call (all on `stream`, one at a time)
+    DevBuf stage_in, stage_out;             // host-mode copies of the caller's arrays (l3d_stage_host), free again when the call returns
 
     // views
     bool have_views = false;
@@ -173,7 +189,7 @@ struct l3d_ctx {
     long long total_rows = 0, pair_evals = 0;
     std::vector<L3DPairDev> h_pairs;
     std::vector<int4> h_units;              // k_match_topk work units: (pair, first source row, rows, 0)
-    DevBuf d_pairs, d_units, d_counts, d_recs, d_rowptr, d_csr, d_dense_dep, d_dense_ov, d_dense_jobs, d_arcs, d_basis, d_arcraw, d_arckeys, d_arckeys2, d_arcvals, d_arcvals2;
+    DevBuf d_pairs, d_units, d_counts, d_recs, d_rowptr, d_csr, d_dense_jobs, d_arcs, d_basis, d_arcraw, d_arckeys, d_arckeys2, d_arcvals, d_arcvals2;
     DevBuf d_rowwin;                        // row windows of the rows of [level1_first, level1_last) (k_row_windows, L3D_RW_WORDS words per row)
     int level1_first = 0, level1_last = 0;  // the pairs whose level-1 tables, bases and row windows the context holds (its own last match call)
 

@@ -3,7 +3,8 @@
 // over a batch of images; and the two C-ABI entry points declared in include/l3d_capi.h.  The arithmetic contract is DESIGN.md §4b;
 // tests/image_prep_model.py restates it.
 //
-// None of these calls belongs to the pipeline: they never drop a stage and touch only the buffers of ImagePrepState.
+// None of these calls belongs to the pipeline: they never drop a stage and touch only the buffers of ImagePrepState and, in host
+// mode, the context's staging pair.
 #include "l3d_ctx.cuh"
 #include "../../include/line3d_io.h"   // preparedImageSize: the one rounding of the prepared size (csrc/line3d_bin.cc)
 
@@ -171,29 +172,21 @@ int l3d_prepare_gray_u8(l3d_ctx* c, int n, const l3d_image_prep_desc* descs, int
     cudaSetDevice(c->device);
     ImagePrepState& s = c->prep;
     int rc;
-    size_t in_bytes = 0, out_bytes = 0;     // host mode: packed copies of every image on the device
+    std::vector<HostBlock> in, out;         // host mode: every source and output
     if (!on_device) {
         for (int i = 0; i < n; ++i) {
-            in_bytes += (size_t)descs[i].width * descs[i].channels * descs[i].height;
-            out_bytes += (size_t)descs[i].out_width * descs[i].out_height;
+            const l3d_image_prep_desc& u = descs[i];
+            in.push_back({u.src, (size_t)u.src_pitch, (size_t)u.width * u.channels, (size_t)u.height});
+            out.push_back({u.dst, (size_t)u.dst_pitch, (size_t)u.out_width, (size_t)u.out_height});
         }
-        L3D_RESERVE(s.d_src, in_bytes, "image preparation source staging");
-        L3D_RESERVE(s.d_dst, out_bytes, "image preparation output staging");
+        if ((rc = l3d_stage_host(c, in.data(), n, out.data(), n))) return rc;
     }
     s.h_imgs.resize(n);
     long long tiles = 0;
-    size_t in_off = 0, out_off = 0;
     for (int i = 0; i < n; ++i) {
         const l3d_image_prep_desc& u = descs[i];
         if (on_device) s.h_imgs[i] = pr_image(u, u.src, u.src_pitch, u.dst, u.dst_pitch);
-        else {
-            const long long row = (long long)u.width * u.channels;
-            unsigned char* src = (unsigned char*)s.d_src.p + in_off;
-            L3D_CUDA(c, cudaMemcpy2DAsync(src, row, u.src, u.src_pitch, row, u.height, cudaMemcpyHostToDevice, c->stream), "upload image");
-            s.h_imgs[i] = pr_image(u, src, row, (unsigned char*)s.d_dst.p + out_off, u.out_width);
-            in_off += (size_t)row * u.height;
-            out_off += (size_t)u.out_width * u.out_height;
-        }
+        else s.h_imgs[i] = pr_image(u, (const unsigned char*)in[i].dev, (long long)in[i].row_bytes, (unsigned char*)out[i].dev, (long long)out[i].row_bytes);
         s.h_imgs[i].tile0 = tiles;
         tiles += (long long)s.h_imgs[i].tiles_x * ((u.out_height + PR_TH - 1) / PR_TH);
     }
@@ -204,16 +197,7 @@ int l3d_prepare_gray_u8(l3d_ctx* c, int n, const l3d_image_prep_desc* descs, int
     k_prepare_gray_u8<<<(unsigned int)tiles, PR_TW, 0, c->stream>>>((const L3DPrepImage*)s.d_imgs.p, n);
     ++c->launches;
     L3D_CUDA(c, cudaGetLastError(), "k_prepare_gray_u8");
-    if (!on_device) {
-        out_off = 0;
-        for (int i = 0; i < n; ++i) {
-            const l3d_image_prep_desc& u = descs[i];
-            L3D_CUDA(c, cudaMemcpy2DAsync(u.dst, u.dst_pitch, (const unsigned char*)s.d_dst.p + out_off, u.out_width, u.out_width, u.out_height,
-                                          cudaMemcpyDeviceToHost, c->stream), "download image");
-            out_off += (size_t)u.out_width * u.out_height;
-        }
-        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "l3d_prepare_gray_u8");
-    }
+    if (!on_device && (rc = l3d_unstage_host(c, out.data(), n, "l3d_prepare_gray_u8"))) return rc;
     return L3D_OK;
 }
 

@@ -6,7 +6,8 @@
 //   k_jpeg_idct     one thread per 8x8 block that holds image pixels: dequantisation and the accurate integer IDCT as OpenCV's
 //                   libjpeg-turbo computes it on x86 (its SIMD jsimd_idct_islow: 16-bit lanes, saturating packs), each pixel stored
 //                   once at its place after the EXIF orientation.
-// The arithmetic contract is DESIGN.md §4c; tests/jpeg_model.py restates it.  Not a pipeline stage: only JpegState's buffers change.
+// The arithmetic contract is DESIGN.md §4c; tests/jpeg_model.py restates it.  Not a pipeline stage: only JpegState's buffers and, in host
+// mode, the context's staging pair change.
 #include "l3d_ctx.cuh"
 #include "l3d_jpeg.h"
 
@@ -295,8 +296,8 @@ extern "C" int l3d_decode_jpeg_gray_u8(l3d_ctx* c, int n, const l3d_jpeg_desc* d
     cudaSetDevice(c->device);
     JpegState& s = c->jpeg;
     int rc;
-    // sizes: Y's scan bytes, Y's coded blocks, the blocks with pixels, segments, host-mode output
-    size_t bytes = 0, out_bytes = 0;
+    // sizes: Y's scan bytes, Y's coded blocks, the blocks with pixels, segments
+    size_t bytes = 0;
     long long coef_blocks = 0, tiles = 0;
     size_t nseg = 0;
     for (int i = 0; i < n; ++i) {
@@ -305,18 +306,21 @@ extern "C" int l3d_decode_jpeg_gray_u8(l3d_ctx* c, int n, const l3d_jpeg_desc* d
         coef_blocks += (long long)h.yblocks_x * h.yblocks_y;
         tiles += (long long)((h.width + 7) / 8) * ((h.height + 7) / 8);
         nseg += h.segs.size();
-        if (!on_device) out_bytes += (size_t)h.out_width * h.out_height;
     }
     if (nseg > (size_t)INT_MAX || (tiles + JP_IDCT_THREADS - 1) / JP_IDCT_THREADS >= (1ll << 31))
         return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_decode_jpeg_gray_u8: too many segments or blocks in one call");
     L3D_RESERVE(s.d_bytes, bytes, "JPEG data staging");
     L3D_RESERVE(s.d_coefs, (size_t)coef_blocks * 128, "JPEG coefficients");
     L3D_RESERVE(s.d_status, sizeof(int) * (size_t)n, "JPEG status");
-    if (!on_device) L3D_RESERVE(s.d_dst, out_bytes, "JPEG output staging");
+    std::vector<HostBlock> out;             // host mode: every output
+    if (!on_device) {
+        for (int i = 0; i < n; ++i) out.push_back({descs[i].dst, (size_t)descs[i].dst_pitch, (size_t)descs[i].out_width, (size_t)descs[i].out_height});
+        if ((rc = l3d_stage_host(c, nullptr, 0, out.data(), n))) return rc;
+    }
     s.h_imgs.assign(n, L3DJpegImage());
     s.h_tabs.resize((size_t)8 * n);
     s.h_segs.clear();
-    size_t boff = 0, ooff = 0;
+    size_t boff = 0;
     long long coef0 = 0, tile0 = 0;
     for (int i = 0; i < n; ++i) {
         const L3DJpegHeader& h = hdr[i];
@@ -334,7 +338,7 @@ extern "C" int l3d_decode_jpeg_gray_u8(l3d_ctx* c, int n, const l3d_jpeg_desc* d
         }
         boff += (size_t)len;
         if (on_device) { d.dst = u.dst; d.dst_pitch = u.dst_pitch; }
-        else { d.dst = (unsigned char*)s.d_dst.p + ooff; d.dst_pitch = h.out_width; ooff += (size_t)h.out_width * h.out_height; }
+        else { d.dst = (unsigned char*)out[i].dev; d.dst_pitch = h.out_width; }
         d.coef0 = coef0; coef0 += (long long)h.yblocks_x * h.yblocks_y;
         d.tile0 = tile0;
         d.width = h.width; d.height = h.height; d.blocks_x = (h.width + 7) / 8;
@@ -379,15 +383,6 @@ extern "C" int l3d_decode_jpeg_gray_u8(l3d_ctx* c, int n, const l3d_jpeg_desc* d
             snprintf(buf, sizeof(buf), "l3d_decode_jpeg_gray_u8: image %d: %s", i, why);
             return l3d_fail(c, L3D_ERR_INVALID, buf);
         }
-    if (!on_device) {
-        ooff = 0;
-        for (int i = 0; i < n; ++i) {
-            const l3d_jpeg_desc& u = descs[i];
-            L3D_CUDA(c, cudaMemcpy2DAsync(u.dst, u.dst_pitch, (const unsigned char*)s.d_dst.p + ooff, u.out_width, u.out_width, u.out_height,
-                                          cudaMemcpyDeviceToHost, c->stream), "download image");
-            ooff += (size_t)u.out_width * u.out_height;
-        }
-        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "l3d_decode_jpeg_gray_u8");
-    }
+    if (!on_device && (rc = l3d_unstage_host(c, out.data(), n, "l3d_decode_jpeg_gray_u8"))) return rc;
     return L3D_OK;
 }

@@ -2,7 +2,7 @@
 // frontend (main_pix4d.cpp:34-70 linearHomTriangulation, 354-372 the loop over every point, 386-418 the median depth of every
 // camera) as the two C-ABI entries l3d_triangulate_points / l3d_median_depths of include/l3d_capi.h.  The arithmetic contract is
 // DESIGN.md §6b.  Like the undistortion calls, neither entry belongs to the pipeline: they never drop a stage and touch only the
-// buffers of TriangulateState.
+// buffers of TriangulateState and, in host mode, the context's staging pair.
 #include "l3d_cub.cuh"
 
 #include <cub/device/device_segmented_sort.cuh>
@@ -186,17 +186,6 @@ __global__ void k_pick_median(int n_cams, const long long* __restrict__ lptr, co
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-// host mode: the arrays are staged into `buf` (grown as needed) and the device address returned through `dev`
-template <class T>
-static int tr_stage(l3d_ctx* c, DevBuf& buf, const T* host, size_t count, const T*& dev, const char* what)
-{
-    int rc;
-    L3D_RESERVE(buf, sizeof(T) * count, what);
-    if (count) L3D_CUDA(c, cudaMemcpyAsync(buf.p, host, sizeof(T) * count, cudaMemcpyHostToDevice, c->stream), what);
-    dev = (const T*)buf.p;
-    return L3D_OK;
-}
-
 extern "C" {
 
 int l3d_triangulate_points(l3d_ctx* c, long long n_points, const int64_t* obs_ptr, const int32_t* obs_cam, const double* obs_xy, int n_cams,
@@ -207,7 +196,6 @@ int l3d_triangulate_points(l3d_ctx* c, long long n_points, const int64_t* obs_pt
         return l3d_fail(c, L3D_ERR_INVALID, "l3d_triangulate_points: bad arguments");
     if (n_points == 0) return L3D_OK;
     cudaSetDevice(c->device);
-    TriangulateState& s = c->tri;
     int rc;
     const long long* ptr = (const long long*)obs_ptr;
     const int32_t* cam = obs_cam;
@@ -215,6 +203,7 @@ int l3d_triangulate_points(l3d_ctx* c, long long n_points, const int64_t* obs_pt
     const double* Pd = P;
     double* X = X_out;
     int32_t* valid = valid_out;
+    HostBlock out[2] = {host_array(X_out, 3 * sizeof(double) * (size_t)n_points), host_array(valid_out, sizeof(int32_t) * (size_t)n_points)};
     if (!on_device) {       // host arrays are checked here; on the device an unknown camera makes its point invalid
         if (obs_ptr[0] != 0) return l3d_fail(c, L3D_ERR_INVALID, "l3d_triangulate_points: obs_ptr[0] must be 0");
         for (long long i = 0; i < n_points; ++i)
@@ -223,13 +212,11 @@ int l3d_triangulate_points(l3d_ctx* c, long long n_points, const int64_t* obs_pt
         if (n_obs && (!obs_cam || !obs_xy)) return l3d_fail(c, L3D_ERR_INVALID, "l3d_triangulate_points: null observation arrays");
         for (long long o = 0; o < n_obs; ++o)
             if (obs_cam[o] < 0 || obs_cam[o] >= n_cams) return l3d_fail(c, L3D_ERR_INVALID, "l3d_triangulate_points: observation of an unknown camera");
-        if ((rc = tr_stage(c, s.d_ptr, (const long long*)obs_ptr, (size_t)n_points + 1, ptr, "triangulation CSR"))) return rc;
-        if ((rc = tr_stage(c, s.d_cam, obs_cam, (size_t)n_obs, cam, "triangulation cameras"))) return rc;
-        if ((rc = tr_stage(c, s.d_xy, obs_xy, 2 * (size_t)n_obs, xy, "triangulation observations"))) return rc;
-        if ((rc = tr_stage(c, s.d_P, P, 12 * (size_t)n_cams, Pd, "triangulation projections"))) return rc;
-        L3D_RESERVE(s.d_X, 3 * sizeof(double) * (size_t)n_points, "triangulated points");
-        L3D_RESERVE(s.d_valid, sizeof(int32_t) * (size_t)n_points, "triangulation flags");
-        X = (double*)s.d_X.p; valid = (int32_t*)s.d_valid.p;
+        HostBlock in[4] = {host_array(obs_ptr, sizeof(long long) * ((size_t)n_points + 1)), host_array(obs_cam, sizeof(int32_t) * (size_t)n_obs),
+                           host_array(obs_xy, 2 * sizeof(double) * (size_t)n_obs), host_array(P, 12 * sizeof(double) * (size_t)n_cams)};
+        if ((rc = l3d_stage_host(c, in, 4, out, 2))) return rc;
+        ptr = (const long long*)in[0].dev; cam = (const int32_t*)in[1].dev; xy = (const double*)in[2].dev; Pd = (const double*)in[3].dev;
+        X = (double*)out[0].dev; valid = (int32_t*)out[1].dev;
     }
     const size_t smem = 12 * sizeof(double) * (size_t)n_cams;
     const int staged = n_cams > 0 && smem <= TR_SMEM_MAX;
@@ -244,11 +231,7 @@ int l3d_triangulate_points(l3d_ctx* c, long long n_points, const int64_t* obs_pt
     k_triangulate<<<(unsigned)blocks, TR_THREADS, staged ? smem : 0, c->stream>>>(n_points, ptr, cam, xy, n_cams, Pd, staged, X, valid);
     ++c->launches;
     L3D_CUDA(c, cudaGetLastError(), "k_triangulate");
-    if (!on_device) {
-        L3D_CUDA(c, cudaMemcpyAsync(X_out, X, 3 * sizeof(double) * (size_t)n_points, cudaMemcpyDeviceToHost, c->stream), "download points");
-        L3D_CUDA(c, cudaMemcpyAsync(valid_out, valid, sizeof(int32_t) * (size_t)n_points, cudaMemcpyDeviceToHost, c->stream), "download flags");
-        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "l3d_triangulate_points");
-    }
+    if (!on_device && (rc = l3d_unstage_host(c, out, 2, "l3d_triangulate_points"))) return rc;
     return L3D_OK;
 }
 
@@ -269,6 +252,7 @@ int l3d_median_depths(l3d_ctx* c, int n_cams, const int64_t* list_ptr, const int
     const int32_t* vd = valid;
     int32_t* cnt = count_out;
     float* med = median_out;
+    HostBlock out[2] = {host_array(count_out, sizeof(int32_t) * (size_t)n_cams), host_array(median_out, sizeof(float) * (size_t)n_cams)};
     if (!on_device) {
         if (list_ptr[0] != 0) return l3d_fail(c, L3D_ERR_INVALID, "l3d_median_depths: list_ptr[0] must be 0");
         for (int i = 0; i < n_cams; ++i)
@@ -277,14 +261,13 @@ int l3d_median_depths(l3d_ctx* c, int n_cams, const int64_t* list_ptr, const int
         if (total && !list_pts) return l3d_fail(c, L3D_ERR_INVALID, "l3d_median_depths: null point list");
         for (long long e = 0; e < total; ++e)
             if (list_pts[e] < 0 || list_pts[e] >= n_points) return l3d_fail(c, L3D_ERR_INVALID, "l3d_median_depths: point id out of range");
-        if ((rc = tr_stage(c, s.d_lptr, (const long long*)list_ptr, (size_t)n_cams + 1, lptr, "median lists CSR"))) return rc;
-        if ((rc = tr_stage(c, s.d_lpts, list_pts, (size_t)total, lpts, "median lists"))) return rc;
-        if ((rc = tr_stage(c, s.d_X, X, 3 * (size_t)n_points, Xd, "median points"))) return rc;
-        if ((rc = tr_stage(c, s.d_valid, valid, (size_t)n_points, vd, "median flags"))) return rc;
-        if ((rc = tr_stage(c, s.d_C, C, 3 * (size_t)n_cams, Cd, "median centres"))) return rc;
-        L3D_RESERVE(s.d_cnt, sizeof(int32_t) * (size_t)n_cams, "median counts");
-        L3D_RESERVE(s.d_med, sizeof(float) * (size_t)n_cams, "medians");
-        cnt = (int32_t*)s.d_cnt.p; med = (float*)s.d_med.p;
+        HostBlock in[5] = {host_array(list_ptr, sizeof(long long) * ((size_t)n_cams + 1)), host_array(list_pts, sizeof(int32_t) * (size_t)total),
+                           host_array(X, 3 * sizeof(double) * (size_t)n_points), host_array(valid, sizeof(int32_t) * (size_t)n_points),
+                           host_array(C, 3 * sizeof(double) * (size_t)n_cams)};
+        if ((rc = l3d_stage_host(c, in, 5, out, 2))) return rc;
+        lptr = (const long long*)in[0].dev; lpts = (const int32_t*)in[1].dev; Xd = (const double*)in[2].dev; vd = (const int32_t*)in[3].dev;
+        Cd = (const double*)in[4].dev;
+        cnt = (int32_t*)out[0].dev; med = (float*)out[1].dev;
     } else {
         L3D_CUDA(c, cudaMemcpyAsync(&total, list_ptr + n_cams, sizeof(long long), cudaMemcpyDeviceToHost, c->stream), "list length");
         L3D_CUDA(c, cudaStreamSynchronize(c->stream), "list length");
@@ -306,11 +289,7 @@ int l3d_median_depths(l3d_ctx* c, int n_cams, const int64_t* list_ptr, const int
     k_pick_median<<<(unsigned)((n_cams + 127) / 128), 128, 0, c->stream>>>(n_cams, lptr, (const unsigned int*)s.d_keys2.p, cnt, med);
     ++c->launches;
     L3D_CUDA(c, cudaGetLastError(), "k_pick_median");
-    if (!on_device) {
-        L3D_CUDA(c, cudaMemcpyAsync(count_out, cnt, sizeof(int32_t) * (size_t)n_cams, cudaMemcpyDeviceToHost, c->stream), "download counts");
-        L3D_CUDA(c, cudaMemcpyAsync(median_out, med, sizeof(float) * (size_t)n_cams, cudaMemcpyDeviceToHost, c->stream), "download medians");
-        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "l3d_median_depths");
-    }
+    if (!on_device && (rc = l3d_unstage_host(c, out, 2, "l3d_median_depths"))) return rc;
     return L3D_OK;
 }
 

@@ -3,7 +3,8 @@
 // C-ABI entry points declared in include/l3d_capi.h.  Two lens models: OpenCV's standard one with up to 8 coefficients (radtan) and
 // cv::fisheye's.  The output may have its own camera matrix and size (OpenCV's newCameraMatrix / newImageSize).  The arithmetic contract is DESIGN.md §4a; tests/undistort_model.py and tests/lens_model.py restate it.
 //
-// None of these calls belongs to the pipeline: they never drop a stage and touch only the buffers of UndistortState.
+// None of these calls belongs to the pipeline: they never drop a stage and touch only the buffers of UndistortState and, in host
+// mode, the context's staging pair.
 #include "l3d_ctx.cuh"
 
 #include <algorithm>
@@ -301,28 +302,20 @@ int l3d_undistort_u8(l3d_ctx* c, int n, const l3d_undistort_desc* descs, int on_
     cudaSetDevice(c->device);
     UndistortState& s = c->undist;
     int rc;
-    size_t staged_src = 0, staged_dst = 0;  // host mode: packed copies of every source and output on the device
+    std::vector<HostBlock> in, out;         // host mode: every source and output
     if (!on_device) {
         for (int i = 0; i < n; ++i) {
-            staged_src += (size_t)descs[i].width * descs[i].channels * descs[i].height;
-            staged_dst += (size_t)ud_out_width(descs[i]) * descs[i].channels * ud_out_height(descs[i]);
+            const l3d_undistort_desc& u = descs[i];
+            in.push_back({u.src, (size_t)u.src_pitch, (size_t)u.width * u.channels, (size_t)u.height});
+            out.push_back({u.dst, (size_t)u.dst_pitch, (size_t)ud_out_width(u) * u.channels, (size_t)ud_out_height(u)});
         }
-        L3D_RESERVE(s.d_src, staged_src, "undistort source staging");
-        L3D_RESERVE(s.d_dst, staged_dst, "undistort output staging");
+        if ((rc = l3d_stage_host(c, in.data(), n, out.data(), n))) return rc;
     }
     s.h_imgs.resize(n);
-    size_t off = 0, off_dst = 0;
     for (int i = 0; i < n; ++i) {
         const l3d_undistort_desc& u = descs[i];
-        const long long row = (long long)u.width * u.channels, out_row = (long long)ud_out_width(u) * u.channels;
         if (on_device) s.h_imgs[i] = ud_image(u, u.src, u.src_pitch, u.dst, u.dst_pitch);
-        else {
-            unsigned char* src = (unsigned char*)s.d_src.p + off;
-            L3D_CUDA(c, cudaMemcpy2DAsync(src, row, u.src, u.src_pitch, row, u.height, cudaMemcpyHostToDevice, c->stream), "upload image");
-            s.h_imgs[i] = ud_image(u, src, row, (unsigned char*)s.d_dst.p + off_dst, out_row);
-            off += (size_t)row * u.height;
-            off_dst += (size_t)out_row * ud_out_height(u);
-        }
+        else s.h_imgs[i] = ud_image(u, (const unsigned char*)in[i].dev, (long long)in[i].row_bytes, (unsigned char*)out[i].dev, (long long)out[i].row_bytes);
     }
     // the images grouped by lens kind: one grid per kind, each numbering its tiles from 0
     std::stable_sort(s.h_imgs.begin(), s.h_imgs.end(), [](const L3DUndistImage& a, const L3DUndistImage& b) { return a.kind < b.kind; });
@@ -348,17 +341,7 @@ int l3d_undistort_u8(l3d_ctx* c, int n, const l3d_undistort_desc* descs, int on_
         ++c->launches;
         L3D_CUDA(c, cudaGetLastError(), "k_undistort_u8");
     }
-    if (!on_device) {
-        off = 0;
-        for (int i = 0; i < n; ++i) {
-            const l3d_undistort_desc& u = descs[i];
-            const size_t row = (size_t)ud_out_width(u) * u.channels;
-            L3D_CUDA(c, cudaMemcpy2DAsync(u.dst, u.dst_pitch, (const unsigned char*)s.d_dst.p + off, row, row, ud_out_height(u), cudaMemcpyDeviceToHost,
-                                          c->stream), "download image");
-            off += row * ud_out_height(u);
-        }
-        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "l3d_undistort_u8");
-    }
+    if (!on_device && (rc = l3d_unstage_host(c, out.data(), n, "l3d_undistort_u8"))) return rc;
     return L3D_OK;
 }
 
@@ -370,26 +353,21 @@ int l3d_undistort_map(l3d_ctx* c, const l3d_undistort_desc* desc, int16_t* map_x
     int rc = ud_check(c, *desc, false, true, "l3d_undistort_map");
     if (rc) return rc;
     cudaSetDevice(c->device);
-    UndistortState& s = c->undist;
     const size_t px = (size_t)ud_out_width(*desc) * ud_out_height(*desc);
     short2* xy = (short2*)map_xy; unsigned short* fr = map_frac;
+    HostBlock out[2] = {host_array(map_xy, 4 * px), host_array(map_frac, 2 * px)};
     if (!on_device) {
-        L3D_RESERVE(s.d_map_xy, 4 * px, "undistort map");
-        L3D_RESERVE(s.d_map_frac, 2 * px, "undistort map fractions");
-        xy = (short2*)s.d_map_xy.p; fr = (unsigned short*)s.d_map_frac.p;
+        if ((rc = l3d_stage_host(c, nullptr, 0, out, 2))) return rc;
+        xy = (short2*)out[0].dev; fr = (unsigned short*)out[1].dev;
     }
     L3DUndistImage d = ud_image(*desc, nullptr, 0, nullptr, 0);
-    if ((rc = ud_column_tables(c, s, &d, 1))) return rc;
+    if ((rc = ud_column_tables(c, c->undist, &d, 1))) return rc;
     void (*const kernels[UD_KINDS])(L3DUndistImage, short2*, unsigned short*) = {k_undistort_map<UD_RADTAN>, k_undistort_map<UD_RATIONAL>,
                                                                                  k_undistort_map<UD_FISHEYE>};
     kernels[d.kind]<<<ud_grid(*desc), UD_TW, 0, c->stream>>>(d, xy, fr);
     ++c->launches;
     L3D_CUDA(c, cudaGetLastError(), "k_undistort_map");
-    if (!on_device) {
-        L3D_CUDA(c, cudaMemcpyAsync(map_xy, xy, 4 * px, cudaMemcpyDeviceToHost, c->stream), "download map");
-        L3D_CUDA(c, cudaMemcpyAsync(map_frac, fr, 2 * px, cudaMemcpyDeviceToHost, c->stream), "download map fractions");
-        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "l3d_undistort_map");
-    }
+    if (!on_device && (rc = l3d_unstage_host(c, out, 2, "l3d_undistort_map"))) return rc;
     return L3D_OK;
 }
 
@@ -401,31 +379,22 @@ int l3d_remap_u8(l3d_ctx* c, const l3d_undistort_desc* desc, const int16_t* map_
     int rc = ud_check(c, *desc, true, false, "l3d_remap_u8");
     if (rc) return rc;
     cudaSetDevice(c->device);
-    UndistortState& s = c->undist;
     const l3d_undistort_desc& u = *desc;
     const size_t px = (size_t)ud_out_width(u) * ud_out_height(u), row = (size_t)u.width * u.channels, out_row = (size_t)ud_out_width(u) * u.channels;
     L3DUndistImage d = ud_image(u, u.src, u.src_pitch, u.dst, u.dst_pitch);
     const short2* xy = (const short2*)map_xy; const unsigned short* fr = map_frac;
+    HostBlock out[1] = {{u.dst, (size_t)u.dst_pitch, out_row, (size_t)ud_out_height(u)}};
     if (!on_device) {
-        L3D_RESERVE(s.d_src, row * u.height, "remap source staging");
-        L3D_RESERVE(s.d_dst, out_row * ud_out_height(u), "remap output staging");
-        L3D_RESERVE(s.d_map_xy, 4 * px, "remap map");
-        L3D_RESERVE(s.d_map_frac, 2 * px, "remap map fractions");
-        L3D_CUDA(c, cudaMemcpy2DAsync(s.d_src.p, row, u.src, u.src_pitch, row, u.height, cudaMemcpyHostToDevice, c->stream), "upload image");
-        L3D_CUDA(c, cudaMemcpyAsync(s.d_map_xy.p, map_xy, 4 * px, cudaMemcpyHostToDevice, c->stream), "upload map");
-        L3D_CUDA(c, cudaMemcpyAsync(s.d_map_frac.p, map_frac, 2 * px, cudaMemcpyHostToDevice, c->stream), "upload map fractions");
-        d.src = (const unsigned char*)s.d_src.p; d.dst = (unsigned char*)s.d_dst.p; d.src_pitch = (long long)row; d.dst_pitch = (long long)out_row;
-        xy = (const short2*)s.d_map_xy.p; fr = (const unsigned short*)s.d_map_frac.p;
+        HostBlock in[3] = {{u.src, (size_t)u.src_pitch, row, (size_t)u.height}, host_array(map_xy, 4 * px), host_array(map_frac, 2 * px)};
+        if ((rc = l3d_stage_host(c, in, 3, out, 1))) return rc;
+        d.src = (const unsigned char*)in[0].dev; d.dst = (unsigned char*)out[0].dev; d.src_pitch = (long long)row; d.dst_pitch = (long long)out_row;
+        xy = (const short2*)in[1].dev; fr = (const unsigned short*)in[2].dev;
     }
     if (u.channels == 3) k_remap_u8<3><<<ud_grid(u), UD_TW, 0, c->stream>>>(d, xy, fr);
     else k_remap_u8<1><<<ud_grid(u), UD_TW, 0, c->stream>>>(d, xy, fr);
     ++c->launches;
     L3D_CUDA(c, cudaGetLastError(), "k_remap_u8");
-    if (!on_device) {
-        L3D_CUDA(c, cudaMemcpy2DAsync(u.dst, u.dst_pitch, s.d_dst.p, out_row, out_row, ud_out_height(u), cudaMemcpyDeviceToHost, c->stream),
-                 "download image");
-        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "l3d_remap_u8");
-    }
+    if (!on_device && (rc = l3d_unstage_host(c, out, 1, "l3d_remap_u8"))) return rc;
     return L3D_OK;
 }
 
