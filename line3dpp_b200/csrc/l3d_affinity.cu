@@ -674,10 +674,11 @@ __global__ void __launch_bounds__(256) k_rdd_symmetrise(long long nnz, const flo
     out[y] = t >= 0 ? fminf(P[y], P[t]) : P[y];
 }
 
-// the diffusion proper on DEVICE edge arrays d_ei/d_ej/d_ew (in_rdd_bufs: they already are R.d_ei/ej/ew); symmetrise: performRDD's
-// min(w12, w21) applied before the download.  Output in row-sorted (i, j) order - the order std::map iterates in (line3D.cc:2063-2071).
+// the diffusion proper on DEVICE edge arrays d_ei/d_ej/d_ew; symmetrise: performRDD's min(w12, w21) applied to the result.  Sets the
+// dev of res[0], res[1], res[2] to the result's weights, rows and columns, in row-sorted (i, j) order - the order std::map iterates in
+// (line3D.cc:2063-2071); the caller downloads them.  timing (optional): two events, recorded around the `iters` diffusion iterations.
 static int rdd_core(l3d_ctx* c, int n, long long nnz, const int* d_ei, const int* d_ej, const float* d_ew, int iters, bool symmetrise,
-                    int* out_i, int* out_j, float* out_w, float* kernel_ms)
+                    HostBlock res[3], ScopedEvent* timing)
 {
     RddState& R = c->rdd;
     int rc;
@@ -728,10 +729,9 @@ static int rdd_core(l3d_ctx* c, int n, long long nnz, const int* d_ei, const int
     const unsigned int nbn = (unsigned int)((4ll * n + 255) / 256);
     auto normalize = [&](float* Pbuf) { k_rdd_normalize_q<<<nbn, 256, 0, st>>>(n, (const int*)R.d_rowptr.p, (const int*)R.d_rp4.p, Pbuf); };
     normalize((float*)R.d_Pp.p);
-    ScopedEvent e0, e1;
-    if (kernel_ms) {
-        if ((rc = e0.create(c)) || (rc = e1.create(c))) return rc;
-        cudaEventRecord(e0.e, st);
+    if (timing) {
+        if ((rc = timing[0].create(c)) || (rc = timing[1].create(c))) return rc;
+        cudaEventRecord(timing[0].e, st);
     }
     float* P = (float*)R.d_Pp.p; float* Pn = (float*)R.d_Pnp.p;
     for (int it = 0; it < iters; ++it) {
@@ -739,21 +739,17 @@ static int rdd_core(l3d_ctx* c, int n, long long nnz, const int* d_ei, const int
         std::swap(P, Pn);
         if (it < iters - 1) normalize(P);       // no normalisation after the last step (cudawrapper.cu:751)
     }
-    if (kernel_ms) cudaEventRecord(e1.e, st);
+    if (timing) cudaEventRecord(timing[1].e, st);
     k_rdd_unpad<<<nb, 256, 0, st>>>(nnz, (const int*)R.d_prow.p, (const int*)R.d_rowptr.p, (const int*)R.d_rp4.p, P, (float*)R.d_P.p);
-    const float* result = (const float*)R.d_P.p;
+    res[0].dev = R.d_P.p;
     if (symmetrise) {
         k_rdd_symmetrise<<<nb, 256, 0, st>>>(nnz, (const float*)R.d_P.p, (const int*)R.d_tslot.p, (float*)R.d_Pn.p);
-        result = (const float*)R.d_Pn.p;
+        res[0].dev = R.d_Pn.p;
         ++c->launches;
     }
     c->launches += 9 + 16 + 10 + 2 * iters;
     L3D_CUDA(c, cudaGetLastError(), "rdd kernels");
-    L3D_CUDA(c, cudaMemcpyAsync(out_w, result, 4 * nnz, cudaMemcpyDeviceToHost, st), "rdd download");
-    L3D_CUDA(c, cudaMemcpyAsync(out_i, R.d_prow.p, 4 * nnz, cudaMemcpyDeviceToHost, st), "rdd download");
-    L3D_CUDA(c, cudaMemcpyAsync(out_j, R.d_pcol.p, 4 * nnz, cudaMemcpyDeviceToHost, st), "rdd download");
-    L3D_CUDA(c, cudaStreamSynchronize(st), "rdd");
-    if (kernel_ms) cudaEventElapsedTime(kernel_ms, e0.e, e1.e);
+    res[1].dev = R.d_prow.p; res[2].dev = R.d_pcol.p;
     return L3D_OK;
 }
 
@@ -764,13 +760,16 @@ int l3d_rdd(l3d_ctx* c, int n, long long nnz, const int* ei, const int* ej, cons
     if (nnz == 0) return L3D_OK;
     if (nnz >= (1ll << 31) - 2) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_rdd: more than 2^31 entries");
     cudaSetDevice(c->device);
-    RddState& R = c->rdd;
     int rc;
-    L3D_RESERVE(R.d_ei, 4 * nnz, "rdd i"); L3D_RESERVE(R.d_ej, 4 * nnz, "rdd j"); L3D_RESERVE(R.d_ew, 4 * nnz, "rdd w");
-    L3D_CUDA(c, cudaMemcpyAsync(R.d_ei.p, ei, 4 * nnz, cudaMemcpyHostToDevice, c->stream), "rdd upload");
-    L3D_CUDA(c, cudaMemcpyAsync(R.d_ej.p, ej, 4 * nnz, cudaMemcpyHostToDevice, c->stream), "rdd upload");
-    L3D_CUDA(c, cudaMemcpyAsync(R.d_ew.p, ew, 4 * nnz, cudaMemcpyHostToDevice, c->stream), "rdd upload");
-    return rdd_core(c, n, nnz, (const int*)R.d_ei.p, (const int*)R.d_ej.p, (const float*)R.d_ew.p, iters, false, out_i, out_j, out_w, kernel_ms);
+    HostBlock in[3] = {host_array(ei, 4 * nnz), host_array(ej, 4 * nnz), host_array(ew, 4 * nnz)};
+    HostBlock res[3] = {host_array(out_w, 4 * nnz), host_array(out_i, 4 * nnz), host_array(out_j, 4 * nnz)};
+    ScopedEvent timing[2];
+    if ((rc = l3d_stage_host(c, in, 3, nullptr, 0)) ||
+        (rc = rdd_core(c, n, nnz, (const int*)in[0].dev, (const int*)in[1].dev, (const float*)in[2].dev, iters, false, res, kernel_ms ? timing : nullptr)) ||
+        (rc = l3d_unstage_host(c, res, 3, "rdd")))
+        return rc;
+    if (kernel_ms) cudaEventElapsedTime(kernel_ms, timing[0].e, timing[1].e);
+    return L3D_OK;
 }
 
 // performRDD (line3D.cc:2026-2076) on the affinity matrix l3d_affinity_matrix left on the device: no download / re-upload of A_, the
@@ -785,8 +784,10 @@ long long l3d_rdd_affinity(l3d_ctx* c, int iters, int* out_i, int* out_j, float*
     if (nnz == 0 || nnz > cap) return nnz;
     if (nnz >= (1ll << 31) - 2) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_rdd_affinity: more than 2^31 entries");
     cudaSetDevice(c->device);
-    const int rc = rdd_core(c, (int)A.n_ids, nnz, (const int*)A.d_ei.p, (const int*)A.d_ej.p, (const float*)A.d_ew.p, iters, true, out_i, out_j, out_w, nullptr);
-    return rc < 0 ? rc : nnz;
+    int rc;
+    HostBlock res[3] = {host_array(out_w, 4 * nnz), host_array(out_i, 4 * nnz), host_array(out_j, 4 * nnz)};
+    if ((rc = rdd_core(c, (int)A.n_ids, nnz, (const int*)A.d_ei.p, (const int*)A.d_ej.p, (const float*)A.d_ew.p, iters, true, res, nullptr))) return rc;
+    return (rc = l3d_unstage_host(c, res, 3, "rdd")) ? rc : nnz;
 }
 
 // Stable ascending argsort of float keys on the device (the edge-weight sort of performClustering, clustering.cc:13-14:
@@ -799,17 +800,16 @@ int l3d_argsort_f32(l3d_ctx* c, long long n, const float* keys, unsigned int* pe
     cudaSetDevice(c->device);
     RddState& R = c->rdd;
     int rc;
-    L3D_RESERVE(R.d_ew, 4 * n, "sort keys"); L3D_RESERVE(R.d_ei, 4 * n, "sort keys"); L3D_RESERVE(R.d_idx, 4 * n, "sort idx"); L3D_RESERVE(R.d_idx2, 4 * n, "sort idx");
+    L3D_RESERVE(R.d_k2, 4 * n, "sort keys"); L3D_RESERVE(R.d_idx, 4 * n, "sort idx");
+    HostBlock in[1] = {host_array(keys, 4 * (size_t)n)}, out[1] = {host_array(perm_out, 4 * (size_t)n)};
+    if ((rc = l3d_stage_host(c, in, 1, out, 1))) return rc;
     cudaStream_t st = c->stream;
-    L3D_CUDA(c, cudaMemcpyAsync(R.d_ew.p, keys, 4 * (size_t)n, cudaMemcpyHostToDevice, st), "sort upload");
     k_iota<<<(unsigned int)((n + 255) / 256), 256, 0, st>>>(n, (unsigned int*)R.d_idx.p);
     if ((rc = l3d_cub(c, "argsort", [&](void* tmp, size_t& bytes) {
-             return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const float*)R.d_ew.p, (float*)R.d_ei.p, (const unsigned int*)R.d_idx.p, (unsigned int*)R.d_idx2.p, (int)n, 0, 32, st); })))
+             return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const float*)in[0].dev, (float*)R.d_k2.p, (const unsigned int*)R.d_idx.p, (unsigned int*)out[0].dev, (int)n, 0, 32, st); })))
         return rc;
     c->launches += 6;
-    L3D_CUDA(c, cudaMemcpyAsync(perm_out, R.d_idx2.p, 4 * (size_t)n, cudaMemcpyDeviceToHost, st), "sort download");
-    L3D_CUDA(c, cudaStreamSynchronize(st), "argsort");
-    return L3D_OK;
+    return l3d_unstage_host(c, out, 1, "argsort");
 }
 
 } // extern "C"

@@ -30,10 +30,11 @@ struct HostBlock {
 };
 inline HostBlock host_array(const void* p, size_t bytes) { return HostBlock{p, bytes, bytes, 1}; }
 
-// Host mode of the calls that are not pipeline stages: packs the `in` blocks into the context's stage_in and the `out` blocks into
-// its stage_out, uploads `in` on the context's stream and sets every block's dev.  l3d_unstage_host then downloads `out` and waits
-// for the stream.  Two calls, so that a call may still fail in between and leave the caller's outputs untouched (the JPEG decode
-// does when the coded data turns out corrupt).
+// Every caller's host array reaches the device here (host mode of the image, dense-matching and triangulation calls; the bundling,
+// diffusion and argsort calls): packs the `in` blocks into the context's stage_in and the `out` blocks into its stage_out, uploads
+// `in` on the context's stream and sets every block's dev.  l3d_unstage_host then downloads `out` from wherever its dev points and
+// waits for the stream.  Two calls, so that a call may still fail in between and leave the caller's outputs untouched (the JPEG
+// decode does when the coded data turns out corrupt).
 int l3d_stage_host(l3d_ctx* c, HostBlock* in, int n_in, HostBlock* out, int n_out);
 int l3d_unstage_host(l3d_ctx* c, const HostBlock* out, int n_out, const char* what);
 
@@ -68,12 +69,12 @@ struct CollinState {
 
 // device state of the line bundling (l3d_optimize.cu)
 struct OptState {
-    DevBuf d_p, d_pout, d_valid, d_resptr, d_rescam, d_resxy, d_obs, d_cams, d_x, d_xc, d_g, d_H, d_S, d_diag, d_free, d_part, d_tot;
+    DevBuf d_obs, d_x, d_xc, d_g, d_H, d_S, d_diag, d_free, d_part, d_tot;
 };
 
-// device buffers of the diffusion (l3d_affinity.cu)
+// device buffers of the diffusion (l3d_affinity.cu); d_idx and d_k2 are also the sort scratch of l3d_argsort_f32
 struct RddState {
-    DevBuf d_ei, d_ej, d_ew, d_krow, d_kcol, d_k2, d_idx, d_idx2, d_P, d_Pn, d_W, d_prow, d_pcol, d_wmaj, d_wmin, d_rowptr, d_colptr, d_tslot, d_len4, d_rp4, d_cp4,
+    DevBuf d_krow, d_kcol, d_k2, d_idx, d_idx2, d_P, d_Pn, d_W, d_prow, d_pcol, d_wmaj, d_wmin, d_rowptr, d_colptr, d_tslot, d_len4, d_rp4, d_cp4,
         d_Pp, d_Pnp, d_Wp, d_plan, d_dst;
 };
 

@@ -333,26 +333,23 @@ int l3d_optimize_lines(l3d_ctx* c, int num_lines, const double* p1p2, const long
     cudaSetDevice(c->device);
     OptState& O = c->opt;
     int rc;
-    L3D_RESERVE(O.d_p, 48ll * L, "opt lines"); L3D_RESERVE(O.d_pout, 48ll * L, "opt lines out"); L3D_RESERVE(O.d_valid, 4ll * L, "opt valid"); L3D_RESERVE(O.d_resptr, 8ll * (L + 1), "opt res ptr");
-    L3D_RESERVE(O.d_rescam, 4 * NR, "opt res cam"); L3D_RESERVE(O.d_resxy, 32 * NR, "opt res xy"); L3D_RESERVE(O.d_obs, (long long)sizeof(OptObs) * NR, "opt observations");
-    L3D_RESERVE(O.d_cams, 128ll * num_cams, "opt cameras"); L3D_RESERVE(O.d_x, 32ll * L, "opt x"); L3D_RESERVE(O.d_xc, 32ll * L, "opt x candidate"); L3D_RESERVE(O.d_g, 32ll * L, "opt gradient");
+    L3D_RESERVE(O.d_obs, (long long)sizeof(OptObs) * NR, "opt observations");
+    L3D_RESERVE(O.d_x, 32ll * L, "opt x"); L3D_RESERVE(O.d_xc, 32ll * L, "opt x candidate"); L3D_RESERVE(O.d_g, 32ll * L, "opt gradient");
     L3D_RESERVE(O.d_H, 80ll * L, "opt JtJ"); L3D_RESERVE(O.d_S, 32ll * L, "opt scaling"); L3D_RESERVE(O.d_diag, 32ll * L, "opt diagonal"); L3D_RESERVE(O.d_free, 4ll * L, "opt free flags");
     L3D_RESERVE(O.d_part, 48ll * L, "opt partial sums"); L3D_RESERVE(O.d_tot, 64, "opt totals");
+    // without residuals, res_cam, res_xy and cams may be null: their blocks are empty and not uploaded
+    HostBlock in[5] = {host_array(p1p2, 48ull * L), host_array(res_ptr, 8ull * (L + 1)), host_array(res_cam, 4ull * NR), host_array(res_xy, 32ull * NR),
+                       host_array(cams, NR ? 128ull * num_cams : 0)};
+    HostBlock out[2] = {host_array(p1p2_out, 48ull * L), host_array(valid_out, 4ull * L)};
+    if ((rc = l3d_stage_host(c, in, 5, out, 2))) return rc;
     cudaStream_t st = c->stream;
-    L3D_CUDA(c, cudaMemcpyAsync(O.d_p.p, p1p2, 48ull * L, cudaMemcpyHostToDevice, st), "opt upload");
-    L3D_CUDA(c, cudaMemcpyAsync(O.d_resptr.p, res_ptr, 8ull * (L + 1), cudaMemcpyHostToDevice, st), "opt upload");
-    if (NR) {
-        L3D_CUDA(c, cudaMemcpyAsync(O.d_rescam.p, res_cam, 4ull * NR, cudaMemcpyHostToDevice, st), "opt upload");
-        L3D_CUDA(c, cudaMemcpyAsync(O.d_resxy.p, res_xy, 32ull * NR, cudaMemcpyHostToDevice, st), "opt upload");
-        L3D_CUDA(c, cudaMemcpyAsync(O.d_cams.p, cams, 128ull * num_cams, cudaMemcpyHostToDevice, st), "opt upload");
-    }
     const unsigned int nbl = (unsigned int)((L + 127) / 128);
     long long launches = 0;
-    if (NR) { k_opt_obs<<<(unsigned int)((NR + 127) / 128), 128, 0, st>>>(NR, (const double*)O.d_resxy.p, (OptObs*)O.d_obs.p); ++launches; }
-    k_opt_init<<<nbl, 128, 0, st>>>(L, (const double*)O.d_p.p, (const long long*)O.d_resptr.p, (double*)O.d_x.p, (int*)O.d_free.p); ++launches;
+    if (NR) { k_opt_obs<<<(unsigned int)((NR + 127) / 128), 128, 0, st>>>(NR, (const double*)in[3].dev, (OptObs*)O.d_obs.p); ++launches; }
+    k_opt_init<<<nbl, 128, 0, st>>>(L, (const double*)in[0].dev, (const long long*)in[1].dev, (double*)O.d_x.p, (int*)O.d_free.p); ++launches;
     const int* isfree = (const int*)O.d_free.p;
-    const OptCam* dcams = (const OptCam*)O.d_cams.p; const OptObs* dobs = (const OptObs*)O.d_obs.p;
-    const long long* dptr = (const long long*)O.d_resptr.p; const int* dcam = (const int*)O.d_rescam.p;
+    const OptCam* dcams = (const OptCam*)in[4].dev; const OptObs* dobs = (const OptObs*)O.d_obs.p;
+    const long long* dptr = (const long long*)in[1].dev; const int* dcam = (const int*)in[2].dev;
     double* x = (double*)O.d_x.p; double* xc = (double*)O.d_xc.p; double* part = (double*)O.d_part.p; double* tot = (double*)O.d_tot.p;
     double h[8];
     auto totals = [&](int nterms, unsigned int maxmask) -> int {
@@ -418,11 +415,9 @@ int l3d_optimize_lines(l3d_ctx* c, int num_lines, const double* p1p2, const long
             }
         }
     }
-    k_opt_finish<<<nbl, 128, 0, st>>>(L, x, (const double*)O.d_p.p, (double*)O.d_pout.p, (int*)O.d_valid.p); ++launches;
+    k_opt_finish<<<nbl, 128, 0, st>>>(L, x, (const double*)in[0].dev, (double*)out[0].dev, (int*)out[1].dev); ++launches;
     L3D_CUDA(c, cudaGetLastError(), "opt kernels");
-    L3D_CUDA(c, cudaMemcpyAsync(p1p2_out, O.d_pout.p, 48ull * L, cudaMemcpyDeviceToHost, st), "opt download");
-    L3D_CUDA(c, cudaMemcpyAsync(valid_out, O.d_valid.p, 4ull * L, cudaMemcpyDeviceToHost, st), "opt download");
-    L3D_CUDA(c, cudaStreamSynchronize(st), "opt");
+    if ((rc = l3d_unstage_host(c, out, 2, "opt"))) return rc;
     c->launches += launches;
     if (summary) { summary[0] = it; summary[1] = cost0; summary[2] = cost; summary[3] = term; summary[4] = nsucc; summary[6] = radius; summary[7] = (double)launches; }
     return L3D_OK;

@@ -1,7 +1,7 @@
-"""The host-mode calls that are not pipeline stages share one pair of staging buffers per context.  One context runs undistortion,
-JPEG decoding, image preparation, remap, undistortion maps, dense matching, triangulation and median depths in host mode,
-interleaved, with sizes that grow and then shrink; every result must be byte for byte what the same call gives on a fresh context.
-A corrupt JPEG in the sequence must leave its host outputs untouched and the next call right."""
+"""The calls that take host arrays share one pair of staging buffers per context.  One context runs undistortion, JPEG decoding,
+image preparation, remap, undistortion maps, dense matching, triangulation and median depths in host mode, and the line bundling,
+the diffusion and the weight argsort, interleaved, with sizes that grow and then shrink; every result must be byte for byte what the
+same call gives on a fresh context.  A corrupt JPEG in the sequence must leave its host outputs untouched and the next call right."""
 import os
 
 import numpy as np
@@ -9,8 +9,11 @@ import pytest
 
 from line3dpp_b200 import capi, synth
 from tests import jpeg_model as jm
+from tests import nvm_util as nu
+from tests import rdd_model as rm
 from tests import tri_model as tm
 from tests import util
+from tests.test_sweep_paths_gpu import argsort_f32, tie_heavy_keys
 
 pytestmark = pytest.mark.gpu
 
@@ -71,15 +74,54 @@ def _steps(scene):
         q = tm.join_medians(tm.median_lists(ncam, n_points=n), tm.median_edges())
         steps.append(("median_depths", lambda c: c.median_depths(*q)))
 
+    before, _, opt_ptr, opt_res = nu.load_opt_pairs()
+    cams, shift = nu.optimizer_inputs(nu.load_inputs())
+    before = before + np.tile(shift, 2)
+
+    def optimize(n, max_iter):
+        ptr = opt_ptr[:n + 1]
+        res = opt_res[:ptr[-1]]
+        steps.append(("optimize_lines", lambda c: c.optimize_lines(before[:n], ptr, res[:, 0].astype(np.int32), res[:, 2:6], cams, max_iter)))
+
+    def optimize_without_residuals(n):
+        """res_cam, res_xy and cams are null while num_cams > 0: nothing of them is staged"""
+        p, ptr = np.ascontiguousarray(before[:n]), np.zeros(n + 1, np.int64)
+
+        def run(c):
+            out, valid, summ = np.zeros((n, 6)), np.zeros(n, np.int32), np.zeros(8)
+            c._chk(c.L.l3d_optimize_lines(c.h, n, capi._p(p), capi._p(ptr), None, None, len(cams), None, 10, capi._p(out), capi._p(valid),
+                                          capi._p(summ)), "l3d_optimize_lines")
+            return out, valid, summ
+        steps.append(("optimize_lines without residuals", run))
+
+    def rdd(name):
+        graph = rm.BUILDERS[name]()
+
+        def run(c):
+            oi, oj, ow, ms = c.rdd(*graph, 10)
+            assert ms > 0
+            return oi, oj, ow
+        steps.append(("rdd", run))
+
+    def argsort(n):
+        keys = tie_heavy_keys(n, n)
+
+        def run(c):
+            rc, perm = argsort_f32(c, keys)
+            assert rc == 0
+            return [perm]
+        steps.append(("argsort_f32", run))
+
     # small
     undistort(41, 57, 3); jpeg(photos[:1]); prepare(45, 61, 0, 32); remap(23, 37, 19, 29); undistort_map(57, 41, None); dense(0, 1)
-    triangulate(500, 4, 64); medians(20, 500)
+    triangulate(500, 4, 64); medians(20, 500); optimize(40, 250); rdd("tiny"); argsort(257)
     # large
     undistort(1080, 1920, 64); steps.append(("corrupt JPEG", None)); jpeg(photos); prepare(1200, 1600, 5, 1000); remap(1001, 1501, 1100, 1700)
-    undistort_map(1920, 1080, (2001, 1203)); dense(2, 3); triangulate(60000, 12, 1500); medians(800, 30000)
-    # small again
-    undistort(17, 29, 0); prepare(33, 47, 2, 0); remap(9, 13, 11, 15); jpeg(photos[1:]); undistort_map(31, 17, (20, 40)); dense(5, 1)
-    triangulate(700, 5, 64); medians(10, 400)
+    undistort_map(1920, 1080, (2001, 1203)); dense(2, 3); triangulate(60000, 12, 1500); medians(800, 30000); argsort((1 << 20) + 3); rdd("ladder")
+    optimize(len(before), 250)
+    # small again, behind staging buffers the large images left
+    undistort(17, 29, 0); optimize_without_residuals(30); rdd("hubs"); prepare(33, 47, 2, 0); argsort(4099); remap(9, 13, 11, 15); jpeg(photos[1:])
+    undistort_map(31, 17, (20, 40)); dense(5, 1); triangulate(700, 5, 64); medians(10, 400); optimize(7, 3)
     return steps
 
 
