@@ -116,6 +116,31 @@ int l3d_match_pairs_host(l3d_ctx* ctx, int num_pairs, const int32_t* pairs, cons
  * and keeps the match lists in the reference's unsorted list order.  There is still no CPU fallback. */
 int l3d_match_pairs_f64(l3d_ctx* ctx, int num_pairs, const int32_t* pairs, const double* Fd, float epi_overlap, int knn,
                         int first_pair, int last_pair);
+/* Caller-given candidates: pair i with restricted[i] != 0 is matched only against its listed (source segment, target segment) cells;
+ * the other pairs are scanned as l3d_match_pairs_range scans them.  triples[3*k..3*k+2] = (pair index, src_seg, tgt_seg), n of them, in
+ * any order, duplicates allowed; src_seg indexes the pair's source view (pairs[2*i]), tgt_seg its target view.  A triple of a pair that
+ * is not restricted, or not in [first_pair, last_pair), is checked and otherwise ignored; a restricted pair without triples has no
+ * matches.  on_device != 0: triples is a device address on this GPU (restricted is always host memory); the call reads it on the
+ * context's stream (l3d_stream), so work the caller queued there to fill it comes first, and work on other streams must be complete
+ * (or made to precede with an event) before the call. */
+typedef struct {
+    const int32_t* restricted;      /* num_pairs flags */
+    const int32_t* triples;         /* 3 * n */
+    long long n;
+    int32_t on_device;
+} l3d_match_cand_desc;
+/* l3d_match_pairs_range / l3d_match_pairs_f64 with candidates (DESIGN.md section 6c).  A row of a restricted pair keeps what the scan
+ * would keep if its other target segments did not exist: the same exact arithmetic of the semantics, overlap > epi_overlap, the four
+ * depth tests, kNN rule and tie order.  The outputs are those of the plain calls (counts, records, stride, l3d_match_total_matches,
+ * l3d_match_gather, l3d_match_restride, l3d_score_sweep), except l3d_match_pair_evals: Ns*Nt for a scanned pair, the distinct triples
+ * for a restricted one.  With every flag 0 the result is byte for byte the plain call's.  Rejected with L3D_ERR_INVALID before anything
+ * is launched: a null descriptor or array, n < 0, a pair index outside [0, num_pairs), a src_seg outside [0, Ns) or a tgt_seg outside
+ * [0, Nt) (l3d_last_error names the first such triple).  Waits for the device once, for the number of distinct triples; on_device also
+ * reads the triples back to check them (3 * n * 4 bytes to the host) and waits for that. */
+int l3d_match_pairs_cand(l3d_ctx* ctx, int num_pairs, const int32_t* pairs, const float* F, float epi_overlap, int knn, int first_pair,
+                         int last_pair, const l3d_match_cand_desc* cand);
+int l3d_match_pairs_cand_f64(l3d_ctx* ctx, int num_pairs, const int32_t* pairs, const double* Fd, float epi_overlap, int knn, int first_pair,
+                             int last_pair, const l3d_match_cand_desc* cand);
 /* slots per row of the record array of the last match result: knn, or the largest row when knn <= 0 was asked for */
 int l3d_match_stride(const l3d_ctx* ctx);
 #define L3D_SEM_REF_GPU 0
@@ -129,7 +154,8 @@ int l3d_match_device_buffers(l3d_ctx* ctx, void** counts_dev, void** recs_dev);
  * skips level 1, 0, then for every arc class c < 8 the first entry of the pair's sorted table inside class c whose arc start is not below
  * ka - 2^(21 + c) and the first whose start is above kb (pair-relative, over the whole class); basis_out[6] the pencil basis u, v;
  * class_off_out[10] the first sorted entry of every class and the end; arc_starts_out[Nt] the arc start of every sorted entry.  NULL
- * skips an output; a pair whose target view has no segments writes none. */
+ * skips an output; a pair whose target view has no segments writes none; a pair restricted to caller-given candidates
+ * (l3d_match_pairs_cand) has no table or windows and is rejected with L3D_ERR_INVALID. */
 int l3d_match_row_windows(l3d_ctx* ctx, int pair, uint32_t* windows_out, double* basis_out, int32_t* class_off_out, uint32_t* arc_starts_out);
 /* row_off_out[num_pairs+1]: first row of every pair in those buffers (prefix sum of Ns), last = total_rows */
 int l3d_pair_row_offsets(l3d_ctx* ctx, long long* row_off_out);
@@ -165,7 +191,7 @@ int l3d_match_restride(l3d_ctx* ctx, int stride);
 /* sizes of the last l3d_match_pairs result */
 long long l3d_match_total_rows(const l3d_ctx* ctx);      /* sum of Ns over pairs */
 long long l3d_match_total_matches(l3d_ctx* ctx);         /* matches of the last result (sum of the row counts), reduced on the device */
-long long l3d_match_pair_evals(const l3d_ctx* ctx);      /* sum of Ns*Nt over pairs */
+long long l3d_match_pair_evals(const l3d_ctx* ctx);      /* sum of Ns*Nt over pairs (distinct candidates of a restricted pair) */
 /* counts_out[row_off(pair)+r] for all pairs (row_off = prefix sum of Ns in pair order); returns total matches */
 long long l3d_get_match_counts(l3d_ctx* ctx, int32_t* counts_out);
 /* one pair: counts_out[Ns], recs_out[Ns*knn] (slot r*knn+i valid for i < counts_out[r]) */

@@ -56,6 +56,10 @@ void l3dpp_push_detections(void* out, const float* xy4, long long n);
 int l3dpp_match_images(void* h, float sp, float sa, unsigned int nn, float epi, int knn, float crd);
 int l3dpp_reconstruct_opt(void* h, unsigned int vis, int diffusion, float collin, int use_ceres, unsigned int max_iter);
 int l3dpp_set_shard(void* h, int rank, int world, l3dpp_exchange_fn fn, void* user);
+/* Line3D::setLineCandidates: seg_pairs[2 * n] = (segment of cam_a, segment of cam_b) per correspondence */
+int l3dpp_set_line_candidates(void* h, unsigned int cam_a, unsigned int cam_b, const unsigned int* seg_pairs, long long n);
+/* Line3D::clearLineCandidates */
+int l3dpp_clear_line_candidates(void* h);
 int l3dpp_stats(void* h, l3dpp_stats_block* out);
 /* the view index of a camID after matchImages, or -1 */
 int l3dpp_view_index(void* h, unsigned int cam);

@@ -35,6 +35,7 @@
 #include <list>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 
 #if !defined(L3DPP_WITH_EIGEN_OPENCV) && defined(__has_include)
@@ -168,7 +169,9 @@ struct FinalLine3D {   /* segment3D.h:155-163 */
     LineCluster3D underlyingCluster_;
 };
 
-/* counters the reference prints to stdout (SURVEY.md §5 "Metrics / logging"); handy parity checkpoints */
+/* counters the reference prints to stdout (SURVEY.md §5 "Metrics / logging"); handy parity checkpoints.  pair_evaluations: the
+ * (source, target) cells matchImages evaluated, Ns*Nt per scanned view pair and the distinct listed correspondences of a pair
+ * restricted by setLineCandidates */
 struct Line3DStats {
     long long view_pairs, pair_evaluations, matches_after_knn, estimates, affinity_entries, affinity_rows, clusters_total,
         clusters_valid, lines3D, collinear_entries, opt_iterations;
@@ -243,6 +246,20 @@ public:
      * no lock held: concurrent addImage calls run it concurrently, so it must be thread-safe.  nullptr: no detector. */
     typedef bool (*SegmentDetectorFn)(void* user, const Image8u& gray, std::vector<Vec4f>& detections);
     void setSegmentDetector(SegmentDetectorFn detector, void* user);
+
+    /* Restrict the matching of the view pair {camA, camB} to the given correspondences (segment of camA, segment of camB), e.g. from a
+     * descriptor or learned line matcher, line tracking or an SfM tool.  For each source segment of a restricted pair matchImages
+     * evaluates only the listed target segments, with everything else as the epipolar scan does it: the exact arithmetic of the
+     * semantics, the epipolar_overlap and depth tests, the kNN rule (kNN <= 0: all, ascending target; kNN > 32: all, then the cut) and
+     * the tie order (overlap descending, then the smaller target segment).  Listing every target segment of a pair gives the scan's
+     * matches.  An empty list restricts the pair to no matches.  Either camera order, duplicates allowed; a second call for the same
+     * pair replaces its list; the lists stay until clearLineCandidates().  Pairs without a list are scanned as before, and the visual
+     * neighbours are chosen as before: a list of a pair matchImages does not evaluate (not neighbours, or a camera never added) is
+     * ignored (verbose mode reports how many).  camA == camB is rejected with lastError() set; a segment ID at or beyond its view's
+     * segment count makes matchImages fail, naming the camera and segment.  stats().pair_evaluations counts Ns*Nt for a scanned pair
+     * and the distinct listed correspondences for a restricted one. */
+    void setLineCandidates(const unsigned int camA, const unsigned int camB, const std::vector<std::pair<unsigned int, unsigned int> >& seg_pairs);
+    void clearLineCandidates();
 
     /* line3D.h:140-145 */
     void matchImages(const float sigma_position = L3D_DEF_SCORING_POS_REGULARIZER, const float sigma_angle = L3D_DEF_SCORING_ANG_REGULARIZER,

@@ -23,6 +23,11 @@ class ViewDesc(C.Structure):
                 ("k", C.c_float), ("median_depth", C.c_float)]
 
 
+class CandDesc(C.Structure):
+    """l3d_match_cand_desc: the caller-given candidates of l3d_match_pairs_cand"""
+    _fields_ = [("restricted", C.c_void_p), ("triples", C.c_void_p), ("n", C.c_longlong), ("on_device", C.c_int32)]
+
+
 class UndistortDesc(C.Structure):
     """l3d_undistort_desc: one 8-bit image and its camera"""
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("channels", C.c_int32), ("src_pitch", C.c_int64), ("dst_pitch", C.c_int64),
@@ -315,6 +320,25 @@ class Context:
         last = len(pairs) if last is None else last
         self._chk(self.L.l3d_match_pairs_f64(self.h, len(pairs), _p(pairs), _p(Fd), epi_overlap, int(knn), int(first), int(last)),
                   "l3d_match_pairs_f64")
+        self._knn = int(self.L.l3d_match_stride(self.h))
+
+    def match_pairs_cand(self, pairs, F, restricted, triples, epi_overlap=0.25, knn=10, first=0, last=None, f64=False, on_device=False):
+        """l3d_match_pairs_cand (f64: _cand_f64 with double F): pairs with restricted[i] != 0 are matched only against their triples
+        (pair, src_seg, tgt_seg), int32 [n, 3]; on_device: triples is (device address of such an array, n)"""
+        pairs = np.ascontiguousarray(pairs, np.int32).reshape(-1, 2)
+        F = np.ascontiguousarray(F, np.float64 if f64 else np.float32).reshape(-1, 9)
+        rs = np.ascontiguousarray(restricted, np.int32).reshape(-1)
+        assert len(pairs) == len(F) == len(rs)
+        last = len(pairs) if last is None else last
+        if on_device:
+            addr, n = triples
+        else:
+            t = np.ascontiguousarray(triples, np.int32).reshape(-1, 3)
+            addr, n = t.ctypes.data, len(t)
+        d = CandDesc(rs.ctypes.data, addr, int(n), int(bool(on_device)))
+        fn = self.L.l3d_match_pairs_cand_f64 if f64 else self.L.l3d_match_pairs_cand
+        self._chk(fn(self.h, len(pairs), _p(pairs), _p(F), epi_overlap, int(knn), int(first), int(last), C.byref(d)),
+                  "l3d_match_pairs_cand" + ("_f64" if f64 else ""))
         self._knn = int(self.L.l3d_match_stride(self.h))
 
     def match_pairs_host(self, pairs, F, counts_ptr: int, recs_ptr: int, epi_overlap=0.25, knn=10, chunks=8):

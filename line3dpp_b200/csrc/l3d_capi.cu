@@ -7,6 +7,7 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_reduce.cuh>
 #include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
 #include <cub/iterator/transform_input_iterator.cuh>
 
 #include <algorithm>
@@ -242,8 +243,10 @@ int l3d_match_pairs(l3d_ctx* c, int num_pairs, const int32_t* pairs, const float
 struct HostOut { int32_t* counts; l3d_match_rec* recs; int chunks; };
 // Checks the arguments, fills h_pairs and the work units of k_match_topk for the pairs [first_pair, last_pair), uploads both and sizes the result buffers.
 // *narcs: the number of level-1 table entries of the matched pairs.
+// restricted (null: none): the per-pair flags of l3d_match_pairs_cand; a restricted pair has no level-1 table and no work units, its
+// rows go to k_match_cand (h_cand_pairs) and its evaluations are counted by stage_candidates.
 static int stage_pairs(l3d_ctx* c, int num_pairs, const int32_t* pairs, const float* F, const double* Fd, float epi_overlap, int knn,
-                       int first_pair, int last_pair, const HostOut* host, long long* narcs)
+                       int first_pair, int last_pair, const HostOut* host, const int32_t* restricted, long long* narcs)
 {
     if (host && (!host->counts || !host->recs || host->chunks < 1)) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs_host: bad arguments");
     if (host && knn <= 0) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs_host: kNN <= 0 has no fixed row stride; use l3d_match_pairs + l3d_get_pair_matches");
@@ -255,6 +258,8 @@ static int stage_pairs(l3d_ctx* c, int num_pairs, const int32_t* pairs, const fl
     L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync before pair staging");   // h_pairs/h_units may still be in flight
     c->h_pairs.resize(num_pairs);
     c->h_units.clear();
+    c->h_cand_pairs.clear(); c->cand_rows = 0;
+    if (restricted) c->h_restricted.assign(restricted, restricted + num_pairs); else c->h_restricted.clear();
     long long rows = 0, evals = 0;
     for (int i = 0; i < num_pairs; ++i) {
         int s = pairs[2 * i], t = pairs[2 * i + 1];
@@ -268,8 +273,10 @@ static int stage_pairs(l3d_ctx* c, int num_pairs, const int32_t* pairs, const fl
         int Ns = c->h_views[s].nseg, Nt = c->h_views[t].nseg;
         if (Nt >= (1 << 24)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: more than 2^24 segments in one view");
         p.arc_off = *narcs;
-        if (i >= first_pair && i < last_pair) *narcs += Nt;
-        if (Nt > 0 && i >= first_pair && i < last_pair) {     // the pair's rows in even units; several passes keep every row's list in a slot
+        const bool here = i >= first_pair && i < last_pair, scan = here && !(restricted && restricted[i]);
+        if (here && !scan && Ns > 0) { c->h_cand_pairs.push_back(make_longlong2(i, c->cand_rows)); c->cand_rows += Ns; }
+        if (scan) *narcs += Nt;
+        if (Nt > 0 && scan) {     // the pair's rows in even units; several passes keep every row's list in a slot
             const int most = Nt <= MK_STAGES * MK_TT ? MK_UNIT_ROWS : MK_NSLOT, n = (Ns + most - 1) / most;
             for (int u = 0; u < n; ++u) {
                 const int r0 = (int)((long long)Ns * u / n), r1 = (int)((long long)Ns * (u + 1) / n);
@@ -277,7 +284,7 @@ static int stage_pairs(l3d_ctx* c, int num_pairs, const int32_t* pairs, const fl
             }
         }
         rows += Ns;
-        if (i >= first_pair && i < last_pair) evals += (long long)Ns * Nt;     // evaluated HERE
+        if (scan) evals += (long long)Ns * Nt;     // evaluated HERE
     }
     c->num_pairs = num_pairs; c->knn = knn; c->epi = epi_overlap; c->total_rows = rows; c->pair_evals = evals;
     c->knn_asked = std::max(knn, 0); c->first_pair = first_pair; c->last_pair = last_pair;
@@ -299,7 +306,8 @@ static float4* level1_segs(l3d_ctx* c, long long narcs) { return (float4*)((uint
 
 // Level-1 tables of the pairs matched here (l3d_device.cuh "pencil parameter"): raw arcs + keys, one sort, packed arcs and their target
 // segments in window order.  Below epi_overlap 0.01 the extended arcs would span the whole line: everything is then handed to the float filter.
-static int build_level1(l3d_ctx* c, int first_pair, int last_pair, long long narcs, float epi_overlap)
+// restricted (device, null: none): pairs restricted to caller-given candidates get empty tables.
+static int build_level1(l3d_ctx* c, int first_pair, int last_pair, long long narcs, float epi_overlap, const int* restricted)
 {
     c->level1_first = c->level1_last = 0;
     if (last_pair <= first_pair || narcs <= 0) return L3D_OK;
@@ -312,7 +320,7 @@ static int build_level1(l3d_ctx* c, int first_pair, int last_pair, long long nar
     L3D_RESERVE(c->d_arcraw, 16 * narcs, "raw arcs"); L3D_RESERVE(c->d_arckeys, 8 * narcs, "arc keys"); L3D_RESERVE(c->d_arckeys2, 8 * narcs, "arc keys");
     L3D_RESERVE(c->d_arcvals, 4 * narcs, "arc order"); L3D_RESERVE(c->d_arcvals2, 4 * narcs, "arc order");
     k_pair_arcs<<<(unsigned int)npr, 256, 0, c->stream>>>(c->segs(), c->views(), (const L3DPairDev*)c->d_pairs.p, first_pair, on ? 1 : 0,
-                                                         1.0 / (double)std::max(epi_overlap, 0.01f) + 0.5, (uint4*)c->d_arcraw.p,
+                                                         1.0 / (double)std::max(epi_overlap, 0.01f) + 0.5, restricted, (uint4*)c->d_arcraw.p,
                                                          (unsigned long long*)c->d_arckeys.p, (unsigned int*)c->d_arcvals.p, (L3DPairBasis*)c->d_basis.p);
     L3D_CUDA(c, cudaGetLastError(), "k_pair_arcs");
     if ((rc = l3d_cub(c, "arc sort", [&](void* tmp, size_t& bytes) {
@@ -357,6 +365,18 @@ static int launch_match(l3d_ctx* c, Keep keep, MatchArgs a, size_t t0, size_t t1
     a.units += t0;
     void* args[] = {&a};
     cudaLaunchKernel((const void*)l3d_match_kernels[c->semantics][(int)keep], dim3((unsigned int)(t1 - t0)), dim3(MK_THREADS), args, l3d_match_smem_bytes(c->semantics), c->stream);
+    ++c->launches;
+    L3D_CUDA(c, cudaGetLastError(), what);
+    return L3D_OK;
+}
+
+// one launch of k_match_cand<c->semantics, keep> over the restricted rows of the call (none: nothing)
+static int launch_cand(l3d_ctx* c, Keep keep, CandArgs a, const char* what)
+{
+    if (c->cand_rows == 0) return L3D_OK;
+    void* args[] = {&a};
+    cudaLaunchKernel((const void*)l3d_cand_kernels[c->semantics][(int)keep], dim3((unsigned int)((c->cand_rows + CAND_WARPS - 1) / CAND_WARPS)),
+                     dim3(32 * CAND_WARPS), args, 0, c->stream);
     ++c->launches;
     L3D_CUDA(c, cudaGetLastError(), what);
     return L3D_OK;
@@ -441,25 +461,29 @@ static int relay_recs(l3d_ctx* c, int stride, long long a, long long z)
 // "Keep all matches" (kNN <= 0, cudawrapper.cu:628-636, line3D.cc:988-996): count pass -> row stride = largest row -> store pass ->
 // rows sorted.  big_k > 0 (kNN > 32 exceeds the fused kernel's per-row key list): the same passes, and every row is cut to its big_k
 // best afterwards (same matches as the reference's priority queue, line3D.cc:999-1006 / cudawrapper.cu:637-645).
-static int run_keep_all(l3d_ctx* c, MatchArgs a, int big_k)
+// Restricted rows (l3d_match_pairs_cand) take the same passes in k_match_cand.
+static int run_keep_all(l3d_ctx* c, MatchArgs a, int big_k, CandArgs ca)
 {
     const long long rows = c->total_rows;
     const size_t nunits = c->h_units.size();
+    const bool any = nunits || c->cand_rows;
     int rc, stride = 1;
-    if (nunits) {
-        a.knn = 0; a.recs = nullptr;
-        if ((rc = launch_match(c, Keep::Count, a, 0, nunits, "k_match_topk (count)"))) return rc;
+    if (any) {
+        a.knn = 0; a.recs = nullptr; ca.knn = 0; ca.recs = nullptr;
+        if (nunits && (rc = launch_match(c, Keep::Count, a, 0, nunits, "k_match_topk (count)"))) return rc;
+        if ((rc = launch_cand(c, Keep::Count, ca, "k_match_cand (count)"))) return rc;
         if ((rc = row_max(c, &stride))) return rc;
     }
     c->knn = stride;
     L3D_RESERVE(c->d_recs, sizeof(l3d_match_rec) * (size_t)std::max<long long>(rows, 1) * stride, "match records");
-    if (nunits) {
+    if (any) {
         const size_t per_warp = sizeof(l3d_match_rec) * (size_t)stride;
         int wpb = 4;
         while (wpb > 1 && per_warp * wpb > SORT_SMEM_MAX) wpb >>= 1;
         if (per_warp * wpb > SORT_SMEM_MAX) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: a row with more than 8500 matches (kNN <= 0)");
-        a.knn = stride; a.recs = (l3d_match_rec*)c->d_recs.p;
-        if ((rc = launch_match(c, Keep::Store, a, 0, nunits, "k_match_topk (store)"))) return rc;
+        a.knn = stride; a.recs = (l3d_match_rec*)c->d_recs.p; ca.knn = stride; ca.recs = a.recs;
+        if (nunits && (rc = launch_match(c, Keep::Store, a, 0, nunits, "k_match_topk (store)"))) return rc;
+        if ((rc = launch_cand(c, Keep::Store, ca, "k_match_cand (store)"))) return rc;
         const long long blocks = std::min<long long>((rows + wpb - 1) / wpb, (long long)c->num_sms * 16);
         k_sort_rows<<<(unsigned int)blocks, wpb * 32, per_warp * wpb, c->stream>>>((int*)c->d_counts.p, (l3d_match_rec*)c->d_recs.p, stride, rows, big_k);
         L3D_CUDA(c, cudaGetLastError(), "k_sort_rows");
@@ -468,22 +492,122 @@ static int run_keep_all(l3d_ctx* c, MatchArgs a, int big_k)
     return L3D_OK;
 }
 
+// The triples of l3d_match_pairs_cand, checked on the host (a device array is read back first, into the context's pinned staging buffer):
+// *ignored counts those of pairs that are not restricted or not evaluated here.  Needs the views; nothing is launched.
+static int check_candidates(l3d_ctx* c, int num_pairs, const int32_t* pairs, const l3d_match_cand_desc* cand, const int32_t** trip,
+                            int first_pair, int last_pair, long long* ignored)
+{
+    if (!cand || cand->n < 0 || (num_pairs > 0 && !cand->restricted) || (cand->n > 0 && !cand->triples))
+        return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs_cand: null candidate descriptor or array, or n < 0");
+    if (!c->have_views) return l3d_fail(c, L3D_ERR_STATE, "l3d_match_pairs: call l3d_set_views first");
+    if (num_pairs < 0 || (num_pairs && !pairs)) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs: bad arguments");
+    if (cand->n >= INT_MAX) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs_cand: 2^31 or more candidates in one call");
+    *trip = cand->triples;
+    if (cand->on_device && cand->n > 0) {
+        cudaSetDevice(c->device);
+        const size_t bytes = sizeof(int32_t) * 3 * (size_t)cand->n;
+        if (bytes > c->h_stage_cap) {
+            void* p = nullptr;
+            L3D_CUDA(c, cudaStreamSynchronize(c->stream), "sync before staging");     // an upload of l3d_set_views may still read it
+            c->h_stage.reset(); c->h_stage_cap = 0;
+            L3D_CUDA(c, cudaMallocHost(&p, bytes), "pinned staging");
+            c->h_stage.reset(p); c->h_stage_cap = bytes;
+        }
+        // on the context's stream: after whatever the caller queued there to fill the triples, before the kernels that read them
+        L3D_CUDA(c, cudaMemcpyAsync(c->h_stage.get(), cand->triples, bytes, cudaMemcpyDeviceToHost, c->stream), "l3d_match_pairs_cand: read the candidates");
+        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "l3d_match_pairs_cand: read the candidates");
+        *trip = (const int32_t*)c->h_stage.get();
+    }
+    std::vector<int2> seg_count((size_t)num_pairs);        // (Ns, Nt) of every pair
+    for (int p = 0; p < num_pairs; ++p) {
+        const int s = pairs[2 * p], t = pairs[2 * p + 1];
+        if (s < 0 || t < 0 || s >= c->num_views || t >= c->num_views) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_pairs: view index out of range");
+        seg_count[p] = make_int2(c->h_views[s].nseg, c->h_views[t].nseg);
+    }
+    *ignored = 0;
+    for (long long k = 0; k < cand->n; ++k) {
+        const int p = (*trip)[3 * k], a = (*trip)[3 * k + 1], b = (*trip)[3 * k + 2];
+        char msg[200];
+        if (p < 0 || p >= num_pairs) {
+            snprintf(msg, sizeof(msg), "l3d_match_pairs_cand: candidate %lld names pair %d outside the pair list of %d", k, p, num_pairs);
+            return l3d_fail(c, L3D_ERR_INVALID, msg);
+        }
+        const int Ns = seg_count[p].x, Nt = seg_count[p].y;
+        if (a < 0 || a >= Ns || b < 0 || b >= Nt) {
+            snprintf(msg, sizeof(msg), "l3d_match_pairs_cand: candidate %lld of pair %d: segment (%d, %d) outside the views' %d x %d segments", k, p, a, b, Ns, Nt);
+            return l3d_fail(c, L3D_ERR_INVALID, msg);
+        }
+        *ignored += !(p >= first_pair && p < last_pair && cand->restricted[p]);
+    }
+    return L3D_OK;
+}
+
+// The candidates of the restricted pairs on the device: one key per triple (k_cand_keys), sorted, duplicates dropped (cub); k_match_cand
+// finds a row's candidates by two binary searches.  *distinct: the distinct candidates of the restricted pairs evaluated here (waits).
+static int stage_candidates(l3d_ctx* c, const l3d_match_cand_desc* cand, const int32_t* trip_host, int first_pair, int last_pair, long long ignored,
+                            long long* distinct)
+{
+    const long long n = cand->n;
+    int rc;
+    if (c->total_rows >= (1ll << 39)) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs_cand: 2^39 or more rows");
+    L3D_RESERVE(c->d_cand_keys, 8 * n, "candidate keys"); L3D_RESERVE(c->d_cand_keys2, 8 * n, "candidate keys"); L3D_RESERVE(c->d_cand_n, sizeof(int), "candidate count");
+    L3D_RESERVE(c->d_cand_pairs, sizeof(longlong2) * c->h_cand_pairs.size(), "restricted pairs");
+    if (!c->h_cand_pairs.empty())
+        L3D_CUDA(c, cudaMemcpyAsync(c->d_cand_pairs.p, c->h_cand_pairs.data(), sizeof(longlong2) * c->h_cand_pairs.size(), cudaMemcpyHostToDevice, c->stream), "upload restricted pairs");
+    int nuniq = 0;
+    if (n > 0) {
+        const int32_t* trip = cand->triples;
+        if (!cand->on_device) {
+            L3D_RESERVE(c->d_cand_trip, sizeof(int32_t) * 3 * n, "candidates");
+            L3D_CUDA(c, cudaMemcpyAsync(c->d_cand_trip.p, trip_host, sizeof(int32_t) * 3 * n, cudaMemcpyHostToDevice, c->stream), "upload candidates");
+            trip = (const int32_t*)c->d_cand_trip.p;
+        }
+        k_cand_keys<<<(unsigned int)((n + 255) / 256), 256, 0, c->stream>>>(n, trip, (const L3DPairDev*)c->d_pairs.p, (const int*)c->d_restricted.p,
+                                                                          first_pair, last_pair, (unsigned long long*)c->d_cand_keys2.p);
+        L3D_CUDA(c, cudaGetLastError(), "k_cand_keys");
+        if ((rc = l3d_cub(c, "candidate sort", [&](void* tmp, size_t& bytes) {
+                 return cub::DeviceRadixSort::SortKeys(tmp, bytes, (const unsigned long long*)c->d_cand_keys2.p, (unsigned long long*)c->d_cand_keys.p,
+                                                       (int)n, 0, 64, c->stream); }))) return rc;
+        if ((rc = l3d_cub(c, "candidate dedup", [&](void* tmp, size_t& bytes) {
+                 return cub::DeviceSelect::Unique(tmp, bytes, (const unsigned long long*)c->d_cand_keys.p, (unsigned long long*)c->d_cand_keys2.p,
+                                                  (int*)c->d_cand_n.p, (int)n, c->stream); }))) return rc;
+        std::swap(c->d_cand_keys, c->d_cand_keys2);
+        c->launches += 1 + 4 + 1;
+        L3D_CUDA(c, cudaMemcpyAsync(&nuniq, c->d_cand_n.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream), "candidate count");
+        L3D_CUDA(c, cudaStreamSynchronize(c->stream), "candidate count");
+    } else L3D_CUDA(c, cudaMemsetAsync(c->d_cand_n.p, 0, sizeof(int), c->stream), "candidate count");
+    *distinct = nuniq - (ignored > 0 ? 1 : 0);      // the ignored triples leave one L3D_CAND_NONE key, sorted last
+    return L3D_OK;
+}
+
 static int match_impl(l3d_ctx* c, int num_pairs, const int32_t* pairs, const float* F, const double* Fd, float epi_overlap, int knn, int first_pair, int last_pair,
-                      const HostOut* host = nullptr)
+                      const HostOut* host = nullptr, const l3d_match_cand_desc* cand = nullptr, bool with_cand = false)
 {
     if (!c) return L3D_ERR_INVALID;
     c->drop(Stage::Matches);
     int rc;
-    long long narcs = 0;
-    if ((rc = stage_pairs(c, num_pairs, pairs, F, Fd, epi_overlap, knn, first_pair, last_pair, host, &narcs))) return rc;
-    if ((rc = build_level1(c, first_pair, last_pair, narcs, epi_overlap))) return rc;
+    long long narcs = 0, ignored = 0, distinct = 0;
+    const int32_t* trip = nullptr;
+    if (with_cand && (rc = check_candidates(c, num_pairs, pairs, cand, &trip, first_pair, last_pair, &ignored))) return rc;
+    if ((rc = stage_pairs(c, num_pairs, pairs, F, Fd, epi_overlap, knn, first_pair, last_pair, host, with_cand ? cand->restricted : nullptr, &narcs))) return rc;
+    if (with_cand) {
+        L3D_RESERVE(c->d_restricted, sizeof(int) * (size_t)num_pairs, "restricted pairs");
+        if (num_pairs) L3D_CUDA(c, cudaMemcpyAsync(c->d_restricted.p, cand->restricted, sizeof(int) * (size_t)num_pairs, cudaMemcpyHostToDevice, c->stream), "upload restricted pairs");
+    }
+    if ((rc = build_level1(c, first_pair, last_pair, narcs, epi_overlap, with_cand ? (const int*)c->d_restricted.p : nullptr))) return rc;
+    if (with_cand && (rc = stage_candidates(c, cand, trip, first_pair, last_pair, ignored, &distinct))) return rc;
+    c->pair_evals += distinct;
     if (Fd && (rc = build_cache_d(c))) return rc;
     c->semantics = Fd ? L3D_SEM_REF_CPU : L3D_SEM_REF_GPU;
     const MatchArgs a = {c->segs(), (const float4*)c->d_cache.p, Fd ? (const double*)c->d_cache_d.p : nullptr, c->views(), (const L3DPairDev*)c->d_pairs.p,
                          (const int4*)c->d_units.p, (const uint4*)c->d_arcs.p, level1_segs(c, narcs), (const L3DPairBasis*)c->d_basis.p,
                          (const uint4*)c->d_rowwin.p, first_pair < num_pairs ? c->h_pairs[first_pair].row_off : 0, (int*)c->d_counts.p,
                          (l3d_match_rec*)c->d_recs.p, knn, epi_overlap};
-    if ((rc = knn > 0 && knn <= 32 ? run_topk(c, a, host) : run_keep_all(c, a, knn > 32 ? knn : 0))) return rc;
+    const CandArgs ca = {a.segs, a.cache, a.cache_d, a.views, a.pairs, (const longlong2*)c->d_cand_pairs.p, (int)c->h_cand_pairs.size(), c->cand_rows,
+                         (const unsigned long long*)c->d_cand_keys.p, (const int*)c->d_cand_n.p, a.counts, a.recs, knn, epi_overlap};
+    if (knn > 0 && knn <= 32) {
+        if ((rc = run_topk(c, a, host)) || (rc = launch_cand(c, Keep::TopK, ca, "k_match_cand"))) return rc;
+    } else if ((rc = run_keep_all(c, a, knn > 32 ? knn : 0, ca))) return rc;
     c->have_matches = true;
     return L3D_OK;
 }
@@ -493,6 +617,14 @@ int l3d_match_pairs_range(l3d_ctx* c, int num_pairs, const int32_t* pairs, const
 
 int l3d_match_pairs_f64(l3d_ctx* c, int num_pairs, const int32_t* pairs, const double* Fd, float epi_overlap, int knn, int first_pair, int last_pair)
 { return match_impl(c, num_pairs, pairs, nullptr, Fd, epi_overlap, knn, first_pair, last_pair); }
+
+int l3d_match_pairs_cand(l3d_ctx* c, int num_pairs, const int32_t* pairs, const float* F, float epi_overlap, int knn, int first_pair, int last_pair,
+                         const l3d_match_cand_desc* cand)
+{ return match_impl(c, num_pairs, pairs, F, nullptr, epi_overlap, knn, first_pair, last_pair, nullptr, cand, true); }
+
+int l3d_match_pairs_cand_f64(l3d_ctx* c, int num_pairs, const int32_t* pairs, const double* Fd, float epi_overlap, int knn, int first_pair,
+                             int last_pair, const l3d_match_cand_desc* cand)
+{ return match_impl(c, num_pairs, pairs, nullptr, Fd, epi_overlap, knn, first_pair, last_pair, nullptr, cand, true); }
 
 int l3d_match_pairs_host(l3d_ctx* c, int num_pairs, const int32_t* pairs, const float* F, float epi_overlap, int knn, int32_t* counts_out,
                          l3d_match_rec* recs_out, int chunks)
@@ -515,6 +647,8 @@ int l3d_match_row_windows(l3d_ctx* c, int pair, uint32_t* windows_out, double* b
     if (!c) return L3D_ERR_INVALID;
     if (!c->have_matches) return l3d_fail(c, L3D_ERR_STATE, "l3d_match_row_windows: no match result");
     if (pair < c->level1_first || pair >= c->level1_last) return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_row_windows: pair not evaluated by the last match call");
+    if (!c->h_restricted.empty() && c->h_restricted[pair])
+        return l3d_fail(c, L3D_ERR_INVALID, "l3d_match_row_windows: the pair was restricted to caller-given candidates: it has no level-1 table or row windows");
     cudaSetDevice(c->device);
     const L3DPairDev& p = c->h_pairs[pair];
     const int Ns = c->h_views[p.src].nseg, Nt = c->h_views[p.tgt].nseg;
@@ -688,8 +822,8 @@ static int gather_rows(l3d_ctx* d, int n, l3d_ctx* const* src, const int32_t* b)
                                      : copy_pitched(d, dr, REC * stride, s, sr, REC * s->knn, REC * s->knn, (size_t)(z - a)),
                  "l3d_match_gather: copy records");
     }
-    long long evals = 0;
-    for (int p = b[0]; p < b[n]; ++p) evals += (long long)d->h_views[d->h_pairs[p].src].nseg * d->h_views[d->h_pairs[p].tgt].nseg;
+    long long evals = 0;                    // each source's own count: Ns*Nt per scanned pair, the distinct candidates of a restricted one
+    for (int i = 0; i < n; ++i) evals += src[i]->pair_evals;
     d->pair_evals = evals; d->first_pair = b[0]; d->last_pair = b[n];
     return L3D_OK;
 }

@@ -177,7 +177,7 @@ struct l3d_ctx {
     std::vector<L3DViewDev> h_views;
     DevBuf d_segs, d_cache, d_cache_d, d_views;
     const float4* segs_ext = nullptr;       // caller-owned device segment array (l3d_set_views_flat on_device)
-    std::unique_ptr<void, cudaError_t (*)(void*)> h_stage{nullptr, cudaFreeHost};    // pinned staging of l3d_set_views
+    std::unique_ptr<void, cudaError_t (*)(void*)> h_stage{nullptr, cudaFreeHost};    // pinned staging of l3d_set_views and of the device triples l3d_match_pairs_cand checks
     size_t h_stage_cap = 0;
 
     // last match result
@@ -193,6 +193,13 @@ struct l3d_ctx {
     DevBuf d_pairs, d_units, d_counts, d_recs, d_rowptr, d_csr, d_dense_jobs, d_arcs, d_basis, d_arcraw, d_arckeys, d_arckeys2, d_arcvals, d_arcvals2;
     DevBuf d_rowwin;                        // row windows of the rows of [level1_first, level1_last) (k_row_windows, L3D_RW_WORDS words per row)
     int level1_first = 0, level1_last = 0;  // the pairs whose level-1 tables, bases and row windows the context holds (its own last match call)
+    // caller-given candidates of the last match call (l3d_match_pairs_cand): its per-pair restricted flags (empty: none), the restricted
+    // pairs it evaluated as (pair, first restricted row), their rows in all (0: every pair scanned); on the device the per-pair flags,
+    // those pairs, the triples (host mode), the sort's two key buffers (d_cand_keys: the sorted distinct keys) and their number
+    std::vector<int> h_restricted;
+    std::vector<longlong2> h_cand_pairs;
+    long long cand_rows = 0;
+    DevBuf d_restricted, d_cand_pairs, d_cand_trip, d_cand_keys, d_cand_keys2, d_cand_n;
 
     SweepState sweep;
     RddState rdd;

@@ -386,11 +386,12 @@ __device__ uint4 target_arc(const L3DPairBasis& B, float4 q, double ext, bool en
     return make_uint4(kc + (unsigned int)lo, (unsigned int)(hi - lo), (unsigned int)(lo - lox), (unsigned int)(hix - hi));
 }
 
-// one CTA per view pair: basis, raw arcs, class sizes and the sort keys (pair, class, start of T)
+// one CTA per view pair: basis, raw arcs, class sizes and the sort keys (pair, class, start of T).  A pair restricted to caller-given
+// candidates (restricted non-null and set for it: l3d_match_pairs_cand) has an empty table.
 __global__ void __launch_bounds__(256)
 k_pair_arcs(const float4* __restrict__ segs, const L3DViewDev* __restrict__ views, const L3DPairDev* __restrict__ pairs, int first_pair,
-            int enabled, double ext, uint4* __restrict__ raw, unsigned long long* __restrict__ keys, unsigned int* __restrict__ vals,
-            L3DPairBasis* __restrict__ basis)
+            int enabled, double ext, const int* __restrict__ restricted, uint4* __restrict__ raw, unsigned long long* __restrict__ keys,
+            unsigned int* __restrict__ vals, L3DPairBasis* __restrict__ basis)
 {
     __shared__ L3DPairBasis B;
     __shared__ int cnt[L3D_ARC_NCLS + 1];
@@ -400,7 +401,7 @@ k_pair_arcs(const float4* __restrict__ segs, const L3DViewDev* __restrict__ view
     __syncthreads();
     const L3DViewDev* vt = views + P->tgt;
     const float4* t = segs + vt->seg_off;
-    const int Nt = vt->nseg;
+    const int Nt = restricted && restricted[first_pair + blockIdx.x] ? 0 : vt->nseg;
     for (int j = threadIdx.x; j < Nt; j += 256) {
         const uint4 r = target_arc(B, t[j], ext, enabled != 0);
         const int c = arc_class(r.y);
@@ -783,6 +784,140 @@ static_assert(L3D_SEM_REF_GPU == 0 && L3D_SEM_REF_CPU == 1 && (int)Keep::TopK ==
 void (*const l3d_match_kernels[2][3])(MatchArgs) = {
     {k_match_topk<L3D_SEM_REF_GPU, Keep::TopK>, k_match_topk<L3D_SEM_REF_GPU, Keep::Count>, k_match_topk<L3D_SEM_REF_GPU, Keep::Store>},
     {k_match_topk<L3D_SEM_REF_CPU, Keep::TopK>, k_match_topk<L3D_SEM_REF_CPU, Keep::Count>, k_match_topk<L3D_SEM_REF_CPU, Keep::Store>},
+};
+
+// ------------------------------------------------------------------------------------------------ caller-given candidates
+__global__ void __launch_bounds__(256) k_cand_keys(long long n, const int32_t* __restrict__ trip, const L3DPairDev* __restrict__ pairs,
+                                                   const int* __restrict__ restricted, int first_pair, int last_pair,
+                                                   unsigned long long* __restrict__ keys)
+{
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int p = trip[3 * i];
+    const bool use = p >= first_pair && p < last_pair && restricted[p];
+    keys[i] = use ? ((unsigned long long)(pairs[p].row_off + trip[3 * i + 1]) << 24) | (unsigned long long)trip[3 * i + 2] : L3D_CAND_NONE;
+}
+
+// first index in the sorted keys [0, n) whose key is not below k
+__device__ __forceinline__ int cand_lower_bound(const unsigned long long* __restrict__ keys, int n, unsigned long long k)
+{
+    int lo = 0, hi = n;
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (__ldg(keys + mid) < k) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+
+// One warp per source row of a restricted pair; lane i takes the row's candidates i, i + 32, ...  The decisions are k_match_topk's on
+// the same values: the row's epipolar lines F*p from the float F (REF_GPU) or the double F (REF_CPU), exact_overlap / exact_overlap_f64
+// on the target segment, the overlap above epi, then the depth test (depths_in_front where only the outcome is needed, the depths
+// themselves where they are stored), keys make_key.  k_match_topk's pre-filters are conservative, so with every target as a candidate
+// the matches are its own.  TopK keeps the row's k best keys in shared memory, sorted best first: every batch of 32 is ranked against
+// them and the list by counting.  Count / Store keep every match; the candidates arrive in ascending target order, so Store writes
+// the row in the order k_sort_rows leaves it.
+template <int SEM, Keep KEEP>
+__global__ void __launch_bounds__(32 * CAND_WARPS) k_match_cand(const CandArgs A)
+{
+    __shared__ unsigned long long best[CAND_WARPS][32];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long g = (long long)blockIdx.x * CAND_WARPS + warp;
+    if (g >= A.nrows) return;
+    const int ip = last_le(A.nrp, g, [&](int i) { return A.rpairs[i].y; });
+    const L3DPairDev* P = A.pairs + A.rpairs[ip].x;
+    const int r = (int)(g - A.rpairs[ip].y);
+    const L3DViewDev* vs = A.views + __ldg(&P->src);
+    const L3DViewDev* vt = A.views + __ldg(&P->tgt);
+    const long long R = __ldg(&P->row_off) + r, sidx = __ldg(&vs->seg_off) + r, toff = __ldg(&vt->seg_off);
+    const int nk = *A.nkeys;
+    const int b = cand_lower_bound(A.keys, nk, (unsigned long long)R << 24), e = cand_lower_bound(A.keys, nk, (unsigned long long)(R + 1) << 24);
+    const float4 s = __ldg(A.segs + sidx);
+    const float3 Cs = make_float3(vs->C[0], vs->C[1], vs->C[2]), Ct = make_float3(vt->C[0], vt->C[1], vt->C[2]);
+    float3 e1, e2;
+    SegRays sr;
+    float snum = 0.0f;
+    D3 e1d, e2d, Csd, Ctd;
+    if (SEM == L3D_SEM_REF_CPU) {
+        e1d = dmulmat(P->Fd, d3((double)s.x, (double)s.y, 1.0)); e2d = dmulmat(P->Fd, d3((double)s.z, (double)s.w, 1.0));
+        Csd = d3(vs->C_d[0], vs->C_d[1], vs->C_d[2]); Ctd = d3(vt->C_d[0], vt->C_d[1], vt->C_d[2]);
+    } else {
+        e1 = mulmat_h(P->F, s.x, s.y); e2 = mulmat_h(P->F, s.z, s.w);
+        sr = load_rays(A.cache, sidx);
+        snum = depth_num(sr.n, Cs, Ct);
+    }
+    const int K = min(A.knn, 32);
+    unsigned long long mine = 0ull;     // TopK: the lane-th best key so far (0: none)
+    int cnt = 0;                        // TopK: keys in the list; Count / Store: matches so far
+    for (int i0 = b; i0 < e; i0 += 32) {
+        const int i = i0 + lane;
+        const bool has = i < e;
+        const unsigned int j = has ? (unsigned int)(__ldg(A.keys + i) & 0xFFFFFFull) : 0u;
+        const float4 q = __ldg(A.segs + toff + j);
+        float ov = 0.0f, d[4];
+        bool pass;
+        if (SEM == L3D_SEM_REF_CPU) {
+            bool valid;
+            ov = exact_overlap_f64(q, e1d, e2d, &valid);
+            pass = has && valid && ov > A.epi;
+            if (pass) {
+                double dd[4];
+                exact_depths_f64(load_rays_d(A.cache_d, sidx), load_rays_d(A.cache_d, toff + j), Csd, Ctd, dd);
+                d[0] = (float)dd[0]; d[1] = (float)dd[1]; d[2] = (float)dd[2]; d[3] = (float)dd[3];
+                pass = dd[0] > L3D_EPS_D && dd[1] > L3D_EPS_D && dd[2] > L3D_EPS_D && dd[3] > L3D_EPS_D;
+            }
+        } else {
+            bool inv;
+            ov = exact_overlap(q, e1, e2, &inv);
+            pass = has && ov > A.epi;
+            if (pass) {
+                const SegRays t = load_rays(A.cache, toff + j);
+                if (KEEP == Keep::Store) { exact_depths(sr, t, Cs, Ct, d); pass = d[0] > 0.0f && d[1] > 0.0f && d[2] > 0.0f && d[3] > 0.0f; }
+                else pass = depths_in_front(sr, t, Cs, Ct, snum);
+            }
+        }
+        const unsigned int bal = __ballot_sync(0xffffffffu, pass);
+        if (KEEP != Keep::TopK) {
+            if (KEEP == Keep::Store && pass) {
+                const int slot = cnt + __popc(bal & ((1u << lane) - 1u));
+                if (slot < A.knn) {
+                    l3d_match_rec rec;
+                    rec.tgt_seg = j; rec.overlap = ov; rec.d_p1 = d[0]; rec.d_p2 = d[1]; rec.d_q1 = d[2]; rec.d_q2 = d[3];
+                    A.recs[R * A.knn + slot] = rec;
+                }
+            }
+            cnt += __popc(bal);
+            continue;
+        }
+        if (!bal) continue;
+        // rank of every new key and of every listed key among both (keys are distinct and > 0; 0 marks no key)
+        const unsigned long long key = pass ? make_key(ov, j) : 0ull;
+        int rk = 0, rm = lane;
+        for (int l = 0; l < 32; ++l) {
+            const unsigned long long ok = __shfl_sync(0xffffffffu, mine, l), nk2 = __shfl_sync(0xffffffffu, key, l);
+            rk += (ok > key) + (nk2 > key);
+            rm += nk2 > mine;
+        }
+        __syncwarp();
+        if (mine && rm < K) best[warp][rm] = mine;
+        if (key && rk < K) best[warp][rk] = key;
+        cnt = min(cnt + __popc(bal), K);
+        __syncwarp();
+        mine = lane < cnt ? best[warp][lane] : 0ull;
+    }
+    if (lane == 0) A.counts[R] = cnt;
+    if (KEEP != Keep::TopK || lane >= cnt) return;
+    const unsigned int j = key_tgt(mine);
+    float d[4];
+    if (SEM == L3D_SEM_REF_CPU) {
+        double dd[4];
+        exact_depths_f64(load_rays_d(A.cache_d, sidx), load_rays_d(A.cache_d, toff + j), Csd, Ctd, dd);
+        d[0] = (float)dd[0]; d[1] = (float)dd[1]; d[2] = (float)dd[2]; d[3] = (float)dd[3];
+    } else exact_depths(sr, load_rays(A.cache, toff + j), Cs, Ct, d);
+    l3d_match_rec rec;
+    rec.tgt_seg = j; rec.overlap = key_overlap(mine); rec.d_p1 = d[0]; rec.d_p2 = d[1]; rec.d_q1 = d[2]; rec.d_q2 = d[3];
+    A.recs[R * A.knn + lane] = rec;
+}
+
+void (*const l3d_cand_kernels[2][3])(CandArgs) = {
+    {k_match_cand<L3D_SEM_REF_GPU, Keep::TopK>, k_match_cand<L3D_SEM_REF_GPU, Keep::Count>, k_match_cand<L3D_SEM_REF_GPU, Keep::Store>},
+    {k_match_cand<L3D_SEM_REF_CPU, Keep::TopK>, k_match_cand<L3D_SEM_REF_CPU, Keep::Count>, k_match_cand<L3D_SEM_REF_CPU, Keep::Store>},
 };
 
 // keep-all rows arrive in queue order; the reference appends them in ascending target order.  One warp per row, the row

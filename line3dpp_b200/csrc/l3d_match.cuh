@@ -70,11 +70,32 @@ enum { MP_SETUP, MP_WINDOW, MP_PIECES, MP_SCAN, MP_EXACT, MP_FINAL, MP_WAIT, MP_
        MP_OVERLAP_PASS, MP_DEPTH_PASS, MP_PUSHED, MP_PRUNES, MP_CTAS, MP_BUSY_MAX, MP_BUSY_MIN, MP_BUSY_SUM, MP_N };
 #endif
 extern void (*const l3d_match_kernels[2][3])(MatchArgs);                   // every instantiation of k_match_topk: [SEM][KEEP]
+// Caller-given candidates (l3d_match_pairs_cand): a candidate is the key (global row << 24) | target segment, global row = the pair's
+// row_off + source segment.  k_cand_keys turns the caller's (pair, src_seg, tgt_seg) triples into keys (L3D_CAND_NONE for a triple of a
+// pair that is not restricted or not evaluated by the call); a radix sort and a unique pass leave them sorted and distinct.
+#define L3D_CAND_NONE 0xFFFFFFFFFFFFFFFFull
+__global__ void k_cand_keys(long long n, const int32_t* __restrict__ trip, const L3DPairDev* __restrict__ pairs, const int* __restrict__ restricted,
+                            int first_pair, int last_pair, unsigned long long* __restrict__ keys);
+// parameters of k_match_cand, passed by value
+struct CandArgs {
+    const float4* segs; const float4* cache; const double* cache_d;       // as MatchArgs
+    const L3DViewDev* views; const L3DPairDev* pairs;
+    const longlong2* rpairs; int nrp; long long nrows;                    // (pair, its first row among the restricted rows) of every restricted
+                                                                          // pair of the call, nrp of them; nrows restricted rows in all
+    const unsigned long long* keys; const int* nkeys;                     // sorted distinct candidate keys, their number (device)
+    int* counts; l3d_match_rec* recs;                                     // as MatchArgs
+    int knn;                                                              // TopK: k; Store: row stride; Count: unused
+    float epi;
+};
+// one warp per restricted row, CAND_WARPS warps per CTA: the row's candidates only, with k_match_topk's exact arithmetic and keep policy
+#define CAND_WARPS 8
+template <int SEM, Keep KEEP> __global__ void k_match_cand(CandArgs A);
+extern void (*const l3d_cand_kernels[2][3])(CandArgs);                     // every instantiation of k_match_cand: [SEM][KEEP]
 // level-1 pre-filter tables: one CTA per view pair of [first_pair, first_pair + gridDim.x): raw arcs + sort keys; after the sort
 // k_arcs_gather writes the packed arcs and, in a parallel array, their target segments, in window order
 __global__ void k_pair_arcs(const float4* __restrict__ segs, const L3DViewDev* __restrict__ views, const L3DPairDev* __restrict__ pairs,
-                            int first_pair, int enabled, double ext, uint4* __restrict__ raw, unsigned long long* __restrict__ keys,
-                            unsigned int* __restrict__ vals, L3DPairBasis* __restrict__ basis);
+                            int first_pair, int enabled, double ext, const int* __restrict__ restricted, uint4* __restrict__ raw,
+                            unsigned long long* __restrict__ keys, unsigned int* __restrict__ vals, L3DPairBasis* __restrict__ basis);
 __global__ void k_arcs_gather(long long n, const unsigned long long* __restrict__ keys, const unsigned int* __restrict__ vals,
                               const uint4* __restrict__ raw, const float4* __restrict__ segs, const L3DViewDev* __restrict__ views,
                               const L3DPairDev* __restrict__ pairs, int first_pair, uint4* __restrict__ out, float4* __restrict__ out_segs);

@@ -215,6 +215,11 @@ struct Line3D::Impl {
     std::set<unsigned int> reserved;
     std::mutex prep_mtx;
     struct { l3dpp_detect_fn fn; void* user; } c_detector{nullptr, nullptr};   // l3dpp_set_segment_detector
+    // setLineCandidates: per view pair (smaller camID, larger camID) its correspondences (segment of the smaller, of the larger); and for
+    // the pairs of one matchImages (stage_candidates) the flags, (pair, src_seg, tgt_seg) triples and listed counts of l3d_match_pairs_cand
+    std::map<std::pair<unsigned int, unsigned int>, std::vector<std::pair<unsigned int, unsigned int> > > cand_lists;
+    std::vector<int32_t> cand_restricted, cand_trip;
+    std::vector<long long> cand_count;
     // index maps (rebuilt at matchImages)
     std::vector<HostView*> vlist;                         // by view index (ascending camID)
     std::map<unsigned int, int> index_of;
@@ -346,11 +351,49 @@ struct Line3D::Impl {
                 for (int i = 0; i < 9; ++i) { F.push_back((float)Fd.m[i]); F_d.push_back(Fd.m[i]); }
             }
     }
-    // the pairs [first, last) in `parts` contiguous shares balanced by Ns*Nt: share p is [bounds[p], bounds[p + 1])
+    // The setLineCandidates lists of the pairs of this matchImages as l3d_match_pairs_cand takes them, in the direction list_pairs() chose;
+    // false (lastError set) for a segment ID beyond its view's segments.  Lists of pairs not matched are ignored.
+    bool stage_candidates()
+    {
+        cand_restricted.clear(); cand_trip.clear(); cand_count.clear();
+        if (cand_lists.empty()) return true;
+        const int npairs = (int)(pairs.size() / 2);
+        std::map<std::pair<unsigned int, unsigned int>, int> pair_of;
+        for (int i = 0; i < npairs; ++i) {
+            const unsigned int s = vlist[pairs[2 * i]]->id, t = vlist[pairs[2 * i + 1]]->id;
+            pair_of[std::make_pair(std::min(s, t), std::max(s, t))] = i;
+        }
+        cand_restricted.assign((size_t)npairs, 0); cand_count.assign((size_t)npairs, 0);
+        size_t ignored = 0;
+        for (const auto& kv : cand_lists) {
+            const auto it = pair_of.find(kv.first);
+            if (it == pair_of.end()) { ++ignored; continue; }
+            const int i = it->second;
+            const HostView &vs = *vlist[pairs[2 * i]], &vt = *vlist[pairs[2 * i + 1]];
+            const bool fwd = vs.id == kv.first.first;
+            cand_restricted[i] = 1; cand_count[i] = (long long)kv.second.size();
+            for (const auto& c : kv.second) {
+                const unsigned int a = fwd ? c.first : c.second, b = fwd ? c.second : c.first;
+                for (const auto& vs_seg : {std::make_pair(&vs, a), std::make_pair(&vt, b)})
+                    if (vs_seg.second >= vs_seg.first->lines.size()) {
+                        fail("setLineCandidates: segment " + std::to_string(vs_seg.second) + " of camera " + std::to_string(vs_seg.first->id) +
+                             " is beyond its " + std::to_string(vs_seg.first->lines.size()) + " segments");
+                        return false;
+                    }
+                cand_trip.push_back(i); cand_trip.push_back((int32_t)a); cand_trip.push_back((int32_t)b);
+            }
+        }
+        if (ignored) log("setLineCandidates: " + std::to_string(ignored) + " candidate list(s) ignored: their view pairs are not matched");
+        return true;
+    }
+    // the pairs [first, last) in `parts` contiguous shares balanced by their cost, Ns*Nt or a restricted pair's listed correspondences:
+    // share p is [bounds[p], bounds[p + 1])
     bool split_pairs(int first, int last, int parts, std::vector<int32_t>& bounds)
     {
         std::vector<long long> cost((size_t)(last - first));
-        for (int i = first; i < last; ++i) cost[i - first] = (long long)vlist[pairs[2 * i]]->lines.size() * (long long)vlist[pairs[2 * i + 1]]->lines.size();
+        for (int i = first; i < last; ++i)
+            cost[i - first] = !cand_restricted.empty() && cand_restricted[i] ? cand_count[i]
+                                                                             : (long long)vlist[pairs[2 * i]]->lines.size() * (long long)vlist[pairs[2 * i + 1]]->lines.size();
         bounds.resize((size_t)parts + 1);
         if (!chk(l3d_balanced_split(cost.data(), last - first, parts, bounds.data()), "l3d_balanced_split")) return false;
         for (int32_t& b : bounds) b += first;
@@ -359,7 +402,7 @@ struct Line3D::Impl {
     // the upload, this rank's share of the pairs (all without setShard) matched on this Line3D's devices, the exchange with the others
     bool match(const std::vector<l3d_view_desc>& d, const std::vector<const float*>& segp, float& ms_gather)
     {
-        if (!chk(l3d_set_views(ctx, (int)d.size(), d.data(), segp.data()), "l3d_set_views")) return false;
+        if (!chk(l3d_set_views(ctx, (int)d.size(), d.data(), segp.data()), "l3d_set_views") || !stage_candidates()) return false;
         const int npairs = (int)(pairs.size() / 2);
         if (shard_world == 1) return match_on_devices(0, npairs, d, segp, ms_gather) && chk(l3d_sync(ctx), "l3d_sync");
         std::vector<int32_t> bounds;
@@ -373,9 +416,14 @@ struct Line3D::Impl {
     {
         // use_GPU selects the reference's semantics, not the processor (line3D.cc:708-757): true = K_match_lines / K_score_matches
         // float arithmetic, false = matchingCPU / scoringCPU double arithmetic.  Both run on the GPU.
-        const char* match_what = use_gpu ? "l3d_match_pairs_range" : "l3d_match_pairs_f64";
+        const bool cand = !cand_restricted.empty();
+        const char* match_what = cand ? (use_gpu ? "l3d_match_pairs_cand" : "l3d_match_pairs_cand_f64") : use_gpu ? "l3d_match_pairs_range" : "l3d_match_pairs_f64";
         const int npairs = (int)(pairs.size() / 2);
+        const l3d_match_cand_desc cd = {cand_restricted.data(), cand_trip.data(), (long long)(cand_trip.size() / 3), 0};
         auto match_on = [&](l3d_ctx* c, int f, int l) {
+            if (cand)
+                return use_gpu ? l3d_match_pairs_cand(c, npairs, pairs.data(), F.data(), epi, kNN, f, l, &cd)
+                               : l3d_match_pairs_cand_f64(c, npairs, pairs.data(), F_d.data(), epi, kNN, f, l, &cd);
             return use_gpu ? l3d_match_pairs_range(c, npairs, pairs.data(), F.data(), epi, kNN, f, l)
                            : l3d_match_pairs_f64(c, npairs, pairs.data(), F_d.data(), epi, kNN, f, l);
         };
@@ -785,6 +833,26 @@ void Line3D::setSegmentDetector(SegmentDetectorFn detector, void* user)
     P.detector = detector; P.detector_user = user;
 }
 
+void Line3D::setLineCandidates(const unsigned int camA, const unsigned int camB, const std::vector<std::pair<unsigned int, unsigned int> >& seg_pairs)
+{
+    Impl& P = *p_;
+    std::lock_guard<std::mutex> g(P.mtx);
+    P.err.clear();
+    if (camA == camB) { P.fail("setLineCandidates: camA == camB (" + std::to_string(camA) + "): a view pair needs two cameras"); return; }
+    std::vector<std::pair<unsigned int, unsigned int> >& L = P.cand_lists[std::make_pair(std::min(camA, camB), std::max(camA, camB))];
+    L.clear();
+    L.reserve(seg_pairs.size());
+    for (const auto& c : seg_pairs) L.push_back(camA < camB ? c : std::make_pair(c.second, c.first));
+}
+
+void Line3D::clearLineCandidates()
+{
+    Impl& P = *p_;
+    std::lock_guard<std::mutex> g(P.mtx);
+    P.err.clear();
+    P.cand_lists.clear();
+}
+
 void Line3D::matchImages(const float sigma_position, const float sigma_angle, const unsigned int num_neighbors, const float epipolar_overlap,
                          const int kNN, const float const_regularization_depth)
 {
@@ -1127,6 +1195,16 @@ int l3dpp_match_images(void* h, float sp, float sa, unsigned int nn, float epi, 
 { Line3D* L = (Line3D*)h; L->matchImages(sp, sa, nn, epi, knn, crd); return L->lastError()[0] ? -1 : 0; }
 int l3dpp_reconstruct_opt(void* h, unsigned int vis, int diffusion, float collin, int use_ceres, unsigned int max_iter)
 { Line3D* L = (Line3D*)h; L->reconstruct3Dlines(vis, diffusion != 0, collin, use_ceres != 0, max_iter); return L->lastError()[0] ? -1 : 0; }
+int l3dpp_set_line_candidates(void* h, unsigned int cam_a, unsigned int cam_b, const unsigned int* seg_pairs, long long n)
+{
+    Line3D* L = (Line3D*)h;
+    if (n < 0 || (n > 0 && !seg_pairs)) { L->impl()->fail("setLineCandidates: n < 0, or no correspondence array for n > 0"); return -1; }
+    std::vector<std::pair<unsigned int, unsigned int> > v((size_t)n);
+    for (size_t i = 0; i < v.size(); ++i) v[i] = std::make_pair(seg_pairs[2 * i], seg_pairs[2 * i + 1]);
+    L->setLineCandidates(cam_a, cam_b, v);
+    return L->lastError()[0] ? -1 : 0;
+}
+int l3dpp_clear_line_candidates(void* h) { Line3D* L = (Line3D*)h; L->clearLineCandidates(); return L->lastError()[0] ? -1 : 0; }
 int l3dpp_set_shard(void* h, int rank, int world, l3dpp_exchange_fn fn, void* user)
 { Line3D* L = (Line3D*)h; L->setShard(rank, world, fn, user); return L->lastError()[0] ? -1 : 0; }
 int l3dpp_stats(void* h, l3dpp_stats_block* out) { memcpy(out, &((Line3D*)h)->stats(), sizeof(*out)); return 0; }

@@ -111,6 +111,19 @@ class Line3D:
         self._detector = cb                     # the library keeps the pointer: keep the callback alive
         self.L.l3dpp_set_segment_detector(self.h, cb, None)
 
+    def set_line_candidates(self, cam_a, cam_b, seg_pairs):
+        """Line3D::setLineCandidates: match the view pair {cam_a, cam_b} only against seg_pairs, an (n, 2) integer array of (segment of
+        cam_a, segment of cam_b); empty: no matches on the pair.  Replaces the pair's earlier list; kept until clear_line_candidates"""
+        a = np.asarray(seg_pairs, np.int64).reshape(-1, 2)
+        if (a < 0).any() or (a > 0xFFFFFFFF).any():
+            raise ValueError("segment IDs must be in [0, 2^32)")
+        a = np.ascontiguousarray(a, np.uint32)
+        self._chk(self.L.l3dpp_set_line_candidates(self.h, int(cam_a), int(cam_b), _p(a), len(a)), "setLineCandidates")
+
+    def clear_line_candidates(self):
+        """Line3D::clearLineCandidates: every view pair is scanned again"""
+        self._chk(self.L.l3dpp_clear_line_candidates(self.h), "clearLineCandidates")
+
     def view_segments(self, cam):
         """float32 [n, 4]: the view's 2D segments as getSegmentCoords2D returns them"""
         n = self.L.l3dpp_view_segments(self.h, int(cam), None, 0)
