@@ -13,7 +13,7 @@
  * 0 on success or a negative l3d_status; l3d_last_error() gives the message (the reference prints CUDA errors to
  * cerr and carries on, dataArray.h:198-237).  A call that fails leaves its stage (views, matches, score sweep,
  * collinear lists, affinity matrix), and every stage computed from it, without a result: later calls that need one
- * return L3D_ERR_STATE.  The image calls (l3d_undistort_u8, l3d_undistort_map, l3d_remap_u8, l3d_prepare_gray_u8, l3d_decode_jpeg_gray_u8) and the tie-point calls
+ * return L3D_ERR_STATE.  The image calls (l3d_undistort_u8, l3d_undistort_map, l3d_remap_u8, l3d_prepare_gray_u8, l3d_decode_jpeg_gray_u8, l3d_decode_png_gray_u8) and the tie-point calls
  * (l3d_triangulate_points, l3d_median_depths) are not part of that chain: whether
  * they succeed or fail, every stage and its result stay as they were.  A context is single-owner (not thread-safe), one per GPU, and runs
  * on its own non-default stream.  There is NO CPU fallback: without a usable CUDA device l3d_ctx_create fails.
@@ -401,6 +401,33 @@ typedef struct {
  * Corrupt entropy-coded data (no Huffman code matches, AC coefficients past index 63, a segment that ends early) is found on the GPU:
  * L3D_ERR_INVALID naming the first such image; host dst buffers are then untouched, device ones hold undefined bytes. */
 int l3d_decode_jpeg_gray_u8(l3d_ctx* ctx, int n, const l3d_jpeg_desc* descs, int on_device);
+
+/* ---- PNG decoding: cv::imread(path, IMREAD_GRAYSCALE) of a PNG file, byte for byte as OpenCV 4.13 returns it on x86 (libpng's
+ * conversions as OpenCV sets them up, then OpenCV's EXIF orientation from an eXIf chunk).  DESIGN.md §4d.
+ * Supported: every colour type and bit depth, Adam7 interlacing, PLTE (indices past its entries read black), tRNS (no effect: alpha
+ * is dropped), gAMA / sRGB on grey images (no effect) and on colour images of 8 bits or less (libpng's gamma tables), eXIf, split and
+ * empty IDAT chunks, ancillary chunks that do not change the pixels.  Rejected with a message that names the reason: a bad CRC in
+ * any chunk, iCCP, cHRM, cICP, gamma on 16-bit colour, APNG chunks, chunks out of place, unknown critical chunks, a palette image
+ * without PLTE, a side above 1,000,000 or more than 2^30 pixels, a bad zlib header or preset dictionary, and corrupt data that
+ * libpng would only warn about (extra compressed data, data after the zlib stream) or fail on.
+ * Not part of the pipeline chain: every stage and its result stay as they were. */
+/* size of imread(IMREAD_GRAYSCALE)'s output (after EXIF orientation); needs no context and no GPU.  L3D_OK, or L3D_ERR_INVALID for a
+ * file outside the subset above (readPNGSize of include/line3d_io.h gives the reason) or a null pointer */
+int l3d_png_info(const uint8_t* data, int64_t size, int32_t* out_width, int32_t* out_height);
+typedef struct {
+    const uint8_t* data; int64_t size;   /* the file's bytes, always HOST memory (the chunks are parsed on the host) */
+    uint8_t* dst; int64_t dst_pitch;     /* out_height rows of out_width grey bytes */
+    int32_t out_width, out_height;       /* from l3d_png_info */
+} l3d_png_desc;
+/* decode n files in three launches (inflate: one warp per image; unfiltering: a diagonal wavefront over bands of rows per Adam7
+ * pass; grey conversion and store: one thread per output pixel); sizes, formats and orientations may all differ.  on_device as for
+ * l3d_decode_jpeg_gray_u8; only the IDAT payload is uploaded, and bytes of dst beyond each row's out_width stay untouched.
+ * A descriptor with no data, a file outside the subset, a null dst, an out size other than l3d_png_info's or a dst_pitch below
+ * out_width is rejected (L3D_ERR_INVALID, l3d_last_error naming the first bad index and the reason) before anything is launched.
+ * A corrupt zlib stream (bad block type, stored length, code-length set or code, a distance past the output start or the window,
+ * too much or too little data, data after the stream, a wrong Adler-32) or a bad filter type is found on the GPU: L3D_ERR_INVALID
+ * naming the first such image; host dst buffers are then untouched, device ones hold undefined bytes. */
+int l3d_decode_png_gray_u8(l3d_ctx* ctx, int n, const l3d_png_desc* descs, int on_device);
 
 /* ---- tie-point triangulation:linearHomTriangulation of the reference's Pix4D frontend (main_pix4d.cpp:34-70, 354-372) for every point
  * in one launch.  Point i has the observations [obs_ptr[i], obs_ptr[i+1]) (obs_ptr[0] = 0): camera obs_cam[o] in [0, n_cams) and image

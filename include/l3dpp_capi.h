@@ -116,6 +116,20 @@ void l3dpp_jpegs_close(void* h);
 /* file i of the batch: its size, and its packed grey pixels into out[cap] when cap >= width * height; -1 with the file's error in err */
 int l3dpp_jpegs_image(void* h, int i, int* width, int* height, unsigned char* out, long long cap, char* err, int errcap);
 
+/* ---- PNG files, and JPEG or PNG by signature (csrc/line3d_png.cc) */
+/* readPNGSize: imread(IMREAD_GRAYSCALE)'s size; 0, or -1 with the reason in err.  No GPU */
+int l3dpp_png_size(const char* path, int* width, int* height, char* err, int errcap);
+/* readPNGsGray of n files on CUDA device cuda_device: a handle for l3dpp_pngs_image (never NULL; failures are per file) */
+void* l3dpp_pngs_read(const char* const* paths, int n, int cuda_device);
+void l3dpp_pngs_close(void* h);
+/* file i of the batch: its size, and its packed grey pixels into out[cap] when cap >= width * height; -1 with the file's error in err */
+int l3dpp_pngs_image(void* h, int i, int* width, int* height, unsigned char* out, long long cap, char* err, int errcap);
+/* readImageSize / readImagesGray: the same for JPEG and PNG files, chosen by each file's signature */
+int l3dpp_image_size(const char* path, int* width, int* height, char* err, int errcap);
+void* l3dpp_images_read(const char* const* paths, int n, int cuda_device);
+void l3dpp_images_close(void* h);
+int l3dpp_images_image(void* h, int i, int* width, int* height, unsigned char* out, long long cap, char* err, int errcap);
+
 /* ---- .nvm models (csrc/line3d_sfm.cc) */
 void* l3dpp_nvm_open(const char* path, char* err, int errcap);
 void l3dpp_nvm_close(void* h);

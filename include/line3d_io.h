@@ -95,6 +95,17 @@ bool readJPEGSize(const std::string& path, int& width, int& height, std::string*
 bool readJPEGGray(const std::string& path, Image8u& image, std::string* error = 0, int cuda_device = 0);
 bool readJPEGsGray(const std::vector<std::string>& paths, std::vector<Image8u>& images, std::vector<std::string>* errors = 0, int cuda_device = 0);
 
+/* The same for PNG files (l3d_decode_png_gray_u8 of include/l3d_capi.h; the subset and the rejections are listed there): readPNGSize,
+ * readPNGGray and readPNGsGray behave as the JPEG trio above.  readImageSize, readImageGray and readImagesGray take JPEG and PNG
+ * files alike, chosen by each file's signature; readImagesGray decodes a mixed list with one JPEG batch and one PNG batch, and any
+ * other file fails on its own with the reason. */
+bool readPNGSize(const std::string& path, int& width, int& height, std::string* error = 0);
+bool readPNGGray(const std::string& path, Image8u& image, std::string* error = 0, int cuda_device = 0);
+bool readPNGsGray(const std::vector<std::string>& paths, std::vector<Image8u>& images, std::vector<std::string>* errors = 0, int cuda_device = 0);
+bool readImageSize(const std::string& path, int& width, int& height, std::string* error = 0);
+bool readImageGray(const std::string& path, Image8u& image, std::string* error = 0, int cuda_device = 0);
+bool readImagesGray(const std::vector<std::string>& paths, std::vector<Image8u>& images, std::vector<std::string>* errors = 0, int cuda_device = 0);
+
 /* K of main_vsfm.cpp:266-278: focal on the diagonal, principal point at the image centre (float arithmetic like the reference) */
 Matrix3d intrinsicsFromFocal(float focal, int image_width, int image_height);
 

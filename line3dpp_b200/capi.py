@@ -133,6 +133,22 @@ def jpeg_info(data):
     return w.value, h.value
 
 
+class PngDesc(C.Structure):
+    """l3d_png_desc: one PNG file (host bytes) and its grey output"""
+    _fields_ = JpegDesc._fields_
+
+
+def png_info(data):
+    """(width, height) of imread(IMREAD_GRAYSCALE)'s output for a PNG file's bytes (l3d_png_info; after EXIF orientation).  Raises
+    L3DError for a file outside the supported subset (line3d.png_size names the reason)."""
+    b = bytes(data)
+    w, h = C.c_int32(), C.c_int32()
+    rc = lib().l3d_png_info(b, len(b), C.byref(w), C.byref(h))
+    if rc < 0:
+        raise L3DError(f"l3d_png_info failed ({rc}): not a PNG file l3d_decode_png_gray_u8 reads")
+    return w.value, h.value
+
+
 def _device_rows(o):
     """(address, row pitch in bytes, (rows, cols)) of a 2-D uint8 array in GPU memory that exposes __cuda_array_interface__"""
     ai = o.__cuda_array_interface__
@@ -559,14 +575,21 @@ class Context:
         new uint8 [h, w] host arrays.  out: one output per file, all host numpy arrays or all GPU arrays exposing
         __cuda_array_interface__ (e.g. torch CUDA tensors) of shape [h, w] with packed rows and any row pitch; GPU outputs are written
         in place (on_device=1), ready for undistort_device / prepare_gray_device.  Returns the outputs."""
+        return self._decode_gray(files, out, jpeg_info, JpegDesc, "l3d_decode_jpeg_gray_u8")
+
+    def decode_png_gray(self, files, out=None):
+        """l3d_decode_png_gray_u8: the same as decode_jpeg_gray for a list of PNG files (bytes)"""
+        return self._decode_gray(files, out, png_info, PngDesc, "l3d_decode_png_gray_u8")
+
+    def _decode_gray(self, files, out, info, Desc, fn):
         n = len(files)
         data = [bytes(f) for f in files]
-        sizes = [jpeg_info(d) for d in data]
+        sizes = [info(d) for d in data]
         device = out is not None and n > 0 and hasattr(out[0], "__cuda_array_interface__")
         outs = [np.empty((h, w), np.uint8) for w, h in sizes] if out is None else list(out)
         if len(outs) != n:
             raise ValueError("out needs one array per file")
-        descs = (JpegDesc * n)()
+        descs = (Desc * n)()
         for i, (d, (w, h)) in enumerate(zip(data, sizes)):
             if device:
                 addr, pitch, shape = _device_rows(outs[i])
@@ -580,12 +603,16 @@ class Context:
             descs[i].data = C.cast(C.c_char_p(d), C.c_void_p).value
             descs[i].size, descs[i].dst, descs[i].dst_pitch = len(d), addr, pitch
             descs[i].out_width, descs[i].out_height = w, h
-        self._chk(self.L.l3d_decode_jpeg_gray_u8(self.h, n, descs, int(device)), "l3d_decode_jpeg_gray_u8")
+        self._chk(getattr(self.L, fn)(self.h, n, descs, int(device)), fn)
         return outs
 
     def decode_jpeg_gray_descs(self, descs, on_device):
         """l3d_decode_jpeg_gray_u8 on a ctypes array of JpegDesc as given (for tests of the checks)"""
         self._chk(self.L.l3d_decode_jpeg_gray_u8(self.h, len(descs), descs, int(on_device)), "l3d_decode_jpeg_gray_u8")
+
+    def decode_png_gray_descs(self, descs, on_device):
+        """l3d_decode_png_gray_u8 on a ctypes array of PngDesc as given (for tests of the checks)"""
+        self._chk(self.L.l3d_decode_png_gray_u8(self.h, len(descs), descs, int(on_device)), "l3d_decode_png_gray_u8")
 
     def prepare_gray_device(self, descs):
         """l3d_prepare_gray_u8 on device addresses (a ctypes array of ImagePrepDesc); asynchronous on the context's stream"""

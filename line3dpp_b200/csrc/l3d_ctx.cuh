@@ -152,6 +152,32 @@ struct JpegState {
     DevBuf d_imgs, d_segs, d_tabs, d_bytes, d_coefs, d_status;
 };
 
+// per-image parameters of the PNG kernels (l3d_png.cu)
+struct L3DPngImage {
+    unsigned char* dst;
+    long long dst_pitch, in0, in_len, raw0, raw_size, pix0;   // in0 / in_len: the zlib stream in d_in; raw0: the filtered rows in d_raw; pix0: first output pixel in the batch grid
+    long long pass_off[7], pass_rb[7];       // per Adam7 pass: offset in the raw bytes, bytes per row (pass 0 only when not interlaced)
+    int width, height, depth, color_type, channels, interlace, window;   // window: the zlib header's window in bytes
+    int out_width, out_height, gamma;
+    int ryy, ryx, ry0, rxy, rxx, rx0;        // EXIF orientation: the pixel (y, x) goes to row ryy*y + ryx*x + ry0, column rxy*y + rxx*x + rx0
+    unsigned char palette[768], to_linear[256], from_linear[256];
+};
+
+// one Adam7 pass of one image for k_png_unfilter: rows of rb bytes (after the filter byte) at raw offset off, bpp bytes per unit
+struct L3DPngPass {
+    long long off;
+    int image, rows, rb, bpp;
+};
+
+// buffers of the PNG decode: not a pipeline stage, nothing else reads them
+struct PngState {
+    std::vector<L3DPngImage> h_imgs;
+    std::vector<L3DPngPass> h_passes;
+    std::vector<unsigned char> h_in;                    // the batch's zlib streams, concatenated
+    std::vector<int> h_status;
+    DevBuf d_imgs, d_passes, d_in, d_raw, d_status;
+};
+
 // buffers of the median-depth call (l3d_triangulate.cu): not a pipeline stage either
 struct TriangulateState {
     DevBuf d_keys, d_keys2;
@@ -209,6 +235,7 @@ struct l3d_ctx {
     UndistortState undist;
     ImagePrepState prep;
     JpegState jpeg;
+    PngState png;
     TriangulateState tri;
 
     const float4* segs() const { return segs_ext ? segs_ext : (const float4*)d_segs.p; }

@@ -9,6 +9,7 @@
 // The arithmetic contract is DESIGN.md §4c; tests/jpeg_model.py restates it.  Not a pipeline stage: only JpegState's buffers and, in host
 // mode, the context's staging pair change.
 #include "l3d_ctx.cuh"
+#include "l3d_exif.h"
 #include "l3d_jpeg.h"
 
 #include <climits>
@@ -255,18 +256,8 @@ static void jp_table(const L3DJpegHuffSpec& s, L3DJpegTable& t)
 // the orientation as an affine map of (y, x) in a width x height frame (OpenCV's ExifTransform)
 static void jp_orientation(L3DJpegImage& d, int o)
 {
-    const int W = d.width, H = d.height;
-    int a[6] = {1, 0, 0, 0, 1, 0};   // row = a0*y + a1*x + a2, col = a3*y + a4*x + a5
-    switch (o) {
-    case 2: { int b[6] = {1, 0, 0, 0, -1, W - 1}; memcpy(a, b, sizeof(a)); break; }
-    case 3: { int b[6] = {-1, 0, H - 1, 0, -1, W - 1}; memcpy(a, b, sizeof(a)); break; }
-    case 4: { int b[6] = {-1, 0, H - 1, 0, 1, 0}; memcpy(a, b, sizeof(a)); break; }
-    case 5: { int b[6] = {0, 1, 0, 1, 0, 0}; memcpy(a, b, sizeof(a)); break; }
-    case 6: { int b[6] = {0, 1, 0, -1, 0, H - 1}; memcpy(a, b, sizeof(a)); break; }
-    case 7: { int b[6] = {0, -1, W - 1, -1, 0, H - 1}; memcpy(a, b, sizeof(a)); break; }
-    case 8: { int b[6] = {0, -1, W - 1, 1, 0, 0}; memcpy(a, b, sizeof(a)); break; }
-    default: break;
-    }
+    int a[6];
+    l3d_orientation_map(o, d.width, d.height, a);
     d.ryy = a[0]; d.ryx = a[1]; d.ry0 = a[2]; d.rxy = a[3]; d.rxx = a[4]; d.rx0 = a[5];
 }
 

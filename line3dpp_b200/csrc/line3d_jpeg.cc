@@ -5,6 +5,8 @@
 // The subset is what libjpeg-turbo decodes to grey without colour conversion or upsampling: baseline and extended-sequential Huffman
 // (SOF0 / SOF1), 8-bit, one or three components with Y at the largest sampling factors, interleaved or not, with or without restart
 // intervals.  Everything else is rejected with a message that names the reason; so is corrupt data, which libjpeg would patch up.
+#include "l3d_exif.h"
+#include "l3d_image_files.h"
 #include "l3d_jpeg.h"
 #include "../../include/line3d_io.h"
 #include "../../include/l3d_capi.h"
@@ -21,26 +23,6 @@ static const uint8_t kZigZag[64] = {0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18
                                     62, 63};
 
 static bool fail(std::string& err, const std::string& msg) { err = msg; return false; }
-
-// OpenCV's ExifReader on an APP1 payload after "Exif\0\0": IFD0's tag 0x0112 as a 16-bit value in the TIFF byte order; 0 when the
-// block is broken or has no such tag (both mean: no transform)
-static int exif_orientation(const uint8_t* p, int64_t n)
-{
-    if (n < 8 || !((p[0] == 'I' && p[1] == 'I') || (p[0] == 'M' && p[1] == 'M'))) return 0;
-    const bool be = p[0] == 'M';
-    auto u16 = [&](int64_t o) { return be ? (p[o] << 8 | p[o + 1]) : (p[o + 1] << 8 | p[o]); };
-    auto u32 = [&](int64_t o) { return be ? ((uint32_t)u16(o) << 16 | (uint32_t)u16(o + 2)) : ((uint32_t)u16(o + 2) << 16 | (uint32_t)u16(o)); };
-    if (u16(2) != 0x2A) return 0;
-    const int64_t off = u32(4);
-    if (off + 2 > n) return 0;
-    const int count = u16(off);
-    for (int i = 0; i < count; ++i) {
-        const int64_t e = off + 2 + 12 * (int64_t)i;
-        if (e + 12 > n) return 0;
-        if (u16(e) == 0x0112) return u16(e + 8);
-    }
-    return 0;
-}
 
 // libjpeg's checks of a DHT table (jpeg_make_d_derived_tbl): no length overflows its code space; DC symbols are sizes up to 15
 static bool huff_ok(const L3DJpegHuffSpec& t, int count, bool dc)
@@ -122,7 +104,7 @@ bool l3d_jpeg_parse(const uint8_t* d, int64_t n, L3DJpegHeader& h, std::string& 
         pos = seg_end;
         if (m >= 0xE0 && m <= 0xEF) {
             if (m == 0xE0 && pn >= 14 && !memcmp(p, "JFIF\0", 5)) jfif = true;
-            else if (m == 0xE1 && !exif_seen && pn >= 6 && !memcmp(p, "Exif\0\0", 6)) { exif_seen = true; orient = exif_orientation(p + 6, pn - 6); }
+            else if (m == 0xE1 && !exif_seen && pn >= 6 && !memcmp(p, "Exif\0\0", 6)) { exif_seen = true; orient = l3d_exif_orientation(p + 6, pn - 6); }
             else if (m == 0xEE && pn >= 12 && !memcmp(p, "Adobe", 5)) adobe = p[11];
         } else if (m == 0xFE) {
         } else if (m == 0xDB) {
@@ -247,21 +229,12 @@ extern "C" int l3d_jpeg_info(const uint8_t* data, int64_t size, int32_t* out_wid
 // ------------------------------------------------------------------------------------------------ files
 namespace L3DPP {
 
-static bool read_file(const std::string& path, std::vector<uint8_t>& bytes, std::string& err)
-{
-    std::ifstream f(path.c_str(), std::ios::binary);
-    if (!f) return fail(err, path + ": cannot open file");
-    bytes.assign(std::istreambuf_iterator<char>(f), std::istreambuf_iterator<char>());
-    if (f.bad()) return fail(err, path + ": read error");
-    return true;
-}
-
 bool readJPEGSize(const std::string& path, int& width, int& height, std::string* error)
 {
     std::vector<uint8_t> bytes;
     std::string err;
     L3DJpegHeader h;
-    if (!read_file(path, bytes, err) || (!l3d_jpeg_parse(bytes.data(), (int64_t)bytes.size(), h, err) && (err = path + ": " + err, true))) {
+    if (!l3d_read_file(path, bytes, err) || (!l3d_jpeg_parse(bytes.data(), (int64_t)bytes.size(), h, err) && (err = path + ": " + err, true))) {
         if (error) *error = err;
         return false;
     }
@@ -271,45 +244,13 @@ bool readJPEGSize(const std::string& path, int& width, int& height, std::string*
 
 bool readJPEGsGray(const std::vector<std::string>& paths, std::vector<Image8u>& images, std::vector<std::string>* errors, int cuda_device)
 {
-    const size_t n = paths.size();
-    images.assign(n, Image8u());
-    std::vector<std::string> errs(n);
-    std::vector<std::vector<uint8_t> > files(n);
-    std::vector<l3d_jpeg_desc> descs;
-    std::vector<size_t> which;
-    for (size_t i = 0; i < n; ++i) {
-        L3DJpegHeader h;
-        std::string err;
-        if (!read_file(paths[i], files[i], err)) { errs[i] = err; continue; }
-        if (!l3d_jpeg_parse(files[i].data(), (int64_t)files[i].size(), h, err)) { errs[i] = paths[i] + ": " + err; continue; }
-        images[i] = Image8u(h.out_height, h.out_width, 1);
-        l3d_jpeg_desc d;
-        d.data = files[i].data(); d.size = (int64_t)files[i].size();
-        d.dst = images[i].data.data(); d.dst_pitch = h.out_width;
-        d.out_width = h.out_width; d.out_height = h.out_height;
-        descs.push_back(d);
-        which.push_back(i);
-    }
-    if (!descs.empty()) {
-        l3d_ctx* ctx = nullptr;
-        if (l3d_ctx_create(cuda_device, &ctx) != L3D_OK) {
-            for (size_t k : which) { errs[k] = paths[k] + ": no usable CUDA device (JPEG files are decoded on the GPU)"; images[k] = Image8u(); }
-        } else if (l3d_decode_jpeg_gray_u8(ctx, (int)descs.size(), descs.data(), 0) != L3D_OK) {
-            // a file whose coded data is corrupt fails the batch: decode one by one so that every file gets its own verdict
-            for (size_t j = 0; j < descs.size(); ++j)
-                if (l3d_decode_jpeg_gray_u8(ctx, 1, &descs[j], 0) != L3D_OK) {
-                    std::string e = l3d_last_error(ctx);
-                    const size_t colon = e.find("image 0: ");
-                    errs[which[j]] = paths[which[j]] + ": " + (colon == std::string::npos ? e : e.substr(colon + 9));
-                    images[which[j]] = Image8u();
-                }
-        }
-        l3d_ctx_destroy(ctx);
-    }
-    bool ok = true;
-    for (size_t i = 0; i < n; ++i) ok = ok && errs[i].empty();
-    if (errors) errors->swap(errs);
-    return ok;
+    auto parse = [](const uint8_t* d, int64_t n, int& w, int& h, std::string& err) {
+        L3DJpegHeader hd;
+        if (!l3d_jpeg_parse(d, n, hd, err)) return false;
+        w = hd.out_width; h = hd.out_height;
+        return true;
+    };
+    return l3d_read_gray_files<l3d_jpeg_desc>(paths, images, errors, cuda_device, parse, l3d_decode_jpeg_gray_u8, "JPEG");
 }
 
 bool readJPEGGray(const std::string& path, Image8u& image, std::string* error, int cuda_device)
@@ -325,11 +266,6 @@ bool readJPEGGray(const std::string& path, Image8u& image, std::string* error, i
 }  // namespace L3DPP
 
 // C wrappers (include/l3dpp_capi.h): a batch of decoded files is a handle
-struct L3DJpegBatch {
-    std::vector<L3DPP::Image8u> images;
-    std::vector<std::string> errors;
-};
-
 extern "C" {
 int l3dpp_jpeg_size(const char* path, int* width, int* height, char* err, int errcap)
 {
@@ -340,21 +276,15 @@ int l3dpp_jpeg_size(const char* path, int* width, int* height, char* err, int er
 
 void* l3dpp_jpegs_read(const char* const* paths, int n, int cuda_device)
 {
-    L3DJpegBatch* b = new L3DJpegBatch();
+    L3DImageBatch* b = new L3DImageBatch();
     L3DPP::readJPEGsGray(std::vector<std::string>(paths, paths + (n > 0 ? n : 0)), b->images, &b->errors, cuda_device);
     return b;
 }
 
-void l3dpp_jpegs_close(void* h) { delete (L3DJpegBatch*)h; }
+void l3dpp_jpegs_close(void* h) { delete (L3DImageBatch*)h; }
 
 int l3dpp_jpegs_image(void* h, int i, int* width, int* height, unsigned char* out, long long cap, char* err, int errcap)
 {
-    const L3DJpegBatch* b = (const L3DJpegBatch*)h;
-    if (i < 0 || i >= (int)b->images.size()) { l3dpp_copy_str("no such image", err, errcap); return -1; }
-    if (!b->errors[i].empty()) { l3dpp_copy_str(b->errors[i], err, errcap); return -1; }
-    const L3DPP::Image8u& im = b->images[i];
-    *width = im.cols; *height = im.rows;
-    if (out && cap >= (long long)im.data.size()) memcpy(out, im.data.data(), im.data.size());
-    return 0;
+    return l3d_batch_image(h, i, width, height, out, cap, err, errcap);
 }
 }

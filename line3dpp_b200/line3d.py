@@ -458,26 +458,60 @@ def read_jpeg_gray(path_or_paths, device=0, errors=None):
     """readJPEGGray / readJPEGsGray: imread(path, IMREAD_GRAYSCALE) as uint8 [h, w], decoded on GPU `device`; a list of paths is one
     batched decode and gives a list.  A file that fails raises L3DError with its message, unless a list `errors` is given: then every
     failed file's entry is None, and errors receives one message per file ("" for the decoded ones)."""
+    return _read_gray("jpegs", path_or_paths, device, errors)
+
+
+def png_size(path):
+    """readPNGSize: jpeg_size for a PNG file"""
+    return _size(capi.lib().l3dpp_png_size, path)
+
+
+def read_png_gray(path_or_paths, device=0, errors=None):
+    """readPNGGray / readPNGsGray: read_jpeg_gray for PNG files"""
+    return _read_gray("pngs", path_or_paths, device, errors)
+
+
+def image_size(path):
+    """readImageSize: jpeg_size or png_size, chosen by the file's signature"""
+    return _size(capi.lib().l3dpp_image_size, path)
+
+
+def read_image_gray(path_or_paths, device=0, errors=None):
+    """readImageGray / readImagesGray: read_jpeg_gray for JPEG and PNG files alike, each chosen by its signature; a mixed list is one
+    JPEG batch and one PNG batch.  Any other file fails with the reason."""
+    return _read_gray("images", path_or_paths, device, errors)
+
+
+def _size(fn, path):
+    w, h = C.c_int(), C.c_int()
+    err = C.create_string_buffer(4096)
+    if fn(str(path).encode(), C.byref(w), C.byref(h), err, 4096) != 0:
+        raise capi.L3DError(err.value.decode(errors="replace"))
+    return w.value, h.value
+
+
+def _read_gray(kind, path_or_paths, device, errors):
     single = isinstance(path_or_paths, (str, bytes)) or hasattr(path_or_paths, "__fspath__")
     paths = [path_or_paths] if single else list(path_or_paths)
     L = capi.lib()
+    read, image, close = (getattr(L, f"l3dpp_{kind}_{f}") for f in ("read", "image", "close"))
     arr = (C.c_char_p * len(paths))(*[str(p).encode() for p in paths])
-    h = L.l3dpp_jpegs_read(arr, len(paths), int(device))
+    h = read(arr, len(paths), int(device))
     outs, msgs = [], []
     try:
         for i in range(len(paths)):
             w, ht = C.c_int(), C.c_int()
             err = C.create_string_buffer(4096)
-            if L.l3dpp_jpegs_image(h, i, C.byref(w), C.byref(ht), None, 0, err, 4096) != 0:
+            if image(h, i, C.byref(w), C.byref(ht), None, 0, err, 4096) != 0:
                 outs.append(None)
                 msgs.append(err.value.decode(errors="replace"))
                 continue
             o = np.empty((ht.value, w.value), np.uint8)
-            L.l3dpp_jpegs_image(h, i, C.byref(w), C.byref(ht), _p(o), o.size, err, 4096)
+            image(h, i, C.byref(w), C.byref(ht), _p(o), o.size, err, 4096)
             outs.append(o)
             msgs.append("")
     finally:
-        L.l3dpp_jpegs_close(h)
+        close(h)
     if errors is not None:
         errors[:] = msgs
     elif any(msgs):
