@@ -13,7 +13,7 @@
  * 0 on success or a negative l3d_status; l3d_last_error() gives the message (the reference prints CUDA errors to
  * cerr and carries on, dataArray.h:198-237).  A call that fails leaves its stage (views, matches, score sweep,
  * collinear lists, affinity matrix), and every stage computed from it, without a result: later calls that need one
- * return L3D_ERR_STATE.  The image calls (l3d_undistort_u8, l3d_undistort_map, l3d_remap_u8, l3d_prepare_gray_u8, l3d_decode_jpeg_gray_u8, l3d_decode_png_gray_u8) and the tie-point calls
+ * return L3D_ERR_STATE.  The image calls (l3d_undistort_u8, l3d_undistort_map, l3d_remap_u8, l3d_undistort_points, l3d_prepare_gray_u8, l3d_decode_jpeg_gray_u8, l3d_decode_png_gray_u8) and the tie-point calls
  * (l3d_triangulate_points, l3d_median_depths) are not part of that chain: whether
  * they succeed or fail, every stage and its result stay as they were.  A context is single-owner (not thread-safe), one per GPU, and runs
  * on its own non-default stream.  There is NO CPU fallback: without a usable CUDA device l3d_ctx_create fails.
@@ -350,6 +350,26 @@ int l3d_undistort_map(l3d_ctx* ctx, const l3d_undistort_desc* desc, int16_t* map
 /* cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) of one image with caller-given maps in that layout, of the output size (the camera and
  * the new K are not used) */
 int l3d_remap_u8(l3d_ctx* ctx, const l3d_undistort_desc* desc, const int16_t* map_xy, const uint16_t* map_frac, int on_device);
+
+/* ---- lens undistortion of points: OpenCV 4.13's cv::undistortPoints(src, dst, K, D, noArray(), P) for a RADTAN lens (its fixed five
+ * iterations, the fallback to the undistorted-camera point when the distortion factor turns negative, the final cast to float) and
+ * cv::fisheye::undistortPoints(src, dst, K, D, I, P) with its default criteria for a FISHEYE lens (at most ten Newton steps; a point that
+ * does not converge or whose angle changes sign gives (-1e6, -1e6)), with P the new camera matrix of `cam` (all zero: K).  The output is
+ * in pixels of P.  Points are float32 (x, y) pairs, e.g. the endpoints of segments (x1, y1, x2, y2); NaN and infinite inputs are computed
+ * as OpenCV computes them.  RADTAN output is bit-identical to OpenCV's; FISHEYE output may differ where the device's tan differs from
+ * the host's (DESIGN.md §4a).  dst == src is allowed; other overlaps between sets are not.  Only the camera, lens and new-K fields of
+ * `cam` are read (width, height, channels, the image pointers, pitches and output size are ignored) and checked as l3d_undistort_u8
+ * checks them, with the same messages; also rejected with L3D_ERR_INVALID: n < 0, a null descriptor array, count < 0, a null src or dst
+ * when count > 0.  on_device as for l3d_undistort_u8 (src and dst are device addresses, or host arrays staged through the context's
+ * buffers).  Not part of the pipeline chain: every stage and its result stay as they were. */
+typedef struct {
+    l3d_undistort_desc cam;        /* the camera, its lens and the new camera matrix */
+    int64_t count;                 /* number of points */
+    const float* src;              /* count (x, y) pairs */
+    float* dst;                    /* count (x, y) pairs */
+} l3d_points_desc;
+/* undistort n point sets in one launch (one thread per point); cameras, lenses and lengths may all differ */
+int l3d_undistort_points(l3d_ctx* ctx, int n, const l3d_points_desc* sets, int on_device);
 
 /* ---- image preparation for line detection: what the reference's detectLineSegments (line3D.cc:249-289) does to an image before LSD
  * sees it.  cvtColor(CV_RGB2GRAY) for 3 channels (channel 0 is R; OpenCV's 15-bit fixed point) or the grey pixels as they are, then,

@@ -49,6 +49,12 @@ int l3dpp_add_image(void* h, unsigned int cam, int w, int hgt, const double* K, 
 /* addImage with an image: rows x cols, 1 or 3 channels, row step in bytes; nseg == 0: no segments given */
 int l3dpp_add_image_pixels(void* h, unsigned int cam, const unsigned char* pixels, int rows, int cols, int channels, long long step, const double* K,
                            const double* R, const double* t, float median_depth, const unsigned int* list, int nlist, const float* segs, int nseg);
+/* the addImage overloads with a lens (include/line3d.h): lens9 = model, k[6], p[2]; the image and the segments are in the distorted image */
+int l3dpp_add_image_lens(void* h, unsigned int cam, int w, int hgt, const double* K, const double* R, const double* t, float median_depth,
+                         const unsigned int* list, int nlist, const double* lens9, const float* segs, int nseg);
+int l3dpp_add_image_pixels_lens(void* h, unsigned int cam, const unsigned char* pixels, int rows, int cols, int channels, long long step,
+                                const double* K, const double* R, const double* t, float median_depth, const unsigned int* list, int nlist,
+                                const double* lens9, const float* segs, int nseg);
 /* the detector of l3dpp_add_image_pixels (NULL: none); the library keeps fn and user */
 int l3dpp_set_segment_detector(void* h, l3dpp_detect_fn fn, void* user);
 /* appends n detections (x1, y1, x2, y2) to the `out` a detector was given; any number of calls */
@@ -100,6 +106,11 @@ int l3dpp_undistort_image_lens(const unsigned char* src, unsigned char* dst, int
  * out_rows x out_cols x channels (rows x cols x channels for 0, 0).  Same returns */
 int l3dpp_undistort_image_newk(const unsigned char* src, unsigned char* dst, int rows, int cols, int channels, const double* lens9, const double* K,
                                const double* newK, int out_rows, int out_cols, int device);
+/* Line3D::undistortPoints of n point sets in one launch on CUDA device `device` (the thread's current device is restored), in place: set i
+ * is counts[i] (x, y) pairs of xy, following set i - 1, with lens9[9 i..] (model, k[6], p[2]), K[9 i..] and newK[9 i..] (row-major; newK
+ * NULL or a set's nine zeros: its K).  0, -1 (std::invalid_argument) or -2 (std::runtime_error), with the message in err */
+int l3dpp_undistort_points(float* xy, const long long* counts, int n, const double* lens9, const double* K, const double* newK, int device, char* err,
+                           int errcap);
 /* Line3D::getOptimalNewCameraMatrix: newK[9] row-major, roi[4] = x, y, width, height.  0, or -1 (std::invalid_argument); no GPU used */
 int l3dpp_optimal_new_camera_matrix(const double* K, const double* lens9, int width, int height, double alpha, int new_width, int new_height,
                                     int center_principal_point, double* newK, int* roi);

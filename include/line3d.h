@@ -220,6 +220,21 @@ public:
                   const float median_depth, const std::list<unsigned int>& wps_or_neighbors,
                   const std::vector<Vec4f>& line_segments = std::vector<Vec4f>());
 
+    /* addImage for a camera with lens distortion (an addition): `image` and `line_segments` are in the DISTORTED image; the view is
+     * added as the undistorted camera K.  Given segments: their endpoints go through undistortPoints(lens, K) (in pixels of K), then as
+     * above.  No segments: the segment cache is read as above and its segments are used as stored (the cache holds detections in the
+     * undistorted image).  On a miss the image is undistorted into K and prepared on the GPU without leaving the device in between
+     * (l3d_undistort_u8 then l3d_prepare_gray_u8), and only the prepared image comes back for the detector: the segments, the cache
+     * written and the detector's input are byte for byte those of undistortImage(image, u, lens, K) followed by addImage(u).  An all-zero
+     * lens is the overload above.  A camera or lens l3d_undistort_u8 rejects rejects the view (lastError() set). */
+    bool addImage(const unsigned int camID, const Image8u& image, const Matrix3d& K, const Matrix3d& R, const Vector3d& t,
+                  const float median_depth, const std::list<unsigned int>& wps_or_neighbors, const LensDistortion& lens,
+                  const std::vector<Vec4f>& line_segments = std::vector<Vec4f>());
+    /* the (image_width, image_height) form: given segments are undistorted as above; an empty list reads the segment cache as stored */
+    bool addImage(const unsigned int camID, const int image_width, const int image_height, const Matrix3d& K, const Matrix3d& R,
+                  const Vector3d& t, const float median_depth, const std::list<unsigned int>& wps_or_neighbors, const LensDistortion& lens,
+                  const std::vector<Vec4f>& line_segments);
+
 #ifdef L3DPP_WITH_EIGEN_OPENCV
     /* The reference's exact signature (line3D.h:104-108) for CV_8UC1 / CV_8UC3 images of any row step: the image overload above.
      * With segments given only the image's size is used.  A template only so that this header also compiles against cv::Mat
@@ -332,6 +347,35 @@ public:
      * radtan lens instead. */
     static Matrix3d estimateNewCameraMatrixForUndistortRectify(const Matrix3d& K, const LensDistortion& lens, int width, int height, double balance = 0.0,
                                                                int new_width = 0, int new_height = 0, double fov_scale = 1.0);
+
+    /* Lens undistortion of points (an addition): cv::undistortPoints(xy, xy, K, D, noArray(), newK) for a RADTAN lens and
+     * cv::fisheye::undistortPoints(xy, xy, K, D, I, newK) for a FISHEYE lens, in place on interleaved x, y float pairs, on the GPU
+     * (include/l3d_capi.h l3d_undistort_points; DESIGN.md §4a).  The result is in pixels of newK; newK all zero (the default): K.  Uses
+     * K(0,0), K(1,1), K(0,2), K(1,2) and the same four entries of newK.  Runs on the calling thread's current CUDA device through a context
+     * that lives for the call.  Throws std::invalid_argument for an odd number of coordinates and for a camera, lens or new K
+     * l3d_undistort_points rejects, std::runtime_error on a CUDA failure or without a usable device. */
+    static void undistortPoints(std::vector<float>& xy, const LensDistortion& lens, const Matrix3d& K, const Matrix3d& newK = Matrix3d());
+    /* the same for both endpoints of every segment (x1, y1, x2, y2): what a segment detected in the distorted image is in the
+     * undistorted one, endpoints only */
+    static void undistortSegments(std::vector<Vec4f>& segs, const LensDistortion& lens, const Matrix3d& K, const Matrix3d& newK = Matrix3d());
+    /* many point sets, each with its own lens, K and new K, in one launch: xy[i] with lenses[i], K[i] and newK[i] (newK empty: every set
+     * into its K).  Same exceptions, and std::invalid_argument when the lists differ in length. */
+    static void undistortPoints(std::vector<std::vector<float> >& xy, const std::vector<LensDistortion>& lenses, const std::vector<Matrix3d>& K,
+                                const std::vector<Matrix3d>& newK = std::vector<Matrix3d>());
+#ifdef L3DPP_WITH_EIGEN_OPENCV
+    /* undistortSegments for cv::Vec4f segments (e.g. from cv::LineSegmentDetector or a segment file read into them) */
+    template <class MatT = cv::Mat>
+    static void undistortSegments(std::vector<cv::Vec4f>& segs, const LensDistortion& lens, const Eigen::Matrix3d& K,
+                                  const Eigen::Matrix3d& newK = Eigen::Matrix3d::Zero())
+    {
+        std::vector<Vec4f> s(segs.size());
+        for (size_t i = 0; i < segs.size(); ++i) for (int k = 0; k < 4; ++k) s[i].v[k] = segs[i](k);
+        Matrix3d Kp, nKp;
+        for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) { Kp(r, c) = K(r, c); nKp(r, c) = newK(r, c); }
+        undistortSegments(s, lens, Kp, nKp);
+        for (size_t i = 0; i < segs.size(); ++i) for (int k = 0; k < 4; ++k) segs[i](k) = s[i].v[k];
+    }
+#endif
 
 #ifdef L3DPP_WITH_EIGEN_OPENCV
     /* The reference's exact signature for CV_8UC1 / CV_8UC3 images; honours the row step of inImg and create()s outImg.  A template

@@ -88,6 +88,20 @@ def lens_desc_args(lens):
     return dict(model=int(lens.get("model", LENS_RADTAN)), radial=k[:3], tangential=p[:2], rational=k[3:6])
 
 
+class PointsDesc(C.Structure):
+    """l3d_points_desc: one set of float32 (x, y) points and its camera (the camera, lens and new-K fields of `cam`)"""
+    _fields_ = [("cam", UndistortDesc), ("count", C.c_int64), ("src", C.c_void_p), ("dst", C.c_void_p)]
+
+
+def make_points_desc(K, lens, count, src, dst, new_K=None):
+    """K: 3x3; lens: a lens dict (lens_desc_args); src / dst: addresses of count (x, y) float32 pairs; new_K: 3x3 (None: K)"""
+    d = PointsDesc()
+    d.cam = make_undistort_desc(0, 0, 0, K, new_K=new_K, **lens_desc_args(lens))
+    d.cam.src_pitch = d.cam.dst_pitch = 0
+    d.count, d.src, d.dst = int(count), int(src) or None, int(dst) or None
+    return d
+
+
 class ImagePrepDesc(C.Structure):
     """l3d_image_prep_desc: one 8-bit image, its max_img_width and the grey output"""
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("channels", C.c_int32), ("max_img_width", C.c_int32),
@@ -158,6 +172,17 @@ def _device_rows(o):
     if strides[1] != 1:
         raise ValueError("device output rows must be packed")
     return int(ai["data"][0]), int(strides[0]), tuple(ai["shape"])
+
+
+def _device_points(o):
+    """(address, number of (x, y) pairs) of a C-contiguous float32 array in GPU memory that exposes __cuda_array_interface__"""
+    ai = o.__cuda_array_interface__
+    if ai["typestr"] != "<f4" or ai.get("strides") is not None:
+        raise ValueError("device points must be a C-contiguous float32 array")
+    size = int(np.prod(ai["shape"]))
+    if size % 2:
+        raise ValueError("device points must hold (x, y) pairs")
+    return int(ai["data"][0]), size // 2
 
 
 def _image_rows(a):
@@ -550,6 +575,38 @@ class Context:
             outs.append(o)
         self._chk(self.L.l3d_undistort_u8(self.h, n, descs, 0), "l3d_undistort_u8")
         return outs
+
+    # ---- lens undistortion of points (stateless: no pipeline stage changes)
+    def undistort_points(self, sets, out=None):
+        """l3d_undistort_points for a list of (points, K, lens, new_K) sets in ONE batched call; points float32 [n, 2] (or anything of
+        2n floats), new_K None: K.  out=None: returns new float32 [n, 2] host arrays.  out: one output per set, all host numpy arrays or
+        all GPU arrays exposing __cuda_array_interface__ (then the points must be on the GPU too: on_device=1); an output may be its
+        set's points (in place).  Returns the outputs."""
+        n = len(sets)
+        descs, keep, outs = (PointsDesc * n)(), [], []
+        device = n > 0 and hasattr(sets[0][0], "__cuda_array_interface__")
+        for i, (pts, K, lens, new_K) in enumerate(sets):
+            if device:
+                src, m = _device_points(pts)
+                o = out[i]
+                dst, mo = _device_points(o)
+                if mo != m:
+                    raise ValueError(f"output {i} holds {mo} points, its set {m}")
+            else:
+                a = np.ascontiguousarray(pts, np.float32).reshape(-1, 2)
+                o = np.empty_like(a) if out is None else out[i]
+                if not isinstance(o, np.ndarray) or o.dtype != np.float32 or not o.flags.c_contiguous or o.size != a.size:
+                    raise ValueError("host output must be a C-contiguous float32 array of the set's size")
+                keep += [a, o]
+                src, dst, m = a.ctypes.data, o.ctypes.data, len(a)
+            descs[i] = make_points_desc(K, lens, m, src, dst, new_K)
+            outs.append(o)
+        self._chk(self.L.l3d_undistort_points(self.h, n, descs, int(device)), "l3d_undistort_points")
+        return outs
+
+    def undistort_points_descs(self, descs, on_device):
+        """l3d_undistort_points on a ctypes array of PointsDesc as given (for tests of the checks)"""
+        self._chk(self.L.l3d_undistort_points(self.h, len(descs), descs, int(on_device)), "l3d_undistort_points")
 
     # ---- image preparation for line detection (stateless: no pipeline stage changes)
     def prepare_gray(self, images, max_img_width):

@@ -93,11 +93,23 @@ struct L3DUndistImage {
     int out_width, out_height;               // the output grid (the source size unless one is given)
 };
 
+// per-set parameters of k_undistort_points (l3d_undistort.cu): the camera, OpenCV's distortion vector and the new camera matrix
+struct L3DPointSet {
+    const float* src;
+    float* dst;
+    long long p0;                            // first point of this set in the batch
+    double fx, fy, cx, cy, ifx, ify;         // the camera; ifx = 1 / fx, ify = 1 / fy (radtan multiplies by them, fisheye divides by f)
+    double k[8];                             // radtan: OpenCV's k[0..7] = k1 k2 p1 p2 k3 k4 k5 k6; fisheye: k1..k4
+    double nfx, nfy, ncx, ncy;               // the new camera matrix (the camera's own K unless one is given)
+    int fisheye;
+};
+
 // buffers of the undistortion calls: not a pipeline stage, nothing else reads them
 struct UndistortState {
     std::vector<L3DUndistImage> h_imgs;
     std::vector<double> h_cols;                          // fisheye column tables, one per distinct (ir0, ir2)
-    DevBuf d_imgs, d_cols;
+    std::vector<L3DPointSet> h_sets;                     // l3d_undistort_points
+    DevBuf d_imgs, d_cols, d_sets;
 };
 
 // per-image parameters of k_prepare_gray_u8 (l3d_image_prep.cu): source (width x height, 1 or 3 channels) -> grey out_w x out_h

@@ -1,6 +1,6 @@
 // l3d_undistort.cu — lens undistortion of 8-bit images: what Line3D::undistortImage computes with OpenCV (line3D.cc:83-109,
-// initUndistortRectifyMap with fixed-point CV_16SC2 + CV_16UC1 maps, then remap INTER_LINEAR / BORDER_CONSTANT 0), and the three
-// C-ABI entry points declared in include/l3d_capi.h.  Two lens models: OpenCV's standard one with up to 8 coefficients (radtan) and
+// initUndistortRectifyMap with fixed-point CV_16SC2 + CV_16UC1 maps, then remap INTER_LINEAR / BORDER_CONSTANT 0), the undistortion of
+// points as cv::undistortPoints / cv::fisheye::undistortPoints compute it, and the four C-ABI entry points declared in include/l3d_capi.h.  Two lens models: OpenCV's standard one with up to 8 coefficients (radtan) and
 // cv::fisheye's.  The output may have its own camera matrix and size (OpenCV's newCameraMatrix / newImageSize).  The arithmetic contract is DESIGN.md §4a; tests/undistort_model.py and tests/lens_model.py restate it.
 //
 // None of these calls belongs to the pipeline: they never drop a stage and touch only the buffers of UndistortState and, in host
@@ -187,7 +187,106 @@ __global__ void __launch_bounds__(UD_TW) k_undistort_u8(const L3DUndistImage* __
     }
 }
 
+// ------------------------------------------------------------------------------------------------ points
+// cv::undistortPoints(src, dst, K, D, noArray(), P) of one point: cvUndistortPointsInternal with TermCriteria(COUNT, 5, 0.01), so five
+// fixed-point steps and no reprojection error.  The identity tilt (invMatTilt) and rectification (RR = P * I) products are spelled
+// out as cv::Matx and cvMatMul sum them: they add only signed zeros to finite values, but make an infinite coordinate NaN.
+__device__ __forceinline__ void up_radtan(const L3DPointSet& s, double u, double v, double& X, double& Y)
+{
+    const double* k = s.k;
+    double x = (u - s.cx) * s.ifx, y = (v - s.cy) * s.ify;
+    const double tx = ((0.0 + 1.0 * x) + 0.0 * y) + 0.0 * 1.0, ty = ((0.0 + 0.0 * x) + 1.0 * y) + 0.0 * 1.0;
+    const double tz = ((0.0 + 0.0 * x) + 0.0 * y) + 1.0 * 1.0, inv = tz != 0.0 ? 1.0 / tz : 1.0;
+    const double x0 = inv * tx, y0 = inv * ty;
+    x = x0; y = y0;
+    for (int j = 0; j < 5; ++j) {
+        const double r2 = x * x + y * y;
+        const double icdist = (1.0 + ((k[7] * r2 + k[6]) * r2 + k[5]) * r2) / (1.0 + ((k[4] * r2 + k[1]) * r2 + k[0]) * r2);
+        if (icdist < 0.0) {                 // OpenCV's regression_14583 fallback: the point as if there were no distortion
+            x = (u - s.cx) * s.ifx;
+            y = (v - s.cy) * s.ify;
+            break;
+        }
+        // k[8..11] (thin prism) are zero; their products stay, for the NaN an infinite r2 gives
+        const double dx = (((2.0 * k[2]) * x) * y + k[3] * (r2 + (2.0 * x) * x) + 0.0 * r2) + (0.0 * r2) * r2;
+        const double dy = ((k[2] * (r2 + (2.0 * y) * y) + ((2.0 * k[3]) * x) * y) + 0.0 * r2) + (0.0 * r2) * r2;
+        x = (x0 - dx) * icdist;
+        y = (y0 - dy) * icdist;
+    }
+    const double xx = (s.nfx * x + 0.0 * y) + s.ncx, yy = (0.0 * x + s.nfy * y) + s.ncy;
+    const double ww = 1.0 / ((0.0 * x + 0.0 * y) + 1.0);
+    X = xx * ww; Y = yy * ww;
+}
+
+// cv::fisheye::undistortPoints(src, dst, K, D, I, P) of one point with its default TermCriteria(MAX_ITER + EPS, 10, 1e-8).  tan is the
+// device's (within an ulp or two of glibc's); the rest is IEEE double in OpenCV's order.
+__device__ __forceinline__ void up_fisheye(const L3DPointSet& s, double u, double v, double& X, double& Y)
+{
+    const double* k = s.k;
+    const double pwx = (u - s.cx) / s.fx, pwy = (v - s.cy) / s.fy;
+    const double hp = 3.14159265358979323846 / 2.0;
+    double td = sqrt(pwx * pwx + pwy * pwy);
+    td = -hp < td ? td : -hp;               // std::max(-pi/2, td): NaN becomes -pi/2
+    td = hp < td ? hp : td;                 // std::min(td, pi/2)
+    double theta = td, scale = 0.0;
+    bool converged = true;
+    if (fabs(td) > 1e-8) {
+        converged = false;
+        for (int j = 0; j < 10; ++j) {
+            const double t2 = theta * theta, t4 = t2 * t2, t6 = t4 * t2, t8 = t6 * t2;
+            const double a = k[0] * t2, b = k[1] * t4, c = k[2] * t6, d = k[3] * t8;
+            const double fix = (theta * (1.0 + a + b + c + d) - td) / (1.0 + 3.0 * a + 5.0 * b + 7.0 * c + 9.0 * d);
+            theta = theta - fix;
+            if (fabs(fix) < 1e-8) { converged = true; break; }
+        }
+        scale = tan(theta) / td;
+    }
+    const bool flipped = (td < 0.0 && theta > 0.0) || (td > 0.0 && theta < 0.0);
+    if (!converged || flipped) { X = -1000000.0; Y = -1000000.0; return; }
+    const double px = pwx * scale, py = pwy * scale;
+    const double rx = ((0.0 + s.nfx * px) + 0.0 * py) + s.ncx * 1.0, ry = ((0.0 + 0.0 * px) + s.nfy * py) + s.ncy * 1.0;
+    const double rz = ((0.0 + 0.0 * px) + 0.0 * py) + 1.0 * 1.0;
+    X = rx / rz; Y = ry / rz;
+}
+
+// one thread per point of all sets; a set is found by binary search over p0.  src and dst may be the same array (each thread reads
+// its point before it writes it).
+#define UP_THREADS 256
+__global__ void __launch_bounds__(UP_THREADS) k_undistort_points(const L3DPointSet* __restrict__ sets, int n, long long total)
+{
+    const long long i = (long long)blockIdx.x * UP_THREADS + threadIdx.x;
+    if (i >= total) return;
+    const L3DPointSet& s = sets[last_le(n, i, [&](int j) { return sets[j].p0; })];
+    const long long q = 2 * (i - s.p0);
+    const double u = s.src[q], v = s.src[q + 1];
+    double X, Y;
+    if (s.fisheye) up_fisheye(s, u, v, X, Y);
+    else up_radtan(s, u, v, X, Y);
+    s.dst[q] = (float)X;
+    s.dst[q + 1] = (float)Y;
+}
+
 // ------------------------------------------------------------------------------------------------ host side
+// the camera, lens and new-K checks of one descriptor
+static int ud_check_camera(l3d_ctx* c, const l3d_undistort_desc& u, const char* what)
+{
+    char buf[160];
+    auto bad = [&](const char* why) { snprintf(buf, sizeof(buf), "%s: %s", what, why); return l3d_fail(c, L3D_ERR_INVALID, buf); };
+    if (!std::isfinite(u.fx) || !std::isfinite(u.fy) || u.fx == 0.0 || u.fy == 0.0) return bad("fx and fy must be finite and non-zero");
+    bool finite = std::isfinite(u.cx) && std::isfinite(u.cy), zero = true;
+    for (int k = 0; k < 3; ++k) { finite = finite && std::isfinite(u.radial[k]) && std::isfinite(u.rational[k]); zero = zero && u.radial[k] == 0.0 && u.rational[k] == 0.0; }
+    for (int k = 0; k < 2; ++k) { finite = finite && std::isfinite(u.tangential[k]); zero = zero && u.tangential[k] == 0.0; }
+    for (int k = 0; k < 4; ++k) finite = finite && std::isfinite(u.fisheye[k]);
+    if (!finite) return bad("principal point and coefficients must be finite");
+    if (u.model != L3D_LENS_RADTAN && u.model != L3D_LENS_FISHEYE) return bad("unknown lens model");
+    if (u.model == L3D_LENS_FISHEYE && !zero) return bad("a fisheye lens takes no radial, tangential or rational coefficients");
+    const bool new_k = u.new_fx != 0.0 || u.new_fy != 0.0 || u.new_cx != 0.0 || u.new_cy != 0.0;
+    if (new_k && (!std::isfinite(u.new_fx) || !std::isfinite(u.new_fy) || u.new_fx == 0.0 || u.new_fy == 0.0))
+        return bad("new_fx and new_fy must be finite and non-zero");
+    if (new_k && (!std::isfinite(u.new_cx) || !std::isfinite(u.new_cy))) return bad("new_cx and new_cy must be finite");
+    return L3D_OK;
+}
+
 // checks one descriptor; `image`: the pixel pointers and pitches are used, `camera`: the intrinsics and coefficients are used
 static int ud_check(l3d_ctx* c, const l3d_undistort_desc& u, bool image, bool camera, const char* what)
 {
@@ -203,21 +302,26 @@ static int ud_check(l3d_ctx* c, const l3d_undistort_desc& u, bool image, bool ca
         if (!u.src || !u.dst) return bad("null image pointer");
         if (u.src == u.dst) return bad("src == dst (no in-place undistortion)");
     }
-    if (camera) {
-        if (!std::isfinite(u.fx) || !std::isfinite(u.fy) || u.fx == 0.0 || u.fy == 0.0) return bad("fx and fy must be finite and non-zero");
-        bool finite = std::isfinite(u.cx) && std::isfinite(u.cy), zero = true;
-        for (int k = 0; k < 3; ++k) { finite = finite && std::isfinite(u.radial[k]) && std::isfinite(u.rational[k]); zero = zero && u.radial[k] == 0.0 && u.rational[k] == 0.0; }
-        for (int k = 0; k < 2; ++k) { finite = finite && std::isfinite(u.tangential[k]); zero = zero && u.tangential[k] == 0.0; }
-        for (int k = 0; k < 4; ++k) finite = finite && std::isfinite(u.fisheye[k]);
-        if (!finite) return bad("principal point and coefficients must be finite");
-        if (u.model != L3D_LENS_RADTAN && u.model != L3D_LENS_FISHEYE) return bad("unknown lens model");
-        if (u.model == L3D_LENS_FISHEYE && !zero) return bad("a fisheye lens takes no radial, tangential or rational coefficients");
-        const bool new_k = u.new_fx != 0.0 || u.new_fy != 0.0 || u.new_cx != 0.0 || u.new_cy != 0.0;
-        if (new_k && (!std::isfinite(u.new_fx) || !std::isfinite(u.new_fy) || u.new_fx == 0.0 || u.new_fy == 0.0))
-            return bad("new_fx and new_fy must be finite and non-zero");
-        if (new_k && (!std::isfinite(u.new_cx) || !std::isfinite(u.new_cy))) return bad("new_cx and new_cy must be finite");
+    return camera ? ud_check_camera(c, u, what) : L3D_OK;
+}
+
+// kernel parameters of one point set (the new K: the camera's own when new_fx .. new_cy are all zero)
+static L3DPointSet up_set(const l3d_undistort_desc& u, const float* src, float* dst, long long p0)
+{
+    L3DPointSet s;
+    memset(&s, 0, sizeof(s));
+    s.src = src; s.dst = dst; s.p0 = p0;
+    s.fx = u.fx; s.fy = u.fy; s.cx = u.cx; s.cy = u.cy; s.ifx = 1.0 / u.fx; s.ify = 1.0 / u.fy;
+    const bool new_k = u.new_fx != 0.0 || u.new_fy != 0.0 || u.new_cx != 0.0 || u.new_cy != 0.0;
+    s.nfx = new_k ? u.new_fx : u.fx; s.nfy = new_k ? u.new_fy : u.fy; s.ncx = new_k ? u.new_cx : u.cx; s.ncy = new_k ? u.new_cy : u.cy;
+    s.fisheye = u.model == L3D_LENS_FISHEYE;
+    if (s.fisheye) {
+        for (int i = 0; i < 4; ++i) s.k[i] = u.fisheye[i];
+    } else {
+        const double k[8] = {u.radial[0], u.radial[1], u.tangential[0], u.tangential[1], u.radial[2], u.rational[0], u.rational[1], u.rational[2]};
+        memcpy(s.k, k, sizeof(k));
     }
-    return L3D_OK;
+    return s;
 }
 
 static int ud_out_width(const l3d_undistort_desc& u) { return u.out_width ? u.out_width : u.width; }
@@ -395,6 +499,57 @@ int l3d_remap_u8(l3d_ctx* c, const l3d_undistort_desc* desc, const int16_t* map_
     ++c->launches;
     L3D_CUDA(c, cudaGetLastError(), "k_remap_u8");
     if (!on_device && (rc = l3d_unstage_host(c, out, 1, "l3d_remap_u8"))) return rc;
+    return L3D_OK;
+}
+
+int l3d_undistort_points(l3d_ctx* c, int n, const l3d_points_desc* sets, int on_device)
+{
+    if (!c) return L3D_ERR_INVALID;
+    if (n < 0 || (n && !sets)) return l3d_fail(c, L3D_ERR_INVALID, "l3d_undistort_points: bad arguments");
+    char buf[160];
+    long long total = 0;
+    for (int i = 0; i < n; ++i) {
+        const l3d_points_desc& d = sets[i];
+        int rc = ud_check_camera(c, d.cam, "l3d_undistort_points");
+        if (rc) return rc;
+        if (d.count < 0 || (d.count > 0 && (!d.src || !d.dst))) {
+            snprintf(buf, sizeof(buf), "l3d_undistort_points: set %d: %s", i, d.count < 0 ? "count < 0" : "null point pointer");
+            return l3d_fail(c, L3D_ERR_INVALID, buf);
+        }
+        if (d.count > (1ll << 38) - total) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_undistort_points: more than 2^38 points in one call");
+        total += d.count;
+    }
+    if (total == 0) return L3D_OK;
+    cudaSetDevice(c->device);
+    UndistortState& s = c->undist;
+    int rc;
+    std::vector<HostBlock> in, out;         // host mode: the points of every non-empty set
+    if (!on_device) {
+        for (int i = 0; i < n; ++i)
+            if (sets[i].count) {
+                in.push_back(host_array(sets[i].src, 8 * (size_t)sets[i].count));
+                out.push_back(host_array(sets[i].dst, 8 * (size_t)sets[i].count));
+            }
+        if ((rc = l3d_stage_host(c, in.data(), (int)in.size(), out.data(), (int)out.size()))) return rc;
+    }
+    // the non-empty sets only: every point then lies in the set the search over p0 finds
+    s.h_sets.clear();
+    long long p0 = 0;
+    for (int i = 0; i < n; ++i) {
+        const l3d_points_desc& d = sets[i];
+        if (!d.count) continue;
+        const size_t j = s.h_sets.size();
+        s.h_sets.push_back(on_device ? up_set(d.cam, d.src, d.dst, p0) : up_set(d.cam, (const float*)in[j].dev, (float*)out[j].dev, p0));
+        p0 += d.count;
+    }
+    const int m = (int)s.h_sets.size();
+    L3D_RESERVE(s.d_sets, sizeof(L3DPointSet) * (size_t)m, "point set descriptors");
+    // pageable host memory: the copy is staged before the call returns, so h_sets may be rewritten by the next call right away
+    L3D_CUDA(c, cudaMemcpyAsync(s.d_sets.p, s.h_sets.data(), sizeof(L3DPointSet) * m, cudaMemcpyHostToDevice, c->stream), "upload point sets");
+    k_undistort_points<<<(unsigned int)((total + UP_THREADS - 1) / UP_THREADS), UP_THREADS, 0, c->stream>>>((const L3DPointSet*)s.d_sets.p, m, total);
+    ++c->launches;
+    L3D_CUDA(c, cudaGetLastError(), "k_undistort_points");
+    if (!on_device && (rc = l3d_unstage_host(c, out.data(), (int)out.size(), "l3d_undistort_points"))) return rc;
     return L3D_OK;
 }
 

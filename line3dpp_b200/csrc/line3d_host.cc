@@ -214,6 +214,11 @@ struct Line3D::Impl {
     Line3D::SegmentDetectorFn detector = nullptr; void* detector_user = nullptr;
     std::set<unsigned int> reserved;
     std::mutex prep_mtx;
+    // addImage with a lens: the source, undistorted and prepared image on the primary device (grow-only, used under prep_mtx)
+    struct DeviceScratch {
+        void* p = nullptr; size_t cap = 0; int device = 0;
+        ~DeviceScratch() { if (p) { int d = 0; cudaGetDevice(&d); cudaSetDevice(device); cudaFree(p); cudaSetDevice(d); } }
+    } prep_scratch;
     struct { l3dpp_detect_fn fn; void* user; } c_detector{nullptr, nullptr};   // l3dpp_set_segment_detector
     // setLineCandidates: per view pair (smaller camID, larger camID) its correspondences (segment of the smaller, of the larger); and for
     // the pairs of one matchImages (stage_candidates) the flags, (pair, src_seg, tgt_seg) triples and listed counts of l3d_match_pairs_cand
@@ -299,8 +304,10 @@ struct Line3D::Impl {
         assert(e >= 0);                                   // cluster members come from the affinity matrix: all have an estimate
         return Segment3D(Vector3d(est_P[6 * e], est_P[6 * e + 1], est_P[6 * e + 2]), Vector3d(est_P[6 * e + 3], est_P[6 * e + 4], est_P[6 * e + 5]));
     }
-    bool segments_from_image(unsigned int camID, const Image8u& image, Line3D::SegmentDetectorFn fn, void* user, std::vector<Vec4f>& segs,
-                             std::string& why);
+    bool segments_from_image(unsigned int camID, const Image8u& image, const LensDistortion* lens, const Matrix3d& K, Line3D::SegmentDetectorFn fn,
+                             void* user, std::vector<Vec4f>& segs, std::string& why);
+    bool prepare_undistorted(const Image8u& image, const LensDistortion& lens, const Matrix3d& K, Image8u& gray, std::string& why);
+    bool check_lens(unsigned int camID, const LensDistortion& lens, const Matrix3d& K);
     bool line_from_cluster(const std::list<Segment2D>& cluster, LineCluster3D& out) const;
     Segment3D project_onto_line(const Segment2D& s2, const Segment3D& s3, bool& ok) const;
     std::list<Segment3D> collinear_segments(const LineCluster3D& cl) const;
@@ -757,8 +764,8 @@ static std::vector<Vec4f> filter_detections(const std::vector<Vec4f>& detections
 
 // the segments of an image without given segments (detectLineSegments line3D.cc:249-372): the segment cache, or the prepared image
 // through the detector and the post-processing, then the cache is written.  false with `why` set if the view has to be rejected.
-bool Line3D::Impl::segments_from_image(unsigned int camID, const Image8u& image, Line3D::SegmentDetectorFn fn, void* user, std::vector<Vec4f>& segs,
-                                       std::string& why)
+bool Line3D::Impl::segments_from_image(unsigned int camID, const Image8u& image, const LensDistortion* lens, const Matrix3d& K,
+                                       Line3D::SegmentDetectorFn fn, void* user, std::vector<Vec4f>& segs, std::string& why)
 {
     const int w = image.cols, h = image.rows;
     if (image.channels != 1 && image.channels != 3) {                                                     // line3D.cc:251-266
@@ -771,7 +778,9 @@ bool Line3D::Impl::segments_from_image(unsigned int camID, const Image8u& image,
     int w_p, h_p;
     preparedImageSize(w, h, max_img_width, w_p, h_p);
     Image8u gray(h_p, w_p, 1);
-    {
+    if (lens) {
+        if (!prepare_undistorted(image, *lens, K, gray, why)) return false;
+    } else {
         // the primary context is single-owner: one preparation at a time
         std::lock_guard<std::mutex> g(prep_mtx);
         l3d_image_prep_desc d;
@@ -797,12 +806,137 @@ bool Line3D::Impl::segments_from_image(unsigned int camID, const Image8u& image,
     return true;
 }
 
+// the camera, lens and new-K fields of an l3d_undistort_desc (include/l3d_capi.h); the image fields are zero
+static l3d_undistort_desc lens_desc(const LensDistortion& lens, const Matrix3d& K, const Matrix3d& newK)
+{
+    l3d_undistort_desc d;
+    std::memset(&d, 0, sizeof(d));
+    d.fx = K(0, 0); d.fy = K(1, 1); d.cx = K(0, 2); d.cy = K(1, 2);
+    d.new_fx = newK(0, 0); d.new_fy = newK(1, 1); d.new_cx = newK(0, 2); d.new_cy = newK(1, 2);
+    d.model = lens.model;
+    d.tangential[0] = lens.p[0]; d.tangential[1] = lens.p[1];
+    if (lens.model == LensDistortion::FISHEYE) {   // k[4], k[5] go where l3d_undistort_u8 rejects them if nonzero
+        for (int k = 0; k < 4; ++k) d.fisheye[k] = lens.k[k];
+        d.radial[0] = lens.k[4]; d.radial[1] = lens.k[5];
+    } else {
+        for (int k = 0; k < 3; ++k) { d.radial[k] = lens.k[k]; d.rational[k] = lens.k[3 + k]; }
+    }
+    return d;
+}
+
+// a zero-initialised LensDistortion: no distortion at all (a fisheye lens with k = 0 still is one)
+static bool lens_is_zero(const LensDistortion& lens)
+{
+    bool zero = lens.model == LensDistortion::RADTAN && lens.p[0] == 0.0 && lens.p[1] == 0.0;
+    for (int k = 0; k < 6; ++k) zero = zero && lens.k[k] == 0.0;
+    return zero;
+}
+
+// the lens of an addImage call, checked as l3d_undistort_u8 checks it (an empty point set: no GPU work); false: the view is rejected
+bool Line3D::Impl::check_lens(unsigned int camID, const LensDistortion& lens, const Matrix3d& K)
+{
+    l3d_points_desc d;
+    std::memset(&d, 0, sizeof(d));
+    d.cam = lens_desc(lens, K, Matrix3d());
+    std::string why;
+    {
+        std::lock_guard<std::mutex> g(prep_mtx);
+        if (l3d_undistort_points(ctx, 1, &d, 0) == L3D_OK) return true;
+        why = std::string("lens: ") + l3d_last_error(ctx);
+    }
+    std::lock_guard<std::mutex> g(mtx);
+    return reject(camID, why);
+}
+
+// The image undistorted into K and prepared for the detector on the primary device, the undistorted image never leaving it: one upload,
+// l3d_undistort_u8 and l3d_prepare_gray_u8 on device buffers, one download of the prepared image into gray (sized by the caller).
+bool Line3D::Impl::prepare_undistorted(const Image8u& image, const LensDistortion& lens, const Matrix3d& K, Image8u& gray, std::string& why)
+{
+    const int w = image.cols, h = image.rows, ch = image.channels;
+    const size_t in_bytes = (size_t)w * h * ch, gray_bytes = gray.data.size();
+    std::lock_guard<std::mutex> g(prep_mtx);                  // the primary context is single-owner: one preparation at a time
+    int prev = 0;
+    cudaGetDevice(&prev);
+    struct Restore { int d; ~Restore() { cudaSetDevice(d); } } restore{prev};
+    cudaSetDevice(devices[0]);
+    DeviceScratch& s = prep_scratch;
+    if (s.cap < 2 * in_bytes + gray_bytes) {
+        if (s.p) cudaFree(s.p);
+        s.p = nullptr; s.cap = 0; s.device = devices[0];
+        if (cudaMalloc(&s.p, 2 * in_bytes + gray_bytes) != cudaSuccess) { s.p = nullptr; why = "lens undistortion: out of device memory"; return false; }
+        s.cap = 2 * in_bytes + gray_bytes;
+    }
+    unsigned char* src = (unsigned char*)s.p;
+    unsigned char* und = src + in_bytes;
+    unsigned char* dst = und + in_bytes;
+    cudaStream_t st = (cudaStream_t)l3d_stream(ctx);
+    if (cudaMemcpyAsync(src, image.data.data(), in_bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) { why = "lens undistortion: upload failed"; return false; }
+    l3d_undistort_desc u = lens_desc(lens, K, Matrix3d());
+    u.width = w; u.height = h; u.channels = ch;
+    u.src_pitch = u.dst_pitch = (int64_t)w * ch;
+    u.src = src; u.dst = und;
+    if (l3d_undistort_u8(ctx, 1, &u, 1) != L3D_OK) { why = std::string("lens undistortion: ") + l3d_last_error(ctx); return false; }
+    l3d_image_prep_desc d;
+    std::memset(&d, 0, sizeof(d));
+    d.width = w; d.height = h; d.channels = ch; d.max_img_width = max_img_width;
+    d.src_pitch = (int64_t)w * ch; d.dst_pitch = gray.cols;
+    d.src = und; d.dst = dst;
+    d.out_width = gray.cols; d.out_height = gray.rows;
+    if (l3d_prepare_gray_u8(ctx, 1, &d, 1) != L3D_OK) { why = std::string("image preparation: ") + l3d_last_error(ctx); return false; }
+    if (cudaMemcpyAsync(gray.data.data(), dst, gray_bytes, cudaMemcpyDeviceToHost, st) != cudaSuccess || l3d_sync(ctx) != L3D_OK) {
+        why = "lens undistortion: download failed";
+        return false;
+    }
+    return true;
+}
+
 bool Line3D::addImage(const unsigned int camID, const Image8u& image, const Matrix3d& K, const Matrix3d& R, const Vector3d& t,
                       const float median_depth, const std::list<unsigned int>& wps_or_neighbors, const std::vector<Vec4f>& line_segments)
 {
+    LensDistortion none;
+    std::memset(&none, 0, sizeof(none));
+    return addImage(camID, image, K, R, t, median_depth, wps_or_neighbors, none, line_segments);
+}
+
+bool Line3D::addImage(const unsigned int camID, const int w, const int h, const Matrix3d& K, const Matrix3d& R, const Vector3d& t,
+                      const float median_depth, const std::list<unsigned int>& wps_or_neighbors, const LensDistortion& lens,
+                      const std::vector<Vec4f>& line_segments)
+{
+    if (lens_is_zero(lens) || line_segments.empty()) {
+        if (!lens_is_zero(lens) && !p_->check_lens(camID, lens, K)) return false;
+        return addImage(camID, w, h, K, R, t, median_depth, wps_or_neighbors, line_segments);
+    }
+    Impl& P = *p_;
+    std::vector<Vec4f> segs(line_segments);
+    l3d_points_desc d;
+    std::memset(&d, 0, sizeof(d));
+    d.cam = lens_desc(lens, K, Matrix3d());
+    d.count = 2 * (int64_t)segs.size();
+    d.src = d.dst = &segs[0].v[0];
+    std::string why;
+    {
+        std::lock_guard<std::mutex> g(P.prep_mtx);
+        if (l3d_undistort_points(P.ctx, 1, &d, 0) != L3D_OK) why = std::string("lens: ") + l3d_last_error(P.ctx);
+    }
+    if (!why.empty()) {
+        std::lock_guard<std::mutex> g(P.mtx);
+        return P.reject(camID, why);
+    }
+    return addImage(camID, w, h, K, R, t, median_depth, wps_or_neighbors, segs);
+}
+
+bool Line3D::addImage(const unsigned int camID, const Image8u& image, const Matrix3d& K, const Matrix3d& R, const Vector3d& t,
+                      const float median_depth, const std::list<unsigned int>& wps_or_neighbors, const LensDistortion& lens,
+                      const std::vector<Vec4f>& line_segments)
+{
     Impl& P = *p_;
     const int w = image.cols, h = image.rows;
-    if (!line_segments.empty()) return addImage(camID, w, h, K, R, t, median_depth, wps_or_neighbors, line_segments);
+    const bool undistort = !lens_is_zero(lens);
+    if (!line_segments.empty()) {
+        if (undistort) return addImage(camID, w, h, K, R, t, median_depth, wps_or_neighbors, lens, line_segments);
+        return addImage(camID, w, h, K, R, t, median_depth, wps_or_neighbors, line_segments);
+    }
+    if (undistort && !P.check_lens(camID, lens, K)) return false;
     // the checks before any image work; the camera ID stays reserved until the view is added or rejected
     Line3D::SegmentDetectorFn fn;
     void* user;
@@ -818,7 +952,7 @@ bool Line3D::addImage(const unsigned int camID, const Image8u& image, const Matr
     } release{P, camID};
     std::vector<Vec4f> segs;
     std::string why;
-    if (!P.segments_from_image(camID, image, fn, user, segs, why)) {
+    if (!P.segments_from_image(camID, image, undistort ? &lens : nullptr, K, fn, user, segs, why)) {
         std::lock_guard<std::mutex> g(P.mtx);
         return P.reject(camID, why);
     }
@@ -1130,29 +1264,66 @@ void Line3D::undistortImage(const Image8u& in, Image8u& out, const LensDistortio
     const bool size_ok = (out_width == 0 && out_height == 0) || (out_width >= 1 && out_width <= 32767 && out_height >= 1 && out_height <= 32767);
     const int ow = out_width == 0 && out_height == 0 ? in.cols : out_width, oh = out_width == 0 && out_height == 0 ? in.rows : out_height;
     Image8u res(size_ok ? oh : 0, size_ok ? ow : 0, in.channels);
-    l3d_undistort_desc d;
-    std::memset(&d, 0, sizeof(d));
+    l3d_undistort_desc d = lens_desc(lens, K, newK);
     d.width = in.cols; d.height = in.rows; d.channels = in.channels;
     d.src_pitch = (int64_t)in.cols * in.channels;
     d.dst_pitch = (int64_t)(size_ok ? ow : in.cols) * in.channels;
     d.src = in.data.data(); d.dst = res.data.data();
-    d.fx = K(0, 0); d.fy = K(1, 1); d.cx = K(0, 2); d.cy = K(1, 2);
-    d.new_fx = newK(0, 0); d.new_fy = newK(1, 1); d.new_cx = newK(0, 2); d.new_cy = newK(1, 2);
     d.out_width = out_width; d.out_height = out_height;
-    d.model = lens.model;
-    d.tangential[0] = lens.p[0]; d.tangential[1] = lens.p[1];
-    if (lens.model == LensDistortion::FISHEYE) {   // k[4], k[5] go where l3d_undistort_u8 rejects them if nonzero
-        for (int k = 0; k < 4; ++k) d.fisheye[k] = lens.k[k];
-        d.radial[0] = lens.k[4]; d.radial[1] = lens.k[5];
-    } else {
-        for (int k = 0; k < 3; ++k) { d.radial[k] = lens.k[k]; d.rational[k] = lens.k[3 + k]; }
-    }
     const int rc = l3d_undistort_u8(ctx, 1, &d, 0);
     const std::string msg = std::string("undistortImage: ") + l3d_last_error(ctx);
     l3d_ctx_destroy(ctx);
     if (rc == L3D_ERR_INVALID) throw std::invalid_argument(msg);
     if (rc != L3D_OK) throw std::runtime_error(msg);
     out = std::move(res);
+}
+
+// l3d_undistort_points of host point sets on the calling thread's device, through a context that lives for the call
+static void undistort_point_sets(std::vector<l3d_points_desc>& sets)
+{
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) throw std::runtime_error("undistortPoints: no usable CUDA device");
+    l3d_ctx* ctx = nullptr;
+    if (l3d_ctx_create(dev, &ctx) != L3D_OK) throw std::runtime_error("undistortPoints: no usable CUDA device");
+    const int rc = l3d_undistort_points(ctx, (int)sets.size(), sets.data(), 0);
+    const std::string msg = std::string("undistortPoints: ") + l3d_last_error(ctx);
+    l3d_ctx_destroy(ctx);
+    if (rc == L3D_ERR_INVALID) throw std::invalid_argument(msg);
+    if (rc != L3D_OK) throw std::runtime_error(msg);
+}
+
+void Line3D::undistortPoints(std::vector<float>& xy, const LensDistortion& lens, const Matrix3d& K, const Matrix3d& newK)
+{
+    if (xy.size() % 2) throw std::invalid_argument("undistortPoints: an odd number of coordinates");
+    std::vector<l3d_points_desc> d(1);
+    d[0].cam = lens_desc(lens, K, newK);
+    d[0].count = (int64_t)(xy.size() / 2);
+    d[0].src = d[0].dst = xy.data();
+    undistort_point_sets(d);
+}
+
+void Line3D::undistortSegments(std::vector<Vec4f>& segs, const LensDistortion& lens, const Matrix3d& K, const Matrix3d& newK)
+{
+    std::vector<l3d_points_desc> d(1);
+    d[0].cam = lens_desc(lens, K, newK);
+    d[0].count = 2 * (int64_t)segs.size();
+    d[0].src = d[0].dst = segs.empty() ? nullptr : &segs[0].v[0];
+    undistort_point_sets(d);
+}
+
+void Line3D::undistortPoints(std::vector<std::vector<float> >& xy, const std::vector<LensDistortion>& lenses, const std::vector<Matrix3d>& K,
+                             const std::vector<Matrix3d>& newK)
+{
+    if (lenses.size() != xy.size() || K.size() != xy.size() || (!newK.empty() && newK.size() != xy.size()))
+        throw std::invalid_argument("undistortPoints: one lens and one K (and one new K, if any) per point set");
+    std::vector<l3d_points_desc> d(xy.size());
+    for (size_t i = 0; i < xy.size(); ++i) {
+        if (xy[i].size() % 2) throw std::invalid_argument("undistortPoints: an odd number of coordinates in set " + std::to_string(i));
+        d[i].cam = lens_desc(lenses[i], K[i], newK.empty() ? Matrix3d() : newK[i]);
+        d[i].count = (int64_t)(xy[i].size() / 2);
+        d[i].src = d[i].dst = xy[i].data();
+    }
+    undistort_point_sets(d);
 }
 
 }  // namespace L3DPP
@@ -1300,6 +1471,62 @@ int l3dpp_add_image_pixels(void* h, unsigned int cam, const unsigned char* pixel
     std::vector<Vec4f> s(nseg); if (nseg) memcpy(s.data(), segs, 16 * (size_t)nseg);
     Line3D* L = (Line3D*)h;
     return L->addImage(cam, img, Km, Rm, Vector3d(t[0], t[1], t[2]), median_depth, std::list<unsigned int>(list, list + nlist), s) ? 0 : -1;
+}
+// L3DPP::LensDistortion from its 9 doubles: model, k[6], p[2]
+static LensDistortion lens_of(const double* lens9)
+{
+    LensDistortion lens;
+    lens.model = (int)lens9[0];
+    for (int k = 0; k < 6; ++k) lens.k[k] = lens9[1 + k];
+    lens.p[0] = lens9[7]; lens.p[1] = lens9[8];
+    return lens;
+}
+int l3dpp_add_image_lens(void* h, unsigned int cam, int w, int hgt, const double* K, const double* R, const double* t, float median_depth,
+                         const unsigned int* list, int nlist, const double* lens9, const float* segs, int nseg)
+{
+    Matrix3d Km, Rm; memcpy(Km.m, K, 72); memcpy(Rm.m, R, 72);
+    std::vector<Vec4f> s(nseg); if (nseg) memcpy(s.data(), segs, 16 * (size_t)nseg);
+    Line3D* L = (Line3D*)h;
+    return L->addImage(cam, w, hgt, Km, Rm, Vector3d(t[0], t[1], t[2]), median_depth, std::list<unsigned int>(list, list + nlist), lens_of(lens9), s) ? 0 : -1;
+}
+int l3dpp_add_image_pixels_lens(void* h, unsigned int cam, const unsigned char* pixels, int rows, int cols, int channels, long long step,
+                                const double* K, const double* R, const double* t, float median_depth, const unsigned int* list, int nlist,
+                                const double* lens9, const float* segs, int nseg)
+{
+    Image8u img(rows, cols, channels);
+    const size_t row = (size_t)std::max(cols, 0) * std::max(channels, 0);
+    for (int r = 0; r < rows && row; ++r) memcpy(img.data.data() + r * row, pixels + r * step, row);
+    Matrix3d Km, Rm; memcpy(Km.m, K, 72); memcpy(Rm.m, R, 72);
+    std::vector<Vec4f> s(nseg); if (nseg) memcpy(s.data(), segs, 16 * (size_t)nseg);
+    Line3D* L = (Line3D*)h;
+    return L->addImage(cam, img, Km, Rm, Vector3d(t[0], t[1], t[2]), median_depth, std::list<unsigned int>(list, list + nlist), lens_of(lens9), s) ? 0 : -1;
+}
+int l3dpp_undistort_points(float* xy, const long long* counts, int n, const double* lens9, const double* K, const double* newK, int device, char* err,
+                           int errcap)
+{
+    auto fail = [&](int rc, const char* what) { if (err && errcap > 0) snprintf(err, (size_t)errcap, "%s", what); return rc; };
+    if (n < 0) return fail(-1, "undistortPoints: n < 0");
+    int prev = 0;
+    if (cudaGetDevice(&prev) != cudaSuccess || cudaSetDevice(device) != cudaSuccess) return fail(-2, "undistortPoints: no usable CUDA device");
+    struct Restore { int d; ~Restore() { cudaSetDevice(d); } } restore{prev};
+    std::vector<std::vector<float> > sets((size_t)n);
+    std::vector<LensDistortion> lenses((size_t)n);
+    std::vector<Matrix3d> Ks((size_t)n), newKs(newK ? (size_t)n : 0);
+    size_t off = 0;
+    for (int i = 0; i < n; ++i) {
+        if (counts[i] < 0) return fail(-1, "undistortPoints: a negative count");
+        sets[i].assign(xy + off, xy + off + 2 * (size_t)counts[i]);
+        off += 2 * (size_t)counts[i];
+        lenses[i] = lens_of(lens9 + 9 * i);
+        memcpy(Ks[i].m, K + 9 * i, 72);
+        if (newK) memcpy(newKs[i].m, newK + 9 * i, 72);
+    }
+    try {
+        Line3D::undistortPoints(sets, lenses, Ks, newKs);
+    } catch (const std::invalid_argument& e) { return fail(-1, e.what()); } catch (const std::exception& e) { return fail(-2, e.what()); }
+    off = 0;
+    for (int i = 0; i < n; ++i) { if (!sets[i].empty()) memcpy(xy + off, sets[i].data(), 4 * sets[i].size()); off += sets[i].size(); }
+    return fail(0, "");
 }
 void l3dpp_push_detections(void* out, const float* xy4, long long n)
 {

@@ -65,26 +65,38 @@ class Line3D:
             raise capi.L3DError(f"{what}: {self.L.l3dpp_last_error(self.h).decode()}")
         return rc
 
-    def add_image(self, cam, width, height, K, R, t, median_depth, wps_or_neighbors, segs=()):
-        """segs: float32 [n, 4]; empty: read the view's segment cache (see __init__)"""
+    def add_image(self, cam, width, height, K, R, t, median_depth, wps_or_neighbors, segs=(), lens=None):
+        """segs: float32 [n, 4]; empty: read the view's segment cache (see __init__).  lens: the camera's lens dict (as read_colmap
+        gives it): segs are then in the distorted image and their endpoints are undistorted into K (a cached list is used as stored)"""
         lst = np.ascontiguousarray(wps_or_neighbors, np.uint32)
         segs = np.ascontiguousarray(segs, np.float32).reshape(-1, 4)
         f64 = lambda a: np.ascontiguousarray(a, np.float64)
-        self._chk(self.L.l3dpp_add_image(self.h, int(cam), int(width), int(height), _p(f64(K)), _p(f64(R)), _p(f64(t)), float(median_depth),
-                                         _p(lst), len(lst), _p(segs), len(segs)), "addImage")
+        if lens is None:
+            rc = self.L.l3dpp_add_image(self.h, int(cam), int(width), int(height), _p(f64(K)), _p(f64(R)), _p(f64(t)), float(median_depth),
+                                        _p(lst), len(lst), _p(segs), len(segs))
+        else:
+            rc = self.L.l3dpp_add_image_lens(self.h, int(cam), int(width), int(height), _p(f64(K)), _p(f64(R)), _p(f64(t)), float(median_depth),
+                                             _p(lst), len(lst), _p(_lens9(lens)), _p(segs), len(segs))
+        self._chk(rc, "addImage")
 
-    def add_image_pixels(self, cam, img, K, R, t, median_depth, wps_or_neighbors, segs=()):
+    def add_image_pixels(self, cam, img, K, R, t, median_depth, wps_or_neighbors, segs=(), lens=None):
         """addImage with the image itself: img uint8 HxW (grey) or HxWx3 (channel 0 is R), any row stride.  Without segs the segment
         cache is read, or the image is prepared on the GPU and handed to the set_segment_detector function.  An exception raised by
-        the detector is raised here again."""
+        the detector is raised here again.  lens: the camera's lens dict; img and segs are then the distorted image and segments in
+        it: the image is undistorted into K on the GPU before it is prepared, the segments' endpoints are undistorted into K."""
         a, sp = capi._image_rows(img)
         lst = np.ascontiguousarray(wps_or_neighbors, np.uint32)
         segs = np.ascontiguousarray(segs, np.float32).reshape(-1, 4)
         f64 = lambda v: np.ascontiguousarray(v, np.float64)
         errors = self.__dict__.setdefault("_detector_errors", {})      # per calling thread: the detector runs on it
         errors.pop(threading.get_ident(), None)
-        rc = self.L.l3dpp_add_image_pixels(self.h, int(cam), a.ctypes.data, a.shape[0], a.shape[1], 1 if a.ndim == 2 else 3, sp, _p(f64(K)),
-                                           _p(f64(R)), _p(f64(t)), float(median_depth), _p(lst), len(lst), _p(segs), len(segs))
+        if lens is None:
+            rc = self.L.l3dpp_add_image_pixels(self.h, int(cam), a.ctypes.data, a.shape[0], a.shape[1], 1 if a.ndim == 2 else 3, sp, _p(f64(K)),
+                                               _p(f64(R)), _p(f64(t)), float(median_depth), _p(lst), len(lst), _p(segs), len(segs))
+        else:
+            rc = self.L.l3dpp_add_image_pixels_lens(self.h, int(cam), a.ctypes.data, a.shape[0], a.shape[1], 1 if a.ndim == 2 else 3, sp,
+                                                    _p(f64(K)), _p(f64(R)), _p(f64(t)), float(median_depth), _p(lst), len(lst),
+                                                    _p(_lens9(lens)), _p(segs), len(segs))
         err = errors.pop(threading.get_ident(), None)
         if err is not None:
             raise err
@@ -418,6 +430,34 @@ def undistort_image(img, K, lens, new_K=None, out_size=None, device=0):
     if rc != 0:
         raise capi.L3DError("undistort_image: no usable CUDA device or a CUDA failure")
     return out
+
+
+def undistort_points(pts, K, lens, new_K=None, device=0):
+    """Line3D::undistortPoints on GPU `device`: cv2.undistortPoints(pts, K, D, None, new_K) for a radtan lens dict and
+    cv2.fisheye.undistortPoints(pts, K, D, R=I, P=new_K) for a fisheye one (DESIGN.md §4a).  pts: float32 (x, y) pairs of any shape
+    [..., 2] (segments [n, 4] are two points each); new_K None: K.  Returns float32 points of pts' shape, in pixels of new_K."""
+    return undistort_points_batch([(pts, K, lens, new_K)], device)[0]
+
+
+def undistort_points_batch(sets, device=0):
+    """the batched Line3D::undistortPoints: a list of (pts, K, lens, new_K) sets undistorted in one launch; returns one array per set"""
+    arrs = [np.asarray(s[0], np.float32) for s in sets]
+    if any(a.size % 2 for a in arrs):
+        raise ValueError("undistort_points: points are (x, y) pairs")
+    cat = lambda parts, dt: np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros(0, dt), dt)
+    xy = cat([a.reshape(-1) for a in arrs], np.float32)
+    counts = np.array([a.size // 2 for a in arrs], np.int64)
+    lens9 = cat([_lens9(s[2]) for s in sets], np.float64)
+    Ks = cat([np.asarray(s[1], np.float64).reshape(9) for s in sets], np.float64)
+    nKs = cat([np.zeros(9) if s[3] is None else np.asarray(s[3], np.float64).reshape(9) for s in sets], np.float64)
+    err = C.create_string_buffer(512)
+    rc = capi.lib().l3dpp_undistort_points(_p(xy), _p(counts), len(sets), _p(lens9), _p(Ks), _p(nKs), int(device), err, 512)
+    if rc == -1:
+        raise ValueError(err.value.decode())
+    if rc != 0:
+        raise capi.L3DError(err.value.decode())
+    offs = np.concatenate([[0], np.cumsum([a.size for a in arrs])]).astype(np.int64)
+    return [xy[offs[i]:offs[i + 1]].reshape(a.shape).copy() for i, a in enumerate(arrs)]
 
 
 def optimal_new_camera_matrix(K, lens, image_size, alpha, new_size=None, center_principal_point=False):
