@@ -465,13 +465,48 @@ def _filter_cases(L):
         L.cases.append(Case("filter", band, 0, s, 3, t[2], band == "perc_above", info=dict(score=s31)))
 
 
-def build(sc, params):
-    """the lists of scene sc under parameter set params (a dict of match_images arguments) and their cases"""
+def _in_band_case(L, u=0):
+    """segment s of view u with X -> u+1 at (a, a) and Y -> u+2 at (c, c), float depths picked so that the similarity of X with Y
+    lies inside the REF_CPU band around sim_t (tests/refcpu_model.py: within the libm error bound of 0.5).  It is X's only
+    partner, so X's score is 0 or ~0.5 depending on the build, and a positive score announces X's inverse entry to view u+1,
+    processed later: the closure U has to follow it there."""
+    from tests import refcpu_model as rm
+    g = L.geo
+    sc = L.sc
+    cams = rm.Cameras.of_scene(sc, g.k)
+    s = L.take(u)
+    v1, v2 = u + 1, u + 2
+    pr = min(g.pos_reg(u, s, D0, D0, v1))
+    c0 = D0 + math.sqrt(-math.log(SIM_T) * pr)
+    A, B = np.meshgrid(ulps(D0, 160), ulps(c0, 160), indexing="ij")
+    A, B = A.ravel(), B.ravel()
+    m = np.zeros(2 * len(A), np.dtype([("src_seg", "<u4"), ("tgt_cam", "<u4"), ("d_p1", "<f4"), ("d_p2", "<f4")]))
+    m["src_seg"] = s
+    m["tgt_cam"][0::2], m["tgt_cam"][1::2] = v1, v2
+    m["d_p1"][0::2] = m["d_p2"][0::2] = A
+    m["d_p1"][1::2] = m["d_p2"][1::2] = B
+    x = rm._Entries(cams, u, m)
+    i, j = np.arange(0, len(m), 2), np.arange(1, len(m), 2)
+    dot = (x.dr[i] * x.dr[j]).sum(1).astype(np.float32)
+    sim, W = rm.sims(dot, x.d1[i] - x.d1[j], x.d2[i] - x.d2[j], x.reg1[i], x.reg2[i], L.geo.angle_reg, np.zeros(len(i), bool))
+    gap = np.abs(sim.astype(np.float64) - 0.5) / W["gpu"]
+    q = int(np.argmin(gap))
+    assert gap[q] < 0.5, float(gap[q])
+    t1, t2 = L.take(v1), L.take(v2)
+    L.add(u, s, v1, t1, (float(A[q]),) * 2, (D0, D0)); L.add(u, s, v2, t2, (float(B[q]),) * 2, (D0, D0))
+    L.cases.append(Case("in_band", "in_band", u, s, v1, t1, None, info=dict(sim=float(sim[q]), W=float(W["gpu"][q]))))
+
+
+def build(sc, params, in_band=False):
+    """the lists of scene sc under parameter set params (a dict of match_images arguments) and their cases; in_band: add the
+    case of _in_band_case"""
     L = Lists(sc, Geometry(sc, params))
     _background(L)
     _orientation_cases(L)
     _similarity_cases(L)
     _filter_cases(L)
+    if in_band:
+        _in_band_case(L)
     return L
 
 
