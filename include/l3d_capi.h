@@ -92,6 +92,8 @@ int l3d_update_view_params(l3d_ctx* ctx, int num_views, const l3d_view_desc* vie
  * 1 <= knn <= 32: the kNN best per src segment.  knn <= 0: keep ALL matches like the reference does (cudawrapper.cu:628-636),
  * in ascending tgt_seg order; the record array then uses the row stride l3d_match_stride() = the largest row of the job
  * (memory: total_rows * stride * 24 B).  knn > 32: the keep-all passes, then every row is cut to its knn best.
+ * knn <= 0 and knn > 32: a row may hold at most 8533 matches before the cut (k_sort_rows sorts one row per warp in at most 200 KiB
+ * of shared memory, 24 B per record); a longer row fails the call with L3D_ERR_UNSUPPORTED and leaves no match result.
  * Every call first builds the level-1 tables of its pairs (DESIGN.md section 2: the target segments of a pair as arcs of the
  * epipolar pencil, sorted): 16 B per (pair, target segment) kept until the next call + 28 B while they are built.
  * Results stay on the device; fetch with the l3d_get_* calls. */

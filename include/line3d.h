@@ -276,7 +276,9 @@ public:
     void setLineCandidates(const unsigned int camA, const unsigned int camB, const std::vector<std::pair<unsigned int, unsigned int> >& seg_pairs);
     void clearLineCandidates();
 
-    /* line3D.h:140-145 */
+    /* line3D.h:140-145.  kNN in 1..32: the kNN best matches of every segment.  kNN <= 0 (keep all) or kNN > 32 (keep all, then cut
+     * every segment to its kNN best): a segment may have at most 8533 matches in one view pair before the cut (the rows are sorted in
+     * 200 KiB of shared memory, 24 B per match); more makes matchImages fail with lastError() naming the limit, where the reference has none. */
     void matchImages(const float sigma_position = L3D_DEF_SCORING_POS_REGULARIZER, const float sigma_angle = L3D_DEF_SCORING_ANG_REGULARIZER,
                      const unsigned int num_neighbors = L3D_DEF_MATCHING_NEIGHBORS, const float epipolar_overlap = L3D_DEF_EPIPOLAR_OVERLAP,
                      const int kNN = L3D_DEF_KNN, const float const_regularization_depth = -1.0f);

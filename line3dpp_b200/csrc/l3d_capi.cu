@@ -86,6 +86,8 @@ struct CastI64 { __host__ __device__ long long operator()(int v) const { return 
 
 // the most dynamic shared memory k_sort_rows gets (run_keep_all: the rows of the CTA's warps at the keep-all stride)
 static const size_t SORT_SMEM_MAX = 200 * 1024;
+// the longest row a keep-all or kNN > 32 call can sort: one warp's row fills the block's shared memory (8533 matches)
+static const int SORT_ROW_MAX = (int)(SORT_SMEM_MAX / sizeof(l3d_match_rec));
 
 extern "C" {
 
@@ -480,7 +482,11 @@ static int run_keep_all(l3d_ctx* c, MatchArgs a, int big_k, CandArgs ca)
         const size_t per_warp = sizeof(l3d_match_rec) * (size_t)stride;
         int wpb = 4;
         while (wpb > 1 && per_warp * wpb > SORT_SMEM_MAX) wpb >>= 1;
-        if (per_warp * wpb > SORT_SMEM_MAX) return l3d_fail(c, L3D_ERR_UNSUPPORTED, "l3d_match_pairs: a row with more than 8500 matches (kNN <= 0)");
+        if (stride > SORT_ROW_MAX) {
+            char msg[120];
+            snprintf(msg, sizeof(msg), "l3d_match_pairs: a row with more than %d matches (kNN <= 0 or kNN > 32)", SORT_ROW_MAX);
+            return l3d_fail(c, L3D_ERR_UNSUPPORTED, msg);
+        }
         a.knn = stride; a.recs = (l3d_match_rec*)c->d_recs.p; ca.knn = stride; ca.recs = a.recs;
         if (nunits && (rc = launch_match(c, Keep::Store, a, 0, nunits, "k_match_topk (store)"))) return rc;
         if ((rc = launch_cand(c, Keep::Store, ca, "k_match_cand (store)"))) return rc;
