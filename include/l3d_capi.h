@@ -471,6 +471,42 @@ int l3d_triangulate_points(l3d_ctx* ctx, long long n_points, const int64_t* obs_
 int l3d_median_depths(l3d_ctx* ctx, int n_cams, const int64_t* list_ptr, const int32_t* list_pts, long long n_points, const double* X,
                       const int32_t* valid, const double* C, int32_t* count_out, float* median_out, int on_device);
 
+/* ---- visual neighbours from camera poses (DESIGN.md §6d): for models without world points (mavmap, SLAM or VIO keyframes, RTK-posed
+ * surveys, SfM exports without structure).  Every view i gets gx * gy virtual world points, the pixel centres ((c + 0.5) width / gx,
+ * (r + 0.5) height / gy) back-projected to camera depth median_depth (sample s = r * gx + c is point i * gx * gy + s).  A point is
+ * observed by its own view and by every other view j that sees it in front (depth > 0) and inside [0, width) x [0, height), without
+ * occlusion or depth-range tests; all of that in IEEE double in the operation order of DESIGN.md §6d.  n_i is the number of points
+ * view i observes (its own included), common(i, j) the number both observe.  The neighbours are then find_visual_neighbors' (i.e.
+ * findVisualNeighborsFromWPs', line3D.cc:578-699) for those points: score 2 common / (n_i + n_j) in float, optical axes under 1.571
+ * rad, common > 4, the 0.8 cut, the distance resort and the greedy baseline > 0.1 loop, with camera centres, axes and distances
+ * computed from K, R, t as addImage computes them (no translation is applied).  Not part of the pipeline chain: every stage and its
+ * result stay as they were. */
+typedef struct {
+    uint32_t cam_id;                /* the camID the lists name; unique */
+    int32_t width, height;          /* image size, at least 1 */
+    int32_t pad;                    /* 0 */
+    double fx, fy, cx, cy, skew;    /* K = [[fx, skew, cx], [0, fy, cy], [0, 0, 1]]; fx, fy nonzero */
+    double R[9];                    /* row-major, x_cam = R X + t */
+    double t[3];
+    double median_depth;            /* depth of the virtual points in front of this view; finite, > 0 */
+} l3d_pose_view;
+#define L3D_POSE_MAX_VIEWS 50000             /* the co-visibility histogram of a view: 4 bytes per view in shared memory */
+#define L3D_POSE_MAX_POINTS (1ll << 26)      /* the largest n * gx * gy (24 bytes of virtual point per sample on the device) */
+/* The neighbours of n views as CSR: view i's are nb_cam[nb_ptr[i] .. nb_ptr[i+1]), camIDs in ascending order (the lists for addImage
+ * with neighbors_by_worldpoints = false).  nb_ptr[n+1] is always written; nb_cam only when the total fits cap (n * min(num_neighbors,
+ * n - 1) always does).  n_obs_out (n entries, or NULL): n_i.  timing_out (2 doubles, or NULL): the device time of the kernels in ms
+ * (CUDA events) and the host time of the selection in ms.  Returns the total number of neighbour entries or a negative status.
+ * Rejected with L3D_ERR_INVALID, l3d_last_error naming the view (index and camID): median_depth <= 0 or not finite, width or height
+ * below 1, fx or fy zero or not finite, cx, cy or skew not finite, R or t not finite, a camID that repeats an earlier view's; and
+ * gx or gy below 1, n < 0, a null views or nb_ptr array.  L3D_ERR_UNSUPPORTED: n above L3D_POSE_MAX_VIEWS, n * gx * gy above
+ * L3D_POSE_MAX_POINTS, more than 2^31 - 1 observations (the sum over points of their observers) or co-visibility slots. */
+long long l3d_pose_neighbors(l3d_ctx* ctx, int n, const l3d_pose_view* views, int gx, int gy, unsigned int num_neighbors, int64_t* nb_ptr,
+                             uint32_t* nb_cam, long long cap, int32_t* n_obs_out, double* timing_out);
+/* test export of the same device pass: n_obs_out (n entries, or NULL) and every nonzero (i, j, common(i, j)), i != j, as view
+ * indices, ascending in (i, j), 3 int32 each in ijc_out when they fit cap triples.  Returns the number of triples or a negative
+ * status; rejections as l3d_pose_neighbors'. */
+long long l3d_pose_covisibility(l3d_ctx* ctx, int n, const l3d_pose_view* views, int gx, int gy, int32_t* n_obs_out, int32_t* ijc_out, long long cap);
+
 /* stable ascending argsort of float keys on the device: the weight sort of performClustering (clustering.cc:13-14) for
  * large edge lists.  perm_out[i] = index of the i-th smallest key, ties in input order. */
 int l3d_argsort_f32(l3d_ctx* ctx, long long n, const float* keys, unsigned int* perm_out);

@@ -70,6 +70,25 @@ bool readMavmap(const std::string& path, std::vector<SfMCamera>& cameras, std::s
 /* up to num_neighbors / 2 earlier cameras, nearest first, then later cameras until num_neighbors (main_mavmap.cpp:312-321) */
 std::list<unsigned int> sequentialNeighbors(unsigned int i, unsigned int n_cams, unsigned int num_neighbors);
 
+/* one posed view for poseNeighbors: what addImage takes of it (K, R, t with x_cam = R X + t, the image size) and the depth at which
+ * its virtual world points are placed; K's upper triangle (fx, skew, cx, fy, cy) is read, its last row is taken as (0, 0, 1) */
+struct PoseView {
+    unsigned int id;                       /* camID */
+    int width, height;
+    Matrix3d K, R;
+    Vector3d t;
+    double median_depth;                   /* mavmap: the constant regularisation depth the frontend matches with */
+};
+
+/* Visual neighbours for models without world points (mavmap, SLAM / VIO keyframes, pose-only surveys): what the world-point rule of
+ * findVisualNeighborsFromWPs (line3D.cc:578-699) chooses when every view's world points are a gx x gy grid of its pixel centres at
+ * median_depth, each seen by every view it projects into (l3d_pose_neighbors of include/l3d_capi.h, DESIGN.md §6d).  neighbors[i]
+ * lists view i's neighbours' camIDs, ascending, for addImage under neighbors_by_worldpoints = false.  Runs on device cuda_device
+ * through a context that lives for the call; returns false with *error naming the view (index and camID) and the problem for the
+ * inputs l3d_pose_neighbors rejects, or without a usable device. */
+bool poseNeighbors(const std::vector<PoseView>& views, unsigned int num_neighbors, std::vector<std::list<unsigned int> >& neighbors, std::string* error = 0,
+                   int gx = 32, int gy = 24, int cuda_device = 0);
+
 /* OpenMVG's sfm_data.json like main_openmvg.cpp:136-410: views, intrinsics (pinhole_radial_k1 / _k3, pinhole_brown_t2; other models
  * carry no distortion; an entry without polymorphic_name keeps the model of the entry before it, as the reference's loop does),
  * extrinsics (t = -R C, C as stored), structure (world point ids and float depths |C - X| per view, file order).  A view is returned,

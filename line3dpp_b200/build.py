@@ -14,7 +14,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libl3d_b200.so")
-SOURCES = ["l3d_match.cu", "l3d_capi.cu", "l3d_pipeline.cu", "l3d_affinity.cu", "l3d_collinear.cu", "l3d_optimize.cu", "l3d_undistort.cu", "l3d_image_prep.cu", "l3d_jpeg.cu", "l3d_png.cu", "l3d_triangulate.cu", "line3d_host.cc", "line3d_bin.cc",
+SOURCES = ["l3d_match.cu", "l3d_capi.cu", "l3d_pipeline.cu", "l3d_affinity.cu", "l3d_collinear.cu", "l3d_optimize.cu", "l3d_undistort.cu", "l3d_image_prep.cu", "l3d_jpeg.cu", "l3d_png.cu", "l3d_triangulate.cu", "l3d_pose.cu", "line3d_host.cc", "line3d_bin.cc",
            "line3d_sfm.cc", "line3d_newk.cc", "line3d_jpeg.cc", "line3d_png.cc"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-fmad=false",

@@ -102,6 +102,32 @@ def make_points_desc(K, lens, count, src, dst, new_K=None):
     return d
 
 
+class PoseView(C.Structure):
+    """l3d_pose_view: one posed view for l3d_pose_neighbors"""
+    _fields_ = [("cam_id", C.c_uint32), ("width", C.c_int32), ("height", C.c_int32), ("pad", C.c_int32), ("fx", C.c_double), ("fy", C.c_double),
+                ("cx", C.c_double), ("cy", C.c_double), ("skew", C.c_double), ("R", C.c_double * 9), ("t", C.c_double * 3),
+                ("median_depth", C.c_double)]
+
+
+def make_pose_views(cam_ids, K, R, t, widths, heights, median_depths):
+    """l3d_pose_view[n] from per-view arrays: K (n, 3, 3) (its upper triangle is read), R (n, 3, 3), t (n, 3); widths, heights and
+    median_depths one value for all views or one per view"""
+    n = len(cam_ids)
+    K = np.asarray(K, np.float64).reshape(n, 3, 3)
+    R = np.asarray(R, np.float64).reshape(n, 9)
+    t = np.asarray(t, np.float64).reshape(n, 3)
+    w, h, md = (np.broadcast_to(np.asarray(a), (n,)) for a in (widths, heights, median_depths))
+    arr = (PoseView * n)()
+    for i in range(n):
+        d = arr[i]
+        d.cam_id, d.width, d.height = int(cam_ids[i]), int(w[i]), int(h[i])
+        d.fx, d.fy, d.cx, d.cy, d.skew = (float(K[i, 0, 0]), float(K[i, 1, 1]), float(K[i, 0, 2]), float(K[i, 1, 2]), float(K[i, 0, 1]))
+        d.R[:] = R[i].tolist()
+        d.t[:] = t[i].tolist()
+        d.median_depth = float(md[i])
+    return arr
+
+
 class ImagePrepDesc(C.Structure):
     """l3d_image_prep_desc: one 8-bit image, its max_img_width and the grey output"""
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("channels", C.c_int32), ("max_img_width", C.c_int32),
@@ -607,6 +633,28 @@ class Context:
     def undistort_points_descs(self, descs, on_device):
         """l3d_undistort_points on a ctypes array of PointsDesc as given (for tests of the checks)"""
         self._chk(self.L.l3d_undistort_points(self.h, len(descs), descs, int(on_device)), "l3d_undistort_points")
+
+    # ---- visual neighbours from camera poses (stateless: no pipeline stage changes)
+    def pose_neighbors(self, views, num_neighbors, gx=32, gy=24):
+        """l3d_pose_neighbors on a ctypes array of PoseView (make_pose_views): (one uint32 array of neighbour camIDs per view, n_i int32
+        [n], (device ms, host selection ms))"""
+        n = len(views)
+        ptr = np.zeros(n + 1, np.int64)
+        cams = np.zeros(max(1, n * min(int(num_neighbors), max(n - 1, 0))), np.uint32)
+        nobs = np.zeros(max(n, 1), np.int32)
+        timing = np.zeros(2, np.float64)
+        self._chk(self.L.l3d_pose_neighbors(self.h, n, views, int(gx), int(gy), int(num_neighbors), _p(ptr), _p(cams), len(cams), _p(nobs),
+                                            _p(timing)), "l3d_pose_neighbors")
+        return [cams[ptr[i]:ptr[i + 1]].copy() for i in range(n)], nobs[:n], (float(timing[0]), float(timing[1]))
+
+    def pose_covisibility(self, views, gx=32, gy=24):
+        """l3d_pose_covisibility: (n_i int32 [n], (i, j, common(i, j)) int32 [m, 3] of every nonzero pair i != j, ascending)"""
+        n = len(views)
+        nobs = np.zeros(max(n, 1), np.int32)
+        m = self._chk(self.L.l3d_pose_covisibility(self.h, n, views, int(gx), int(gy), _p(nobs), None, 0), "l3d_pose_covisibility")
+        ijc = np.zeros((max(m, 1), 3), np.int32)
+        self._chk(self.L.l3d_pose_covisibility(self.h, n, views, int(gx), int(gy), _p(nobs), _p(ijc), m), "l3d_pose_covisibility")
+        return nobs[:n], ijc[:m]
 
     # ---- image preparation for line detection (stateless: no pipeline stage changes)
     def prepare_gray(self, images, max_img_width):

@@ -11,6 +11,7 @@
 #include <nvtx3/nvToolsExt.h>      // header-only; ranges show up in nsys / ncu timelines
 #include "../../include/l3d_capi.h"
 #include "../../include/l3dpp_capi.h"
+#include "l3d_pose_select.h"
 #include <cuda_runtime_api.h>          // cudaGetDevice: undistortImage runs on the caller's current device
 
 #include <algorithm>
@@ -620,6 +621,45 @@ struct Line3D::Impl {
     }
 };
 
+// The candidate half of findVisualNeighborsFromWPs (line3D.cc:618-697), shared by the world-point path below and l3d_pose_neighbors
+// (pose_select_neighbors): `ranked` holds view v's candidates with more than 4 common points as (camID, score), by score descending with
+// ties in ascending camID (the stable sort of line3D.cc:638 over the camID-ordered map); view_of(camID) gives a candidate's HostView.
+// The axis gate keeps that order, so it may come after the sort.
+template <class ViewOf>
+static void select_visual_neighbors(const HostView& v, const std::vector<std::pair<unsigned int, float> >& ranked, unsigned int num_neighbors,
+                                    ViewOf view_of, std::set<unsigned int>& out)
+{
+    struct Cand { unsigned int cam; float score, axis, dist; };
+    std::vector<Cand> cand;
+    for (const auto& r : ranked) {
+        const HostView& o = view_of(r.first);
+        Cand c; c.cam = r.first; c.score = r.second;
+        c.axis = (float)std::acos(std::fmin(std::fmax(dot(v.ray(v.pp.x, v.pp.y), o.ray(o.pp.x, o.pp.y)), -1.0), 1.0));      // opticalAxesAngle view.cc:457-463
+        const Vector3d ct = matvec(v.R, o.C) + v.t;                                                                        // distanceVisualNeighborScore view.cc:487-501
+        c.dist = std::fabs((float)ct.x) + std::fabs((float)ct.y);
+        if (c.axis < 1.571f) cand.push_back(c);
+    }
+    if (cand.size() > num_neighbors) {
+        const std::vector<Cand> all = cand;
+        const float score_t = 0.80f * cand.front().score;
+        size_t nbig = 0;
+        while (nbig < cand.size() && cand[nbig].score > score_t) ++nbig;
+        cand.resize(nbig);
+        std::stable_sort(cand.begin(), cand.end(), [](const Cand& a, const Cand& b) { return a.dist > b.dist; });
+        if (cand.size() > num_neighbors / 2) cand.resize(num_neighbors / 2);
+        cand.insert(cand.end(), all.begin(), all.end());
+    }
+    const float min_baseline = 0.1f;
+    auto baseline = [&](unsigned int b) { return (float)norm(v.C - view_of(b).C); };
+    for (size_t i = 0; i < cand.size() && out.size() < num_neighbors; ++i) {
+        const unsigned int n = cand[i].cam;
+        if (out.count(n) || !(baseline(n) > min_baseline)) continue;
+        bool valid = true;
+        for (unsigned int u : out) if (!(baseline(u) > min_baseline)) { valid = false; break; }
+        if (valid) out.insert(n);
+    }
+}
+
 // visual neighbours (line3D.cc:463-485): the given ones that were added, or findVisualNeighborsFromWPs (578-699)
 void Line3D::Impl::find_visual_neighbors(unsigned int camID)
 {
@@ -634,37 +674,47 @@ void Line3D::Impl::find_visual_neighbors(unsigned int camID)
     for (unsigned int wp : v.wps_or_neighbors)
         for (unsigned int other : wps2views[wp]) if (other != camID) ++common[other];
     if (common.empty()) return;
-    struct Cand { unsigned int cam; float score, axis, dist; };
-    std::vector<Cand> cand;
-    for (auto& kv : common) {
-        const HostView& o = views[kv.first];
-        Cand c; c.cam = kv.first;
-        c.score = 2.0f * float(kv.second) / float(v.wps_or_neighbors.size() + o.wps_or_neighbors.size());
-        c.axis = (float)std::acos(std::fmin(std::fmax(dot(v.ray(v.pp.x, v.pp.y), o.ray(o.pp.x, o.pp.y)), -1.0), 1.0));      // opticalAxesAngle view.cc:457-463
-        const Vector3d ct = matvec(v.R, o.C) + v.t;                                                                        // distanceVisualNeighborScore view.cc:487-501
-        c.dist = std::fabs((float)ct.x) + std::fabs((float)ct.y);
-        if (c.axis < 1.571f && kv.second > 4) cand.push_back(c);
+    std::vector<std::pair<unsigned int, float> > ranked;
+    for (auto& kv : common)
+        if (kv.second > 4) ranked.emplace_back(kv.first, 2.0f * float(kv.second) / float(v.wps_or_neighbors.size() + views[kv.first].wps_or_neighbors.size()));
+    std::stable_sort(ranked.begin(), ranked.end(), [](const std::pair<unsigned int, float>& a, const std::pair<unsigned int, float>& b) { return a.second > b.second; });
+    select_visual_neighbors(v, ranked, num_neighbors, [&](unsigned int cam) -> const HostView& { return views.find(cam)->second; }, out);
+}
+
+// K, R, t of a view and what View::View derives from them (view.cc:6-42): the principal point, R^T K^-1, the centre and their float copies
+static void set_camera(HostView& v, const Matrix3d& K, const Matrix3d& R, const Vector3d& t)
+{
+    v.K = K; v.R = R; v.t = t;
+    v.pp = Vector3d(K(0, 2), K(1, 2), 1.0);
+    const Matrix3d Rt = transposed(R);
+    v.RtKinv = matmul(Rt, inverted(K));
+    v.C = matvec(Rt, t * -1.0);
+    v.C_f3[0] = (float)v.C.x; v.C_f3[1] = (float)v.C.y; v.C_f3[2] = (float)v.C.z;
+    for (int i = 0; i < 9; ++i) v.RtKinv_f[i] = (float)v.RtKinv.m[i];
+}
+
+void pose_select_neighbors(int n, const l3d_pose_view* views, const long long* cand_off, const PoseCandidate* cand, unsigned int num_neighbors,
+                           std::vector<std::vector<unsigned int> >& out)
+{
+    std::vector<HostView> hv((size_t)n);
+    std::map<unsigned int, int> index_of;
+    for (int i = 0; i < n; ++i) {
+        const l3d_pose_view& d = views[i];
+        Matrix3d K, R;
+        K(0, 0) = d.fx; K(0, 1) = d.skew; K(0, 2) = d.cx; K(1, 0) = 0.0; K(1, 1) = d.fy; K(1, 2) = d.cy; K(2, 0) = 0.0; K(2, 1) = 0.0; K(2, 2) = 1.0;
+        memcpy(R.m, d.R, sizeof(R.m));
+        hv[i].id = d.cam_id; hv[i].width = d.width; hv[i].height = d.height;
+        set_camera(hv[i], K, R, Vector3d(d.t[0], d.t[1], d.t[2]));
+        index_of[d.cam_id] = i;
     }
-    std::stable_sort(cand.begin(), cand.end(), [](const Cand& a, const Cand& b) { return a.score > b.score; });
-    if (cand.size() > num_neighbors) {
-        const std::vector<Cand> all = cand;
-        const float score_t = 0.80f * cand.front().score;
-        size_t nbig = 0;
-        while (nbig < cand.size() && cand[nbig].score > score_t) ++nbig;
-        cand.resize(nbig);
-        std::stable_sort(cand.begin(), cand.end(), [](const Cand& a, const Cand& b) { return a.dist > b.dist; });
-        if (cand.size() > num_neighbors / 2) cand.resize(num_neighbors / 2);
-        cand.insert(cand.end(), all.begin(), all.end());
-    }
-    const float min_baseline = 0.1f;
-    auto baseline = [&](unsigned int a, unsigned int b) { return (float)norm(views[a].C - views[b].C); };
-    for (size_t i = 0; i < cand.size() && out.size() < num_neighbors; ++i) {
-        const unsigned int n = cand[i].cam;
-        if (out.count(n) || !(baseline(camID, n) > min_baseline)) continue;
-        bool valid = true;
-        for (unsigned int u : out) if (!(baseline(camID, u) > min_baseline)) { valid = false; break; }
-        if (valid) out.insert(n);
-    }
+    out.assign((size_t)n, std::vector<unsigned int>());
+    parallel_for((size_t)n, [&](size_t i) {
+        std::vector<std::pair<unsigned int, float> > ranked;
+        for (long long k = cand_off[i]; k < cand_off[i + 1]; ++k) ranked.emplace_back(cand[k].cam, cand[k].score);
+        std::set<unsigned int> nb;
+        select_visual_neighbors(hv[i], ranked, num_neighbors, [&](unsigned int cam) -> const HostView& { return hv[index_of.find(cam)->second]; }, nb);
+        out[i].assign(nb.begin(), nb.end());
+    });
 }
 
 // ------------------------------------------------------------------------------------------------ Line3D
@@ -714,16 +764,11 @@ bool Line3D::addImage(const unsigned int camID, const int w, const int h, const 
     Impl& P = *p_;
     // everything that needs no shared state first (the reference's frontends call addImage from an OpenMP loop) ...
     HostView v;
-    v.id = camID; v.width = w; v.height = h; v.K = K; v.R = R; v.t = t; v.lines = line_segments; v.wps_or_neighbors = wps_or_neighbors;
+    v.id = camID; v.width = w; v.height = h; v.lines = line_segments; v.wps_or_neighbors = wps_or_neighbors;
     std::string no_segments;
     if (line_segments.empty()) P.read_segment_cache(camID, w, h, v.lines, no_segments);
     v.min_line_length = std::sqrt(float((unsigned)w * (unsigned)w + (unsigned)h * (unsigned)h)) * 0.005f;                           // view.cc:17-18
-    v.pp = Vector3d(K(0, 2), K(1, 2), 1.0);
-    const Matrix3d Rt = transposed(R);
-    v.RtKinv = matmul(Rt, inverted(K));
-    v.C = matvec(Rt, t * -1.0);
-    v.C_f3[0] = (float)v.C.x; v.C_f3[1] = (float)v.C.y; v.C_f3[2] = (float)v.C.z;
-    for (int i = 0; i < 9; ++i) v.RtKinv_f[i] = (float)v.RtKinv.m[i];
+    set_camera(v, K, R, t);
     // ... then one critical section for the checks, the insertion and the error string.  A failure is reported through the return
     // value AND stays in lastError() (a later successful addImage does not clear it) until the next non-addImage call.
     std::lock_guard<std::mutex> g(P.mtx);
@@ -1324,6 +1369,39 @@ void Line3D::undistortPoints(std::vector<std::vector<float> >& xy, const std::ve
         d[i].src = d[i].dst = xy[i].data();
     }
     undistort_point_sets(d);
+}
+
+bool poseNeighbors(const std::vector<PoseView>& views, unsigned int num_neighbors, std::vector<std::list<unsigned int> >& neighbors, std::string* error,
+                   int gx, int gy, int cuda_device)
+{
+    auto fail = [&](const std::string& what) { if (error) *error = "poseNeighbors: " + what; return false; };
+    if (views.size() > (size_t)L3D_POSE_MAX_VIEWS) return fail("more than L3D_POSE_MAX_VIEWS views");
+    const int n = (int)views.size();
+    std::vector<l3d_pose_view> d((size_t)n);
+    for (int i = 0; i < n; ++i) {
+        const PoseView& v = views[i];
+        l3d_pose_view& q = d[i];
+        memset(&q, 0, sizeof(q));
+        q.cam_id = v.id; q.width = v.width; q.height = v.height;
+        q.fx = v.K(0, 0); q.skew = v.K(0, 1); q.cx = v.K(0, 2); q.fy = v.K(1, 1); q.cy = v.K(1, 2);
+        memcpy(q.R, v.R.m, sizeof(q.R));
+        q.t[0] = v.t.x; q.t[1] = v.t.y; q.t[2] = v.t.z;
+        q.median_depth = v.median_depth;
+    }
+    int prev = 0;
+    if (cudaGetDevice(&prev) != cudaSuccess || cudaSetDevice(cuda_device) != cudaSuccess) return fail("no usable CUDA device");
+    struct Restore { int d; ~Restore() { cudaSetDevice(d); } } restore{prev};
+    l3d_ctx* ctx = nullptr;
+    if (l3d_ctx_create(cuda_device, &ctx) != L3D_OK) return fail("no usable CUDA device");
+    std::vector<int64_t> ptr((size_t)n + 1);
+    std::vector<uint32_t> cams((size_t)n * std::min<size_t>(num_neighbors, n > 0 ? (size_t)n - 1 : 0));
+    const long long rc = l3d_pose_neighbors(ctx, n, d.data(), gx, gy, num_neighbors, ptr.data(), cams.data(), (long long)cams.size(), nullptr, nullptr);
+    const std::string msg = l3d_last_error(ctx);
+    l3d_ctx_destroy(ctx);
+    if (rc < 0) { if (error) *error = msg; return false; }
+    neighbors.assign((size_t)n, std::list<unsigned int>());
+    for (int i = 0; i < n; ++i) neighbors[i].assign(cams.begin() + ptr[i], cams.begin() + ptr[i + 1]);
+    return true;
 }
 
 }  // namespace L3DPP

@@ -581,6 +581,17 @@ def sequential_neighbors(i, n_cams, num_neighbors):
     return out[:n].tolist()
 
 
+def pose_neighbors(cam_ids, K, R, t, widths, heights, median_depths, num_neighbors=10, gx=32, gy=24, device=0):
+    """poseNeighbors (include/line3d_io.h): visual neighbours from camera poses alone, for add_image with neighbors_by_worldpoints=False.
+    K (n, 3, 3), R (n, 3, 3), t (n, 3) with x_cam = R X + t; widths, heights, median_depths one value or one per view.  Returns one
+    uint32 array of neighbour camIDs (ascending) per view.  Raises L3DError naming the view for the inputs l3d_pose_neighbors rejects."""
+    ctx = capi.Context(device)
+    try:
+        return ctx.pose_neighbors(capi.make_pose_views(cam_ids, K, R, t, widths, heights, median_depths), num_neighbors, gx, gy)[0]
+    finally:
+        ctx.close()
+
+
 def rotation_from_rpy(roll, pitch, yaw):
     """Line3D::rotationFromRPY"""
     R = np.zeros(9)
